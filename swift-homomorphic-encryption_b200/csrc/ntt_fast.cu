@@ -3,12 +3,13 @@
 // Persistent CTAs: each CTA (T = N/16 threads; as many CTAs per SM as the register budget of ntt_min_ctas allows) walks
 // over rows task = blockIdx.x, blockIdx.x + gridDim.x, ...  For every row
 //   1. TMA in: one thread issues bulk-tensor copies (cp.async.bulk.tensor.2d, 256 lines = 32 KB each, 128-byte
-//      swizzle) that land the row in shared memory and complete on an mbarrier; it also prefetches the CTA's next row
-//      into L2 (cp.async.bulk.prefetch.tensor) and, when the row's modulus differs from the previous row's, bulk-copies
-//      the first N/16 twiddles (all the LB > 0 passes need) into the CTA's shared-memory twiddle cache;
+//      swizzle) that land a row in a shared-memory row buffer and complete on that buffer's mbarrier -- with two
+//      buffers (N = 2^13, ntt_row_buffers) the CTA's next row, otherwise this row; it also prefetches the row after
+//      that into L2 (cp.async.bulk.prefetch.tensor) and, when the row's modulus differs from the previous row's,
+//      bulk-copies the first N/16 twiddles (all the LB > 0 passes need) into the CTA's shared-memory twiddle cache;
 //   2. 3-4 register passes over the row in shared memory (ntt_fast.cuh), one __syncthreads between passes;
-//   3. TMA out: bulk-tensor copies shared -> global of the finished row (same swizzle, undone by the copy engine);
-//      the next row's TMA-in is issued by the same thread once the copy engine has read the buffer.
+//   3. TMA out: bulk-tensor copies shared -> global of the finished row (same swizzle, undone by the copy engine), one
+//      bulk group per row; a buffer is refilled once the copy engine has read it.
 // NARROW / MID / WIDE rows (different lazy-reduction schedules) are mixed in one launch: the row's class selects the
 // instruction stream, rows are ordered class-major so all CTAs walk the classes in step, and there is one tail per
 // NTT call instead of one per class.
@@ -77,7 +78,9 @@ __device__ __forceinline__ void tma_prefetch_box(const CUtensorMap *map, int lin
     asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(map), "r"(0), "r"(line) : "memory");
 }
 __device__ __forceinline__ void tma_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// the copy engine has read the buffers of all but the PENDING most recently committed store groups
+template <int PENDING>
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(PENDING) : "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
@@ -140,16 +143,24 @@ __device__ __forceinline__ void inv_row(u64 *sm, int tau, const RowMod &m) {
     inv_row_pass<LOGN, CLS, P - 1>(x, sm, tau, m);
 }
 
-// Shared memory of a CTA: [row: N words][twiddle cache: N/16 entries][2 mbarriers].
+// Row buffers of a CTA.  With one CTA per SM (N = 2^13) nothing else on the SM runs while the CTA waits for its copies,
+// so the next row's TMA-in and the previous row's TMA-out run under the current row's butterflies (C2 on H100 at a
+// 400 W power limit: +4 % over one buffer; three buffers measured 1-2 % behind two).  With several CTAs per SM
+// (N <= 2^12) the other CTAs fill those gaps, and at N = 2^14 a second 128 KB buffer does not fit.
+HE_HD constexpr int ntt_row_buffers(int logn) { return logn == 13 ? 2 : 1; }
+
+// Shared memory of a CTA: [row buffers: B x N words][twiddle cache: N/16 entries][B + 1 mbarriers].
 template <int LOGN>
 constexpr size_t ntt_smem_bytes() {
-    return sizeof(u64) * ((size_t)1 << LOGN) + sizeof(ulonglong2) * ((size_t)1 << (LOGN - 4)) + 16;
+    constexpr int B = ntt_row_buffers(LOGN);
+    return sizeof(u64) * B * ((size_t)1 << LOGN) + sizeof(ulonglong2) * ((size_t)1 << (LOGN - 4)) + sizeof(u64) * (B + 1);
 }
 
 // CTAs per SM the register budget is sized for.  1024 threads per SM (64 registers a thread, some spills) except at
 // N = 2^13, where one 512-thread CTA with 128 registers and no spills is faster on H100 (C2, runs alternated in one
-// session: +2.7 % at a 700 W power limit, +6 % at 400 W; DESIGN.md section 4); at N = 2^12 the 64-register budget beat
-// 80 and 128 registers by 3-4 % (C1, C2-u32).
+// session: +2.7 % at a 700 W power limit, +6 % at 400 W; DESIGN.md section 4); at 64 registers that kernel still spills
+// (about 450 bytes a thread), and its two row buffers (136 KB) leave room for one CTA per SM in any case.  At N = 2^12
+// the 64-register budget beat 80 and 128 registers by 3-4 % (C1, C2-u32).
 constexpr int ntt_min_ctas(int logn) { return logn == 13 ? 1 : 1024 / ((1 << logn) / 16); }
 
 template <int LOGN, bool INVERSE>
@@ -157,54 +168,72 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
     ntt_rows_kernel(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_out,
                     const ModSlot *__restrict__ slots, const __grid_constant__ RowList rl, const int polys,
                     const int scale_mode, const int debug_flags) {
-    extern __shared__ __align__(1024) u64 sm[];  // row first: the 128-byte swizzle wants it 1024-byte aligned
+    extern __shared__ __align__(1024) u64 smem[];  // row buffers first: the 128-byte swizzle wants them 1024-byte aligned
     constexpr int kLines = (1 << LOGN) / kLineWords;
     constexpr int kBoxes = kLines > kBoxLines ? kLines / kBoxLines : 1;
     constexpr int kLinesPerBox = kLines / kBoxes;
     constexpr u32 kRowBytes = (u32)sizeof(u64) << LOGN, kTwBytes = (u32)sizeof(ulonglong2) << (LOGN - 4);
-    ulonglong2 *tw_cache = reinterpret_cast<ulonglong2 *>(sm + (1 << LOGN));
-    u64 *bar_row = reinterpret_cast<u64 *>(tw_cache + (1 << (LOGN - 4)));
-    u64 *bar_tw = bar_row + 1;
+    // B row buffers; row k of the CTA uses buffer k % B, and its TMA-in is issued AHEAD rows before the CTA starts on it
+    constexpr int B = ntt_row_buffers(LOGN), AHEAD = B > 1 ? 1 : 0;
+    ulonglong2 *tw_cache = reinterpret_cast<ulonglong2 *>(smem + B * (1 << LOGN));
+    u64 *bar_row = reinterpret_cast<u64 *>(tw_cache + (1 << (LOGN - 4)));  // one per buffer
+    u64 *bar_tw = bar_row + B;
     const int tau = threadIdx.x;
     const int tasks = polys * rl.count;  // < 2^31 (checked by the launcher)
+    // global position (in 16-word lines) of task t's input row
+    auto in_line = [&](int t) {
+        const int w = t / polys, p = t - w * polys;
+        const int64_t word = INVERSE ? ((int64_t)p * rl.rows_per_poly + rl.row[w]) << LOGN
+                                     : (int64_t)p * rl.src_poly_stride + ((int64_t)rl.src_row[w] << LOGN);
+        return (int)(word >> 4);
+    };
+    auto load_row = [&](int t, int buf) {
+        mbar_arrive_expect_tx(&bar_row[buf], kRowBytes);
+        const int line = in_line(t);
+        u64 *dst = smem + buf * (1 << LOGN);
+#pragma unroll
+        for (int b = 0; b < kBoxes; ++b) tma_load_box(dst + b * kLinesPerBox * kLineWords, &map_in, line + b * kLinesPerBox, &bar_row[buf]);
+    };
     if (tau == 0) {
-        if (smem_u32(sm) & 1023) __trap();  // dynamic shared memory starts at the window base when there is no static part
-        mbar_init(bar_row, 1);
+        if (smem_u32(smem) & 1023) __trap();  // dynamic shared memory starts at the window base when there is no static part
+#pragma unroll
+        for (int b = 0; b < B; ++b) mbar_init(&bar_row[b], 1);
         mbar_init(bar_tw, 1);
+        if (AHEAD && (int)blockIdx.x < tasks) load_row(blockIdx.x, 0);
     }
     __syncthreads();
-    u32 phase_row = 0, phase_tw = 0;
+    u32 phase_row = 0, phase_tw = 0;  // phase_row: bit b = parity of buffer b's next completion
     int cached_slot = -1;
+    int buf = 0;
     for (int task = blockIdx.x; task < tasks; task += gridDim.x) {
         const int which = task / polys;
         const int poly = task - which * polys;
         const int flags = rl.flags[which];
         const int slot = rl.slot[which];
         const ModSlot &S = slots[slot];
+        u64 *sm = smem + buf * (1 << LOGN);
         // line index (16-word lines) of the row inside the buffer each tensor map describes
         const int64_t out_word = ((int64_t)poly * rl.rows_per_poly + rl.row[which]) << LOGN;
-        const int64_t in_word = INVERSE ? out_word : (int64_t)poly * rl.src_poly_stride + ((int64_t)rl.src_row[which] << LOGN);
         const bool new_slot = slot != cached_slot;  // uniform over the CTA
         cached_slot = slot;
         if (tau == 0) {
-            // the previous row's TMA-out has finished reading the buffer (wait_group.read below, same thread), and every
-            // thread has passed the barrier that follows its last use of the twiddle cache
+            // every thread has passed the barrier that follows its last use of the twiddle cache
             if (new_slot) {
                 mbar_arrive_expect_tx(bar_tw, kTwBytes);
                 tma_load_1d(tw_cache, INVERSE ? S.itw : S.tw, kTwBytes, bar_tw);
             }
-            mbar_arrive_expect_tx(bar_row, kRowBytes);
-            const int line = (int)(in_word >> 4);
+            // the row AHEAD tasks on goes into a buffer whose last row's TMA-out was committed B - AHEAD rows ago: the
+            // copy engine must have read it, which leaves the B - 1 - AHEAD stores committed since then in flight
+            const int fill = task + AHEAD * gridDim.x;
+            if (fill < tasks) {
+                tma_store_wait_read<B - 1 - AHEAD>();
+                load_row(fill, (buf + AHEAD) % B);
+            }
+            const int next = fill + gridDim.x;
+            if (next < tasks && !(debug_flags & 1)) {  // L2 prefetch of the row after that
+                const int line = in_line(next);
 #pragma unroll
-            for (int b = 0; b < kBoxes; ++b) tma_load_box(sm + b * kLinesPerBox * kLineWords, &map_in, line + b * kLinesPerBox, bar_row);
-            const int next = task + gridDim.x;
-            if (next < tasks && !(debug_flags & 1)) {
-                const int nw = next / polys;
-                const int np_ = next - nw * polys;
-                const int64_t nword = INVERSE ? ((int64_t)np_ * rl.rows_per_poly + rl.row[nw]) << LOGN
-                                              : (int64_t)np_ * rl.src_poly_stride + ((int64_t)rl.src_row[nw] << LOGN);
-#pragma unroll
-                for (int b = 0; b < kBoxes; ++b) tma_prefetch_box(&map_in, (int)(nword >> 4) + b * kLinesPerBox);
+                for (int b = 0; b < kBoxes; ++b) tma_prefetch_box(&map_in, line + b * kLinesPerBox);
             }
         }
         const int cls = flags & 7;
@@ -220,8 +249,8 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
             mbar_wait(bar_tw, phase_tw);
             phase_tw ^= 1;
         }
-        mbar_wait(bar_row, phase_row);
-        phase_row ^= 1;
+        mbar_wait(&bar_row[buf], (phase_row >> buf) & 1);
+        phase_row ^= 1u << buf;
         if (debug_flags & 4) {  // experiments: data movement only
         } else
 #ifndef HE_EXPERIMENT_ONLY_CLASS
@@ -250,9 +279,9 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
             const int line = (int)(out_word >> 4);
 #pragma unroll
             for (int b = 0; b < kBoxes; ++b) tma_store_box(&map_out, line + b * kLinesPerBox, sm + b * kLinesPerBox * kLineWords);
-            tma_commit();
-            tma_store_wait_read();  // the buffer may be refilled once the copy engine has read it
+            tma_commit();  // one group per row: the buffer is refilled once the copy engine has read it (above)
         }
+        buf = buf + 1 == B ? 0 : buf + 1;
     }
     if (tau == 0) tma_store_wait_all();
 }

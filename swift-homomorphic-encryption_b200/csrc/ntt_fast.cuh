@@ -414,26 +414,33 @@ HE_HD void ct_butterfly(u64 &x, u64 &y, const ulonglong2 w, const RowMod &m) {
     }
 }
 
-template <int LOGN, int LB, int C, int CLS>
-HE_HD void fwd_pass(u64 (&x)[16], int tau, const RowMod &m) {
+// one forward stage (local index J).  The stage index is a template parameter, like the inverse's, so every loop below
+// has a compile-time trip count and fully unrolls: with a run-time stage loop around them the register array x got
+// an address and lived in local memory.
+template <int LOGN, int LB, int C, int CLS, int J>
+HE_HD void fwd_stage(u64 (&x)[16], int tau, const RowMod &m) {
     constexpr int E = pass_e(LB, C), F = 1 << E, S0 = LOGN - LB - C, T = (1 << LOGN) / 16;
+    constexpr int H = 1 << (C - 1 - J);
     const int hi = tau >> (LB - E);
     const ulonglong2 *tw_t = LB == 0 ? m.tw_t() + tau : nullptr;
 #pragma unroll
-    for (int j = 0; j < C; ++j) {
-        const int h = 1 << (C - 1 - j);
+    for (int grp = 0; grp < (1 << J); ++grp) {
+        const ulonglong2 w = LB == 0 ? ld_tw(tw_t + ((1 << J) - 1 + grp) * T)
+                                     : ld_tw_cached(m, (1 << (S0 + J)) + (hi << J) + grp);
 #pragma unroll
-        for (int grp = 0; grp < (1 << j); ++grp) {
-            const ulonglong2 w = LB == 0 ? ld_tw(tw_t + ((1 << j) - 1 + grp) * T)
-                                         : ld_tw_cached(m, (1 << (S0 + j)) + (hi << j) + grp);
+        for (int k = 0; k < H; ++k) {
+            const int a = grp * 2 * H + k;
 #pragma unroll
-            for (int k = 0; k < h; ++k) {
-                const int a = grp * 2 * h + k;
-#pragma unroll
-                for (int f = 0; f < F; ++f) ct_butterfly<CLS>(x[a * F + f], x[(a + h) * F + f], w, m);
-            }
+            for (int f = 0; f < F; ++f) ct_butterfly<CLS>(x[a * F + f], x[(a + H) * F + f], w, m);
         }
     }
+}
+template <int LOGN, int LB, int C, int CLS>
+HE_HD void fwd_pass(u64 (&x)[16], int tau, const RowMod &m) {
+    fwd_stage<LOGN, LB, C, CLS, 0>(x, tau, m);
+    if (C > 1) fwd_stage<LOGN, LB, C, CLS, (C > 1 ? 1 : 0)>(x, tau, m);
+    if (C > 2) fwd_stage<LOGN, LB, C, CLS, (C > 2 ? 2 : 0)>(x, tau, m);
+    if (C > 3) fwd_stage<LOGN, LB, C, CLS, (C > 3 ? 3 : 0)>(x, tau, m);
 }
 
 // reduce the outputs of the last forward stage to canonical residues
