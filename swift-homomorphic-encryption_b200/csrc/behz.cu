@@ -54,15 +54,15 @@ __device__ __forceinline__ void stc(u64 *p, const u64 (&v)[COLS]) {
 template <int L, int COLS>
 __global__ void __launch_bounds__(kThreads) lift_kernel(const u64 *__restrict__ in, int polys_in, u64 *__restrict__ ext,
                                                        int ext_polys, int out_poly_offset,
-                                                       const __grid_constant__ LiftConsts c, int n) {
-    constexpr int R = 2 * L + 1;
+                                                       const __grid_constant__ LiftConsts c, int n, bool q_rows) {
+    const int rows_out = q_rows ? 2 * L + 1 : L + 1, aux0 = q_rows ? L : 0;
     const int coeff = (blockIdx.x * kThreads + threadIdx.x) * COLS;
     if (coeff >= n) return;
     const int64_t poly = (int64_t)blockIdx.z * gridDim.y + blockIdx.y;  // index among items * polys_in
     const int64_t item = polys_in == 2 ? (poly >> 1) : poly / polys_in;  // (no 64-bit division on the hot path)
     const int pin = (int)(poly - item * polys_in);
     const u64 *src = in + poly * L * n + coeff;
-    u64 *dst = ext + ((item * ext_polys + out_poly_offset + pin) * R) * n + coeff;
+    u64 *dst = ext + ((item * ext_polys + out_poly_offset + pin) * rows_out) * n + coeff;
     u64 z[COLS][L];
     u32 acc_mt[COLS];
 #pragma unroll
@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(kThreads) lift_kernel(const u64 *__restrict__ 
 #pragma unroll
     for (int i = 0; i < L; ++i) {
         const Cols<COLS> x = ldc<COLS>(src + (int64_t)i * n);
-        stc<COLS>(dst + (int64_t)i * n, x.v);
+        if (q_rows) stc<COLS>(dst + (int64_t)i * n, x.v);
 #pragma unroll
         for (int k = 0; k < COLS; ++k) {
             // canonical: z is reinterpreted mod b_j and mod m~ below
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(kThreads) lift_kernel(const u64 *__restrict__ 
             const u64 red = mont_reduce(acc, c.b[j], c.b_ninv[j]);
             o[k] = c.wide_sums ? barrett64(red, c.b[j], c.b_mu1[j]) : csub(red, c.b[j]);
         }
-        stc<COLS>(dst + (int64_t)(L + j) * n, o);
+        stc<COLS>(dst + (int64_t)(aux0 + j) * n, o);
     }
 }
 
@@ -255,20 +255,20 @@ __global__ void __launch_bounds__(kThreads) floor_kernel(const u64 *__restrict__
 // parameter sets are rare and slow on every platform; this keeps them correct rather than fast.
 __global__ void __launch_bounds__(kThreads) lift_generic_kernel(const u64 *__restrict__ in, int polys_in, u64 *__restrict__ ext,
                                                                int ext_polys, int out_poly_offset,
-                                                               const __grid_constant__ LiftConsts c, int n) {
-    const int L = c.L, R = 2 * L + 1;
+                                                               const __grid_constant__ LiftConsts c, int n, bool q_rows) {
+    const int L = c.L, rows_out = q_rows ? 2 * L + 1 : L + 1, aux0 = q_rows ? L : 0;
     const int coeff = blockIdx.x * kThreads + threadIdx.x;
     if (coeff >= n) return;
     const int64_t poly = (int64_t)blockIdx.z * gridDim.y + blockIdx.y;
     const int64_t item = poly / polys_in;
     const int pin = (int)(poly - item * polys_in);
     const u64 *src = in + poly * L * n + coeff;
-    u64 *dst = ext + ((item * ext_polys + out_poly_offset + pin) * R) * n + coeff;
+    u64 *dst = ext + ((item * ext_polys + out_poly_offset + pin) * rows_out) * n + coeff;
     u64 z[kMaxL];
     u32 acc_mt = 0;
     for (int i = 0; i < L; ++i) {
         const u64 x = src[(int64_t)i * n];
-        dst[(int64_t)i * n] = x;
+        if (q_rows) dst[(int64_t)i * n] = x;
         z[i] = shoup_mul(x, c.in_w[i], c.in_wp[i], c.q[i]);
         acc_mt += (u32)z[i] * c.punct_mt[i];
     }
@@ -279,7 +279,7 @@ __global__ void __launch_bounds__(kThreads) lift_generic_kernel(const u64 *__res
         u128 acc = (u128)rc * c.qr[j];
         for (int i = 0; i < L; ++i) mac128(acc, z[i], c.mat[j][i]);
         const u64 red = mont_reduce(acc, c.b[j], c.b_ninv[j]);
-        dst[(int64_t)(L + j) * n] = c.wide_sums ? barrett64(red, c.b[j], c.b_mu1[j]) : csub(red, c.b[j]);
+        dst[(int64_t)(aux0 + j) * n] = c.wide_sums ? barrett64(red, c.b[j], c.b_mu1[j]) : csub(red, c.b[j]);
     }
 }
 
@@ -345,7 +345,7 @@ static inline dim3 poly_grid(int64_t n, int64_t polys, int cols) {
 }
 
 cudaError_t launch_lift(const Context &ctx, const u64 *in, int polys_in, u64 *ext, int ext_polys, int out_poly_offset,
-                        int64_t items, cudaStream_t stream, bool reference_base) {
+                        int64_t items, cudaStream_t stream, bool reference_base, bool q_rows) {
     const LiftConsts &consts = reference_base ? ctx.lift : ctx.lift_mul;
     int64_t polys = items * polys_in;
     if (polys == 0) return cudaSuccess;
@@ -357,17 +357,17 @@ cudaError_t launch_lift(const Context &ctx, const u64 *in, int polys_in, u64 *ex
         const dim3 grid = poly_grid(ctx.n, slab, cols);
         ++g_kernel_launches;
         if (ctx.L > 16) {
-            lift_generic_kernel<<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys, out_poly_offset, consts, (int)ctx.n);
+            lift_generic_kernel<<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys, out_poly_offset, consts, (int)ctx.n, q_rows);
         } else if (cols == 2) {
             HE_DISPATCH_L(ctx.L, (lift_kernel<LL, 2><<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys,
-                                                                                 out_poly_offset, consts, (int)ctx.n)));
+                                                                                 out_poly_offset, consts, (int)ctx.n, q_rows)));
         } else {
             HE_DISPATCH_L(ctx.L, (lift_kernel<LL, 1><<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys,
-                                                                                 out_poly_offset, consts, (int)ctx.n)));
+                                                                                 out_poly_offset, consts, (int)ctx.n, q_rows)));
         }
         // advance whole items only (32768 is even and polys_in is 1 or 2)
         in += slab * pstride_in;
-        ext += (slab / polys_in) * (int64_t)ext_polys * (2 * ctx.L + 1) * ctx.n;
+        ext += (slab / polys_in) * (int64_t)ext_polys * (q_rows ? 2 * ctx.L + 1 : ctx.L + 1) * ctx.n;
         polys -= slab;
     }
     return cudaGetLastError();

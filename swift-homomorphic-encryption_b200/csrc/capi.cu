@@ -124,6 +124,15 @@ cudaError_t multiply_chunk(const Context &c, u64 *scratch, const u64 *lhs, const
     cudaError_t e;
     u64 *ext = scratch, *ten = scratch + 4 * poly_words * items;
     const NttRowMap map = c.map_qaux();
+    if (ntt_forward_tensor_supported(c)) {
+        // computeBehzPolys + tensor product with the NTT outputs kept on chip (ntt_fast.cu): the lift writes only the
+        // auxiliary rows, the kernel reads the Q rows from lhs / rhs
+        if ((e = launch_lift(c, lhs, 2, ext, 4, 0, items, s, false, false)) != cudaSuccess) return e;
+        if ((e = launch_lift(c, rhs, 2, ext, 4, 2, items, s, false, false)) != cudaSuccess) return e;
+        if ((e = launch_ntt_forward_tensor(c, map, lhs, rhs, ext, ten, items, s)) != cudaSuccess) return e;
+        if ((e = launch_ntt_inverse(c, map, ten, ten, items * 3 * R, kScaleTMont, s)) != cudaSuccess) return e;
+        return launch_floor(c, ten, out, items * 3, s);
+    }
     // computeBehzPolys for both operands: lift + forward NTT      (Bfv+Multiply.swift:51-57)
     if ((e = launch_lift(c, lhs, 2, ext, 4, 0, items, s)) != cudaSuccess) return e;
     if ((e = launch_lift(c, rhs, 2, ext, 4, 2, items, s)) != cudaSuccess) return e;

@@ -31,12 +31,20 @@ cudaError_t launch_ntt_forward_fast(const Context &ctx, const NttRowMap &map, co
                                     cudaStream_t stream);
 cudaError_t launch_ntt_inverse_fast(const Context &ctx, const NttRowMap &map, const u64 *in, u64 *out, int64_t rows,
                                     int scale_mode, cudaStream_t stream);
+// forward NTT of the lifted operands + tensor product in one kernel (ntt_fast.cu), N = 2^13 with the fast kernels
+// enabled: lhs / rhs (items x 2 x L x N, Coeff, 16-byte aligned) and their auxiliary rows (launch_lift into
+// ext[item][4] with q_rows = false) -> ten[item][3][R][N] (Eval, Montgomery form like launch_tensor)
+bool ntt_forward_tensor_supported(const Context &ctx);
+cudaError_t launch_ntt_forward_tensor(const Context &ctx, const NttRowMap &map, const u64 *lhs, const u64 *rhs,
+                                      const u64 *ext, u64 *ten, int64_t items, cudaStream_t stream);
 
 // ---- BEHZ steps of ct x ct multiply (behz.cu).  reference_base: compute over the reference's [Q, Bsk] (stage-level
 // entry points) instead of the [Q, aux] base the fused multiply uses (context.hpp).
-// lift: `items` x polys_in x L x N  ->  ext[item][out_poly_offset + p][R][N]  with ext item stride ext_polys*R*N
+// lift: `items` x polys_in x L x N  ->  ext[item][out_poly_offset + p][R][N]  with ext item stride ext_polys*R*N;
+// q_rows = false: the L + 1 auxiliary rows only (ext[item][out_poly_offset + p][L + 1][N]), for a consumer that reads
+// the Q rows from the input itself
 cudaError_t launch_lift(const Context &ctx, const u64 *in, int polys_in, u64 *ext, int ext_polys, int out_poly_offset,
-                        int64_t items, cudaStream_t stream, bool reference_base = false);
+                        int64_t items, cudaStream_t stream, bool reference_base = false, bool q_rows = true);
 // tensor: ext[item][4][R][N] (Eval) -> ten[item][3][R][N]
 cudaError_t launch_tensor(const Context &ctx, const u64 *ext, u64 *ten, int64_t items, cudaStream_t stream,
                           bool reference_base = false);

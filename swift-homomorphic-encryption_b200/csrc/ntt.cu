@@ -28,4 +28,6 @@ cudaError_t launch_ntt_inverse(const Context &ctx, const NttRowMap &map, const u
     return launch_ntt_inverse_simple(ctx, map, in, out, rows, scale_mode, stream);
 }
 
+bool ntt_forward_tensor_supported(const Context &ctx) { return use_fast(ctx) && ctx.logn == 13; }
+
 }  // namespace hecuda

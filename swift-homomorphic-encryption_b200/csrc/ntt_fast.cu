@@ -286,6 +286,188 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
     if (tau == 0) tma_store_wait_all();
 }
 
+// ------------------------------------------------------------------------------------ forward NTT + tensor product
+__device__ __forceinline__ u32 cluster_ctarank() {
+    u32 r;
+    asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ int cluster_id_x() {
+    u32 r;
+    asm("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+    return (int)r;
+}
+__device__ __forceinline__ int cluster_count_x() {
+    u32 r;
+    asm("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
+    return (int)r;
+}
+// every thread of the cluster: arrive (release: this thread's shared-memory writes) / wait (acquire)
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+// arrive without ordering memory: for a thread whose reads of the peer's rows have all returned (their values are
+// used before it arrives); a release here would also wait for this thread's global stores
+__device__ __forceinline__ void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
+// the address of the same shared-memory location in CTA `rank` of the cluster
+__device__ __forceinline__ u32 cluster_map(u32 addr, u32 rank) {
+    u32 r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ ulonglong2 ld_cluster_v2(u32 addr) {
+    ulonglong2 v;
+    asm volatile("ld.shared::cluster.v2.u64 {%0, %1}, [%2];" : "=l"(v.x), "=l"(v.y) : "r"(addr) : "memory");
+    return v;
+}
+// a b 2^-64 mod p, canonical (behz.cu:tensor_kernel's arithmetic: the inverse NTT's kScaleTMont restores the 2^64)
+__device__ __forceinline__ u64 mont_product(u64 a, u64 b, u64 p, u64 ninv) { return csub(mont_reduce((u128)a * b, p, ninv), p); }
+
+// The N = 2^13 ct x ct multiply's forward NTT and tensor product (Bfv+Multiply.swift:51-57, :80-82) in one kernel, so
+// the 4 R transformed operand rows of a pair never go to HBM.  A task is one (pair, row r of [Q, aux]); tasks are
+// r-major like the row NTT's, so consecutive tasks share the twiddle cache.  Clusters of two CTAs walk the tasks
+// persistently, both CTAs the same sequence.  CTA rank k transforms a_k and b_k (polynomial k of lhs and of rhs) into
+// its own row buffers, the same TMA-in and register passes as ntt_rows_kernel; then rank 0 computes c0 = a0 b0 and
+// rank 1 c2 = a1 b1 from their own rows, and each computes half the columns of c1 = a0 b1 + a1 b0 with the peer's two
+// rows read through distributed shared memory.  (Splitting the rows a0 a1 | b0 b1 instead would put a remote operand
+// in every product; this split reads N remote words per CTA and task.)  Both CTAs' buffers carry the same 128-byte
+// swizzle, so one shared-memory offset holds the same coefficient in all four rows; the products are stored straight
+// to `ten` with the swizzle undone, in the layout the inverse NTT reads.
+//
+// The Q rows (r < L) are read from lhs / rhs themselves, the auxiliary rows from what the lift wrote,
+// ext[pair][4][L + 1][N] (polynomials a0 a1 b0 b1).
+//
+// Shared memory: [row buffers: operand j of the task in buffer j, 2 x N words][twiddle cache: N/16 entries][3 mbarriers].
+// A task's rows stay in their buffers until the cluster barrier that ends its tensor step; the next task's two rows
+// are loaded after it, the second under the first one's passes.  (A third buffer that took the next task's first row
+// under the current task's second row and tensor step measured no faster: C2 on H100 at a 400 W power limit, three
+// runs each, 136.3-137.1 k mult/s with three buffers, 136.3-137.7 k with two.)
+template <int LOGN>
+constexpr size_t ntt_tensor_smem_bytes() {
+    return sizeof(u64) * 2 * ((size_t)1 << LOGN) + sizeof(ulonglong2) * ((size_t)1 << (LOGN - 4)) + sizeof(u64) * 3;
+}
+
+template <int LOGN>
+__global__ void __launch_bounds__((1 << LOGN) / 16, 1)
+    ntt_forward_tensor_kernel(const __grid_constant__ CUtensorMap map_lhs, const __grid_constant__ CUtensorMap map_rhs,
+                              const __grid_constant__ CUtensorMap map_ext, u64 *__restrict__ ten,
+                              const ModSlot *__restrict__ slots, const __grid_constant__ RowList rl, const int items,
+                              const int L) {
+    extern __shared__ __align__(1024) u64 smem[];  // row buffers first: the 128-byte swizzle wants them 1024-byte aligned
+    constexpr int N = 1 << LOGN, T = N / 16;
+    constexpr int kBoxes = N / kLineWords / kBoxLines;
+    constexpr u32 kRowBytes = (u32)sizeof(u64) << LOGN, kTwBytes = (u32)sizeof(ulonglong2) << (LOGN - 4);
+    static_assert(kBoxes >= 1, "one row is at least one box");
+    ulonglong2 *tw_cache = reinterpret_cast<ulonglong2 *>(smem + 2 * N);
+    u64 *bar_row = reinterpret_cast<u64 *>(tw_cache + N / 16);  // one per buffer
+    u64 *bar_tw = bar_row + 2;
+    const int tau = threadIdx.x;
+    const u32 rank = cluster_ctarank();
+    const int first = cluster_id_x(), stride = cluster_count_x();
+    const int R = rl.rows_per_poly;
+    const int tasks = items * rl.count;  // < 2^31 (checked by the launcher)
+    // operand j's row of task t into buffer j: polynomial `rank` of lhs (j = 0) or rhs (j = 1)
+    auto load_row = [&](int t, int j) {
+        const int w = t / items, item = t - w * items, r = rl.row[w];
+        const CUtensorMap *map;
+        int64_t word;
+        if (r < L) {
+            map = j ? &map_rhs : &map_lhs;
+            word = ((int64_t)(2 * item + (int)rank) * L + r) << LOGN;
+        } else {
+            map = &map_ext;
+            word = ((int64_t)(4 * item + 2 * j + (int)rank) * (L + 1) + r - L) << LOGN;
+        }
+        const int line = (int)(word >> 4);
+        mbar_arrive_expect_tx(&bar_row[j], kRowBytes);
+#pragma unroll
+        for (int b = 0; b < kBoxes; ++b) tma_load_box(smem + j * N + b * kBoxLines * kLineWords, map, line + b * kBoxLines, &bar_row[j]);
+    };
+    if (tau == 0) {
+        if (smem_u32(smem) & 1023) __trap();  // dynamic shared memory starts at the window base when there is no static part
+        mbar_init(&bar_row[0], 1);
+        mbar_init(&bar_row[1], 1);
+        mbar_init(bar_tw, 1);
+    }
+    // both CTAs have started (and initialised their barriers) before either reads the other's shared memory
+    cluster_arrive();
+    cluster_wait();
+    u32 phase_row = 0, phase_tw = 0;  // both row buffers complete once per task
+    int cached_slot = -1;
+    for (int task = first; task < tasks; task += stride) {
+        // the previous task's tensor step is over in both CTAs: its two buffers may be refilled
+        if (task != first) cluster_wait();
+        const int which = task / items;
+        const int item = task - which * items;
+        const int slot = rl.slot[which], r = rl.row[which], cls = rl.flags[which] & 7;
+        const ModSlot &S = slots[slot];
+        const bool new_slot = slot != cached_slot;  // uniform over the cluster
+        cached_slot = slot;
+        if (tau == 0) {
+            // every thread has passed the barrier that follows its last use of the twiddle cache
+            if (new_slot) {
+                mbar_arrive_expect_tx(bar_tw, kTwBytes);
+                tma_load_1d(tw_cache, S.tw, kTwBytes, bar_tw);
+            }
+            load_row(task, 0);
+            load_row(task, 1);
+        }
+        RowMod m;
+        m.np = 0 - S.p;
+        m.kp = (cls == kWide || cls == kSmall) ? 2 * S.p : 4 * S.p;
+        m.tw = nullptr;
+        m.tw_s = smem_u32(tw_cache);
+        m.slot = &S;
+        m.scale_mode = -1;
+        m.partial = false;
+        if (new_slot) {
+            mbar_wait(bar_tw, phase_tw);
+            phase_tw ^= 1;
+        }
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+            mbar_wait(&bar_row[j], phase_row);
+            u64 *sm = smem + j * N;
+            if (kNarrowHEnabled && cls == kNarrowH) fwd_row<LOGN, kNarrowHEnabled ? kNarrowH : kNarrow>(sm, tau, m, false);
+            else if (cls == kNarrow) fwd_row<LOGN, kNarrow>(sm, tau, m, false);
+            else if (cls == kSmall) fwd_row<LOGN, kSmall>(sm, tau, m, false);
+            else if (cls == kMid) fwd_row<LOGN, kMid>(sm, tau, m, false);
+            else fwd_row<LOGN, kWide>(sm, tau, m, false);
+        }
+        phase_row ^= 1;
+        // ---- tensor step
+        __syncthreads();
+        cluster_arrive();  // this CTA's two rows are final
+        const u64 p = S.p, ninv = S.ninv;
+        const u64 *x = smem, *y = smem + N;  // a_rank, b_rank
+        const int64_t comp = (int64_t)R * N;                   // words between the components of ten
+        u64 *out = ten + ((int64_t)3 * item * R + r) * N;
+        u64 *own = out + (rank ? 2 * comp : 0);  // c0 (rank 0) or c2 (rank 1): this CTA's rows only
+#pragma unroll 4
+        for (int w = 2 * tau; w < N; w += 2 * T) {
+            const ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(x + w), b = *reinterpret_cast<const ulonglong2 *>(y + w);
+            *reinterpret_cast<ulonglong2 *>(own + smem_phys(w)) = make_ulonglong2(mont_product(a.x, b.x, p, ninv), mont_product(a.y, b.y, p, ninv));
+        }
+        cluster_wait();  // the peer's rows are final
+        // c1 = a0 b1 + a1 b0 = x Y + X y over this CTA's half of the columns (X, Y: the peer's rows), summed at 128 bits
+        // before its one reduction
+        const u32 px = cluster_map(smem_u32(x), rank ^ 1), py = cluster_map(smem_u32(y), rank ^ 1);
+#pragma unroll 4
+        for (int w = (int)rank * (N / 2) + 2 * tau; w < ((int)rank + 1) * (N / 2); w += 2 * T) {
+            const ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(x + w), b = *reinterpret_cast<const ulonglong2 *>(y + w);
+            const ulonglong2 A = ld_cluster_v2(px + 8u * w), Bv = ld_cluster_v2(py + 8u * w);
+            u128 m0 = (u128)a.x * Bv.x, m1 = (u128)a.y * Bv.y;
+            mac128(m0, A.x, b.x);
+            mac128(m1, A.y, b.y);
+            *reinterpret_cast<ulonglong2 *>(out + comp + smem_phys(w)) =
+                make_ulonglong2(csub(mont_reduce(m0, p, ninv), p), csub(mont_reduce(m1, p, ninv), p));
+        }
+        // the generic-proxy accesses to these buffers come before their next TMA refill
+        fence_proxy_async_smem();
+        cluster_arrive_relaxed();  // this CTA has finished reading the peer's rows (waited for before the next refill / exit)
+    }
+    if (first < tasks) cluster_wait();  // the peer may still be reading this CTA's rows
+}
+
 // ---------------------------------------------------------------------------------------------- launch
 static void build_row_list(const Context &ctx, const NttRowMap &map, bool inverse, RowList &rl) {
     rl.rows_per_poly = map.rows_per_poly;
@@ -528,6 +710,56 @@ cudaError_t launch_ntt_forward_fast(const Context &ctx, const NttRowMap &map, co
 cudaError_t launch_ntt_inverse_fast(const Context &ctx, const NttRowMap &map, const u64 *in, u64 *out, int64_t rows,
                                     int scale_mode, cudaStream_t stream) {
     return launch_fast<true>(ctx, map, in, out, rows, scale_mode, stream);
+}
+
+cudaError_t launch_ntt_forward_tensor(const Context &ctx, const NttRowMap &map, const u64 *lhs, const u64 *rhs,
+                                      const u64 *ext, u64 *ten, int64_t items, cudaStream_t stream) {
+    constexpr int LOGN = 13;
+    if (ctx.logn != LOGN) return cudaErrorInvalidValue;
+    if (items == 0) return cudaSuccess;
+    // every line index of ext (the largest buffer read) fits an int
+    if (items * 4 * map.rows_per_poly * (ctx.n / kLineWords) > 0x7fffffffLL) return cudaErrorInvalidValue;
+    RowList rl;
+    build_row_list(ctx, map, false, rl);
+    CUtensorMap map_lhs, map_rhs, map_ext;
+    if (!make_line_map(&map_lhs, lhs, LOGN) || !make_line_map(&map_rhs, rhs, LOGN) || !make_line_map(&map_ext, ext, LOGN))
+        return cudaErrorInvalidValue;
+    constexpr int threads = (1 << LOGN) / 16;
+    constexpr size_t smem = ntt_tensor_smem_bytes<LOGN>();
+    auto k = ntt_forward_tensor_kernel<LOGN>;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(threads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    static int clusters_per_device[64] = {0};  // clusters of two CTAs the device holds at once
+    static std::mutex mu;
+    int clusters;
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        int &c = clusters_per_device[ctx.device & 63];
+        if (c == 0) {
+            cudaError_t e;
+            if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
+            cfg.gridDim = dim3(2 * ctx.sm_count);
+            int n = 0;
+            if ((e = cudaOccupancyMaxActiveClusters(&n, k, &cfg)) != cudaSuccess) return e;
+            if (n < 1) return cudaErrorInvalidConfiguration;
+            c = n;
+        }
+        clusters = c;
+    }
+    const int64_t tasks = items * rl.count;
+    cfg.gridDim = dim3((unsigned)(2 * std::min<int64_t>(tasks, clusters)));
+    ++g_kernel_launches;
+    cudaError_t e = cudaLaunchKernelEx(&cfg, k, map_lhs, map_rhs, map_ext, ten, (const ModSlot *)ctx.d_slots, rl, (int)items, ctx.L);
+    return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 }  // namespace hecuda
