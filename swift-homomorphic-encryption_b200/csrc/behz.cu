@@ -13,6 +13,7 @@
 #include <cstdlib>
 
 #include "kernels.cuh"
+#include "ntt_fast.cuh"
 
 namespace hecuda {
 
@@ -51,7 +52,8 @@ __device__ __forceinline__ void stc(u64 *p, const u64 (&v)[COLS]) {
 
 // Bounds (checked for the actual moduli by Context::create): every 128-bit accumulator below stays < 2^127 and the
 // Montgomery-reduced sums are < 2p (lift, f_j, out_i: one or two conditional subtractions) or < 4p (alpha).
-template <int L, int COLS>
+// H: every b_j is h 2^32 + 1 (LiftConsts / FloorConsts::h_primes), so the reductions modulo b_j take mont_reduce_h.
+template <int L, int COLS, bool H>
 __global__ void __launch_bounds__(kThreads) lift_kernel(const u64 *__restrict__ in, int polys_in, u64 *__restrict__ ext,
                                                        int ext_polys, int out_poly_offset,
                                                        const __grid_constant__ LiftConsts c, int n, bool q_rows) {
@@ -94,7 +96,7 @@ __global__ void __launch_bounds__(kThreads) lift_kernel(const u64 *__restrict__ 
             u128 acc = (u128)rc * c.qr[j];
 #pragma unroll
             for (int i = 0; i < L; ++i) mac128(acc, z[k][i], c.mat[j][i]);
-            const u64 red = mont_reduce(acc, c.b[j], c.b_ninv[j]);
+            const u64 red = mont_reduce_c<H>(acc, c.b[j], c.b_ninv[j]);
             o[k] = c.wide_sums ? barrett64(red, c.b[j], c.b_mu1[j]) : csub(red, c.b[j]);
         }
         stc<COLS>(dst + (int64_t)(aux0 + j) * n, o);
@@ -106,9 +108,25 @@ __global__ void __launch_bounds__(kThreads) lift_kernel(const u64 *__restrict__ 
 struct TensorConsts {
     int R;
     u64 p[kMaxRows], ninv[kMaxRows];
+    unsigned char h[kMaxRows];  // p = h 2^32 + 1 < 2^55: mont_reduce_h
 };
 
-template <int COLS>
+template <int COLS, bool H>
+__device__ __forceinline__ void tensor_cols(const Cols<COLS> &a0, const Cols<COLS> &a1, const Cols<COLS> &b0,
+                                            const Cols<COLS> &b1, u64 p, u64 ninv, u64 (&o0)[COLS], u64 (&o1)[COLS],
+                                            u64 (&o2)[COLS]) {
+#pragma unroll
+    for (int k = 0; k < COLS; ++k) {
+        o0[k] = csub(mont_reduce_c<H>((u128)a0.v[k] * b0.v[k], p, ninv), p);
+        u128 m = (u128)a0.v[k] * b1.v[k];
+        mac128(m, a1.v[k], b0.v[k]);
+        o1[k] = csub(mont_reduce_c<H>(m, p, ninv), p);
+        o2[k] = csub(mont_reduce_c<H>((u128)a1.v[k] * b1.v[k], p, ninv), p);
+    }
+}
+
+// ANY_H: some row's prime is h 2^32 + 1 (the others keep the kernel without that branch)
+template <int COLS, bool ANY_H>
 __global__ void __launch_bounds__(kThreads) tensor_kernel(const u64 *__restrict__ ext, u64 *__restrict__ ten,
                                                          const __grid_constant__ TensorConsts c, int n) {
     const int R = c.R;
@@ -122,14 +140,8 @@ __global__ void __launch_bounds__(kThreads) tensor_kernel(const u64 *__restrict_
     const Cols<COLS> a0 = ldc<COLS>(e), a1 = ldc<COLS>(e + ps), b0 = ldc<COLS>(e + 2 * ps), b1 = ldc<COLS>(e + 3 * ps);
     u64 *o = ten + (item * 3 * R + row) * n + coeff;
     u64 o0[COLS], o1[COLS], o2[COLS];
-#pragma unroll
-    for (int k = 0; k < COLS; ++k) {
-        o0[k] = csub(mont_reduce((u128)a0.v[k] * b0.v[k], p, ninv), p);
-        u128 m = (u128)a0.v[k] * b1.v[k];
-        mac128(m, a1.v[k], b0.v[k]);
-        o1[k] = csub(mont_reduce(m, p, ninv), p);
-        o2[k] = csub(mont_reduce((u128)a1.v[k] * b1.v[k], p, ninv), p);
-    }
+    if (ANY_H && c.h[row]) tensor_cols<COLS, true>(a0, a1, b0, b1, p, ninv, o0, o1, o2);
+    else tensor_cols<COLS, false>(a0, a1, b0, b1, p, ninv, o0, o1, o2);
     stc<COLS>(o, o0);
     stc<COLS>(o + ps, o1);
     stc<COLS>(o + 2 * ps, o2);
@@ -193,7 +205,7 @@ __global__ void __launch_bounds__(kThreads) tensor_sum_kernel(const u64 *__restr
     stc<2>(o + 2 * ps, o2);
 }
 
-template <int L, int COLS>
+template <int L, int COLS, bool H>
 __global__ void __launch_bounds__(kThreads) floor_kernel(const u64 *__restrict__ in, u64 *__restrict__ out,
                                                         const __grid_constant__ FloorConsts c, int n) {
     constexpr int R = 2 * L + 1;
@@ -219,7 +231,7 @@ __global__ void __launch_bounds__(kThreads) floor_kernel(const u64 *__restrict__
             u128 acc = (u128)xb.v[k] * c.fq[j];
 #pragma unroll
             for (int i = 0; i < L; ++i) mac128(acc, y[k][i], c.fmat[j][i]);
-            f[k][j] = mont_reduce(acc, c.b[j], c.b_ninv[j]);
+            f[k][j] = mont_reduce_c<H>(acc, c.b[j], c.b_ninv[j]);
         }
     }
     // convertApproximateBskToQ, RnsTool.swift:402-450
@@ -234,7 +246,7 @@ __global__ void __launch_bounds__(kThreads) floor_kernel(const u64 *__restrict__
             w[i] = shoup_mul(f[k][i], c.inb_w[i], c.inb_wp[i], c.b[i]);  // canonical: reinterpreted mod m_sk and q_i
             mac128(acc, w[i], c.amat[i]);
         }
-        u64 alpha = mont_reduce(acc, msk, c.b_ninv[L]);
+        u64 alpha = mont_reduce_c<H>(acc, msk, c.b_ninv[L]);
         alpha = c.wide_sums ? barrett64(alpha, msk, c.msk_mu1) : csub(csub(csub(alpha, 4 * msk), 2 * msk), msk);
         const bool exceeds = alpha > (msk >> 1);
         const u64 alpha_c = exceeds ? msk - alpha : alpha;
@@ -337,6 +349,20 @@ __global__ void __launch_bounds__(kThreads) floor_generic_kernel(const u64 *__re
         default: return cudaErrorInvalidValue;                                                                        \
     }
 
+template <int COLS, bool H>
+static cudaError_t launch_lift_kernel(int L, dim3 grid, cudaStream_t stream, const u64 *in, int polys_in, u64 *ext,
+                                      int ext_polys, int out_poly_offset, const LiftConsts &consts, int n, bool q_rows) {
+    HE_DISPATCH_L(L, (lift_kernel<LL, COLS, H><<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys, out_poly_offset,
+                                                                              consts, n, q_rows)));
+    return cudaSuccess;
+}
+template <int COLS, bool H>
+static cudaError_t launch_floor_kernel(int L, dim3 grid, cudaStream_t stream, const u64 *in, u64 *out,
+                                       const FloorConsts &consts, int n) {
+    HE_DISPATCH_L(L, (floor_kernel<LL, COLS, H><<<grid, kThreads, 0, stream>>>(in, out, consts, n)));
+    return cudaSuccess;
+}
+
 // grid over (coefficient pairs, polys) with polys folded into y (<= 32768) and z
 static inline dim3 poly_grid(int64_t n, int64_t polys, int cols) {
     const unsigned gx = (unsigned)((n / cols + kThreads - 1) / kThreads);
@@ -358,12 +384,11 @@ cudaError_t launch_lift(const Context &ctx, const u64 *in, int polys_in, u64 *ex
         ++g_kernel_launches;
         if (ctx.L > 16) {
             lift_generic_kernel<<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys, out_poly_offset, consts, (int)ctx.n, q_rows);
-        } else if (cols == 2) {
-            HE_DISPATCH_L(ctx.L, (lift_kernel<LL, 2><<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys,
-                                                                                 out_poly_offset, consts, (int)ctx.n, q_rows)));
         } else {
-            HE_DISPATCH_L(ctx.L, (lift_kernel<LL, 1><<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys,
-                                                                                 out_poly_offset, consts, (int)ctx.n, q_rows)));
+            auto launch = cols == 2 ? (consts.h_primes ? launch_lift_kernel<2, true> : launch_lift_kernel<2, false>)
+                                    : (consts.h_primes ? launch_lift_kernel<1, true> : launch_lift_kernel<1, false>);
+            const cudaError_t e = launch(ctx.L, grid, stream, in, polys_in, ext, ext_polys, out_poly_offset, consts, (int)ctx.n, q_rows);
+            if (e != cudaSuccess) return e;
         }
         // advance whole items only (32768 is even and polys_in is 1 or 2)
         in += slab * pstride_in;
@@ -382,19 +407,18 @@ cudaError_t launch_tensor(const Context &ctx, const u64 *ext, u64 *ten, int64_t 
     for (int r = 0; r < tc.R; ++r) {
         tc.p[r] = ctx.slots[map.slot[r]].dev.p;
         tc.ninv[r] = ctx.slots[map.slot[r]].dev.ninv;
+        tc.h[r] = fast::class_of_modulus(tc.p[r], ctx.slots[map.slot[r]].dev.bits) == fast::kNarrowH ? 1 : 0;
     }
     const int cols = ctx.n >= 2 ? cols_per_thread() : 1;
+    bool any_h = false;
+    for (int r = 0; r < tc.R; ++r) any_h |= tc.h[r] != 0;
+    auto k = cols == 2 ? (any_h ? tensor_kernel<2, true> : tensor_kernel<2, false>) : (any_h ? tensor_kernel<1, true> : tensor_kernel<1, false>);
     const unsigned gx = (unsigned)((ctx.n / cols + kThreads - 1) / kThreads);
     for (int64_t done = 0; done < items;) {  // gridDim.z <= 65535
         const int64_t chunk = (items - done) > 65535 ? 65535 : (items - done);
         dim3 grid(gx ? gx : 1, (unsigned)tc.R, (unsigned)chunk);
         ++g_kernel_launches;
-        if (cols == 2)
-            tensor_kernel<2><<<grid, kThreads, 0, stream>>>(ext + done * 4 * tc.R * ctx.n, ten + done * 3 * tc.R * ctx.n, tc,
-                                                            (int)ctx.n);
-        else
-            tensor_kernel<1><<<grid, kThreads, 0, stream>>>(ext + done * 4 * tc.R * ctx.n, ten + done * 3 * tc.R * ctx.n, tc,
-                                                            (int)ctx.n);
+        k<<<grid, kThreads, 0, stream>>>(ext + done * 4 * tc.R * ctx.n, ten + done * 3 * tc.R * ctx.n, tc, (int)ctx.n);
         done += chunk;
     }
     return cudaGetLastError();
@@ -445,10 +469,11 @@ cudaError_t launch_floor(const Context &ctx, const u64 *in, u64 *out, int64_t po
         ++g_kernel_launches;
         if (ctx.L > 16) {
             floor_generic_kernel<<<grid, kThreads, 0, stream>>>(in, out, consts, (int)ctx.n);
-        } else if (cols == 2) {
-            HE_DISPATCH_L(ctx.L, (floor_kernel<LL, 2><<<grid, kThreads, 0, stream>>>(in, out, consts, (int)ctx.n)));
         } else {
-            HE_DISPATCH_L(ctx.L, (floor_kernel<LL, 1><<<grid, kThreads, 0, stream>>>(in, out, consts, (int)ctx.n)));
+            auto launch = cols == 2 ? (consts.h_primes ? launch_floor_kernel<2, true> : launch_floor_kernel<2, false>)
+                                    : (consts.h_primes ? launch_floor_kernel<1, true> : launch_floor_kernel<1, false>);
+            const cudaError_t e = launch(ctx.L, grid, stream, in, out, consts, (int)ctx.n);
+            if (e != cudaSuccess) return e;
         }
         in += slab * (int64_t)R * ctx.n;
         out += slab * (int64_t)ctx.L * ctx.n;

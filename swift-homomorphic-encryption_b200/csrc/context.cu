@@ -143,7 +143,9 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
     // fast base conversion of [t D]_q, a function of the q residues alone) are fixed integers, and the
     // Shenoy-Kumaresan conversion back to q is exact (RnsTool.swift:324-456).  So the multiply runs over L + 1 primes
     // below 2^55, whose NTT rows never need a conditional subtraction (ntt_fast.cuh, NARROW class), instead of the
-    // reference's 61-bit Bsk; the reference base stays available for the stage-level entry points.  Conditions checked:
+    // reference's 61-bit Bsk; the reference base stays available for the stage-level entry points.  The 55-bit primes
+    // are the smallest of the form h 2^32 + 1: their butterflies (NARROW-H) and Montgomery reductions (mont_reduce_h)
+    // need fewer multiplies.  Conditions checked:
     //   q * B_aux > 8 N q^2   (D is represented exactly),   B_aux(L primes) * m_sk > 16 t N q   (F survives SK)
     c->aux = c->bsk;
     {
@@ -155,11 +157,9 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
         for (u64 v : c->q) log_q += std::log2((double)v);
         const double log_n = (double)c->logn, log_t = std::log2((double)t);
         for (int wi = 0; wi < 2 && want_fast && c->aux == c->bsk && word_bits == 64; ++wi) {
-            // (primes h 2^32 + 1 -- the NTT's NARROW-H class, -DHE_NTT_NARROW_H -- were measured here too: a wash, see
-            //  ntt_fast.cuh; the plain smallest primes stay)
-            const bool h_primes = fast::kNarrowHEnabled && std::getenv("HECUDA_AUX_H_PRIMES") != nullptr;
-            std::vector<u64> cand = (widths[wi] == 55 && h_primes) ? smallest_ntt_primes(55, L + 1 + nmod, 1ull << 31)
-                                                                   : smallest_ntt_primes(widths[wi], L + 1 + nmod, (u64)n);
+            // 55 bits: primes = 1 mod 2^32 (NTT-friendly for every supported N)
+            std::vector<u64> cand = widths[wi] == 55 ? smallest_ntt_primes(55, L + 1 + nmod, 1ull << 31)
+                                                     : smallest_ntt_primes(widths[wi], L + 1 + nmod, (u64)n);
             std::vector<u64> pick;
             for (u64 v : cand) {
                 bool used = false;
@@ -268,6 +268,9 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
     auto slot_of = [&](int j) { return reference_base ? c->slot_bsk(j) : c->slot_aux(j); };
     std::memset(&lf, 0, sizeof(lf));
     lf.L = L;
+    bool h_primes = true;  // reductions modulo every b_j can take mont_reduce_h
+    for (int j = 0; j <= L; ++j) h_primes &= fast::class_of_modulus(BSK[j], bit_length(BSK[j])) == fast::kNarrowH;
+    lf.h_primes = h_primes ? 1 : 0;
     {
         const u64 q_mod_mt = prod_mod(Q, L, kMTilde);
         lf.neg_inv_q_mt = (u32)((kMTilde - invmod(q_mod_mt, kMTilde)) % kMTilde);
@@ -294,6 +297,7 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
     }
     std::memset(&fl, 0, sizeof(fl));
     fl.L = L;
+    fl.h_primes = lf.h_primes;
     const u64 b_mod_msk = prod_mod(BSK, L, msk);
     const u64 r64_msk = c->slots[slot_of(L)].dev.r64;
     const u64 b_inv_msk = mulmod(invmod(b_mod_msk, msk), r64_msk, msk);  // B^-1 2^64

@@ -75,6 +75,7 @@ struct LiftConsts {
     u64 b[kMaxL + 1], b_ninv[kMaxL + 1];
     u64 mat[kMaxL + 1][kMaxL];       // (Q/q_i) m~^-1 2^64 mod b_j
     u64 qr[kMaxL + 1];               // Q m~^-1 2^64 mod b_j
+    int h_primes;                    // every b_j is h 2^32 + 1 < 2^55: reduce with mont_reduce_h
 };
 
 // floorQBskToQ (RnsTool.swift:378-456) fused to (all matrix constants pre-multiplied by 2^64, sums Montgomery-reduced):
@@ -95,6 +96,7 @@ struct FloorConsts {
     u64 a_msk;                         // -B^-1 2^64 mod m_sk
     u64 omat[kMaxL][kMaxL];            // (B/b_k) 2^64 mod q_i
     u64 b_mod_q[kMaxL], neg_b_mod_q[kMaxL];  // +-B 2^64 mod q_i
+    int h_primes;                      // every b_j is h 2^32 + 1 < 2^55: reduce f_j and alpha with mont_reduce_h
 };
 
 // divideAndRoundQLast (PolyRq.swift:365-393) for a base [m_0..m_{l-2}, m_last]

@@ -93,6 +93,18 @@ HE_HD u64 mont_reduce(u128 acc, u64 p, u64 ninv) {
     const u64 m = lo * ninv;
     return hi + mulhi64(m, p) + (lo != 0 ? 1ull : 0ull);
 }
+// mont_reduce for p = h 2^32 + 1 < 2^55 (the multiply's 55-bit auxiliary primes, context.cu), the same value in every
+// case.  ninv = h 2^32 - 1, so m = lo ninv mod 2^64 = ((lo0 h) << 32) - lo takes one 32-bit multiply, and with
+// m p = m0 + 2^32 (m1 + m0 h) + 2^64 m1 h, hi64(m p) = m1 h + hi32(m0 h + m1) takes two 32 x 32 -> 64 ones.  The generic
+// form spends three multiplies on m and four wide ones on the 64-bit mulhi.
+HE_HD u64 mont_reduce_h(u128 acc, u64 p) {
+    const u64 lo = (u64)acc, hi = (u64)(acc >> 64);
+    const u32 h = (u32)(p >> 32), lo0 = (u32)lo, lo1 = (u32)(lo >> 32);
+    const u32 m0 = 0u - lo0, m1 = lo0 * h - lo1 - (lo0 != 0 ? 1u : 0u);  // m = 2^32 m1 + m0
+    return hi + (u64)m1 * h + (((u64)m0 * h + m1) >> 32) + (lo != 0 ? 1ull : 0ull);
+}
+template <bool H>
+HE_HD u64 mont_reduce_c(u128 acc, u64 p, u64 ninv) { return H ? mont_reduce_h(acc, p) : mont_reduce(acc, p, ninv); }
 
 // Product Barrett: (hi:lo) mod p for values < 4 p^2, p < 2^61 (tensor products and sums of two of them).
 // s = bits(p) - 2, mu = floor(2^(s+64) / p).  Result canonical.

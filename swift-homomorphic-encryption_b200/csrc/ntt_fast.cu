@@ -12,7 +12,8 @@
 //      bulk group per row; a buffer is refilled once the copy engine has read it.
 // NARROW / MID / WIDE rows (different lazy-reduction schedules) are mixed in one launch: the row's class selects the
 // instruction stream, rows are ordered class-major so all CTAs walk the classes in step, and there is one tail per
-// NTT call instead of one per class.
+// NTT call instead of one per class.  Each kernel is compiled for a class set (ntt_fast.cuh): the all-class set, and at
+// N = 2^13 also NARROW + NARROW-H for the multiply's rows.
 #include <cuda.h>
 
 #include <mutex>
@@ -143,6 +144,25 @@ __device__ __forceinline__ void inv_row(u64 *sm, int tau, const RowMod &m) {
     inv_row_pass<LOGN, CLS, P - 1>(x, sm, tau, m);
 }
 
+// the instruction stream of a row of class `cls` among the streams of the class set CLASSES (ntt_fast.cuh); a row whose
+// class is not in the set is a launcher error, except NARROW-H, which takes NARROW's stream when the set lacks its own
+template <int LOGN, unsigned CLASSES>
+__device__ __forceinline__ void fwd_row_of(int cls, u64 *sm, int tau, const RowMod &m, bool reduce_in) {
+    if (has_class(CLASSES, kNarrowH) && cls == kNarrowH) fwd_row<LOGN, kNarrowH>(sm, tau, m, reduce_in);
+    else if (has_class(CLASSES, kNarrow) && narrow_like(cls)) fwd_row<LOGN, kNarrow>(sm, tau, m, reduce_in);
+    else if (has_class(CLASSES, kSmall) && cls == kSmall) fwd_row<LOGN, kSmall>(sm, tau, m, reduce_in);
+    else if (has_class(CLASSES, kMid) && cls == kMid) fwd_row<LOGN, kMid>(sm, tau, m, reduce_in);
+    else if (has_class(CLASSES, kWide)) fwd_row<LOGN, kWide>(sm, tau, m, reduce_in);
+}
+template <int LOGN, unsigned CLASSES>
+__device__ __forceinline__ void inv_row_of(int cls, u64 *sm, int tau, const RowMod &m) {
+    if (has_class(CLASSES, kNarrowH) && cls == kNarrowH) inv_row<LOGN, kNarrowH>(sm, tau, m);
+    else if (has_class(CLASSES, kNarrow) && narrow_like(cls)) inv_row<LOGN, kNarrow>(sm, tau, m);
+    else if (has_class(CLASSES, kSmall) && cls == kSmall) inv_row<LOGN, kSmall>(sm, tau, m);
+    else if (has_class(CLASSES, kMid) && cls == kMid) inv_row<LOGN, kMid>(sm, tau, m);
+    else if (has_class(CLASSES, kWide)) inv_row<LOGN, kWide>(sm, tau, m);
+}
+
 // Row buffers of a CTA.  With one CTA per SM (N = 2^13) nothing else on the SM runs while the CTA waits for its copies,
 // so the next row's TMA-in and the previous row's TMA-out run under the current row's butterflies (C2 on H100 at a
 // 400 W power limit: +4 % over one buffer; three buffers measured 1-2 % behind two).  With several CTAs per SM
@@ -163,7 +183,7 @@ constexpr size_t ntt_smem_bytes() {
 // the 64-register budget beat 80 and 128 registers by 3-4 % (C1, C2-u32).
 constexpr int ntt_min_ctas(int logn) { return logn == 13 ? 1 : 1024 / ((1 << logn) / 16); }
 
-template <int LOGN, bool INVERSE>
+template <int LOGN, bool INVERSE, unsigned CLASSES>
 __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
     ntt_rows_kernel(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_out,
                     const ModSlot *__restrict__ slots, const __grid_constant__ RowList rl, const int polys,
@@ -254,20 +274,8 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
         if (debug_flags & 4) {  // experiments: data movement only
         } else
 #ifndef HE_EXPERIMENT_ONLY_CLASS
-        if (INVERSE) {
-            if (kNarrowHEnabled && cls == kNarrowH) inv_row<LOGN, kNarrowHEnabled ? kNarrowH : kNarrow>(sm, tau, m);
-            else if (cls == kNarrow) inv_row<LOGN, kNarrow>(sm, tau, m);
-            else if (cls == kSmall) inv_row<LOGN, kSmall>(sm, tau, m);
-            else if (cls == kMid) inv_row<LOGN, kMid>(sm, tau, m);
-            else inv_row<LOGN, kWide>(sm, tau, m);
-        } else {
-            const bool reduce_in = (flags & 8) != 0;
-            if (kNarrowHEnabled && cls == kNarrowH) fwd_row<LOGN, kNarrowHEnabled ? kNarrowH : kNarrow>(sm, tau, m, reduce_in);
-            else if (cls == kNarrow) fwd_row<LOGN, kNarrow>(sm, tau, m, reduce_in);
-            else if (cls == kSmall) fwd_row<LOGN, kSmall>(sm, tau, m, reduce_in);
-            else if (cls == kMid) fwd_row<LOGN, kMid>(sm, tau, m, reduce_in);
-            else fwd_row<LOGN, kWide>(sm, tau, m, reduce_in);
-        }
+        if (INVERSE) inv_row_of<LOGN, CLASSES>(cls, sm, tau, m);
+        else fwd_row_of<LOGN, CLASSES>(cls, sm, tau, m, (flags & 8) != 0);
 #else  // register-pressure experiments: one class only
         if (INVERSE) inv_row<LOGN, HE_EXPERIMENT_ONLY_CLASS>(sm, tau, m);
         else fwd_row<LOGN, HE_EXPERIMENT_ONLY_CLASS>(sm, tau, m, (flags & 8) != 0);
@@ -319,8 +327,10 @@ __device__ __forceinline__ ulonglong2 ld_cluster_v2(u32 addr) {
     asm volatile("ld.shared::cluster.v2.u64 {%0, %1}, [%2];" : "=l"(v.x), "=l"(v.y) : "r"(addr) : "memory");
     return v;
 }
-// a b 2^-64 mod p, canonical (behz.cu:tensor_kernel's arithmetic: the inverse NTT's kScaleTMont restores the 2^64)
-__device__ __forceinline__ u64 mont_product(u64 a, u64 b, u64 p, u64 ninv) { return csub(mont_reduce((u128)a * b, p, ninv), p); }
+// a b 2^-64 mod p, canonical (behz.cu:tensor_kernel's arithmetic: the inverse NTT's kScaleTMont restores the 2^64);
+// H: p = h 2^32 + 1 (mont_reduce_h, the same value)
+template <bool H>
+__device__ __forceinline__ u64 mont_product(u64 a, u64 b, u64 p, u64 ninv) { return csub(mont_reduce_c<H>((u128)a * b, p, ninv), p); }
 
 // The N = 2^13 ct x ct multiply's forward NTT and tensor product (Bfv+Multiply.swift:51-57, :80-82) in one kernel, so
 // the 4 R transformed operand rows of a pair never go to HBM.  A task is one (pair, row r of [Q, aux]); tasks are
@@ -346,14 +356,42 @@ constexpr size_t ntt_tensor_smem_bytes() {
     return sizeof(u64) * 2 * ((size_t)1 << LOGN) + sizeof(ulonglong2) * ((size_t)1 << (LOGN - 4)) + sizeof(u64) * 3;
 }
 
-template <int LOGN>
+// The tensor step of one task: c0 (rank 0) or c2 (rank 1) from this CTA's rows x = a_rank, y = b_rank, then, once the
+// peer's rows are final, this CTA's half of the columns of c1.  H: the row's prime is h 2^32 + 1.
+template <int LOGN, bool H>
+__device__ __forceinline__ void tensor_step(const u64 *x, const u64 *y, u64 *out, int64_t comp, u32 rank, int tau, u64 p, u64 ninv) {
+    constexpr int N = 1 << LOGN, T = N / 16;
+    u64 *own = out + (rank ? 2 * comp : 0);  // c0 (rank 0) or c2 (rank 1): this CTA's rows only
+#pragma unroll 4
+    for (int w = 2 * tau; w < N; w += 2 * T) {
+        const ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(x + w), b = *reinterpret_cast<const ulonglong2 *>(y + w);
+        *reinterpret_cast<ulonglong2 *>(own + smem_phys(w)) =
+            make_ulonglong2(mont_product<H>(a.x, b.x, p, ninv), mont_product<H>(a.y, b.y, p, ninv));
+    }
+    cluster_wait();  // the peer's rows are final
+    // c1 = a0 b1 + a1 b0 = x Y + X y over this CTA's half of the columns (X, Y: the peer's rows), summed at 128 bits
+    // before its one reduction
+    const u32 px = cluster_map(smem_u32(x), rank ^ 1), py = cluster_map(smem_u32(y), rank ^ 1);
+#pragma unroll 4
+    for (int w = (int)rank * (N / 2) + 2 * tau; w < ((int)rank + 1) * (N / 2); w += 2 * T) {
+        const ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(x + w), b = *reinterpret_cast<const ulonglong2 *>(y + w);
+        const ulonglong2 A = ld_cluster_v2(px + 8u * w), Bv = ld_cluster_v2(py + 8u * w);
+        u128 m0 = (u128)a.x * Bv.x, m1 = (u128)a.y * Bv.y;
+        mac128(m0, A.x, b.x);
+        mac128(m1, A.y, b.y);
+        *reinterpret_cast<ulonglong2 *>(out + comp + smem_phys(w)) =
+            make_ulonglong2(csub(mont_reduce_c<H>(m0, p, ninv), p), csub(mont_reduce_c<H>(m1, p, ninv), p));
+    }
+}
+
+template <int LOGN, unsigned CLASSES>
 __global__ void __launch_bounds__((1 << LOGN) / 16, 1)
     ntt_forward_tensor_kernel(const __grid_constant__ CUtensorMap map_lhs, const __grid_constant__ CUtensorMap map_rhs,
                               const __grid_constant__ CUtensorMap map_ext, u64 *__restrict__ ten,
                               const ModSlot *__restrict__ slots, const __grid_constant__ RowList rl, const int items,
                               const int L) {
     extern __shared__ __align__(1024) u64 smem[];  // row buffers first: the 128-byte swizzle wants them 1024-byte aligned
-    constexpr int N = 1 << LOGN, T = N / 16;
+    constexpr int N = 1 << LOGN;
     constexpr int kBoxes = N / kLineWords / kBoxLines;
     constexpr u32 kRowBytes = (u32)sizeof(u64) << LOGN, kTwBytes = (u32)sizeof(ulonglong2) << (LOGN - 4);
     static_assert(kBoxes >= 1, "one row is at least one box");
@@ -426,41 +464,16 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, 1)
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
             mbar_wait(&bar_row[j], phase_row);
-            u64 *sm = smem + j * N;
-            if (kNarrowHEnabled && cls == kNarrowH) fwd_row<LOGN, kNarrowHEnabled ? kNarrowH : kNarrow>(sm, tau, m, false);
-            else if (cls == kNarrow) fwd_row<LOGN, kNarrow>(sm, tau, m, false);
-            else if (cls == kSmall) fwd_row<LOGN, kSmall>(sm, tau, m, false);
-            else if (cls == kMid) fwd_row<LOGN, kMid>(sm, tau, m, false);
-            else fwd_row<LOGN, kWide>(sm, tau, m, false);
+            fwd_row_of<LOGN, CLASSES>(cls, smem + j * N, tau, m, false);
         }
         phase_row ^= 1;
         // ---- tensor step
         __syncthreads();
         cluster_arrive();  // this CTA's two rows are final
-        const u64 p = S.p, ninv = S.ninv;
-        const u64 *x = smem, *y = smem + N;  // a_rank, b_rank
-        const int64_t comp = (int64_t)R * N;                   // words between the components of ten
+        const int64_t comp = (int64_t)R * N;  // words between the components of ten
         u64 *out = ten + ((int64_t)3 * item * R + r) * N;
-        u64 *own = out + (rank ? 2 * comp : 0);  // c0 (rank 0) or c2 (rank 1): this CTA's rows only
-#pragma unroll 4
-        for (int w = 2 * tau; w < N; w += 2 * T) {
-            const ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(x + w), b = *reinterpret_cast<const ulonglong2 *>(y + w);
-            *reinterpret_cast<ulonglong2 *>(own + smem_phys(w)) = make_ulonglong2(mont_product(a.x, b.x, p, ninv), mont_product(a.y, b.y, p, ninv));
-        }
-        cluster_wait();  // the peer's rows are final
-        // c1 = a0 b1 + a1 b0 = x Y + X y over this CTA's half of the columns (X, Y: the peer's rows), summed at 128 bits
-        // before its one reduction
-        const u32 px = cluster_map(smem_u32(x), rank ^ 1), py = cluster_map(smem_u32(y), rank ^ 1);
-#pragma unroll 4
-        for (int w = (int)rank * (N / 2) + 2 * tau; w < ((int)rank + 1) * (N / 2); w += 2 * T) {
-            const ulonglong2 a = *reinterpret_cast<const ulonglong2 *>(x + w), b = *reinterpret_cast<const ulonglong2 *>(y + w);
-            const ulonglong2 A = ld_cluster_v2(px + 8u * w), Bv = ld_cluster_v2(py + 8u * w);
-            u128 m0 = (u128)a.x * Bv.x, m1 = (u128)a.y * Bv.y;
-            mac128(m0, A.x, b.x);
-            mac128(m1, A.y, b.y);
-            *reinterpret_cast<ulonglong2 *>(out + comp + smem_phys(w)) =
-                make_ulonglong2(csub(mont_reduce(m0, p, ninv), p), csub(mont_reduce(m1, p, ninv), p));
-        }
+        if (has_class(CLASSES, kNarrowH) && cls == kNarrowH) tensor_step<LOGN, true>(smem, smem + N, out, comp, rank, tau, S.p, S.ninv);
+        else tensor_step<LOGN, false>(smem, smem + N, out, comp, rank, tau, S.p, S.ninv);
         // the generic-proxy accesses to these buffers come before their next TMA refill
         fence_proxy_async_smem();
         cluster_arrive_relaxed();  // this CTA has finished reading the peer's rows (waited for before the next refill / exit)
@@ -526,21 +539,28 @@ static bool make_line_map(CUtensorMap *map, const u64 *base, int logn) {
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int LOGN, bool INVERSE>
-static cudaError_t launch_logn(const Context &ctx, const NttRowMap &map, const u64 *in, u64 *out, int64_t rows,
+// Whether a launch has NARROW-H rows and every other row is NARROW: at N = 2^13 such launches (the multiply's [Q, aux]
+// rows) run the kernels compiled for kNarrowClasses.  Launches of NARROW rows alone keep the all-class kernels: the
+// two-class kernel measured 0.5-0.9 % slower on them (C2 with plain auxiliary primes, C1-8192; DESIGN.md section 4).
+// Other sizes have the all-class kernels only.
+static bool narrow_h_rows(const RowList &rl) {
+    bool any_h = false;
+    for (int i = 0; i < rl.count; ++i) {
+        const int cls = rl.flags[i] & 7;
+        if (!narrow_like(cls)) return false;
+        any_h |= cls == kNarrowH;
+    }
+    return any_h;
+}
+
+template <int LOGN, bool INVERSE, unsigned CLASSES>
+static cudaError_t launch_rows(const Context &ctx, const RowList &rl, const u64 *in, u64 *out, int polys, int64_t rows,
                                int scale_mode, cudaStream_t stream) {
-    if (rows % map.rows_per_poly) return cudaErrorInvalidValue;
-    if (rows == 0) return cudaSuccess;
-    if (rows > 0x7fffffffLL) return cudaErrorInvalidValue;
-    RowList rl;
-    build_row_list(ctx, map, INVERSE, rl);
-    if (rl.src_poly_stride % kLineWords) return cudaErrorInvalidValue;
     CUtensorMap map_in, map_out;
     if (!make_line_map(&map_in, in, LOGN) || !make_line_map(&map_out, out, LOGN)) return cudaErrorInvalidValue;
-    const int polys = (int)(rows / map.rows_per_poly);
     constexpr int threads = (1 << LOGN) / 16;
     constexpr size_t smem = ntt_smem_bytes<LOGN>();
-    auto k = ntt_rows_kernel<LOGN, INVERSE>;
+    auto k = ntt_rows_kernel<LOGN, INVERSE, CLASSES>;
     static int ctas_per_sm[64] = {0};  // per instantiation and device
     static std::mutex mu;
     int per_sm;
@@ -565,6 +585,21 @@ static cudaError_t launch_logn(const Context &ctx, const NttRowMap &map, const u
     }();
     k<<<(unsigned)grid, threads, smem, stream>>>(map_in, map_out, ctx.d_slots, rl, polys, scale_mode, debug_flags);
     return cudaGetLastError();
+}
+
+template <int LOGN, bool INVERSE>
+static cudaError_t launch_logn(const Context &ctx, const NttRowMap &map, const u64 *in, u64 *out, int64_t rows,
+                               int scale_mode, cudaStream_t stream) {
+    if (rows % map.rows_per_poly) return cudaErrorInvalidValue;
+    if (rows == 0) return cudaSuccess;
+    if (rows > 0x7fffffffLL) return cudaErrorInvalidValue;
+    RowList rl;
+    build_row_list(ctx, map, INVERSE, rl);
+    if (rl.src_poly_stride % kLineWords) return cudaErrorInvalidValue;
+    const int polys = (int)(rows / map.rows_per_poly);
+    if (LOGN == 13 && narrow_h_rows(rl))
+        return launch_rows<LOGN, INVERSE, (LOGN == 13 ? kNarrowClasses : kAllClasses)>(ctx, rl, in, out, polys, rows, scale_mode, stream);
+    return launch_rows<LOGN, INVERSE, kAllClasses>(ctx, rl, in, out, polys, rows, scale_mode, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- N = 2^15
@@ -668,7 +703,7 @@ static cudaError_t launch_split(const Context &ctx, const NttRowMap &map, const 
     {
         constexpr int threads = (1 << LOGN) / 16;
         constexpr size_t smem = ntt_smem_bytes<LOGN>();
-        auto k = ntt_rows_kernel<LOGN, INVERSE>;
+        auto k = ntt_rows_kernel<LOGN, INVERSE, kAllClasses>;
         cudaError_t e;
         if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
         int per_sm = 0;
@@ -712,21 +747,16 @@ cudaError_t launch_ntt_inverse_fast(const Context &ctx, const NttRowMap &map, co
     return launch_fast<true>(ctx, map, in, out, rows, scale_mode, stream);
 }
 
-cudaError_t launch_ntt_forward_tensor(const Context &ctx, const NttRowMap &map, const u64 *lhs, const u64 *rhs,
-                                      const u64 *ext, u64 *ten, int64_t items, cudaStream_t stream) {
+template <unsigned CLASSES>
+static cudaError_t launch_forward_tensor(const Context &ctx, const RowList &rl, const u64 *lhs, const u64 *rhs,
+                                         const u64 *ext, u64 *ten, int64_t items, cudaStream_t stream) {
     constexpr int LOGN = 13;
-    if (ctx.logn != LOGN) return cudaErrorInvalidValue;
-    if (items == 0) return cudaSuccess;
-    // every line index of ext (the largest buffer read) fits an int
-    if (items * 4 * map.rows_per_poly * (ctx.n / kLineWords) > 0x7fffffffLL) return cudaErrorInvalidValue;
-    RowList rl;
-    build_row_list(ctx, map, false, rl);
     CUtensorMap map_lhs, map_rhs, map_ext;
     if (!make_line_map(&map_lhs, lhs, LOGN) || !make_line_map(&map_rhs, rhs, LOGN) || !make_line_map(&map_ext, ext, LOGN))
         return cudaErrorInvalidValue;
     constexpr int threads = (1 << LOGN) / 16;
     constexpr size_t smem = ntt_tensor_smem_bytes<LOGN>();
-    auto k = ntt_forward_tensor_kernel<LOGN>;
+    auto k = ntt_forward_tensor_kernel<LOGN, CLASSES>;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2;
@@ -760,6 +790,18 @@ cudaError_t launch_ntt_forward_tensor(const Context &ctx, const NttRowMap &map, 
     ++g_kernel_launches;
     cudaError_t e = cudaLaunchKernelEx(&cfg, k, map_lhs, map_rhs, map_ext, ten, (const ModSlot *)ctx.d_slots, rl, (int)items, ctx.L);
     return e != cudaSuccess ? e : cudaGetLastError();
+}
+
+cudaError_t launch_ntt_forward_tensor(const Context &ctx, const NttRowMap &map, const u64 *lhs, const u64 *rhs,
+                                      const u64 *ext, u64 *ten, int64_t items, cudaStream_t stream) {
+    if (ctx.logn != 13) return cudaErrorInvalidValue;
+    if (items == 0) return cudaSuccess;
+    // every line index of ext (the largest buffer read) fits an int
+    if (items * 4 * map.rows_per_poly * (ctx.n / kLineWords) > 0x7fffffffLL) return cudaErrorInvalidValue;
+    RowList rl;
+    build_row_list(ctx, map, false, rl);
+    if (narrow_h_rows(rl)) return launch_forward_tensor<kNarrowClasses>(ctx, rl, lhs, rhs, ext, ten, items, stream);
+    return launch_forward_tensor<kAllClasses>(ctx, rl, lhs, rhs, ext, ten, items, stream);
 }
 
 }  // namespace hecuda

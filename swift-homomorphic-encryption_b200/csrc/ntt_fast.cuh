@@ -63,17 +63,19 @@ HE_HD constexpr int class_of_bits(int bits) {
 }
 // NARROW primes of the form h 2^32 + 1 (the auxiliary primes context.cu picks for the multiply): the q p product of a
 // Shoup multiplication collapses to q + ((q0 h) << 32)
-// Compiled in only with -DHE_NTT_NARROW_H: a fifth instruction stream in the kernel slowed the NARROW rows by about
-// what the NARROW-H rows of the multiply's auxiliary base gained.
-#if defined(HE_NTT_NARROW_H)
-constexpr bool kNarrowHEnabled = true;
-#else
-constexpr bool kNarrowHEnabled = false;
-#endif
 HE_HD constexpr int class_of_modulus(u64 p, int bits) {
-    return (kNarrowHEnabled && class_of_bits(bits) == kNarrow && (u32)p == 1u) ? kNarrowH : class_of_bits(bits);
+    return (class_of_bits(bits) == kNarrow && (u32)p == 1u) ? kNarrowH : class_of_bits(bits);
 }
 HE_HD constexpr bool narrow_like(int cls) { return cls == kNarrow || cls == kNarrowH; }
+
+// Class sets: the instruction streams one kernel instantiation carries (ntt_fast.cu).  Every class's passes are fully
+// unrolled, so each stream costs several thousand instructions of code.  The all-class kernels carry no NARROW-H stream:
+// there a NARROW-H row runs NARROW's butterflies, which are valid for every p < 2^55.  The N = 2^13 multiply's rows
+// ([Q, aux] with 55-bit q_i and h 2^32 + 1 auxiliary primes) get a kernel with just the two streams they use.
+HE_HD constexpr unsigned class_bit(int cls) { return 1u << cls; }
+constexpr unsigned kAllClasses = (1u << kNarrow) | (1u << kMid) | (1u << kWide) | (1u << kSmall);
+constexpr unsigned kNarrowClasses = (1u << kNarrow) | (1u << kNarrowH);
+HE_HD constexpr bool has_class(unsigned set, int cls) { return (set & class_bit(cls)) != 0; }
 
 // ---- pass plans: stage counts of the forward passes, in execution order; the inverse runs the mirrored list
 HE_HD constexpr int plan_passes(int logn) { return logn <= 12 ? 3 : 4; }
