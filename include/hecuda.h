@@ -238,6 +238,48 @@ int32_t hecuda_plaintext_to_eval(const hecuda_context *ctx, const uint64_t *plai
 int32_t hecuda_plaintext_to_eval_device(const hecuda_context *ctx, const uint64_t *plain, int32_t moduli_count,
                                         uint64_t *out, int64_t count, void *stream);
 
+/* ---- the plaintext side of Bfv: SIMD batching and ciphertext +- plaintext ----
+ * Context.supportsSimdEncoding (Context.swift:63-65): the plaintext modulus t is a prime = 1 mod 2N (isNttModulus,
+ * PolyRq+Ntt.swift:24-27).  Such a context also holds t's NTT tables (Context.plaintextContext), so
+ * hecuda_ntt_forward_rows / hecuda_ntt_inverse_rows and hecuda_context_root_tables accept `modulus` = t. */
+int32_t hecuda_context_supports_simd(const hecuda_context *ctx, int32_t *supported);
+/* Context.encode(values:format: .simd) (Encoding.swift:197-235, encodeSimd) and, with moduli_count = l >= 1,
+ * Bfv.encode(context:values:format:moduliCount:) (Bfv+Encode.swift:45-50, + Plaintext.convertToEvalFormat).
+ * values: count x value_count (value_count <= N, each < t; slots past value_count are zero).  moduli_count 0 -> out
+ * count x N Coeff plaintexts; l in [1, L] -> out count x l x N Eval plaintexts.  HECUDA_ERR_UNSUPPORTED without SIMD
+ * support (HeError.simdEncodingNotSupported); value_count > N (encodingDataCountExceedsLimit) or, on the host entry
+ * point, a value >= t (encodingDataOutOfBounds, Encoding.swift:147-156) -> HECUDA_ERR_INVALID_ARGUMENT.  The _device
+ * variant takes values < t as a precondition. */
+int32_t hecuda_bfv_encode_simd(const hecuda_context *ctx, const uint64_t *values, int32_t value_count,
+                               int32_t moduli_count, uint64_t *out, int64_t count);
+int32_t hecuda_bfv_encode_simd_device(const hecuda_context *ctx, const uint64_t *values, int32_t value_count,
+                                      int32_t moduli_count, uint64_t *out, int64_t count, void *stream);
+/* Context.decode(plaintext:format: .simd) (Encoding.swift:237-245, decodeSimd) and Bfv.decodeEval (Bfv+Encode.swift:76-80,
+ * Plaintext.convertToCoeffFormat, Plaintext.swift:176-194).  moduli_count 0: plaintexts count x N Coeff (< t);
+ * l in [1, L]: count x l x N Eval plaintexts.  values: count x N slots in [0, t). */
+int32_t hecuda_bfv_decode_simd(const hecuda_context *ctx, const uint64_t *plaintexts, int32_t moduli_count,
+                               uint64_t *values, int64_t count);
+int32_t hecuda_bfv_decode_simd_device(const hecuda_context *ctx, const uint64_t *plaintexts, int32_t moduli_count,
+                                      uint64_t *values, int64_t count, void *stream);
+/* Bfv.addAssignCoeff / subAssignCoeff (Bfv/Bfv.swift:110-117) and HeScheme.subCoeff (plaintext - ciphertext,
+ * HeScheme.swift:1540-1542 = plaintext + -ciphertext): plaintextTranslate (Bfv+Encrypt.swift:75-139) adds or subtracts
+ * floor(Q/t) m + floor(([Q]_t m + ceil(t/2)) / t) on poly 0, Q = q_0..q_{l-1}.  ADD and SUB change poly 0 only; SUB_FROM
+ * gives [that - c_0] on poly 0 and negates the other polys.  ct, out: batch x poly_count x l x N (Coeff, poly_count 2
+ * or 3, l = moduli_count in [1, L], correction factor 1: the caller refuses others, HeError.invalidCorrectionFactor,
+ * Bfv+Encrypt.swift:80-82); plaintexts: plaintext_count x N coefficients < t, plaintext_count 1 (shared by every
+ * ciphertext) or batch; out may equal ct.  The host entry point refuses a coefficient >= t; the _device variant takes
+ * it as a precondition.  Works whether or not the context supports SIMD encoding.  Eval-format ciphertext +- plaintext
+ * is not offered: the reference throws unsupportedHeOperation (Bfv.swift:153-160). */
+#define HECUDA_PLAINTEXT_ADD 0      /* ct + pt */
+#define HECUDA_PLAINTEXT_SUB 1      /* ct - pt */
+#define HECUDA_PLAINTEXT_SUB_FROM 2 /* pt - ct */
+int32_t hecuda_bfv_plaintext_translate(const hecuda_context *ctx, const uint64_t *ct, int32_t poly_count,
+                                       int32_t moduli_count, const uint64_t *plaintexts, int64_t plaintext_count,
+                                       int32_t op, uint64_t *out, int64_t batch);
+int32_t hecuda_bfv_plaintext_translate_device(const hecuda_context *ctx, const uint64_t *ct, int32_t poly_count,
+                                              int32_t moduli_count, const uint64_t *plaintexts, int64_t plaintext_count,
+                                              int32_t op, uint64_t *out, int64_t batch, void *stream);
+
 /* ---- MulPir index-PIR server (SURVEY.md section 8f, rank 3) ----
  * Device-resident ProcessedDatabase: `count` optional plaintexts in the order MulPirServer.process emits them
  * (IndexPir/MulPir.swift:433-556: chunk-major, then column-major over the first dimension).  plaintexts is
@@ -424,6 +466,13 @@ int32_t hecuda_u32_bfv_inner_product(const hecuda_context *ctx, const uint32_t *
                                      int64_t pair_count, int64_t group_count);
 int32_t hecuda_u32_rnstool_lift_q_to_qbsk(const hecuda_context *ctx, const uint32_t *polys, uint32_t *out, int64_t poly_count);
 int32_t hecuda_u32_rnstool_floor_qbsk_to_q(const hecuda_context *ctx, const uint32_t *polys, uint32_t *out, int64_t poly_count);
+int32_t hecuda_u32_bfv_encode_simd(const hecuda_context *ctx, const uint32_t *values, int32_t value_count,
+                                   int32_t moduli_count, uint32_t *out, int64_t count);
+int32_t hecuda_u32_bfv_decode_simd(const hecuda_context *ctx, const uint32_t *plaintexts, int32_t moduli_count,
+                                   uint32_t *values, int64_t count);
+int32_t hecuda_u32_bfv_plaintext_translate(const hecuda_context *ctx, const uint32_t *ct, int32_t poly_count,
+                                           int32_t moduli_count, const uint32_t *plaintexts, int64_t plaintext_count,
+                                           int32_t op, uint32_t *out, int64_t batch);
 
 #ifdef __cplusplus
 }

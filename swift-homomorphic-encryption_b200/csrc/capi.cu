@@ -1070,6 +1070,194 @@ int32_t hecuda_plaintext_to_eval(const hecuda_context *h, const uint64_t *plain,
                          });
 }
 
+// ---------------------------------------------------------------- plaintext side: SIMD encode / decode, ct +- pt
+
+int32_t hecuda_context_supports_simd(const hecuda_context *h, int32_t *supported) {
+    if (!h || !h->ctx || !supported) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *supported = h->ctx->simd ? 1 : 0;
+    return HECUDA_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+int32_t need_simd(const hecuda_context *h) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (!h->ctx->simd)
+        return fail(HECUDA_ERR_UNSUPPORTED, "simdEncodingNotSupported: the plaintext modulus is not a prime = 1 mod 2N");
+    return HECUDA_OK;
+}
+
+// encodingDataOutOfBounds (Encoding.swift:147-156): host buffers of uint64 (or uint32 inside a hecuda_u32_ call)
+bool host_values_below(const void *p, size_t count, u64 t) {
+    if (tl_io32) {
+        const uint32_t *v = static_cast<const uint32_t *>(p);
+        return std::all_of(v, v + count, [t](uint32_t x) { return x < t; });
+    }
+    const uint64_t *v = static_cast<const uint64_t *>(p);
+    return std::all_of(v, v + count, [t](uint64_t x) { return x < t; });
+}
+
+int32_t check_encode(const hecuda_context *h, const void *values, int32_t value_count, int32_t l, const void *out,
+                     int64_t count) {
+    int32_t rc = need_simd(h);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    if (value_count < 0 || value_count > c.n)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "encodingDataCountExceedsLimit: value_count must be in [0, N]");
+    if (l < 0 || l > c.L) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidPolyContext: moduli_count must be in [0, L]");
+    if (count < 0 || (count && (!out || (value_count && !values)))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null buffer");
+    return HECUDA_OK;
+}
+
+int32_t check_decode(const hecuda_context *h, const void *plain, int32_t l, const void *values, int64_t count) {
+    int32_t rc = need_simd(h);
+    if (rc) return rc;
+    if (l < 0 || l > h->ctx->L) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidPolyContext: moduli_count must be in [0, L]");
+    if (count < 0 || (count && (!plain || !values))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null buffer");
+    return HECUDA_OK;
+}
+
+int32_t check_translate(const hecuda_context *h, const void *ct, int32_t polys, int32_t l, const void *pt, int64_t pt_count,
+                        int32_t op, const void *out, int64_t batch) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (polys < 2 || polys > 3) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: poly_count must be 2 or 3");
+    if (l < 1 || l > h->ctx->L) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: moduli_count must be in [1, L]");
+    if (op < HECUDA_PLAINTEXT_ADD || op > HECUDA_PLAINTEXT_SUB_FROM) return fail(HECUDA_ERR_INVALID_ARGUMENT, "unknown op");
+    if (batch < 0) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: negative batch");
+    if (pt_count != 1 && pt_count != batch)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "incompatibleCiphertextAndPlaintext: plaintext_count must be 1 or batch");
+    if (batch && (!ct || !pt || !out)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null buffer");
+    return HECUDA_OK;
+}
+
+// items per device-side chunk of the encode / decode pipelines: scratch of at most 2^25 words
+int64_t simd_chunk(const Context &c) { return std::max<int64_t>(1, ((int64_t)1 << 25) / c.n); }
+
+}  // namespace
+
+extern "C" {
+
+int32_t hecuda_bfv_encode_simd_device(const hecuda_context *h, const uint64_t *values, int32_t value_count,
+                                      int32_t moduli_count, uint64_t *out, int64_t count, void *stream) {
+    int32_t rc = check_encode(h, values, value_count, moduli_count, out, count);
+    if (rc || count == 0) return rc;
+    const Context &c = *h->ctx;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int64_t chunk = std::min<int64_t>(simd_chunk(c), count);
+    const size_t scratch_words = simd_scratch_words(c, true, moduli_count) * (size_t)chunk;
+    u64 *scratch = nullptr;
+    if (scratch_words) CK(cudaMallocAsync(&scratch, scratch_words * sizeof(u64), s));
+    const int64_t out_words = (int64_t)(moduli_count ? moduli_count : 1) * c.n;
+    cudaError_t e = cudaSuccess;
+    for (int64_t done = 0; e == cudaSuccess && done < count; done += chunk)
+        e = launch_encode_simd(c, (const u64 *)values + done * value_count, value_count, moduli_count,
+                               (u64 *)out + done * out_words, scratch, std::min<int64_t>(chunk, count - done), s);
+    if (scratch) cudaFreeAsync(scratch, s);
+    return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "encodeSimd");
+}
+
+int32_t hecuda_bfv_encode_simd(const hecuda_context *h, const uint64_t *values, int32_t value_count, int32_t moduli_count,
+                               uint64_t *out, int64_t count) {
+    int32_t rc = check_encode(h, values, value_count, moduli_count, out, count);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    if (!host_values_below(values, (size_t)count * value_count, c.t))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "encodingDataOutOfBounds: values must be below the plaintext modulus");
+    const int l = moduli_count;
+    std::vector<HostIo> in;
+    if (value_count) in.push_back({(const u64 *)values, (size_t)value_count});
+    const size_t out_words = (size_t)(l ? l : 1) * c.n;
+    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / out_words));
+    return host_pipeline(h, count, chunk, simd_scratch_words(c, true, l), in, (u64 *)out, out_words,
+                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
+                             return launch_encode_simd(c, d_in.empty() ? nullptr : d_in[0], value_count, l, d_out, w.buf[0],
+                                                       items, w.stream);
+                         });
+}
+
+int32_t hecuda_bfv_decode_simd_device(const hecuda_context *h, const uint64_t *plaintexts, int32_t moduli_count,
+                                      uint64_t *values, int64_t count, void *stream) {
+    int32_t rc = check_decode(h, plaintexts, moduli_count, values, count);
+    if (rc || count == 0) return rc;
+    const Context &c = *h->ctx;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int64_t chunk = std::min<int64_t>(simd_chunk(c), count);
+    u64 *scratch = nullptr;
+    CK(cudaMallocAsync(&scratch, simd_scratch_words(c, false, moduli_count) * (size_t)chunk * sizeof(u64), s));
+    const int64_t in_words = (int64_t)(moduli_count ? moduli_count : 1) * c.n;
+    cudaError_t e = cudaSuccess;
+    for (int64_t done = 0; e == cudaSuccess && done < count; done += chunk)
+        e = launch_decode_simd(c, (const u64 *)plaintexts + done * in_words, moduli_count, (u64 *)values + done * c.n, scratch,
+                               std::min<int64_t>(chunk, count - done), s);
+    cudaFreeAsync(scratch, s);
+    return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "decodeSimd");
+}
+
+int32_t hecuda_bfv_decode_simd(const hecuda_context *h, const uint64_t *plaintexts, int32_t moduli_count, uint64_t *values,
+                               int64_t count) {
+    int32_t rc = check_decode(h, plaintexts, moduli_count, values, count);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    const int l = moduli_count;
+    const size_t in_words = (size_t)(l ? l : 1) * c.n;
+    std::vector<HostIo> in = {{(const u64 *)plaintexts, in_words}};
+    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / in_words));
+    return host_pipeline(h, count, chunk, simd_scratch_words(c, false, l), in, (u64 *)values, (size_t)c.n,
+                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
+                             return launch_decode_simd(c, d_in[0], l, d_out, w.buf[0], items, w.stream);
+                         });
+}
+
+int32_t hecuda_bfv_plaintext_translate_device(const hecuda_context *h, const uint64_t *ct, int32_t poly_count,
+                                              int32_t moduli_count, const uint64_t *plaintexts, int64_t plaintext_count,
+                                              int32_t op, uint64_t *out, int64_t batch, void *stream) {
+    int32_t rc = check_translate(h, ct, poly_count, moduli_count, plaintexts, plaintext_count, op, out, batch);
+    if (rc) return rc;
+    cudaError_t e = launch_plaintext_translate(*h->ctx, (const u64 *)ct, poly_count, moduli_count, (const u64 *)plaintexts,
+                                               plaintext_count == 1, op, (u64 *)out, batch, (cudaStream_t)stream);
+    return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "plaintextTranslate");
+}
+
+int32_t hecuda_bfv_plaintext_translate(const hecuda_context *h, const uint64_t *ct, int32_t poly_count, int32_t moduli_count,
+                                       const uint64_t *plaintexts, int64_t plaintext_count, int32_t op, uint64_t *out,
+                                       int64_t batch) {
+    int32_t rc = check_translate(h, ct, poly_count, moduli_count, plaintexts, plaintext_count, op, out, batch);
+    if (rc || batch == 0) return rc;
+    const Context &c = *h->ctx;
+    if (!host_values_below(plaintexts, (size_t)plaintext_count * c.n, c.t))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "encodingDataOutOfBounds: plaintext coefficients must be below t");
+    const bool broadcast = plaintext_count == 1;
+    const int l = moduli_count;
+    const size_t ct_words = (size_t)poly_count * l * c.n;
+    std::vector<HostIo> in = {{(const u64 *)ct, ct_words}};
+    u64 *d_pt = nullptr;  // the shared plaintext, uploaded once
+    if (broadcast) {
+        std::vector<u64> pt(c.n);
+        if (tl_io32) std::copy((const uint32_t *)plaintexts, (const uint32_t *)plaintexts + c.n, pt.begin());
+        else std::copy(plaintexts, plaintexts + c.n, pt.begin());
+        CK(cudaMalloc(&d_pt, sizeof(u64) * (size_t)c.n));
+        cudaError_t e = upload(d_pt, pt.data(), sizeof(u64) * (size_t)c.n);
+        if (e != cudaSuccess) {
+            cudaFree(d_pt);
+            return cuda_fail(e, "plaintext upload");
+        }
+    } else {
+        in.push_back({(const u64 *)plaintexts, (size_t)c.n});
+    }
+    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / ct_words));
+    rc = host_pipeline(h, batch, chunk, 0, in, (u64 *)out, ct_words,
+                       [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
+                           return launch_plaintext_translate(c, d_in[0], poly_count, l, broadcast ? d_pt : d_in[1], broadcast,
+                                                             op, d_out, items, w.stream);
+                       });
+    if (d_pt) cudaFree(d_pt);
+    return rc;
+}
+
 // ---------------------------------------------------------------- ct x ct inner product (SURVEY.md 8f rank 2)
 
 static int32_t check_ipc(const hecuda_context *h, const uint64_t *lhs, const uint64_t *rhs, uint64_t *out, int64_t pairs,
@@ -1240,6 +1428,32 @@ int32_t hecuda_u32_rnstool_floor_qbsk_to_q(const hecuda_context *h, const uint32
     if (rc) return rc;
     Io32Scope scope;
     return hecuda_rnstool_floor_qbsk_to_q(h, reinterpret_cast<const uint64_t *>(polys), reinterpret_cast<uint64_t *>(out), count);
+}
+int32_t hecuda_u32_bfv_encode_simd(const hecuda_context *h, const uint32_t *values, int32_t value_count, int32_t moduli_count,
+                                   uint32_t *out, int64_t count) {
+    int32_t rc = need_word32(h);
+    if (rc) return rc;
+    Io32Scope scope;
+    return hecuda_bfv_encode_simd(h, reinterpret_cast<const uint64_t *>(values), value_count, moduli_count,
+                                  reinterpret_cast<uint64_t *>(out), count);
+}
+int32_t hecuda_u32_bfv_decode_simd(const hecuda_context *h, const uint32_t *plaintexts, int32_t moduli_count, uint32_t *values,
+                                   int64_t count) {
+    int32_t rc = need_word32(h);
+    if (rc) return rc;
+    Io32Scope scope;
+    return hecuda_bfv_decode_simd(h, reinterpret_cast<const uint64_t *>(plaintexts), moduli_count,
+                                  reinterpret_cast<uint64_t *>(values), count);
+}
+int32_t hecuda_u32_bfv_plaintext_translate(const hecuda_context *h, const uint32_t *ct, int32_t poly_count, int32_t moduli_count,
+                                           const uint32_t *plaintexts, int64_t plaintext_count, int32_t op, uint32_t *out,
+                                           int64_t batch) {
+    int32_t rc = need_word32(h);
+    if (rc) return rc;
+    Io32Scope scope;
+    return hecuda_bfv_plaintext_translate(h, reinterpret_cast<const uint64_t *>(ct), poly_count, moduli_count,
+                                          reinterpret_cast<const uint64_t *>(plaintexts), plaintext_count, op,
+                                          reinterpret_cast<uint64_t *>(out), batch);
 }
 
 }  // extern "C"

@@ -178,10 +178,13 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
     }
     c->aux_is_reference = c->aux == c->bsk;
 
-    // ---- NTT slots
-    const int nslots = c->aux_is_reference ? 2 * L + 2 : 3 * L + 3;
+    // ---- NTT slots.  The plaintext modulus gets one when it is NTT-friendly (SIMD encoding, Encoding.swift:197-201), after
+    // every other slot so that the ciphertext-side slot indices do not depend on t.
+    c->simd = is_prime(t) && (t - 1) % (2 * (u64)n) == 0;
+    const int nslots = (c->aux_is_reference ? 2 * L + 2 : 3 * L + 3) + (c->simd ? 1 : 0);
     c->slots.resize(nslots);
     std::vector<u64> slot_mod(nslots);
+    if (c->simd) slot_mod[c->slot_t()] = t;
     for (int i = 0; i < L; ++i) slot_mod[c->slot_q(i)] = c->q[i];
     for (int j = 0; j <= L; ++j) slot_mod[c->slot_bsk(j)] = c->bsk[j];
     slot_mod[c->slot_ks()] = c->q_ks;
@@ -372,6 +375,42 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
         }
     }
 
+    // ---- plaintext translate constants per level (Bfv+Encrypt.swift:75-139 with getRnsTool(moduliCount: l))
+    c->translate.resize(L + 1);
+    for (int l = 1; l <= L; ++l) {
+        TranslateConsts &tc = c->translate[l];
+        std::memset(&tc, 0, sizeof(tc));
+        tc.l = l;
+        tc.t = t;
+        tc.t_threshold = (t + 1) / 2;
+        tc.q_mod_t = prod_mod(Q, l, t);
+        tc.q_mod_t_p = shoup_factor(tc.q_mod_t, t);
+        for (int i = 0; i < l; ++i) {
+            const u64 qi = Q[i];
+            tc.q[i] = qi;
+            // Q_l = t floor(Q_l / t) + [Q_l]_t and Q_l = 0 mod q_i  ->  floor(Q_l / t) = -[Q_l]_t t^-1 mod q_i
+            tc.delta[i] = mulmod((qi - tc.q_mod_t % qi) % qi, invmod(t % qi, qi), qi);
+            tc.delta_p[i] = shoup_factor(tc.delta[i], qi);
+        }
+    }
+
+    // ---- SIMD encoding permutation (generateEncodingMatrix, Encoding.swift:197-219; generator 3, Galois.swift:169-171)
+    if (c->simd) {
+        std::vector<int32_t> matrix(n), inverse(n);
+        const u64 mask = 2 * (u64)n - 1;
+        u64 g = 1;
+        for (int64_t i = 0; i < n / 2; ++i) {
+            matrix[i] = (int32_t)bitrev((unsigned)((g - 1) >> 1), c->logn);
+            matrix[n / 2 + i] = (int32_t)bitrev((unsigned)((mask - g) >> 1), c->logn);
+            g = (g * 3) & mask;
+        }
+        for (int64_t i = 0; i < n; ++i) inverse[matrix[i]] = (int32_t)i;
+        if (cudaMalloc(&c->d_simd_matrix, sizeof(int32_t) * 2 * (size_t)n) != cudaSuccess) { err = "cudaMalloc failed"; delete c; return nullptr; }
+        c->d_simd_inverse = c->d_simd_matrix + n;
+        cudaMemcpy(c->d_simd_matrix, matrix.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice);
+        cudaMemcpy(c->d_simd_inverse, inverse.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice);
+    }
+
     // ---- divide-and-round constants
     c->ks_divround.resize(L + 1);
     c->ms_divround.resize(L + 1);
@@ -390,6 +429,7 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
 Context::~Context() {
     if (d_pool) cudaFree(d_pool);
     if (d_slots) cudaFree(d_slots);
+    if (d_simd_matrix) cudaFree(d_simd_matrix);
 }
 
 NttRowMap Context::map_q(int rows) const {

@@ -15,7 +15,7 @@
 namespace hecuda {
 
 constexpr int kMaxL = 32;               // coefficient moduli: the reference allows 32 (EncryptionParameters.swift:148)
-constexpr int kMaxSlots = 3 * kMaxL + 3;  // q_0..q_{L-1} | bsk_0..bsk_L | q_ks | aux_0..aux_L
+constexpr int kMaxSlots = 3 * kMaxL + 4;  // q_0..q_{L-1} | bsk_0..bsk_L | q_ks | aux_0..aux_L | t
 constexpr int kMaxRows = 2 * kMaxL + 1;
 
 // One NTT-capable modulus.  Twiddle tables are interleaved (w, floor(w 2^64 / p)) pairs, indexed like the
@@ -108,6 +108,19 @@ struct DivRoundConsts {
     u64 inv_w[kMaxL + 1], inv_wp[kMaxL + 1];  // m_last^-1 mod m_i
 };
 
+// Plaintext translate at level l (Bfv+Encrypt.swift:75-139) over Q_l = q_0..q_{l-1} (getRnsTool(moduliCount: l)):
+//   adjust = floor(([Q_l]_t m + tThreshold) / t),   c0_i +-= [floor(Q_l / t) m + adjust]_{q_i}
+// [Q_l]_t m + tThreshold < t^2 may exceed 64 bits (t up to 2^62): with w = [Q_l]_t and r = [w m]_t,
+// floor((w m + tThreshold) / t) = floor(w m / t) + (r + tThreshold >= t), and floor(w m / t) is the quotient of the
+// Shoup multiplication by w modulo t (wp = floor(w 2^64 / t)) -- exact without a 128-bit division.
+struct TranslateConsts {
+    int l;
+    u64 t, t_threshold;                  // t, (t + 1) / 2   (RnsTool.tThreshold, RnsTool.swift:123-125)
+    u64 q_mod_t, q_mod_t_p;              // [Q_l]_t and its Shoup factor modulo t   (RnsTool.qModT, :167)
+    u64 q[kMaxL];
+    u64 delta[kMaxL], delta_p[kMaxL];    // floor(Q_l / t) mod q_i and Shoup factors (RnsTool.qDivT, :176-182)
+};
+
 struct HostSlot {
     ModSlot dev;                      // with device pointers filled in
     std::vector<u64> roots, inv_roots;  // host copies (w only) for parity checks
@@ -134,7 +147,7 @@ class Context {
     std::vector<u64> bsk;  // L+1 primes: the reference's BEHZ base (RnsTool.swift:30-33)
     std::vector<u64> aux;  // L+1 primes: the base ct x ct multiply actually computes in (context.cu); == bsk when
     bool aux_is_reference = true;  // the conditions for the faster base do not hold (or HECUDA_AUX_BASE=reference)
-    std::vector<HostSlot> slots;  // L q's, L+1 bsk, 1 q_ks, then L+1 aux (when different from bsk)
+    std::vector<HostSlot> slots;  // L q's, L+1 bsk, 1 q_ks, then L+1 aux (when different from bsk), then t (SIMD)
     ModSlot *d_slots = nullptr;   // device array: the slots, then (N = 2^15 only) 2 virtual half-transform slots per slot
     int split_slot_base = 0;      // index of the first virtual slot (slot s, half h -> split_slot_base + 2 s + h)
     LiftConsts lift;        // over [Q, Bsk]: stage-level entry points
@@ -144,11 +157,18 @@ class Context {
     std::vector<DivRoundConsts> ks_divround;   // index l (1..L): base [q_0..q_{l-1}, q_ks]
     std::vector<DivRoundConsts> ms_divround;   // index l (2..L): base [q_0..q_{l-1}]
     void *d_pool = nullptr;  // twiddle storage
+    // SIMD encoding (Encoding.swift:197-245): present when t is a prime = 1 mod 2N (isNttModulus, PolyRq+Ntt.swift:24-27)
+    bool simd = false;
+    int32_t *d_simd_matrix = nullptr;  // [N] generateEncodingMatrix: slot i <-> Eval position matrix[i]
+    int32_t *d_simd_inverse = nullptr; // [N] inverse permutation: Eval position j holds slot inverse[j]
+    std::vector<TranslateConsts> translate;  // index l (1..L)
 
     int slot_q(int i) const { return i; }
     int slot_bsk(int j) const { return L + j; }
     int slot_ks() const { return 2 * L + 1; }
     int slot_aux(int j) const { return aux_is_reference ? slot_bsk(j) : 2 * L + 2 + j; }
+    // the plaintext modulus, after every other slot (Context.plaintextContext); -1 without SIMD support
+    int slot_t() const { return simd ? (aux_is_reference ? 2 * L + 2 : 3 * L + 3) : -1; }
     NttRowMap map_q(int rows) const;      // rows of the ciphertext context
     NttRowMap map_qbsk() const;           // [Q, Bsk]
     NttRowMap map_qaux() const;           // [Q, aux]

@@ -81,6 +81,20 @@ cudaError_t launch_inner_product_plain_small(const Context &ctx, const u64 *cts,
 cudaError_t launch_plaintext_to_eval(const Context &ctx, const u64 *plain, int l, u64 *out, int64_t count,
                                      cudaStream_t stream);
 
+// ---- the plaintext side of Bfv (plaintext.cu); the context must support SIMD encoding for encode / decode
+// encodeSimd (+ convertToEvalFormat when l >= 1): values count x value_count (< t) -> out count x N (Coeff, l = 0) or
+// count x l x N (Eval).  decodeSimd / decodeEval: plain count x N (l = 0) or count x l x N -> values count x N.
+// scratch: simd_scratch_words per item (stream-ordered, caller-owned).
+size_t simd_scratch_words(const Context &ctx, bool encode, int l);
+cudaError_t launch_encode_simd(const Context &ctx, const u64 *values, int value_count, int l, u64 *out, u64 *scratch,
+                               int64_t count, cudaStream_t stream);
+cudaError_t launch_decode_simd(const Context &ctx, const u64 *plain, int l, u64 *values, u64 *scratch, int64_t count,
+                               cudaStream_t stream);
+// plaintextTranslate: ct, out batch x polys x l x N (Coeff); pt N values (< t) shared by all (broadcast) or batch x N;
+// op = HECUDA_PLAINTEXT_ADD / SUB / SUB_FROM; out may equal ct
+cudaError_t launch_plaintext_translate(const Context &ctx, const u64 *ct, int polys, int l, const u64 *pt, bool broadcast,
+                                       int op, u64 *out, int64_t batch, cudaStream_t stream);
+
 // ---- wire format (codec.cu): PolyRq.serialize / load, PolyRq+Serialize.swift:28-84
 struct CodecConsts {
     int rows;

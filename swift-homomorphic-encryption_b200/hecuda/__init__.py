@@ -134,7 +134,21 @@ SYMBOLS = {
     "hecuda_poly_mul_scalars": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int32, C.c_int64]),
     "hecuda_poly_mul_scalars_device": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int32, C.c_int64, _VP]),
     "hecuda_kernel_launch_count": (C.c_uint64, []),
+    "hecuda_context_supports_simd": (C.c_int32, [_VP, C.POINTER(C.c_int32)]),
+    "hecuda_bfv_encode_simd": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int32, _VP, C.c_int64]),
+    "hecuda_bfv_encode_simd_device": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int32, _VP, C.c_int64, _VP]),
+    "hecuda_bfv_decode_simd": (C.c_int32, [_VP, _VP, C.c_int32, _VP, C.c_int64]),
+    "hecuda_bfv_decode_simd_device": (C.c_int32, [_VP, _VP, C.c_int32, _VP, C.c_int64, _VP]),
+    "hecuda_bfv_plaintext_translate": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int32, _VP, C.c_int64, C.c_int32, _VP, C.c_int64]),
+    "hecuda_bfv_plaintext_translate_device": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int32, _VP, C.c_int64, C.c_int32, _VP,
+                                                          C.c_int64, _VP]),
+    "hecuda_u32_bfv_encode_simd": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int32, _VP, C.c_int64]),
+    "hecuda_u32_bfv_decode_simd": (C.c_int32, [_VP, _VP, C.c_int32, _VP, C.c_int64]),
+    "hecuda_u32_bfv_plaintext_translate": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int32, _VP, C.c_int64, C.c_int32, _VP,
+                                                       C.c_int64]),
 }
+
+PLAINTEXT_ADD, PLAINTEXT_SUB, PLAINTEXT_SUB_FROM = 0, 1, 2  # HECUDA_PLAINTEXT_* (plaintextTranslate ops)
 
 _lib = None
 
@@ -293,6 +307,13 @@ class Context:
     def ciphertextModuli(self):
         return self.coefficientModuli[: self.L]
 
+    @property
+    def supportsSimdEncoding(self) -> bool:
+        """Context.supportsSimdEncoding (Context.swift:63-65): t is a prime = 1 mod 2N."""
+        v = C.c_int32(0)
+        _check(load_library().hecuda_context_supports_simd(self._h, C.byref(v)))
+        return bool(v.value)
+
     def close(self):
         if getattr(self, "_h", None) is not None:
             load_library().hecuda_context_destroy(self._h)
@@ -361,6 +382,48 @@ class EvaluationKey:
             self.close()
         except Exception:
             pass
+
+
+def _encode_simd(context: Context, values, moduliCount: int, host, dtype, fn):
+    v = host(values)
+    if v.ndim == 0 or v.ndim > 2:
+        raise HeError(-1, "encodeSimd takes (valueCount,) or (count, valueCount) values")
+    vals = v.reshape(-1, v.shape[-1]) if v.ndim == 2 else v.reshape(1, -1)
+    n = context.degree
+    shape = (vals.shape[0], moduliCount, n) if moduliCount else (vals.shape[0], n)
+    out = np.empty(shape, dtype=dtype)
+    _check(getattr(load_library(), fn)(context._h, _ptr(vals), vals.shape[1], moduliCount, _ptr(out), vals.shape[0]))
+    return out if v.ndim == 2 else out[0]
+
+
+def _decode_simd(context: Context, plaintexts, moduliCount: int, host, dtype, fn):
+    p = host(plaintexts)
+    n = context.degree
+    per = (moduliCount * n) if moduliCount else n
+    if p.size % per or p.shape[-1] != n or (moduliCount and (p.ndim < 2 or p.shape[-2] != moduliCount)):
+        raise HeError(-1, f"invalidPlaintext: expected (..., {moduliCount}, {n})" if moduliCount else f"expected (..., {n})")
+    count = p.size // per
+    out = np.empty((count, n), dtype=dtype)
+    _check(getattr(load_library(), fn)(context._h, _ptr(p), moduliCount, _ptr(out), count))
+    lead = p.shape[:-2] if moduliCount else p.shape[:-1]
+    return out.reshape(lead + (n,))
+
+
+def _translate(context: Context, ciphertext, plaintext, op: int, host, dtype, fn, out=None):
+    c, p = host(ciphertext), host(plaintext)
+    n = context.degree
+    if c.ndim < 3 or c.shape[-1] != n or c.shape[-3] not in (2, 3):
+        raise HeError(-1, f"invalidCiphertext: expected (..., 2 or 3, l, {n}) Coeff ciphertexts")
+    polys, l = c.shape[-3], c.shape[-2]
+    batch = c.size // (polys * l * n)
+    if p.shape[-1] != n or p.size not in (n, batch * n):
+        raise HeError(-1, f"incompatibleCiphertextAndPlaintext: plaintexts must be ({n},) or (batch, {n})")
+    if out is None:
+        out = np.empty_like(c)
+    elif out.dtype != np.dtype(dtype) or out.shape != c.shape or not out.flags.c_contiguous:
+        raise HeError(-1, "out must be a C-contiguous array shaped like the ciphertexts")
+    _check(getattr(load_library(), fn)(context._h, _ptr(c), polys, l, _ptr(p), p.size // n, op, _ptr(out), batch))
+    return out
 
 
 class Bfv:
@@ -511,6 +574,36 @@ class Bfv:
         out = np.empty((d.shape[0], l, context.degree), dtype=np.uint64)
         _check(load_library().hecuda_plaintext_to_eval(context._h, _ptr(d), l, _ptr(out), d.shape[0]))
         return out
+
+    @staticmethod
+    def encodeSimd(context: Context, values, moduliCount: int = 0):
+        """Context.encode(values:format: .simd) (Encoding.swift:197-235): (valueCount,) or (count, valueCount) values < t
+        -> (N,) / (count, N) Coeff plaintexts; moduliCount = l >= 1 gives Eval plaintexts (l, N) / (count, l, N)
+        (Bfv+Encode.swift:45-50)."""
+        return _encode_simd(context, values, moduliCount, _host, np.uint64, "hecuda_bfv_encode_simd")
+
+    @staticmethod
+    def decodeSimd(context: Context, plaintexts, moduliCount: int = 0):
+        """decodeSimd (Encoding.swift:237-245) of (..., N) Coeff plaintexts, or Bfv.decodeEval (Bfv+Encode.swift:76-80) of
+        (..., l, N) Eval plaintexts with moduliCount = l -> (..., N) slot values."""
+        return _decode_simd(context, plaintexts, moduliCount, _host, np.uint64, "hecuda_bfv_decode_simd")
+
+    @staticmethod
+    def addAssignCoeff(context: Context, ciphertext, plaintext, out=None):
+        """Bfv.addAssignCoeff (Bfv.swift:110-112): (..., polys, l, N) Coeff ciphertexts (correction factor 1) + (N,) or
+        (batch, N) Coeff plaintexts.  out=ciphertext updates in place."""
+        return _translate(context, ciphertext, plaintext, PLAINTEXT_ADD, _host, np.uint64, "hecuda_bfv_plaintext_translate", out)
+
+    @staticmethod
+    def subAssignCoeff(context: Context, ciphertext, plaintext, out=None):
+        """Bfv.subAssignCoeff (Bfv.swift:115-117): ciphertext - plaintext."""
+        return _translate(context, ciphertext, plaintext, PLAINTEXT_SUB, _host, np.uint64, "hecuda_bfv_plaintext_translate", out)
+
+    @staticmethod
+    def subCoeff(context: Context, plaintext, ciphertext, out=None):
+        """HeScheme.subCoeff(plaintext, ciphertext) (HeScheme.swift:1540-1542): plaintext - ciphertext."""
+        return _translate(context, ciphertext, plaintext, PLAINTEXT_SUB_FROM, _host, np.uint64,
+                          "hecuda_bfv_plaintext_translate", out)
 
     @staticmethod
     def randomPolys(context: Context, seeds, moduliCount: int = 0) -> np.ndarray:
@@ -790,3 +883,24 @@ class Bfv32:
         out = np.empty(d.shape[:-2] + (L, n), dtype=np.uint32)
         _check(load_library().hecuda_u32_rnstool_floor_qbsk_to_q(context._h, _ptr(d), _ptr(out), d.size // ((2 * L + 1) * n)))
         return out
+
+    @staticmethod
+    def encodeSimd(context: Context, values, moduliCount: int = 0):
+        return _encode_simd(context, values, moduliCount, _host32, np.uint32, "hecuda_u32_bfv_encode_simd")
+
+    @staticmethod
+    def decodeSimd(context: Context, plaintexts, moduliCount: int = 0):
+        return _decode_simd(context, plaintexts, moduliCount, _host32, np.uint32, "hecuda_u32_bfv_decode_simd")
+
+    @staticmethod
+    def addAssignCoeff(context: Context, ciphertext, plaintext, out=None):
+        return _translate(context, ciphertext, plaintext, PLAINTEXT_ADD, _host32, np.uint32, "hecuda_u32_bfv_plaintext_translate", out)
+
+    @staticmethod
+    def subAssignCoeff(context: Context, ciphertext, plaintext, out=None):
+        return _translate(context, ciphertext, plaintext, PLAINTEXT_SUB, _host32, np.uint32, "hecuda_u32_bfv_plaintext_translate", out)
+
+    @staticmethod
+    def subCoeff(context: Context, plaintext, ciphertext, out=None):
+        return _translate(context, ciphertext, plaintext, PLAINTEXT_SUB_FROM, _host32, np.uint32,
+                          "hecuda_u32_bfv_plaintext_translate", out)

@@ -10,6 +10,8 @@
 //   he::Bfv::relinearize        Bfv.relinearize                 Bfv/Bfv.swift:201-219
 //   he::Bfv::modSwitchDown      Bfv.modSwitchDown               Bfv/Bfv.swift:163-171
 //   he::Bfv::forwardNtt/inverseNtt  PolyRq.forwardNtt/inverseNtt  PolyRq/PolyRq+Ntt.swift:230,541
+//   he::Bfv::encodeSimd/decodeSimd  Bfv.encode / decodeCoeff / decodeEval (.simd)  Encoding.swift:197-245, Bfv+Encode.swift
+//   he::Bfv::addAssignCoeff/subAssignCoeff/subCoeff  Bfv.swift:110-117, HeScheme.swift:1540-1542
 //   he::HeError                 HeError                         Error.swift:17-54
 //
 // Batched overloads take a span of ciphertexts so one call saturates the GPU (SURVEY.md section 8b, "Threading").
@@ -302,6 +304,58 @@ struct Bfv {
         Ciphertext out(first.context, first.polyCount, first.moduliCount);
         check(hecuda_bfv_inner_product_plaintexts(first.context->handle(), cts.data(), first.polyCount, first.moduliCount,
                                                   (int64_t)ciphertexts.size(), pts.data(), present.data(), out.data.data(), 1));
+        return out;
+    }
+
+    // ---- the plaintext side.  A Coeff plaintext is its N coefficients (< t); an Eval plaintext is a PolyRq.
+    // Context.supportsSimdEncoding (Context.swift:63-65)
+    static bool supportsSimdEncoding(const Context &context) {
+        int32_t supported = 0;
+        check(hecuda_context_supports_simd(context.handle(), &supported));
+        return supported != 0;
+    }
+    // Bfv.encode(context:values:format: .simd) (Encoding.swift:197-235): up to N values < t -> Coeff plaintext
+    static std::vector<uint64_t> encodeSimd(const Context &context, const std::vector<uint64_t> &values) {
+        std::vector<uint64_t> out((size_t)context.degree);
+        check(hecuda_bfv_encode_simd(context.handle(), values.data(), (int32_t)values.size(), 0, out.data(), 1));
+        return out;
+    }
+    // Bfv.encode(context:values:format: .simd, moduliCount:) (Bfv+Encode.swift:45-50) -> Eval plaintext
+    static PolyRq encodeSimd(const std::shared_ptr<const Context> &context, const std::vector<uint64_t> &values, int moduliCount) {
+        PolyRq out(context, moduliCount);
+        check(hecuda_bfv_encode_simd(context->handle(), values.data(), (int32_t)values.size(), moduliCount, out.data.data(), 1));
+        return out;
+    }
+    // Bfv.decodeCoeff(plaintext:format: .simd) (Encoding.swift:237-245): N slot values
+    static std::vector<uint64_t> decodeSimd(const Context &context, const std::vector<uint64_t> &plaintext) {
+        if (plaintext.size() != (size_t)context.degree) throw HeError(HeError::invalidPolyContext, "plaintext must have N coefficients");
+        std::vector<uint64_t> out((size_t)context.degree);
+        check(hecuda_bfv_decode_simd(context.handle(), plaintext.data(), 0, out.data(), 1));
+        return out;
+    }
+    // Bfv.decodeEval(plaintext:format: .simd) (Bfv+Encode.swift:76-80)
+    static std::vector<uint64_t> decodeSimd(const PolyRq &plaintext) {
+        std::vector<uint64_t> out((size_t)plaintext.context->degree);
+        check(hecuda_bfv_decode_simd(plaintext.context->handle(), plaintext.data.data(), plaintext.moduliCount, out.data(), 1));
+        return out;
+    }
+    // plaintextTranslate's guards (Bfv+Encrypt.swift:80-83)
+    static void validateTranslate(const Ciphertext &ct, const std::vector<uint64_t> &plaintext) {
+        if (ct.correctionFactor != 1) throw HeError(HeError::invalidCiphertext, "invalidCorrectionFactor: correction factor must be 1");
+        if (plaintext.size() != (size_t)ct.context->degree) throw HeError(HeError::invalidPolyContext, "plaintext must have N coefficients");
+    }
+    static void translate(Ciphertext &ct, const std::vector<uint64_t> &plaintext, int32_t op) {
+        validateTranslate(ct, plaintext);
+        check(hecuda_bfv_plaintext_translate(ct.context->handle(), ct.data.data(), ct.polyCount, ct.moduliCount, plaintext.data(), 1,
+                                             op, ct.data.data(), 1));
+    }
+    // Bfv.addAssignCoeff / subAssignCoeff (Bfv.swift:110-117): ciphertext +-= Coeff plaintext
+    static void addAssignCoeff(Ciphertext &ct, const std::vector<uint64_t> &plaintext) { translate(ct, plaintext, HECUDA_PLAINTEXT_ADD); }
+    static void subAssignCoeff(Ciphertext &ct, const std::vector<uint64_t> &plaintext) { translate(ct, plaintext, HECUDA_PLAINTEXT_SUB); }
+    // HeScheme.subCoeff(plaintext, ciphertext) (HeScheme.swift:1540-1542): plaintext - ciphertext
+    static Ciphertext subCoeff(const std::vector<uint64_t> &plaintext, const Ciphertext &ct) {
+        Ciphertext out = ct;
+        translate(out, plaintext, HECUDA_PLAINTEXT_SUB_FROM);
         return out;
     }
 
