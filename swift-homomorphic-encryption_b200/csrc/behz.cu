@@ -4,29 +4,19 @@
 //   tensor = Bfv.multiplyWithoutScaling      Bfv+Multiply.swift:80-82
 //   floor  = _RnsTool.floorQBskToQ           RnsTool.swift:378-456
 //
-// Layout/launch: a thread owns two adjacent coefficient columns (16-byte loads/stores, coalesced along the
-// coefficient axis; rows are strided by N); blockIdx.y/z select the polynomial, so there is no integer division.
+// Layout/launch: lift and floor run persistent CTAs over column tiles (below); the tensor kernels give a thread two
+// adjacent coefficient columns (16-byte loads/stores, coalesced along the coefficient axis; rows are strided by N) and
+// select the polynomial with blockIdx.y/z, so there is no integer division.
 // Arithmetic: each step evaluates the reference's chain of exact modular operations with pre-multiplied constants
 // (context.hpp) as one 128-bit multiply-accumulate pass per output residue followed by ONE Montgomery reduction
 // (the 2^64 factor lives in the constants); the stored residues are the same canonical values.  All kernels are
 // instruction-issue bound (64-bit integer multiplies), not HBM bound -- see DESIGN.md.
-#include <cstdlib>
-
 #include "kernels.cuh"
 #include "ntt_fast.cuh"
 
 namespace hecuda {
 
 constexpr int kThreads = 128;
-
-// columns per thread: 2 (16-byte accesses) by default; HECUDA_BEHZ_COLS=1 selects 1 (more warps, 8-byte accesses)
-static int cols_per_thread() {
-    static const int v = [] {
-        const char *e = std::getenv("HECUDA_BEHZ_COLS");
-        return (e && e[0] == '1') ? 1 : 2;
-    }();
-    return v;
-}
 
 template <int COLS>
 struct Cols {
@@ -35,10 +25,13 @@ struct Cols {
 template <int COLS>
 __device__ __forceinline__ Cols<COLS> ldc(const u64 *p) {
     Cols<COLS> r;
-    if (COLS == 2) {
-        const ulonglong2 t = *reinterpret_cast<const ulonglong2 *>(p);
-        r.v[0] = t.x;
-        r.v[COLS - 1] = t.y;
+    if (COLS % 2 == 0) {
+#pragma unroll
+        for (int h = 0; h < COLS / 2; ++h) {
+            const ulonglong2 t = reinterpret_cast<const ulonglong2 *>(p)[h];
+            r.v[2 * h] = t.x;
+            r.v[2 * h + (COLS > 1)] = t.y;
+        }
     } else {
         r.v[0] = *p;
     }
@@ -46,60 +39,100 @@ __device__ __forceinline__ Cols<COLS> ldc(const u64 *p) {
 }
 template <int COLS>
 __device__ __forceinline__ void stc(u64 *p, const u64 (&v)[COLS]) {
-    if (COLS == 2) *reinterpret_cast<ulonglong2 *>(p) = make_ulonglong2(v[0], v[COLS - 1]);
-    else *p = v[0];
+    if (COLS % 2 == 0) {
+#pragma unroll
+        for (int h = 0; h < COLS / 2; ++h)
+            reinterpret_cast<ulonglong2 *>(p)[h] = make_ulonglong2(v[2 * h], v[2 * h + (COLS > 1)]);
+    } else {
+        *p = v[0];
+    }
+}
+
+// ---- lift and floor: CTA b owns column tile b, kThreads * COLS consecutive coefficients of one polynomial (1-D grid,
+// tiles of a polynomial adjacent).  A thread issues every row load of its tile before any arithmetic, so it makes one
+// trip to memory, and the many resident CTAs overlap one another's loads and multiplies.  Two columns per thread
+// (16-byte accesses) up to L = 8; one above that, which keeps every instantiation free of spills.
+template <int L>
+struct BehzCols {
+    static constexpr int value = L <= 8 ? 2 : 1;
+};
+
+struct ColTiles {
+    long long count;  // polynomials << shift
+    int shift;        // log2(tiles per polynomial); N < kThreads * COLS: one partial tile per polynomial
+};
+
+// first column of tile t owned by this thread
+template <int COLS>
+__device__ __forceinline__ int tile_col(long long t, const ColTiles &tl) {
+    return (int)(t & ((1ll << tl.shift) - 1)) * (kThreads * COLS) + (int)threadIdx.x * COLS;
+}
+
+template <int ROWS, int COLS>
+__device__ __forceinline__ void load_rows(Cols<COLS> (&x)[ROWS], const u64 *src, int64_t n) {
+#pragma unroll
+    for (int i = 0; i < ROWS; ++i) x[i] = ldc<COLS>(src + (int64_t)i * n);
 }
 
 // Bounds (checked for the actual moduli by Context::create): every 128-bit accumulator below stays < 2^127 and the
 // Montgomery-reduced sums are < 2p (lift, f_j, out_i: one or two conditional subtractions) or < 4p (alpha).
 // H: every b_j is h 2^32 + 1 (LiftConsts / FloorConsts::h_primes), so the reductions modulo b_j take mont_reduce_h.
-template <int L, int COLS, bool H>
-__global__ void __launch_bounds__(kThreads) lift_kernel(const u64 *__restrict__ in, int polys_in, u64 *__restrict__ ext,
-                                                       int ext_polys, int out_poly_offset,
-                                                       const __grid_constant__ LiftConsts c, int n, bool q_rows) {
-    const int rows_out = q_rows ? 2 * L + 1 : L + 1, aux0 = q_rows ? L : 0;
-    const int coeff = (blockIdx.x * kThreads + threadIdx.x) * COLS;
-    if (coeff >= n) return;
-    const int64_t poly = (int64_t)blockIdx.z * gridDim.y + blockIdx.y;  // index among items * polys_in
-    const int64_t item = polys_in == 2 ? (poly >> 1) : poly / polys_in;  // (no 64-bit division on the hot path)
-    const int pin = (int)(poly - item * polys_in);
-    const u64 *src = in + poly * L * n + coeff;
-    u64 *dst = ext + ((item * ext_polys + out_poly_offset + pin) * rows_out) * n + coeff;
-    u64 z[COLS][L];
-    u32 acc_mt[COLS];
+// Output polynomial g = (item * ops + op) * 2^pin_shift + pin of ext (ops = 2 with rhs, else 1) is the lift of input
+// polynomial item * 2^pin_shift + pin of lhs (op 0) or rhs (op 1); it has the L + 1 auxiliary rows, after the L Q rows
+// when Q_ROWS.
+template <int L, bool H, bool Q_ROWS>
+__global__ void __launch_bounds__(kThreads) lift_kernel(const u64 *__restrict__ lhs, const u64 *__restrict__ rhs,
+                                                       int pin_shift, u64 *__restrict__ ext,
+                                                       const __grid_constant__ LiftConsts c, int n, ColTiles tiles) {
+    constexpr int COLS = BehzCols<L>::value, ROWS_OUT = Q_ROWS ? 2 * L + 1 : L + 1, AUX0 = Q_ROWS ? L : 0;
+    if ((int)threadIdx.x * COLS >= n) return;
+    const int op_shift = rhs ? 1 : 0;
+    auto src_of = [&](long long t) {
+        const int64_t g = t >> tiles.shift, item = g >> (pin_shift + op_shift);
+        const int64_t pin = g & ((1 << pin_shift) - 1);
+        const u64 *base = (op_shift && ((g >> pin_shift) & 1)) ? rhs : lhs;
+        return base + ((item << pin_shift) + pin) * L * n + tile_col<COLS>(t, tiles);
+    };
+    const long long t = blockIdx.x;
+    {
+        Cols<COLS> x[L];
+        load_rows<L, COLS>(x, src_of(t), n);
+        u64 *dst = ext + (t >> tiles.shift) * ROWS_OUT * n + tile_col<COLS>(t, tiles);
+        u64 z[COLS][L];
+        u32 acc_mt[COLS];
 #pragma unroll
-    for (int k = 0; k < COLS; ++k) acc_mt[k] = 0;
+        for (int k = 0; k < COLS; ++k) acc_mt[k] = 0;
 #pragma unroll
-    for (int i = 0; i < L; ++i) {
-        const Cols<COLS> x = ldc<COLS>(src + (int64_t)i * n);
-        if (q_rows) stc<COLS>(dst + (int64_t)i * n, x.v);
+        for (int i = 0; i < L; ++i) {
+            if (Q_ROWS) stc<COLS>(dst + (int64_t)i * n, x[i].v);
+#pragma unroll
+            for (int k = 0; k < COLS; ++k) {
+                // canonical: z is reinterpreted mod b_j and mod m~ below
+                z[k][i] = shoup_mul(x[i].v[k], c.in_w[i], c.in_wp[i], c.q[i]);
+                acc_mt[k] += (u32)z[k][i] * c.punct_mt[i];
+            }
+        }
+        u32 r[COLS];
+        bool neg[COLS];
 #pragma unroll
         for (int k = 0; k < COLS; ++k) {
-            // canonical: z is reinterpreted mod b_j and mod m~ below
-            z[k][i] = shoup_mul(x.v[k], c.in_w[i], c.in_wp[i], c.q[i]);
-            acc_mt[k] += (u32)z[k][i] * c.punct_mt[i];
+            r[k] = (acc_mt[k] * c.neg_inv_q_mt) & c.mt_mask;  // [-x' Q^-1]_{m~}, RnsTool.swift:343-348
+            neg[k] = r[k] >= c.mt_half;                       // centered representative r - m~ (:357-360)
         }
-    }
-    u32 r[COLS];
-    bool neg[COLS];
 #pragma unroll
-    for (int k = 0; k < COLS; ++k) {
-        r[k] = (acc_mt[k] * c.neg_inv_q_mt) & c.mt_mask;  // [-x' Q^-1]_{m~}, RnsTool.swift:343-348
-        neg[k] = r[k] >= c.mt_half;                       // centered representative r - m~ (:357-360)
-    }
+        for (int j = 0; j <= L; ++j) {
+            u64 o[COLS];
 #pragma unroll
-    for (int j = 0; j <= L; ++j) {
-        u64 o[COLS];
+            for (int k = 0; k < COLS; ++k) {
+                const u64 rc = neg[k] ? (u64)r[k] + c.neg_off[j] : (u64)r[k];
+                u128 acc = (u128)rc * c.qr[j];
 #pragma unroll
-        for (int k = 0; k < COLS; ++k) {
-            const u64 rc = neg[k] ? (u64)r[k] + c.neg_off[j] : (u64)r[k];
-            u128 acc = (u128)rc * c.qr[j];
-#pragma unroll
-            for (int i = 0; i < L; ++i) mac128(acc, z[k][i], c.mat[j][i]);
-            const u64 red = mont_reduce_c<H>(acc, c.b[j], c.b_ninv[j]);
-            o[k] = c.wide_sums ? barrett64(red, c.b[j], c.b_mu1[j]) : csub(red, c.b[j]);
+                for (int i = 0; i < L; ++i) mac128(acc, z[k][i], c.mat[j][i]);
+                const u64 red = mont_reduce_c<H>(acc, c.b[j], c.b_ninv[j]);
+                o[k] = c.wide_sums ? barrett64(red, c.b[j], c.b_mu1[j]) : csub(red, c.b[j]);
+            }
+            stc<COLS>(dst + (int64_t)(AUX0 + j) * n, o);
         }
-        stc<COLS>(dst + (int64_t)(aux0 + j) * n, o);
     }
 }
 
@@ -205,61 +238,62 @@ __global__ void __launch_bounds__(kThreads) tensor_sum_kernel(const u64 *__restr
     stc<2>(o + 2 * ps, o2);
 }
 
-template <int L, int COLS, bool H>
-__global__ void __launch_bounds__(kThreads) floor_kernel(const u64 *__restrict__ in, u64 *__restrict__ out,
-                                                        const __grid_constant__ FloorConsts c, int n) {
-    constexpr int R = 2 * L + 1;
-    const int coeff = (blockIdx.x * kThreads + threadIdx.x) * COLS;
-    if (coeff >= n) return;
-    const int64_t poly = (int64_t)blockIdx.z * gridDim.y + blockIdx.y;
-    const u64 *src = in + poly * R * n + coeff;
-    u64 *dst = out + poly * L * n + coeff;
-    u64 y[COLS][L];
+// Q_SCALED: the Q rows arrive as y_i = [x_i (Q/q_i)^-1]_{q_i} already (the inverse NTT's kScaleTMontFloor)
+// (a minimum of one CTA per SM from L = 8 lets ptxas use the registers that keep those instantiations free of spills)
+template <int L, bool H, bool Q_SCALED>
+__global__ void __launch_bounds__(kThreads, L >= 8 ? 1 : 0) floor_kernel(const u64 *__restrict__ in, u64 *__restrict__ out,
+                                                        const __grid_constant__ FloorConsts c, int n, ColTiles tiles) {
+    constexpr int R = 2 * L + 1, COLS = BehzCols<L>::value;
+    if ((int)threadIdx.x * COLS >= n) return;
+    const long long t = blockIdx.x;
+    {
+        Cols<COLS> x[R];
+        load_rows<R, COLS>(x, in + (t >> tiles.shift) * R * n + tile_col<COLS>(t, tiles), n);
+        u64 y[COLS][L];
 #pragma unroll
-    for (int i = 0; i < L; ++i) {
-        const Cols<COLS> x = ldc<COLS>(src + (int64_t)i * n);
+        for (int i = 0; i < L; ++i)
 #pragma unroll
-        for (int k = 0; k < COLS; ++k) y[k][i] = shoup_mul(x.v[k], c.inq_w[i], c.inq_wp[i], c.q[i]);
-    }
-    // approximateFloor, RnsTool.swift:378-398: f_j = (x_bj - FBC(x_Q)_j) Q^-1 mod b_j   (kept lazy, < 2 b_j)
-    u64 f[COLS][L + 1];
+            for (int k = 0; k < COLS; ++k)
+                y[k][i] = Q_SCALED ? x[i].v[k] : shoup_mul(x[i].v[k], c.inq_w[i], c.inq_wp[i], c.q[i]);
+        // approximateFloor, RnsTool.swift:378-398: f_j = (x_bj - FBC(x_Q)_j) Q^-1 mod b_j; for j < L the constants
+        // carry (B/b_j)^-1 as well, so f_j is w_j of the conversion below (canonical); f_L is kept lazy (< 2 m_sk)
+        u64 f[COLS][L + 1];
 #pragma unroll
-    for (int j = 0; j <= L; ++j) {
-        const Cols<COLS> xb = ldc<COLS>(src + (int64_t)(L + j) * n);
+        for (int j = 0; j <= L; ++j) {
+#pragma unroll
+            for (int k = 0; k < COLS; ++k) {
+                u128 acc = (u128)x[L + j].v[k] * c.fq[j];
+#pragma unroll
+                for (int i = 0; i < L; ++i) mac128(acc, y[k][i], c.fmat[j][i]);
+                const u64 red = mont_reduce_c<H>(acc, c.b[j], c.b_ninv[j]);
+                f[k][j] = j == L ? red : c.wide_sums ? barrett64(red, c.b[j], c.b_mu1[j]) : csub(red, c.b[j]);
+            }
+        }
+        // convertApproximateBskToQ, RnsTool.swift:402-450
+        const u64 msk = c.b[L];
+        u64 outv[L][COLS];
 #pragma unroll
         for (int k = 0; k < COLS; ++k) {
-            u128 acc = (u128)xb.v[k] * c.fq[j];
+            const u64 *w = f[k];  // w_i = [f_i (B/b_i)^-1]_{b_i}, canonical: reinterpreted mod m_sk and q_i
+            u128 acc = (u128)f[k][L] * c.a_msk;
 #pragma unroll
-            for (int i = 0; i < L; ++i) mac128(acc, y[k][i], c.fmat[j][i]);
-            f[k][j] = mont_reduce_c<H>(acc, c.b[j], c.b_ninv[j]);
+            for (int i = 0; i < L; ++i) mac128(acc, w[i], c.amat[i]);
+            u64 alpha = mont_reduce_c<H>(acc, msk, c.b_ninv[L]);
+            alpha = c.wide_sums ? barrett64(alpha, msk, c.msk_mu1) : csub(csub(csub(alpha, 4 * msk), 2 * msk), msk);
+            const bool exceeds = alpha > (msk >> 1);
+            const u64 alpha_c = exceeds ? msk - alpha : alpha;
+#pragma unroll
+            for (int i = 0; i < L; ++i) {
+                u128 o = (u128)alpha_c * (exceeds ? c.b_mod_q[i] : c.neg_b_mod_q[i]);
+#pragma unroll
+                for (int kk = 0; kk < L; ++kk) mac128(o, w[kk], c.omat[i][kk]);
+                outv[i][k] = csub(csub(mont_reduce(o, c.q[i], c.q_ninv[i]), 2 * c.q[i]), c.q[i]);
+            }
         }
+        u64 *dst = out + (t >> tiles.shift) * L * n + tile_col<COLS>(t, tiles);
+#pragma unroll
+        for (int i = 0; i < L; ++i) stc<COLS>(dst + (int64_t)i * n, outv[i]);
     }
-    // convertApproximateBskToQ, RnsTool.swift:402-450
-    const u64 msk = c.b[L];
-    u64 outv[L][COLS];
-#pragma unroll
-    for (int k = 0; k < COLS; ++k) {
-        u64 w[L];
-        u128 acc = (u128)f[k][L] * c.a_msk;
-#pragma unroll
-        for (int i = 0; i < L; ++i) {
-            w[i] = shoup_mul(f[k][i], c.inb_w[i], c.inb_wp[i], c.b[i]);  // canonical: reinterpreted mod m_sk and q_i
-            mac128(acc, w[i], c.amat[i]);
-        }
-        u64 alpha = mont_reduce_c<H>(acc, msk, c.b_ninv[L]);
-        alpha = c.wide_sums ? barrett64(alpha, msk, c.msk_mu1) : csub(csub(csub(alpha, 4 * msk), 2 * msk), msk);
-        const bool exceeds = alpha > (msk >> 1);
-        const u64 alpha_c = exceeds ? msk - alpha : alpha;
-#pragma unroll
-        for (int i = 0; i < L; ++i) {
-            u128 o = (u128)alpha_c * (exceeds ? c.b_mod_q[i] : c.neg_b_mod_q[i]);
-#pragma unroll
-            for (int kk = 0; kk < L; ++kk) mac128(o, w[kk], c.omat[i][kk]);
-            outv[i][k] = csub(csub(mont_reduce(o, c.q[i], c.q_ninv[i]), 2 * c.q[i]), c.q[i]);
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < L; ++i) stc<COLS>(dst + (int64_t)i * n, outv[i]);
 }
 
 // ---- more than 16 ciphertext moduli (the reference allows 32 coefficient moduli, EncryptionParameters.swift:148): the
@@ -303,19 +337,18 @@ __global__ void __launch_bounds__(kThreads) floor_generic_kernel(const u64 *__re
     const int64_t poly = (int64_t)blockIdx.z * gridDim.y + blockIdx.y;
     const u64 *src = in + poly * R * n + coeff;
     u64 *dst = out + poly * L * n + coeff;
-    u64 y[kMaxL], f[kMaxL + 1], w[kMaxL];
+    u64 y[kMaxL], f[kMaxL + 1];
     for (int i = 0; i < L; ++i) y[i] = shoup_mul(src[(int64_t)i * n], c.inq_w[i], c.inq_wp[i], c.q[i]);
-    for (int j = 0; j <= L; ++j) {
+    for (int j = 0; j <= L; ++j) {  // f_j for j < L is w_j (FloorConsts)
         u128 acc = (u128)src[(int64_t)(L + j) * n] * c.fq[j];
         for (int i = 0; i < L; ++i) mac128(acc, y[i], c.fmat[j][i]);
-        f[j] = mont_reduce(acc, c.b[j], c.b_ninv[j]);
+        const u64 red = mont_reduce(acc, c.b[j], c.b_ninv[j]);
+        f[j] = j == L ? red : barrett64(red, c.b[j], c.b_mu1[j]);
     }
+    const u64 *w = f;
     const u64 msk = c.b[L];
     u128 acc = (u128)f[L] * c.a_msk;
-    for (int i = 0; i < L; ++i) {
-        w[i] = shoup_mul(f[i], c.inb_w[i], c.inb_wp[i], c.b[i]);
-        mac128(acc, w[i], c.amat[i]);
-    }
+    for (int i = 0; i < L; ++i) mac128(acc, w[i], c.amat[i]);
     u64 alpha = mont_reduce(acc, msk, c.b_ninv[L]);
     alpha = c.wide_sums ? barrett64(alpha, msk, c.msk_mu1) : csub(csub(csub(alpha, 4 * msk), 2 * msk), msk);
     const bool exceeds = alpha > (msk >> 1);
@@ -349,53 +382,84 @@ __global__ void __launch_bounds__(kThreads) floor_generic_kernel(const u64 *__re
         default: return cudaErrorInvalidValue;                                                                        \
     }
 
-template <int COLS, bool H>
-static cudaError_t launch_lift_kernel(int L, dim3 grid, cudaStream_t stream, const u64 *in, int polys_in, u64 *ext,
-                                      int ext_polys, int out_poly_offset, const LiftConsts &consts, int n, bool q_rows) {
-    HE_DISPATCH_L(L, (lift_kernel<LL, COLS, H><<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys, out_poly_offset,
-                                                                              consts, n, q_rows)));
-    return cudaSuccess;
-}
-template <int COLS, bool H>
-static cudaError_t launch_floor_kernel(int L, dim3 grid, cudaStream_t stream, const u64 *in, u64 *out,
-                                       const FloorConsts &consts, int n) {
-    HE_DISPATCH_L(L, (floor_kernel<LL, COLS, H><<<grid, kThreads, 0, stream>>>(in, out, consts, n)));
-    return cudaSuccess;
+static ColTiles col_tiles(int64_t n, int64_t polys, int cols) {
+    ColTiles tl;
+    tl.shift = 0;
+    while (((int64_t)kThreads * cols << tl.shift) < n) ++tl.shift;
+    tl.count = (long long)polys << tl.shift;
+    return tl;
 }
 
-// grid over (coefficient pairs, polys) with polys folded into y (<= 32768) and z
-static inline dim3 poly_grid(int64_t n, int64_t polys, int cols) {
-    const unsigned gx = (unsigned)((n / cols + kThreads - 1) / kThreads);
+// a lift / floor launch: one CTA per tile
+template <typename... KArgs, typename... Args>
+static cudaError_t launch_tiles(void (*kernel)(KArgs...), const ColTiles &tl, cudaStream_t stream, Args... args) {
+    if (tl.count == 0) return cudaSuccess;
+    if (tl.count > 0x7fffffffLL) return cudaErrorInvalidConfiguration;  // gridDim.x
+    ++g_kernel_launches;
+    kernel<<<(unsigned)tl.count, kThreads, 0, stream>>>(args..., tl);
+    return cudaGetLastError();
+}
+
+template <bool H, bool Q_ROWS>
+static cudaError_t launch_lift_tiles(const Context &ctx, const u64 *lhs, const u64 *rhs, int pin_shift, u64 *ext,
+                                     int64_t polys_out, const LiftConsts &consts, cudaStream_t stream) {
+    cudaError_t e;
+    HE_DISPATCH_L(ctx.L, (e = launch_tiles(lift_kernel<LL, H, Q_ROWS>, col_tiles(ctx.n, polys_out, BehzCols<LL>::value),
+                                           stream, lhs, rhs, pin_shift, ext, consts, (int)ctx.n)));
+    return e;
+}
+template <bool H, bool Q_SCALED>
+static cudaError_t launch_floor_tiles(const Context &ctx, const u64 *in, u64 *out, int64_t polys,
+                                      const FloorConsts &consts, cudaStream_t stream) {
+    cudaError_t e;
+    HE_DISPATCH_L(ctx.L, (e = launch_tiles(floor_kernel<LL, H, Q_SCALED>, col_tiles(ctx.n, polys, BehzCols<LL>::value),
+                                           stream, in, out, consts, (int)ctx.n)));
+    return e;
+}
+
+// grid over (coefficients, polys) with polys folded into y (<= 32768) and z: the kernels above 16 moduli
+static inline dim3 poly_grid(int64_t n, int64_t polys) {
+    const unsigned gx = (unsigned)((n + kThreads - 1) / kThreads);
     const int64_t gy = polys < 32768 ? polys : 32768;
     return dim3(gx ? gx : 1, (unsigned)gy, (unsigned)((polys + gy - 1) / gy));
 }
 
-cudaError_t launch_lift(const Context &ctx, const u64 *in, int polys_in, u64 *ext, int ext_polys, int out_poly_offset,
-                        int64_t items, cudaStream_t stream, bool reference_base, bool q_rows) {
-    const LiftConsts &consts = reference_base ? ctx.lift : ctx.lift_mul;
+static cudaError_t launch_lift_generic(const Context &ctx, const u64 *in, int polys_in, u64 *ext, int ext_polys,
+                                       int out_poly_offset, int64_t items, cudaStream_t stream, const LiftConsts &consts,
+                                       bool q_rows) {
     int64_t polys = items * polys_in;
-    if (polys == 0) return cudaSuccess;
     const int64_t pstride_in = (int64_t)ctx.L * ctx.n;
     // the z dimension must divide exactly: launch in slabs of y = 32768 polys, then the remainder
     while (polys > 0) {
         int64_t slab = polys >= 32768 ? (polys / 32768) * 32768 : polys;
-        const int cols = ctx.L > 16 ? 1 : (ctx.n >= 2 ? cols_per_thread() : 1);
-        const dim3 grid = poly_grid(ctx.n, slab, cols);
         ++g_kernel_launches;
-        if (ctx.L > 16) {
-            lift_generic_kernel<<<grid, kThreads, 0, stream>>>(in, polys_in, ext, ext_polys, out_poly_offset, consts, (int)ctx.n, q_rows);
-        } else {
-            auto launch = cols == 2 ? (consts.h_primes ? launch_lift_kernel<2, true> : launch_lift_kernel<2, false>)
-                                    : (consts.h_primes ? launch_lift_kernel<1, true> : launch_lift_kernel<1, false>);
-            const cudaError_t e = launch(ctx.L, grid, stream, in, polys_in, ext, ext_polys, out_poly_offset, consts, (int)ctx.n, q_rows);
-            if (e != cudaSuccess) return e;
-        }
+        lift_generic_kernel<<<poly_grid(ctx.n, slab), kThreads, 0, stream>>>(in, polys_in, ext, ext_polys, out_poly_offset,
+                                                                              consts, (int)ctx.n, q_rows);
         // advance whole items only (32768 is even and polys_in is 1 or 2)
         in += slab * pstride_in;
         ext += (slab / polys_in) * (int64_t)ext_polys * (q_rows ? 2 * ctx.L + 1 : ctx.L + 1) * ctx.n;
         polys -= slab;
     }
     return cudaGetLastError();
+}
+
+cudaError_t launch_lift(const Context &ctx, const u64 *lhs, const u64 *rhs, int polys_in, u64 *ext, int64_t items,
+                        cudaStream_t stream, bool reference_base, bool q_rows) {
+    const LiftConsts &consts = reference_base ? ctx.lift : ctx.lift_mul;
+    if (items == 0) return cudaSuccess;
+    if (polys_in != 1 && polys_in != 2) return cudaErrorInvalidValue;
+    const int ops = rhs ? 2 : 1;
+    if (ctx.L > 16) {
+        cudaError_t e = launch_lift_generic(ctx, lhs, polys_in, ext, ops * polys_in, 0, items, stream, consts, q_rows);
+        if (e == cudaSuccess && rhs)
+            e = launch_lift_generic(ctx, rhs, polys_in, ext, ops * polys_in, polys_in, items, stream, consts, q_rows);
+        return e;
+    }
+    const int64_t polys_out = items * ops * polys_in;
+    const int pin_shift = polys_in == 2 ? 1 : 0;
+    auto launch = consts.h_primes ? (q_rows ? launch_lift_tiles<true, true> : launch_lift_tiles<true, false>)
+                                  : (q_rows ? launch_lift_tiles<false, true> : launch_lift_tiles<false, false>);
+    return launch(ctx, lhs, rhs, pin_shift, ext, polys_out, consts, stream);
 }
 
 cudaError_t launch_tensor(const Context &ctx, const u64 *ext, u64 *ten, int64_t items, cudaStream_t stream,
@@ -409,11 +473,10 @@ cudaError_t launch_tensor(const Context &ctx, const u64 *ext, u64 *ten, int64_t 
         tc.ninv[r] = ctx.slots[map.slot[r]].dev.ninv;
         tc.h[r] = fast::class_of_modulus(tc.p[r], ctx.slots[map.slot[r]].dev.bits) == fast::kNarrowH ? 1 : 0;
     }
-    const int cols = ctx.n >= 2 ? cols_per_thread() : 1;
     bool any_h = false;
     for (int r = 0; r < tc.R; ++r) any_h |= tc.h[r] != 0;
-    auto k = cols == 2 ? (any_h ? tensor_kernel<2, true> : tensor_kernel<2, false>) : (any_h ? tensor_kernel<1, true> : tensor_kernel<1, false>);
-    const unsigned gx = (unsigned)((ctx.n / cols + kThreads - 1) / kThreads);
+    auto k = any_h ? tensor_kernel<2, true> : tensor_kernel<2, false>;  // N >= 2: two columns per thread
+    const unsigned gx = (unsigned)((ctx.n / 2 + kThreads - 1) / kThreads);
     for (int64_t done = 0; done < items;) {  // gridDim.z <= 65535
         const int64_t chunk = (items - done) > 65535 ? 65535 : (items - done);
         dim3 grid(gx ? gx : 1, (unsigned)tc.R, (unsigned)chunk);
@@ -457,24 +520,23 @@ cudaError_t launch_tensor_sum(const Context &ctx, const u64 *ext, u64 *ten, int6
     return cudaGetLastError();
 }
 
+bool floor_takes_scaled_q(const Context &ctx) { return ctx.L <= 16; }
+
 cudaError_t launch_floor(const Context &ctx, const u64 *in, u64 *out, int64_t polys, cudaStream_t stream,
-                         bool reference_base) {
+                         bool reference_base, bool q_scaled) {
     if (polys == 0) return cudaSuccess;
     const FloorConsts &consts = reference_base ? ctx.floor : ctx.floor_mul;
+    if (ctx.L <= 16) {
+        auto launch = consts.h_primes ? (q_scaled ? launch_floor_tiles<true, true> : launch_floor_tiles<true, false>)
+                                      : (q_scaled ? launch_floor_tiles<false, true> : launch_floor_tiles<false, false>);
+        return launch(ctx, in, out, polys, consts, stream);
+    }
+    if (q_scaled) return cudaErrorInvalidValue;  // floor_takes_scaled_q
     const int R = 2 * ctx.L + 1;
     while (polys > 0) {
         int64_t slab = polys >= 32768 ? (polys / 32768) * 32768 : polys;
-        const int cols = ctx.L > 16 ? 1 : (ctx.n >= 2 ? cols_per_thread() : 1);
-        const dim3 grid = poly_grid(ctx.n, slab, cols);
         ++g_kernel_launches;
-        if (ctx.L > 16) {
-            floor_generic_kernel<<<grid, kThreads, 0, stream>>>(in, out, consts, (int)ctx.n);
-        } else {
-            auto launch = cols == 2 ? (consts.h_primes ? launch_floor_kernel<2, true> : launch_floor_kernel<2, false>)
-                                    : (consts.h_primes ? launch_floor_kernel<1, true> : launch_floor_kernel<1, false>);
-            const cudaError_t e = launch(ctx.L, grid, stream, in, out, consts, (int)ctx.n);
-            if (e != cudaSuccess) return e;
-        }
+        floor_generic_kernel<<<poly_grid(ctx.n, slab), kThreads, 0, stream>>>(in, out, consts, (int)ctx.n);
         in += slab * (int64_t)R * ctx.n;
         out += slab * (int64_t)ctx.L * ctx.n;
         polys -= slab;

@@ -124,24 +124,25 @@ cudaError_t multiply_chunk(const Context &c, u64 *scratch, const u64 *lhs, const
     cudaError_t e;
     u64 *ext = scratch, *ten = scratch + 4 * poly_words * items;
     const NttRowMap map = c.map_qaux();
+    // dropExtendedBase: (* t) and the floor's first step ((Q/q_i)^-1 on the Q rows) folded into the inverse NTT
+    const bool scaled = floor_takes_scaled_q(c);
+    const int inv_scale = scaled ? kScaleTMontFloor : kScaleTMont;
     if (ntt_forward_tensor_supported(c)) {
         // computeBehzPolys + tensor product with the NTT outputs kept on chip (ntt_fast.cu): the lift writes only the
         // auxiliary rows, the kernel reads the Q rows from lhs / rhs
-        if ((e = launch_lift(c, lhs, 2, ext, 4, 0, items, s, false, false)) != cudaSuccess) return e;
-        if ((e = launch_lift(c, rhs, 2, ext, 4, 2, items, s, false, false)) != cudaSuccess) return e;
+        if ((e = launch_lift(c, lhs, rhs, 2, ext, items, s, false, false)) != cudaSuccess) return e;
         if ((e = launch_ntt_forward_tensor(c, map, lhs, rhs, ext, ten, items, s)) != cudaSuccess) return e;
-        if ((e = launch_ntt_inverse(c, map, ten, ten, items * 3 * R, kScaleTMont, s)) != cudaSuccess) return e;
-        return launch_floor(c, ten, out, items * 3, s);
+        if ((e = launch_ntt_inverse(c, map, ten, ten, items * 3 * R, inv_scale, s)) != cudaSuccess) return e;
+        return launch_floor(c, ten, out, items * 3, s, false, scaled);
     }
     // computeBehzPolys for both operands: lift + forward NTT      (Bfv+Multiply.swift:51-57)
-    if ((e = launch_lift(c, lhs, 2, ext, 4, 0, items, s)) != cudaSuccess) return e;
-    if ((e = launch_lift(c, rhs, 2, ext, 4, 2, items, s)) != cudaSuccess) return e;
+    if ((e = launch_lift(c, lhs, rhs, 2, ext, items, s)) != cudaSuccess) return e;
     if ((e = launch_ntt_forward(c, map, ext, ext, items * 4 * R, s)) != cudaSuccess) return e;
     // tensor product                                               (Bfv+Multiply.swift:80-82)
     if ((e = launch_tensor(c, ext, ten, items, s)) != cudaSuccess) return e;
-    // dropExtendedBase: (* t) folded into the inverse NTT, floor    (Bfv+Multiply.swift:31-48)
-    if ((e = launch_ntt_inverse(c, map, ten, ten, items * 3 * R, kScaleTMont, s)) != cudaSuccess) return e;
-    return launch_floor(c, ten, out, items * 3, s);
+    // dropExtendedBase: inverse NTT, floor                          (Bfv+Multiply.swift:31-48)
+    if ((e = launch_ntt_inverse(c, map, ten, ten, items * 3 * R, inv_scale, s)) != cudaSuccess) return e;
+    return launch_floor(c, ten, out, items * 3, s, false, scaled);
 }
 
 // _computeKeySwitchingUpdate (Bfv+Keys.swift:123-208) of `target` (l rows per item, items `target_stride` words apart)
@@ -191,12 +192,13 @@ cudaError_t inner_product_chunk(const Context &c, u64 *scratch, const u64 *lhs, 
     u64 *ext = scratch, *ten = scratch + 4 * poly_words * items;
     const NttRowMap map = c.map_qaux();
     cudaError_t e;
-    if ((e = launch_lift(c, lhs, 2, ext, 4, 0, items, s)) != cudaSuccess) return e;
-    if ((e = launch_lift(c, rhs, 2, ext, 4, 2, items, s)) != cudaSuccess) return e;
+    const bool scaled = floor_takes_scaled_q(c);
+    if ((e = launch_lift(c, lhs, rhs, 2, ext, items, s)) != cudaSuccess) return e;
     if ((e = launch_ntt_forward(c, map, ext, ext, items * 4 * R, s)) != cudaSuccess) return e;
     if ((e = launch_tensor_sum(c, ext, ten, pairs, groups, s)) != cudaSuccess) return e;
-    if ((e = launch_ntt_inverse(c, map, ten, ten, groups * 3 * R, kScaleTMont, s)) != cudaSuccess) return e;
-    return launch_floor(c, ten, out, groups * 3, s);
+    if ((e = launch_ntt_inverse(c, map, ten, ten, groups * 3 * R, scaled ? kScaleTMontFloor : kScaleTMont, s)) != cudaSuccess)
+        return e;
+    return launch_floor(c, ten, out, groups * 3, s, false, scaled);
 }
 size_t inner_product_scratch_words(const Context &c, int64_t pairs) {
     return (size_t)(4 * pairs + 3) * (2 * c.L + 1) * c.n;
@@ -560,7 +562,7 @@ int32_t hecuda_rnstool_lift_q_to_qbsk(const hecuda_context *h, const uint64_t *p
     std::vector<HostIo> in = {{(const u64 *)polys, in_words}};
     return host_pipeline(h, count, std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / out_words)), 0, in, (u64 *)out, out_words,
                          [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t n_items) {
-                             return launch_lift(c, d_in[0], 1, d_out, 1, 0, n_items, w.stream, /*reference_base=*/true);
+                             return launch_lift(c, d_in[0], nullptr, 1, d_out, n_items, w.stream, /*reference_base=*/true);
                          });
 }
 int32_t hecuda_rnstool_floor_qbsk_to_q(const hecuda_context *h, const uint64_t *polys, uint64_t *out, int64_t count) {

@@ -21,7 +21,8 @@ static void fill_barrett(u64 p, u64 &mu1, u64 &mu_hi, u64 &mu_lo) {
     mu_lo = (u64)mu;
 }
 
-static bool build_slot(HostSlot &hs, u64 p, int64_t n, int logn, u64 t, std::vector<ulonglong2> &tw,
+// floor_w: the extra factor of kScaleTMontFloor ((Q/q_i)^-1 mod q_i on a ciphertext modulus, 1 elsewhere)
+static bool build_slot(HostSlot &hs, u64 p, int64_t n, int logn, u64 t, u64 floor_w, std::vector<ulonglong2> &tw,
                        std::vector<ulonglong2> &itw, std::string &err) {
     if (!is_prime(p) || (p - 1) % (2 * (u64)n) != 0) {
         err = "invalidNttModulus: " + std::to_string(p) + " is not a prime = 1 mod 2N";
@@ -67,8 +68,8 @@ static bool build_slot(HostSlot &hs, u64 p, int64_t n, int logn, u64 t, std::vec
         for (int i = 0; i < 6; ++i) inv *= 2 - p * inv;
         d.ninv = 0 - inv;
     }
-    const u64 scalings[3] = {1 % p, mulmod(t % p, d.r64, p), d.r64};
-    for (int k = 0; k < 3; ++k) {
+    const u64 scalings[4] = {1 % p, mulmod(t % p, d.r64, p), d.r64, mulmod(mulmod(t % p, d.r64, p), floor_w % p, p)};
+    for (int k = 0; k < 4; ++k) {
         ModSlot::InvScale &sc = d.inv_scale[k];
         sc.c0 = mulmod(n_inv, scalings[k], p);
         sc.c0p = shoup_factor(sc.c0, p);
@@ -210,7 +211,8 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
             dev_slots[s] = c->slots[s].dev;
             continue;
         }
-        if (!build_slot(c->slots[s], slot_mod[s], n, c->logn, t, tw, itw, err)) { delete c; return nullptr; }
+        const u64 floor_w = s < L ? invmod(punctured_mod(c->q.data(), L, s, slot_mod[s]), slot_mod[s]) : 1;  // slot_q(i) = i
+        if (!build_slot(c->slots[s], slot_mod[s], n, c->logn, t, floor_w, tw, itw, err)) { delete c; return nullptr; }
         char *base = (char *)c->d_pool + slot_bytes * s;
         cudaMemcpy(base, tw.data(), table_bytes, cudaMemcpyHostToDevice);
         cudaMemcpy(base + table_bytes, itw.data(), table_bytes, cudaMemcpyHostToDevice);
@@ -321,19 +323,17 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
         const u64 bj = BSK[j];
         fl.b[j] = bj;
         fl.b_ninv[j] = c->slots[slot_of(j)].dev.ninv;
-        const u64 q_inv = mulmod(invmod(prod_mod(Q, L, bj), bj), c->slots[slot_of(j)].dev.r64, bj);  // Q^-1 2^64
+        fl.b_mu1[j] = (u64)(((u128)1 << 64) / bj);
+        // Q^-1 2^64, times (B/b_j)^-1 on the rows whose f_j only feeds w_j = [f_j (B/b_j)^-1]_{b_j}
+        u64 q_inv = mulmod(invmod(prod_mod(Q, L, bj), bj), c->slots[slot_of(j)].dev.r64, bj);
+        if (j < L) q_inv = mulmod(q_inv, invmod(punctured_mod(BSK, L, j, bj), bj), bj);
         fl.fq[j] = q_inv;
         for (int i = 0; i < L; ++i) {
             const u64 v = mulmod(punctured_mod(Q, L, i, bj), q_inv, bj);
             fl.fmat[j][i] = (bj - v) % bj;
         }
     }
-    for (int k = 0; k < L; ++k) {
-        const u64 bk = BSK[k];
-        fl.inb_w[k] = invmod(punctured_mod(BSK, L, k, bk), bk);
-        fl.inb_wp[k] = shoup_factor(fl.inb_w[k], bk);
-        fl.amat[k] = mulmod(punctured_mod(BSK, L, k, msk), b_inv_msk, msk);
-    }
+    for (int k = 0; k < L; ++k) fl.amat[k] = mulmod(punctured_mod(BSK, L, k, msk), b_inv_msk, msk);
     };
     build_behz(c->bsk, true, c->lift, c->floor);
     if (c->aux_is_reference) {

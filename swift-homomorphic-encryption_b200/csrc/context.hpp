@@ -36,7 +36,9 @@ struct ModSlot {
     //   kScalePlain  s = 1                 the reference's inverseNtt
     //   kScaleTMont  s = t 2^64            after the Montgomery-form tensor product; folds `poly * tVec` (Bfv+Multiply.swift:40)
     //   kScaleMont   s = 2^64              after the Montgomery-reduced key-switch accumulation
-    struct InvScale { u64 c0, c0p, c1, c1p; } inv_scale[3];
+    //   kScaleTMontFloor  s = t 2^64 (Q/q_i)^-1 on the ciphertext moduli q_i, t 2^64 elsewhere: kScaleTMont with the
+    //                     floor's first step y_i = [x_i (Q/q_i)^-1]_{q_i} (RnsTool.swift:378-398) folded in
+    struct InvScale { u64 c0, c0p, c1, c1p; } inv_scale[4];
     const ulonglong2 *tw;     // forward twiddles  [N]
     const ulonglong2 *itw;    // inverse twiddles  [N]  (itw[m+i] = tw[m+i]^-1)
     // transposed copies for the register-tiled kernels' line-owning pass (ntt_fast.cuh): entry k (< 15) of thread
@@ -45,7 +47,7 @@ struct ModSlot {
     const ulonglong2 *itw_t;
 };
 
-enum { kScalePlain = 0, kScaleTMont = 1, kScaleMont = 2 };
+enum { kScalePlain = 0, kScaleTMont = 1, kScaleMont = 2, kScaleTMontFloor = 3 };
 
 struct NttRowMap {       // which modulus slot each row of a polynomial uses:
     int rows_per_poly;   //   slot[((row % rows_per_poly) / group)]
@@ -79,8 +81,10 @@ struct LiftConsts {
 };
 
 // floorQBskToQ (RnsTool.swift:378-456) fused to (all matrix constants pre-multiplied by 2^64, sums Montgomery-reduced):
-//   y_i = [x_i inq_w_i]_{q_i} (canonical);  f_j = [x_bj fq[j] + sum_i y_i fmat[j][i]]_{b_j}  (approximateFloor, lazy < 2 b_j)
-//   w_k = [f_k inb_w_k]_{b_k} (canonical);  alpha = [sum_k w_k amat[k] + f_msk a_msk]_{m_sk}  (Shenoy-Kumaresan)
+//   y_i = [x_i inq_w_i]_{q_i} (canonical);  f_j = [x_bj fq[j] + sum_i y_i fmat[j][i]]_{b_j}  (approximateFloor)
+//   for j = k < L the row constants also carry (B/b_k)^-1, so f_k is already w_k = [f_k (B/b_k)^-1]_{b_k} (canonical
+//   after a conditional subtraction, or a Barrett reduction with wide_sums);  f_msk = f_L stays lazy (< 2 m_sk)
+//   alpha = [sum_k w_k amat[k] + f_msk a_msk]_{m_sk}  (Shenoy-Kumaresan)
 //   out_i = [sum_k w_k omat[i][k] + alpha' D_i]_{q_i},  (alpha', D) = alpha > m_sk/2 ? (m_sk-alpha, B) : (alpha, -B)
 struct FloorConsts {
     int L;
@@ -89,9 +93,9 @@ struct FloorConsts {
     u64 q[kMaxL], q_ninv[kMaxL], q_mu1[kMaxL];
     u64 inq_w[kMaxL], inq_wp[kMaxL];   // (Q/q_i)^-1 mod q_i
     u64 b[kMaxL + 1], b_ninv[kMaxL + 1];
-    u64 fq[kMaxL + 1];                 // Q^-1 2^64 mod b_j
-    u64 fmat[kMaxL + 1][kMaxL];        // -(Q/q_i) Q^-1 2^64 mod b_j
-    u64 inb_w[kMaxL], inb_wp[kMaxL];   // (B/b_k)^-1 mod b_k
+    u64 b_mu1[kMaxL + 1];              // floor(2^64 / b_j)
+    u64 fq[kMaxL + 1];                 // Q^-1 2^64 [(B/b_j)^-1 for j < L] mod b_j
+    u64 fmat[kMaxL + 1][kMaxL];        // -(Q/q_i) Q^-1 2^64 [(B/b_j)^-1 for j < L] mod b_j
     u64 amat[kMaxL];                   // (B/b_k) B^-1 2^64 mod m_sk
     u64 a_msk;                         // -B^-1 2^64 mod m_sk
     u64 omat[kMaxL][kMaxL];            // (B/b_k) 2^64 mod q_i

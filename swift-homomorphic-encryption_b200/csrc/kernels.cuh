@@ -40,20 +40,22 @@ cudaError_t launch_ntt_forward_tensor(const Context &ctx, const NttRowMap &map, 
 
 // ---- BEHZ steps of ct x ct multiply (behz.cu).  reference_base: compute over the reference's [Q, Bsk] (stage-level
 // entry points) instead of the [Q, aux] base the fused multiply uses (context.hpp).
-// lift: `items` x polys_in x L x N  ->  ext[item][out_poly_offset + p][R][N]  with ext item stride ext_polys*R*N;
-// q_rows = false: the L + 1 auxiliary rows only (ext[item][out_poly_offset + p][L + 1][N]), for a consumer that reads
-// the Q rows from the input itself
-cudaError_t launch_lift(const Context &ctx, const u64 *in, int polys_in, u64 *ext, int ext_polys, int out_poly_offset,
-                        int64_t items, cudaStream_t stream, bool reference_base = false, bool q_rows = true);
+// lift: lhs (and rhs, unless null), each `items` x polys_in x L x N (polys_in 1 or 2), in one launch  ->
+// ext[item][op][p][R][N] with op 0 for lhs, 1 for rhs; q_rows = false: the L + 1 auxiliary rows only
+// (ext[item][op][p][L + 1][N]), for a consumer that reads the Q rows from the input itself
+cudaError_t launch_lift(const Context &ctx, const u64 *lhs, const u64 *rhs, int polys_in, u64 *ext, int64_t items,
+                        cudaStream_t stream, bool reference_base = false, bool q_rows = true);
 // tensor: ext[item][4][R][N] (Eval) -> ten[item][3][R][N]
 cudaError_t launch_tensor(const Context &ctx, const u64 *ext, u64 *ten, int64_t items, cudaStream_t stream,
                           bool reference_base = false);
 // tensor sum: ext[group][pair][4][R][N] (Eval) -> ten[group][3][R][N]  (Bfv.innerProduct(_:_:), Bfv.swift:315-361)
 cudaError_t launch_tensor_sum(const Context &ctx, const u64 *ext, u64 *ten, int64_t pairs, int64_t groups,
                               cudaStream_t stream, bool reference_base = false);
-// floor: polys x R x N (Coeff, already scaled by t) -> polys x L x N
+// floor: polys x R x N (Coeff, already scaled by t) -> polys x L x N.  q_scaled: the Q rows are already multiplied
+// by (Q/q_i)^-1 (an inverse NTT with kScaleTMontFloor instead of kScaleTMont); only where floor_takes_scaled_q
+bool floor_takes_scaled_q(const Context &ctx);
 cudaError_t launch_floor(const Context &ctx, const u64 *in, u64 *out, int64_t polys, cudaStream_t stream,
-                         bool reference_base = false);
+                         bool reference_base = false, bool q_scaled = false);
 
 // ---- key switching and modulus switching (keyswitch.cu)
 // mac: dig (Eval) x key -> prod[item][2][l+1][N] (Eval)
