@@ -291,7 +291,7 @@ int32_t hecuda_pir_database_create(const hecuda_context *ctx, const uint64_t *pl
 int32_t hecuda_pir_database_destroy(hecuda_pir_database *db);
 /* The resident rows (for a device-to-device copy between ranks).  When every ciphertext modulus is below 2^31 -- the
  * reference's default PIR parameters -- the rows are kept as uint32 (half the bytes per first-dimension scan) and
- * `bytes` = count * L * N * 4; otherwise uint64 and `bytes` = count * L * N * 8.  HECUDA_PIR_COMPACT=0 forces uint64. */
+ * `bytes` = count * L * N * 4; otherwise uint64 and `bytes` = count * L * N * 8. */
 int32_t hecuda_pir_database_device_buffer(hecuda_pir_database *db, void **device_ptr, uint64_t *bytes);
 
 /* PirUtil.expand(ciphertexts:outputCount:using:) -- IndexPir/PirUtil.swift:321-355 (expandCiphertext :249-304,

@@ -53,15 +53,9 @@ namespace hecuda {
 namespace api {
 
 cudaError_t wait_stream(cudaStream_t s) {
-    // Default: yield the CPU while waiting (an event created with cudaEventBlockingSync).  Spinning in
-    // cudaStreamSynchronize burns a core per waiting thread; with many serving threads inside a CPU-quota'd container
-    // the spinners get throttled and throughput collapses and swings from run to run.  HECUDA_BLOCKING_SYNC=0 restores
-    // the spin wait.
-    static const bool blocking = [] {
-        const char *env = std::getenv("HECUDA_BLOCKING_SYNC");
-        return !(env && env[0] == '0');
-    }();
-    if (!blocking) return cudaStreamSynchronize(s);
+    // Yield the CPU while waiting (an event created with cudaEventBlockingSync).  Spinning in cudaStreamSynchronize
+    // burns a core per waiting thread; with many serving threads inside a CPU-quota'd container the spinners get
+    // throttled and throughput collapses and swings from run to run.
     thread_local cudaEvent_t event = nullptr;
     thread_local int event_device = -1;
     int device = 0;

@@ -132,7 +132,7 @@ struct WsGuard {
 int32_t check_ctx(const hecuda_context *h);
 
 // Wait for a stream from a host thread: yields the CPU (an event created with cudaEventBlockingSync, one per thread)
-// unless HECUDA_BLOCKING_SYNC=0 asks for the spinning cudaStreamSynchronize.
+// instead of spinning in cudaStreamSynchronize.
 cudaError_t wait_stream(cudaStream_t s);
 bool make_map(const Context &c, int32_t base, int32_t rows, NttRowMap &map, std::string &err);
 

@@ -25,34 +25,26 @@ __device__ __forceinline__ u128w to_w(u128 v) {
     return r;
 }
 
-// ROWS output rows per thread: every query-ciphertext value fetched through L2 is used ROWS times, so the L2 traffic
-// per streamed plaintext byte drops from 3x to (1 + 2/ROWS)x.
-template <int NPOLY, int ROWS, bool HAS_PRESENT>
+// One output row (blockIdx.z) per thread: more rows per thread, each reusing the query-ciphertext values fetched
+// through L2, cost registers and measured slower.
+template <int NPOLY, bool HAS_PRESENT>
 __global__ void __launch_bounds__(128) inner_product_plain_kernel(const u64 *__restrict__ cts, const u64 *__restrict__ pts,
                                                                  const unsigned char *__restrict__ present,
                                                                  u64 *__restrict__ out,
                                                                  const __grid_constant__ IpConsts c, int n,
-                                                                 long long terms, long long out_count) {
+                                                                 long long terms) {
     const int coeff = (blockIdx.x * 128 + threadIdx.x) * 2;
     if (coeff >= n) return;
     const int r = blockIdx.y, l = c.l;
-    const long long o0 = (long long)blockIdx.z * ROWS;
+    const long long o = blockIdx.z;
     const u64 p = c.p[r], mu_hi = c.mu_hi[r], mu_lo = c.mu_lo[r];
-    u128 acc[ROWS][NPOLY][2];
+    u128 acc[NPOLY][2];
 #pragma unroll
-    for (int i = 0; i < ROWS; ++i)
-#pragma unroll
-        for (int q = 0; q < NPOLY; ++q) acc[i][q][0] = acc[i][q][1] = 0;
+    for (int q = 0; q < NPOLY; ++q) acc[q][0] = acc[q][1] = 0;
     const long long pt_stride = (long long)l * n, ct_stride = (long long)NPOLY * l * n;
     const u64 *ct = cts + (long long)r * n + coeff;
-    const u64 *pt[ROWS];
-    const unsigned char *pres[ROWS];
-#pragma unroll
-    for (int i = 0; i < ROWS; ++i) {
-        const long long o = o0 + i < out_count ? o0 + i : out_count - 1;  // clamp: surplus rows recompute the last one
-        pt[i] = pts + ((o * terms) * l + r) * (long long)n + coeff;
-        pres[i] = HAS_PRESENT ? present + o * terms : nullptr;
-    }
+    const u64 *pt = pts + ((o * terms) * l + r) * (long long)n + coeff;
+    const unsigned char *pres = HAS_PRESENT ? present + o * terms : nullptr;
     long long since_reduce = 0;
 #pragma unroll 2
     for (long long k = 0; k < terms; ++k) {
@@ -60,44 +52,29 @@ __global__ void __launch_bounds__(128) inner_product_plain_kernel(const u64 *__r
 #pragma unroll
         for (int q = 0; q < NPOLY; ++q)
             cv[q] = __ldg(reinterpret_cast<const ulonglong2 *>(ct + k * ct_stride + (long long)q * pt_stride));
-#pragma unroll
-        for (int i = 0; i < ROWS; ++i) {
-            if (HAS_PRESENT && !pres[i][k]) continue;  // nil plaintext (Bfv.swift:493), uniform across the block
-            const ulonglong2 pv = __ldcs(reinterpret_cast<const ulonglong2 *>(pt[i] + k * pt_stride));
+        if (!HAS_PRESENT || pres[k]) {  // nil plaintext (Bfv.swift:493), uniform across the block
+            const ulonglong2 pv = __ldcs(reinterpret_cast<const ulonglong2 *>(pt + k * pt_stride));
 #pragma unroll
             for (int q = 0; q < NPOLY; ++q) {
-                mac128(acc[i][q][0], cv[q].x, pv.x);
-                mac128(acc[i][q][1], cv[q].y, pv.y);
+                mac128(acc[q][0], cv[q].x, pv.x);
+                mac128(acc[q][1], cv[q].y, pv.y);
             }
         }
         if (++since_reduce >= c.max_terms) {  // reduceInPlace, Bfv.swift:365-377
             since_reduce = 0;
 #pragma unroll
-            for (int i = 0; i < ROWS; ++i)
-#pragma unroll
-                for (int q = 0; q < NPOLY; ++q) {
-                    acc[i][q][0] = barrett128(to_w(acc[i][q][0]), p, mu_hi, mu_lo);
-                    acc[i][q][1] = barrett128(to_w(acc[i][q][1]), p, mu_hi, mu_lo);
-                }
+            for (int q = 0; q < NPOLY; ++q) {
+                acc[q][0] = barrett128(to_w(acc[q][0]), p, mu_hi, mu_lo);
+                acc[q][1] = barrett128(to_w(acc[q][1]), p, mu_hi, mu_lo);
+            }
         }
     }
 #pragma unroll
-    for (int i = 0; i < ROWS; ++i) {
-        if (o0 + i >= out_count) break;
-#pragma unroll
-        for (int q = 0; q < NPOLY; ++q) {  // reduceToCiphertext, Bfv.swift:380-394
-            u64 *dst = out + ((((o0 + i) * NPOLY + q) * l + r) * (long long)n) + coeff;
-            *reinterpret_cast<ulonglong2 *>(dst) = make_ulonglong2(barrett128(to_w(acc[i][q][0]), p, mu_hi, mu_lo),
-                                                                   barrett128(to_w(acc[i][q][1]), p, mu_hi, mu_lo));
-        }
+    for (int q = 0; q < NPOLY; ++q) {  // reduceToCiphertext, Bfv.swift:380-394
+        u64 *dst = out + (((o * NPOLY + q) * l + r) * (long long)n) + coeff;
+        *reinterpret_cast<ulonglong2 *>(dst) =
+            make_ulonglong2(barrett128(to_w(acc[q][0]), p, mu_hi, mu_lo), barrett128(to_w(acc[q][1]), p, mu_hi, mu_lo));
     }
-}
-
-template <int NPOLY, int ROWS>
-static void launch_ip(dim3 grid, cudaStream_t stream, const u64 *cts, const u64 *pt, const unsigned char *pr, u64 *o,
-                      const IpConsts &c, int n, long long terms, long long rows) {
-    if (pr) inner_product_plain_kernel<NPOLY, ROWS, true><<<grid, 128, 0, stream>>>(cts, pt, pr, o, c, n, terms, rows);
-    else inner_product_plain_kernel<NPOLY, ROWS, false><<<grid, 128, 0, stream>>>(cts, pt, pr, o, c, n, terms, rows);
 }
 
 cudaError_t launch_inner_product_plain(const Context &ctx, const u64 *cts, int npoly, int l, int64_t terms, const u64 *pts,
@@ -118,24 +95,19 @@ cudaError_t launch_inner_product_plain(const Context &ctx, const u64 *cts, int n
     const u128 max_count = ((~(u128)0) - qmax) / max_product;
     c.max_terms = max_count > (u128)0x7fffffffffffffffLL ? 0x7fffffffffffffffLL : (long long)max_count;
     const unsigned gx = (unsigned)((ctx.n / 2 + 127) / 128);
-    const int rows_per_thread = 1;  // more rows per thread cost registers; one row per thread was the fastest
-    const int64_t max_rows = (int64_t)65535 * rows_per_thread;
+    // [npoly - 1][present given]
+    static void (*const kernels[3][2])(const u64 *, const u64 *, const unsigned char *, u64 *, IpConsts, int, long long) = {
+        {inner_product_plain_kernel<1, false>, inner_product_plain_kernel<1, true>},
+        {inner_product_plain_kernel<2, false>, inner_product_plain_kernel<2, true>},
+        {inner_product_plain_kernel<3, false>, inner_product_plain_kernel<3, true>}};
     for (int64_t done = 0; done < out_count;) {
-        const int64_t chunk = (out_count - done) > max_rows ? max_rows : (out_count - done);
-        dim3 grid(gx ? gx : 1, (unsigned)l, (unsigned)((chunk + rows_per_thread - 1) / rows_per_thread));
+        const int64_t chunk = (out_count - done) > 65535 ? 65535 : (out_count - done);
+        dim3 grid(gx ? gx : 1, (unsigned)l, (unsigned)chunk);
         const u64 *pt = pts + done * terms * l * ctx.n;
         const unsigned char *pr = present ? present + done * terms : nullptr;
         u64 *o = out + done * npoly * l * ctx.n;
         ++g_kernel_launches;
-        const int key = npoly * 10 + rows_per_thread;
-        switch (key) {
-            case 11: launch_ip<1, 1>(grid, stream, cts, pt, pr, o, c, (int)ctx.n, terms, chunk); break;
-            case 12: launch_ip<1, 2>(grid, stream, cts, pt, pr, o, c, (int)ctx.n, terms, chunk); break;
-            case 21: launch_ip<2, 1>(grid, stream, cts, pt, pr, o, c, (int)ctx.n, terms, chunk); break;
-            case 22: launch_ip<2, 2>(grid, stream, cts, pt, pr, o, c, (int)ctx.n, terms, chunk); break;
-            case 31: launch_ip<3, 1>(grid, stream, cts, pt, pr, o, c, (int)ctx.n, terms, chunk); break;
-            default: launch_ip<3, 2>(grid, stream, cts, pt, pr, o, c, (int)ctx.n, terms, chunk); break;
-        }
+        kernels[npoly - 1][pr != nullptr]<<<grid, 128, 0, stream>>>(cts, pt, pr, o, c, (int)ctx.n, terms);
         done += chunk;
     }
     return cudaGetLastError();
@@ -149,75 +121,54 @@ struct IpSmallConsts {
     int max_terms;
     u64 p[kMaxL], mu1[kMaxL];
 };
-// ROWS database rows per thread: each query-ciphertext value fetched through L2 (8 bytes per residue, against 4 bytes of
-// streamed database) is used ROWS times.
-template <int NPOLY, int ROWS, bool HAS_PRESENT>
+// One database row (blockIdx.z) per thread: at the config-4 shape (437 terms x 75 rows) so few rows make the grid, not
+// L2, the limit.
+template <int NPOLY, bool HAS_PRESENT>
 __global__ void __launch_bounds__(128) inner_product_plain_small_kernel(const u64 *__restrict__ cts, const u32 *__restrict__ pts,
                                                                        const unsigned char *__restrict__ present,
                                                                        u64 *__restrict__ out,
                                                                        const __grid_constant__ IpSmallConsts c, int n,
-                                                                       long long terms, long long out_count) {
+                                                                       long long terms) {
     const int coeff = (blockIdx.x * 128 + threadIdx.x) * 4;  // four adjacent coefficients: 16-byte loads of the uint32 rows
     if (coeff >= n) return;
     const int r = blockIdx.y, l = c.l;
-    const long long o0 = (long long)blockIdx.z * ROWS;
+    const long long o = blockIdx.z;
     const u64 p = c.p[r], mu1 = c.mu1[r];
-    u64 acc[ROWS][NPOLY][4];
+    u64 acc[NPOLY][4];
 #pragma unroll
-    for (int i = 0; i < ROWS; ++i)
-#pragma unroll
-        for (int q = 0; q < NPOLY; ++q) acc[i][q][0] = acc[i][q][1] = acc[i][q][2] = acc[i][q][3] = 0;
+    for (int q = 0; q < NPOLY; ++q) acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0;
     const long long pt_stride = (long long)l * n, ct_stride = (long long)NPOLY * l * n;
     const u64 *ct = cts + (long long)r * n + coeff;
-    const u32 *pt[ROWS];
-    const unsigned char *pres[ROWS];
-#pragma unroll
-    for (int i = 0; i < ROWS; ++i) {
-        const long long o = o0 + i < out_count ? o0 + i : out_count - 1;  // clamp: surplus rows recompute the last one
-        pt[i] = pts + ((o * terms) * l + r) * (long long)n + coeff;
-        pres[i] = HAS_PRESENT ? present + o * terms : nullptr;
-    }
+    const u32 *pt = pts + ((o * terms) * l + r) * (long long)n + coeff;
+    const unsigned char *pres = HAS_PRESENT ? present + o * terms : nullptr;
     int since_reduce = 0;
 #pragma unroll 2
     for (long long k = 0; k < terms; ++k) {
-        uint4 pv[ROWS];
-#pragma unroll
-        for (int i = 0; i < ROWS; ++i) pv[i] = __ldcs(reinterpret_cast<const uint4 *>(pt[i] + k * pt_stride));
+        const uint4 pv = __ldcs(reinterpret_cast<const uint4 *>(pt + k * pt_stride));
 #pragma unroll
         for (int q = 0; q < NPOLY; ++q) {
             const u64 *cq = ct + k * ct_stride + (long long)q * pt_stride;
             const ulonglong2 c01 = __ldg(reinterpret_cast<const ulonglong2 *>(cq));
             const ulonglong2 c23 = __ldg(reinterpret_cast<const ulonglong2 *>(cq + 2));
-#pragma unroll
-            for (int i = 0; i < ROWS; ++i) {
-                if (HAS_PRESENT && !pres[i][k]) continue;  // nil plaintext (Bfv.swift:493), uniform across the block
-                acc[i][q][0] += (u64)(u32)c01.x * pv[i].x;
-                acc[i][q][1] += (u64)(u32)c01.y * pv[i].y;
-                acc[i][q][2] += (u64)(u32)c23.x * pv[i].z;
-                acc[i][q][3] += (u64)(u32)c23.y * pv[i].w;
-            }
+            if (HAS_PRESENT && !pres[k]) continue;  // nil plaintext (Bfv.swift:493), uniform across the block
+            acc[q][0] += (u64)(u32)c01.x * pv.x;
+            acc[q][1] += (u64)(u32)c01.y * pv.y;
+            acc[q][2] += (u64)(u32)c23.x * pv.z;
+            acc[q][3] += (u64)(u32)c23.y * pv.w;
         }
         if (++since_reduce >= c.max_terms) {  // reduceInPlace, Bfv.swift:365-377
             since_reduce = 0;
 #pragma unroll
-            for (int i = 0; i < ROWS; ++i)
+            for (int q = 0; q < NPOLY; ++q)
 #pragma unroll
-                for (int q = 0; q < NPOLY; ++q)
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) acc[i][q][j] = barrett64(acc[i][q][j], p, mu1);
+                for (int j = 0; j < 4; ++j) acc[q][j] = barrett64(acc[q][j], p, mu1);
         }
     }
 #pragma unroll
-    for (int i = 0; i < ROWS; ++i) {
-        if (o0 + i >= out_count) break;
-#pragma unroll
-        for (int q = 0; q < NPOLY; ++q) {  // reduceToCiphertext, Bfv.swift:380-394
-            u64 *dst = out + ((((o0 + i) * NPOLY + q) * l + r) * (long long)n) + coeff;
-            reinterpret_cast<ulonglong2 *>(dst)[0] =
-                make_ulonglong2(barrett64(acc[i][q][0], p, mu1), barrett64(acc[i][q][1], p, mu1));
-            reinterpret_cast<ulonglong2 *>(dst)[1] =
-                make_ulonglong2(barrett64(acc[i][q][2], p, mu1), barrett64(acc[i][q][3], p, mu1));
-        }
+    for (int q = 0; q < NPOLY; ++q) {  // reduceToCiphertext, Bfv.swift:380-394
+        u64 *dst = out + (((o * NPOLY + q) * l + r) * (long long)n) + coeff;
+        reinterpret_cast<ulonglong2 *>(dst)[0] = make_ulonglong2(barrett64(acc[q][0], p, mu1), barrett64(acc[q][1], p, mu1));
+        reinterpret_cast<ulonglong2 *>(dst)[1] = make_ulonglong2(barrett64(acc[q][2], p, mu1), barrett64(acc[q][3], p, mu1));
     }
 }
 
@@ -247,33 +198,19 @@ cudaError_t launch_inner_product_plain_small(const Context &ctx, const u64 *cts,
     c.max_terms = max_count > 0x7fffffff ? 0x7fffffff : (int)max_count;
     if (c.max_terms < 1) return cudaErrorInvalidValue;
     const unsigned gx = (unsigned)((ctx.n / 4 + 127) / 128);
-    // one row per thread: at the config-4 shape (437 terms x 75 rows) so few rows make the grid, not L2, the limit;
-    // HECUDA_IPS_ROWS overrides
-    static const int rows_per_thread = [] {
-        const char *env = std::getenv("HECUDA_IPS_ROWS");
-        const int v = env ? std::atoi(env) : 1;
-        return v >= 4 ? 4 : v >= 2 ? 2 : 1;
-    }();
-    const int rows = npoly == 3 ? 1 : rows_per_thread;
-    const int64_t max_rows = (int64_t)65535 * rows;
+    // [npoly - 1][present given]
+    static void (*const kernels[3][2])(const u64 *, const u32 *, const unsigned char *, u64 *, IpSmallConsts, int, long long) = {
+        {inner_product_plain_small_kernel<1, false>, inner_product_plain_small_kernel<1, true>},
+        {inner_product_plain_small_kernel<2, false>, inner_product_plain_small_kernel<2, true>},
+        {inner_product_plain_small_kernel<3, false>, inner_product_plain_small_kernel<3, true>}};
     for (int64_t done = 0; done < out_count;) {
-        const int64_t chunk = (out_count - done) > max_rows ? max_rows : (out_count - done);
-        dim3 grid(gx ? gx : 1, (unsigned)l, (unsigned)((chunk + rows - 1) / rows));
+        const int64_t chunk = (out_count - done) > 65535 ? 65535 : (out_count - done);
+        dim3 grid(gx ? gx : 1, (unsigned)l, (unsigned)chunk);
         const u32 *pt = pts + done * terms * l * ctx.n;
         const unsigned char *pr = present ? present + done * terms : nullptr;
         u64 *o = out + done * npoly * l * ctx.n;
         ++g_kernel_launches;
-#define HE_IPS(NP, RW)                                                                                                       \
-    if (pr) inner_product_plain_small_kernel<NP, RW, true><<<grid, 128, 0, stream>>>(cts, pt, pr, o, c, (int)ctx.n, terms, chunk); \
-    else inner_product_plain_small_kernel<NP, RW, false><<<grid, 128, 0, stream>>>(cts, pt, pr, o, c, (int)ctx.n, terms, chunk);
-        if (npoly == 3) { HE_IPS(3, 1) }
-        else if (npoly == 2 && rows == 4) { HE_IPS(2, 4) }
-        else if (npoly == 2 && rows == 2) { HE_IPS(2, 2) }
-        else if (npoly == 2) { HE_IPS(2, 1) }
-        else if (rows == 4) { HE_IPS(1, 4) }
-        else if (rows == 2) { HE_IPS(1, 2) }
-        else { HE_IPS(1, 1) }
-#undef HE_IPS
+        kernels[npoly - 1][pr != nullptr]<<<grid, 128, 0, stream>>>(cts, pt, pr, o, c, (int)ctx.n, terms);
         done += chunk;
     }
     return cudaGetLastError();

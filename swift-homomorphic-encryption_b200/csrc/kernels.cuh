@@ -25,14 +25,13 @@ cudaError_t launch_ntt_forward_simple(const Context &ctx, const NttRowMap &map, 
 cudaError_t launch_ntt_inverse_simple(const Context &ctx, const NttRowMap &map, const u64 *in, u64 *out, int64_t rows,
                                       int scale_mode, cudaStream_t stream);
 
-// register-tiled kernels (ntt_fast.cu), N = 2^10 .. 2^14
+// register-tiled kernels (ntt_fast.cu), N = 2^10 .. 2^15
 bool ntt_fast_supported(const Context &ctx);
 cudaError_t launch_ntt_forward_fast(const Context &ctx, const NttRowMap &map, const u64 *in, u64 *out, int64_t rows,
                                     cudaStream_t stream);
 cudaError_t launch_ntt_inverse_fast(const Context &ctx, const NttRowMap &map, const u64 *in, u64 *out, int64_t rows,
                                     int scale_mode, cudaStream_t stream);
-// forward NTT of the lifted operands + tensor product in one kernel (ntt_fast.cu), N = 2^13 with the fast kernels
-// enabled: lhs / rhs (items x 2 x L x N, Coeff, 16-byte aligned) and their auxiliary rows (launch_lift into
+// forward NTT of the lifted operands + tensor product in one kernel (ntt_fast.cu), N = 2^13: lhs / rhs (items x 2 x L x N, Coeff, 16-byte aligned) and their auxiliary rows (launch_lift into
 // ext[item][4] with q_rows = false) -> ten[item][3][R][N] (Eval, Montgomery form like launch_tensor)
 bool ntt_forward_tensor_supported(const Context &ctx);
 cudaError_t launch_ntt_forward_tensor(const Context &ctx, const NttRowMap &map, const u64 *lhs, const u64 *rhs,

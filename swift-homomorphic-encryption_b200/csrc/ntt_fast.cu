@@ -19,7 +19,6 @@
 #include <mutex>
 
 #include <algorithm>
-#include <cstdlib>
 #include "kernels.cuh"
 #include "ntt_fast.cuh"
 
@@ -187,7 +186,7 @@ template <int LOGN, bool INVERSE, unsigned CLASSES>
 __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
     ntt_rows_kernel(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_out,
                     const ModSlot *__restrict__ slots, const __grid_constant__ RowList rl, const int polys,
-                    const int scale_mode, const int debug_flags) {
+                    const int scale_mode) {
     extern __shared__ __align__(1024) u64 smem[];  // row buffers first: the 128-byte swizzle wants them 1024-byte aligned
     constexpr int kLines = (1 << LOGN) / kLineWords;
     constexpr int kBoxes = kLines > kBoxLines ? kLines / kBoxLines : 1;
@@ -250,7 +249,7 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
                 load_row(fill, (buf + AHEAD) % B);
             }
             const int next = fill + gridDim.x;
-            if (next < tasks && !(debug_flags & 1)) {  // L2 prefetch of the row after that
+            if (next < tasks) {  // L2 prefetch of the row after that
                 const int line = in_line(next);
 #pragma unroll
                 for (int b = 0; b < kBoxes; ++b) tma_prefetch_box(&map_in, line + b * kLinesPerBox);
@@ -271,19 +270,12 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
         }
         mbar_wait(&bar_row[buf], (phase_row >> buf) & 1);
         phase_row ^= 1u << buf;
-        if (debug_flags & 4) {  // experiments: data movement only
-        } else
-#ifndef HE_EXPERIMENT_ONLY_CLASS
         if (INVERSE) inv_row_of<LOGN, CLASSES>(cls, sm, tau, m);
         else fwd_row_of<LOGN, CLASSES>(cls, sm, tau, m, (flags & 8) != 0);
-#else  // register-pressure experiments: one class only
-        if (INVERSE) inv_row<LOGN, HE_EXPERIMENT_ONLY_CLASS>(sm, tau, m);
-        else fwd_row<LOGN, HE_EXPERIMENT_ONLY_CLASS>(sm, tau, m, (flags & 8) != 0);
-#endif
         // ---- TMA out: every thread makes its generic-proxy writes visible to the async proxy, then one thread copies
         fence_proxy_async_smem();
         __syncthreads();
-        if (tau == 0 && !(debug_flags & 2)) {
+        if (tau == 0) {
             const int line = (int)(out_word >> 4);
 #pragma unroll
             for (int b = 0; b < kBoxes; ++b) tma_store_box(&map_out, line + b * kLinesPerBox, sm + b * kLinesPerBox * kLineWords);
@@ -579,11 +571,7 @@ static cudaError_t launch_rows(const Context &ctx, const RowList &rl, const u64 
     }
     const int64_t grid = std::min<int64_t>(rows, (int64_t)ctx.sm_count * per_sm);
     ++g_kernel_launches;
-    static const int debug_flags = [] {  // experiments only: bit 0 = no L2 prefetch of the next row, bit 1 = no TMA-out, bit 2 = no compute
-        const char *env = std::getenv("HECUDA_NTT_DEBUG");
-        return env ? std::atoi(env) : 0;
-    }();
-    k<<<(unsigned)grid, threads, smem, stream>>>(map_in, map_out, ctx.d_slots, rl, polys, scale_mode, debug_flags);
+    k<<<(unsigned)grid, threads, smem, stream>>>(map_in, map_out, ctx.d_slots, rl, polys, scale_mode);
     return cudaGetLastError();
 }
 
@@ -697,23 +685,10 @@ static cudaError_t launch_split(const Context &ctx, const NttRowMap &map, const 
         if (e != cudaSuccess) return e;
         in = out;
     }
-    // the 2^14 kernel, in place over `out` (forward) / from `in` to `out` (inverse); rows addressed like inverse rows
-    CUtensorMap map_in, map_out;
-    if (!make_line_map(&map_in, in, LOGN) || !make_line_map(&map_out, out, LOGN)) return cudaErrorInvalidValue;
-    {
-        constexpr int threads = (1 << LOGN) / 16;
-        constexpr size_t smem = ntt_smem_bytes<LOGN>();
-        auto k = ntt_rows_kernel<LOGN, INVERSE, kAllClasses>;
-        cudaError_t e;
-        if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
-        int per_sm = 0;
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, threads, smem)) != cudaSuccess) return e;
-        if (per_sm < 1) return cudaErrorInvalidConfiguration;
-        const int64_t grid = std::min<int64_t>(2 * rows, (int64_t)ctx.sm_count * per_sm);
-        ++g_kernel_launches;
-        k<<<(unsigned)grid, threads, smem, stream>>>(map_in, map_out, ctx.d_slots, rl, polys, scale_mode, 0);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
+    // the 2^14 kernel over the 2 x rows half rows, in place over `out` (forward) / from `in` to `out` (inverse); rows
+    // addressed like inverse rows
+    cudaError_t e = launch_rows<LOGN, INVERSE, kAllClasses>(ctx, rl, in, out, polys, 2 * rows, scale_mode, stream);
+    if (e != cudaSuccess) return e;
     if (INVERSE) {
         ++g_kernel_launches;
         ntt_merge_inverse_kernel<<<egrid, 256, 0, stream>>>(out, ctx.d_slots, sr, polys, ctx.logn, scale_mode);

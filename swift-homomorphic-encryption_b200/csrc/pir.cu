@@ -413,7 +413,6 @@ int32_t check_response_args(const hecuda_context *h, const hecuda_evk *k, const 
 // therefore captures the pipeline of a (database, evaluation key, shape) triple into a CUDA graph the first time it
 // sees it and replays it afterwards: one graph launch per query.  An instance owns its query / reply buffers (the
 // addresses are baked into the graph) and serves one query at a time; concurrent callers get instances of their own.
-// HECUDA_PIR_GRAPH=0 disables this.
 }  // namespace
 namespace hecuda {
 namespace api {
@@ -471,14 +470,6 @@ void pir_graphs_purge(hecuda_context *h, const void *handle) {
 }  // namespace api
 }  // namespace hecuda
 namespace {
-
-bool pir_graphs_enabled() {
-    static const bool on = [] {
-        const char *env = std::getenv("HECUDA_PIR_GRAPH");
-        return !(env && env[0] == '0');
-    }();
-    return on;
-}
 
 // Finds an idle instance for this call or builds one; nullptr (with *rc == OK) when capture is not possible.
 PirGraph *acquire_graph(const hecuda_context *hc, const hecuda_evk *k, const hecuda_pir_database *db, const ResponseShape &shape,
@@ -607,11 +598,7 @@ int32_t hecuda_pir_database_create(const hecuda_context *h, const uint64_t *plai
             cudaFree(d_coeff);
         }
     }
-    static const bool compact_ok = [] {
-        const char *env = std::getenv("HECUDA_PIR_COMPACT");
-        return !(env && env[0] == '0');
-    }();
-    if (e == cudaSuccess && compact_ok && inner_product_plain_small_supported(c, c.L)) {
+    if (e == cudaSuccess && inner_product_plain_small_supported(c, c.L)) {
         // small moduli (the default PIR parameters): keep the rows as uint32 -- half the bytes per scan, half the HBM
         e = cudaMalloc(&db->d_plain32, row_words * count * sizeof(u32));
         if (e == cudaSuccess) e = launch_narrow(db->d_plain, db->d_plain32, (int64_t)(row_words * count), nullptr);
@@ -702,7 +689,7 @@ int32_t hecuda_mulpir_compute_response(const hecuda_context *h, const hecuda_evk
     const Context &c = *h->ctx;
     const size_t ct_words = (size_t)2 * c.L * c.n, out_words = (size_t)2 * c.n * chunk_count * indices_count;
     cudaStream_t s = g.w->stream;
-    if (indices_count == 1 && db_count == 1 && pir_graphs_enabled()) {
+    if (indices_count == 1 && db_count == 1) {
         PirGraph *pg = acquire_graph(h, k, dbs[0], shape, query_ct_count, s, &rc);
         if (rc) return rc;
         if (pg) {

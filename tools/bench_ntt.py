@@ -24,4 +24,4 @@ for label, fn in (("fwd", lib.hecuda_ntt_forward_device), ("inv", lib.hecuda_ntt
     e1.record(s); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / reps
     out[label] = {"rows": polys * R, "ms": round(ms, 4), "Mrows_per_s": round(polys * R / ms / 1e3, 3), "GBps": round(polys * R * 2 * n * 8 / ms / 1e6, 1)}
-print(json.dumps({"workload": name, "n": n, "polys": polys, "debug": os.environ.get("HECUDA_NTT_DEBUG"), **out}))
+print(json.dumps({"workload": name, "n": n, "polys": polys, **out}))

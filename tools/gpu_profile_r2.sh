@@ -16,10 +16,6 @@ timeout 600 ncu --set full --clock-control none -k regex:"inner_product_plain|te
     python tools/prof_kernels.py ip > gpurun_out/ncu_ip.log 2>&1
 echo "inner-product kernels rc=$?"
 ls -la gpurun_out/*.ncu-rep gpurun_out/r02_launches.csv
-HECUDA_PIR_GRAPH=0 timeout 600 ncu --set full --clock-control none -k regex:inner_product_plain -s 2 -c 1 -f -o gpurun_out/r02_pir_scan \
-    python tools/prof_pir_scan.py > gpurun_out/ncu_pir_scan.log 2>&1
-echo "PIR scan rc=$?"
-python tools/summarize_ncu.py gpurun_out/r02_pir_scan.ncu-rep gpurun_out/r02_pir_scan.txt; rm -f gpurun_out/r02_pir_scan.ncu-rep
 # summaries on the box (the reports together exceed what travels back); keep only the C2 report
 for r in r02_c2_kernels r02_c3_kernels r02_ip_kernels; do python tools/summarize_ncu.py gpurun_out/$r.ncu-rep gpurun_out/$r.txt; done
 python tools/summarize_ncu.py --launches gpurun_out/r02_launches.csv gpurun_out/r02_launches.txt

@@ -1,13 +1,9 @@
 #!/bin/bash
-# two PIR server processes, one per GPU, at once (run with gpurun --gpus 2): spinning vs blocking waits
+# two PIR server processes, one per GPU, at once (needs two GPUs)
 mkdir -p gpurun_out
-run2() { # label env threads
-  ( env $2 timeout 120 python tools/diag_pir_threads.py plain 0 $3 2>&1 | sed "s/^/[$1 gpu0] /" ) &
-  ( env $2 timeout 120 python tools/diag_pir_threads.py plain 1 $3 2>&1 | sed "s/^/[$1 gpu1] /" ); wait
-}
 {
-run2 spin X=1 8
-run2 block HECUDA_BLOCKING_SYNC=1 8
+( timeout 120 python tools/diag_pir_threads.py plain 0 8 2>&1 | sed "s/^/[gpu0] /" ) &
+( timeout 120 python tools/diag_pir_threads.py plain 1 8 2>&1 | sed "s/^/[gpu1] /" ); wait
 nproc; cat /sys/fs/cgroup/cpu.max 2>/dev/null
 } > gpurun_out/diag_pir_2proc.log 2>&1
 grep -v Warning gpurun_out/diag_pir_2proc.log

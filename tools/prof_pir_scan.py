@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """A few MulPir queries at the BASELINE config 4 shape (2^20 x 64 B, default 27/28/28-bit parameters), for an ncu capture of
-the first-dimension scan:  HECUDA_PIR_GRAPH=0 ncu --set full -k regex:inner_product_plain python tools/prof_pir_scan.py"""
+the first-dimension scan:  ncu --set full -k regex:inner_product_plain python tools/prof_pir_scan.py"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "swift-homomorphic-encryption_b200")); sys.path.insert(0, os.path.join(ROOT, "tools"))
