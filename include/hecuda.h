@@ -322,6 +322,32 @@ int32_t hecuda_mulpir_compute_response_device(const hecuda_context *ctx, const h
                                               const uint64_t *query, int32_t query_ciphertext_count,
                                               int32_t indices_count, uint64_t *out, void *stream);
 
+/* Many clients' queries in one call: the same PirUtil.computeResponse (PirUtil.swift:490-568) that
+ * MulPirServer.computeResponse (MulPir.swift:414) runs once per Query, for client_count queries of the same shape
+ * against the same databases.  Client c is answered with evks[c]; its query ciphertexts are
+ * queries + c * query_ciphertext_count * 2 * L * N and its reply (bit-identical to what hecuda_mulpir_compute_response
+ * returns for that client alone) is out + c * indices_count * chunk_count * 2 * N, so out is
+ * client_count x indices_count x chunk_count x 2 x 1 x N.  Clients are processed in groups of at most
+ * HECUDA_MULPIR_CLIENT_GROUP; every stage is one pass over a group (its launch count does not depend on the group's
+ * size), the first-dimension scan streams each database once per group, and temporaries scale with the group, not
+ * with client_count.  Every client is checked like a single call (a failure's message names the client).  At every
+ * expansion level all clients' Galois keys must resolve to the same element, as keys generated for the same
+ * IndexPirParameter do; HECUDA_ERR_INVALID_ARGUMENT otherwise (answer such a client with the single-client call).
+ * The _device variant takes device buffers and only enqueues on `stream`; the first call with a new query shape
+ * uploads that shape's expansion plan to the context once, synchronously. */
+#define HECUDA_MULPIR_CLIENT_GROUP 16
+int32_t hecuda_mulpir_compute_response_clients(const hecuda_context *ctx, const hecuda_evk *const *evks, int32_t client_count,
+                                               const hecuda_pir_database *const *databases, int32_t database_count,
+                                               const int32_t *dimensions, int32_t dimension_count, int32_t chunk_count,
+                                               const uint64_t *queries, int32_t query_ciphertext_count,
+                                               int32_t indices_count, uint64_t *out);
+int32_t hecuda_mulpir_compute_response_clients_device(const hecuda_context *ctx, const hecuda_evk *const *evks,
+                                                      int32_t client_count, const hecuda_pir_database *const *databases,
+                                                      int32_t database_count, const int32_t *dimensions,
+                                                      int32_t dimension_count, int32_t chunk_count, const uint64_t *queries,
+                                                      int32_t query_ciphertext_count, int32_t indices_count, uint64_t *out,
+                                                      void *stream);
+
 /* The same, bytes in / bytes out: the query ciphertexts as they travel (SerializedCiphertext.seeded: poly0 serialized with
  * skipLSBs 0 over all L rows, plus the 32-byte seed; SerializedCiphertext.swift:41-49,150-154) and the reply ciphertexts as
  * they leave (SerializedCiphertext.full with Bfv.skipLSBsForDecryption, Bfv+Decrypt.swift:51-110: single modulus, poly 0 and

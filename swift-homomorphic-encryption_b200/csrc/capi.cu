@@ -143,29 +143,29 @@ cudaError_t multiply_chunk(const Context &c, u64 *scratch, const u64 *lhs, const
 // + the caller's accumulation: out[item][c] = update[c] (+ base[item][c] for the components in base_mask).
 cudaError_t keyswitch_chunk(const Context &c, u64 *scratch, const u64 *key, const u64 *target, int64_t target_stride,
                             int l, const u64 *base, int64_t base_stride, int base_mask, u64 *out, int64_t items,
-                            cudaStream_t s) {
+                            cudaStream_t s, const KsKeyTable *keys) {
     const size_t dig_words = (size_t)(l + 1) * l * c.n;
     cudaError_t e;
     u64 *dig = scratch, *prod = scratch + dig_words * items;
     // digits: forward NTT that gathers [target row j]_{m_r} straight from the source      (Bfv+Keys.swift:165-179)
     if ((e = launch_ntt_forward(c, c.map_ks_digits(l, target_stride), target, dig, items * (l + 1) * l, s)) != cudaSuccess)
         return e;
-    if ((e = launch_ks_mac(c, dig, key, l, prod, items, s)) != cudaSuccess) return e;
+    if ((e = launch_ks_mac(c, dig, key, l, prod, items, s, keys)) != cudaSuccess) return e;
     if ((e = launch_ntt_inverse(c, c.map_ks(l), prod, prod, items * 2 * (l + 1), kScaleMont, s)) != cudaSuccess) return e;
     return launch_ks_finish(c, prod, base, base_stride, base_mask, l, out, items, s);
 }
 
 // Bfv.relinearize (Bfv.swift:201-219): key-switch poly 2, add the update to polys 0 and 1
 cudaError_t relinearize_chunk(const Context &c, u64 *scratch, const u64 *key, const u64 *ct3, int l, u64 *out,
-                              int64_t items, cudaStream_t s) {
+                              int64_t items, cudaStream_t s, const KsKeyTable *keys) {
     const int64_t ct_stride = (int64_t)3 * l * c.n;
-    return keyswitch_chunk(c, scratch, key, ct3 + (int64_t)2 * l * c.n, ct_stride, l, ct3, ct_stride, 3, out, items, s);
+    return keyswitch_chunk(c, scratch, key, ct3 + (int64_t)2 * l * c.n, ct_stride, l, ct3, ct_stride, 3, out, items, s, keys);
 }
 
 // Bfv.applyGalois (Bfv.swift:174-198): c0' = galois(c0) + update[0], c1' = update[1], update = keyswitch(galois(c1))
 size_t galois_scratch_words(const Context &c, int l) { return relinearize_scratch_words(c, l) + (size_t)l * c.n; }
 cudaError_t apply_galois_chunk(const Context &c, u64 *scratch, const u64 *key, const u64 *ct, int l, unsigned element,
-                               u64 *out, int64_t items, cudaStream_t s) {
+                               u64 *out, int64_t items, cudaStream_t s, const KsKeyTable *keys) {
     const int64_t poly = (int64_t)l * c.n, ct_stride = 2 * poly;
     u64 *perm1 = scratch;                      // items x l x N
     u64 *ks_scratch = scratch + poly * items;
@@ -173,7 +173,7 @@ cudaError_t apply_galois_chunk(const Context &c, u64 *scratch, const u64 *key, c
     cudaError_t e;
     if ((e = launch_galois_coeff(c, map, element, ct, ct_stride, out, ct_stride, items, s)) != cudaSuccess) return e;
     if ((e = launch_galois_coeff(c, map, element, ct + poly, ct_stride, perm1, poly, items, s)) != cudaSuccess) return e;
-    return keyswitch_chunk(c, ks_scratch, key, perm1, poly, l, out, ct_stride, 1, out, items, s);
+    return keyswitch_chunk(c, ks_scratch, key, perm1, poly, l, out, ct_stride, 1, out, items, s, keys);
 }
 
 // Bfv.innerProduct(_:_:) (Bfv.swift:315-361): sum of the tensor products of `pairs` ciphertext pairs in [Q, Bsk],
@@ -447,6 +447,7 @@ int32_t hecuda_context_destroy(hecuda_context *h) {
     cudaDeviceSynchronize();
     pir_graphs_purge(h, nullptr);
     context_registered(h, false);
+    for (auto &kv : h->expand_steps) cudaFree(kv.second);
     for (Workspace *w : h->free_ws) {
         w->release();
         delete w;

@@ -81,6 +81,8 @@ void context_registered(const hecuda_context *h, bool alive);            // cont
 struct hecuda_context {
     hecuda::Context *ctx = nullptr;
     std::vector<hecuda::api::PirGraph *> pir_graphs;  // guarded by mu
+    // device copies of MulPir expansion plans by (query ciphertexts, outputs), uploaded once; guarded by mu
+    std::map<std::pair<int64_t, int64_t>, void *> expand_steps;
     int64_t chunk = 32;  // ciphertexts per pipeline stage
     std::mutex mu;
     std::vector<hecuda::api::Workspace *> free_ws;  // pooled workspaces (each with its own stream)
@@ -144,13 +146,14 @@ size_t inner_product_scratch_words(const Context &c, int64_t pairs);
 
 cudaError_t multiply_chunk(const Context &c, u64 *scratch, const u64 *lhs, const u64 *rhs, u64 *out, int64_t items,
                            cudaStream_t s);
+// keys: one key per client (launch_ks_mac) in place of `key`
 cudaError_t keyswitch_chunk(const Context &c, u64 *scratch, const u64 *key, const u64 *target, int64_t target_stride,
                             int l, const u64 *base, int64_t base_stride, int base_mask, u64 *out, int64_t items,
-                            cudaStream_t s);
+                            cudaStream_t s, const KsKeyTable *keys = nullptr);
 cudaError_t relinearize_chunk(const Context &c, u64 *scratch, const u64 *key, const u64 *ct3, int l, u64 *out,
-                              int64_t items, cudaStream_t s);
+                              int64_t items, cudaStream_t s, const KsKeyTable *keys = nullptr);
 cudaError_t apply_galois_chunk(const Context &c, u64 *scratch, const u64 *key, const u64 *ct, int l, unsigned element,
-                               u64 *out, int64_t items, cudaStream_t s);
+                               u64 *out, int64_t items, cudaStream_t s, const KsKeyTable *keys = nullptr);
 cudaError_t expand_seeded_device(const Context &c, int l, const unsigned char *d_poly0, const unsigned char *d_seeds, u64 *d_out,
                                  int64_t batch, cudaStream_t s);
 cudaError_t inner_product_chunk(const Context &c, u64 *scratch, const u64 *lhs, const u64 *rhs, int64_t pairs, u64 *out,

@@ -77,10 +77,7 @@ __global__ void __launch_bounds__(128) inner_product_plain_kernel(const u64 *__r
     }
 }
 
-cudaError_t launch_inner_product_plain(const Context &ctx, const u64 *cts, int npoly, int l, int64_t terms, const u64 *pts,
-                                       const unsigned char *present, u64 *out, int64_t out_count, cudaStream_t stream) {
-    if (out_count == 0) return cudaSuccess;
-    if (npoly < 1 || npoly > 3 || l < 1 || l > ctx.L || ctx.n < 2) return cudaErrorInvalidValue;
+static IpConsts ip_consts(const Context &ctx, int l) {
     IpConsts c;
     c.l = l;
     u64 qmax = 0;
@@ -94,6 +91,14 @@ cudaError_t launch_inner_product_plain(const Context &ctx, const u64 *cts, int n
     const u128 max_product = (u128)(qmax - 1) * (qmax - 1);
     const u128 max_count = ((~(u128)0) - qmax) / max_product;
     c.max_terms = max_count > (u128)0x7fffffffffffffffLL ? 0x7fffffffffffffffLL : (long long)max_count;
+    return c;
+}
+
+cudaError_t launch_inner_product_plain(const Context &ctx, const u64 *cts, int npoly, int l, int64_t terms, const u64 *pts,
+                                       const unsigned char *present, u64 *out, int64_t out_count, cudaStream_t stream) {
+    if (out_count == 0) return cudaSuccess;
+    if (npoly < 1 || npoly > 3 || l < 1 || l > ctx.L || ctx.n < 2) return cudaErrorInvalidValue;
+    const IpConsts c = ip_consts(ctx, l);
     const unsigned gx = (unsigned)((ctx.n / 2 + 127) / 128);
     // [npoly - 1][present given]
     static void (*const kernels[3][2])(const u64 *, const u64 *, const unsigned char *, u64 *, IpConsts, int, long long) = {
@@ -179,10 +184,7 @@ bool inner_product_plain_small_supported(const Context &ctx, int l) {
     return true;
 }
 
-cudaError_t launch_inner_product_plain_small(const Context &ctx, const u64 *cts, int npoly, int l, int64_t terms, const u32 *pts,
-                                             const unsigned char *present, u64 *out, int64_t out_count, cudaStream_t stream) {
-    if (out_count == 0) return cudaSuccess;
-    if (npoly < 1 || npoly > 3 || l < 1 || l > ctx.L || !inner_product_plain_small_supported(ctx, l)) return cudaErrorInvalidValue;
+static IpSmallConsts ip_small_consts(const Context &ctx, int l) {
     IpSmallConsts c;
     c.l = l;
     u64 qmax = 0;
@@ -196,6 +198,14 @@ cudaError_t launch_inner_product_plain_small(const Context &ctx, const u64 *cts,
     const u128 room = (~(u128)0 >> 64) - qmax;
     const u128 max_count = room / ((u128)(qmax - 1) * (qmax - 1));
     c.max_terms = max_count > 0x7fffffff ? 0x7fffffff : (int)max_count;
+    return c;
+}
+
+cudaError_t launch_inner_product_plain_small(const Context &ctx, const u64 *cts, int npoly, int l, int64_t terms, const u32 *pts,
+                                             const unsigned char *present, u64 *out, int64_t out_count, cudaStream_t stream) {
+    if (out_count == 0) return cudaSuccess;
+    if (npoly < 1 || npoly > 3 || l < 1 || l > ctx.L || !inner_product_plain_small_supported(ctx, l)) return cudaErrorInvalidValue;
+    const IpSmallConsts c = ip_small_consts(ctx, l);
     if (c.max_terms < 1) return cudaErrorInvalidValue;
     const unsigned gx = (unsigned)((ctx.n / 4 + 127) / 128);
     // [npoly - 1][present given]
@@ -212,6 +222,192 @@ cudaError_t launch_inner_product_plain_small(const Context &ctx, const u64 *cts,
         ++g_kernel_launches;
         kernels[npoly - 1][pr != nullptr]<<<grid, 128, 0, stream>>>(cts, pt, pr, o, c, (int)ctx.n, terms);
         done += chunk;
+    }
+    return cudaGetLastError();
+}
+
+// ---- both scans for several clients' 2-poly queries against the same database rows (hecuda_mulpir_compute_response_
+// clients).  A thread accumulates a tile of kScanClientTile clients x kScanRowTile database rows: each database value
+// it streams feeds kScanClientTile clients, each query value it fetches through L2 feeds kScanRowTile rows.  The
+// group's client tiles are adjacent blocks (blockIdx.x = coefficient block x tiles + tile) that read the same database
+// words at about the same time, so the later tiles find them in L2.  (The tiles as threadIdx.y slices of one block
+// measured slower from 8 clients up: a 256-thread block at ~200 registers leaves one block per SM.)  A missing plaintext contributes a zero product, and the reductions fall on
+// the same terms as in the single-client kernels, so every sum is the same integer.
+struct ScanTile {  // the clamped pointers of one thread's tile (surplus clients / rows repeat the last one)
+    int clients, rows;
+    long long client_off[kScanClientTile], row[kScanRowTile];
+};
+__device__ __forceinline__ ScanTile scan_tile(int c0, int clients, long long out_count) {
+    ScanTile t;
+    const long long o0 = (long long)blockIdx.z * kScanRowTile;
+    t.clients = min(kScanClientTile, clients - c0);
+    t.rows = (int)min((long long)kScanRowTile, out_count - o0);
+#pragma unroll
+    for (int j = 0; j < kScanClientTile; ++j) t.client_off[j] = c0 + min(j, t.clients - 1);
+#pragma unroll
+    for (int i = 0; i < kScanRowTile; ++i) t.row[i] = o0 + min(i, t.rows - 1);
+    return t;
+}
+
+template <bool HAS_PRESENT>
+__global__ void __launch_bounds__(64) inner_product_plain_small_clients_kernel(
+    const u64 *__restrict__ cts, long long client_stride, int clients, const u32 *__restrict__ pts,
+    const unsigned char *__restrict__ present, u64 *__restrict__ out, long long out_client_stride, long long out_count,
+    const __grid_constant__ IpSmallConsts c, int n, long long terms) {
+    constexpr int CT = kScanClientTile, RT = kScanRowTile;
+    const int tiles = (clients + CT - 1) / CT, c0 = (blockIdx.x % tiles) * CT;
+    const int coeff = ((blockIdx.x / tiles) * 64 + threadIdx.x) * 2;  // two adjacent coefficients: 8-byte loads of the uint32 rows
+    if (coeff >= n) return;
+    const int r = blockIdx.y, l = c.l;
+    const u64 p = c.p[r], mu1 = c.mu1[r];
+    const ScanTile t = scan_tile(c0, clients, out_count);
+    const long long pt_stride = (long long)l * n, ct_stride = 2LL * l * n;
+    const u64 *ct[CT];
+    const u32 *pt[RT];
+#pragma unroll
+    for (int j = 0; j < CT; ++j) ct[j] = cts + t.client_off[j] * client_stride + (long long)r * n + coeff;
+#pragma unroll
+    for (int i = 0; i < RT; ++i) pt[i] = pts + ((t.row[i] * terms) * l + r) * (long long)n + coeff;
+    u64 acc[CT][RT][2][2];
+#pragma unroll
+    for (int j = 0; j < CT; ++j)
+#pragma unroll
+        for (int i = 0; i < RT; ++i) acc[j][i][0][0] = acc[j][i][0][1] = acc[j][i][1][0] = acc[j][i][1][1] = 0;
+    int since_reduce = 0;
+    for (long long k = 0; k < terms; ++k) {
+        uint2 pv[RT];
+#pragma unroll
+        for (int i = 0; i < RT; ++i)  // nil plaintext (Bfv.swift:493): a zero row
+            pv[i] = (!HAS_PRESENT || present[t.row[i] * terms + k]) ? __ldcs(reinterpret_cast<const uint2 *>(pt[i] + k * pt_stride))
+                                                                   : make_uint2(0u, 0u);
+#pragma unroll
+        for (int j = 0; j < CT; ++j)
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                const uint4 cv = __ldg(reinterpret_cast<const uint4 *>(ct[j] + k * ct_stride + q * pt_stride));  // low words .x .z
+#pragma unroll
+                for (int i = 0; i < RT; ++i) {
+                    acc[j][i][q][0] += (u64)cv.x * pv[i].x;
+                    acc[j][i][q][1] += (u64)cv.z * pv[i].y;
+                }
+            }
+        if (++since_reduce >= c.max_terms) {  // reduceInPlace, Bfv.swift:365-377
+            since_reduce = 0;
+#pragma unroll
+            for (int j = 0; j < CT; ++j)
+#pragma unroll
+                for (int i = 0; i < RT; ++i)
+#pragma unroll
+                    for (int q = 0; q < 2; ++q) {
+                        acc[j][i][q][0] = barrett64(acc[j][i][q][0], p, mu1);
+                        acc[j][i][q][1] = barrett64(acc[j][i][q][1], p, mu1);
+                    }
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < CT; ++j)
+#pragma unroll
+        for (int i = 0; i < RT; ++i) {
+            if (j >= t.clients || i >= t.rows) continue;
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {  // reduceToCiphertext, Bfv.swift:380-394
+                u64 *dst = out + (c0 + j) * out_client_stride + (((t.row[i] * 2 + q) * l + r) * (long long)n) + coeff;
+                *reinterpret_cast<ulonglong2 *>(dst) =
+                    make_ulonglong2(barrett64(acc[j][i][q][0], p, mu1), barrett64(acc[j][i][q][1], p, mu1));
+            }
+        }
+}
+
+template <bool HAS_PRESENT>
+__global__ void __launch_bounds__(64) inner_product_plain_clients_kernel(
+    const u64 *__restrict__ cts, long long client_stride, int clients, const u64 *__restrict__ pts,
+    const unsigned char *__restrict__ present, u64 *__restrict__ out, long long out_client_stride, long long out_count,
+    const __grid_constant__ IpConsts c, int n, long long terms) {
+    constexpr int CT = kScanClientTile, RT = kScanRowTile;
+    const int tiles = (clients + CT - 1) / CT, c0 = (blockIdx.x % tiles) * CT;
+    const int coeff = (blockIdx.x / tiles) * 64 + threadIdx.x;  // one coefficient: 128-bit accumulators
+    if (coeff >= n) return;
+    const int r = blockIdx.y, l = c.l;
+    const u64 p = c.p[r], mu_hi = c.mu_hi[r], mu_lo = c.mu_lo[r];
+    const ScanTile t = scan_tile(c0, clients, out_count);
+    const long long pt_stride = (long long)l * n, ct_stride = 2LL * l * n;
+    const u64 *ct[CT];
+    const u64 *pt[RT];
+#pragma unroll
+    for (int j = 0; j < CT; ++j) ct[j] = cts + t.client_off[j] * client_stride + (long long)r * n + coeff;
+#pragma unroll
+    for (int i = 0; i < RT; ++i) pt[i] = pts + ((t.row[i] * terms) * l + r) * (long long)n + coeff;
+    u128 acc[CT][RT][2];
+#pragma unroll
+    for (int j = 0; j < CT; ++j)
+#pragma unroll
+        for (int i = 0; i < RT; ++i) acc[j][i][0] = acc[j][i][1] = 0;
+    long long since_reduce = 0;
+    for (long long k = 0; k < terms; ++k) {
+        u64 pv[RT];
+#pragma unroll
+        for (int i = 0; i < RT; ++i)  // nil plaintext (Bfv.swift:493): a zero row
+            pv[i] = (!HAS_PRESENT || present[t.row[i] * terms + k]) ? __ldcs(pt[i] + k * pt_stride) : 0;
+#pragma unroll
+        for (int j = 0; j < CT; ++j)
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                const u64 cv = __ldg(ct[j] + k * ct_stride + q * pt_stride);
+#pragma unroll
+                for (int i = 0; i < RT; ++i) mac128(acc[j][i][q], cv, pv[i]);
+            }
+        if (++since_reduce >= c.max_terms) {  // reduceInPlace, Bfv.swift:365-377
+            since_reduce = 0;
+#pragma unroll
+            for (int j = 0; j < CT; ++j)
+#pragma unroll
+                for (int i = 0; i < RT; ++i)
+#pragma unroll
+                    for (int q = 0; q < 2; ++q) acc[j][i][q] = barrett128(to_w(acc[j][i][q]), p, mu_hi, mu_lo);
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < CT; ++j)
+#pragma unroll
+        for (int i = 0; i < RT; ++i) {
+            if (j >= t.clients || i >= t.rows) continue;
+#pragma unroll
+            for (int q = 0; q < 2; ++q)  // reduceToCiphertext, Bfv.swift:380-394
+                out[(c0 + j) * out_client_stride + (((t.row[i] * 2 + q) * l + r) * (long long)n) + coeff] =
+                    barrett128(to_w(acc[j][i][q]), p, mu_hi, mu_lo);
+        }
+}
+
+cudaError_t launch_inner_product_plain_clients(const Context &ctx, const u64 *cts, int64_t client_stride, int clients, int l,
+                                               int64_t terms, const u64 *pts, const u32 *pts32, const unsigned char *present,
+                                               u64 *out, int64_t out_client_stride, int64_t out_count, cudaStream_t stream) {
+    if (out_count == 0) return cudaSuccess;
+    if (clients < 1 || clients > kScanClientTile * kScanClientTiles || l < 1 || l > ctx.L || ctx.n < 2 ||
+        (pts32 != nullptr) == (pts != nullptr) || (pts32 && !inner_product_plain_small_supported(ctx, l)))
+        return cudaErrorInvalidValue;
+    const IpSmallConsts cs = pts32 ? ip_small_consts(ctx, l) : IpSmallConsts{};
+    const IpConsts cw = pts32 ? IpConsts{} : ip_consts(ctx, l);
+    if (pts32 && cs.max_terms < 1) return cudaErrorInvalidValue;
+    const unsigned tiles = (unsigned)((clients + kScanClientTile - 1) / kScanClientTile);
+    const unsigned gx = (unsigned)(((pts32 ? ctx.n / 2 : ctx.n) + 63) / 64) * tiles;
+    const int block = 64;
+    const int64_t max_rows = (int64_t)65535 * kScanRowTile;
+    for (int64_t done = 0; done < out_count;) {
+        const int64_t rows = (out_count - done) > max_rows ? max_rows : (out_count - done);
+        dim3 grid(gx ? gx : 1, (unsigned)l, (unsigned)((rows + kScanRowTile - 1) / kScanRowTile));
+        const unsigned char *pr = present ? present + done * terms : nullptr;
+        u64 *o = out + done * 2 * l * ctx.n;
+        ++g_kernel_launches;
+        if (pts32) {
+            const u32 *pt = pts32 + done * terms * l * ctx.n;
+            (pr ? inner_product_plain_small_clients_kernel<true> : inner_product_plain_small_clients_kernel<false>)
+                <<<grid, block, 0, stream>>>(cts, client_stride, clients, pt, pr, o, out_client_stride, rows, cs, (int)ctx.n, terms);
+        } else {
+            const u64 *pt = pts + done * terms * l * ctx.n;
+            (pr ? inner_product_plain_clients_kernel<true> : inner_product_plain_clients_kernel<false>)
+                <<<grid, block, 0, stream>>>(cts, client_stride, clients, pt, pr, o, out_client_stride, rows, cw, (int)ctx.n, terms);
+        }
+        done += rows;
     }
     return cudaGetLastError();
 }

@@ -57,9 +57,16 @@ cudaError_t launch_floor(const Context &ctx, const u64 *in, u64 *out, int64_t po
                          bool reference_base = false, bool q_scaled = false);
 
 // ---- key switching and modulus switching (keyswitch.cu)
-// mac: dig (Eval) x key -> prod[item][2][l+1][N] (Eval)
+// One key-switching key per client for a launch that switches several clients' items: item i (counted from item0)
+// belongs to client i / items_per_client.  Passed in the kernel's parameter block.
+constexpr int kKeyTableSize = 16;
+struct KsKeyTable {
+    const u64 *key[kKeyTableSize];
+    long long items_per_client, item0;
+};
+// mac: dig (Eval) x key -> prod[item][2][l+1][N] (Eval); keys: per-client keys instead of `key`
 cudaError_t launch_ks_mac(const Context &ctx, const u64 *dig, const u64 *key, int l, u64 *prod, int64_t items,
-                          cudaStream_t stream);
+                          cudaStream_t stream, const KsKeyTable *keys = nullptr);
 // finish: out[item][c][i] = divround(prod[item][c])[i] (+ base[item][c][i] for the components in base_mask)
 cudaError_t launch_ks_finish(const Context &ctx, const u64 *prod, const u64 *base, int64_t base_item_stride, int base_mask,
                              int l, u64 *out, int64_t items, cudaStream_t stream);
@@ -79,6 +86,14 @@ cudaError_t launch_inner_product_plain(const Context &ctx, const u64 *cts, int n
 bool inner_product_plain_small_supported(const Context &ctx, int l);
 cudaError_t launch_inner_product_plain_small(const Context &ctx, const u64 *cts, int npoly, int l, int64_t terms, const u32 *pts,
                                              const unsigned char *present, u64 *out, int64_t out_count, cudaStream_t stream);
+// The same scans for `clients` (<= kScanClientTile * kScanClientTiles) 2-poly queries at once: client j's `terms`
+// ciphertexts start at cts + j * client_stride, its out_count x 2 x l x N results at out + j * out_client_stride.
+// The client tiles of a row tile are adjacent blocks, so a database row comes from HBM about once per launch; every
+// value is the one the single-client scan computes.
+constexpr int kScanClientTile = 4, kScanClientTiles = 4, kScanRowTile = 2;  // clients, tiles per launch, rows
+cudaError_t launch_inner_product_plain_clients(const Context &ctx, const u64 *cts, int64_t client_stride, int clients, int l,
+                                               int64_t terms, const u64 *pts, const u32 *pts32, const unsigned char *present,
+                                               u64 *out, int64_t out_client_stride, int64_t out_count, cudaStream_t stream);
 cudaError_t launch_plaintext_to_eval(const Context &ctx, const u64 *plain, int l, u64 *out, int64_t count,
                                      cudaStream_t stream);
 

@@ -21,8 +21,12 @@ struct KsMacConsts {
 // prod[item][comp][r][.] = [ sum_j dig[item][r][j][.] * key[j][comp][keyrow(r)][.] ]_{m_r} * 2^-64   (Bfv+Keys.swift:180-202)
 // 128-bit lazy accumulation like the reference (:187-190), one Montgomery reduction; the 2^-64 is undone by the
 // kScaleMont scaling of the inverse NTT that follows.  sum < l p^2 < 2^127, reduced value < (1 + l/4) p <= 5p.
+// CLIENT_KEYS: item i (counted from keys.item0) uses keys.key[i / keys.items_per_client] instead of `key`; the table
+// lives in the parameter block, so switching many clients' items in one launch needs no upload.
+template <bool CLIENT_KEYS>
 __global__ void __launch_bounds__(128) ks_mac_kernel(const u64 *__restrict__ dig, const u64 *__restrict__ key,
-                                                    u64 *__restrict__ prod, const __grid_constant__ KsMacConsts c, int n) {
+                                                    u64 *__restrict__ prod, const __grid_constant__ KsMacConsts c, int n,
+                                                    const __grid_constant__ KsKeyTable keys) {
     const int l = c.l, K = c.K;
     const int r = blockIdx.y;
     const int64_t item = blockIdx.z;
@@ -32,6 +36,7 @@ __global__ void __launch_bounds__(128) ks_mac_kernel(const u64 *__restrict__ dig
     const u64 p = c.p[r], ninv = c.ninv[r];
     u128 a00 = 0, a01 = 0, a10 = 0, a11 = 0;
     const u64 *d = dig + ((item * (l + 1) + r) * l) * n + coeff;
+    if (CLIENT_KEYS) key = keys.key[(keys.item0 + item) / keys.items_per_client];
     const u64 *kj = key + (int64_t)key_row * n + coeff;
     for (int j = 0; j < l; ++j) {
         const ulonglong2 dv = *reinterpret_cast<const ulonglong2 *>(d + (int64_t)j * n);
@@ -91,7 +96,7 @@ __global__ void __launch_bounds__(256) mod_switch_kernel(const u64 *__restrict__
 static inline int pick_threads(int64_t n) { return n >= 256 ? 256 : (n < 32 ? 32 : (int)n); }
 
 cudaError_t launch_ks_mac(const Context &ctx, const u64 *dig, const u64 *key, int l, u64 *prod, int64_t items,
-                          cudaStream_t stream) {
+                          cudaStream_t stream, const KsKeyTable *keys) {
     if (items == 0) return cudaSuccess;
     if (ctx.n < 2) return cudaErrorInvalidValue;
     const NttRowMap map = ctx.map_ks(l);
@@ -102,13 +107,21 @@ cudaError_t launch_ks_mac(const Context &ctx, const u64 *dig, const u64 *key, in
         c.p[r] = ctx.slots[map.slot[r]].dev.p;
         c.ninv[r] = ctx.slots[map.slot[r]].dev.ninv;
     }
+    if (keys && keys->items_per_client < 1) return cudaErrorInvalidValue;
+    KsKeyTable table = keys ? *keys : KsKeyTable{};
     const unsigned gx = (unsigned)((ctx.n / 2 + 127) / 128);
     for (int64_t done = 0; done < items;) {
         const int64_t chunk = (items - done) > 65535 ? 65535 : (items - done);
         dim3 grid(gx ? gx : 1, (unsigned)(l + 1), (unsigned)chunk);
         ++g_kernel_launches;
-        ks_mac_kernel<<<grid, 128, 0, stream>>>(dig + done * (l + 1) * l * ctx.n, key, prod + done * 2 * (l + 1) * ctx.n, c,
-                                                (int)ctx.n);
+        const u64 *d = dig + done * (l + 1) * l * ctx.n;
+        u64 *o = prod + done * 2 * (l + 1) * ctx.n;
+        if (keys) {
+            table.item0 = keys->item0 + done;
+            ks_mac_kernel<true><<<grid, 128, 0, stream>>>(d, nullptr, o, c, (int)ctx.n, table);
+        } else {
+            ks_mac_kernel<false><<<grid, 128, 0, stream>>>(d, key, o, c, (int)ctx.n, table);
+        }
         done += chunk;
     }
     return cudaGetLastError();

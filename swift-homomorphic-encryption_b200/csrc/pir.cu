@@ -52,18 +52,24 @@ __device__ __forceinline__ u64 add_mod(u64 a, u64 b, u64 p) {
 
 // expandCiphertextForOneStep after the Galois step (PirUtil.swift:230-235) for every node of a level:
 //   p0 = c1 + ct,  p1 = multiplyPowerOfX(ct - c1, -2^(logStep-1))   [gather form of PolyRq.swift:398-422]
+// Item item0 + blockIdx.z is node (item % nodes) of client (item / nodes); a client's children go `next_cts`
+// ciphertexts into `next` and its leaves `out_cts` ciphertexts into `out` after the previous client's.
 __global__ void __launch_bounds__(256) expand_combine_kernel(const u64 *__restrict__ cur, const u64 *__restrict__ c1,
                                                             u64 *__restrict__ next, u64 *__restrict__ out,
                                                             const ExpandStep *__restrict__ steps,
-                                                            const __grid_constant__ RowConsts c, int logn, unsigned s) {
+                                                            const __grid_constant__ RowConsts c, int logn, unsigned s,
+                                                            int64_t item0, int nodes, int64_t next_cts, int64_t out_cts) {
     const int n = 1 << logn;
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n) return;
     const int pr = blockIdx.y;  // poly * rows + row
     const u64 p = c.p[pr % c.rows];
     const int64_t ct_words = (int64_t)2 * c.rows * n;
-    const int64_t base = (int64_t)blockIdx.z * ct_words + (int64_t)pr * n;
-    const ExpandStep st = steps[blockIdx.z];
+    const int64_t item = item0 + blockIdx.z, client = item / nodes;
+    const int64_t base = item * ct_words + (int64_t)pr * n;
+    const ExpandStep st = steps[item - client * nodes];
+    next += client * next_cts * ct_words;
+    out += client * out_cts * ct_words;
     u64 sum = add_mod(cur[base + e], c1[base + e], p);
     const unsigned raw = ((unsigned)e - s) & (2u * n - 1u);
     const unsigned src = raw & (n - 1u);
@@ -205,27 +211,77 @@ struct StreamBuffers {  // stream-ordered temporaries, freed (stream-ordered) on
     }
 };
 
-// PirUtil.expand on device buffers: d_in = ct_count canonical (Coeff) ciphertexts of L rows, d_out = output_count
+// The Galois element, repeat count and key that every expansion level of `plan` applies, for clients
+// first_client .. first_client + clients - 1 (keys[j] belongs to client first_client + j).  All clients must resolve
+// to the same element at every level.  first_client < 0: one client answered alone, whose errors name no client.
+struct LevelKeys {
+    unsigned element = 0;
+    int times = 0;
+    std::vector<const u64 *> key;  // [j]
+};
+int32_t resolve_level_keys(const hecuda_evk *const *keys, int clients, int first_client, int64_t n, const ExpandPlan &plan,
+                           std::vector<LevelKeys> &out) {
+    out.assign(plan.levels.size(), LevelKeys{});
+    const int first = std::max(first_client, 0);
+    for (size_t li = 0; li < plan.levels.size(); ++li) {
+        LevelKeys &lk = out[li];
+        lk.key.resize((size_t)clients);
+        for (int j = 0; j < clients; ++j) {
+            unsigned element = 0;
+            int times = 0;
+            const std::string who = "client " + std::to_string(first + j);
+            int32_t rc32 = pick_galois(keys[j], n, plan.levels[li].log_step, &element, &times, &lk.key[j]);
+            if (rc32) return first_client < 0 ? rc32 : fail(rc32, who + ": " + last_error_cstr());
+            if (j > 0 && (element != lk.element || times != lk.times))
+                return fail(HECUDA_ERR_INVALID_ARGUMENT,
+                            who + ": its Galois keys apply element " + std::to_string(element) + " at expansion level " +
+                                std::to_string(plan.levels[li].log_step) + ", client " + std::to_string(first) +
+                                "'s apply " + std::to_string(lk.element) + "; answer it with hecuda_mulpir_compute_response");
+            lk.element = element;
+            lk.times = times;
+        }
+    }
+    return HECUDA_OK;
+}
+
+// PirUtil.expand on device buffers for `clients` queries of the same shape: client j's ct_count canonical (Coeff)
+// ciphertexts of L rows at d_in + j * ct_count ciphertexts, its output_count outputs at d_out + j * output_count,
+// expanded with keys[j].  Every stage is one pass over all clients.
 // d_steps_ready: the plan's steps already on the device (captured graphs upload them once, outside the capture)
-int32_t expand_device(const hecuda_context *h, const hecuda_evk *k, const u64 *d_in, int64_t ct_count, int64_t output_count,
-                      u64 *d_out, cudaStream_t s, const void *d_steps_ready = nullptr) {
+// first_client: the call-wide index of keys[0] for error messages (resolve_level_keys)
+int32_t expand_device(const hecuda_context *h, const hecuda_evk *const *keys, int clients, const u64 *d_in, int64_t ct_count,
+                      int64_t output_count, u64 *d_out, cudaStream_t s, const void *d_steps_ready = nullptr,
+                      int first_client = -1) {
     const Context &c = *h->ctx;
     const int l = c.L;
     const int64_t n = c.n;
     const size_t ct_words = (size_t)2 * l * n;
     const ExpandPlan plan = build_expand_plan(n, ct_count, output_count);
+    // resolve every level's Galois key for every client before anything is enqueued
+    std::vector<LevelKeys> level_keys;
+    int32_t rc_keys = resolve_level_keys(keys, clients, first_client, n, plan, level_keys);
+    if (rc_keys) return rc_keys;
+    if (clients > kKeyTableSize) return fail(HECUDA_ERR_UNSUPPORTED, "expand: more clients than one key table holds");
+    std::vector<KsKeyTable> tables(plan.levels.size(), KsKeyTable{});
+    for (size_t li = 0; li < plan.levels.size(); ++li) {
+        tables[li].items_per_client = plan.levels[li].nodes;
+        for (int j = 0; j < clients && j < kKeyTableSize; ++j) tables[li].key[j] = level_keys[li].key[j];
+    }
+    const size_t in_pitch = ct_words * ct_count * sizeof(u64), out_pitch = ct_words * output_count * sizeof(u64);
     for (const auto &leaf : plan.root_leaves)
-        CK(cudaMemcpyAsync(d_out + ct_words * leaf.second, d_in + ct_words * leaf.first, ct_words * sizeof(u64),
-                           cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpy2DAsync(d_out + ct_words * leaf.second, out_pitch, d_in + ct_words * leaf.first, in_pitch,
+                             ct_words * sizeof(u64), (size_t)clients, cudaMemcpyDeviceToDevice, s));
     if (plan.levels.empty()) return HECUDA_OK;
     StreamBuffers tmp(s);
     u64 *level_buf[2] = {nullptr, nullptr}, *c1_buf[2] = {nullptr, nullptr}, *scratch = nullptr;
     ExpandStep *d_steps = nullptr;
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, plan.max_nodes));
-    CK(tmp.alloc(&level_buf[0], ct_words * plan.max_nodes));
-    CK(tmp.alloc(&level_buf[1], ct_words * plan.max_nodes));
-    CK(tmp.alloc(&c1_buf[0], ct_words * plan.max_nodes));
-    CK(tmp.alloc(&c1_buf[1], ct_words * plan.max_nodes));
+    // items per applyGalois pass: grows with the number of clients, so the launch count does not
+    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, plan.max_nodes)) * clients;
+    const size_t level_words = ct_words * plan.max_nodes * clients;
+    CK(tmp.alloc(&level_buf[0], level_words));
+    CK(tmp.alloc(&level_buf[1], level_words));
+    CK(tmp.alloc(&c1_buf[0], level_words));
+    CK(tmp.alloc(&c1_buf[1], level_words));
     CK(tmp.alloc(&scratch, galois_scratch_words(c, l) * (size_t)chunk));
     if (d_steps_ready) {
         d_steps = (ExpandStep *)d_steps_ready;
@@ -236,34 +292,42 @@ int32_t expand_device(const hecuda_context *h, const hecuda_evk *k, const u64 *d
     }
     const RowConsts rc = row_consts(c, l);
     const int threads = n >= 256 ? 256 : (n < 32 ? 32 : (int)n);
-    const u64 *cur = d_in;  // the active roots are a prefix of the input (only the last one can be a single output)
+    // the active roots are a prefix of each input (only the last one can be a single output); a level's nodes must be
+    // contiguous over all clients, so several clients' roots are gathered when a single-output root sits between them
+    const u64 *cur = d_in;
+    if (clients > 1 && plan.active_roots != ct_count) {
+        CK(cudaMemcpy2DAsync(level_buf[1], ct_words * plan.active_roots * sizeof(u64), d_in, in_pitch,
+                             ct_words * plan.active_roots * sizeof(u64), (size_t)clients, cudaMemcpyDeviceToDevice, s));
+        cur = level_buf[1];
+    }
     int flip = 0;
-    for (const PlanLevel &level : plan.levels) {
-        unsigned element = 0;
-        int times = 0;
-        const u64 *key = nullptr;
-        int32_t rc32 = pick_galois(k, n, level.log_step, &element, &times, &key);
-        if (rc32) return rc32;
+    for (size_t li = 0; li < plan.levels.size(); ++li) {
+        const PlanLevel &level = plan.levels[li];
+        const LevelKeys &lk = level_keys[li];
+        KsKeyTable &table = tables[li];
+        const int64_t total = level.nodes * clients;
         const u64 *c1 = cur;
-        for (int t = 0; t < times; ++t) {  // c1.applyGalois(element:using:) `times` times (:223-227)
+        for (int t = 0; t < lk.times; ++t) {  // c1.applyGalois(element:using:) `times` times (:223-227)
             u64 *dst = c1_buf[t & 1];
-            for (int64_t done = 0; done < level.nodes; done += chunk) {
-                const int64_t items = std::min<int64_t>(chunk, level.nodes - done);
-                cudaError_t e = apply_galois_chunk(c, scratch, key, c1 + ct_words * done, l, element, dst + ct_words * done,
-                                                   items, s);
+            for (int64_t done = 0; done < total; done += chunk) {
+                const int64_t items = std::min<int64_t>(chunk, total - done);
+                table.item0 = done;
+                cudaError_t e = apply_galois_chunk(c, scratch, lk.key[0], c1 + ct_words * done, l, lk.element,
+                                                   dst + ct_words * done, items, s, clients > 1 ? &table : nullptr);
                 if (e != cudaSuccess) return cuda_fail(e, "expand: applyGalois");
             }
             c1 = dst;
         }
         u64 *next = level_buf[flip];
         flip ^= 1;
+        const int64_t next_nodes = li + 1 < plan.levels.size() ? plan.levels[li + 1].nodes : 0;
         const unsigned shift = (unsigned)(2 * n) - (1u << (level.log_step - 1));  // -2^(logStep-1) mod 2N
-        for (int64_t done = 0; done < level.nodes;) {
-            const int64_t items = std::min<int64_t>(level.nodes - done, 65535);
+        for (int64_t done = 0; done < total;) {
+            const int64_t items = std::min<int64_t>(total - done, 65535);
             dim3 grid((unsigned)((n + threads - 1) / threads), (unsigned)(2 * l), (unsigned)items);
             ++g_kernel_launches;
-            expand_combine_kernel<<<grid, threads, 0, s>>>(cur + ct_words * done, c1 + ct_words * done, next, d_out,
-                                                           d_steps + level.step_offset + done, rc, c.logn, shift);
+            expand_combine_kernel<<<grid, threads, 0, s>>>(cur, c1, next, d_out, d_steps + level.step_offset, rc, c.logn, shift,
+                                                           done, (int)level.nodes, next_nodes, output_count);
             done += items;
         }
         CK(cudaGetLastError());
@@ -306,7 +370,7 @@ int32_t compute_response_device(const hecuda_context *h, const hecuda_evk *k, co
     u64 *expanded = nullptr, *first_eval = nullptr, *results[2] = {nullptr, nullptr}, *lhs = nullptr, *ct3 = nullptr,
         *scratch = nullptr;
     CK(tmp.alloc(&expanded, ct_words * eqc * indices_count));
-    int32_t rc = expand_device(h, k, d_query, query_ct_count, eqc * indices_count, expanded, s, d_steps_ready);
+    int32_t rc = expand_device(h, &k, 1, d_query, query_ct_count, eqc * indices_count, expanded, s, d_steps_ready);
     if (rc) return rc;
     CK(tmp.alloc(&first_eval, ct_words * dim0));
     CK(tmp.alloc(&results[0], ct_words * rows));
@@ -404,6 +468,157 @@ int32_t check_response_args(const hecuda_context *h, const hecuda_evk *k, const 
                                                          ", expected " + std::to_string(shape.chunk_count * shape.per_chunk));
     }
     return check_expand_args(h, k, query, query_ct_count, shape.expanded_query_count * indices_count, out);
+}
+
+// ---------------------------------------------------------------- many clients per call
+static_assert(HECUDA_MULPIR_CLIENT_GROUP == kKeyTableSize, "one key-table entry per client of a group");
+static_assert(HECUDA_MULPIR_CLIENT_GROUP == kScanClientTile * kScanClientTiles, "one scan launch per client group");
+
+// Every client checked like a single call, and every client's Galois keys resolved for every expansion level, before
+// any group is enqueued: a failure leaves the caller's stream and `out` untouched, and its message names the client
+// by its index in the call.
+int32_t check_clients_args(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count,
+                           const hecuda_pir_database *const *dbs, int32_t db_count, const int32_t *dims, int32_t dim_count,
+                           int32_t chunk_count, const uint64_t *queries, int32_t query_ct_count, int32_t indices_count,
+                           const void *out, ResponseShape &shape) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (!evks) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (client_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "client_count must be at least 1");
+    for (int32_t j = 0; j < client_count; ++j) {
+        rc = check_response_args(h, evks[j], dbs, db_count, dims, dim_count, chunk_count, queries, query_ct_count,
+                                 indices_count, out, shape);
+        if (rc) return fail(rc, "client " + std::to_string(j) + ": " + last_error_cstr());
+    }
+    const ExpandPlan plan = build_expand_plan(h->ctx->n, query_ct_count, shape.expanded_query_count * indices_count);
+    std::vector<LevelKeys> level_keys;
+    return resolve_level_keys(evks, client_count, 0, h->ctx->n, plan, level_keys);
+}
+
+// The expansion plan of a query shape on the device, uploaded the first time the context sees the shape, so that
+// later calls enqueue without waiting for a copy.  The upload runs outside the context's lock; when two threads race
+// on a new shape, the second copy is dropped.
+int32_t expand_steps_on_device(const hecuda_context *hc, int64_t n, int64_t ct_count, int64_t output_count, const void **out) {
+    hecuda_context *h = const_cast<hecuda_context *>(hc);
+    const std::pair<int64_t, int64_t> shape{ct_count, output_count};
+    {
+        std::lock_guard<std::mutex> lock(h->mu);
+        auto it = h->expand_steps.find(shape);
+        if (it != h->expand_steps.end()) {
+            *out = it->second;
+            return HECUDA_OK;
+        }
+    }
+    const ExpandPlan plan = build_expand_plan(n, ct_count, output_count);
+    void *d = nullptr;
+    cudaError_t e = cudaMalloc(&d, std::max<size_t>(plan.steps.size(), 1) * sizeof(ExpandStep));
+    if (e == cudaSuccess && !plan.steps.empty()) e = upload(d, plan.steps.data(), plan.steps.size() * sizeof(ExpandStep));
+    if (e != cudaSuccess) {
+        if (d) cudaFree(d);
+        return cuda_fail(e, "expansion plan upload");
+    }
+    std::lock_guard<std::mutex> lock(h->mu);
+    auto ins = h->expand_steps.insert({shape, d});
+    if (!ins.second) cudaFree(d);  // another thread uploaded the same plan first; nothing has used this copy
+    *out = ins.first->second;
+    return HECUDA_OK;
+}
+
+// PirUtil.computeResponse for `clients` (<= HECUDA_MULPIR_CLIENT_GROUP) queries of the same shape, client j with
+// keys[j]: d_query = clients x query_ct_count ciphertexts, d_out = clients x indices_count x chunk_count x 2 x 1 x N.
+// Each stage is one pass over all clients; the first dimension streams every database once for the whole group.
+// first_client: the call-wide index of keys[0] (the keys were resolved by check_clients_args).
+int32_t compute_response_clients_device(const hecuda_context *h, const hecuda_evk *const *keys, int clients,
+                                        int first_client, const hecuda_pir_database *const *dbs, int32_t db_count,
+                                        const ResponseShape &shape, const u64 *d_query, int64_t query_ct_count,
+                                        int64_t indices_count, u64 *d_out, cudaStream_t s) {
+    const Context &c = *h->ctx;
+    const int L = c.L;
+    const int64_t n = c.n;
+    const size_t ct_words = (size_t)2 * L * n, reply_words = (size_t)2 * n * shape.chunk_count;
+    const int64_t eqc = shape.expanded_query_count, dim0 = shape.dims[0];
+    const int64_t rows = shape.chunk_count * shape.columns;
+    const int64_t client_cts = eqc * indices_count;  // expanded ciphertexts per client
+    const void *d_steps = nullptr;
+    int32_t rc = expand_steps_on_device(h, n, query_ct_count, client_cts, &d_steps);
+    if (rc) return rc;
+    StreamBuffers tmp(s);
+    u64 *expanded = nullptr, *query_eval = nullptr, *results[2] = {nullptr, nullptr}, *lhs = nullptr, *ct3 = nullptr,
+        *scratch = nullptr, *replies = nullptr;
+    CK(tmp.alloc(&expanded, ct_words * client_cts * clients));
+    rc = expand_device(h, keys, clients, d_query, query_ct_count, client_cts, expanded, s, d_steps, first_client);
+    if (rc) return rc;
+    // firstDimensionQueries: convertToEvalFormat (:523-532).  All expanded ciphertexts go through one forward NTT, so
+    // the first-dimension slices of every client and index are transformed in one launch.  Only those slices are read;
+    // the others (dims[1..] per index: 75 of 512 ciphertexts at the C4 shape, ~15 % of this NTT) are transformed for
+    // nothing, which moves fewer bytes than gathering the first-dimension slices into a contiguous buffer would.
+    CK(tmp.alloc(&query_eval, ct_words * client_cts * clients));
+    CK(tmp.alloc(&results[0], ct_words * rows * clients));
+    CK(tmp.alloc(&results[1], ct_words * rows * clients));
+    CK(tmp.alloc(&replies, reply_words * clients));
+    size_t scratch_words = 0, lhs_words = 0, ct3_words = 0;
+    {
+        int64_t count = rows;
+        for (size_t d = 1; d < shape.dims.size(); ++d) {
+            const int64_t size = shape.dims[d], groups = count / size;
+            scratch_words = std::max(scratch_words, inner_product_scratch_words(c, size) * (size_t)(groups * clients));
+            scratch_words = std::max(scratch_words, relinearize_scratch_words(c, L) * (size_t)(groups * clients));
+            lhs_words = std::max(lhs_words, ct_words * (size_t)(size * groups * clients));
+            ct3_words = std::max(ct3_words, (size_t)3 * L * n * groups * clients);
+            count = groups;
+        }
+    }
+    CK(tmp.alloc(&scratch, scratch_words));
+    CK(tmp.alloc(&lhs, lhs_words));
+    CK(tmp.alloc(&ct3, ct3_words));
+    KsKeyTable relin{};
+    for (int j = 0; j < clients; ++j) relin.key[j] = keys[j]->d_relin;
+    const NttRowMap map = c.map_q(L);
+    cudaError_t e;
+    if ((e = launch_ntt_forward(c, map, expanded, query_eval, client_cts * clients * 2 * L, s)) != cudaSuccess)
+        return cuda_fail(e, "ntt");
+    const size_t client_pitch = ct_words * client_cts * sizeof(u64);
+    for (int64_t qi = 0; qi < indices_count; ++qi) {
+        const hecuda_pir_database *db = dbs[db_count == 1 ? 0 : qi];
+        // every column of every chunk for every client: Scheme.innerProduct(ciphertexts:plaintexts:) (:427-435)
+        e = launch_inner_product_plain_clients(c, query_eval + ct_words * eqc * qi, (int64_t)ct_words * client_cts, clients, L,
+                                               dim0, db->d_plain, db->d_plain32, db->d_present, results[0],
+                                               (int64_t)ct_words * rows, rows, s);
+        if (e != cudaSuccess) return cuda_fail(e, "innerProduct(ciphertexts:plaintexts:)");
+        if ((e = launch_ntt_inverse(c, map, results[0], results[0], rows * clients * 2 * L, kScalePlain, s)) != cudaSuccess)
+            return cuda_fail(e, "ntt");
+        int64_t count = rows, query_start = dim0;
+        int cur = 0;
+        for (size_t d = 1; d < shape.dims.size(); ++d) {  // remaining dimensions (:447-480)
+            const int64_t size = shape.dims[d], groups = count / size;
+            const size_t slice = ct_words * size * sizeof(u64);
+            for (int64_t g = 0; g < groups; ++g)  // vector0 = the client's query slice, for each of its groups
+                CK(cudaMemcpy2DAsync(lhs + ct_words * size * g, slice * groups, expanded + ct_words * (eqc * qi + query_start),
+                                     client_pitch, slice, (size_t)clients, cudaMemcpyDeviceToDevice, s));
+            if ((e = inner_product_chunk(c, scratch, lhs, results[cur], size, ct3, groups * clients, s)) != cudaSuccess)
+                return cuda_fail(e, "innerProduct");
+            relin.items_per_client = groups;
+            if ((e = relinearize_chunk(c, scratch, nullptr, ct3, L, results[cur ^ 1], groups * clients, s, &relin)) != cudaSuccess)
+                return cuda_fail(e, "relinearize");
+            cur ^= 1;
+            count = groups;
+            query_start += size;
+        }
+        if (count != shape.chunk_count)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "There should be only 1 ciphertext in the final result for each chunk");
+        // modSwitchDownToSingle (HeScheme.swift:1481-1485); BFV's canonical format is already Coeff
+        const u64 *single = results[cur];
+        for (int l = L; l > 1; --l) {
+            u64 *dst = l == 2 ? replies : results[cur ^ 1];
+            if ((e = launch_mod_switch(c, results[cur], l, dst, count * 2 * clients, s)) != cudaSuccess)
+                return cuda_fail(e, "modSwitchDown");
+            cur ^= 1;
+            single = dst;
+        }
+        CK(cudaMemcpy2DAsync(d_out + reply_words * qi, reply_words * indices_count * sizeof(u64), single,
+                             reply_words * sizeof(u64), reply_words * sizeof(u64), (size_t)clients, cudaMemcpyDeviceToDevice, s));
+    }
+    return HECUDA_OK;
 }
 
 
@@ -638,7 +853,7 @@ int32_t hecuda_mulpir_expand_device(const hecuda_context *h, const hecuda_evk *k
                                     int64_t output_count, uint64_t *out, void *stream) {
     int32_t rc = check_expand_args(h, k, cts, ct_count, output_count, out);
     if (rc) return rc;
-    return expand_device(h, k, (const u64 *)cts, ct_count, output_count, (u64 *)out, (cudaStream_t)stream);
+    return expand_device(h, &k, 1, (const u64 *)cts, ct_count, output_count, (u64 *)out, (cudaStream_t)stream);
 }
 
 int32_t hecuda_mulpir_expand(const hecuda_context *h, const hecuda_evk *k, const uint64_t *cts, int32_t ct_count,
@@ -654,7 +869,7 @@ int32_t hecuda_mulpir_expand(const hecuda_context *h, const hecuda_evk *k, const
     CK(tmp.alloc(&d_in, ct_words * ct_count));
     CK(tmp.alloc(&d_out, ct_words * output_count));
     CK(cudaMemcpyAsync(d_in, cts, ct_words * ct_count * sizeof(u64), cudaMemcpyHostToDevice, s));
-    rc = expand_device(h, k, d_in, ct_count, output_count, d_out, s);
+    rc = expand_device(h, &k, 1, d_in, ct_count, output_count, d_out, s);
     if (rc) {
         wait_stream(s);
         return rc;
@@ -714,6 +929,59 @@ int32_t hecuda_mulpir_compute_response(const hecuda_context *h, const hecuda_evk
         return rc;
     }
     CK(cudaMemcpyAsync(out, d_out, out_words * sizeof(u64), cudaMemcpyDeviceToHost, s));
+    CK(wait_stream(s));
+    return HECUDA_OK;
+}
+
+int32_t hecuda_mulpir_compute_response_clients_device(const hecuda_context *h, const hecuda_evk *const *evks,
+                                                      int32_t client_count, const hecuda_pir_database *const *dbs,
+                                                      int32_t db_count, const int32_t *dims, int32_t dim_count,
+                                                      int32_t chunk_count, const uint64_t *queries, int32_t query_ct_count,
+                                                      int32_t indices_count, uint64_t *out, void *stream) {
+    ResponseShape shape;
+    int32_t rc = check_clients_args(h, evks, client_count, dbs, db_count, dims, dim_count, chunk_count, queries,
+                                    query_ct_count, indices_count, out, shape);
+    if (rc) return rc;
+    const size_t query_words = (size_t)2 * h->ctx->L * h->ctx->n * query_ct_count;
+    const size_t out_words = (size_t)2 * h->ctx->n * chunk_count * indices_count;
+    for (int32_t first = 0; first < client_count; first += HECUDA_MULPIR_CLIENT_GROUP) {
+        const int clients = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count - first);
+        rc = compute_response_clients_device(h, evks + first, clients, first, dbs, db_count, shape, (const u64 *)queries + query_words * first,
+                                             query_ct_count, indices_count, (u64 *)out + out_words * first, (cudaStream_t)stream);
+        if (rc) return rc;
+    }
+    return HECUDA_OK;
+}
+
+int32_t hecuda_mulpir_compute_response_clients(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count,
+                                               const hecuda_pir_database *const *dbs, int32_t db_count, const int32_t *dims,
+                                               int32_t dim_count, int32_t chunk_count, const uint64_t *queries,
+                                               int32_t query_ct_count, int32_t indices_count, uint64_t *out) {
+    ResponseShape shape;
+    int32_t rc = check_clients_args(h, evks, client_count, dbs, db_count, dims, dim_count, chunk_count, queries,
+                                    query_ct_count, indices_count, out, shape);
+    if (rc) return rc;
+    WsGuard g(h);
+    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    cudaStream_t s = g.w->stream;
+    const size_t query_words = (size_t)2 * h->ctx->L * h->ctx->n * query_ct_count;
+    const size_t out_words = (size_t)2 * h->ctx->n * chunk_count * indices_count;
+    const int group = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count);
+    StreamBuffers tmp(s);
+    u64 *d_query = nullptr, *d_out = nullptr;
+    CK(tmp.alloc(&d_query, query_words * group));
+    CK(tmp.alloc(&d_out, out_words * group));
+    for (int32_t first = 0; first < client_count; first += group) {
+        const int clients = std::min<int32_t>(group, client_count - first);
+        CK(cudaMemcpyAsync(d_query, queries + query_words * first, query_words * clients * sizeof(u64), cudaMemcpyHostToDevice, s));
+        rc = compute_response_clients_device(h, evks + first, clients, first, dbs, db_count, shape, d_query, query_ct_count,
+                                             indices_count, d_out, s);
+        if (rc) {
+            wait_stream(s);
+            return rc;
+        }
+        CK(cudaMemcpyAsync(out + out_words * first, d_out, out_words * clients * sizeof(u64), cudaMemcpyDeviceToHost, s));
+    }
     CK(wait_stream(s));
     return HECUDA_OK;
 }

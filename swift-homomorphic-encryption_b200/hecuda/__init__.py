@@ -105,6 +105,12 @@ SYMBOLS = {
                                                    C.c_int32, _VP, C.c_int32, C.c_int32, _VP]),
     "hecuda_mulpir_compute_response_device": (C.c_int32, [_VP, _VP, C.POINTER(_VP), C.c_int32, C.POINTER(C.c_int32),
                                                           C.c_int32, C.c_int32, _VP, C.c_int32, C.c_int32, _VP, _VP]),
+    "hecuda_mulpir_compute_response_clients": (C.c_int32, [_VP, C.POINTER(_VP), C.c_int32, C.POINTER(_VP), C.c_int32,
+                                                           C.POINTER(C.c_int32), C.c_int32, C.c_int32, _VP, C.c_int32,
+                                                           C.c_int32, _VP]),
+    "hecuda_mulpir_compute_response_clients_device": (C.c_int32, [_VP, C.POINTER(_VP), C.c_int32, C.POINTER(_VP), C.c_int32,
+                                                                  C.POINTER(C.c_int32), C.c_int32, C.c_int32, _VP, C.c_int32,
+                                                                  C.c_int32, _VP, _VP]),
     "hecuda_mulpir_compute_response_wire": (C.c_int32, [_VP, _VP, C.POINTER(_VP), C.c_int32, C.POINTER(C.c_int32), C.c_int32,
                                                         C.c_int32, _VP, _VP, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _VP]),
     "hecuda_pnns_matrix_create": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.POINTER(_VP)]),

@@ -383,3 +383,24 @@ class MulPirServer:
             ctx._h, evaluationKey._h, handles, len(self.databases), dims, len(self.parameter.dimensions), self.chunkCount,
             _ptr(cts), cts.size // words, indicesCount, _ptr(out)))
         return out
+
+    def computeResponses(self, queries, evaluationKeys: Sequence[EvaluationKey], indicesCount: int = 1) -> np.ndarray:
+        """computeResponse for many clients in one C-ABI call: client c's query with evaluationKeys[c], each reply
+        bit-identical to `computeResponse(queries[c], evaluationKeys[c], indicesCount)`.  Groups of up to
+        HECUDA_MULPIR_CLIENT_GROUP clients share one pass over each database.
+
+        queries: (clients, queryCiphertextCount, 2, L, N) Coeff.  Returns (clients, indicesCount, chunkCount, 2, 1, N)."""
+        ctx = self.context
+        keys = list(evaluationKeys)
+        cts = _host(queries)
+        words = 2 * ctx.L * ctx.degree
+        if not keys or cts.size % (words * len(keys)):
+            raise HeError(-1, "invalidCiphertext: queries must be one set of 2 x L x N ciphertexts per evaluation key")
+        handles = (C.c_void_p * len(self.databases))(*[db._h for db in self.databases])
+        key_handles = (C.c_void_p * len(keys))(*[k._h for k in keys])
+        dims = (C.c_int32 * len(self.parameter.dimensions))(*self.parameter.dimensions)
+        out = np.empty((len(keys), indicesCount, self.chunkCount, 2, 1, ctx.degree), dtype=np.uint64)
+        _check(load_library().hecuda_mulpir_compute_response_clients(
+            ctx._h, key_handles, len(keys), handles, len(self.databases), dims, len(self.parameter.dimensions),
+            self.chunkCount, _ptr(cts), cts.size // (words * len(keys)), indicesCount, _ptr(out)))
+        return out
