@@ -193,6 +193,18 @@ int32_t hecuda_evk_set_galois_key(hecuda_evk *evk, uint32_t element, const uint6
 /* Device buffer of the key for `element` (allocated if absent), for multi-GPU setups that fill it with a collective
  * the way hecuda_evk_device_buffer does for the relinearization key. */
 int32_t hecuda_evk_galois_device_buffer(hecuda_evk *evk, uint32_t element, void **device_ptr, uint64_t *bytes);
+/* EvaluationKey(deserialize:context:) -- SerializedKeys.swift:141-157, every key ciphertext .seeded(poly0:seed:)
+ * (SerializedCiphertext.swift:126-154; encryptZero keeps its seed, Bfv+Keys.swift:69-103).  B =
+ * hecuda_poly_serialized_byte_count(ctx, HECUDA_BASE_KEYSWITCH, L+1, 0).  relin_poly0: L x B, relin_seeds: L x 32
+ * (both NULL = no relinearization key); galois_poly0: element_count x L x B, galois_seeds: element_count x L x 32, in the
+ * order of elements[].  The DRBG expansion of `a` over [q_0..q_{L-1}, q_ks] and the unpacking of poly0 run on the device
+ * and write the key buffers directly (Eval format: no NTT).  The result is an ordinary evaluation key.  It returns once
+ * the keys are written.  HECUDA_ERR_UNSUPPORTED with a single coefficient modulus; HECUDA_ERR_INVALID_ARGUMENT when exactly
+ * one of relin_poly0 / relin_seeds is NULL, for a negative element_count or NULL Galois arrays, and for an invalid or
+ * repeated element.  On error *out is NULL.  A Bfv<UInt32> context takes the same bytes. */
+int32_t hecuda_evk_create_serialized(const hecuda_context *ctx, const uint8_t *relin_poly0, const uint8_t *relin_seeds,
+                                     const uint32_t *elements, int32_t element_count, const uint8_t *galois_poly0,
+                                     const uint8_t *galois_seeds, hecuda_evk **out);
 /* Bfv.applyGalois(ciphertext:element:using:) -- Bfv/Bfv.swift:174-198 (rotateColumns / swapRows call this with
  * GaloisElement.rotatingColumns / swappingRows, HeScheme.swift:1463-1478).  ct, out: batch x 2 x l x N (Coeff). */
 int32_t hecuda_bfv_apply_galois(const hecuda_context *ctx, const hecuda_evk *evk, const uint64_t *ct,
@@ -360,6 +372,20 @@ int32_t hecuda_mulpir_compute_response_wire(const hecuda_context *ctx, const hec
                                             const uint8_t *query_poly0, const uint8_t *query_seeds,
                                             int32_t query_ciphertext_count, int32_t indices_count, int32_t skip_lsbs_poly0,
                                             int32_t skip_lsbs_poly1, uint8_t *out);
+
+/* hecuda_mulpir_compute_response_clients on the wire: each client's bytes are what hecuda_mulpir_compute_response_wire
+ * returns for that client alone.  query_poly0: client_count x query_ciphertext_count x byteCount(L rows, skipLSBs 0),
+ * query_seeds: client_count x query_ciphertext_count x 32; out: client_count x indices_count x chunk_count x
+ * (byteCount(1 row, skip0) + byteCount(1 row, skip1)).  Arguments are checked and keys resolved as by the two calls it
+ * combines.  Per group of HECUDA_MULPIR_CLIENT_GROUP clients: one seeded expansion of all the group's query ciphertexts,
+ * the many-clients response pipeline, and one packing pass per reply poly. */
+int32_t hecuda_mulpir_compute_response_clients_wire(const hecuda_context *ctx, const hecuda_evk *const *evks,
+                                                    int32_t client_count, const hecuda_pir_database *const *databases,
+                                                    int32_t database_count, const int32_t *dimensions,
+                                                    int32_t dimension_count, int32_t chunk_count, const uint8_t *query_poly0,
+                                                    const uint8_t *query_seeds, int32_t query_ciphertext_count,
+                                                    int32_t indices_count, int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1,
+                                                    uint8_t *out);
 
 /* ---- PNNS server: encrypted vector x plaintext matrix (SURVEY.md section 8f, rank 3) ----
  * Device-resident PlaintextMatrix in `.diagonal(babyStepGiantStep:)` packing (PrivateNearestNeighborSearch/

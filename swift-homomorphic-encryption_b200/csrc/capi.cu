@@ -901,6 +901,86 @@ int32_t hecuda_evk_galois_device_buffer(hecuda_evk *k, uint32_t element, void **
     return HECUDA_OK;
 }
 
+// EvaluationKey(deserialize:context:) (SerializedKeys.swift:141-157) with every key ciphertext .seeded: one DRBG chain
+// pass over all the key's seeds, then one fused kernel that writes poly0 and poly1 of every ciphertext into the key's
+// device buffers (drbg.cu).
+int32_t hecuda_evk_create_serialized(const hecuda_context *h, const uint8_t *relin_poly0, const uint8_t *relin_seeds,
+                                     const uint32_t *elements, int32_t element_count, const uint8_t *galois_poly0,
+                                     const uint8_t *galois_seeds, hecuda_evk **out) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (!out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    const Context &c = *h->ctx;
+    if (!c.has_ks)
+        return fail(HECUDA_ERR_UNSUPPORTED, "unsupportedHeOperation: a single coefficient modulus leaves no key-switching modulus");
+    if ((relin_poly0 == nullptr) != (relin_seeds == nullptr))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "relin_poly0 and relin_seeds must both be given or both be null");
+    if (element_count < 0 || (element_count > 0 && (!elements || !galois_poly0 || !galois_seeds)))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    std::vector<uint32_t> sorted(elements, elements + element_count);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint32_t e : sorted)
+        if (!valid_galois_element(e, c.n)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid Galois element " + std::to_string(e));
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "repeated Galois element " + std::to_string(*std::adjacent_find(sorted.begin(), sorted.end())));
+    uint64_t poly_bytes = 0;
+    if ((rc = hecuda_poly_serialized_byte_count(h, HECUDA_BASE_KEYSWITCH, c.L + 1, 0, &poly_bytes))) return rc;
+    const bool relin = relin_poly0 != nullptr;
+    const int64_t count = (int64_t)(relin + element_count) * c.L;  // key ciphertexts
+    hecuda_evk *k = nullptr;
+    if ((rc = hecuda_evk_create_empty(h, &k))) return rc;
+    // ciphertext i of key j lands at key_j + i x 2 x K x N: the relinearization key, then galois[elements[e]]
+    std::vector<u64 *> dst;
+    dst.reserve((size_t)count);
+    const size_t ct_words = k->words / c.L;
+    cudaError_t e = cudaSuccess;
+    for (int32_t j = -1; j < element_count && e == cudaSuccess; ++j) {
+        u64 *key = nullptr;
+        if (j < 0) {
+            if (!relin) continue;
+            key = k->d_relin;
+        } else if ((e = cudaMalloc(&key, k->words * sizeof(u64))) == cudaSuccess) {
+            k->galois[elements[j]] = key;
+        }
+        for (int i = 0; key && i < c.L; ++i) dst.push_back(key + ct_words * i);
+    }
+    if (e == cudaSuccess && count > 0) {
+        WsGuard g(h);
+        if (!g.w) {
+            hecuda_evk_destroy(k);
+            return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+        }
+        cudaStream_t s = g.w->stream;
+        const size_t relin_cts = relin ? (size_t)c.L : 0, galois_cts = (size_t)element_count * c.L;
+        unsigned char *d_poly0 = nullptr, *d_seeds = nullptr;
+        u64 **d_dst = nullptr;
+        e = cudaMallocAsync((void **)&d_poly0, poly_bytes * count, s);
+        if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_seeds, (size_t)32 * count, s);
+        if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_dst, sizeof(u64 *) * count, s);
+        if (e == cudaSuccess && relin) e = cudaMemcpyAsync(d_poly0, relin_poly0, poly_bytes * relin_cts, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess && relin) e = cudaMemcpyAsync(d_seeds, relin_seeds, 32 * relin_cts, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess && galois_cts)
+            e = cudaMemcpyAsync(d_poly0 + poly_bytes * relin_cts, galois_poly0, poly_bytes * galois_cts, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess && galois_cts)
+            e = cudaMemcpyAsync(d_seeds + 32 * relin_cts, galois_seeds, 32 * galois_cts, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_dst, dst.data(), sizeof(u64 *) * count, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = expand_seeded_keys_device(c, d_poly0, d_seeds, d_dst, count, s);
+        for (void *p : {(void *)d_poly0, (void *)d_seeds, (void *)d_dst})
+            if (p) cudaFreeAsync(p, s);
+        // the keys are read on other non-blocking streams: return once the kernel has written them (see upload())
+        const cudaError_t e2 = wait_stream(s);
+        if (e == cudaSuccess) e = e2;
+    }
+    if (e != cudaSuccess) {
+        hecuda_evk_destroy(k);
+        return cuda_fail(e, "evk_create_serialized");
+    }
+    k->loaded = relin;
+    *out = k;
+    return HECUDA_OK;
+}
+
 static int32_t check_galois(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct, int32_t l, uint32_t element,
                             uint64_t *out, int64_t batch, const u64 **key) {
     int32_t rc = check_ctx(h);

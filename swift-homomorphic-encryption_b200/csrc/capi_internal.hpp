@@ -156,6 +156,10 @@ cudaError_t apply_galois_chunk(const Context &c, u64 *scratch, const u64 *key, c
                                u64 *out, int64_t items, cudaStream_t s, const KsKeyTable *keys = nullptr);
 cudaError_t expand_seeded_device(const Context &c, int l, const unsigned char *d_poly0, const unsigned char *d_seeds, u64 *d_out,
                                  int64_t batch, cudaStream_t s);
+// `count` seeded key-switching ciphertexts (K = L + 1 rows, Eval): d_poly0 count x byteCount(K rows) bytes, d_seeds
+// count x 32; ciphertext i's 2 x K x N words go to d_dst[i] (a device table of pointers into evaluation keys)
+cudaError_t expand_seeded_keys_device(const Context &c, const unsigned char *d_poly0, const unsigned char *d_seeds,
+                                      u64 *const *d_dst, int64_t count, cudaStream_t s);
 cudaError_t inner_product_chunk(const Context &c, u64 *scratch, const u64 *lhs, const u64 *rhs, int64_t pairs, u64 *out,
                                 int64_t groups, cudaStream_t s);
 

@@ -22,21 +22,9 @@ __global__ void __launch_bounds__(256) poly_load_kernel(const unsigned char *__r
     if (i >= n) return;
     const int row = blockIdx.y;
     const int64_t poly = blockIdx.z;
-    const int w = c.width[row];
     const long long row_bytes = c.byte_offset[row + 1] - c.byte_offset[row];
     const unsigned char *src = bytes + poly * c.byte_offset[c.rows] + c.byte_offset[row];
-    const long long bit = (long long)i * w;
-    const long long first = bit >> 3;
-    const int shift = (int)(bit & 7);
-    u128 acc = 0;  // 9 bytes cover shift + w <= 7 + 64 bits
-#pragma unroll
-    for (int k = 0; k < 9; ++k) {
-        const long long at = first + k;
-        acc = (acc << 8) | (u128)(at < row_bytes ? src[at] : 0);
-    }
-    const u64 mask = w >= 64 ? ~0ull : ((1ull << w) - 1);
-    const u64 v = (u64)(acc >> (72 - shift - w)) & mask;
-    out[(poly * c.rows + row) * n + i] = v << skip;
+    out[(poly * c.rows + row) * n + i] = codec_unpack(src, row_bytes, c.width[row], i) << skip;
 }
 
 // coefficients -> bytes: one thread per output byte

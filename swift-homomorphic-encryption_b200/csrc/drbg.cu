@@ -9,7 +9,9 @@
 // (key_{s+1}, V_{s+1}) come from two more blocks of the same keystream.  One thread per seed walks that chain (it is
 // inherently sequential, 2 block encryptions + 1 key schedule per segment) and leaves the expanded round keys; then
 // every 16-byte block of every segment is independent: one CTA per segment, one thread per block = per coefficient
-// (a coefficient consumes exactly one little-endian 128-bit word, reduced modulo its row modulus).
+// (a coefficient consumes exactly one little-endian 128-bit word, reduced modulo its row modulus).  Seeded evaluation
+// keys (EvaluationKey(deserialize:), SerializedKeys.swift:141-157) use the same chain over K = L + 1 rows, then one fused
+// kernel that also unpacks poly0 and writes both polys into the key buffers.
 // AES is FIPS-197 written from the specification (S-box, ShiftRows, MixColumns over GF(2^8)); the reference gets it
 // from swift-crypto.  Pinned by the reference's NIST vectors through the oracle (tests/test_oracle_drbg.py).
 #include <algorithm>
@@ -103,10 +105,41 @@ __global__ void __launch_bounds__(kSegmentBlocks) drbg_fill_kernel(const u32w *_
     out[(size_t)b * c.rows * n + k] = (u64)((((u128)hi << 64) | lo) % c.p[row]);
 }
 
-cudaError_t random_polys_device(const Context &c, int l, const unsigned char *d_seeds, u64 *d_out, int64_t batch,
-                                cudaStream_t s) {
-    int device = 0;
-    cudaGetDevice(&device);
+// EvaluationKey(deserialize:) of seeded key-switching ciphertexts (SerializedCiphertext.swift:53-60 with Format = Eval):
+// one CTA per (segment, ciphertext), one thread per coefficient k of the K x N stream.  poly1 = the DRBG word reduced
+// modulo its row's modulus, already in the key's Eval format (encryptZero samples `a` in Eval, Bfv+Encrypt.swift:156-157,
+// and convertFormat to Eval is the identity); poly0 = coefficient k unpacked from the ciphertext's serialized bytes.
+// Both go straight into the ciphertext's 2 x K x N words at dst[ciphertext].
+__global__ void __launch_bounds__(kSegmentBlocks) key_expand_kernel(const u32w *__restrict__ round_keys,
+                                                                    const u64 *__restrict__ counters,
+                                                                    const unsigned char *__restrict__ poly0,
+                                                                    u64 *const *__restrict__ dst, const __grid_constant__ FillConsts c,
+                                                                    const __grid_constant__ CodecConsts cc, int n, int segments) {
+    __shared__ unsigned char sbox[256];
+    __shared__ u32w te0[256];
+    __shared__ u32w rk[kRoundKeyWords];
+    const long long b = blockIdx.y;
+    const int s = blockIdx.x;
+    if (threadIdx.x < kRoundKeyWords) rk[threadIdx.x] = round_keys[((size_t)b * segments + s) * kRoundKeyWords + threadIdx.x];
+    load_tables(sbox, te0);
+    const long long k = (long long)s * kSegmentBlocks + threadIdx.x;
+    if (k >= (long long)c.rows * n) return;
+    u32w blk[4];
+    counter_block(counters[2 * ((size_t)b * segments + s)], counters[2 * ((size_t)b * segments + s) + 1], 1 + (u64)threadIdx.x, blk);
+    encrypt_block(blk, rk, te0, sbox);
+    const u64 lo = (u64)__byte_perm(blk[0], 0, 0x0123) | ((u64)__byte_perm(blk[1], 0, 0x0123) << 32);
+    const u64 hi = (u64)__byte_perm(blk[2], 0, 0x0123) | ((u64)__byte_perm(blk[3], 0, 0x0123) << 32);
+    const int row = (int)(k / n);
+    const long long i = k - (long long)row * n;
+    const unsigned char *src = poly0 + b * cc.byte_offset[cc.rows] + cc.byte_offset[row];
+    u64 *out = dst[b];
+    out[k] = codec_unpack(src, cc.byte_offset[row + 1] - cc.byte_offset[row], cc.width[row], i);
+    out[(long long)c.rows * n + k] = (u64)((((u128)hi << 64) | lo) % c.p[row]);
+}
+
+// The AES tables, then every seed's chain: (round keys, V) of each of its `segments` segments into *d_rk / *d_ctr, both
+// allocated on `s` and released by free_chains.
+cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, u32w **d_rk, u64 **d_ctr, cudaStream_t s) {
     unsigned char sbox[256];
     u32w te0[256];
     make_tables(sbox, te0);
@@ -115,16 +148,30 @@ cudaError_t random_polys_device(const Context &c, int l, const unsigned char *d_
     if (e != cudaSuccess) return e;
     e = cudaStreamSynchronize(s);  // the tables live on this stack frame
     if (e != cudaSuccess) return e;
+    e = cudaMallocAsync((void **)d_rk, (size_t)batch * segments * kRoundKeyWords * sizeof(u32w), s);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)d_ctr, (size_t)batch * segments * 2 * sizeof(u64), s);
+    if (e == cudaSuccess) {
+        ++g_kernel_launches;
+        drbg_chain_kernel<<<(unsigned)((batch + 31) / 32), 64, 0, s>>>(d_seeds, *d_rk, *d_ctr, segments, batch);
+        e = cudaGetLastError();
+    }
+    return e;
+}
+
+void free_chains(u32w *d_rk, u64 *d_ctr, int segments, int64_t batch, cudaStream_t s) {
+    if (d_rk) {
+        cudaMemsetAsync(d_rk, 0, (size_t)batch * segments * kRoundKeyWords * sizeof(u32w), s);  // key material
+        cudaFreeAsync(d_rk, s);
+    }
+    if (d_ctr) cudaFreeAsync(d_ctr, s);
+}
+
+cudaError_t random_polys_device(const Context &c, int l, const unsigned char *d_seeds, u64 *d_out, int64_t batch,
+                                cudaStream_t s) {
     const int segments = (int)(((size_t)l * c.n * 16 + kSegmentBytes - 1) / kSegmentBytes);
     u32w *d_rk = nullptr;
     u64 *d_ctr = nullptr;
-    e = cudaMallocAsync((void **)&d_rk, (size_t)batch * segments * kRoundKeyWords * sizeof(u32w), s);
-    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_ctr, (size_t)batch * segments * 2 * sizeof(u64), s);
-    if (e == cudaSuccess) {
-        ++g_kernel_launches;
-        drbg_chain_kernel<<<(unsigned)((batch + 31) / 32), 64, 0, s>>>(d_seeds, d_rk, d_ctr, segments, batch);
-        e = cudaGetLastError();
-    }
+    cudaError_t e = drbg_chains(d_seeds, segments, batch, &d_rk, &d_ctr, s);
     FillConsts fc;
     fc.rows = l;
     for (int r = 0; r < l; ++r) fc.p[r] = c.slots[c.slot_q(r)].dev.p;
@@ -137,11 +184,7 @@ cudaError_t random_polys_device(const Context &c, int l, const unsigned char *d_
         e = cudaGetLastError();
         done += part;
     }
-    if (d_rk) {
-        cudaMemsetAsync(d_rk, 0, (size_t)batch * segments * kRoundKeyWords * sizeof(u32w), s);  // key material
-        cudaFreeAsync(d_rk, s);
-    }
-    if (d_ctr) cudaFreeAsync(d_ctr, s);
+    free_chains(d_rk, d_ctr, segments, batch, s);
     return e;
 }
 
@@ -177,6 +220,33 @@ cudaError_t expand_seeded_device(const Context &c, int l, const unsigned char *d
     if (e == cudaSuccess) e = cudaMemcpy2DAsync(d_out + poly_words, 2 * pw, d_a, pw, pw, (size_t)batch, cudaMemcpyDeviceToDevice, s);
     if (d_a) cudaFreeAsync(d_a, s);
     if (d_p0) cudaFreeAsync(d_p0, s);
+    return e;
+}
+
+cudaError_t expand_seeded_keys_device(const Context &c, const unsigned char *d_poly0, const unsigned char *d_seeds,
+                                      u64 *const *d_dst, int64_t count, cudaStream_t s) {
+    const NttRowMap map = c.map_ks(c.L);  // row K-1 is q_ks
+    CodecConsts cc;
+    std::string err;
+    if (!codec_consts(c, map, 0, cc, err)) return cudaErrorInvalidValue;
+    const int rows = c.L + 1;
+    const int segments = (int)(((size_t)rows * c.n * 16 + kSegmentBytes - 1) / kSegmentBytes);
+    u32w *d_rk = nullptr;
+    u64 *d_ctr = nullptr;
+    cudaError_t e = drbg_chains(d_seeds, segments, count, &d_rk, &d_ctr, s);
+    FillConsts fc;
+    fc.rows = rows;
+    for (int r = 0; r < rows; ++r) fc.p[r] = c.slots[map.slot[r]].dev.p;
+    for (int64_t done = 0; e == cudaSuccess && done < count;) {
+        const int64_t part = std::min<int64_t>(count - done, 65535);
+        ++g_kernel_launches;
+        key_expand_kernel<<<dim3((unsigned)segments, (unsigned)part), kSegmentBlocks, 0, s>>>(
+            d_rk + (size_t)done * segments * kRoundKeyWords, d_ctr + (size_t)done * segments * 2,
+            d_poly0 + (size_t)done * serialized_poly_bytes(cc), d_dst + done, fc, cc, (int)c.n, segments);
+        e = cudaGetLastError();
+        done += part;
+    }
+    free_chains(d_rk, d_ctr, segments, count, s);
     return e;
 }
 

@@ -117,6 +117,20 @@ struct CodecConsts {
     int width[kMaxRows];                  // serialized bits per coefficient of each row
     long long byte_offset[kMaxRows + 1];  // of each row inside one serialized polynomial
 };
+// field i of one row: the `w` bits at bit i * w of the big-endian stream of the row's `row_bytes` bytes at `src`
+__device__ __forceinline__ u64 codec_unpack(const unsigned char *__restrict__ src, long long row_bytes, int w, long long i) {
+    const long long bit = i * w;
+    const long long first = bit >> 3;
+    const int shift = (int)(bit & 7);
+    u128 acc = 0;  // 9 bytes cover shift + w <= 7 + 64 bits
+#pragma unroll
+    for (int k = 0; k < 9; ++k) {
+        const long long at = first + k;
+        acc = (acc << 8) | (u128)(at < row_bytes ? src[at] : 0);
+    }
+    const u64 mask = w >= 64 ? ~0ull : ((1ull << w) - 1);
+    return (u64)(acc >> (72 - shift - w)) & mask;
+}
 bool codec_consts(const Context &ctx, const NttRowMap &map, int skip, CodecConsts &c, std::string &err);
 long long serialized_poly_bytes(const CodecConsts &c);
 cudaError_t launch_poly_load(const Context &ctx, const CodecConsts &c, int skip, const unsigned char *bytes, u64 *out,

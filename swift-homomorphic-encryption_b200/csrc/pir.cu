@@ -621,6 +621,54 @@ int32_t compute_response_clients_device(const hecuda_context *h, const hecuda_ev
     return HECUDA_OK;
 }
 
+// ---------------------------------------------------------------- wire format
+// Query ciphertexts arrive as SerializedCiphertext.seeded (SerializedCiphertext.swift:41-49: poly0 over all L rows,
+// skipLSBs 0, plus the seed).  Replies leave as .full(polys:skipLSBs:) with Bfv.skipLSBsForDecryption
+// (Bfv+Decrypt.swift:51-110): poly 0 and poly 1 are packed with different numbers of dropped low bits.
+struct WireCodec {
+    CodecConsts in, out[2];
+    int skip[2] = {0, 0};
+    size_t query_bytes = 0, bytes[2] = {0, 0};  // one serialized query poly0; one packed reply poly 0 / poly 1
+    u64 *polys = nullptr;                        // 2 x replies x N: poly p of every reply, contiguous
+    unsigned char *packed[2] = {nullptr, nullptr}, *reply = nullptr;  // replies x bytes[p]; replies x reply_bytes()
+    size_t reply_bytes() const { return bytes[0] + bytes[1]; }
+    int32_t setup(const Context &c, int skip0, int skip1) {
+        std::string err;
+        if (!codec_consts(c, c.map_q(c.L), 0, in, err) || !codec_consts(c, c.map_q(1), skip0, out[0], err) ||
+            !codec_consts(c, c.map_q(1), skip1, out[1], err))
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+        skip[0] = skip0, skip[1] = skip1;
+        query_bytes = (size_t)serialized_poly_bytes(in);
+        for (int p = 0; p < 2; ++p) bytes[p] = (size_t)serialized_poly_bytes(out[p]);
+        return HECUDA_OK;
+    }
+    cudaError_t alloc(StreamBuffers &tmp, const Context &c, int64_t replies) {  // buffers for up to `replies` replies
+        cudaError_t e = tmp.alloc(&polys, (size_t)2 * c.n * replies);
+        for (int p = 0; p < 2 && e == cudaSuccess; ++p)
+            e = tmp.alloc_bytes((void **)&packed[p], ((bytes[p] + 7) & ~(size_t)7) * replies + 8);
+        if (e == cudaSuccess) e = tmp.alloc_bytes((void **)&reply, reply_bytes() * replies);
+        return e;
+    }
+    // resp: replies x 2 x 1 x N (Coeff) -> reply: replies x (bytes[0] + bytes[1])
+    int32_t pack(const Context &c, const u64 *resp, int64_t replies, cudaStream_t s) {
+        const size_t pw = (size_t)c.n * sizeof(u64);
+        for (int p = 0; p < 2; ++p) {
+            CK(cudaMemcpy2DAsync(polys + (size_t)p * c.n * replies, pw, resp + (size_t)p * c.n, 2 * pw, pw, (size_t)replies,
+                                 cudaMemcpyDeviceToDevice, s));
+            cudaError_t e = launch_poly_serialize(c, out[p], skip[p], polys + (size_t)p * c.n * replies, packed[p], replies, s);
+            if (e != cudaSuccess) return cuda_fail(e, "serialize response");
+            CK(cudaMemcpy2DAsync(reply + (p ? bytes[0] : 0), reply_bytes(), packed[p], bytes[p], bytes[p], (size_t)replies,
+                                 cudaMemcpyDeviceToDevice, s));
+        }
+        return HECUDA_OK;
+    }
+};
+
+struct DrainOnExit {  // every return path after the caller's buffers are in flight on `s` waits for the stream
+    cudaStream_t s;
+    ~DrainOnExit() { wait_stream(s); }
+};
+
 
 // ---------------------------------------------------------------- captured response pipelines
 // One query is ~100 small launches (level-by-level expansion, first-dimension scan, ct x ct folding, modulus switches);
@@ -996,34 +1044,24 @@ int32_t hecuda_mulpir_compute_response_wire(const hecuda_context *h, const hecud
                                      query_ct_count, indices_count, out, shape);
     if (rc) return rc;
     if (!query_seeds) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    WireCodec wc;
+    if ((rc = wc.setup(*h->ctx, skip_lsbs_poly0, skip_lsbs_poly1))) return rc;
     const Context &c = *h->ctx;
-    CodecConsts in_codec, out_codec[2];
-    std::string err;
-    if (!codec_consts(c, c.map_q(c.L), 0, in_codec, err) || !codec_consts(c, c.map_q(1), skip_lsbs_poly0, out_codec[0], err) ||
-        !codec_consts(c, c.map_q(1), skip_lsbs_poly1, out_codec[1], err))
-        return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
     WsGuard g(h);
     if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
     cudaStream_t s = g.w->stream;
     StreamBuffers tmp(s);
-    const size_t ct_words = (size_t)2 * c.L * c.n, in_bytes = (size_t)serialized_poly_bytes(in_codec);
+    const size_t ct_words = (size_t)2 * c.L * c.n, in_bytes = wc.query_bytes;
     const int64_t replies = (int64_t)indices_count * chunk_count;
-    const size_t b0 = (size_t)serialized_poly_bytes(out_codec[0]), b1 = (size_t)serialized_poly_bytes(out_codec[1]);
-    unsigned char *d_poly0 = nullptr, *d_seeds = nullptr, *d_bytes[2] = {nullptr, nullptr}, *d_reply = nullptr;
-    u64 *d_query = nullptr, *d_resp = nullptr, *d_polys = nullptr;
+    unsigned char *d_poly0 = nullptr, *d_seeds = nullptr;
+    u64 *d_query = nullptr, *d_resp = nullptr;
     CK(tmp.alloc_bytes((void **)&d_poly0, in_bytes * query_ct_count));
     CK(tmp.alloc_bytes((void **)&d_seeds, (size_t)32 * query_ct_count));
     CK(tmp.alloc(&d_query, ct_words * query_ct_count));
     CK(tmp.alloc(&d_resp, (size_t)2 * c.n * replies));
-    CK(tmp.alloc(&d_polys, (size_t)2 * c.n * replies));
-    CK(tmp.alloc_bytes((void **)&d_bytes[0], ((b0 + 7) & ~(size_t)7) * replies + 8));
-    CK(tmp.alloc_bytes((void **)&d_bytes[1], ((b1 + 7) & ~(size_t)7) * replies + 8));
-    CK(tmp.alloc_bytes((void **)&d_reply, (b0 + b1) * replies));
+    CK(wc.alloc(tmp, c, replies));
     // from here on copies of the caller's buffers are in flight on `s`: every return path waits for the stream first
-    struct DrainOnExit {
-        cudaStream_t s;
-        ~DrainOnExit() { wait_stream(s); }
-    } drain{s};
+    DrainOnExit drain{s};
     CK(cudaMemcpyAsync(d_poly0, query_poly0, in_bytes * query_ct_count, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d_seeds, query_seeds, (size_t)32 * query_ct_count, cudaMemcpyHostToDevice, s));
     // Query.ciphertexts arrive as SerializedCiphertext.seeded (SerializedCiphertext.swift:41-49)
@@ -1031,19 +1069,55 @@ int32_t hecuda_mulpir_compute_response_wire(const hecuda_context *h, const hecud
     if (e != cudaSuccess) return cuda_fail(e, "expand seeded query");
     rc = compute_response_device(h, k, dbs, db_count, shape, d_query, query_ct_count, indices_count, d_resp, s);
     if (rc) return rc;
-    // Response ciphertexts leave as .full(polys:skipLSBs:) with Bfv.skipLSBsForDecryption (Bfv+Decrypt.swift:51-110):
-    // poly 0 and poly 1 are packed with different numbers of dropped low bits
-    const size_t pw = (size_t)c.n * sizeof(u64);
-    for (int p = 0; p < 2; ++p) {
-        const size_t bytes = p ? b1 : b0;
-        CK(cudaMemcpy2DAsync(d_polys + (size_t)p * c.n * replies, pw, d_resp + (size_t)p * c.n, 2 * pw, pw, (size_t)replies,
-                             cudaMemcpyDeviceToDevice, s));
-        if ((e = launch_poly_serialize(c, out_codec[p], p ? skip_lsbs_poly1 : skip_lsbs_poly0, d_polys + (size_t)p * c.n * replies,
-                                       d_bytes[p], replies, s)) != cudaSuccess)
-            return cuda_fail(e, "serialize response");
-        CK(cudaMemcpy2DAsync(d_reply + (p ? b0 : 0), b0 + b1, d_bytes[p], bytes, bytes, (size_t)replies, cudaMemcpyDeviceToDevice, s));
+    if ((rc = wc.pack(c, d_resp, replies, s))) return rc;
+    CK(cudaMemcpyAsync(out, wc.reply, wc.reply_bytes() * replies, cudaMemcpyDeviceToHost, s));
+    CK(wait_stream(s));
+    return HECUDA_OK;
+}
+
+int32_t hecuda_mulpir_compute_response_clients_wire(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count,
+                                                    const hecuda_pir_database *const *dbs, int32_t db_count, const int32_t *dims,
+                                                    int32_t dim_count, int32_t chunk_count, const uint8_t *query_poly0,
+                                                    const uint8_t *query_seeds, int32_t query_ct_count, int32_t indices_count,
+                                                    int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1, uint8_t *out) {
+    ResponseShape shape;
+    int32_t rc = check_clients_args(h, evks, client_count, dbs, db_count, dims, dim_count, chunk_count,
+                                    (const uint64_t *)query_poly0, query_ct_count, indices_count, out, shape);
+    if (rc) return rc;
+    if (!query_seeds) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    WireCodec wc;
+    if ((rc = wc.setup(*h->ctx, skip_lsbs_poly0, skip_lsbs_poly1))) return rc;
+    const Context &c = *h->ctx;
+    WsGuard g(h);
+    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    cudaStream_t s = g.w->stream;
+    StreamBuffers tmp(s);
+    const int group = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count);
+    const size_t ct_words = (size_t)2 * c.L * c.n, poly0_bytes = wc.query_bytes * query_ct_count, seed_bytes = (size_t)32 * query_ct_count;
+    const int64_t replies = (int64_t)indices_count * chunk_count;  // per client
+    const size_t out_bytes = wc.reply_bytes() * replies;
+    unsigned char *d_poly0 = nullptr, *d_seeds = nullptr;
+    u64 *d_query = nullptr, *d_resp = nullptr;
+    CK(tmp.alloc_bytes((void **)&d_poly0, poly0_bytes * group));
+    CK(tmp.alloc_bytes((void **)&d_seeds, seed_bytes * group));
+    CK(tmp.alloc(&d_query, ct_words * query_ct_count * group));
+    CK(tmp.alloc(&d_resp, (size_t)2 * c.n * replies * group));
+    CK(wc.alloc(tmp, c, replies * group));
+    DrainOnExit drain{s};  // copies of the caller's buffers are in flight on `s` from here on
+    for (int32_t first = 0; first < client_count; first += group) {
+        const int clients = std::min<int32_t>(group, client_count - first);
+        CK(cudaMemcpyAsync(d_poly0, query_poly0 + poly0_bytes * first, poly0_bytes * clients, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_seeds, query_seeds + seed_bytes * first, seed_bytes * clients, cudaMemcpyHostToDevice, s));
+        // every query ciphertext of the group in one expansion
+        cudaError_t e = expand_seeded_device(c, c.L, d_poly0, d_seeds, d_query, (int64_t)query_ct_count * clients, s);
+        if (e != cudaSuccess) return cuda_fail(e, "expand seeded query");
+        rc = compute_response_clients_device(h, evks + first, clients, first, dbs, db_count, shape, d_query, query_ct_count,
+                                             indices_count, d_resp, s);
+        if (rc) return rc;
+        // the group's replies are client-major, like `out`: one packing pass per reply poly
+        if ((rc = wc.pack(c, d_resp, replies * clients, s))) return rc;
+        CK(cudaMemcpyAsync(out + out_bytes * first, wc.reply, out_bytes * clients, cudaMemcpyDeviceToHost, s));
     }
-    CK(cudaMemcpyAsync(out, d_reply, (b0 + b1) * replies, cudaMemcpyDeviceToHost, s));
     CK(wait_stream(s));
     return HECUDA_OK;
 }

@@ -85,6 +85,7 @@ SYMBOLS = {
     "hecuda_bfv_mod_switch_down_device": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int32, _VP, C.c_int64, _VP]),
     "hecuda_evk_set_galois_key": (C.c_int32, [_VP, C.c_uint32, _VP]),
     "hecuda_evk_galois_device_buffer": (C.c_int32, [_VP, C.c_uint32, C.POINTER(_VP), C.POINTER(C.c_uint64)]),
+    "hecuda_evk_create_serialized": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int32, _VP, _VP, C.POINTER(_VP)]),
     "hecuda_bfv_apply_galois": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_uint32, _VP, C.c_int64]),
     "hecuda_bfv_apply_galois_device": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_uint32, _VP, C.c_int64, _VP]),
     "hecuda_poly_apply_galois": (C.c_int32, [_VP, C.c_int32, C.c_int32, _VP, _VP, C.c_int32, C.c_int64, C.c_uint32]),
@@ -113,6 +114,9 @@ SYMBOLS = {
                                                                   C.c_int32, _VP, _VP]),
     "hecuda_mulpir_compute_response_wire": (C.c_int32, [_VP, _VP, C.POINTER(_VP), C.c_int32, C.POINTER(C.c_int32), C.c_int32,
                                                         C.c_int32, _VP, _VP, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _VP]),
+    "hecuda_mulpir_compute_response_clients_wire": (C.c_int32, [_VP, C.POINTER(_VP), C.c_int32, C.POINTER(_VP), C.c_int32,
+                                                                C.POINTER(C.c_int32), C.c_int32, C.c_int32, _VP, _VP, C.c_int32,
+                                                                C.c_int32, C.c_int32, C.c_int32, _VP]),
     "hecuda_pnns_matrix_create": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.POINTER(_VP)]),
     "hecuda_pnns_matrix_destroy": (C.c_int32, [_VP]),
     "hecuda_pnns_matrix_result_count": (C.c_int32, [_VP, C.POINTER(C.c_int64)]),
@@ -355,6 +359,43 @@ class EvaluationKey:
                 raise HeError(-1, "invalidContext: relinearization key must be L x 2 x (L+1) x N")
             _check(load_library().hecuda_evk_create(context._h, _ptr(key), C.byref(h)))
         self._h = h
+
+    @classmethod
+    def fromSerialized(cls, context: Context, relinPoly0=None, relinSeeds=None, galois=None) -> "EvaluationKey":
+        """EvaluationKey(deserialize:context:) (SerializedKeys.swift:141-157) with every key ciphertext .seeded: the seeds
+        are expanded and poly0 unpacked on the device (hecuda_evk_create_serialized).  relinPoly0: (L, B) uint8 and
+        relinSeeds: (L, 32) uint8, B = Bfv.serializationByteCount(context, L + 1, base=BASE_KEYSWITCH), or both None;
+        galois: {element: (poly0 (L, B) uint8, seeds (L, 32) uint8)}."""
+        L = context.L
+        size = Bfv.serializationByteCount(context, L + 1, base=BASE_KEYSWITCH)
+
+        def arrays(poly0, seeds):
+            p = np.ascontiguousarray(np.asarray(poly0, dtype=np.uint8))
+            s = np.ascontiguousarray(np.asarray(seeds, dtype=np.uint8))
+            if p.size != L * size or s.size != L * 32:
+                raise HeError(-1, f"serializedBufferSizeMismatch(poly0: {p.size} bytes, seeds: {s.size} bytes, expected "
+                                  f"{L * size} and {L * 32})")
+            return p, s
+
+        relin = None
+        if relinPoly0 is not None or relinSeeds is not None:
+            if relinPoly0 is None or relinSeeds is None:
+                raise HeError(-1, "relinPoly0 and relinSeeds must both be given or both be None")
+            relin = arrays(relinPoly0, relinSeeds)
+        galois = dict(galois or {})
+        elements = [int(e) for e in galois]
+        keys = [arrays(*galois[e]) for e in galois]
+        elems = np.ascontiguousarray(elements, dtype=np.uint32)
+        gp = np.ascontiguousarray(np.concatenate([k[0].reshape(-1) for k in keys])) if keys else None
+        gs = np.ascontiguousarray(np.concatenate([k[1].reshape(-1) for k in keys])) if keys else None
+        h = C.c_void_p()
+        _check(load_library().hecuda_evk_create_serialized(
+            context._h, _ptr(relin[0]) if relin else None, _ptr(relin[1]) if relin else None,
+            _ptr(elems) if elements else None, len(elements), _ptr(gp) if keys else None, _ptr(gs) if keys else None,
+            C.byref(h)))
+        key = cls.__new__(cls)
+        key.context, key.galoisElements, key._h = context, elements, h
+        return key
 
     def setGaloisKey(self, element: int, key):
         """GaloisKey.keys[element] (Keys.swift:150-163): (L, 2, L+1, N) uint64, Eval format."""

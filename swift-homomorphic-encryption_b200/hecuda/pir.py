@@ -292,6 +292,37 @@ class PirWire:
             out.ctypes.data_as(C.c_void_p)))
         return out, skips
 
+    @staticmethod
+    def computeResponses(server: "MulPirServer", queryPoly0, querySeeds, evaluationKeys: Sequence[EvaluationKey],
+                         indicesCount: int = 1):
+        """computeResponse for many clients in one C-ABI call (hecuda_mulpir_compute_response_clients_wire): client c's
+        serialized seeded query with evaluationKeys[c], its reply bytes identical to
+        `computeResponse(server, queryPoly0[c], querySeeds[c], evaluationKeys[c], indicesCount)`.
+        queryPoly0: (clients, count, byteCount(L rows)) uint8; querySeeds: (clients, count, 32) uint8.  Returns
+        (replies, skipLSBs) with replies of shape (clients, indicesCount, chunkCount, bytes(poly0) + bytes(poly1))."""
+        from . import Bfv
+        ctx = server.context
+        keys = list(evaluationKeys)
+        seeds = np.ascontiguousarray(np.asarray(querySeeds, dtype=np.uint8))
+        poly0 = np.ascontiguousarray(np.asarray(queryPoly0, dtype=np.uint8))
+        size = Bfv.serializationByteCount(ctx, ctx.L)
+        if not keys or seeds.size % (32 * len(keys)):
+            raise HeError(-1, "serializedBufferSizeMismatch: querySeeds must be one set of 32-byte seeds per evaluation key")
+        count = seeds.size // (32 * len(keys))
+        if poly0.size != len(keys) * count * size:
+            raise HeError(-1, f"serializedBufferSizeMismatch(poly0: {poly0.size} bytes, expected {len(keys) * count * size})")
+        skips = skipLSBsForDecryption(ctx)
+        sizes = [Bfv.serializationByteCount(ctx, 1, s) for s in skips]
+        out = np.empty((len(keys), indicesCount, server.chunkCount, sum(sizes)), dtype=np.uint8)
+        handles = (C.c_void_p * len(server.databases))(*[db._h for db in server.databases])
+        key_handles = (C.c_void_p * len(keys))(*[k._h for k in keys])
+        dims = (C.c_int32 * len(server.parameter.dimensions))(*server.parameter.dimensions)
+        _check(load_library().hecuda_mulpir_compute_response_clients_wire(
+            ctx._h, key_handles, len(keys), handles, len(server.databases), dims, len(server.parameter.dimensions),
+            server.chunkCount, poly0.ctypes.data_as(C.c_void_p), seeds.ctypes.data_as(C.c_void_p), count, indicesCount,
+            skips[0], skips[1], out.ctypes.data_as(C.c_void_p)))
+        return out, skips
+
 
 class PirUtil:
     """enum PirUtil<Bfv<UInt64>> (PirUtil.swift:573): expansion and response computation on the device."""

@@ -118,6 +118,28 @@ class EvaluationKey {
             throw HeError(HeError::invalidContext, "Galois key must be L x 2 x (L+1) x N");
         check(hecuda_evk_set_galois_key(handle_, element, key.data()));
     }
+    // EvaluationKey(deserialize:context:) (SerializedKeys.swift:141-157) with every key ciphertext
+    // .seeded(poly0:seed:): relinPoly0 L x B bytes and relinSeeds L x 32 (both empty: no relinearization key), B =
+    // hecuda_poly_serialized_byte_count(BASE_KEYSWITCH, L+1 rows, skipLSBs 0); galoisPoly0 / galoisSeeds hold the same
+    // for each of `elements`, in that order.  The seeds are expanded and poly0 unpacked on the device.
+    static std::unique_ptr<EvaluationKey> deserialize(std::shared_ptr<const Context> c, const std::vector<uint8_t> &relinPoly0,
+                                                      const std::vector<uint8_t> &relinSeeds,
+                                                      const std::vector<uint32_t> &elements,
+                                                      const std::vector<uint8_t> &galoisPoly0,
+                                                      const std::vector<uint8_t> &galoisSeeds) {
+        const size_t L = c->ciphertextModuliCount();
+        uint64_t bytes = 0;
+        check(hecuda_poly_serialized_byte_count(c->handle(), HECUDA_BASE_KEYSWITCH, (int32_t)L + 1, 0, &bytes));
+        const bool relin = !relinPoly0.empty() || !relinSeeds.empty();
+        if (relin && (relinPoly0.size() != L * bytes || relinSeeds.size() != L * 32))
+            throw HeError(HeError::invalidContext, "serializedBufferSizeMismatch: relinearization key must be L x B and L x 32 bytes");
+        if (galoisPoly0.size() != elements.size() * L * bytes || galoisSeeds.size() != elements.size() * L * 32)
+            throw HeError(HeError::invalidContext, "serializedBufferSizeMismatch: Galois keys must be L x B and L x 32 bytes each");
+        hecuda_evk *h = nullptr;
+        check(hecuda_evk_create_serialized(c->handle(), relin ? relinPoly0.data() : nullptr, relin ? relinSeeds.data() : nullptr,
+                                           elements.data(), (int32_t)elements.size(), galoisPoly0.data(), galoisSeeds.data(), &h));
+        return std::unique_ptr<EvaluationKey>(new EvaluationKey(std::move(c), h));
+    }
     ~EvaluationKey() { hecuda_evk_destroy(handle_); }
     EvaluationKey(const EvaluationKey &) = delete;
     EvaluationKey &operator=(const EvaluationKey &) = delete;
@@ -125,6 +147,7 @@ class EvaluationKey {
     hecuda_evk *handle() const { return handle_; }
 
    private:
+    EvaluationKey(std::shared_ptr<const Context> c, hecuda_evk *h) : context(std::move(c)), handle_(h) {}
     hecuda_evk *handle_ = nullptr;
 };
 
