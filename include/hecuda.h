@@ -310,7 +310,10 @@ int32_t hecuda_pir_database_device_buffer(hecuda_pir_database *db, void **device
  * expandCiphertextForOneStep :204-236).  ciphertexts: ciphertext_count x 2 x L x N (Coeff); out: output_count x 2 x L x N,
  * output i encrypting the constant polynomial whose constant is coefficient i of the inputs (x 2^ceilLog2(count)).
  * The Galois keys come from `evk` (hecuda_evk_set_galois_key); the largest configured element <= 2^(logN-logStep+1)+1
- * is applied repeatedly, HECUDA_ERR_MISSING_KEY if none fits (HeError.missingGaloisKey, :216-220). */
+ * is applied repeatedly, HECUDA_ERR_MISSING_KEY if none fits (HeError.missingGaloisKey, :216-220).
+ * The MulPir _device variants (here and below) take device buffers and only enqueue on `stream`.  The first MulPir call
+ * with a new query shape uploads that shape's expansion plan to the context once, synchronously: make one call with a
+ * shape before capturing calls with it into a graph. */
 int32_t hecuda_mulpir_expand(const hecuda_context *ctx, const hecuda_evk *evk, const uint64_t *ciphertexts,
                              int32_t ciphertext_count, int64_t output_count, uint64_t *out);
 int32_t hecuda_mulpir_expand_device(const hecuda_context *ctx, const hecuda_evk *evk, const uint64_t *ciphertexts,
@@ -340,13 +343,12 @@ int32_t hecuda_mulpir_compute_response_device(const hecuda_context *ctx, const h
  * queries + c * query_ciphertext_count * 2 * L * N and its reply (bit-identical to what hecuda_mulpir_compute_response
  * returns for that client alone) is out + c * indices_count * chunk_count * 2 * N, so out is
  * client_count x indices_count x chunk_count x 2 x 1 x N.  Clients are processed in groups of at most
- * HECUDA_MULPIR_CLIENT_GROUP; every stage is one pass over a group (its launch count does not depend on the group's
- * size), the first-dimension scan streams each database once per group, and temporaries scale with the group, not
- * with client_count.  Every client is checked like a single call (a failure's message names the client).  At every
- * expansion level all clients' Galois keys must resolve to the same element, as keys generated for the same
- * IndexPirParameter do; HECUDA_ERR_INVALID_ARGUMENT otherwise (answer such a client with the single-client call).
- * The _device variant takes device buffers and only enqueues on `stream`; the first call with a new query shape
- * uploads that shape's expansion plan to the context once, synchronously. */
+ * HECUDA_MULPIR_CLIENT_GROUP; every stage is one pass over a group (from two clients up, its launch count does not
+ * depend on the group's size), the first-dimension scan streams each database once per group, and temporaries scale
+ * with the group, not with client_count.  A group of one client runs the kernels of hecuda_mulpir_compute_response.
+ * Every client is checked like a single call (a failure's message names the client).  At every expansion level all
+ * clients' Galois keys must resolve to the same element, as keys generated for the same IndexPirParameter do;
+ * HECUDA_ERR_INVALID_ARGUMENT otherwise (answer such a client with the single-client call). */
 #define HECUDA_MULPIR_CLIENT_GROUP 16
 int32_t hecuda_mulpir_compute_response_clients(const hecuda_context *ctx, const hecuda_evk *const *evks, int32_t client_count,
                                                const hecuda_pir_database *const *databases, int32_t database_count,

@@ -385,6 +385,9 @@ cudaError_t launch_inner_product_plain_clients(const Context &ctx, const u64 *ct
     if (clients < 1 || clients > kScanClientTile * kScanClientTiles || l < 1 || l > ctx.L || ctx.n < 2 ||
         (pts32 != nullptr) == (pts != nullptr) || (pts32 && !inner_product_plain_small_supported(ctx, l)))
         return cudaErrorInvalidValue;
+    if (clients == 1)  // a lone client: the single-client scans (same layout), not a tile of four clients' work
+        return pts32 ? launch_inner_product_plain_small(ctx, cts, 2, l, terms, pts32, present, out, out_count, stream)
+                     : launch_inner_product_plain(ctx, cts, 2, l, terms, pts, present, out, out_count, stream);
     const IpSmallConsts cs = pts32 ? ip_small_consts(ctx, l) : IpSmallConsts{};
     const IpConsts cw = pts32 ? IpConsts{} : ip_consts(ctx, l);
     if (pts32 && cs.max_terms < 1) return cudaErrorInvalidValue;

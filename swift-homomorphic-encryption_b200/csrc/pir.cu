@@ -11,8 +11,9 @@
 // leaves (doubled where the reference adds the ciphertext to itself) straight to their final, interleaved position.
 // The first dimension is one streaming pass over the device-resident plaintext database
 // (inner_product_plain_kernel), further dimensions are lazy ct x ct inner products + relinearization.
-// Everything is enqueued on one stream; concurrent queries (different clients, different keys) run on different
-// streams from different host threads.
+// One pipeline (respond_group) answers every call: a group of up to HECUDA_MULPIR_CLIENT_GROUP clients goes through
+// each stage in one pass, each client with its own keys, and a group of one runs the single-client kernels.
+// Everything is enqueued on one stream; concurrent calls run on different streams from different host threads.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -244,14 +245,41 @@ int32_t resolve_level_keys(const hecuda_evk *const *keys, int clients, int first
     return HECUDA_OK;
 }
 
+// The expansion plan of a query shape on the device, uploaded the first time the context sees the shape, so that
+// later calls enqueue without waiting for a copy.  The upload runs outside the context's lock; when two threads race
+// on a new shape, the second copy is dropped.
+int32_t expand_steps_on_device(const hecuda_context *hc, int64_t n, int64_t ct_count, int64_t output_count, const ExpandStep **out) {
+    hecuda_context *h = const_cast<hecuda_context *>(hc);
+    const std::pair<int64_t, int64_t> shape{ct_count, output_count};
+    {
+        std::lock_guard<std::mutex> lock(h->mu);
+        auto it = h->expand_steps.find(shape);
+        if (it != h->expand_steps.end()) {
+            *out = (const ExpandStep *)it->second;
+            return HECUDA_OK;
+        }
+    }
+    const ExpandPlan plan = build_expand_plan(n, ct_count, output_count);
+    void *d = nullptr;
+    cudaError_t e = cudaMalloc(&d, std::max<size_t>(plan.steps.size(), 1) * sizeof(ExpandStep));
+    if (e == cudaSuccess && !plan.steps.empty()) e = upload(d, plan.steps.data(), plan.steps.size() * sizeof(ExpandStep));
+    if (e != cudaSuccess) {
+        if (d) cudaFree(d);
+        return cuda_fail(e, "expansion plan upload");
+    }
+    std::lock_guard<std::mutex> lock(h->mu);
+    auto ins = h->expand_steps.insert({shape, d});
+    if (!ins.second) cudaFree(d);  // another thread uploaded the same plan first; nothing has used this copy
+    *out = (const ExpandStep *)ins.first->second;
+    return HECUDA_OK;
+}
+
 // PirUtil.expand on device buffers for `clients` queries of the same shape: client j's ct_count canonical (Coeff)
 // ciphertexts of L rows at d_in + j * ct_count ciphertexts, its output_count outputs at d_out + j * output_count,
 // expanded with keys[j].  Every stage is one pass over all clients.
-// d_steps_ready: the plan's steps already on the device (captured graphs upload them once, outside the capture)
 // first_client: the call-wide index of keys[0] for error messages (resolve_level_keys)
 int32_t expand_device(const hecuda_context *h, const hecuda_evk *const *keys, int clients, const u64 *d_in, int64_t ct_count,
-                      int64_t output_count, u64 *d_out, cudaStream_t s, const void *d_steps_ready = nullptr,
-                      int first_client = -1) {
+                      int64_t output_count, u64 *d_out, cudaStream_t s, int first_client = -1) {
     const Context &c = *h->ctx;
     const int l = c.L;
     const int64_t n = c.n;
@@ -262,6 +290,8 @@ int32_t expand_device(const hecuda_context *h, const hecuda_evk *const *keys, in
     int32_t rc_keys = resolve_level_keys(keys, clients, first_client, n, plan, level_keys);
     if (rc_keys) return rc_keys;
     if (clients > kKeyTableSize) return fail(HECUDA_ERR_UNSUPPORTED, "expand: more clients than one key table holds");
+    const ExpandStep *d_steps = nullptr;
+    if ((rc_keys = expand_steps_on_device(h, n, ct_count, output_count, &d_steps))) return rc_keys;
     std::vector<KsKeyTable> tables(plan.levels.size(), KsKeyTable{});
     for (size_t li = 0; li < plan.levels.size(); ++li) {
         tables[li].items_per_client = plan.levels[li].nodes;
@@ -274,7 +304,6 @@ int32_t expand_device(const hecuda_context *h, const hecuda_evk *const *keys, in
     if (plan.levels.empty()) return HECUDA_OK;
     StreamBuffers tmp(s);
     u64 *level_buf[2] = {nullptr, nullptr}, *c1_buf[2] = {nullptr, nullptr}, *scratch = nullptr;
-    ExpandStep *d_steps = nullptr;
     // items per applyGalois pass: grows with the number of clients, so the launch count does not
     const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, plan.max_nodes)) * clients;
     const size_t level_words = ct_words * plan.max_nodes * clients;
@@ -283,13 +312,6 @@ int32_t expand_device(const hecuda_context *h, const hecuda_evk *const *keys, in
     CK(tmp.alloc(&c1_buf[0], level_words));
     CK(tmp.alloc(&c1_buf[1], level_words));
     CK(tmp.alloc(&scratch, galois_scratch_words(c, l) * (size_t)chunk));
-    if (d_steps_ready) {
-        d_steps = (ExpandStep *)d_steps_ready;
-    } else {
-        CK(tmp.alloc_bytes((void **)&d_steps, plan.steps.size() * sizeof(ExpandStep)));
-        CK(cudaMemcpyAsync(d_steps, plan.steps.data(), plan.steps.size() * sizeof(ExpandStep), cudaMemcpyHostToDevice, s));
-        CK(wait_stream(s));  // plan.steps is a pageable temporary
-    }
     const RowConsts rc = row_consts(c, l);
     const int threads = n >= 256 ? 256 : (n < 32 ? 32 : (int)n);
     // the active roots are a prefix of each input (only the last one can be a single output); a level's nodes must be
@@ -355,86 +377,6 @@ struct ResponseShape {
     int64_t chunk_count, per_chunk, columns, expanded_query_count;
 };
 
-// PirUtil.computeResponse (PirUtil.swift:490-568) for device-resident query ciphertexts; d_out receives
-// indices_count x chunk_count ciphertexts of 2 x 1 x N (Coeff, one modulus)
-int32_t compute_response_device(const hecuda_context *h, const hecuda_evk *k, const hecuda_pir_database *const *dbs,
-                                int32_t db_count, const ResponseShape &shape, const u64 *d_query, int64_t query_ct_count,
-                                int64_t indices_count, u64 *d_out, cudaStream_t s, const void *d_steps_ready = nullptr) {
-    const Context &c = *h->ctx;
-    const int L = c.L;
-    const int64_t n = c.n;
-    const size_t ct_words = (size_t)2 * L * n;
-    const int64_t eqc = shape.expanded_query_count, dim0 = shape.dims[0];
-    const int64_t rows = shape.chunk_count * shape.columns;  // first-dimension inner products per query
-    StreamBuffers tmp(s);
-    u64 *expanded = nullptr, *first_eval = nullptr, *results[2] = {nullptr, nullptr}, *lhs = nullptr, *ct3 = nullptr,
-        *scratch = nullptr;
-    CK(tmp.alloc(&expanded, ct_words * eqc * indices_count));
-    int32_t rc = expand_device(h, &k, 1, d_query, query_ct_count, eqc * indices_count, expanded, s, d_steps_ready);
-    if (rc) return rc;
-    CK(tmp.alloc(&first_eval, ct_words * dim0));
-    CK(tmp.alloc(&results[0], ct_words * rows));
-    CK(tmp.alloc(&results[1], ct_words * rows));
-    size_t scratch_words = 0, lhs_words = 0, ct3_words = 0;
-    {
-        int64_t count = rows;
-        for (size_t d = 1; d < shape.dims.size(); ++d) {
-            const int64_t size = shape.dims[d], groups = count / size;
-            scratch_words = std::max(scratch_words, inner_product_scratch_words(c, size) * (size_t)groups);
-            scratch_words = std::max(scratch_words, relinearize_scratch_words(c, L) * (size_t)groups);
-            lhs_words = std::max(lhs_words, ct_words * (size_t)(size * groups));
-            ct3_words = std::max(ct3_words, (size_t)3 * L * n * groups);
-            count = groups;
-        }
-    }
-    CK(tmp.alloc(&scratch, scratch_words));
-    CK(tmp.alloc(&lhs, lhs_words));
-    CK(tmp.alloc(&ct3, ct3_words));
-    const NttRowMap map = c.map_q(L);
-    for (int64_t qi = 0; qi < indices_count; ++qi) {
-        const u64 *cts = expanded + ct_words * eqc * qi;
-        const hecuda_pir_database *db = dbs[db_count == 1 ? 0 : qi];
-        cudaError_t e;
-        // firstDimensionQueries: convertToEvalFormat (:523-532)
-        if ((e = launch_ntt_forward(c, map, cts, first_eval, dim0 * 2 * L, s)) != cudaSuccess) return cuda_fail(e, "ntt");
-        // every column of every chunk: Scheme.innerProduct(ciphertexts:plaintexts:) then convertToCanonicalFormat (:427-435)
-        e = db->d_plain32 ? launch_inner_product_plain_small(c, first_eval, 2, L, dim0, db->d_plain32, db->d_present, results[0], rows, s)
-                          : launch_inner_product_plain(c, first_eval, 2, L, dim0, db->d_plain, db->d_present, results[0], rows, s);
-        if (e != cudaSuccess)
-            return cuda_fail(e, "innerProduct(ciphertexts:plaintexts:)");
-        if ((e = launch_ntt_inverse(c, map, results[0], results[0], rows * 2 * L, kScalePlain, s)) != cudaSuccess)
-            return cuda_fail(e, "ntt");
-        int64_t count = rows, query_start = dim0;
-        int cur = 0;
-        for (size_t d = 1; d < shape.dims.size(); ++d) {  // remaining dimensions (:447-480)
-            const int64_t size = shape.dims[d], groups = count / size;
-            for (int64_t g = 0; g < groups; ++g)  // vector0 = the same query slice for every group
-                CK(cudaMemcpyAsync(lhs + ct_words * size * g, cts + ct_words * query_start, ct_words * size * sizeof(u64),
-                                   cudaMemcpyDeviceToDevice, s));
-            if ((e = inner_product_chunk(c, scratch, lhs, results[cur], size, ct3, groups, s)) != cudaSuccess)
-                return cuda_fail(e, "innerProduct");
-            if ((e = relinearize_chunk(c, scratch, k->d_relin, ct3, L, results[cur ^ 1], groups, s)) != cudaSuccess)
-                return cuda_fail(e, "relinearize");
-            cur ^= 1;
-            count = groups;
-            query_start += size;
-        }
-        if (count != shape.chunk_count)
-            return fail(HECUDA_ERR_INVALID_ARGUMENT, "There should be only 1 ciphertext in the final result for each chunk");
-        // modSwitchDownToSingle (HeScheme.swift:1481-1485); BFV's canonical format is already Coeff
-        u64 *final_out = d_out + (size_t)2 * n * shape.chunk_count * qi;
-        if (L == 1) {
-            CK(cudaMemcpyAsync(final_out, results[cur], (size_t)2 * n * count * sizeof(u64), cudaMemcpyDeviceToDevice, s));
-        }
-        for (int l = L; l > 1; --l) {
-            u64 *dst = l == 2 ? final_out : results[cur ^ 1];
-            if ((e = launch_mod_switch(c, results[cur], l, dst, count * 2, s)) != cudaSuccess) return cuda_fail(e, "modSwitchDown");
-            cur ^= 1;
-        }
-    }
-    return HECUDA_OK;
-}
-
 int32_t check_response_args(const hecuda_context *h, const hecuda_evk *k, const hecuda_pir_database *const *dbs,
                             int32_t db_count, const int32_t *dims, int32_t dim_count, int32_t chunk_count,
                             const uint64_t *query, int32_t query_ct_count, int32_t indices_count, const void *out,
@@ -495,67 +437,41 @@ int32_t check_clients_args(const hecuda_context *h, const hecuda_evk *const *evk
     return resolve_level_keys(evks, client_count, 0, h->ctx->n, plan, level_keys);
 }
 
-// The expansion plan of a query shape on the device, uploaded the first time the context sees the shape, so that
-// later calls enqueue without waiting for a copy.  The upload runs outside the context's lock; when two threads race
-// on a new shape, the second copy is dropped.
-int32_t expand_steps_on_device(const hecuda_context *hc, int64_t n, int64_t ct_count, int64_t output_count, const void **out) {
-    hecuda_context *h = const_cast<hecuda_context *>(hc);
-    const std::pair<int64_t, int64_t> shape{ct_count, output_count};
-    {
-        std::lock_guard<std::mutex> lock(h->mu);
-        auto it = h->expand_steps.find(shape);
-        if (it != h->expand_steps.end()) {
-            *out = it->second;
-            return HECUDA_OK;
-        }
-    }
-    const ExpandPlan plan = build_expand_plan(n, ct_count, output_count);
-    void *d = nullptr;
-    cudaError_t e = cudaMalloc(&d, std::max<size_t>(plan.steps.size(), 1) * sizeof(ExpandStep));
-    if (e == cudaSuccess && !plan.steps.empty()) e = upload(d, plan.steps.data(), plan.steps.size() * sizeof(ExpandStep));
-    if (e != cudaSuccess) {
-        if (d) cudaFree(d);
-        return cuda_fail(e, "expansion plan upload");
-    }
-    std::lock_guard<std::mutex> lock(h->mu);
-    auto ins = h->expand_steps.insert({shape, d});
-    if (!ins.second) cudaFree(d);  // another thread uploaded the same plan first; nothing has used this copy
-    *out = ins.first->second;
-    return HECUDA_OK;
-}
-
-// PirUtil.computeResponse for `clients` (<= HECUDA_MULPIR_CLIENT_GROUP) queries of the same shape, client j with
-// keys[j]: d_query = clients x query_ct_count ciphertexts, d_out = clients x indices_count x chunk_count x 2 x 1 x N.
-// Each stage is one pass over all clients; the first dimension streams every database once for the whole group.
-// first_client: the call-wide index of keys[0] (the keys were resolved by check_clients_args).
-int32_t compute_response_clients_device(const hecuda_context *h, const hecuda_evk *const *keys, int clients,
-                                        int first_client, const hecuda_pir_database *const *dbs, int32_t db_count,
-                                        const ResponseShape &shape, const u64 *d_query, int64_t query_ct_count,
-                                        int64_t indices_count, u64 *d_out, cudaStream_t s) {
+// PirUtil.computeResponse (PirUtil.swift:490-568) for `clients` (<= HECUDA_MULPIR_CLIENT_GROUP) queries of the same
+// shape, client j with keys[j]: d_query = clients x query_ct_count ciphertexts (Coeff), d_out = clients x indices_count x
+// chunk_count ciphertexts of 2 x 1 x N (Coeff, one modulus).  Each stage is one pass over all clients; the first
+// dimension streams every database once for the whole group.  A group of one keeps the single-client kernels: its
+// forward NTT covers only the first-dimension slice of each index, the scan is the single-client scan, and the
+// relinearization reads one key instead of a key table.
+// first_client: the call-wide index of keys[0] (the keys were resolved by check_clients_args); < 0 for a single-client
+// call, whose errors name no client.
+int32_t respond_group(const hecuda_context *h, const hecuda_evk *const *keys, int clients, int first_client,
+                      const hecuda_pir_database *const *dbs, int32_t db_count, const ResponseShape &shape, const u64 *d_query,
+                      int64_t query_ct_count, int64_t indices_count, u64 *d_out, cudaStream_t s) {
     const Context &c = *h->ctx;
     const int L = c.L;
     const int64_t n = c.n;
     const size_t ct_words = (size_t)2 * L * n, reply_words = (size_t)2 * n * shape.chunk_count;
     const int64_t eqc = shape.expanded_query_count, dim0 = shape.dims[0];
-    const int64_t rows = shape.chunk_count * shape.columns;
-    const int64_t client_cts = eqc * indices_count;  // expanded ciphertexts per client
-    const void *d_steps = nullptr;
-    int32_t rc = expand_steps_on_device(h, n, query_ct_count, client_cts, &d_steps);
-    if (rc) return rc;
+    const int64_t rows = shape.chunk_count * shape.columns;  // first-dimension inner products per query
+    const int64_t client_cts = eqc * indices_count;            // expanded ciphertexts per client
+    // the replies of index qi go straight to `out` unless several clients' replies interleave with other indices'
+    const bool direct = clients == 1 || indices_count == 1;
     StreamBuffers tmp(s);
     u64 *expanded = nullptr, *query_eval = nullptr, *results[2] = {nullptr, nullptr}, *lhs = nullptr, *ct3 = nullptr,
         *scratch = nullptr, *replies = nullptr;
     CK(tmp.alloc(&expanded, ct_words * client_cts * clients));
-    rc = expand_device(h, keys, clients, d_query, query_ct_count, client_cts, expanded, s, d_steps, first_client);
+    int32_t rc = expand_device(h, keys, clients, d_query, query_ct_count, client_cts, expanded, s, first_client);
     if (rc) return rc;
-    // firstDimensionQueries: convertToEvalFormat (:523-532).  All expanded ciphertexts go through one forward NTT, so
-    // the first-dimension slices of every client and index are transformed in one launch.  Only those slices are read;
-    // the others (dims[1..] per index: 75 of 512 ciphertexts at the C4 shape, ~15 % of this NTT) are transformed for
-    // nothing, which moves fewer bytes than gathering the first-dimension slices into a contiguous buffer would.
-    CK(tmp.alloc(&query_eval, ct_words * client_cts * clients));
+    // firstDimensionQueries: convertToEvalFormat (:523-532).  One client transforms only each index's first-dimension
+    // slice, into a buffer of dims[0] ciphertexts: captured graphs pin their temporaries, and the slice is 437 of 512
+    // ciphertexts at the C4 shape.  A group transforms all its expanded ciphertexts in one launch: the slices of later
+    // dimensions (~15 % of this NTT at the C4 shape) are transformed for nothing, which moves fewer bytes than
+    // gathering the first-dimension slices into a contiguous buffer would.
+    CK(tmp.alloc(&query_eval, clients == 1 ? ct_words * dim0 : ct_words * client_cts * clients));
     CK(tmp.alloc(&results[0], ct_words * rows * clients));
     CK(tmp.alloc(&results[1], ct_words * rows * clients));
-    CK(tmp.alloc(&replies, reply_words * clients));
+    if (!direct) CK(tmp.alloc(&replies, reply_words * clients));
     size_t scratch_words = 0, lhs_words = 0, ct3_words = 0;
     {
         int64_t count = rows;
@@ -575,15 +491,18 @@ int32_t compute_response_clients_device(const hecuda_context *h, const hecuda_ev
     for (int j = 0; j < clients; ++j) relin.key[j] = keys[j]->d_relin;
     const NttRowMap map = c.map_q(L);
     cudaError_t e;
-    if ((e = launch_ntt_forward(c, map, expanded, query_eval, client_cts * clients * 2 * L, s)) != cudaSuccess)
+    if (clients > 1 && (e = launch_ntt_forward(c, map, expanded, query_eval, client_cts * clients * 2 * L, s)) != cudaSuccess)
         return cuda_fail(e, "ntt");
     const size_t client_pitch = ct_words * client_cts * sizeof(u64);
     for (int64_t qi = 0; qi < indices_count; ++qi) {
         const hecuda_pir_database *db = dbs[db_count == 1 ? 0 : qi];
-        // every column of every chunk for every client: Scheme.innerProduct(ciphertexts:plaintexts:) (:427-435)
-        e = launch_inner_product_plain_clients(c, query_eval + ct_words * eqc * qi, (int64_t)ct_words * client_cts, clients, L,
-                                               dim0, db->d_plain, db->d_plain32, db->d_present, results[0],
-                                               (int64_t)ct_words * rows, rows, s);
+        const u64 *first_eval = clients == 1 ? query_eval : query_eval + ct_words * eqc * qi;
+        if (clients == 1 && (e = launch_ntt_forward(c, map, expanded + ct_words * eqc * qi, query_eval, dim0 * 2 * L, s)) != cudaSuccess)
+            return cuda_fail(e, "ntt");
+        // every column of every chunk for every client: Scheme.innerProduct(ciphertexts:plaintexts:) then
+        // convertToCanonicalFormat (:427-435)
+        e = launch_inner_product_plain_clients(c, first_eval, (int64_t)ct_words * client_cts, clients, L, dim0, db->d_plain,
+                                               db->d_plain32, db->d_present, results[0], (int64_t)ct_words * rows, rows, s);
         if (e != cudaSuccess) return cuda_fail(e, "innerProduct(ciphertexts:plaintexts:)");
         if ((e = launch_ntt_inverse(c, map, results[0], results[0], rows * clients * 2 * L, kScalePlain, s)) != cudaSuccess)
             return cuda_fail(e, "ntt");
@@ -598,8 +517,9 @@ int32_t compute_response_clients_device(const hecuda_context *h, const hecuda_ev
             if ((e = inner_product_chunk(c, scratch, lhs, results[cur], size, ct3, groups * clients, s)) != cudaSuccess)
                 return cuda_fail(e, "innerProduct");
             relin.items_per_client = groups;
-            if ((e = relinearize_chunk(c, scratch, nullptr, ct3, L, results[cur ^ 1], groups * clients, s, &relin)) != cudaSuccess)
-                return cuda_fail(e, "relinearize");
+            e = clients == 1 ? relinearize_chunk(c, scratch, keys[0]->d_relin, ct3, L, results[cur ^ 1], groups, s)
+                             : relinearize_chunk(c, scratch, nullptr, ct3, L, results[cur ^ 1], groups * clients, s, &relin);
+            if (e != cudaSuccess) return cuda_fail(e, "relinearize");
             cur ^= 1;
             count = groups;
             query_start += size;
@@ -607,16 +527,18 @@ int32_t compute_response_clients_device(const hecuda_context *h, const hecuda_ev
         if (count != shape.chunk_count)
             return fail(HECUDA_ERR_INVALID_ARGUMENT, "There should be only 1 ciphertext in the final result for each chunk");
         // modSwitchDownToSingle (HeScheme.swift:1481-1485); BFV's canonical format is already Coeff
+        u64 *out = d_out + reply_words * qi;
         const u64 *single = results[cur];
         for (int l = L; l > 1; --l) {
-            u64 *dst = l == 2 ? replies : results[cur ^ 1];
+            u64 *dst = l > 2 ? results[cur ^ 1] : direct ? out : replies;
             if ((e = launch_mod_switch(c, results[cur], l, dst, count * 2 * clients, s)) != cudaSuccess)
                 return cuda_fail(e, "modSwitchDown");
             cur ^= 1;
             single = dst;
         }
-        CK(cudaMemcpy2DAsync(d_out + reply_words * qi, reply_words * indices_count * sizeof(u64), single,
-                             reply_words * sizeof(u64), reply_words * sizeof(u64), (size_t)clients, cudaMemcpyDeviceToDevice, s));
+        if (single != out)  // one modulus already, or the staged replies of several clients and indices
+            CK(cudaMemcpy2DAsync(out, reply_words * indices_count * sizeof(u64), single, reply_words * sizeof(u64),
+                                 reply_words * sizeof(u64), (size_t)clients, cudaMemcpyDeviceToDevice, s));
     }
     return HECUDA_OK;
 }
@@ -688,7 +610,6 @@ struct PirGraph {
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     u64 *d_query = nullptr, *d_out = nullptr;
-    void *d_steps = nullptr;
     unsigned long long launches = 0;  // kernels inside the graph (for hecuda_kernel_launch_count)
     bool busy = false;
     void release() {
@@ -696,7 +617,6 @@ struct PirGraph {
         if (graph) cudaGraphDestroy(graph);
         if (d_query) cudaFree(d_query);
         if (d_out) cudaFree(d_out);
-        if (d_steps) cudaFree(d_steps);
     }
 };
 // Handles may outlive their context (a garbage-collected host destroys them in any order): only touch a live context.
@@ -749,6 +669,10 @@ PirGraph *acquire_graph(const hecuda_context *hc, const hecuda_evk *k, const hec
             }
     }
     const Context &c = *h->ctx;
+    // the shape's expansion plan goes to the context's cache before the capture: a miss inside it would allocate and
+    // copy synchronously, which invalidates the capture
+    const ExpandStep *d_steps = nullptr;
+    if ((*rc = expand_steps_on_device(hc, c.n, query_ct_count, shape.expanded_query_count, &d_steps))) return nullptr;
     const size_t ct_words = (size_t)2 * c.L * c.n, out_words = (size_t)2 * c.n * shape.chunk_count;
     PirGraph *g = new (std::nothrow) PirGraph();
     if (!g) return nullptr;
@@ -758,11 +682,8 @@ PirGraph *acquire_graph(const hecuda_context *hc, const hecuda_evk *k, const hec
     g->dims = shape.dims;
     g->chunk_count = shape.chunk_count;
     g->query_ct_count = query_ct_count;
-    const ExpandPlan plan = build_expand_plan(c.n, query_ct_count, shape.expanded_query_count);
     cudaError_t e = cudaMalloc(&g->d_query, ct_words * query_ct_count * sizeof(u64));
     if (e == cudaSuccess) e = cudaMalloc(&g->d_out, out_words * sizeof(u64));
-    if (e == cudaSuccess) e = cudaMalloc(&g->d_steps, std::max<size_t>(plan.steps.size(), 1) * sizeof(ExpandStep));
-    if (e == cudaSuccess && !plan.steps.empty()) e = upload(g->d_steps, plan.steps.data(), plan.steps.size() * sizeof(ExpandStep));
     if (e != cudaSuccess) {
         g->release();
         delete g;
@@ -772,8 +693,7 @@ PirGraph *acquire_graph(const hecuda_context *hc, const hecuda_evk *k, const hec
     e = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
     int32_t body = HECUDA_OK;
     if (e == cudaSuccess) {
-        const hecuda_pir_database *dbs[1] = {db};
-        body = compute_response_device(hc, k, dbs, 1, shape, g->d_query, query_ct_count, 1, g->d_out, s, g->d_steps);
+        body = respond_group(hc, &k, 1, -1, &db, 1, shape, g->d_query, query_ct_count, 1, g->d_out, s);
         e = cudaStreamEndCapture(s, &g->graph);
     }
     if (e == cudaSuccess && body == HECUDA_OK) e = cudaGraphInstantiate(&g->exec, g->graph, 0);
@@ -822,6 +742,81 @@ void release_graph(const hecuda_context *hc, PirGraph *g) {
     hecuda_context *h = const_cast<hecuda_context *>(hc);
     std::lock_guard<std::mutex> lock(h->mu);
     g->busy = false;
+}
+
+// ---------------------------------------------------------------- host bodies
+// The host calls run client_count clients' queries through one workspace stream, group by group: stage a group's
+// queries, answer the group, copy its replies back.  Temporaries are sized for one group.  single: a single-client
+// call, whose errors name no client.
+int32_t respond_words(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count, bool single,
+                      const hecuda_pir_database *const *dbs, int32_t db_count, const ResponseShape &shape,
+                      const uint64_t *queries, int32_t query_ct_count, int32_t indices_count, uint64_t *out) {
+    WsGuard g(h);
+    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    cudaStream_t s = g.w->stream;
+    const size_t query_words = (size_t)2 * h->ctx->L * h->ctx->n * query_ct_count;
+    const size_t out_words = (size_t)2 * h->ctx->n * shape.chunk_count * indices_count;
+    const int group = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count);
+    StreamBuffers tmp(s);
+    u64 *d_query = nullptr, *d_out = nullptr;
+    CK(tmp.alloc(&d_query, query_words * group));
+    CK(tmp.alloc(&d_out, out_words * group));
+    DrainOnExit drain{s};  // copies of the caller's buffers are in flight on `s` from here on
+    for (int32_t first = 0; first < client_count; first += group) {
+        const int clients = std::min<int32_t>(group, client_count - first);
+        CK(cudaMemcpyAsync(d_query, queries + query_words * first, query_words * clients * sizeof(u64), cudaMemcpyHostToDevice, s));
+        const int32_t rc = respond_group(h, evks + first, clients, single ? -1 : first, dbs, db_count, shape, d_query,
+                                         query_ct_count, indices_count, d_out, s);
+        if (rc) return rc;
+        CK(cudaMemcpyAsync(out + out_words * first, d_out, out_words * clients * sizeof(u64), cudaMemcpyDeviceToHost, s));
+    }
+    CK(wait_stream(s));
+    return HECUDA_OK;
+}
+
+// The same with seeded queries in and packed replies out: per group, one seeded expansion of all the group's query
+// ciphertexts, the group's responses, and one packing pass per reply poly over the group's replies.
+int32_t respond_wire(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count, bool single,
+                     const hecuda_pir_database *const *dbs, int32_t db_count, const ResponseShape &shape,
+                     const uint8_t *query_poly0, const uint8_t *query_seeds, int32_t query_ct_count, int32_t indices_count,
+                     int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1, uint8_t *out) {
+    if (!query_seeds) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    WireCodec wc;
+    int32_t rc = wc.setup(*h->ctx, skip_lsbs_poly0, skip_lsbs_poly1);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    WsGuard g(h);
+    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    cudaStream_t s = g.w->stream;
+    StreamBuffers tmp(s);
+    const int group = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count);
+    const size_t ct_words = (size_t)2 * c.L * c.n, poly0_bytes = wc.query_bytes * query_ct_count, seed_bytes = (size_t)32 * query_ct_count;
+    const int64_t replies = (int64_t)indices_count * shape.chunk_count;  // per client
+    const size_t out_bytes = wc.reply_bytes() * replies;
+    unsigned char *d_poly0 = nullptr, *d_seeds = nullptr;
+    u64 *d_query = nullptr, *d_resp = nullptr;
+    CK(tmp.alloc_bytes((void **)&d_poly0, poly0_bytes * group));
+    CK(tmp.alloc_bytes((void **)&d_seeds, seed_bytes * group));
+    CK(tmp.alloc(&d_query, ct_words * query_ct_count * group));
+    CK(tmp.alloc(&d_resp, (size_t)2 * c.n * replies * group));
+    CK(wc.alloc(tmp, c, replies * group));
+    DrainOnExit drain{s};  // copies of the caller's buffers are in flight on `s` from here on
+    for (int32_t first = 0; first < client_count; first += group) {
+        const int clients = std::min<int32_t>(group, client_count - first);
+        CK(cudaMemcpyAsync(d_poly0, query_poly0 + poly0_bytes * first, poly0_bytes * clients, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_seeds, query_seeds + seed_bytes * first, seed_bytes * clients, cudaMemcpyHostToDevice, s));
+        // Query.ciphertexts arrive as SerializedCiphertext.seeded (SerializedCiphertext.swift:41-49)
+        cudaError_t e = expand_seeded_device(c, c.L, d_poly0, d_seeds, d_query, (int64_t)query_ct_count * clients, s);
+        if (e != cudaSuccess) return cuda_fail(e, "expand seeded query");
+        rc = respond_group(h, evks + first, clients, single ? -1 : first, dbs, db_count, shape, d_query, query_ct_count,
+                           indices_count, d_resp, s);
+        if (rc) return rc;
+        // the group's replies are client-major, like `out`
+        if ((rc = wc.pack(c, d_resp, replies * clients, s))) return rc;
+        CK(cudaMemcpyAsync(out + out_bytes * first, wc.reply, out_bytes * clients, cudaMemcpyDeviceToHost, s));
+    }
+    CK(wait_stream(s));
+    return HECUDA_OK;
 }
 
 }  // namespace
@@ -916,12 +911,9 @@ int32_t hecuda_mulpir_expand(const hecuda_context *h, const hecuda_evk *k, const
     u64 *d_in = nullptr, *d_out = nullptr;
     CK(tmp.alloc(&d_in, ct_words * ct_count));
     CK(tmp.alloc(&d_out, ct_words * output_count));
+    DrainOnExit drain{s};  // copies of the caller's buffers are in flight on `s` from here on
     CK(cudaMemcpyAsync(d_in, cts, ct_words * ct_count * sizeof(u64), cudaMemcpyHostToDevice, s));
-    rc = expand_device(h, &k, 1, d_in, ct_count, output_count, d_out, s);
-    if (rc) {
-        wait_stream(s);
-        return rc;
-    }
+    if ((rc = expand_device(h, &k, 1, d_in, ct_count, output_count, d_out, s))) return rc;
     CK(cudaMemcpyAsync(out, d_out, ct_words * output_count * sizeof(u64), cudaMemcpyDeviceToHost, s));
     CK(wait_stream(s));
     return HECUDA_OK;
@@ -935,8 +927,8 @@ int32_t hecuda_mulpir_compute_response_device(const hecuda_context *h, const hec
     int32_t rc = check_response_args(h, k, dbs, db_count, dims, dim_count, chunk_count, query, query_ct_count,
                                      indices_count, out, shape);
     if (rc) return rc;
-    return compute_response_device(h, k, dbs, db_count, shape, (const u64 *)query, query_ct_count, indices_count,
-                                   (u64 *)out, (cudaStream_t)stream);
+    return respond_group(h, &k, 1, -1, dbs, db_count, shape, (const u64 *)query, query_ct_count, indices_count, (u64 *)out,
+                         (cudaStream_t)stream);
 }
 
 int32_t hecuda_mulpir_compute_response(const hecuda_context *h, const hecuda_evk *k, const hecuda_pir_database *const *dbs,
@@ -947,38 +939,28 @@ int32_t hecuda_mulpir_compute_response(const hecuda_context *h, const hecuda_evk
     int32_t rc = check_response_args(h, k, dbs, db_count, dims, dim_count, chunk_count, query, query_ct_count,
                                      indices_count, out, shape);
     if (rc) return rc;
-    WsGuard g(h);
-    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
-    const Context &c = *h->ctx;
-    const size_t ct_words = (size_t)2 * c.L * c.n, out_words = (size_t)2 * c.n * chunk_count * indices_count;
-    cudaStream_t s = g.w->stream;
-    if (indices_count == 1 && db_count == 1) {
+    if (indices_count == 1 && db_count == 1) {  // replay the captured pipeline of this (database, key, shape)
+        WsGuard g(h);
+        if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+        cudaStream_t s = g.w->stream;
         PirGraph *pg = acquire_graph(h, k, dbs[0], shape, query_ct_count, s, &rc);
         if (rc) return rc;
         if (pg) {
-            cudaError_t e = cudaMemcpyAsync(pg->d_query, query, ct_words * query_ct_count * sizeof(u64), cudaMemcpyHostToDevice, s);
+            const Context &c = *h->ctx;
+            cudaError_t e = cudaMemcpyAsync(pg->d_query, query, (size_t)2 * c.L * c.n * query_ct_count * sizeof(u64),
+                                            cudaMemcpyHostToDevice, s);
             if (e == cudaSuccess) e = cudaGraphLaunch(pg->exec, s);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(out, pg->d_out, out_words * sizeof(u64), cudaMemcpyDeviceToHost, s);
-            if (e == cudaSuccess) e = wait_stream(s);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(out, pg->d_out, (size_t)2 * c.n * chunk_count * sizeof(u64), cudaMemcpyDeviceToHost, s);
+            // on every path: the instance and the caller's buffers are only free once `s` has drained
+            const cudaError_t drained = wait_stream(s);
+            if (e == cudaSuccess) e = drained;
             g_kernel_launches += pg->launches;
             release_graph(h, pg);
             if (e != cudaSuccess) return cuda_fail(e, "response graph");
             return HECUDA_OK;
         }
-    }
-    StreamBuffers tmp(s);
-    u64 *d_query = nullptr, *d_out = nullptr;
-    CK(tmp.alloc(&d_query, ct_words * query_ct_count));
-    CK(tmp.alloc(&d_out, out_words));
-    CK(cudaMemcpyAsync(d_query, query, ct_words * query_ct_count * sizeof(u64), cudaMemcpyHostToDevice, s));
-    rc = compute_response_device(h, k, dbs, db_count, shape, d_query, query_ct_count, indices_count, d_out, s);
-    if (rc) {
-        wait_stream(s);
-        return rc;
-    }
-    CK(cudaMemcpyAsync(out, d_out, out_words * sizeof(u64), cudaMemcpyDeviceToHost, s));
-    CK(wait_stream(s));
-    return HECUDA_OK;
+    }  // not capturable on this setup, or several indices / databases: the direct path
+    return respond_words(h, &k, 1, true, dbs, db_count, shape, query, query_ct_count, indices_count, out);
 }
 
 int32_t hecuda_mulpir_compute_response_clients_device(const hecuda_context *h, const hecuda_evk *const *evks,
@@ -994,8 +976,8 @@ int32_t hecuda_mulpir_compute_response_clients_device(const hecuda_context *h, c
     const size_t out_words = (size_t)2 * h->ctx->n * chunk_count * indices_count;
     for (int32_t first = 0; first < client_count; first += HECUDA_MULPIR_CLIENT_GROUP) {
         const int clients = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count - first);
-        rc = compute_response_clients_device(h, evks + first, clients, first, dbs, db_count, shape, (const u64 *)queries + query_words * first,
-                                             query_ct_count, indices_count, (u64 *)out + out_words * first, (cudaStream_t)stream);
+        rc = respond_group(h, evks + first, clients, first, dbs, db_count, shape, (const u64 *)queries + query_words * first,
+                           query_ct_count, indices_count, (u64 *)out + out_words * first, (cudaStream_t)stream);
         if (rc) return rc;
     }
     return HECUDA_OK;
@@ -1009,29 +991,7 @@ int32_t hecuda_mulpir_compute_response_clients(const hecuda_context *h, const he
     int32_t rc = check_clients_args(h, evks, client_count, dbs, db_count, dims, dim_count, chunk_count, queries,
                                     query_ct_count, indices_count, out, shape);
     if (rc) return rc;
-    WsGuard g(h);
-    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
-    cudaStream_t s = g.w->stream;
-    const size_t query_words = (size_t)2 * h->ctx->L * h->ctx->n * query_ct_count;
-    const size_t out_words = (size_t)2 * h->ctx->n * chunk_count * indices_count;
-    const int group = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count);
-    StreamBuffers tmp(s);
-    u64 *d_query = nullptr, *d_out = nullptr;
-    CK(tmp.alloc(&d_query, query_words * group));
-    CK(tmp.alloc(&d_out, out_words * group));
-    for (int32_t first = 0; first < client_count; first += group) {
-        const int clients = std::min<int32_t>(group, client_count - first);
-        CK(cudaMemcpyAsync(d_query, queries + query_words * first, query_words * clients * sizeof(u64), cudaMemcpyHostToDevice, s));
-        rc = compute_response_clients_device(h, evks + first, clients, first, dbs, db_count, shape, d_query, query_ct_count,
-                                             indices_count, d_out, s);
-        if (rc) {
-            wait_stream(s);
-            return rc;
-        }
-        CK(cudaMemcpyAsync(out + out_words * first, d_out, out_words * clients * sizeof(u64), cudaMemcpyDeviceToHost, s));
-    }
-    CK(wait_stream(s));
-    return HECUDA_OK;
+    return respond_words(h, evks, client_count, false, dbs, db_count, shape, queries, query_ct_count, indices_count, out);
 }
 
 int32_t hecuda_mulpir_compute_response_wire(const hecuda_context *h, const hecuda_evk *k, const hecuda_pir_database *const *dbs,
@@ -1043,36 +1003,8 @@ int32_t hecuda_mulpir_compute_response_wire(const hecuda_context *h, const hecud
     int32_t rc = check_response_args(h, k, dbs, db_count, dims, dim_count, chunk_count, (const uint64_t *)query_poly0,
                                      query_ct_count, indices_count, out, shape);
     if (rc) return rc;
-    if (!query_seeds) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
-    WireCodec wc;
-    if ((rc = wc.setup(*h->ctx, skip_lsbs_poly0, skip_lsbs_poly1))) return rc;
-    const Context &c = *h->ctx;
-    WsGuard g(h);
-    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
-    cudaStream_t s = g.w->stream;
-    StreamBuffers tmp(s);
-    const size_t ct_words = (size_t)2 * c.L * c.n, in_bytes = wc.query_bytes;
-    const int64_t replies = (int64_t)indices_count * chunk_count;
-    unsigned char *d_poly0 = nullptr, *d_seeds = nullptr;
-    u64 *d_query = nullptr, *d_resp = nullptr;
-    CK(tmp.alloc_bytes((void **)&d_poly0, in_bytes * query_ct_count));
-    CK(tmp.alloc_bytes((void **)&d_seeds, (size_t)32 * query_ct_count));
-    CK(tmp.alloc(&d_query, ct_words * query_ct_count));
-    CK(tmp.alloc(&d_resp, (size_t)2 * c.n * replies));
-    CK(wc.alloc(tmp, c, replies));
-    // from here on copies of the caller's buffers are in flight on `s`: every return path waits for the stream first
-    DrainOnExit drain{s};
-    CK(cudaMemcpyAsync(d_poly0, query_poly0, in_bytes * query_ct_count, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(d_seeds, query_seeds, (size_t)32 * query_ct_count, cudaMemcpyHostToDevice, s));
-    // Query.ciphertexts arrive as SerializedCiphertext.seeded (SerializedCiphertext.swift:41-49)
-    cudaError_t e = expand_seeded_device(c, c.L, d_poly0, d_seeds, d_query, query_ct_count, s);
-    if (e != cudaSuccess) return cuda_fail(e, "expand seeded query");
-    rc = compute_response_device(h, k, dbs, db_count, shape, d_query, query_ct_count, indices_count, d_resp, s);
-    if (rc) return rc;
-    if ((rc = wc.pack(c, d_resp, replies, s))) return rc;
-    CK(cudaMemcpyAsync(out, wc.reply, wc.reply_bytes() * replies, cudaMemcpyDeviceToHost, s));
-    CK(wait_stream(s));
-    return HECUDA_OK;
+    return respond_wire(h, &k, 1, true, dbs, db_count, shape, query_poly0, query_seeds, query_ct_count, indices_count,
+                        skip_lsbs_poly0, skip_lsbs_poly1, out);
 }
 
 int32_t hecuda_mulpir_compute_response_clients_wire(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count,
@@ -1084,42 +1016,8 @@ int32_t hecuda_mulpir_compute_response_clients_wire(const hecuda_context *h, con
     int32_t rc = check_clients_args(h, evks, client_count, dbs, db_count, dims, dim_count, chunk_count,
                                     (const uint64_t *)query_poly0, query_ct_count, indices_count, out, shape);
     if (rc) return rc;
-    if (!query_seeds) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
-    WireCodec wc;
-    if ((rc = wc.setup(*h->ctx, skip_lsbs_poly0, skip_lsbs_poly1))) return rc;
-    const Context &c = *h->ctx;
-    WsGuard g(h);
-    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
-    cudaStream_t s = g.w->stream;
-    StreamBuffers tmp(s);
-    const int group = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count);
-    const size_t ct_words = (size_t)2 * c.L * c.n, poly0_bytes = wc.query_bytes * query_ct_count, seed_bytes = (size_t)32 * query_ct_count;
-    const int64_t replies = (int64_t)indices_count * chunk_count;  // per client
-    const size_t out_bytes = wc.reply_bytes() * replies;
-    unsigned char *d_poly0 = nullptr, *d_seeds = nullptr;
-    u64 *d_query = nullptr, *d_resp = nullptr;
-    CK(tmp.alloc_bytes((void **)&d_poly0, poly0_bytes * group));
-    CK(tmp.alloc_bytes((void **)&d_seeds, seed_bytes * group));
-    CK(tmp.alloc(&d_query, ct_words * query_ct_count * group));
-    CK(tmp.alloc(&d_resp, (size_t)2 * c.n * replies * group));
-    CK(wc.alloc(tmp, c, replies * group));
-    DrainOnExit drain{s};  // copies of the caller's buffers are in flight on `s` from here on
-    for (int32_t first = 0; first < client_count; first += group) {
-        const int clients = std::min<int32_t>(group, client_count - first);
-        CK(cudaMemcpyAsync(d_poly0, query_poly0 + poly0_bytes * first, poly0_bytes * clients, cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(d_seeds, query_seeds + seed_bytes * first, seed_bytes * clients, cudaMemcpyHostToDevice, s));
-        // every query ciphertext of the group in one expansion
-        cudaError_t e = expand_seeded_device(c, c.L, d_poly0, d_seeds, d_query, (int64_t)query_ct_count * clients, s);
-        if (e != cudaSuccess) return cuda_fail(e, "expand seeded query");
-        rc = compute_response_clients_device(h, evks + first, clients, first, dbs, db_count, shape, d_query, query_ct_count,
-                                             indices_count, d_resp, s);
-        if (rc) return rc;
-        // the group's replies are client-major, like `out`: one packing pass per reply poly
-        if ((rc = wc.pack(c, d_resp, replies * clients, s))) return rc;
-        CK(cudaMemcpyAsync(out + out_bytes * first, wc.reply, out_bytes * clients, cudaMemcpyDeviceToHost, s));
-    }
-    CK(wait_stream(s));
-    return HECUDA_OK;
+    return respond_wire(h, evks, client_count, false, dbs, db_count, shape, query_poly0, query_seeds, query_ct_count,
+                        indices_count, skip_lsbs_poly0, skip_lsbs_poly1, out);
 }
 
 }  // extern "C"

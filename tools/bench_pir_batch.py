@@ -34,7 +34,8 @@ import hecuda
 from hecuda import pir
 
 PIR_MODULI = [134176769, 268369921, 268361729]  # n_4096_logq_27_28_28_logt_5 (EncryptionParameters.swift:357-367)
-SCAN_KERNELS = ("inner_product_plain_small_clients_kernel", "inner_product_plain_clients_kernel")
+SCAN_KERNELS = ("inner_product_plain_small_clients_kernel", "inner_product_plain_clients_kernel",  # a group's scans
+                "inner_product_plain_small_kernel", "inner_product_plain_kernel")  # a lone client's scans
 
 
 def uniform(rng, moduli, shape_prefix, n):
