@@ -197,10 +197,13 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
     const int half_logn = c->logn - 1;
     const int64_t half_n = n / 2;
     const int threads = (int)((split ? half_n : n) / 16);
-    const size_t tr_bytes = (fast || split) ? sizeof(ulonglong2) * (size_t)15 * threads : 0;  // transposed line-owning-pass tables
+    // N = 2^13: the resident twiddle images instead of the transposed tables (ntt_fast.cuh)
+    const bool resident = fast && fast::resident_twiddles(c->logn);
+    const size_t tr_bytes = (fast || split) && !resident ? sizeof(ulonglong2) * (size_t)15 * threads : 0;  // transposed line-owning-pass tables
+    const size_t img_bytes = resident ? sizeof(ulonglong2) * (size_t)fast::image_entries(c->logn) : 0;
     const size_t half_bytes = sizeof(ulonglong2) * (size_t)half_n;
-    // per slot: [tw][itw] then, unsplit: [tw_t][itw_t]; split: per half [tw_h][itw_h][tw_t_h][itw_t_h]
-    const size_t slot_bytes = 2 * table_bytes + (split ? 2 * (2 * half_bytes + 2 * tr_bytes) : 2 * tr_bytes);
+    // per slot: [tw][itw] then, unsplit: [tw_t][itw_t] or [tw_img][itw_img]; split: per half [tw_h][itw_h][tw_t_h][itw_t_h]
+    const size_t slot_bytes = 2 * table_bytes + (split ? 2 * (2 * half_bytes + 2 * tr_bytes) : 2 * tr_bytes + 2 * img_bytes);
     if (cudaMalloc(&c->d_pool, slot_bytes * nslots) != cudaSuccess) { err = "cudaMalloc failed for twiddle tables"; delete c; return nullptr; }
     std::vector<ulonglong2> tw, itw, tr(15 * (size_t)threads), itr(15 * (size_t)threads), twh, itwh;
     std::vector<ModSlot> dev_slots(split ? 3 * nslots : nslots);
@@ -218,7 +221,27 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
         cudaMemcpy(base + table_bytes, itw.data(), table_bytes, cudaMemcpyHostToDevice);
         c->slots[s].dev.tw = (const ulonglong2 *)base;
         c->slots[s].dev.itw = (const ulonglong2 *)(base + table_bytes);
-        if (fast) {
+        if (resident) {
+            // the image keeps the even groups of the stage with N/2 twiddles only: check w_i = w_(i-1) zeta for every odd
+            // i there, zeta = psi^(N/2) = tw[1] (inverse psi^(-N/2) = itw[1])
+            const u64 p = slot_mod[s];
+            for (int64_t i = n / 2 + 1; i < n; i += 2)
+                if (tw[i].x != mulmod(tw[i - 1].x, tw[1].x, p) || itw[i].x != mulmod(itw[i - 1].x, itw[1].x, p)) {
+                    err = "internal error: twiddle table of " + std::to_string(p) + " is not in bit-reversed order";
+                    delete c;
+                    return nullptr;
+                }
+            const int entries = fast::image_entries(c->logn);
+            std::vector<ulonglong2> img(entries), iimg(entries);
+            for (int i = 0; i < entries; ++i) {
+                img[i] = tw[fast::image_source(c->logn, false, i)];
+                iimg[i] = itw[fast::image_source(c->logn, true, i)];
+            }
+            cudaMemcpy(base + 2 * table_bytes, img.data(), img_bytes, cudaMemcpyHostToDevice);
+            cudaMemcpy(base + 2 * table_bytes + img_bytes, iimg.data(), img_bytes, cudaMemcpyHostToDevice);
+            c->slots[s].dev.tw_img = (const ulonglong2 *)(base + 2 * table_bytes);
+            c->slots[s].dev.itw_img = (const ulonglong2 *)(base + 2 * table_bytes + img_bytes);
+        } else if (fast) {
             for (int k = 0; k < 15; ++k)
                 for (int tau = 0; tau < threads; ++tau) {
                     tr[(size_t)k * threads + tau] = tw[fast::fwd_last_source(c->logn, k, tau)];

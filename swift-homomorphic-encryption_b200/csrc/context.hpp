@@ -42,9 +42,13 @@ struct ModSlot {
     const ulonglong2 *tw;     // forward twiddles  [N]
     const ulonglong2 *itw;    // inverse twiddles  [N]  (itw[m+i] = tw[m+i]^-1)
     // transposed copies for the register-tiled kernels' line-owning pass (ntt_fast.cuh): entry k (< 15) of thread
-    // tau (< N/16) at [k * N/16 + tau]; null when N is outside the fast kernels' range
+    // tau (< N/16) at [k * N/16 + tau]; null when N is outside the fast kernels' range or has the resident image
     const ulonglong2 *tw_t;
     const ulonglong2 *itw_t;
+    // N = 2^13: every twiddle the fast kernels read, laid out as a CTA keeps them in shared memory (ntt_fast.cuh,
+    // resident_twiddles); null at other sizes
+    const ulonglong2 *tw_img;
+    const ulonglong2 *itw_img;
 };
 
 enum { kScalePlain = 0, kScaleTMont = 1, kScaleMont = 2, kScaleTMontFloor = 3 };

@@ -6,7 +6,8 @@
 //      swizzle) that land a row in a shared-memory row buffer and complete on that buffer's mbarrier -- with two
 //      buffers (N = 2^13, ntt_row_buffers) the CTA's next row, otherwise this row; it also prefetches the row after
 //      that into L2 (cp.async.bulk.prefetch.tensor) and, when the row's modulus differs from the previous row's,
-//      bulk-copies the first N/16 twiddles (all the LB > 0 passes need) into the CTA's shared-memory twiddle cache;
+//      bulk-copies the first N/16 twiddles (all the LB > 0 passes need; at N = 2^13 the resident image of all the
+//      twiddles, ntt_fast.cuh) into the CTA's shared-memory twiddle cache;
 //   2. 3-4 register passes over the row in shared memory (ntt_fast.cuh), one __syncthreads between passes;
 //   3. TMA out: bulk-tensor copies shared -> global of the finished row (same swizzle, undone by the copy engine), one
 //      bulk group per row; a buffer is refilled once the copy engine has read it.
@@ -167,13 +168,29 @@ __device__ __forceinline__ void inv_row_of(int cls, u64 *sm, int tau, const RowM
 // 400 W power limit: +4 % over one buffer; three buffers measured 1-2 % behind two).  With several CTAs per SM
 // (N <= 2^12) the other CTAs fill those gaps, and at N = 2^14 a second 128 KB buffer does not fit.
 HE_HD constexpr int ntt_row_buffers(int logn) { return logn == 13 ? 2 : 1; }
+// The twiddle cache of a CTA: at N = 2^13 (resident_twiddles, ntt_fast.cuh) the resident image of every twiddle the
+// transform reads (96 KB: the two row buffers leave just room for it), otherwise the first N/16 twiddles (the LB > 0
+// passes; the LB == 0 pass reads the transposed table in global memory).  Both arrive by one 1-D bulk copy.
+template <int LOGN>
+HE_HD constexpr u32 ntt_twiddle_bytes() {
+    return (u32)sizeof(ulonglong2) * (resident_twiddles(LOGN) ? image_entries(LOGN) : 1 << (LOGN - 4));
+}
+// cp.async.bulk moves a multiple of 16 bytes, and an mbarrier's pending transaction count stays below 2^20
+static_assert(ntt_twiddle_bytes<13>() == 98304 && ntt_twiddle_bytes<13>() % 16 == 0 && ntt_twiddle_bytes<13>() < (1u << 20),
+              "the resident image is one 1-D bulk copy on one mbarrier");
+template <int LOGN, bool INVERSE>
+__device__ __forceinline__ const ulonglong2 *ntt_twiddle_source(const ModSlot &S) {
+    if (resident_twiddles(LOGN)) return INVERSE ? S.itw_img : S.tw_img;
+    return INVERSE ? S.itw : S.tw;
+}
 
-// Shared memory of a CTA: [row buffers: B x N words][twiddle cache: N/16 entries][B + 1 mbarriers].
+// Shared memory of a CTA: [row buffers: B x N words][twiddle cache][B + 1 mbarriers].
 template <int LOGN>
 constexpr size_t ntt_smem_bytes() {
     constexpr int B = ntt_row_buffers(LOGN);
-    return sizeof(u64) * B * ((size_t)1 << LOGN) + sizeof(ulonglong2) * ((size_t)1 << (LOGN - 4)) + sizeof(u64) * (B + 1);
+    return sizeof(u64) * B * ((size_t)1 << LOGN) + ntt_twiddle_bytes<LOGN>() + sizeof(u64) * (B + 1);
 }
+static_assert(ntt_smem_bytes<13>() == 229400 && ntt_smem_bytes<13>() <= 232448, "N = 2^13: 227 KB of shared memory a CTA");
 
 // CTAs per SM the register budget is sized for.  1024 threads per SM (64 registers a thread, some spills) except at
 // N = 2^13, where one 512-thread CTA with 128 registers and no spills is faster on H100 (C2, runs alternated in one
@@ -191,11 +208,11 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
     constexpr int kLines = (1 << LOGN) / kLineWords;
     constexpr int kBoxes = kLines > kBoxLines ? kLines / kBoxLines : 1;
     constexpr int kLinesPerBox = kLines / kBoxes;
-    constexpr u32 kRowBytes = (u32)sizeof(u64) << LOGN, kTwBytes = (u32)sizeof(ulonglong2) << (LOGN - 4);
+    constexpr u32 kRowBytes = (u32)sizeof(u64) << LOGN, kTwBytes = ntt_twiddle_bytes<LOGN>();
     // B row buffers; row k of the CTA uses buffer k % B, and its TMA-in is issued AHEAD rows before the CTA starts on it
     constexpr int B = ntt_row_buffers(LOGN), AHEAD = B > 1 ? 1 : 0;
     ulonglong2 *tw_cache = reinterpret_cast<ulonglong2 *>(smem + B * (1 << LOGN));
-    u64 *bar_row = reinterpret_cast<u64 *>(tw_cache + (1 << (LOGN - 4)));  // one per buffer
+    u64 *bar_row = reinterpret_cast<u64 *>(tw_cache + kTwBytes / sizeof(ulonglong2));  // one per buffer
     u64 *bar_tw = bar_row + B;
     const int tau = threadIdx.x;
     const int tasks = polys * rl.count;  // < 2^31 (checked by the launcher)
@@ -239,7 +256,7 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, ntt_min_ctas(LOGN))
             // every thread has passed the barrier that follows its last use of the twiddle cache
             if (new_slot) {
                 mbar_arrive_expect_tx(bar_tw, kTwBytes);
-                tma_load_1d(tw_cache, INVERSE ? S.itw : S.tw, kTwBytes, bar_tw);
+                tma_load_1d(tw_cache, ntt_twiddle_source<LOGN, INVERSE>(S), kTwBytes, bar_tw);
             }
             // the row AHEAD tasks on goes into a buffer whose last row's TMA-out was committed B - AHEAD rows ago: the
             // copy engine must have read it, which leaves the B - 1 - AHEAD stores committed since then in flight
@@ -338,15 +355,16 @@ __device__ __forceinline__ u64 mont_product(u64 a, u64 b, u64 p, u64 ninv) { ret
 // The Q rows (r < L) are read from lhs / rhs themselves, the auxiliary rows from what the lift wrote,
 // ext[pair][4][L + 1][N] (polynomials a0 a1 b0 b1).
 //
-// Shared memory: [row buffers: operand j of the task in buffer j, 2 x N words][twiddle cache: N/16 entries][3 mbarriers].
+// Shared memory: [row buffers: operand j of the task in buffer j, 2 x N words][twiddle cache: the resident image][3 mbarriers].
 // A task's rows stay in their buffers until the cluster barrier that ends its tensor step; the next task's two rows
 // are loaded after it, the second under the first one's passes.  (A third buffer that took the next task's first row
 // under the current task's second row and tensor step measured no faster: C2 on H100 at a 400 W power limit, three
 // runs each, 136.3-137.1 k mult/s with three buffers, 136.3-137.7 k with two.)
 template <int LOGN>
 constexpr size_t ntt_tensor_smem_bytes() {
-    return sizeof(u64) * 2 * ((size_t)1 << LOGN) + sizeof(ulonglong2) * ((size_t)1 << (LOGN - 4)) + sizeof(u64) * 3;
+    return sizeof(u64) * 2 * ((size_t)1 << LOGN) + ntt_twiddle_bytes<LOGN>() + sizeof(u64) * 3;
 }
+static_assert(ntt_tensor_smem_bytes<13>() == 229400, "N = 2^13: 227 KB of shared memory a CTA");
 
 // The tensor step of one task: c0 (rank 0) or c2 (rank 1) from this CTA's rows x = a_rank, y = b_rank, then, once the
 // peer's rows are final, this CTA's half of the columns of c1.  H: the row's prime is h 2^32 + 1.
@@ -385,10 +403,10 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, 1)
     extern __shared__ __align__(1024) u64 smem[];  // row buffers first: the 128-byte swizzle wants them 1024-byte aligned
     constexpr int N = 1 << LOGN;
     constexpr int kBoxes = N / kLineWords / kBoxLines;
-    constexpr u32 kRowBytes = (u32)sizeof(u64) << LOGN, kTwBytes = (u32)sizeof(ulonglong2) << (LOGN - 4);
+    constexpr u32 kRowBytes = (u32)sizeof(u64) << LOGN, kTwBytes = ntt_twiddle_bytes<LOGN>();
     static_assert(kBoxes >= 1, "one row is at least one box");
     ulonglong2 *tw_cache = reinterpret_cast<ulonglong2 *>(smem + 2 * N);
-    u64 *bar_row = reinterpret_cast<u64 *>(tw_cache + N / 16);  // one per buffer
+    u64 *bar_row = reinterpret_cast<u64 *>(tw_cache + kTwBytes / sizeof(ulonglong2));  // one per buffer
     u64 *bar_tw = bar_row + 2;
     const int tau = threadIdx.x;
     const u32 rank = cluster_ctarank();
@@ -436,7 +454,7 @@ __global__ void __launch_bounds__((1 << LOGN) / 16, 1)
             // every thread has passed the barrier that follows its last use of the twiddle cache
             if (new_slot) {
                 mbar_arrive_expect_tx(bar_tw, kTwBytes);
-                tma_load_1d(tw_cache, S.tw, kTwBytes, bar_tw);
+                tma_load_1d(tw_cache, ntt_twiddle_source<LOGN, false>(S), kTwBytes, bar_tw);
             }
             load_row(task, 0);
             load_row(task, 1);

@@ -20,7 +20,8 @@
 //       N^-1 psi^-(N/2) (optionally times t or 2^64).
 // The LB == 0 pass (last forward / first inverse) gives every thread its own 15 twiddles; they come from a transposed
 // copy of the table (entry k of thread tau at [k * T + tau]) so each load instruction of a warp is one contiguous
-// 512-byte request.
+// 512-byte request.  At N = 2^13 that copy lives in shared memory with the rest of the twiddles (the resident image,
+// see resident_twiddles below); the other sizes read it from global memory.
 //
 // Shared-memory layout: the TMA unit's 128-byte swizzle (CU_TENSOR_MAP_SWIZZLE_128B) -- the 16-byte chunk c of the
 // 128-byte line r is stored at chunk c ^ (r & 7), i.e. word index phys(e) = e ^ (((e >> 4) & 7) << 1).  The row needs
@@ -206,7 +207,8 @@ struct RowMod {
     u64 np;           // 2^64 - p: lets the Shoup product be all multiply-adds (y w + q np)
     u64 kp;           // NARROW / MID: 4p, WIDE: 2p  (the offset that keeps x - v non-negative)
     const ulonglong2 *tw;    // twiddles of this direction, indexed like the reference's rootOfUnityPowers (host emulation)
-    unsigned tw_s;           // device: shared-memory address of the CTA's copy of tw[0 .. N/16) (the LB > 0 passes)
+    unsigned tw_s;           // device: shared-memory address of the CTA's copy of tw[0 .. N/16) (the LB > 0 passes), or
+                             // at N = 2^13 of the resident image
     const ModSlot *slot;     // p, mu1, red_shift, red_recip, inv_scale[scale_mode], tw_t / itw_t
     int scale_mode;          // < 0: forward transform
     bool partial;            // inverse only: this row is one half of a 2^15 transform -- its last stage is an ordinary
@@ -214,6 +216,26 @@ struct RowMod {
     // transposed copy of the twiddles for the LB == 0 pass: entry k of thread tau at [k * T + tau]
     HE_HD const ulonglong2 *tw_t() const { return scale_mode < 0 ? slot->tw_t : slot->itw_t; }
 };
+
+// ---- resident twiddle image (N = 2^13)
+// There one CTA runs per SM (ntt_fast.cu) and walks many consecutive rows of one modulus, but the transposed table of
+// the LB == 0 pass is 15 x 8 KB = 120 KB, read once per row from L2 -- nearly twice the row itself.  So the CTA keeps
+// every twiddle of the transform in shared memory, loaded by one bulk copy when the row's modulus changes:
+//     image = [tw[0 .. T): the LB > 0 passes][LB == 0 pass: slot k' (< 11) of thread tau at T + k' T + tau]
+// Of the LB == 0 stage with N/2 twiddles (forward stage j = 3, inverse stage J = 0) only the even groups are kept:
+// entries i - 1 and i (i odd) of that stage differ in bit 0 of i, i.e. by N/2 in the exponent of psi (the tables are
+// bit-reversed), so w_i = w_(i-1) zeta with zeta = psi^(N/2) = tw[1] (inverse: psi^(-N/2) = itw[1]), which is image
+// entry 1.  The odd groups multiply their operand by zeta and then by the even group's twiddle.  11 slots a thread
+// instead of 15: the image is 8 KB + 11 x 8 KB = 96 KB, and with the two 64 KB row buffers a CTA needs 229 400 bytes of
+// the 232 448 it may have (with all 15 slots, 262 168 would not fit).  N <= 2^12 (several CTAs per SM) and N = 2^14
+// (one 128 KB row buffer) keep the global transposed table.
+HE_HD constexpr bool resident_twiddles(int logn) { return logn == 13; }
+constexpr int kImageSlots = 11;
+HE_HD constexpr int image_entries(int logn) { return (1 << (logn - 4)) * (1 + kImageSlots); }
+// the transposed entry k (< 15, see fwd_last_source / inv_first_source) that image slot k' holds
+HE_HD constexpr int fwd_image_k(int kp) { return kp < 7 ? kp : 7 + 2 * (kp - 7); }    // stage j = 3: even groups
+HE_HD constexpr int inv_image_k(int kp) { return kp < 4 ? 2 * kp : kp + 4; }          // stage J = 0: even groups
+
 // twiddle `index` (< N/16) of the LB > 0 passes: from the CTA's shared-memory copy on the device
 HE_HD ulonglong2 ld_tw_cached(const RowMod &m, int index) {
 #if defined(__CUDA_ARCH__)
@@ -222,6 +244,17 @@ HE_HD ulonglong2 ld_tw_cached(const RowMod &m, int index) {
     return v;
 #else
     return m.tw[index];
+#endif
+}
+// slot k' of thread tau (< T = N/16) of the resident image: on the device from the CTA's shared-memory image; the host
+// emulation reads the transposed entry that slot holds from the transposed table, so it replays which entries the
+// kernels keep and the zeta step.  (The image itself is checked against the transposed order by
+// tests/test_ntt_resident_image.py.)
+HE_HD ulonglong2 ld_tw_image(const RowMod &m, int kp, int tau, int T) {
+#if defined(__CUDA_ARCH__)
+    return ld_tw_cached(m, T + kp * T + tau);
+#else
+    return m.tw_t()[(m.scale_mode < 0 ? fwd_image_k(kp) : inv_image_k(kp)) * T + tau];
 #endif
 }
 HE_HD u64 ld_u64(const u64 *p) {
@@ -390,6 +423,16 @@ HE_HD u32 shoup32(u32 y, u32 w, u32 wp, u32 p) {  // y w mod p in [0, 2p) for an
     return y * w - mul_hi_u32(y, wp) * p;
 }
 
+// y w mod p with the class's twiddle product, landing where the butterflies' products land: SMALL [0, 2p) for any
+// y < 2^32, NARROW / NARROW-H / MID [0, 4p) and WIDE [0, 2p) for any y < 2^64
+template <int CLS>
+HE_HD u64 tw_mul(u64 y, const ulonglong2 w, const RowMod &m) {
+    if (CLS == kSmall) return shoup32((u32)y, (u32)w.x, (u32)(w.y >> 32), (u32)(0 - m.np));
+    if (narrow_like(CLS)) return shoup4c<CLS>(y, w.x, w.y, m.np);
+    if (CLS == kMid) return shoup4(y, w.x, w.y, m.np);
+    return shoup2(y, w.x, w.y, m.np);
+}
+
 template <int CLS>
 HE_HD void ct_butterfly(u64 &x, u64 &y, const ulonglong2 w, const RowMod &m) {
     if (CLS == kSmall) {  // [0, 4p) < 2^32
@@ -423,17 +466,27 @@ template <int LOGN, int LB, int C, int CLS, int J>
 HE_HD void fwd_stage(u64 (&x)[16], int tau, const RowMod &m) {
     constexpr int E = pass_e(LB, C), F = 1 << E, S0 = LOGN - LB - C, T = (1 << LOGN) / 16;
     constexpr int H = 1 << (C - 1 - J);
+    constexpr bool kImage = LB == 0 && resident_twiddles(LOGN);  // LB == 0 twiddles from the resident image
+    constexpr bool kZeta = kImage && J == 3;                       // the stage with N/2 twiddles: odd groups via zeta
     const int hi = tau >> (LB - E);
-    const ulonglong2 *tw_t = LB == 0 ? m.tw_t() + tau : nullptr;
+    const ulonglong2 *tw_t = LB == 0 && !kImage ? m.tw_t() + tau : nullptr;
+    const ulonglong2 zeta = kZeta ? ld_tw_cached(m, 1) : make_ulonglong2(0, 0);
+    ulonglong2 w = make_ulonglong2(0, 0);
 #pragma unroll
     for (int grp = 0; grp < (1 << J); ++grp) {
-        const ulonglong2 w = LB == 0 ? ld_tw(tw_t + ((1 << J) - 1 + grp) * T)
-                                     : ld_tw_cached(m, (1 << (S0 + J)) + (hi << J) + grp);
+        const bool odd = kZeta && (grp & 1);  // w_grp = w_(grp-1) zeta: keep the even group's twiddle
+        if (!odd)
+            w = kImage  ? ld_tw_image(m, kZeta ? 7 + grp / 2 : (1 << J) - 1 + grp, tau, T)
+                : LB == 0 ? ld_tw(tw_t + ((1 << J) - 1 + grp) * T)
+                          : ld_tw_cached(m, (1 << (S0 + J)) + (hi << J) + grp);
 #pragma unroll
         for (int k = 0; k < H; ++k) {
             const int a = grp * 2 * H + k;
 #pragma unroll
-            for (int f = 0; f < F; ++f) ct_butterfly<CLS>(x[a * F + f], x[(a + H) * F + f], w, m);
+            for (int f = 0; f < F; ++f) {
+                if (odd) x[(a + H) * F + f] = tw_mul<CLS>(x[(a + H) * F + f], zeta, m);
+                ct_butterfly<CLS>(x[a * F + f], x[(a + H) * F + f], w, m);
+            }
         }
     }
 }
@@ -458,24 +511,33 @@ HE_HD void fwd_finish(u64 (&x)[16], const RowMod &m) {
 }
 
 // ------------------------------------------------------------------------------------------------ inverse
+// zeta (non-null): the difference is multiplied by *zeta before w (an odd group of the resident image's zeta stage)
 template <int CLS>
-HE_HD void gs_butterfly(u64 &x, u64 &y, const ulonglong2 w, const RowMod &m, u64 kp) {
+HE_HD void gs_butterfly(u64 &x, u64 &y, const ulonglong2 w, const RowMod &m, u64 kp, const ulonglong2 *zeta = nullptr) {
     if (CLS == kSmall) {  // inputs < 2p, outputs < 2p
         const u32 p = (u32)(0 - m.np), p2 = 2 * p;
         const u32 s = csub32((u32)x + (u32)y, p2);
-        y = shoup32((u32)x - (u32)y + p2, (u32)w.x, (u32)(w.y >> 32), p);
+        u32 d = (u32)x - (u32)y + p2;
+        if (zeta) d = (u32)tw_mul<CLS>(d, *zeta, m);
+        y = shoup32(d, (u32)w.x, (u32)(w.y >> 32), p);
         x = s;
     } else if (narrow_like(CLS)) {  // inputs < kp (a multiple of p), outputs x < 2 kp, y < 4p
         const u64 s = x + y;
-        y = shoup4c<CLS>(x - y + kp, w.x, w.y, m.np);
+        u64 d = x - y + kp;
+        if (zeta) d = tw_mul<CLS>(d, *zeta, m);
+        y = shoup4c<CLS>(d, w.x, w.y, m.np);
         x = s;
     } else if (CLS == kMid) {  // inputs < 4p, outputs < 4p
         const u64 s = csub(x + y, kp);
-        y = shoup4(x - y + kp, w.x, w.y, m.np);
+        u64 d = x - y + kp;
+        if (zeta) d = tw_mul<CLS>(d, *zeta, m);
+        y = shoup4(d, w.x, w.y, m.np);
         x = s;
     } else {  // inputs < 2p, outputs < 2p
         const u64 s = csub(x + y, kp);
-        y = shoup2(x - y + kp, w.x, w.y, m.np);
+        u64 d = x - y + kp;
+        if (zeta) d = tw_mul<CLS>(d, *zeta, m);
+        y = shoup2(d, w.x, w.y, m.np);
         x = s;
     }
 }
@@ -489,18 +551,25 @@ HE_HD void inv_stage(u64 (&x)[16], const int tau, const RowMod &m) {
     constexpr int kGroups = 1 << (LOGN - 1 - LB - J);
     const int hi = tau >> (LB - E);
     const u64 kp = narrow_like(CLS) ? (0 - m.np) * (u64)inv_bound_after(BIN, J) : m.kp;  // inputs < kp
-    const ulonglong2 *tw_t = LB == 0 ? m.tw_t() + tau : nullptr;
+    constexpr bool kImage = LB == 0 && resident_twiddles(LOGN);  // LB == 0 twiddles from the resident image
+    constexpr bool kZeta = kImage && J == 0;                       // the stage with N/2 twiddles: odd groups via zeta
+    const ulonglong2 *tw_t = LB == 0 && !kImage ? m.tw_t() + tau : nullptr;
+    const ulonglong2 zeta = kZeta ? ld_tw_cached(m, 1) : make_ulonglong2(0, 0);
+    ulonglong2 w = make_ulonglong2(0, 0);
 #pragma unroll
     for (int grp = 0; grp < (1 << (C - 1 - J)); ++grp) {
         if (!kLast || m.partial) {
+            const bool odd = kZeta && (grp & 1);  // w_grp = w_(grp-1) zeta: keep the even group's twiddle
             // LB == 0: entry index inside the thread's 15 = (groups of the earlier stages) + grp
-            const ulonglong2 w = LB == 0 ? ld_tw(tw_t + (16 - (16 >> J) + grp) * T)
-                                         : ld_tw_cached(m, kGroups + (hi << (C - 1 - J)) + grp);
+            if (!odd)
+                w = kImage  ? ld_tw_image(m, kZeta ? grp / 2 : 16 - (16 >> J) + grp - 4, tau, T)
+                    : LB == 0 ? ld_tw(tw_t + (16 - (16 >> J) + grp) * T)
+                              : ld_tw_cached(m, kGroups + (hi << (C - 1 - J)) + grp);
 #pragma unroll
             for (int k = 0; k < HH; ++k) {
                 const int a = grp * 2 * HH + k;
 #pragma unroll
-                for (int f = 0; f < F; ++f) gs_butterfly<CLS>(x[a * F + f], x[(a + HH) * F + f], w, m, kp);
+                for (int f = 0; f < F; ++f) gs_butterfly<CLS>(x[a * F + f], x[(a + HH) * F + f], w, m, kp, odd ? &zeta : nullptr);
             }
         } else {
             const u64 *sc = &m.slot->inv_scale[m.scale_mode].c0;  // c0, c0p, c1, c1p
@@ -553,6 +622,14 @@ HE_HD int inv_first_source(int logn, int k, int tau) {
     while (16 - (16 >> (J + 1)) <= k) ++J;
     const int grp = k - (16 - (16 >> J));
     return (1 << (logn - 1 - J)) + (tau << (3 - J)) + grp;
+}
+// the resident image (resident_twiddles): entry i (< image_entries) = tw[image_source(logn, false, i)] forward,
+// itw[image_source(logn, true, i)] inverse
+HE_HD int image_source(int logn, bool inverse, int i) {
+    const int T = 1 << (logn - 4);
+    if (i < T) return i;
+    const int kp = i / T - 1, tau = i % T;
+    return inverse ? inv_first_source(logn, inv_image_k(kp), tau) : fwd_last_source(logn, fwd_image_k(kp), tau);
 }
 
 }  // namespace fast
