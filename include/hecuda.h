@@ -432,6 +432,43 @@ int32_t hecuda_pnns_mul_transpose_matrix(const hecuda_context *ctx, const hecuda
                                          int32_t pack_rotation_count, int32_t mod_switch_to_single, uint64_t *out,
                                          int64_t out_capacity, int64_t *out_count);
 
+/* Many PNNS clients in one call: Server.computeResponse (PrivateNearestNeighborSearch/Server.swift:61-88) for one
+ * plaintext matrix -- mulTranspose(matrix:using:) + modSwitchDownToSingle -- for client_count queries of the same shape,
+ * client c answered with evks[c].  ciphertexts: client_count x ciphertext_count x 2 x L x N (Coeff); the row descriptors
+ * are those of hecuda_pnns_mul_transpose_matrix, shared by all clients.  out: client_count x out_capacity ciphertexts of
+ * 2 x 1 x N; *out_count replies per client.  Client c's replies (out + c * out_capacity * 2 * N) are bit-identical to what
+ * hecuda_pnns_mul_transpose_matrix(..., mod_switch_to_single = 1) returns for that client alone.  Clients are processed
+ * in groups of at most HECUDA_PNNS_CLIENT_GROUP: every rotation is one key-switching pass over a group, each client with
+ * its own keys, and the matrix streams from HBM once per group (from two clients up, the launch count does not depend
+ * on the group's size); temporaries scale with the group.  A group of one runs the kernels of
+ * hecuda_pnns_mul_transpose_matrix.  Every client's key is checked and every Galois key it needs found before anything
+ * is enqueued (a failure's message starts with "client <c>: " and leaves out untouched); out_capacity too small:
+ * HECUDA_ERR_INVALID_ARGUMENT with *out_count set to the replies needed per client. */
+#define HECUDA_PNNS_CLIENT_GROUP 16
+int32_t hecuda_pnns_compute_response_clients(const hecuda_context *ctx, const hecuda_evk *const *evks, int32_t client_count,
+                                             const hecuda_pnns_matrix *matrix, const uint64_t *ciphertexts,
+                                             int32_t ciphertext_count, int32_t query_row_count,
+                                             const int32_t *row_ciphertext_index, const uint64_t *row_masks,
+                                             const int32_t *row_rotate_count, int32_t column_step,
+                                             const int32_t *pack_rotations, int32_t pack_rotation_count, uint64_t *out,
+                                             int64_t out_capacity, int64_t *out_count);
+
+/* The same on the wire (ApplicationProtobuf/PnnsConversionApi.swift:48): the query ciphertexts as
+ * SerializedCiphertext.seeded (query_poly0: client_count x ciphertext_count x byteCount(L rows, skipLSBs 0),
+ * query_seeds: client_count x ciphertext_count x 32; SerializedCiphertext.swift:41-49,126-154) and the replies serialized
+ * forDecryption with skip_lsbs_poly0 / skip_lsbs_poly1 dropped bits (Bfv.skipLSBsForDecryption,
+ * Bfv+Decrypt.swift:51-110).  out: client_count x out_capacity x (byteCount(1 row, skip0) + byteCount(1 row, skip1))
+ * bytes.  Invalid skips: HECUDA_ERR_INVALID_ARGUMENT. */
+int32_t hecuda_pnns_compute_response_clients_wire(const hecuda_context *ctx, const hecuda_evk *const *evks,
+                                                  int32_t client_count, const hecuda_pnns_matrix *matrix,
+                                                  const uint8_t *query_poly0, const uint8_t *query_seeds,
+                                                  int32_t ciphertext_count, int32_t query_row_count,
+                                                  const int32_t *row_ciphertext_index, const uint64_t *row_masks,
+                                                  const int32_t *row_rotate_count, int32_t column_step,
+                                                  const int32_t *pack_rotations, int32_t pack_rotation_count,
+                                                  int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1, uint8_t *out,
+                                                  int64_t out_capacity, int64_t *out_count);
+
 /* ---- coefficient-wise PolyRq arithmetic (SURVEY.md section 8a, row a7) ----
  * PolyRq += / -= (PolyRq/PolyRq.swift:147-174), *= in Eval format (:184-204, Modulus.multiplyMod Modulus.swift:89-94),
  * negation (negateMod, ModularArithmetic/Scalar.swift:167-175) and *= [T] with one reduced scalar per RNS row

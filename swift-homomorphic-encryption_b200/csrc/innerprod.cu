@@ -382,7 +382,8 @@ cudaError_t launch_inner_product_plain_clients(const Context &ctx, const u64 *ct
                                                int64_t terms, const u64 *pts, const u32 *pts32, const unsigned char *present,
                                                u64 *out, int64_t out_client_stride, int64_t out_count, cudaStream_t stream) {
     if (out_count == 0) return cudaSuccess;
-    if (clients < 1 || clients > kScanClientTile * kScanClientTiles || l < 1 || l > ctx.L || ctx.n < 2 ||
+    const int64_t coeff_blocks = ((pts32 ? ctx.n / 2 : ctx.n) + 63) / 64;
+    if (clients < 1 || coeff_blocks * ((clients + kScanClientTile - 1) / kScanClientTile) > 0x7fffffff || l < 1 || l > ctx.L || ctx.n < 2 ||
         (pts32 != nullptr) == (pts != nullptr) || (pts32 && !inner_product_plain_small_supported(ctx, l)))
         return cudaErrorInvalidValue;
     if (clients == 1)  // a lone client: the single-client scans (same layout), not a tile of four clients' work
@@ -392,7 +393,7 @@ cudaError_t launch_inner_product_plain_clients(const Context &ctx, const u64 *ct
     const IpConsts cw = pts32 ? IpConsts{} : ip_consts(ctx, l);
     if (pts32 && cs.max_terms < 1) return cudaErrorInvalidValue;
     const unsigned tiles = (unsigned)((clients + kScanClientTile - 1) / kScanClientTile);
-    const unsigned gx = (unsigned)(((pts32 ? ctx.n / 2 : ctx.n) + 63) / 64) * tiles;
+    const unsigned gx = (unsigned)coeff_blocks * tiles;
     const int block = 64;
     const int64_t max_rows = (int64_t)65535 * kScanRowTile;
     for (int64_t done = 0; done < out_count;) {

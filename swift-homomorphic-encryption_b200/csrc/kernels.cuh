@@ -86,11 +86,12 @@ cudaError_t launch_inner_product_plain(const Context &ctx, const u64 *cts, int n
 bool inner_product_plain_small_supported(const Context &ctx, int l);
 cudaError_t launch_inner_product_plain_small(const Context &ctx, const u64 *cts, int npoly, int l, int64_t terms, const u32 *pts,
                                              const unsigned char *present, u64 *out, int64_t out_count, cudaStream_t stream);
-// The same scans for `clients` (<= kScanClientTile * kScanClientTiles) 2-poly queries at once: client j's `terms`
-// ciphertexts start at cts + j * client_stride, its out_count x 2 x l x N results at out + j * out_client_stride.
-// The client tiles of a row tile are adjacent blocks, so a database row comes from HBM about once per launch; every
-// value is the one the single-client scan computes.  One client runs the single-client scan itself.
-constexpr int kScanClientTile = 4, kScanClientTiles = 4, kScanRowTile = 2;  // clients, tiles per launch, rows
+// The same scans for `clients` 2-poly queries at once: client j's `terms` ciphertexts start at cts + j * client_stride,
+// its out_count x 2 x l x N results at out + j * out_client_stride.  The client tiles of a row tile are adjacent
+// blocks, so a database row comes from HBM about once per launch; every value is the one the single-client scan
+// computes.  One client runs the single-client scan itself.  A MulPir group is kScanClientTiles tiles; the PNNS group
+// pipeline passes every rotated-state set of its group (clients x query rows) as a client.
+constexpr int kScanClientTile = 4, kScanClientTiles = 4, kScanRowTile = 2;  // clients, tiles per MulPir group, rows
 cudaError_t launch_inner_product_plain_clients(const Context &ctx, const u64 *cts, int64_t client_stride, int clients, int l,
                                                int64_t terms, const u64 *pts, const u32 *pts32, const unsigned char *present,
                                                u64 *out, int64_t out_client_stride, int64_t out_count, cudaStream_t stream);

@@ -9,9 +9,14 @@
 // `babyStep` consecutive plaintexts (absent ones flagged), which makes step 2 of the algorithm a single launch of the
 // streaming ct x pt inner-product kernel per query vector.  Query vectors that share an evaluation key are batched
 // through the rotation chains (babyStep - 1 rotations by -1, giantStep - 1 rotations by -babyStep).
+//
+// Many clients, each with its own evaluation key, are answered in groups of up to HECUDA_PNNS_CLIENT_GROUP: every
+// buffer is client-major, each rotation is one key-switching pass over the whole group with a per-client key table,
+// and the matrix streams once per group (the many-clients scan).  A group of one issues the single-client launches.
 #include <algorithm>
 
 #include "capi_internal.hpp"
+#include "wire_codec.hpp"
 
 using namespace hecuda;
 using namespace hecuda::api;
@@ -26,28 +31,39 @@ struct hecuda_pnns_matrix {
 
 namespace {
 
+static_assert(HECUDA_PNNS_CLIENT_GROUP == kKeyTableSize, "one key-table entry per client of a group");
+
 struct RowConsts {
     int rows;
     u64 p[kMaxRows];
 };
 
-// acc[item] (+)= src[item * src_stride]   over ciphertexts of 2 x rows x N
+// Where the items of an accumulate live: they form clients of `per_client` items each, and item k of client j is the
+// ciphertext at acc + j * acc_client + k * (2 x rows x N) and at src + j * src_client + k * src_stride (all in words).
+struct AccLayout {
+    long long per_client, src_stride, src_client, acc_client;
+};
+
+// acc[item] (+)= src[item]   over ciphertexts of 2 x rows x N
 // modes (optional, per item): 0 = leave acc alone, 1 = copy, 2 = add; without modes every item uses `add`
 __global__ void __launch_bounds__(256) accumulate_kernel(u64 *__restrict__ acc, const u64 *__restrict__ src,
-                                                        int64_t src_item_stride, const __grid_constant__ RowConsts c,
-                                                        int n, int add, const signed char *__restrict__ modes) {
+                                                        const __grid_constant__ AccLayout lay, long long item0,
+                                                        const __grid_constant__ RowConsts c, int n, int add,
+                                                        const signed char *__restrict__ modes) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n) return;
+    const long long item = item0 + blockIdx.z;
     if (modes) {
-        const int mode = modes[blockIdx.z];
+        const int mode = modes[item];
         if (mode == 0) return;
         add = mode == 2;
     }
+    const long long client = item / lay.per_client, k = item - client * lay.per_client;
     const int pr = blockIdx.y;
     const int64_t ct_words = (int64_t)2 * c.rows * n;
     const int64_t off = (int64_t)pr * n + e;
-    const u64 v = src[(int64_t)blockIdx.z * src_item_stride + off];
-    u64 *dst = acc + (int64_t)blockIdx.z * ct_words + off;
+    const u64 v = src[client * lay.src_client + k * lay.src_stride + off];
+    u64 *dst = acc + client * lay.acc_client + k * ct_words + off;
     if (add) {
         const u64 p = c.p[pr % c.rows];
         const u64 s = *dst + v;
@@ -57,20 +73,76 @@ __global__ void __launch_bounds__(256) accumulate_kernel(u64 *__restrict__ acc, 
     }
 }
 
-cudaError_t launch_accumulate(const Context &c, int l, u64 *acc, const u64 *src, int64_t src_item_stride, int64_t items,
-                              bool add, cudaStream_t s, const signed char *modes = nullptr) {
+RowConsts row_consts(const Context &c, int l) {
     RowConsts rc;
     const NttRowMap map = c.map_q(l);
     rc.rows = l;
     for (int r = 0; r < l; ++r) rc.p[r] = c.slots[map.slot[r]].dev.p;
+    return rc;
+}
+
+// acc[k] (+)= src[k * src_item_stride] for k < items; per_client > 0 splits the items into clients (AccLayout)
+cudaError_t launch_accumulate(const Context &c, int l, u64 *acc, const u64 *src, int64_t src_item_stride, int64_t items,
+                              bool add, cudaStream_t s, const signed char *modes = nullptr, int64_t per_client = 0,
+                              int64_t src_client_stride = 0, int64_t acc_client_stride = 0) {
+    const RowConsts rc = row_consts(c, l);
+    const AccLayout lay{per_client > 0 ? per_client : std::max<int64_t>(items, 1), src_item_stride, src_client_stride,
+                        acc_client_stride};
     const int threads = c.n >= 256 ? 256 : (c.n < 32 ? 32 : (int)c.n);
-    const int64_t ct_words = (int64_t)2 * l * c.n;
     for (int64_t done = 0; done < items;) {
         const int64_t chunk = std::min<int64_t>(items - done, 65535);
         dim3 grid((unsigned)((c.n + threads - 1) / threads), (unsigned)(2 * l), (unsigned)chunk);
         ++g_kernel_launches;
-        accumulate_kernel<<<grid, threads, 0, s>>>(acc + done * ct_words, src + done * src_item_stride, src_item_stride, rc,
-                                                   (int)c.n, add ? 1 : 0, modes ? modes + done : nullptr);
+        accumulate_kernel<<<grid, threads, 0, s>>>(acc, src, lay, done, rc, (int)c.n, add ? 1 : 0, modes);
+        done += chunk;
+    }
+    return cudaGetLastError();
+}
+
+struct MaskConsts {
+    int rows;
+    u64 p[kMaxRows], mu_hi[kMaxRows], mu_lo[kMaxRows];
+};
+
+// ciphertextEval *= plaintextMask of CiphertextMatrix.extractDenseRow (CiphertextMatrix.swift:322-324) for every query
+// row of every client of a group in one launch: item = j * rows_per_client + r,
+//   y[item] = ct_eval[j * ct_count + index[r]] (.) mask_eval[r]      (Eval, canonical residues)
+// ct_eval: the clients' query ciphertexts after one forward NTT (gathering after the NTT gives the values of NTT after
+// gathering); mask_eval: rows_per_client x L x N.
+__global__ void __launch_bounds__(256) mask_product_kernel(const u64 *__restrict__ ct_eval, const u64 *__restrict__ mask_eval,
+                                                          const int *__restrict__ index, u64 *__restrict__ y,
+                                                          const __grid_constant__ MaskConsts c, int n, int rows_per_client,
+                                                          long long ct_count, long long item0) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const int pr = blockIdx.y, row = pr % c.rows;  // poly * rows + RNS row
+    const long long item = item0 + blockIdx.z, client = item / rows_per_client;
+    const int r = (int)(item - client * rows_per_client);
+    const long long ct_words = 2LL * c.rows * n, off = (long long)pr * n + e;
+    const u64 a = ct_eval[(client * ct_count + index[r]) * ct_words + off];
+    const u64 m = mask_eval[((long long)r * c.rows + row) * n + e];
+    y[item * ct_words + off] = barrett128(mul_wide(a, m), c.p[row], c.mu_hi[row], c.mu_lo[row]);
+}
+
+cudaError_t launch_mask_product(const Context &c, const u64 *ct_eval, int64_t ct_count, const u64 *mask_eval, const int *index,
+                                int64_t rows_per_client, int clients, u64 *y, cudaStream_t s) {
+    MaskConsts mc;
+    const NttRowMap map = c.map_q(c.L);
+    mc.rows = c.L;
+    for (int r = 0; r < c.L; ++r) {
+        const ModSlot &S = c.slots[map.slot[r]].dev;
+        mc.p[r] = S.p;
+        mc.mu_hi[r] = S.mu_hi;
+        mc.mu_lo[r] = S.mu_lo;
+    }
+    const int threads = c.n >= 256 ? 256 : (c.n < 32 ? 32 : (int)c.n);
+    const int64_t items = rows_per_client * clients;
+    for (int64_t done = 0; done < items;) {
+        const int64_t chunk = std::min<int64_t>(items - done, 65535);
+        dim3 grid((unsigned)((c.n + threads - 1) / threads), (unsigned)(2 * c.L), (unsigned)chunk);
+        ++g_kernel_launches;
+        mask_product_kernel<<<grid, threads, 0, s>>>(ct_eval, mask_eval, index, y, mc, (int)c.n, (int)rows_per_client,
+                                                     ct_count, done);
         done += chunk;
     }
     return cudaGetLastError();
@@ -97,83 +169,149 @@ int32_t find_key(const hecuda_evk *k, unsigned element, const u64 **key) {
     return HECUDA_OK;
 }
 
-struct Tmp {
-    cudaStream_t s;
-    std::vector<void *> ptrs;
-    explicit Tmp(cudaStream_t stream) : s(stream) {}
-    ~Tmp() {
-        for (void *p : ptrs) cudaFreeAsync(p, s);
-    }
-    cudaError_t alloc(u64 **out, size_t words) {
-        cudaError_t e = cudaMallocAsync((void **)out, std::max<size_t>(words, 1) * sizeof(u64), s);
-        if (e == cudaSuccess) ptrs.push_back(*out);
-        return e;
-    }
+struct MatrixQuery {
+    int32_t rows;                      // ciphertextMatrix.rowCount
+    const int32_t *ciphertext_index;   // per row
+    const u64 *host_masks;             // rows x N coefficient plaintexts
+    const int32_t *rotate_count;       // per row
+    int32_t column_step;
+    const int32_t *pack_rotations;     // single rotations composing rotateColumnsMultiStep(by: matrix.rowCount)
+    int32_t pack_rotation_count;
 };
 
-int32_t mul_transpose_device(const hecuda_context *h, const hecuda_evk *k, const hecuda_pnns_matrix *m, const u64 *d_vec,
-                             int64_t batch, bool to_single, u64 *d_out, cudaStream_t s) {
+// What the matrix and query shapes fix: S query rows per SIMD row of a packed result, G packing groups, the ciphertexts
+// of one reply, the top packing position and the longest replication chain.
+struct MatrixShape {
+    int64_t S, G, outputs, top;
+    int32_t max_rot;
+};
+MatrixShape matrix_shape(const Context &c, const hecuda_pnns_matrix *m, const MatrixQuery &q) {
+    MatrixShape sh;
+    const int64_t R = q.rows;
+    sh.S = (c.n / 2) / m->row_count;
+    sh.G = sh.S > 0 ? (R + sh.S - 1) / sh.S : 0;
+    sh.outputs = sh.S > 0 ? (sh.G + 1) / 2 : R * m->result_count;
+    sh.top = std::min<int64_t>(sh.S, R) - 1;  // the longest group: positions above it hold nothing
+    sh.max_rot = 0;
+    for (int64_t r = 0; r < R && R > 1; ++r) sh.max_rot = std::max(sh.max_rot, q.rotate_count[r]);
+    return sh;
+}
+
+// The key-switching keys of one client's call, found before anything is enqueued.
+struct PnnsKeys {
+    const u64 *rot1 = nullptr, *rotb = nullptr;  // mulTranspose(vector:): rotateColumns(by: -1), (by: -babyStep)
+    const u64 *step = nullptr, *swap = nullptr;  // extractDenseRow: rotateColumns(by: column_step), swapRows
+    std::vector<const u64 *> pack;              // the single rotations of rotateColumnsMultiStep(by: rowCount)
+};
+int32_t vector_keys(const hecuda_evk *k, int64_t n, const hecuda_pnns_matrix *m, PnnsKeys &keys) {
+    int32_t rc;
+    if (m->baby > 1 && (rc = find_key(k, rotating_columns(-1, n), &keys.rot1))) return rc;
+    if (m->giant > 1 && (rc = find_key(k, rotating_columns(-m->baby, n), &keys.rotb))) return rc;
+    return HECUDA_OK;
+}
+int32_t matrix_keys(const hecuda_evk *k, int64_t n, const hecuda_pnns_matrix *m, const MatrixQuery &q, const MatrixShape &sh,
+                    PnnsKeys &keys) {
+    int32_t rc;
+    if (q.rows > 1) {
+        if (sh.max_rot > 0 && (rc = find_key(k, rotating_columns(q.column_step, n), &keys.step))) return rc;
+        if ((rc = find_key(k, (unsigned)(2 * n - 1), &keys.swap))) return rc;
+    }
+    if ((rc = vector_keys(k, n, m, keys))) return rc;
+    keys.pack.assign((size_t)q.pack_rotation_count, nullptr);
+    for (int32_t i = 0; i < q.pack_rotation_count && sh.S > 1; ++i)
+        if ((rc = find_key(k, rotating_columns(q.pack_rotations[i], n), &keys.pack[(size_t)i]))) return rc;
+    return HECUDA_OK;
+}
+
+// One rotation's keys for a group: client j's pick(keys[j]) for its per_client consecutive items
+template <class Pick>
+KsKeyTable key_table(const PnnsKeys *keys, int clients, int64_t per_client, Pick pick) {
+    KsKeyTable t{};
+    for (int j = 0; j < clients; ++j) t.key[j] = pick(keys[j]);
+    t.items_per_client = per_client;
+    return t;
+}
+
+// batched applyGalois over `items` contiguous ciphertexts, chunked by the scratch size; with clients > 1 every
+// launch switches each client's items with the client's key (table)
+int32_t galois_batch(const Context &c, u64 *scratch, int64_t chunk, KsKeyTable table, int clients, unsigned element,
+                     const u64 *in, u64 *out, int64_t items, cudaStream_t s) {
+    const size_t ct_words = (size_t)2 * c.L * c.n;
+    for (int64_t done = 0; done < items; done += chunk) {
+        const int64_t part = std::min<int64_t>(chunk, items - done);
+        table.item0 = done;
+        cudaError_t e = apply_galois_chunk(c, scratch, table.key[0], in + ct_words * done, c.L, element, out + ct_words * done,
+                                           part, s, clients > 1 ? &table : nullptr);
+        if (e != cudaSuccess) return cuda_fail(e, "applyGalois");
+    }
+    return HECUDA_OK;
+}
+
+// PlaintextMatrix.mulTranspose(vector:using:) for `clients` clients' `batch` query vectors each: d_vec = clients x batch
+// ciphertexts (Coeff), client j with keys[j]; d_out = clients x batch x results ciphertexts.  Every stage is one pass
+// over all the vectors; a single client issues the single-client launches (one scan per vector).
+int32_t mul_transpose_device(const hecuda_context *h, const PnnsKeys *keys, int clients, const hecuda_pnns_matrix *m,
+                             const u64 *d_vec, int64_t batch, bool to_single, u64 *d_out, cudaStream_t s) {
     const Context &c = *h->ctx;
     const int L = c.L;
     const int64_t n = c.n;
     const size_t ct_words = (size_t)2 * L * n;
     const int baby = m->baby, giant = m->giant;
-    const int64_t results = m->result_count;
-    const u64 *key1 = nullptr, *keyb = nullptr;
+    const int64_t results = m->result_count, vectors = batch * clients;
     const unsigned e1 = n > 2 ? rotating_columns(-1, n) : 0, eb = rotating_columns(-baby, n);
     int32_t rc;
-    if (baby > 1 && (rc = find_key(k, e1, &key1))) return rc;
-    if (giant > 1 && (rc = find_key(k, eb, &keyb))) return rc;
-    Tmp tmp(s);
+    StreamBuffers tmp(s);
     u64 *states = nullptr, *rotated = nullptr, *ip = nullptr, *acc[2] = {nullptr, nullptr}, *scratch = nullptr, *ms = nullptr;
     const int64_t gal_items = std::max<int64_t>(batch, batch * results);
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, gal_items));
-    CK(tmp.alloc(&states, ct_words * baby * batch));
-    CK(tmp.alloc(&rotated, ct_words * baby * batch));
-    CK(tmp.alloc(&ip, ct_words * results * giant * batch));
-    CK(tmp.alloc(&acc[0], ct_words * results * batch));
-    CK(tmp.alloc(&acc[1], ct_words * results * batch));
+    // items per applyGalois pass: grows with the number of clients, so the launch count does not
+    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, gal_items)) * clients;
+    CK(tmp.alloc(&states, ct_words * baby * vectors));
+    CK(tmp.alloc(&rotated, ct_words * baby * vectors));
+    CK(tmp.alloc(&ip, ct_words * results * giant * vectors));
+    CK(tmp.alloc(&acc[0], ct_words * results * vectors));
+    CK(tmp.alloc(&acc[1], ct_words * results * vectors));
     CK(tmp.alloc(&scratch, galois_scratch_words(c, L) * (size_t)chunk));
-    CK(tmp.alloc(&ms, ct_words * results * batch));
+    CK(tmp.alloc(&ms, ct_words * results * vectors));
     cudaError_t e;
-    // 1) v_j = theta^j(v): states[j][b]                                    (MatrixMultiplication.swift:180-189)
-    CK(cudaMemcpyAsync(states, d_vec, ct_words * batch * sizeof(u64), cudaMemcpyDeviceToDevice, s));
+    // 1) v_j = theta^j(v): states[j][vector]                                (MatrixMultiplication.swift:180-189)
+    CK(cudaMemcpyAsync(states, d_vec, ct_words * vectors * sizeof(u64), cudaMemcpyDeviceToDevice, s));
+    const KsKeyTable key1 = key_table(keys, clients, batch, [](const PnnsKeys &k) { return k.rot1; });
     for (int j = 1; j < baby; ++j)
-        for (int64_t done = 0; done < batch; done += chunk) {
-            const int64_t items = std::min<int64_t>(chunk, batch - done);
-            if ((e = apply_galois_chunk(c, scratch, key1, states + ct_words * ((j - 1) * batch + done), L, e1,
-                                        states + ct_words * (j * batch + done), items, s)) != cudaSuccess)
-                return cuda_fail(e, "rotateColumns");
-        }
-    // convertToEvalFormat (:190-193), then [j][b] -> [b][j] so that each vector's states are consecutive
+        if ((rc = galois_batch(c, scratch, chunk, key1, clients, e1, states + ct_words * (j - 1) * vectors,
+                               states + ct_words * j * vectors, vectors, s)))
+            return rc;
+    // convertToEvalFormat (:190-193), then [j][vector] -> [vector][j] so that each vector's states are consecutive
     const NttRowMap map = c.map_q(L);
-    if ((e = launch_ntt_forward(c, map, states, states, (int64_t)baby * batch * 2 * L, s)) != cudaSuccess) return cuda_fail(e, "ntt");
-    if (batch == 1) {
+    if ((e = launch_ntt_forward(c, map, states, states, (int64_t)baby * vectors * 2 * L, s)) != cudaSuccess) return cuda_fail(e, "ntt");
+    if (vectors == 1) {
         std::swap(states, rotated);
     } else {
         for (int j = 0; j < baby; ++j)
-            CK(cudaMemcpy2DAsync(rotated + ct_words * j, ct_words * baby * sizeof(u64), states + ct_words * j * batch,
-                                 ct_words * sizeof(u64), ct_words * sizeof(u64), (size_t)batch, cudaMemcpyDeviceToDevice, s));
+            CK(cudaMemcpy2DAsync(rotated + ct_words * j, ct_words * baby * sizeof(u64), states + ct_words * j * vectors,
+                                 ct_words * sizeof(u64), ct_words * sizeof(u64), (size_t)vectors, cudaMemcpyDeviceToDevice, s));
     }
     // 2) w_k: one inner product per (result ciphertext, giant step)                         (:197-216)
-    for (int64_t b = 0; b < batch; ++b)
-        if ((e = launch_inner_product_plain(c, rotated + ct_words * baby * b, 2, L, baby, m->d_plain, m->d_present,
-                                            ip + ct_words * results * giant * b, results * giant, s)) != cudaSuccess)
+    if (clients == 1) {
+        for (int64_t b = 0; b < batch; ++b)
+            if ((e = launch_inner_product_plain(c, rotated + ct_words * baby * b, 2, L, baby, m->d_plain, m->d_present,
+                                                ip + ct_words * results * giant * b, results * giant, s)) != cudaSuccess)
+                return cuda_fail(e, "innerProduct(ciphertexts:plaintexts:)");
+    } else {  // the matrix streams once for the group: each vector's rotated states are one "client" of the scan
+        if ((e = launch_inner_product_plain_clients(c, rotated, (int64_t)ct_words * baby, (int)vectors, L, baby, m->d_plain,
+                                                    nullptr, m->d_present, ip, (int64_t)ct_words * results * giant,
+                                                    results * giant, s)) != cudaSuccess)
             return cuda_fail(e, "innerProduct(ciphertexts:plaintexts:)");
-    if ((e = launch_ntt_inverse(c, map, ip, ip, batch * results * giant * 2 * L, kScalePlain, s)) != cudaSuccess)
+    }
+    if ((e = launch_ntt_inverse(c, map, ip, ip, vectors * results * giant * 2 * L, kScalePlain, s)) != cudaSuccess)
         return cuda_fail(e, "ntt");
     // 3) rotateColumnsAndSum(by: -babyStep): Horner over the giant steps, all (vector, result) pairs at once (:218-226)
-    const int64_t items = batch * results;
+    const int64_t items = vectors * results;
+    const KsKeyTable keyb = key_table(keys, clients, batch * results, [](const PnnsKeys &k) { return k.rotb; });
     int cur = 0;
     if ((e = launch_accumulate(c, L, acc[cur], ip + ct_words * (giant - 1), (int64_t)ct_words * giant, items, false, s)) != cudaSuccess)
         return cuda_fail(e, "sum");
     for (int g = giant - 2; g >= 0; --g) {
-        for (int64_t done = 0; done < items; done += chunk) {
-            const int64_t part = std::min<int64_t>(chunk, items - done);
-            if ((e = apply_galois_chunk(c, scratch, keyb, acc[cur] + ct_words * done, L, eb, acc[cur ^ 1] + ct_words * done,
-                                        part, s)) != cudaSuccess)
-                return cuda_fail(e, "rotateColumns");
-        }
+        if ((rc = galois_batch(c, scratch, chunk, keyb, clients, eb, acc[cur], acc[cur ^ 1], items, s))) return rc;
         cur ^= 1;
         if ((e = launch_accumulate(c, L, acc[cur], ip + ct_words * g, (int64_t)ct_words * giant, items, true, s)) != cudaSuccess)
             return cuda_fail(e, "sum");
@@ -192,161 +330,147 @@ int32_t mul_transpose_device(const hecuda_context *h, const hecuda_evk *k, const
     return HECUDA_OK;
 }
 
-// batched applyGalois over `items` contiguous ciphertexts, chunked by the scratch size
-int32_t galois_batch(const Context &c, u64 *scratch, int64_t chunk, const u64 *key, unsigned element, const u64 *in, u64 *out,
-                     int64_t items, cudaStream_t s) {
-    const size_t ct_words = (size_t)2 * c.L * c.n;
-    for (int64_t done = 0; done < items; done += chunk) {
-        const int64_t part = std::min<int64_t>(chunk, items - done);
-        cudaError_t e = apply_galois_chunk(c, scratch, key, in + ct_words * done, c.L, element, out + ct_words * done, part, s);
-        if (e != cudaSuccess) return cuda_fail(e, "applyGalois");
-    }
-    return HECUDA_OK;
-}
-
-struct MatrixQuery {
-    int32_t rows;                      // ciphertextMatrix.rowCount
-    const int32_t *ciphertext_index;   // per row
-    const u64 *host_masks;             // rows x N coefficient plaintexts
-    const int32_t *rotate_count;       // per row
-    int32_t column_step;
-    const int32_t *pack_rotations;     // single rotations composing rotateColumnsMultiStep(by: matrix.rowCount)
-    int32_t pack_rotation_count;
-};
-
 // PlaintextMatrix.mulTranspose(matrix:using:) (MatrixMultiplication.swift:236-298) with CiphertextMatrix.extractDenseRow
-// (CiphertextMatrix.swift:245-352) batched over all query rows.
-int32_t mul_transpose_matrix_device(const hecuda_context *h, const hecuda_evk *k, const hecuda_pnns_matrix *m,
-                                    const u64 *d_cts, const MatrixQuery &q, bool to_single, u64 *d_out, int64_t out_capacity,
-                                    int64_t *out_count, cudaStream_t s) {
+// (CiphertextMatrix.swift:245-352) batched over all query rows, for `clients` clients' queries of the same shape:
+// d_cts = clients x ct_count ciphertexts (Coeff), client j with keys[j]; d_out = clients x outputs ciphertexts.
+int32_t mul_transpose_matrix_device(const hecuda_context *h, const PnnsKeys *keys, int clients, const hecuda_pnns_matrix *m,
+                                    const u64 *d_cts, int64_t ct_count, const MatrixQuery &q, bool to_single, u64 *d_out,
+                                    cudaStream_t s) {
     const Context &c = *h->ctx;
     const int L = c.L;
-    const int64_t n = c.n, R = q.rows, results = m->result_count;
+    const int64_t n = c.n, R = q.rows, results = m->result_count, rows = R * clients;
     const size_t ct_words = (size_t)2 * L * n;
-    const int64_t per_simd_row = (n / 2) / m->row_count;
-    const int64_t S = per_simd_row, G = S > 0 ? (R + S - 1) / S : 0;
-    const int64_t outputs = S > 0 ? (G + 1) / 2 : R * results;
-    *out_count = outputs;
-    if (outputs > out_capacity) return fail(HECUDA_ERR_INVALID_ARGUMENT, "output buffer too small: needs " + std::to_string(outputs) + " ciphertexts");
-    Tmp tmp(s);
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, R));
+    const MatrixShape sh = matrix_shape(c, m, q);
+    const int64_t S = sh.S, G = sh.G, outputs = sh.outputs, top = sh.top;
+    StreamBuffers tmp(s);
+    const int64_t per_client_chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, R)), chunk = per_client_chunk * clients;
     u64 *x = nullptr, *y = nullptr, *z = nullptr, *scratch = nullptr, *inner = nullptr, *masks = nullptr, *mask_eval = nullptr;
     signed char *d_modes = nullptr;
-    CK(tmp.alloc(&x, ct_words * R));
-    CK(tmp.alloc(&y, ct_words * R));
-    CK(tmp.alloc(&z, ct_words * R));
+    CK(tmp.alloc(&x, ct_words * rows));
+    CK(tmp.alloc(&y, ct_words * rows));
+    CK(tmp.alloc(&z, ct_words * rows));
     CK(tmp.alloc(&scratch, galois_scratch_words(c, L) * (size_t)chunk));
-    CK(tmp.alloc(&inner, ct_words * R * results));
+    CK(tmp.alloc(&inner, ct_words * rows * results));
     const NttRowMap map = c.map_q(L);
     const unsigned swap_element = (unsigned)(2 * n - 1);
     cudaError_t e;
     int32_t rc;
-    // mode tables: replication steps (extractDenseRow) then packing positions
-    int32_t max_rot = 0;
-    for (int64_t r = 0; r < R && R > 1; ++r) max_rot = std::max(max_rot, q.rotate_count[r]);
+    // mode tables, one row of the group's items per step: replication steps (extractDenseRow) then packing positions
     std::vector<signed char> modes;
-    for (int32_t t = 1; t <= max_rot; ++t)
-        for (int64_t r = 0; r < R; ++r) modes.push_back(t <= q.rotate_count[r] ? 2 : 0);
+    for (int32_t t = 1; t <= sh.max_rot; ++t)
+        for (int j = 0; j < clients; ++j)
+            for (int64_t r = 0; r < R; ++r) modes.push_back(t <= q.rotate_count[r] ? 2 : 0);
     const size_t pack_modes_offset = modes.size();
-    const int64_t top = std::min<int64_t>(S, R) - 1;  // the longest group: positions above it hold nothing
     for (int64_t p = top; p >= 0 && S > 0; --p)
-        for (int64_t g = 0; g < G; ++g) {
-            const int64_t size = std::min<int64_t>(S, R - g * S);
-            modes.push_back(p == size - 1 ? 1 : (p < size - 1 ? 2 : 0));
-        }
-    CK(cudaMallocAsync((void **)&d_modes, std::max<size_t>(modes.size(), 8), s));
-    tmp.ptrs.push_back(d_modes);
+        for (int j = 0; j < clients; ++j)
+            for (int64_t g = 0; g < G; ++g) {
+                const int64_t size = std::min<int64_t>(S, R - g * S);
+                modes.push_back(p == size - 1 ? 1 : (p < size - 1 ? 2 : 0));
+            }
+    CK(tmp.alloc_bytes((void **)&d_modes, modes.size()));
     if (!modes.empty()) CK(cudaMemcpyAsync(d_modes, modes.data(), modes.size(), cudaMemcpyHostToDevice, s));
     if (R == 1) {  // extractDenseRow is the identity for a single row (:263-265)
-        CK(cudaMemcpyAsync(y, d_cts, ct_words * sizeof(u64), cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpy2DAsync(y, ct_words * sizeof(u64), d_cts, ct_words * ct_count * sizeof(u64), ct_words * sizeof(u64),
+                             (size_t)clients, cudaMemcpyDeviceToDevice, s));
     } else {
-        const u64 *key_step = nullptr, *key_swap = nullptr;
         const unsigned step_element = rotating_columns(q.column_step, n);
-        if (max_rot > 0 && (rc = find_key(k, step_element, &key_step))) return rc;
-        if ((rc = find_key(k, swap_element, &key_swap))) return rc;
         CK(tmp.alloc(&masks, (size_t)n * R));
         CK(tmp.alloc(&mask_eval, (size_t)L * n * R));
         CK(cudaMemcpyAsync(masks, q.host_masks, (size_t)n * R * sizeof(u64), cudaMemcpyHostToDevice, s));
-        for (int64_t r = 0; r < R; ++r)
-            CK(cudaMemcpyAsync(x + ct_words * r, d_cts + ct_words * q.ciphertext_index[r], ct_words * sizeof(u64),
-                               cudaMemcpyDeviceToDevice, s));
         // ciphertextEval *= plaintextMask (:322-324)
-        if ((e = launch_ntt_forward(c, map, x, x, R * 2 * L, s)) != cudaSuccess) return cuda_fail(e, "ntt");
-        if ((e = launch_plaintext_to_eval(c, masks, L, mask_eval, R, s)) != cudaSuccess) return cuda_fail(e, "plaintext_to_eval");
-        for (int64_t r = 0; r < R; ++r)
-            if ((e = launch_inner_product_plain(c, x + ct_words * r, 2, L, 1, mask_eval + (size_t)L * n * r, nullptr,
-                                                y + ct_words * r, 1, s)) != cudaSuccess)
+        if (clients == 1) {
+            for (int64_t r = 0; r < R; ++r)
+                CK(cudaMemcpyAsync(x + ct_words * r, d_cts + ct_words * q.ciphertext_index[r], ct_words * sizeof(u64),
+                                   cudaMemcpyDeviceToDevice, s));
+            if ((e = launch_ntt_forward(c, map, x, x, R * 2 * L, s)) != cudaSuccess) return cuda_fail(e, "ntt");
+            if ((e = launch_plaintext_to_eval(c, masks, L, mask_eval, R, s)) != cudaSuccess) return cuda_fail(e, "plaintext_to_eval");
+            for (int64_t r = 0; r < R; ++r)
+                if ((e = launch_inner_product_plain(c, x + ct_words * r, 2, L, 1, mask_eval + (size_t)L * n * r, nullptr,
+                                                    y + ct_words * r, 1, s)) != cudaSuccess)
+                    return cuda_fail(e, "multiply by mask");
+        } else {  // each client's query ciphertexts through one forward NTT, then every row's product in one launch
+            u64 *ct_eval = nullptr;
+            int *d_index = nullptr;
+            CK(tmp.alloc(&ct_eval, ct_words * ct_count * clients));
+            CK(tmp.alloc_bytes((void **)&d_index, sizeof(int) * (size_t)R));
+            CK(cudaMemcpyAsync(d_index, q.ciphertext_index, sizeof(int) * (size_t)R, cudaMemcpyHostToDevice, s));
+            if ((e = launch_ntt_forward(c, map, d_cts, ct_eval, ct_count * clients * 2 * L, s)) != cudaSuccess) return cuda_fail(e, "ntt");
+            if ((e = launch_plaintext_to_eval(c, masks, L, mask_eval, R, s)) != cudaSuccess) return cuda_fail(e, "plaintext_to_eval");
+            if ((e = launch_mask_product(c, ct_eval, ct_count, mask_eval, d_index, R, clients, y, s)) != cudaSuccess)
                 return cuda_fail(e, "multiply by mask");
-        if ((e = launch_ntt_inverse(c, map, y, y, R * 2 * L, kScalePlain, s)) != cudaSuccess) return cuda_fail(e, "ntt");
+        }
+        if ((e = launch_ntt_inverse(c, map, y, y, rows * 2 * L, kScalePlain, s)) != cudaSuccess) return cuda_fail(e, "ntt");
         // replicate across one SIMD row: rotate the copy, add where the row still needs copies (:331-336)
+        const KsKeyTable key_step = key_table(keys, clients, R, [](const PnnsKeys &k) { return k.step; });
         const u64 *copy = y;
         u64 *ping[2] = {x, z};
-        for (int32_t t = 1; t <= max_rot; ++t) {
+        for (int32_t t = 1; t <= sh.max_rot; ++t) {
             u64 *dst = ping[t & 1];
-            if ((rc = galois_batch(c, scratch, chunk, key_step, step_element, copy, dst, R, s))) return rc;
+            if ((rc = galois_batch(c, scratch, chunk, key_step, clients, step_element, copy, dst, rows, s))) return rc;
             copy = dst;
-            if ((e = launch_accumulate(c, L, y, copy, (int64_t)ct_words, R, true, s, d_modes + (size_t)(t - 1) * R)) != cudaSuccess)
+            if ((e = launch_accumulate(c, L, y, copy, (int64_t)ct_words, rows, true, s, d_modes + (size_t)(t - 1) * rows)) != cudaSuccess)
                 return cuda_fail(e, "sum");
         }
         // both SIMD rows: ciphertext += swapRows(ciphertext) (:342-345)
-        if ((rc = galois_batch(c, scratch, chunk, key_swap, swap_element, y, x, R, s))) return rc;
-        if ((e = launch_accumulate(c, L, y, x, (int64_t)ct_words, R, true, s)) != cudaSuccess) return cuda_fail(e, "sum");
+        const KsKeyTable key_swap = key_table(keys, clients, R, [](const PnnsKeys &k) { return k.swap; });
+        if ((rc = galois_batch(c, scratch, chunk, key_swap, clients, swap_element, y, x, rows, s))) return rc;
+        if ((e = launch_accumulate(c, L, y, x, (int64_t)ct_words, rows, true, s)) != cudaSuccess) return cuda_fail(e, "sum");
     }
-    if ((rc = mul_transpose_device(h, k, m, y, R, false, inner, s))) return rc;
+    if ((rc = mul_transpose_device(h, keys, clients, m, y, R, false, inner, s))) return rc;
     u64 *final_cts = inner;
-    if (S > 0) {  // pack the result columns (:262-283); here results == 1
+    if (S > 0) {  // pack the result columns (:262-283); here results == 1, so client j's products are inner[j * R ...]
         u64 *acc[2] = {x, y};
         int cur = 0;
-        CK(cudaMemsetAsync(acc[0], 0, ct_words * G * sizeof(u64), s));
-        std::vector<std::pair<unsigned, const u64 *>> rotations;
-        for (int32_t i = 0; i < q.pack_rotation_count; ++i) {
-            const unsigned element = rotating_columns(q.pack_rotations[i], n);
-            const u64 *key = nullptr;
-            if (S > 1 && (rc = find_key(k, element, &key))) return rc;
-            rotations.push_back({element, key});
-        }
-        const int64_t gchunk = std::max<int64_t>(1, std::min<int64_t>(chunk, G));
+        CK(cudaMemsetAsync(acc[0], 0, ct_words * G * clients * sizeof(u64), s));
+        const int64_t gchunk = std::max<int64_t>(1, std::min<int64_t>(per_client_chunk, G)) * clients;
         size_t mode_row = pack_modes_offset;
-        for (int64_t p = top; p >= 0; --p, mode_row += (size_t)G) {
+        for (int64_t p = top; p >= 0; --p, mode_row += (size_t)(G * clients)) {
             if (p < top)
-                for (const auto &rot : rotations) {  // rotateColumnsMultiStep(by: dimensions.rowCount)
-                    if ((rc = galois_batch(c, scratch, gchunk, rot.second, rot.first, acc[cur], acc[cur ^ 1], G, s))) return rc;
+                for (int32_t i = 0; i < q.pack_rotation_count; ++i) {  // rotateColumnsMultiStep(by: dimensions.rowCount)
+                    const KsKeyTable key = key_table(keys, clients, G, [i](const PnnsKeys &k) { return k.pack[(size_t)i]; });
+                    if ((rc = galois_batch(c, scratch, gchunk, key, clients, rotating_columns(q.pack_rotations[i], n), acc[cur],
+                                           acc[cur ^ 1], G * clients, s)))
+                        return rc;
                     cur ^= 1;
                 }
-            if ((e = launch_accumulate(c, L, acc[cur], inner + ct_words * p, (int64_t)ct_words * S, G, true, s,
-                                       d_modes + mode_row)) != cudaSuccess)
+            if ((e = launch_accumulate(c, L, acc[cur], inner + ct_words * p, (int64_t)ct_words * S, G * clients, true, s,
+                                       d_modes + mode_row, G, (int64_t)ct_words * R, (int64_t)ct_words * G)) != cudaSuccess)
                 return cuda_fail(e, "sum");
         }
         // swapRowsAndAdd(swapping: packedRows[1], addingTo: packedRows[0]) for every full pair (:277-281)
         const int64_t pairs = G / 2;
         u64 *packed = z;
-        if ((e = launch_accumulate(c, L, packed, acc[cur], (int64_t)ct_words * 2, outputs, false, s)) != cudaSuccess)
+        if ((e = launch_accumulate(c, L, packed, acc[cur], (int64_t)ct_words * 2, outputs * clients, false, s, nullptr, outputs,
+                                   (int64_t)ct_words * G, (int64_t)ct_words * outputs)) != cudaSuccess)
             return cuda_fail(e, "copy");
         if (pairs > 0) {
-            const u64 *key_swap = nullptr;
-            if ((rc = find_key(k, swap_element, &key_swap))) return rc;
             u64 *odd = acc[cur ^ 1];
-            if ((e = launch_accumulate(c, L, odd, acc[cur] + ct_words, (int64_t)ct_words * 2, pairs, false, s)) != cudaSuccess)
+            if ((e = launch_accumulate(c, L, odd, acc[cur] + ct_words, (int64_t)ct_words * 2, pairs * clients, false, s, nullptr,
+                                       pairs, (int64_t)ct_words * G, (int64_t)ct_words * pairs)) != cudaSuccess)
                 return cuda_fail(e, "copy");
-            if ((rc = galois_batch(c, scratch, std::max<int64_t>(1, std::min<int64_t>(chunk, pairs)), key_swap, swap_element, odd,
-                                   inner, pairs, s)))
+            const KsKeyTable key_swap = key_table(keys, clients, pairs, [](const PnnsKeys &k) { return k.swap; });
+            if ((rc = galois_batch(c, scratch, std::max<int64_t>(1, std::min<int64_t>(per_client_chunk, pairs)) * clients, key_swap,
+                                   clients, swap_element, odd, inner, pairs * clients, s)))
                 return rc;
-            if ((e = launch_accumulate(c, L, packed, inner, (int64_t)ct_words, pairs, true, s)) != cudaSuccess) return cuda_fail(e, "sum");
+            if ((e = launch_accumulate(c, L, packed, inner, (int64_t)ct_words, pairs * clients, true, s, nullptr, pairs,
+                                       (int64_t)ct_words * pairs, (int64_t)ct_words * outputs)) != cudaSuccess)
+                return cuda_fail(e, "sum");
         }
         final_cts = packed;
     }
+    const int64_t replies = outputs * clients;
     if (!to_single || L == 1) {
-        CK(cudaMemcpyAsync(d_out, final_cts, ct_words * outputs * sizeof(u64), cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpyAsync(d_out, final_cts, ct_words * replies * sizeof(u64), cudaMemcpyDeviceToDevice, s));
     } else {
         const u64 *src = final_cts;
         u64 *spare[2] = {nullptr, nullptr};  // sized for the outputs (more than R ciphertexts when rowCount > N)
-        CK(tmp.alloc(&spare[0], ct_words * outputs));
-        CK(tmp.alloc(&spare[1], ct_words * outputs));
+        CK(tmp.alloc(&spare[0], ct_words * replies));
+        CK(tmp.alloc(&spare[1], ct_words * replies));
         int which = 0;
         for (int l = L; l > 1; --l) {
             u64 *dst = l == 2 ? d_out : spare[which];
             which ^= 1;
-            if ((e = launch_mod_switch(c, src, l, dst, outputs * 2, s)) != cudaSuccess) return cuda_fail(e, "modSwitchDown");
+            if ((e = launch_mod_switch(c, src, l, dst, replies * 2, s)) != cudaSuccess) return cuda_fail(e, "modSwitchDown");
             src = dst;
         }
     }
@@ -362,6 +486,104 @@ int32_t check_args(const hecuda_context *h, const hecuda_evk *k, const hecuda_pn
     if (!k) return fail(HECUDA_ERR_MISSING_KEY, "missingGaloisKey");
     if (k->owner != h) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidContext: evaluation key belongs to another context");
     if (batch < 0 || (batch && (!vectors || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: null buffer");
+    return HECUDA_OK;
+}
+
+// the query-shape checks of mulTranspose(matrix:), common to the single-client and the many-clients calls
+int32_t check_matrix_query(const Context &c, int32_t ciphertext_count, const MatrixQuery &q) {
+    if (ciphertext_count < 1 || q.rows < 1 || q.pack_rotation_count < 0 || (q.pack_rotation_count && !q.pack_rotations))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
+    if (q.rows > 1) {
+        if (!q.ciphertext_index || !q.host_masks || !q.rotate_count) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null row descriptors");
+        if (q.column_step < 1 || q.column_step > c.n / 2) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
+        for (int32_t r = 0; r < q.rows; ++r)
+            if (q.ciphertext_index[r] < 0 || q.ciphertext_index[r] >= ciphertext_count || q.rotate_count[r] < 0)
+                return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongCiphertextCount: row descriptor out of range");
+    }
+    return HECUDA_OK;
+}
+
+int32_t check_capacity(const MatrixShape &sh, int64_t out_capacity, int64_t *out_count) {
+    *out_count = sh.outputs;
+    if (sh.outputs > out_capacity)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "output buffer too small: needs " + std::to_string(sh.outputs) + " ciphertexts");
+    return HECUDA_OK;
+}
+
+// Every client checked, and every Galois key of every client found, before anything is enqueued: a failure leaves
+// `out` untouched, and its message names the client by its index in the call.
+int32_t check_clients(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count, const hecuda_pnns_matrix *m,
+                      const void *cts, int32_t ciphertext_count, const MatrixQuery &q, const void *out, int64_t out_capacity,
+                      int64_t *out_count, std::vector<PnnsKeys> &keys) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (!evks || !cts || !out || !out_count) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (client_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "client_count must be at least 1");
+    if (!m || m->owner != h) return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongContext: plaintext matrix belongs to another context");
+    const Context &c = *h->ctx;
+    if ((rc = check_matrix_query(c, ciphertext_count, q))) return rc;
+    const MatrixShape sh = matrix_shape(c, m, q);
+    if ((rc = check_capacity(sh, out_capacity, out_count))) return rc;
+    keys.assign((size_t)client_count, PnnsKeys{});
+    for (int32_t j = 0; j < client_count; ++j) {
+        const std::string who = "client " + std::to_string(j) + ": ";
+        if (!evks[j]) return fail(HECUDA_ERR_MISSING_KEY, who + "missingGaloisKey");
+        if (evks[j]->owner != h)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, who + "invalidContext: evaluation key belongs to another context");
+        if ((rc = matrix_keys(evks[j], c.n, m, q, sh, keys[(size_t)j]))) return fail(rc, who + last_error_cstr());
+    }
+    return HECUDA_OK;
+}
+
+// Server.computeResponse for every client of a call through one workspace stream, group by group: stage a group's
+// queries (words, or seeded bytes expanded on the device when `wc` is given), answer the group, copy its replies back
+// (packed by `wc`).  Temporaries are sized for one group.  Reply j of client c goes to out + (c * out_capacity + j)
+// replies.
+int32_t respond_clients(const hecuda_context *h, const std::vector<PnnsKeys> &keys, const hecuda_pnns_matrix *m,
+                        const MatrixQuery &q, int32_t ciphertext_count, int64_t outputs, const void *queries,
+                        const uint8_t *query_seeds, WireCodec *wc, void *out, int64_t out_capacity) {
+    const Context &c = *h->ctx;
+    const int32_t client_count = (int32_t)keys.size();
+    WsGuard g(h);
+    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    cudaStream_t s = g.w->stream;
+    StreamBuffers tmp(s);
+    const int group = std::min<int32_t>(HECUDA_PNNS_CLIENT_GROUP, client_count);
+    const size_t query_words = (size_t)2 * c.L * c.n * ciphertext_count;
+    const size_t reply_bytes = wc ? wc->reply_bytes() : (size_t)2 * c.n * sizeof(u64);
+    const size_t poly0_bytes = wc ? wc->query_bytes * ciphertext_count : 0, seed_bytes = (size_t)32 * ciphertext_count;
+    u64 *d_query = nullptr, *d_reply = nullptr;
+    unsigned char *d_poly0 = nullptr, *d_seeds = nullptr;
+    CK(tmp.alloc(&d_query, query_words * group));
+    CK(tmp.alloc(&d_reply, (size_t)2 * c.n * outputs * group));
+    if (wc) {
+        CK(tmp.alloc_bytes((void **)&d_poly0, poly0_bytes * group));
+        CK(tmp.alloc_bytes((void **)&d_seeds, seed_bytes * group));
+        CK(wc->alloc(tmp, c, outputs * group));
+    }
+    DrainOnExit drain{s};  // copies of the caller's buffers are in flight on `s` from here on
+    for (int32_t first = 0; first < client_count; first += group) {
+        const int clients = std::min<int32_t>(group, client_count - first);
+        if (wc) {  // Query.ciphertexts arrive as SerializedCiphertext.seeded (SerializedCiphertext.swift:41-49)
+            CK(cudaMemcpyAsync(d_poly0, (const uint8_t *)queries + poly0_bytes * first, poly0_bytes * clients, cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(d_seeds, query_seeds + seed_bytes * first, seed_bytes * clients, cudaMemcpyHostToDevice, s));
+            cudaError_t e = expand_seeded_device(c, c.L, d_poly0, d_seeds, d_query, (int64_t)ciphertext_count * clients, s);
+            if (e != cudaSuccess) return cuda_fail(e, "expand seeded query");
+        } else {
+            CK(cudaMemcpyAsync(d_query, (const u64 *)queries + query_words * first, query_words * clients * sizeof(u64),
+                               cudaMemcpyHostToDevice, s));
+        }
+        int32_t rc = mul_transpose_matrix_device(h, keys.data() + first, clients, m, d_query, ciphertext_count, q, true, d_reply, s);
+        if (rc) return rc;
+        const void *replies = d_reply;
+        if (wc) {  // ApplicationProtobuf/PnnsConversionApi.swift:48: serialized forDecryption
+            if ((rc = wc->pack(c, d_reply, outputs * clients, s))) return rc;
+            replies = wc->reply;
+        }
+        CK(cudaMemcpy2DAsync((uint8_t *)out + reply_bytes * out_capacity * first, reply_bytes * out_capacity, replies,
+                             reply_bytes * outputs, reply_bytes * outputs, (size_t)clients, cudaMemcpyDeviceToHost, s));
+    }
+    CK(wait_stream(s));
     return HECUDA_OK;
 }
 
@@ -455,7 +677,10 @@ int32_t hecuda_pnns_mul_transpose_vector_device(const hecuda_context *h, const h
                                                 uint64_t *out, void *stream) {
     int32_t rc = check_args(h, k, m, vectors, batch, out);
     if (rc || batch == 0) return rc;
-    return mul_transpose_device(h, k, m, (const u64 *)vectors, batch, mod_switch_to_single != 0, (u64 *)out, (cudaStream_t)stream);
+    PnnsKeys keys;
+    if ((rc = vector_keys(k, h->ctx->n, m, keys))) return rc;
+    return mul_transpose_device(h, &keys, 1, m, (const u64 *)vectors, batch, mod_switch_to_single != 0, (u64 *)out,
+                                (cudaStream_t)stream);
 }
 
 int32_t hecuda_pnns_mul_transpose_vector(const hecuda_context *h, const hecuda_evk *k, const hecuda_pnns_matrix *m,
@@ -463,18 +688,20 @@ int32_t hecuda_pnns_mul_transpose_vector(const hecuda_context *h, const hecuda_e
                                          uint64_t *out) {
     int32_t rc = check_args(h, k, m, vectors, batch, out);
     if (rc || batch == 0) return rc;
+    PnnsKeys keys;
+    if ((rc = vector_keys(k, h->ctx->n, m, keys))) return rc;
     WsGuard g(h);
     if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
     const Context &c = *h->ctx;
     const size_t ct_words = (size_t)2 * c.L * c.n;
     const size_t out_words = (size_t)2 * (mod_switch_to_single ? 1 : c.L) * c.n * m->result_count * batch;
     cudaStream_t s = g.w->stream;
-    Tmp tmp(s);
+    StreamBuffers tmp(s);
     u64 *d_in = nullptr, *d_out = nullptr;
     CK(tmp.alloc(&d_in, ct_words * batch));
     CK(tmp.alloc(&d_out, ct_words * m->result_count * batch));
     CK(cudaMemcpyAsync(d_in, vectors, ct_words * batch * sizeof(u64), cudaMemcpyHostToDevice, s));
-    rc = mul_transpose_device(h, k, m, d_in, batch, mod_switch_to_single != 0, d_out, s);
+    rc = mul_transpose_device(h, &keys, 1, m, d_in, batch, mod_switch_to_single != 0, d_out, s);
     if (rc) {
         cudaStreamSynchronize(s);
         return rc;
@@ -492,29 +719,25 @@ int32_t hecuda_pnns_mul_transpose_matrix(const hecuda_context *h, const hecuda_e
                                          int64_t out_capacity, int64_t *out_count) {
     int32_t rc = check_args(h, k, m, ciphertexts, ciphertext_count, out);
     if (rc) return rc;
-    if (!out_count || ciphertext_count < 1 || query_row_count < 1 || pack_rotation_count < 0 ||
-        (pack_rotation_count && !pack_rotations))
-        return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
+    if (!out_count) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
     const Context &c = *h->ctx;
-    if (query_row_count > 1) {
-        if (!row_ciphertext_index || !row_masks || !row_rotate_count) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null row descriptors");
-        if (column_step < 1 || column_step > c.n / 2) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
-        for (int32_t r = 0; r < query_row_count; ++r)
-            if (row_ciphertext_index[r] < 0 || row_ciphertext_index[r] >= ciphertext_count || row_rotate_count[r] < 0)
-                return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongCiphertextCount: row descriptor out of range");
-    }
+    const MatrixQuery q{query_row_count, row_ciphertext_index, (const u64 *)row_masks, row_rotate_count, column_step,
+                        pack_rotations, pack_rotation_count};
+    if ((rc = check_matrix_query(c, ciphertext_count, q))) return rc;
+    const MatrixShape sh = matrix_shape(c, m, q);
+    if ((rc = check_capacity(sh, out_capacity, out_count))) return rc;
+    PnnsKeys keys;
+    if ((rc = matrix_keys(k, c.n, m, q, sh, keys))) return rc;
     WsGuard g(h);
     if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
     const size_t ct_words = (size_t)2 * c.L * c.n;
     cudaStream_t s = g.w->stream;
-    Tmp tmp(s);
+    StreamBuffers tmp(s);
     u64 *d_in = nullptr, *d_out = nullptr;
     CK(tmp.alloc(&d_in, ct_words * ciphertext_count));
-    CK(tmp.alloc(&d_out, ct_words * (size_t)std::max<int64_t>(out_capacity, 1)));
+    CK(tmp.alloc(&d_out, ct_words * (size_t)std::max<int64_t>(sh.outputs, 1)));
     CK(cudaMemcpyAsync(d_in, ciphertexts, ct_words * ciphertext_count * sizeof(u64), cudaMemcpyHostToDevice, s));
-    const MatrixQuery q{query_row_count, row_ciphertext_index, (const u64 *)row_masks, row_rotate_count, column_step,
-                        pack_rotations, pack_rotation_count};
-    rc = mul_transpose_matrix_device(h, k, m, d_in, q, mod_switch_to_single != 0, d_out, out_capacity, out_count, s);
+    rc = mul_transpose_matrix_device(h, &keys, 1, m, d_in, ciphertext_count, q, mod_switch_to_single != 0, d_out, s);
     if (rc) {
         cudaStreamSynchronize(s);
         return rc;
@@ -523,6 +746,39 @@ int32_t hecuda_pnns_mul_transpose_matrix(const hecuda_context *h, const hecuda_e
     CK(cudaMemcpyAsync(out, d_out, out_words * sizeof(u64), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     return HECUDA_OK;
+}
+
+int32_t hecuda_pnns_compute_response_clients(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count,
+                                             const hecuda_pnns_matrix *m, const uint64_t *ciphertexts, int32_t ciphertext_count,
+                                             int32_t query_row_count, const int32_t *row_ciphertext_index,
+                                             const uint64_t *row_masks, const int32_t *row_rotate_count, int32_t column_step,
+                                             const int32_t *pack_rotations, int32_t pack_rotation_count, uint64_t *out,
+                                             int64_t out_capacity, int64_t *out_count) {
+    const MatrixQuery q{query_row_count, row_ciphertext_index, (const u64 *)row_masks, row_rotate_count, column_step,
+                        pack_rotations, pack_rotation_count};
+    std::vector<PnnsKeys> keys;
+    int32_t rc = check_clients(h, evks, client_count, m, ciphertexts, ciphertext_count, q, out, out_capacity, out_count, keys);
+    if (rc) return rc;
+    return respond_clients(h, keys, m, q, ciphertext_count, *out_count, ciphertexts, nullptr, nullptr, out, out_capacity);
+}
+
+int32_t hecuda_pnns_compute_response_clients_wire(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count,
+                                                  const hecuda_pnns_matrix *m, const uint8_t *query_poly0,
+                                                  const uint8_t *query_seeds, int32_t ciphertext_count, int32_t query_row_count,
+                                                  const int32_t *row_ciphertext_index, const uint64_t *row_masks,
+                                                  const int32_t *row_rotate_count, int32_t column_step,
+                                                  const int32_t *pack_rotations, int32_t pack_rotation_count,
+                                                  int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1, uint8_t *out,
+                                                  int64_t out_capacity, int64_t *out_count) {
+    const MatrixQuery q{query_row_count, row_ciphertext_index, (const u64 *)row_masks, row_rotate_count, column_step,
+                        pack_rotations, pack_rotation_count};
+    std::vector<PnnsKeys> keys;
+    int32_t rc = check_clients(h, evks, client_count, m, query_poly0, ciphertext_count, q, out, out_capacity, out_count, keys);
+    if (rc) return rc;
+    if (!query_seeds) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    WireCodec wc;
+    if ((rc = wc.setup(*h->ctx, skip_lsbs_poly0, skip_lsbs_poly1))) return rc;
+    return respond_clients(h, keys, m, q, ciphertext_count, *out_count, query_poly0, query_seeds, &wc, out, out_capacity);
 }
 
 }  // extern "C"

@@ -125,6 +125,14 @@ SYMBOLS = {
     "hecuda_pnns_mul_transpose_matrix": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int32, C.c_int32, C.POINTER(C.c_int32), _VP,
                                                      C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32,
                                                      _VP, C.c_int64, C.POINTER(C.c_int64)]),
+    "hecuda_pnns_compute_response_clients": (C.c_int32, [_VP, C.POINTER(_VP), C.c_int32, _VP, _VP, C.c_int32, C.c_int32,
+                                                         C.POINTER(C.c_int32), _VP, C.POINTER(C.c_int32), C.c_int32,
+                                                         C.POINTER(C.c_int32), C.c_int32, _VP, C.c_int64,
+                                                         C.POINTER(C.c_int64)]),
+    "hecuda_pnns_compute_response_clients_wire": (C.c_int32, [_VP, C.POINTER(_VP), C.c_int32, _VP, _VP, _VP, C.c_int32,
+                                                              C.c_int32, C.POINTER(C.c_int32), _VP, C.POINTER(C.c_int32),
+                                                              C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32,
+                                                              C.c_int32, _VP, C.c_int64, C.POINTER(C.c_int64)]),
     "hecuda_poly_serialized_byte_count": (C.c_int32, [_VP, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
     "hecuda_poly_serialize": (C.c_int32, [_VP, C.c_int32, _VP, C.c_int32, _VP, C.c_int32, C.c_int64]),
     "hecuda_poly_load": (C.c_int32, [_VP, C.c_int32, _VP, C.c_int32, _VP, C.c_int32, C.c_int64]),

@@ -325,21 +325,61 @@ class PlaintextMatrix:
         CiphertextMatrix (count, 2, L, N); returns the dense-column packed result ciphertexts (count', 2, L or 1, N)."""
         ctx = self.context
         n = ctx.degree
-        if queryDimensions.columnCount != self.dimensions.columnCount:
-            raise PnnsError(f"invalidMatrixDimensions(rowCount: {queryDimensions.rowCount}, columnCount: {queryDimensions.columnCount})")
         cts = _host(ciphertexts)
         words = 2 * ctx.L * n
         count = cts.size // words
-        rows = queryDimensions.rowCount
-        expected = CiphertextMatrix.ciphertextCount(n, queryDimensions)
-        if cts.size % words or count != expected:
+        self._checkQuery(queryDimensions, count, cts.size % words == 0)
+        d = self._rowDescriptors(queryDimensions, count, evaluationKey.galoisElements)
+        out = np.empty((d["capacity"], 2, 1 if modSwitchDownToSingle else ctx.L, n), dtype=np.uint64)
+        produced = C.c_int64(0)
+        _check(load_library().hecuda_pnns_mul_transpose_matrix(
+            ctx._h, evaluationKey._h, self._h, _ptr(cts), count, queryDimensions.rowCount, d["index"], _ptr(d["masks"]),
+            d["rotate"], d["step"], d["plan"], d["planCount"], 1 if modSwitchDownToSingle else 0, _ptr(out), d["capacity"],
+            C.byref(produced)))
+        return out[: produced.value]
+
+    def computeResponses(self, ciphertexts, queryDimensions: MatrixDimensions, evaluationKeys) -> np.ndarray:
+        """Server.computeResponse (Server.swift:61-88) for many clients in one C-ABI call
+        (hecuda_pnns_compute_response_clients): client c's dense-row query ciphertexts with evaluationKeys[c], its replies
+        bit-identical to `mulTransposeMatrix(ciphertexts[c], queryDimensions, evaluationKeys[c], modSwitchDownToSingle=True)`.
+        Groups of up to HECUDA_PNNS_CLIENT_GROUP clients share every pass, including one pass over the matrix.  The
+        packing rotations are planned with the first key's Galois elements (every key must hold them).
+
+        ciphertexts: (clients, count, 2, L, N) Coeff.  Returns (clients, count', 2, 1, N)."""
+        ctx = self.context
+        n = ctx.degree
+        keys = list(evaluationKeys)
+        cts = _host(ciphertexts)
+        words = 2 * ctx.L * n
+        if not keys or cts.size % (words * len(keys)):
+            raise HeError(-1, "invalidCiphertext: ciphertexts must be one query of 2 x L x N ciphertexts per evaluation key")
+        count = cts.size // (words * len(keys))
+        self._checkQuery(queryDimensions, count, True)
+        d = self._rowDescriptors(queryDimensions, count, keys[0].galoisElements)
+        out = np.empty((len(keys), d["capacity"], 2, 1, n), dtype=np.uint64)
+        produced = C.c_int64(0)
+        key_handles = (C.c_void_p * len(keys))(*[k._h for k in keys])
+        _check(load_library().hecuda_pnns_compute_response_clients(
+            ctx._h, key_handles, len(keys), self._h, _ptr(cts), count, queryDimensions.rowCount, d["index"], _ptr(d["masks"]),
+            d["rotate"], d["step"], d["plan"], d["planCount"], _ptr(out), d["capacity"], C.byref(produced)))
+        return out[:, : produced.value]
+
+    def _checkQuery(self, queryDimensions: MatrixDimensions, count: int, whole: bool):
+        if queryDimensions.columnCount != self.dimensions.columnCount:
+            raise PnnsError(f"invalidMatrixDimensions(rowCount: {queryDimensions.rowCount}, columnCount: {queryDimensions.columnCount})")
+        expected = CiphertextMatrix.ciphertextCount(self.context.degree, queryDimensions)
+        if not whole or count != expected:
             raise PnnsError(f"wrongCiphertextCount(got: {count}, expected: {expected})")
+
+    def _rowDescriptors(self, queryDimensions: MatrixDimensions, count: int, galoisElements) -> dict:
+        """What extractDenseRow derives for every query row, and the packing rotations, as the C ABI takes them."""
+        n = self.context.degree
+        rows = queryDimensions.rowCount
         index = (C.c_int32 * rows)()
         rotate = (C.c_int32 * rows)()
         masks = np.zeros((rows, n), dtype=np.uint64)
-        step = _next_power_of_two(queryDimensions.columnCount)
         if rows > 1:
-            encoder = SimdEncoder(n, ctx.plaintextModulus)
+            encoder = SimdEncoder(n, self.context.plaintextModulus)
             values = np.zeros((rows, n), dtype=np.uint64)
             for r in range(rows):
                 index[r], mask, rotate[r] = CiphertextMatrix.denseRowExtraction(n, queryDimensions, count, r)
@@ -348,15 +388,10 @@ class PlaintextMatrix:
         per_simd_row = (n // 2) // self.dimensions.rowCount
         sequence = []
         if per_simd_row > 1 and rows > 1:
-            sequence = GaloisElement.rotationSequence(evaluationKey.galoisElements, self.dimensions.rowCount, n)
-        plan = (C.c_int32 * max(1, len(sequence)))(*sequence)
-        capacity = rows * self.resultCiphertextCount
-        out = np.empty((capacity, 2, 1 if modSwitchDownToSingle else ctx.L, n), dtype=np.uint64)
-        produced = C.c_int64(0)
-        _check(load_library().hecuda_pnns_mul_transpose_matrix(
-            ctx._h, evaluationKey._h, self._h, _ptr(cts), count, rows, index, _ptr(masks), rotate, step, plan, len(sequence),
-            1 if modSwitchDownToSingle else 0, _ptr(out), capacity, C.byref(produced)))
-        return out[: produced.value]
+            sequence = GaloisElement.rotationSequence(galoisElements, self.dimensions.rowCount, n)
+        return dict(index=index, rotate=rotate, masks=masks, step=_next_power_of_two(queryDimensions.columnCount),
+                    plan=(C.c_int32 * max(1, len(sequence)))(*sequence), planCount=len(sequence),
+                    capacity=rows * self.resultCiphertextCount)
 
     def close(self):
         if getattr(self, "_h", None) is not None:
@@ -368,6 +403,42 @@ class PlaintextMatrix:
             self.close()
         except Exception:
             pass
+
+
+class PnnsWire:
+    """Request / reply bytes of the PNNS server (the payloads of the reference's protobuf messages)."""
+
+    @staticmethod
+    def computeResponses(matrix: PlaintextMatrix, queryPoly0, querySeeds, queryDimensions: MatrixDimensions, evaluationKeys):
+        """PlaintextMatrix.computeResponses on the wire, one C-ABI call (hecuda_pnns_compute_response_clients_wire): the
+        queries as seeded serialized ciphertexts (SerializedCiphertext.seeded), the replies serialized forDecryption
+        (PnnsConversionApi.swift:48) with skipLSBsForDecryption.
+        queryPoly0: (clients, count, byteCount(L rows)) uint8; querySeeds: (clients, count, 32) uint8.  Returns
+        (replies, skipLSBs) with replies of shape (clients, count', bytes(poly0) + bytes(poly1))."""
+        from . import Bfv
+        from .pir import skipLSBsForDecryption
+        ctx = matrix.context
+        keys = list(evaluationKeys)
+        seeds = np.ascontiguousarray(np.asarray(querySeeds, dtype=np.uint8))
+        poly0 = np.ascontiguousarray(np.asarray(queryPoly0, dtype=np.uint8))
+        size = Bfv.serializationByteCount(ctx, ctx.L)
+        if not keys or seeds.size % (32 * len(keys)):
+            raise HeError(-1, "serializedBufferSizeMismatch: querySeeds must be one set of 32-byte seeds per evaluation key")
+        count = seeds.size // (32 * len(keys))
+        if poly0.size != len(keys) * count * size:
+            raise HeError(-1, f"serializedBufferSizeMismatch(poly0: {poly0.size} bytes, expected {len(keys) * count * size})")
+        matrix._checkQuery(queryDimensions, count, True)
+        d = matrix._rowDescriptors(queryDimensions, count, keys[0].galoisElements)
+        skips = skipLSBsForDecryption(ctx)
+        sizes = [Bfv.serializationByteCount(ctx, 1, s) for s in skips]
+        out = np.empty((len(keys), d["capacity"], sum(sizes)), dtype=np.uint8)
+        produced = C.c_int64(0)
+        key_handles = (C.c_void_p * len(keys))(*[k._h for k in keys])
+        _check(load_library().hecuda_pnns_compute_response_clients_wire(
+            ctx._h, key_handles, len(keys), matrix._h, poly0.ctypes.data_as(C.c_void_p), seeds.ctypes.data_as(C.c_void_p),
+            count, queryDimensions.rowCount, d["index"], _ptr(d["masks"]), d["rotate"], d["step"], d["plan"], d["planCount"],
+            skips[0], skips[1], out.ctypes.data_as(C.c_void_p), d["capacity"], C.byref(produced)))
+        return out[:, : produced.value], skips
 
 
 def denseRowVector(context, vector) -> np.ndarray:
