@@ -305,6 +305,33 @@ int32_t hecuda_pir_database_destroy(hecuda_pir_database *db);
  * reference's default PIR parameters -- the rows are kept as uint32 (half the bytes per first-dimension scan) and
  * `bytes` = count * L * N * 4; otherwise uint64 and `bytes` = count * L * N * 8. */
 int32_t hecuda_pir_database_device_buffer(hecuda_pir_database *db, void **device_ptr, uint64_t *bytes);
+/* The database's presence flags copied to the host: out[i] = 0 for a nil plaintext the scan skips, 1 otherwise (all 1
+ * when it was created without flags).  capacity >= the database's plaintext count. */
+int32_t hecuda_pir_database_present(const hecuda_pir_database *db, uint8_t *out, int64_t capacity);
+
+/* MulPirServer.process(database:with:using:) -- IndexPir/MulPir.swift:433-556 (processPackEntries,
+ * processSplitLargeEntries, CoefficientPacking.bytesToCoefficients with floor(log2 t) bits per coefficient) on the
+ * device.  entries: the concatenated entry bytes; offsets: entry_count + 1 byte offsets (entry i = [offsets[i],
+ * offsets[i+1])), or NULL when every entry is exactly entry_size bytes.  entry_size = IndexPirParameter.entrySizeInBytes,
+ * encode_entry_size = IndexPirParameter.encodingEntrySize (a little-endian length prefix per entry), dims =
+ * IndexPirParameter.dimensions (1 or 2).  count = chunkCount * prod(dims), chunkCount = ceil(encodedEntrySize /
+ * bytesPerPlaintext).  Only the entry bytes (and offsets) cross PCIe; each thread of the packing kernel reads the
+ * bytes its coefficient needs straight from them.
+ * hecuda_pir_process_entries: plaintexts count x N coefficients (< t) and present[count] (0 = nil: all-zero, MulPir.swift:480,
+ * 536) in process order -- what hecuda/pir.py plaintextRows computes on the host.
+ * hecuda_pir_database_create_from_entries: the resident database hecuda_pir_database_create(those plaintexts,
+ * eval_format = 0, present) builds, word for word, converted in slabs; peak device memory is the entries, the database
+ * and one 64 MB slab.  A Bfv<UInt32> context works as with hecuda_pir_database_create.
+ * Checked on the host before anything is allocated (HECUDA_ERR_INVALID_ARGUMENT, *out NULL): null pointers, dim_count,
+ * decreasing offsets, an entry longer than entry_size (invalidDatabaseEntrySize), more entries (split) or packed plaintexts
+ * than prod(dims) holds (invalidDatabaseEntryCount), and a wrong `count`. */
+int32_t hecuda_pir_process_entries(const hecuda_context *ctx, const uint8_t *entries, const uint64_t *offsets,
+                                   int64_t entry_count, int64_t entry_size, int32_t encode_entry_size,
+                                   const int32_t *dims, int32_t dim_count, uint64_t *plaintexts, uint8_t *present,
+                                   int64_t count);
+int32_t hecuda_pir_database_create_from_entries(const hecuda_context *ctx, const uint8_t *entries, const uint64_t *offsets,
+                                                int64_t entry_count, int64_t entry_size, int32_t encode_entry_size,
+                                                const int32_t *dims, int32_t dim_count, hecuda_pir_database **out);
 
 /* PirUtil.expand(ciphertexts:outputCount:using:) -- IndexPir/PirUtil.swift:321-355 (expandCiphertext :249-304,
  * expandCiphertextForOneStep :204-236).  ciphertexts: ciphertext_count x 2 x L x N (Coeff); out: output_count x 2 x L x N,
@@ -400,6 +427,31 @@ int32_t hecuda_pnns_matrix_create(const hecuda_context *ctx, const uint64_t *pla
                                   hecuda_pnns_matrix **out);
 int32_t hecuda_pnns_matrix_destroy(hecuda_pnns_matrix *matrix);
 int32_t hecuda_pnns_matrix_result_count(const hecuda_pnns_matrix *matrix, int64_t *count); /* ceil(row_count / N) */
+
+/* PlaintextMatrix.init(context:dimensions:packing: .diagonal, signedValues:reduce:) -- PlaintextMatrix.swift:155-190 --
+ * with diagonalPlaintexts (:417-482) on the device.  values: row_count x column_count signed values, row-major; each
+ * becomes Modulus.reduce(value) (reduce = 1) or value.centeredToRemainder(t), which requires value in
+ * [-floor(t/2), floor((t-1)/2)] (HECUDA_ERR_INVALID_ARGUMENT otherwise).  Diagonal d holds
+ * data[c][(c + d) mod nextPow2(cols)] (0 past cols); each N-chunk of it has both SIMD half-rows rotated by
+ * floor(d / baby_step) * baby_step and is SIMD-encoded.  One kernel does the conversion, gather, rotation and encodeSimd
+ * scatter; the inverse NTT mod t follows.  HECUDA_ERR_UNSUPPORTED without SIMD support (simdEncodingNotSupported),
+ * invalidMatrixDimensions when column_count > N/2.
+ * hecuda_pnns_diagonal_plaintexts: out = nextPow2(cols) * ceil(rows / N) Coeff plaintexts x N, in the order
+ * hecuda_pnns_matrix_create takes them (out is unspecified when a value is out of range).
+ * hecuda_pnns_matrix_create_from_values: the handle hecuda_pnns_matrix_create(those plaintexts, eval_format = 0, ...)
+ * builds -- the same resident words, flags and shape -- written in its slot order and converted to Eval in slabs;
+ * baby_step / giant_step are checked as there.  On error *out is NULL and nothing stays allocated. */
+int32_t hecuda_pnns_diagonal_plaintexts(const hecuda_context *ctx, const int64_t *values, int32_t reduce,
+                                        int64_t row_count, int64_t column_count, int32_t baby_step, uint64_t *out);
+int32_t hecuda_pnns_matrix_create_from_values(const hecuda_context *ctx, const int64_t *values, int32_t reduce,
+                                              int64_t row_count, int64_t column_count, int32_t baby_step,
+                                              int32_t giant_step, hecuda_pnns_matrix **out);
+/* The resident plaintexts, [result][giant][baby] x L x N uint64 Eval words (bytes = result_count * giant * baby * L * N * 8),
+ * as hecuda_pir_database_device_buffer gives a database's (device-to-device copies between ranks). */
+int32_t hecuda_pnns_matrix_device_buffer(hecuda_pnns_matrix *matrix, void **device_ptr, uint64_t *bytes);
+/* The matrix's presence flags in its resident slot order ([result][giant][baby]) copied to the host: 0 for a slot past
+ * the padded dimension (an absent plaintext).  capacity >= result_count * giant * baby. */
+int32_t hecuda_pnns_matrix_present(const hecuda_pnns_matrix *matrix, uint8_t *out, int64_t capacity);
 
 /* PlaintextMatrix.mulTranspose(vector:using:) -- MatrixMultiplication.swift:131-226, for `batch` dense-row query
  * ciphertexts (batch x 2 x L x N, Coeff) that share `evk`: babyStep-1 rotateColumns(by: -1), forward NTTs, one

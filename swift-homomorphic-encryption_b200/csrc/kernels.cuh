@@ -6,6 +6,7 @@
 #include <string>
 
 #include "context.hpp"
+#include "process_db.cuh"
 
 namespace hecuda {
 
@@ -107,6 +108,8 @@ cudaError_t launch_encode_simd(const Context &ctx, const u64 *values, int value_
                                int64_t count, cudaStream_t stream);
 cudaError_t launch_decode_simd(const Context &ctx, const u64 *plain, int l, u64 *values, u64 *scratch, int64_t count,
                                cudaStream_t stream);
+// NTT of `rows` rows (rows x N), all mod the modulus of one slot (e.g. ctx.slot_t()); the inverse scales by N^-1 only
+cudaError_t ntt_single(const Context &ctx, int slot, bool inverse, const u64 *in, u64 *out, int64_t rows, cudaStream_t s);
 // plaintextTranslate: ct, out batch x polys x l x N (Coeff); pt N values (< t) shared by all (broadcast) or batch x N;
 // op = HECUDA_PLAINTEXT_ADD / SUB / SUB_FROM; out may equal ct
 cudaError_t launch_plaintext_translate(const Context &ctx, const u64 *ct, int polys, int l, const u64 *pt, bool broadcast,
@@ -142,6 +145,22 @@ cudaError_t launch_poly_serialize(const Context &ctx, const CodecConsts &c, int 
 // uint32 <-> uint64 residues at the boundary of a Bfv<UInt32> context (elementwise.cu); both buffers 16-byte aligned
 cudaError_t launch_widen(const u32 *in, u64 *out, int64_t words, cudaStream_t stream);
 cudaError_t launch_narrow(const u64 *in, u32 *out, int64_t words, cudaStream_t stream);
+
+// ---- the server's data into plaintexts (process_db.cu; index maps in process_db.cuh)
+// Plaintexts per slab when a database is packed and converted to Eval piecewise: <= 64 MB of coefficients
+inline int64_t coefficient_slab(const Context &ctx) {
+    const int64_t per = (int64_t)((size_t)8 * 1024 * 1024 / ctx.n);
+    return per > 1 ? per : 1;
+}
+// MulPirServer.process: plaintexts first .. first + items of the database `s` (entries / offsets on the device) ->
+// out items x N coefficients (< t), present[items] (0 = nil plaintext)
+cudaError_t launch_pir_pack(const procdb::PirShape &s, int n, int64_t first, int64_t items, u64 *out,
+                            unsigned char *present, cudaStream_t stream);
+// PlaintextMatrix(signedValues:) .diagonal packing + encodeSimd: plaintexts first .. first + items (diagonalPlaintexts'
+// order, or hecuda_pnns_matrix's slot order when `resident`) of the row-major matrix `values` (on the device) ->
+// out items x N (Coeff, < t).  A value outside the centered range without `reduce` sets *bad.  Needs ctx.simd.
+cudaError_t launch_pnns_diagonal(const Context &ctx, const procdb::PnnsShape &s, const int64_t *values, bool reduce,
+                                 bool resident, int64_t first, int64_t items, u64 *out, int *bad, cudaStream_t stream);
 
 // divideAndRoundQLast over polys x l x N -> polys x (l-1) x N
 cudaError_t launch_mod_switch(const Context &ctx, const u64 *in, int l, u64 *out, int64_t polys, cudaStream_t stream);

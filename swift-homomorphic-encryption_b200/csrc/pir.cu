@@ -756,9 +756,168 @@ int32_t respond_wire(const hecuda_context *h, const hecuda_evk *const *evks, int
     return HECUDA_OK;
 }
 
+// Small moduli (the default PIR parameters): keep the rows as uint32 -- half the bytes per scan, half the HBM
+cudaError_t narrow_database(const Context &c, hecuda_pir_database *db) {
+    if (!inner_product_plain_small_supported(c, c.L)) return cudaSuccess;
+    const size_t words = (size_t)c.L * c.n * db->count;
+    cudaError_t e = cudaMalloc(&db->d_plain32, words * sizeof(u32));
+    if (e == cudaSuccess) e = launch_narrow(db->d_plain, db->d_plain32, (int64_t)words, nullptr);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
+    if (e == cudaSuccess) {
+        cudaFree(db->d_plain);
+        db->d_plain = nullptr;
+    }
+    return e;
+}
+
+std::string describe(const char *fmt, long long a, long long b) {
+    char buf[160];
+    snprintf(buf, sizeof buf, fmt, a, b);
+    return buf;
+}
+
+// MulPirServer.process's arguments (MulPir.swift:433-556; the checks of hecuda/pir.py plaintextRows), all on the
+// host: on success `s` describes the database except for its device pointers, `bytes` is how many entry bytes to
+// upload and `count` = chunkCount * prod(dimensions).
+int32_t pir_process_shape(const hecuda_context *h, const uint8_t *entries, const uint64_t *offsets, int64_t entry_count,
+                          int64_t entry_size, int32_t encode_entry_size, const int32_t *dims, int32_t dim_count,
+                          procdb::PirShape &s, size_t &bytes, int64_t &count) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (!entries || !dims) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (dim_count != 1 && dim_count != 2)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT,
+                    "invalidDimensionCount(dimensionCount: " + std::to_string(dim_count) + ", expected: [1, 2])");
+    if (entry_count < 0 || entry_size < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "negative entry count / empty entry size");
+    int64_t per_chunk = 1;
+    for (int i = 0; i < dim_count; ++i) {
+        if (dims[i] < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "dimensions must be positive");
+        per_chunk *= dims[i];
+    }
+    const Context &c = *h->ctx;
+    s = procdb::pir_shape(c.n, c.t, entry_count, entry_size, encode_entry_size != 0, per_chunk, dims[0]);
+    if (s.bits < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "plaintext modulus below 2");
+    int64_t longest = entry_count ? entry_size : 0;
+    if (offsets) {
+        longest = 0;
+        for (int64_t i = 0; i < entry_count; ++i) {
+            if (offsets[i + 1] < offsets[i]) return fail(HECUDA_ERR_INVALID_ARGUMENT, "offsets must not decrease");
+            longest = std::max<int64_t>(longest, (int64_t)(offsets[i + 1] - offsets[i]));
+        }
+        bytes = (size_t)offsets[entry_count];
+    } else {
+        bytes = (size_t)(entry_count * entry_size);
+    }
+    if (longest > entry_size)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT,
+                    describe("invalidDatabaseEntrySize(maximumEntrySize: %lld, expected: %lld)", longest, entry_size));
+    const int64_t chunks = procdb::pir_chunk_count(s);
+    if (chunks > 1) {  // processSplitLargeEntries: one entry per plaintext and chunk
+        if (entry_count > per_chunk)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT,
+                        describe("invalidDatabaseEntryCount(entryCount: %lld, expected: at most %lld)", entry_count, per_chunk));
+    } else {  // processPackEntries
+        const int64_t pieces = (entry_count * s.encoded + s.stride - 1) / s.stride;
+        if (pieces > per_chunk)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT,
+                        describe("invalidDatabaseEntryCount(entryCount: %lld, expected: at most %lld)", entry_count,
+                               per_chunk * (s.stride / s.encoded)));
+    }
+    count = chunks * per_chunk;
+    return HECUDA_OK;
+}
+
+// Uploads the entry bytes (and offsets) once, then packs the `count` plaintexts slab by slab on the default stream:
+// present flags into d_present[count], each slab's coefficients handed to sink(first, items, d_coeff).  Frees its
+// buffers before it returns.
+template <class Sink>
+cudaError_t pir_pack_slabs(const Context &c, procdb::PirShape s, const uint8_t *entries, const uint64_t *offsets,
+                           size_t bytes, int64_t count, unsigned char *d_present, Sink sink) {
+    unsigned char *d_entries = nullptr;
+    uint64_t *d_offsets = nullptr;
+    u64 *d_coeff = nullptr;
+    const int64_t slab = coefficient_slab(c);
+    cudaError_t e = cudaMalloc(&d_entries, std::max<size_t>(bytes, 1));
+    if (e == cudaSuccess && bytes) e = upload(d_entries, entries, bytes);
+    if (e == cudaSuccess && offsets) {
+        const size_t offset_bytes = (size_t)(s.entry_count + 1) * sizeof(uint64_t);
+        e = cudaMalloc(&d_offsets, offset_bytes);
+        if (e == cudaSuccess) e = upload(d_offsets, offsets, offset_bytes);
+    }
+    s.entries = d_entries;
+    s.offsets = d_offsets;
+    if (e == cudaSuccess) e = cudaMalloc(&d_coeff, (size_t)std::min(slab, count) * c.n * sizeof(u64));
+    for (int64_t done = 0; e == cudaSuccess && done < count; done += slab) {
+        const int64_t items = std::min(slab, count - done);
+        e = launch_pir_pack(s, (int)c.n, done, items, d_coeff, d_present + done, nullptr);
+        if (e == cudaSuccess) e = sink(done, items, d_coeff);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
+    cudaFree(d_coeff);
+    cudaFree(d_offsets);
+    cudaFree(d_entries);
+    return e;
+}
+
 }  // namespace
 
 extern "C" {
+
+int32_t hecuda_pir_process_entries(const hecuda_context *h, const uint8_t *entries, const uint64_t *offsets,
+                                   int64_t entry_count, int64_t entry_size, int32_t encode_entry_size, const int32_t *dims,
+                                   int32_t dim_count, uint64_t *plaintexts, uint8_t *present, int64_t count) {
+    procdb::PirShape s;
+    size_t bytes = 0;
+    int64_t expected = 0;
+    int32_t rc = pir_process_shape(h, entries, offsets, entry_count, entry_size, encode_entry_size, dims, dim_count, s,
+                                   bytes, expected);
+    if (rc) return rc;
+    if (!plaintexts || !present) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (count != expected)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, describe("count %lld != chunkCount * prod(dimensions) = %lld", count, expected));
+    const Context &c = *h->ctx;
+    unsigned char *d_present = nullptr;
+    cudaError_t e = cudaMalloc(&d_present, (size_t)count);
+    if (e == cudaSuccess)
+        e = pir_pack_slabs(c, s, entries, offsets, bytes, count, d_present, [&](int64_t first, int64_t items, const u64 *d) {
+            return cudaMemcpy(plaintexts + (size_t)first * c.n, d, (size_t)items * c.n * sizeof(u64), cudaMemcpyDeviceToHost);
+        });
+    if (e == cudaSuccess) e = cudaMemcpy(present, d_present, (size_t)count, cudaMemcpyDeviceToHost);
+    cudaFree(d_present);
+    return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "pir process entries");
+}
+
+int32_t hecuda_pir_database_create_from_entries(const hecuda_context *h, const uint8_t *entries, const uint64_t *offsets,
+                                                int64_t entry_count, int64_t entry_size, int32_t encode_entry_size,
+                                                const int32_t *dims, int32_t dim_count, hecuda_pir_database **out) {
+    if (!out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    procdb::PirShape s;
+    size_t bytes = 0;
+    int64_t count = 0;
+    int32_t rc = pir_process_shape(h, entries, offsets, entry_count, entry_size, encode_entry_size, dims, dim_count, s,
+                                   bytes, count);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    const size_t row_words = (size_t)c.L * c.n;
+    hecuda_pir_database *db = new (std::nothrow) hecuda_pir_database();
+    if (!db) return fail(HECUDA_ERR_CUDA, "out of host memory");
+    db->owner = h;
+    db->count = count;
+    cudaError_t e = cudaMalloc(&db->d_plain, row_words * count * sizeof(u64));
+    if (e == cudaSuccess) e = cudaMalloc(&db->d_present, (size_t)count);
+    if (e == cudaSuccess)  // Plaintext.convertToEvalFormat (Plaintext.swift:149-171), one slab at a time
+        e = pir_pack_slabs(c, s, entries, offsets, bytes, count, db->d_present, [&](int64_t first, int64_t items, const u64 *d) {
+            return launch_plaintext_to_eval(c, d, c.L, db->d_plain + row_words * first, items, nullptr);
+        });
+    if (e == cudaSuccess) e = narrow_database(c, db);
+    if (e != cudaSuccess) {
+        hecuda_pir_database_destroy(db);
+        return cuda_fail(e, "pir database from entries");
+    }
+    *out = db;
+    return HECUDA_OK;
+}
 
 int32_t hecuda_pir_database_create(const hecuda_context *h, const uint64_t *plaintexts, int32_t eval_format,
                                    const uint8_t *present, int64_t count, hecuda_pir_database **out) {
@@ -781,7 +940,7 @@ int32_t hecuda_pir_database_create(const hecuda_context *h, const uint64_t *plai
         if (eval_format) {
             e = upload(db->d_plain, plaintexts, row_words * count * sizeof(u64));
         } else {  // Plaintext.convertToEvalFormat (Plaintext.swift:149-171) in slabs of <= 64 MB of coefficients
-            const int64_t slab = std::max<int64_t>(1, (int64_t)((size_t)8 * 1024 * 1024 / c.n));
+            const int64_t slab = coefficient_slab(c);
             u64 *d_coeff = nullptr;
             e = cudaMalloc(&d_coeff, (size_t)std::min(slab, count) * c.n * sizeof(u64));
             for (int64_t done = 0; e == cudaSuccess && done < count; done += slab) {
@@ -793,16 +952,7 @@ int32_t hecuda_pir_database_create(const hecuda_context *h, const uint64_t *plai
             cudaFree(d_coeff);
         }
     }
-    if (e == cudaSuccess && inner_product_plain_small_supported(c, c.L)) {
-        // small moduli (the default PIR parameters): keep the rows as uint32 -- half the bytes per scan, half the HBM
-        e = cudaMalloc(&db->d_plain32, row_words * count * sizeof(u32));
-        if (e == cudaSuccess) e = launch_narrow(db->d_plain, db->d_plain32, (int64_t)(row_words * count), nullptr);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
-        if (e == cudaSuccess) {
-            cudaFree(db->d_plain);
-            db->d_plain = nullptr;
-        }
-    }
+    if (e == cudaSuccess) e = narrow_database(c, db);
     if (e != cudaSuccess) {
         hecuda_pir_database_destroy(db);
         return cuda_fail(e, "pir database upload");
@@ -826,6 +976,17 @@ int32_t hecuda_pir_database_device_buffer(hecuda_pir_database *db, void **device
     // (uint32 rows when every ciphertext modulus is below 2^31: the bytes say which)
     *device_ptr = db->d_plain32 ? (void *)db->d_plain32 : (void *)db->d_plain;
     *bytes = (uint64_t)db->count * db->owner->ctx->L * db->owner->ctx->n * (db->d_plain32 ? sizeof(u32) : sizeof(u64));
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pir_database_present(const hecuda_pir_database *db, uint8_t *out, int64_t capacity) {
+    if (!db || !out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (capacity < db->count) return fail(HECUDA_ERR_INVALID_ARGUMENT, "capacity below the plaintext count");
+    if (!db->d_present) {
+        memset(out, 1, (size_t)db->count);
+        return HECUDA_OK;
+    }
+    CK(cudaMemcpy(out, db->d_present, (size_t)db->count, cudaMemcpyDeviceToHost));
     return HECUDA_OK;
 }
 

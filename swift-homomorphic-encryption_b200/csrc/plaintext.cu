@@ -143,7 +143,9 @@ __global__ void __launch_bounds__(kThreads) uncenter_kernel(u64 *data, u64 thres
 
 int threads_for(int64_t n) { return n >= kThreads ? kThreads : (n < 32 ? 32 : (int)n); }
 
-// NTT of `rows` rows mod one slot, at most 65535 rows per call when N = 2^15 (the split path puts rows in grid z)
+}  // namespace
+
+// at most 65535 rows per call when N = 2^15 (the split path puts rows in grid z)
 cudaError_t ntt_single(const Context &ctx, int slot, bool inverse, const u64 *in, u64 *out, int64_t rows, cudaStream_t s) {
     const int64_t step = ctx.logn >= fast::kSplitLogN ? kMaxGridY : rows;
     const NttRowMap map = ctx.map_single(slot);
@@ -156,6 +158,8 @@ cudaError_t ntt_single(const Context &ctx, int slot, bool inverse, const u64 *in
     }
     return cudaSuccess;
 }
+
+namespace {
 
 cudaError_t launch_simd_gather(const Context &ctx, bool encode, const u64 *in, int value_count, u64 *out, int64_t count,
                                cudaStream_t s) {

@@ -587,9 +587,155 @@ int32_t respond_clients(const hecuda_context *h, const std::vector<PnnsKeys> &ke
     return HECUDA_OK;
 }
 
+// The matrix shape a .diagonal PlaintextMatrix accepts; dimension = nextPow2(column_count)
+int32_t check_dimensions(const Context &c, int64_t row_count, int64_t column_count, int64_t &dimension) {
+    if (row_count < 1 || column_count < 1 || column_count > c.n / 2)  // PnnsError.invalidMatrixDimensions (PlaintextMatrix.swift:429-431)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
+    dimension = 1;
+    while (dimension < column_count) dimension <<= 1;
+    return HECUDA_OK;
+}
+
+// The BabyStepGiantStep a resident matrix of padded dimension `dimension` accepts (MatrixMultiplication.swift:26-62)
+int32_t check_steps(const Context &c, int64_t dimension, int32_t baby_step, int32_t giant_step) {
+    if (baby_step < 1 || giant_step < 1 || baby_step < giant_step || (int64_t)baby_step * giant_step < dimension ||
+        (int64_t)baby_step * (giant_step - 1) >= dimension || baby_step >= c.n / 2)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongMatrixPacking: babyStep / giantStep do not cover the padded dimension");
+    return HECUDA_OK;
+}
+
+// PlaintextMatrix.init(signedValues:) + diagonalPlaintexts (PlaintextMatrix.swift:155-190, 417-482) on the default
+// stream: uploads the row-major values once, then SIMD-encodes `count` plaintexts slab by slab (in slot order when
+// `resident`), handing each slab's coefficients to sink(first, items, d_coeff).  Frees its buffers before it returns;
+// HECUDA_ERR_INVALID_ARGUMENT when a value is outside centeredToRemainder's range and `reduce` is off.
+template <class Sink>
+int32_t pnns_encode_slabs(const Context &c, const procdb::PnnsShape &shape, const int64_t *values, bool reduce,
+                          bool resident, int64_t count, Sink sink) {
+    const size_t value_bytes = (size_t)shape.rows * shape.cols * sizeof(int64_t);
+    const int64_t slab = coefficient_slab(c);
+    int64_t *d_values = nullptr;
+    int *d_bad = nullptr;
+    u64 *d_coeff = nullptr;
+    int bad = 0;
+    cudaError_t e = cudaMalloc(&d_values, value_bytes);
+    if (e == cudaSuccess) e = upload(d_values, values, value_bytes);
+    if (e == cudaSuccess) e = cudaMalloc(&d_bad, sizeof(int));
+    if (e == cudaSuccess) e = fill(d_bad, 0, sizeof(int));
+    if (e == cudaSuccess) e = cudaMalloc(&d_coeff, (size_t)std::min(slab, count) * c.n * sizeof(u64));
+    for (int64_t done = 0; e == cudaSuccess && done < count; done += slab) {
+        const int64_t items = std::min(slab, count - done);
+        e = launch_pnns_diagonal(c, shape, d_values, reduce, resident, done, items, d_coeff, d_bad, nullptr);
+        if (e == cudaSuccess) e = sink(done, items, d_coeff);
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost);
+    cudaFree(d_coeff);
+    cudaFree(d_bad);
+    cudaFree(d_values);
+    if (e != cudaSuccess) return cuda_fail(e, "pnns diagonal packing");
+    if (bad)  // Scalar.centeredToRemainder's precondition (Scalar.swift:85-87)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "signed value outside [-floor(t/2), floor((t-1)/2)]; pass reduce to reduce mod t");
+    return HECUDA_OK;
+}
+
+// resident: a matrix handle, whose baby and giant step are checked as hecuda_pnns_matrix_create checks them;
+// otherwise diagonalPlaintexts, which needs only a positive baby step (giant_step is ignored)
+int32_t check_values(const hecuda_context *h, const int64_t *values, int64_t row_count, int64_t column_count,
+                     int32_t baby_step, int32_t giant_step, bool resident, procdb::PnnsShape &shape) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (!values) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    const Context &c = *h->ctx;
+    int64_t dimension = 0;
+    if ((rc = check_dimensions(c, row_count, column_count, dimension))) return rc;
+    if (resident) {
+        if ((rc = check_steps(c, dimension, baby_step, giant_step))) return rc;
+    } else if (baby_step < 1) {
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongMatrixPacking: babyStep must be positive");
+    }
+    if (!c.simd) return fail(HECUDA_ERR_UNSUPPORTED, "simdEncodingNotSupported");
+    shape = procdb::PnnsShape{row_count, column_count, (row_count + c.n - 1) / c.n, (int)dimension, baby_step,
+                              resident ? giant_step : 1, c.logn};
+    return HECUDA_OK;
+}
+
 }  // namespace
 
 extern "C" {
+
+int32_t hecuda_pnns_diagonal_plaintexts(const hecuda_context *h, const int64_t *values, int32_t reduce, int64_t row_count,
+                                        int64_t column_count, int32_t baby_step, uint64_t *out) {
+    procdb::PnnsShape shape;
+    int32_t rc = check_values(h, values, row_count, column_count, baby_step, 0, false, shape);
+    if (rc) return rc;
+    if (!out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    const Context &c = *h->ctx;
+    return pnns_encode_slabs(c, shape, values, reduce != 0, false, (int64_t)shape.dimension * shape.results,
+                             [&](int64_t first, int64_t items, const u64 *d) {
+                                 return cudaMemcpy(out + (size_t)first * c.n, d, (size_t)items * c.n * sizeof(u64),
+                                                   cudaMemcpyDeviceToHost);
+                             });
+}
+
+int32_t hecuda_pnns_matrix_create_from_values(const hecuda_context *h, const int64_t *values, int32_t reduce,
+                                              int64_t row_count, int64_t column_count, int32_t baby_step,
+                                              int32_t giant_step, hecuda_pnns_matrix **out) {
+    if (!out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    procdb::PnnsShape shape;
+    int32_t rc = check_values(h, values, row_count, column_count, baby_step, giant_step, true, shape);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    const size_t row_words = (size_t)c.L * c.n;
+    const int64_t slots = shape.results * giant_step * baby_step;
+    hecuda_pnns_matrix *m = new (std::nothrow) hecuda_pnns_matrix();
+    if (!m) return fail(HECUDA_ERR_CUDA, "out of host memory");
+    m->owner = h;
+    m->row_count = row_count;
+    m->column_count = column_count;
+    m->result_count = shape.results;
+    m->baby = baby_step;
+    m->giant = giant_step;
+    m->dimension = shape.dimension;
+    // slot (r, g, j) holds diagonal baby * g + j of chunk r; slots past the padded dimension are absent (all zero)
+    std::vector<unsigned char> present((size_t)slots, 0);
+    for (int64_t slot = 0; slot < slots; ++slot) present[(size_t)slot] = slot % ((int64_t)giant_step * baby_step) < shape.dimension;
+    cudaError_t e = cudaMalloc(&m->d_plain, row_words * slots * sizeof(u64));
+    if (e == cudaSuccess) e = cudaMalloc(&m->d_present, (size_t)slots);
+    if (e == cudaSuccess) e = upload(m->d_present, present.data(), (size_t)slots);
+    if (e != cudaSuccess) {
+        hecuda_pnns_matrix_destroy(m);
+        return cuda_fail(e, "pnns matrix from values");
+    }
+    // Plaintext.convertToEvalFormat (MatrixMultiplication.swift:206-208), one slab of slots at a time
+    rc = pnns_encode_slabs(c, shape, values, reduce != 0, true, slots, [&](int64_t first, int64_t items, const u64 *d) {
+        return launch_plaintext_to_eval(c, d, c.L, m->d_plain + row_words * first, items, nullptr);
+    });
+    if (rc == HECUDA_OK) {
+        e = cudaStreamSynchronize(nullptr);
+        if (e != cudaSuccess) rc = cuda_fail(e, "pnns matrix from values");
+    }
+    if (rc) {
+        hecuda_pnns_matrix_destroy(m);
+        return rc;
+    }
+    *out = m;
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pnns_matrix_device_buffer(hecuda_pnns_matrix *m, void **device_ptr, uint64_t *bytes) {
+    if (!m || !device_ptr || !bytes) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *device_ptr = m->d_plain;
+    *bytes = (uint64_t)m->result_count * m->giant * m->baby * m->owner->ctx->L * m->owner->ctx->n * sizeof(u64);
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pnns_matrix_present(const hecuda_pnns_matrix *m, uint8_t *out, int64_t capacity) {
+    if (!m || !out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    const int64_t slots = m->result_count * m->giant * m->baby;
+    if (capacity < slots) return fail(HECUDA_ERR_INVALID_ARGUMENT, "capacity below the slot count");
+    CK(cudaMemcpy(out, m->d_present, (size_t)slots, cudaMemcpyDeviceToHost));
+    return HECUDA_OK;
+}
 
 int32_t hecuda_pnns_matrix_create(const hecuda_context *h, const uint64_t *plaintexts, int32_t eval_format,
                                   int64_t row_count, int64_t column_count, int32_t baby_step, int32_t giant_step,
@@ -600,13 +746,9 @@ int32_t hecuda_pnns_matrix_create(const hecuda_context *h, const uint64_t *plain
     *out = nullptr;
     const Context &c = *h->ctx;
     const int64_t n = c.n;
-    if (row_count < 1 || column_count < 1 || column_count > n / 2)  // PnnsError.invalidMatrixDimensions (PlaintextMatrix.swift:429-431)
-        return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
-    int64_t dimension = 1;
-    while (dimension < column_count) dimension <<= 1;
-    if (baby_step < 1 || giant_step < 1 || baby_step < giant_step || (int64_t)baby_step * giant_step < dimension ||
-        (int64_t)baby_step * (giant_step - 1) >= dimension || baby_step >= n / 2)
-        return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongMatrixPacking: babyStep / giantStep do not cover the padded dimension");
+    int64_t dimension = 0;
+    if ((rc = check_dimensions(c, row_count, column_count, dimension))) return rc;
+    if ((rc = check_steps(c, dimension, baby_step, giant_step))) return rc;
     const int64_t results = (row_count + n - 1) / n;  // plaintextsPerColumnCount / resultCiphertextCount
     const int64_t count = dimension * results;       // PlaintextMatrix.plaintextCount, .diagonal (:269-273)
     const int64_t slots = results * giant_step * baby_step;

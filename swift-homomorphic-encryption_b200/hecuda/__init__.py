@@ -100,6 +100,11 @@ SYMBOLS = {
     "hecuda_pir_database_create": (C.c_int32, [_VP, _VP, C.c_int32, _VP, C.c_int64, C.POINTER(_VP)]),
     "hecuda_pir_database_destroy": (C.c_int32, [_VP]),
     "hecuda_pir_database_device_buffer": (C.c_int32, [_VP, C.POINTER(_VP), C.POINTER(C.c_uint64)]),
+    "hecuda_pir_database_present": (C.c_int32, [_VP, _VP, C.c_int64]),
+    "hecuda_pir_process_entries": (C.c_int32, [_VP, _VP, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, C.c_int32, _VP, _VP,
+                                               C.c_int64]),
+    "hecuda_pir_database_create_from_entries": (C.c_int32, [_VP, _VP, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, C.c_int32,
+                                                            C.POINTER(_VP)]),
     "hecuda_mulpir_expand": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP]),
     "hecuda_mulpir_expand_device": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP, _VP]),
     "hecuda_mulpir_compute_response": (C.c_int32, [_VP, _VP, C.POINTER(_VP), C.c_int32, C.POINTER(C.c_int32), C.c_int32,
@@ -120,6 +125,11 @@ SYMBOLS = {
     "hecuda_pnns_matrix_create": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.POINTER(_VP)]),
     "hecuda_pnns_matrix_destroy": (C.c_int32, [_VP]),
     "hecuda_pnns_matrix_result_count": (C.c_int32, [_VP, C.POINTER(C.c_int64)]),
+    "hecuda_pnns_diagonal_plaintexts": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int64, C.c_int64, C.c_int32, _VP]),
+    "hecuda_pnns_matrix_create_from_values": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32,
+                                                          C.POINTER(_VP)]),
+    "hecuda_pnns_matrix_device_buffer": (C.c_int32, [_VP, C.POINTER(_VP), C.POINTER(C.c_uint64)]),
+    "hecuda_pnns_matrix_present": (C.c_int32, [_VP, _VP, C.c_int64]),
     "hecuda_pnns_mul_transpose_vector": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int64, C.c_int32, _VP]),
     "hecuda_pnns_mul_transpose_vector_device": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int64, C.c_int32, _VP, _VP]),
     "hecuda_pnns_mul_transpose_matrix": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int32, C.c_int32, C.POINTER(C.c_int32), _VP,

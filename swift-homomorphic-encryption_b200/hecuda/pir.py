@@ -255,6 +255,24 @@ class ProcessedDatabase:
                                                         self.count, C.byref(h)))
         self._h = h
 
+    @classmethod
+    def _adopt(cls, context: Context, handle: C.c_void_p, count: int) -> "ProcessedDatabase":
+        db = cls.__new__(cls)
+        db.context, db.count, db._h = context, count, handle
+        return db
+
+    def deviceBuffer(self):
+        """(device pointer, bytes) of the resident rows: uint32 words when every ciphertext modulus is below 2^31."""
+        p, n = C.c_void_p(), C.c_uint64(0)
+        _check(load_library().hecuda_pir_database_device_buffer(self._h, C.byref(p), C.byref(n)))
+        return p.value, n.value
+
+    def presentFlags(self) -> np.ndarray:
+        """The resident presence flags (count,): 0 for a nil plaintext the scan skips."""
+        out = np.empty(self.count, dtype=np.uint8)
+        _check(load_library().hecuda_pir_database_present(self._h, _ptr(out), self.count))
+        return out
+
     def close(self):
         if getattr(self, "_h", None) is not None:
             load_library().hecuda_pir_database_destroy(self._h)
@@ -265,6 +283,31 @@ class ProcessedDatabase:
             self.close()
         except Exception:
             pass
+
+
+def _entry_arguments(database: Sequence[bytes], parameter: IndexPirParameter):
+    """The entries as the C ABI takes them: concatenated bytes, entry_count + 1 offsets, and the dimensions."""
+    if len(database) != parameter.entryCount:
+        raise PirError(f"invalidDatabaseEntryCount(entryCount: {len(database)}, expected: {parameter.entryCount})")
+    blobs = [bytes(e) for e in database]
+    offsets = np.zeros(len(blobs) + 1, dtype=np.uint64)
+    offsets[1:] = np.cumsum([len(b) for b in blobs], dtype=np.uint64)
+    data = np.frombuffer(b"".join(blobs) or b"\0", dtype=np.uint8)
+    dims = (C.c_int32 * len(parameter.dimensions))(*parameter.dimensions)
+    return data, offsets, dims
+
+
+def packEntries(database: Sequence[bytes], context: Context, parameter: IndexPirParameter):
+    """MulPirServer.plaintextRows on the device (hecuda_pir_process_entries): the coefficient rows (count x N) and the
+    presence flags (count) of `process`, word for word."""
+    data, offsets, dims = _entry_arguments(database, parameter)
+    count = -(-parameter.encodedEntrySize // bytesPerPlaintext(context)) * int(np.prod(parameter.dimensions, dtype=np.int64))
+    rows = np.empty((count, context.degree), dtype=np.uint64)
+    present = np.empty(count, dtype=np.uint8)
+    _check(load_library().hecuda_pir_process_entries(
+        context._h, _ptr(data), _ptr(offsets), len(offsets) - 1, parameter.entrySizeInBytes,
+        1 if parameter.encodingEntrySize else 0, dims, len(parameter.dimensions), _ptr(rows), _ptr(present), count))
+    return rows, present
 
 
 class PirWire:
@@ -397,6 +440,19 @@ class MulPirServer:
             packed += [None] * (per_chunk - len(packed))
             pieces = [packed[row] for skip in range(columns) for row in range(skip, per_chunk, columns)]
         return _pack_rows(pieces, bits, context.degree)
+
+    @staticmethod
+    def processOnDevice(database: Sequence[bytes], context: Context, parameter: IndexPirParameter) -> ProcessedDatabase:
+        """MulPirServer.process (MulPir.swift:433-556) with the packing on the device as well
+        (hecuda_pir_database_create_from_entries): only the entry bytes cross PCIe.  The resident words equal those of
+        `process(database, context, parameter)`."""
+        data, offsets, dims = _entry_arguments(database, parameter)
+        h = C.c_void_p()
+        _check(load_library().hecuda_pir_database_create_from_entries(
+            context._h, _ptr(data), _ptr(offsets), len(offsets) - 1, parameter.entrySizeInBytes,
+            1 if parameter.encodingEntrySize else 0, dims, len(parameter.dimensions), C.byref(h)))
+        count = -(-parameter.encodedEntrySize // bytesPerPlaintext(context)) * int(np.prod(parameter.dimensions, dtype=np.int64))
+        return ProcessedDatabase._adopt(context, h, count)
 
     def computeResponse(self, query, evaluationKey: EvaluationKey, indicesCount: int = 1) -> np.ndarray:
         """computeResponse(to:using:) -> Response.ciphertexts as (indicesCount, chunkCount, 2, 1, N) (Coeff, modulus q_0).

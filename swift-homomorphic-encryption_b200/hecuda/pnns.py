@@ -255,6 +255,21 @@ class SimdEncoder:
         return self.forwardNtt(plaintexts)[:, self.encodingMatrix]
 
 
+def _signed(values, dimensions: MatrixDimensions) -> np.ndarray:
+    v = np.ascontiguousarray(np.asarray(values, dtype=np.int64)).reshape(-1)
+    if v.size != dimensions.rowCount * dimensions.columnCount:
+        raise PnnsError(f"wrongValueCount(got: {v.size}, expected: {dimensions.rowCount * dimensions.columnCount})")
+    return v
+
+
+def centeredToRemainder(values, modulus: int) -> np.ndarray:
+    """Scalar.centeredToRemainder (ModularArithmetic/Scalar.swift:85-95): x in [-floor(t/2), floor((t-1)/2)] -> x mod t."""
+    v = np.asarray(values, dtype=np.int64)
+    if v.size and (int(v.max()) > (modulus - 1) // 2 or int(v.min()) < -(modulus // 2)):
+        raise PnnsError("centeredToRemainder: value outside [-floor(t/2), floor((t-1)/2)]")
+    return np.where(v < 0, v + modulus, v).astype(np.uint64)
+
+
 class PlaintextMatrix:
     """PlaintextMatrix<Bfv<UInt64>, Eval> in .diagonal packing, resident in HBM."""
 
@@ -277,6 +292,50 @@ class PlaintextMatrix:
                                                        C.byref(h)))
         self._h = h
         self.resultCiphertextCount = -(-dimensions.rowCount // context.degree)
+
+    @classmethod
+    def fromSignedValues(cls, context: Context, dimensions: MatrixDimensions, signedValues,
+                         babyStepGiantStep: BabyStepGiantStep = None, reduce: bool = False) -> "PlaintextMatrix":
+        """PlaintextMatrix.init(context:dimensions:packing: .diagonal, signedValues:reduce:) (PlaintextMatrix.swift:155-190)
+        followed by convertToEvalFormat, all on the device (hecuda_pnns_matrix_create_from_values): only the values
+        cross PCIe.  The resident words equal those of `PlaintextMatrix(context, dimensions, v)` with each value v
+        mapped by centeredToRemainder (or reduced mod t with `reduce`)."""
+        bsgs = babyStepGiantStep or BabyStepGiantStep.forVectorDimension(dimensions.columnCount)
+        values = _signed(signedValues, dimensions)
+        h = C.c_void_p()
+        _check(load_library().hecuda_pnns_matrix_create_from_values(
+            context._h, _ptr(values), 1 if reduce else 0, dimensions.rowCount, dimensions.columnCount, bsgs.babyStep,
+            bsgs.giantStep, C.byref(h)))
+        m = cls.__new__(cls)
+        m.context, m.dimensions, m.babyStepGiantStep, m._h = context, dimensions, bsgs, h
+        m.resultCiphertextCount = -(-dimensions.rowCount // context.degree)
+        return m
+
+    @staticmethod
+    def diagonalPlaintextsOnDevice(context: Context, dimensions: MatrixDimensions, bsgs: BabyStepGiantStep, signedValues,
+                                   reduce: bool = False) -> np.ndarray:
+        """diagonalPlaintexts of signed values on the device (hecuda_pnns_diagonal_plaintexts): count x N coefficient
+        rows, equal to `diagonalPlaintexts(context, dimensions, bsgs, centeredToRemainder(signedValues))`."""
+        values = _signed(signedValues, dimensions)
+        count = _next_power_of_two(dimensions.columnCount) * -(-dimensions.rowCount // context.degree)
+        out = np.empty((count, context.degree), dtype=np.uint64)
+        _check(load_library().hecuda_pnns_diagonal_plaintexts(context._h, _ptr(values), 1 if reduce else 0,
+                                                              dimensions.rowCount, dimensions.columnCount, bsgs.babyStep,
+                                                              _ptr(out)))
+        return out
+
+    def deviceBuffer(self):
+        """(device pointer, bytes) of the resident [result][giant][baby] x L x N Eval words."""
+        p, n = C.c_void_p(), C.c_uint64(0)
+        _check(load_library().hecuda_pnns_matrix_device_buffer(self._h, C.byref(p), C.byref(n)))
+        return p.value, n.value
+
+    def presentFlags(self) -> np.ndarray:
+        """The resident presence flags in [result][giant][baby] slot order: 0 for an absent plaintext."""
+        count = self.resultCiphertextCount * self.babyStepGiantStep.giantStep * self.babyStepGiantStep.babyStep
+        out = np.empty(count, dtype=np.uint8)
+        _check(load_library().hecuda_pnns_matrix_present(self._h, _ptr(out), count))
+        return out
 
     @staticmethod
     def diagonalPlaintexts(context, dimensions: MatrixDimensions, bsgs: BabyStepGiantStep, values) -> np.ndarray:
