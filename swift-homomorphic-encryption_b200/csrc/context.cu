@@ -96,6 +96,15 @@ static DivRoundConsts build_divround(const std::vector<u64> &base) {
     return c;
 }
 
+// PolyContext.maxLazyProductAccumulationCount (PolyContext.swift:246-253): the largest count of products
+// (q_max - 1)^2 that, added to q_max, stays within the double word of the scalar type
+static int64_t max_lazy_product_count(u64 qmax, int word_bits) {
+    if (qmax < 2) return INT64_MAX;
+    const u128 double_max = word_bits == 64 ? ~(u128)0 : (u128)~(u64)0;
+    const u128 count = (double_max - qmax) / ((u128)(qmax - 1) * (qmax - 1));
+    return count > (u128)INT64_MAX ? INT64_MAX : (int64_t)count;
+}
+
 Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, std::string &err, int word_bits) {
     if (word_bits != 64 && word_bits != 32) { err = "invalidEncryptionParameters: word size must be 32 or 64"; return nullptr; }
     for (int i = 0; i < nmod; ++i)  // Modulus<T>.max = 2^(bitWidth - 2) - 1, Sources/ModularArithmetic/Modulus.swift:177-180
@@ -111,6 +120,14 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
     for (int i = 0; i < nmod; ++i)
         for (int j = 0; j < i; ++j)
             if (coeff_moduli[i] == coeff_moduli[j]) { err = "coprimeModuli: repeated coefficient modulus"; return nullptr; }
+    if (nmod >= 2) {  // the largest key-switching context holds every modulus (Context.swift:114-124)
+        u64 qmax = 0;
+        for (int i = 0; i < nmod; ++i) qmax = coeff_moduli[i] > qmax ? coeff_moduli[i] : qmax;
+        if (nmod >= max_lazy_product_count(qmax, word_bits)) {
+            err = "invalidEncryptionParameters: " + std::to_string(nmod) + " moduli reach maxLazyProductAccumulationCount of the key-switching context";
+            return nullptr;
+        }
+    }
 
     Context *c = new Context();
     c->n = n;

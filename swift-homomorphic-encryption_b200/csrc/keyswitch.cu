@@ -20,7 +20,15 @@ struct KsMacConsts {
 
 // prod[item][comp][r][.] = [ sum_j dig[item][r][j][.] * key[j][comp][keyrow(r)][.] ]_{m_r} * 2^-64   (Bfv+Keys.swift:180-202)
 // 128-bit lazy accumulation like the reference (:187-190), one Montgomery reduction; the 2^-64 is undone by the
-// kScaleMont scaling of the inverse NTT that follows.  sum < l p^2 < 2^127, reduced value < (1 + l/4) p <= 5p.
+// kScaleMont scaling of the inverse NTT that follows.  The sum is below l p^2, so its high word is below l p / 4 < 4p
+// (context.cu keeps l below maxLazyProductAccumulationCount: l <= 14 at 62 bits, and l <= 31 at 61 bits and below).
+// Montgomery's result is below high word + p, which at l >= 13 and 62 bits would pass 2^64; subtracting 2p 2^64 (a
+// multiple of p) from a sum whose high word is >= 2p keeps it below 3p.
+__device__ __forceinline__ u64 ks_reduce(u128 acc, u64 p, u64 ninv) {
+    if ((u64)(acc >> 64) >= 2 * p) acc -= (u128)(2 * p) << 64;
+    return csub(csub(mont_reduce(acc, p, ninv), 2 * p), p);
+}
+
 // CLIENT_KEYS: item i (counted from keys.item0) uses keys.key[i / keys.items_per_client] instead of `key`; the table
 // lives in the parameter block, so switching many clients' items in one launch needs no upload.
 template <bool CLIENT_KEYS>
@@ -48,11 +56,8 @@ __global__ void __launch_bounds__(128) ks_mac_kernel(const u64 *__restrict__ dig
         mac128(a11, dv.y, k1.y);
     }
     u64 *o = prod + ((item * 2) * (l + 1) + r) * n + coeff;
-    *reinterpret_cast<ulonglong2 *>(o) = make_ulonglong2(csub(csub(csub(mont_reduce(a00, p, ninv), 4 * p), 2 * p), p),
-                                                        csub(csub(csub(mont_reduce(a01, p, ninv), 4 * p), 2 * p), p));
-    *reinterpret_cast<ulonglong2 *>(o + (int64_t)(l + 1) * n) =
-        make_ulonglong2(csub(csub(csub(mont_reduce(a10, p, ninv), 4 * p), 2 * p), p),
-                        csub(csub(csub(mont_reduce(a11, p, ninv), 4 * p), 2 * p), p));
+    *reinterpret_cast<ulonglong2 *>(o) = make_ulonglong2(ks_reduce(a00, p, ninv), ks_reduce(a01, p, ninv));
+    *reinterpret_cast<ulonglong2 *>(o + (int64_t)(l + 1) * n) = make_ulonglong2(ks_reduce(a10, p, ninv), ks_reduce(a11, p, ninv));
 }
 
 // divide-and-round by the last modulus of `in` (rows c.l), optionally adding `base`, write c.l - 1 rows
