@@ -333,6 +333,80 @@ int32_t hecuda_pir_database_create_from_entries(const hecuda_context *ctx, const
                                                 int64_t entry_count, int64_t entry_size, int32_t encode_entry_size,
                                                 const int32_t *dims, int32_t dim_count, hecuda_pir_database **out);
 
+/* ---- Keyword PIR: KeywordPir/HashBucket.swift, CuckooTable.swift, KeywordPirProtocol.swift ------------------------
+ * Keywords and values are passed as concatenated bytes with count + 1 byte offsets (row i = [offsets[i], offsets[i+1])).
+ * Errors are HECUDA_ERR_INVALID_ARGUMENT with the reference's error name in hecuda_last_error(); on error *out is NULL
+ * and nothing stays allocated. */
+
+/* HashKeyword.hash (HashBucket.swift:264-269): hashes[i] = the first 8 bytes of SHA-256(keyword i) as a little-endian
+ * UInt64, one device thread per keyword.  Keyword.shardIndex (KeywordDatabase.swift:56-62) is hashes[i] % shardCount. */
+int32_t hecuda_keyword_hash(const uint8_t *keywords, const uint64_t *offsets, int64_t count, uint64_t *hashes);
+/* HashKeyword.hashIndices (HashBucket.swift:221-257) of each keyword hash: out = count x hash_function_count candidate
+ * bucket indices in [0, bucket_count), each retried with counters 1..10 while it repeats an earlier candidate. */
+int32_t hecuda_keyword_hash_indices(const uint64_t *hashes, int64_t count, int64_t bucket_count,
+                                    int32_t hash_function_count, int64_t *out);
+
+typedef struct hecuda_cuckoo_table hecuda_cuckoo_table; /* CuckooTable, CuckooTable.swift:256-505 */
+/* CuckooTableConfig (CuckooTable.swift:19-157).  fixed_bucket_count = 0 selects .allowExpansion(expansion_factor,
+ * target_load_factor), otherwise .fixedSize(fixed_bucket_count).  defaultKeywordPir is {2, 100, size, 255, 1, 0, 1.1, 0.9}. */
+typedef struct hecuda_cuckoo_config {
+    int32_t hash_function_count;
+    int64_t max_eviction_count;
+    int64_t max_serialized_bucket_size;
+    int32_t slot_count;       /* <= 255 (HashBucket.maxSlotCount) */
+    int32_t multiple_tables;  /* one table per hash function */
+    int64_t fixed_bucket_count;
+    double expansion_factor;
+    double target_load_factor;
+} hecuda_cuckoo_config;
+/* The generator behind CuckooTable's randomElement(using:) evictions, drawn through Swift's next(upperBound:).
+ * COUNTER(seed) is _TestUtilities' TestRng(counter: seed) (TestUtilities.swift:45-61), which reproduces the reference's
+ * tests; SPLITMIX64(seed) is the production choice (the reference's SystemRandomNumberGenerator is not reproducible). */
+enum { HECUDA_CUCKOO_RNG_COUNTER = 0, HECUDA_CUCKOO_RNG_SPLITMIX64 = 1 };
+typedef struct hecuda_cuckoo_summary {
+    int64_t entry_count, bucket_count, buckets_per_table, empty_bucket_count;
+    int64_t serialized_bytes;          /* sum of the serialized bucket sizes */
+    int64_t max_serialized_bucket_size; /* the largest one: CuckooTable.maxSerializedBucketSize() */
+} hecuda_cuckoo_summary;
+
+/* CuckooTable.init(config:database:using:) (CuckooTable.swift:328-357, insert / insertLoop :386-458, expand :466-490):
+ * the rows inserted in the order given.  The keywords are hashed on the device once and the candidate indices of every
+ * row are computed on the device once per bucket count the placement reaches; the eviction loop itself runs on the host,
+ * because the table depends on the order of the generator's draws.  The values are uploaded once and stay on the device
+ * with the table.
+ * One deliberate divergence: when no candidate bucket has a swap index, the reference expands the table and returns
+ * without inserting the pair in hand (:455-457), losing that row; here the pair is inserted again after the expansion,
+ * as the branch at :402-406 does.  The tables are identical whenever that branch is not taken.
+ * Refused: invalidCuckooConfig (validate, :138-156, plus a target load factor <= 0 and, with expansion, a
+ * max_eviction_count < 1, both of which the reference cannot build a table with), an unknown rng, decreasing offsets,
+ * invalidHashBucketEntryValueSize (a value over 65535 bytes) and failedToConstructCuckooTable (a value too large for
+ * any bucket, or a fixed-size table that overflows).  Rows repeating a keyword after the first are skipped, as in the
+ * reference. */
+int32_t hecuda_cuckoo_table_create(const hecuda_context *ctx, const uint8_t *keywords, const uint64_t *keyword_offsets,
+                                   const uint8_t *values, const uint64_t *value_offsets, int64_t count,
+                                   const hecuda_cuckoo_config *config, int32_t rng, uint64_t seed,
+                                   hecuda_cuckoo_table **out);
+/* The inputs of CuckooTable.summarize() (:361-373; loadFactor = Float(serialized_bytes) / Float(bucket_count *
+ * maxSerializedBucketSize)) and of maxSerializedBucketSize() (:381-383). */
+int32_t hecuda_cuckoo_table_summarize(const hecuda_cuckoo_table *table, hecuda_cuckoo_summary *out);
+/* CuckooTable.serializeBuckets() (:376-378): bucket b's HashBucket bytes (HashBucket.swift:89-103, 176-187: slot count,
+ * then per slot the keyword hash, the value length and the value) are bytes[offsets[b], offsets[b+1]).  offsets holds
+ * bucket_count + 1 entries; capacity >= serialized_bytes.  The bytes are written by a device kernel. */
+int32_t hecuda_cuckoo_table_serialize_buckets(const hecuda_cuckoo_table *table, uint8_t *bytes, uint64_t capacity,
+                                              uint64_t *offsets);
+int32_t hecuda_cuckoo_table_destroy(hecuda_cuckoo_table *table);
+
+/* KeywordPirServer.process (KeywordPirProtocol.swift:191-247) after its IndexPirParameter: out[t] (t < hash function
+ * count) is table t's MulPir database, word for word what hecuda_pir_database_create_from_entries builds from that
+ * table's serialized buckets with entry_size, encode_entry_size = 0 and dims (uint32 rows on contexts whose moduli are
+ * below 2^31 included).  The buckets are serialized on the device and each table's slice of them is packed and converted
+ * to Eval there: bucket bytes never cross PCIe.  Needs a table built with multiple_tables (KeywordPirConfig,
+ * :75-77: invalidCuckooConfig otherwise) and the context the table was built on.  Answer with
+ * hecuda_mulpir_compute_response* over the hash-function-count databases with indices_count = hash function count. */
+int32_t hecuda_keyword_pir_databases_create(const hecuda_context *ctx, const hecuda_cuckoo_table *table,
+                                            int64_t entry_size, const int32_t *dims, int32_t dim_count,
+                                            hecuda_pir_database **out);
+
 /* PirUtil.expand(ciphertexts:outputCount:using:) -- IndexPir/PirUtil.swift:321-355 (expandCiphertext :249-304,
  * expandCiphertextForOneStep :204-236).  ciphertexts: ciphertext_count x 2 x L x N (Coeff); out: output_count x 2 x L x N,
  * output i encrypting the constant polynomial whose constant is coefficient i of the inputs (x 2^ceilLog2(count)).

@@ -162,6 +162,10 @@ cudaError_t expand_seeded_keys_device(const Context &c, const unsigned char *d_p
                                       u64 *const *d_dst, int64_t count, cudaStream_t s);
 cudaError_t inner_product_chunk(const Context &c, u64 *scratch, const u64 *lhs, const u64 *rhs, int64_t pairs, u64 *out,
                                 int64_t groups, cudaStream_t s);
+// `tables` MulPir databases from entry bytes already on the device (pir.cu; used by keyword_pir.cu)
+int32_t pir_databases_from_device_entries(const hecuda_context *h, const unsigned char *d_entries, const uint64_t *h_offsets,
+                                          const uint64_t *d_offsets, int64_t per_table, int tables, int64_t entry_size,
+                                          const int32_t *dims, int32_t dim_count, hecuda_pir_database **out);
 
 }  // namespace api
 }  // namespace hecuda

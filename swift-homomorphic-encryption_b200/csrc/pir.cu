@@ -827,16 +827,32 @@ int32_t pir_process_shape(const hecuda_context *h, const uint8_t *entries, const
     return HECUDA_OK;
 }
 
-// Uploads the entry bytes (and offsets) once, then packs the `count` plaintexts slab by slab on the default stream:
-// present flags into d_present[count], each slab's coefficients handed to sink(first, items, d_coeff).  Frees its
-// buffers before it returns.
+// Packs the `count` plaintexts of a database whose entry bytes (and offsets) are already on the device (`s` holds the
+// device pointers) slab by slab on the default stream: present flags into d_present[count], each slab's coefficients
+// handed to sink(first, items, d_coeff).
+template <class Sink>
+cudaError_t pir_pack_device_slabs(const Context &c, const procdb::PirShape &s, int64_t count, unsigned char *d_present,
+                                  Sink sink) {
+    u64 *d_coeff = nullptr;
+    const int64_t slab = coefficient_slab(c);
+    cudaError_t e = cudaMalloc(&d_coeff, (size_t)std::max<int64_t>(1, std::min(slab, count)) * c.n * sizeof(u64));
+    for (int64_t done = 0; e == cudaSuccess && done < count; done += slab) {
+        const int64_t items = std::min(slab, count - done);
+        e = launch_pir_pack(s, (int)c.n, done, items, d_coeff, d_present + done, nullptr);
+        if (e == cudaSuccess) e = sink(done, items, d_coeff);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
+    cudaFree(d_coeff);
+    return e;
+}
+
+// Uploads the entry bytes (and offsets) once, then packs them with pir_pack_device_slabs.  Frees its buffers before it
+// returns.
 template <class Sink>
 cudaError_t pir_pack_slabs(const Context &c, procdb::PirShape s, const uint8_t *entries, const uint64_t *offsets,
                            size_t bytes, int64_t count, unsigned char *d_present, Sink sink) {
     unsigned char *d_entries = nullptr;
     uint64_t *d_offsets = nullptr;
-    u64 *d_coeff = nullptr;
-    const int64_t slab = coefficient_slab(c);
     cudaError_t e = cudaMalloc(&d_entries, std::max<size_t>(bytes, 1));
     if (e == cudaSuccess && bytes) e = upload(d_entries, entries, bytes);
     if (e == cudaSuccess && offsets) {
@@ -846,20 +862,73 @@ cudaError_t pir_pack_slabs(const Context &c, procdb::PirShape s, const uint8_t *
     }
     s.entries = d_entries;
     s.offsets = d_offsets;
-    if (e == cudaSuccess) e = cudaMalloc(&d_coeff, (size_t)std::min(slab, count) * c.n * sizeof(u64));
-    for (int64_t done = 0; e == cudaSuccess && done < count; done += slab) {
-        const int64_t items = std::min(slab, count - done);
-        e = launch_pir_pack(s, (int)c.n, done, items, d_coeff, d_present + done, nullptr);
-        if (e == cudaSuccess) e = sink(done, items, d_coeff);
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
-    cudaFree(d_coeff);
+    if (e == cudaSuccess) e = pir_pack_device_slabs(c, s, count, d_present, sink);
     cudaFree(d_offsets);
     cudaFree(d_entries);
     return e;
 }
 
+// Plaintext.convertToEvalFormat (Plaintext.swift:149-171) of every packed slab, straight into the database's rows
+cudaError_t pir_fill_database(const Context &c, const procdb::PirShape &device_shape, hecuda_pir_database *db) {
+    const size_t row_words = (size_t)c.L * c.n;
+    cudaError_t e = cudaMalloc(&db->d_plain, row_words * db->count * sizeof(u64));
+    if (e == cudaSuccess) e = cudaMalloc(&db->d_present, (size_t)db->count);
+    if (e == cudaSuccess)
+        e = pir_pack_device_slabs(c, device_shape, db->count, db->d_present, [&](int64_t first, int64_t items, const u64 *d) {
+            return launch_plaintext_to_eval(c, d, c.L, db->d_plain + row_words * first, items, nullptr);
+        });
+    return e;
+}
+
 }  // namespace
+
+namespace hecuda {
+namespace api {
+
+// hecuda_keyword_pir_databases_create's databases (keyword_pir.cu): `tables` MulPir databases, table t made of entries
+// [t * per_table, (t + 1) * per_table) of device bytes d_entries with global offsets (h_offsets on the host, d_offsets
+// on the device).  Each database is word for word what hecuda_pir_database_create_from_entries builds from the same
+// entries with encode_entry_size = 0.  On error every out[t] is NULL and nothing stays allocated.
+int32_t pir_databases_from_device_entries(const hecuda_context *h, const unsigned char *d_entries, const uint64_t *h_offsets,
+                                          const uint64_t *d_offsets, int64_t per_table, int tables, int64_t entry_size,
+                                          const int32_t *dims, int32_t dim_count, hecuda_pir_database **out) {
+    for (int t = 0; t < tables; ++t) out[t] = nullptr;
+    std::vector<procdb::PirShape> shapes((size_t)tables);
+    int64_t count = 0;
+    for (int t = 0; t < tables; ++t) {
+        size_t bytes = 0;
+        int32_t rc = pir_process_shape(h, d_entries, h_offsets + (size_t)t * per_table, per_table, entry_size, 0, dims,
+                                       dim_count, shapes[t], bytes, count);
+        if (rc) return rc;
+        shapes[t].entries = d_entries;
+        shapes[t].offsets = d_offsets + (size_t)t * per_table;
+    }
+    const Context &c = *h->ctx;
+    cudaError_t e = cudaSuccess;
+    for (int t = 0; t < tables && e == cudaSuccess; ++t) {
+        hecuda_pir_database *db = new (std::nothrow) hecuda_pir_database();
+        if (!db) {
+            e = cudaErrorMemoryAllocation;
+            break;
+        }
+        db->owner = h;
+        db->count = count;
+        out[t] = db;
+        e = pir_fill_database(c, shapes[t], db);
+        if (e == cudaSuccess) e = narrow_database(c, db);
+    }
+    if (e != cudaSuccess) {
+        for (int t = 0; t < tables; ++t) {
+            if (out[t]) hecuda_pir_database_destroy(out[t]);
+            out[t] = nullptr;
+        }
+        return cuda_fail(e, "keyword pir databases");
+    }
+    return HECUDA_OK;
+}
+
+}  // namespace api
+}  // namespace hecuda
 
 extern "C" {
 
@@ -899,17 +968,24 @@ int32_t hecuda_pir_database_create_from_entries(const hecuda_context *h, const u
                                    bytes, count);
     if (rc) return rc;
     const Context &c = *h->ctx;
-    const size_t row_words = (size_t)c.L * c.n;
     hecuda_pir_database *db = new (std::nothrow) hecuda_pir_database();
     if (!db) return fail(HECUDA_ERR_CUDA, "out of host memory");
     db->owner = h;
     db->count = count;
-    cudaError_t e = cudaMalloc(&db->d_plain, row_words * count * sizeof(u64));
-    if (e == cudaSuccess) e = cudaMalloc(&db->d_present, (size_t)count);
-    if (e == cudaSuccess)  // Plaintext.convertToEvalFormat (Plaintext.swift:149-171), one slab at a time
-        e = pir_pack_slabs(c, s, entries, offsets, bytes, count, db->d_present, [&](int64_t first, int64_t items, const u64 *d) {
-            return launch_plaintext_to_eval(c, d, c.L, db->d_plain + row_words * first, items, nullptr);
-        });
+    unsigned char *d_entries = nullptr;
+    uint64_t *d_offsets = nullptr;
+    cudaError_t e = cudaMalloc(&d_entries, std::max<size_t>(bytes, 1));
+    if (e == cudaSuccess && bytes) e = upload(d_entries, entries, bytes);
+    if (e == cudaSuccess && offsets) {
+        const size_t offset_bytes = (size_t)(entry_count + 1) * sizeof(uint64_t);
+        e = cudaMalloc(&d_offsets, offset_bytes);
+        if (e == cudaSuccess) e = upload(d_offsets, offsets, offset_bytes);
+    }
+    s.entries = d_entries;
+    s.offsets = d_offsets;
+    if (e == cudaSuccess) e = pir_fill_database(c, s, db);  // one slab at a time
+    cudaFree(d_offsets);
+    cudaFree(d_entries);
     if (e == cudaSuccess) e = narrow_database(c, db);
     if (e != cudaSuccess) {
         hecuda_pir_database_destroy(db);

@@ -105,6 +105,14 @@ SYMBOLS = {
                                                C.c_int64]),
     "hecuda_pir_database_create_from_entries": (C.c_int32, [_VP, _VP, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, C.c_int32,
                                                             C.POINTER(_VP)]),
+    "hecuda_keyword_hash": (C.c_int32, [_VP, _VP, C.c_int64, _VP]),
+    "hecuda_keyword_hash_indices": (C.c_int32, [_VP, C.c_int64, C.c_int64, C.c_int32, _VP]),
+    "hecuda_cuckoo_table_create": (C.c_int32, [_VP, _VP, _VP, _VP, _VP, C.c_int64, _VP, C.c_int32, C.c_uint64,
+                                               C.POINTER(_VP)]),
+    "hecuda_cuckoo_table_summarize": (C.c_int32, [_VP, _VP]),
+    "hecuda_cuckoo_table_serialize_buckets": (C.c_int32, [_VP, _VP, C.c_uint64, _VP]),
+    "hecuda_cuckoo_table_destroy": (C.c_int32, [_VP]),
+    "hecuda_keyword_pir_databases_create": (C.c_int32, [_VP, _VP, C.c_int64, _VP, C.c_int32, _VP]),
     "hecuda_mulpir_expand": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP]),
     "hecuda_mulpir_expand_device": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP, _VP]),
     "hecuda_mulpir_compute_response": (C.c_int32, [_VP, _VP, C.POINTER(_VP), C.c_int32, C.POINTER(C.c_int32), C.c_int32,
