@@ -17,7 +17,12 @@
  *   - Pointers are borrowed for the duration of the call only.  Functions without a `_device` suffix take HOST
  *     pointers and return when the outputs are complete; `_device` variants take device pointers on the current
  *     device and enqueue on `stream` (a cudaStream_t passed as void*; NULL = the legacy default stream) without
- *     synchronizing.
+ *     synchronizing.  Every kernel and copy of a `_device` call runs on `stream`, and its scratch is allocated and
+ *     freed stream-ordered there (cudaMallocAsync / cudaFreeAsync), so the calls can be captured into a CUDA graph;
+ *     make one call with a shape before capturing it (the first call sets kernel attributes).  Device buffers must
+ *     be 16-byte aligned (the TMA row copies and the 16-byte vector loads rely on it; cudaMalloc and torch give
+ *     256-byte alignment).  Exceptions are stated at the entry point (hecuda_poly_mul_scalars_device takes its
+ *     scalars on the host).
  *   - Return value: HECUDA_OK or a negative status; hecuda_last_error() gives the message for the calling thread
  *     (maps onto the reference's `throws HeError`, Sources/HomomorphicEncryption/Error.swift:17-54).
  *   - All entry points are thread-safe (HeScheme statics are called from concurrent TaskGroup tasks,
@@ -617,6 +622,8 @@ int32_t hecuda_poly_mul_device(const hecuda_context *ctx, int32_t base, uint64_t
                                int32_t row_count, int64_t poly_count, void *stream);
 int32_t hecuda_poly_neg_device(const hecuda_context *ctx, int32_t base, uint64_t *data, int32_t row_count,
                                int64_t poly_count, void *stream);
+/* scalars: a HOST array of row_count values, scalars[r] < the modulus of row r (read when the call is made), also for
+ * the _device variant; only data is a device buffer. */
 int32_t hecuda_poly_mul_scalars_device(const hecuda_context *ctx, int32_t base, uint64_t *data, const uint64_t *scalars,
                                        int32_t row_count, int64_t poly_count, void *stream);
 

@@ -626,41 +626,43 @@ __global__ void __launch_bounds__(256) ntt_split_forward_kernel(const u64 *__res
                                                                const __grid_constant__ SplitRows sr, int polys, int logn) {
     const int64_t n = (int64_t)1 << logn, half = n >> 1;
     const int which = blockIdx.y;
-    const int64_t poly = blockIdx.z;
     const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;  // two adjacent coefficients per thread
     if (i >= half) return;
     const ModSlot &S = slots[sr.slot[which]];
     const u64 p = S.p;
     const ulonglong2 w = S.tw[1];
-    const u64 *src = in + poly * sr.src_poly_stride + ((int64_t)sr.src_row[which] << logn) + i;
-    u64 *dst = out + (((poly * sr.rows_per_poly) + sr.row[which]) << logn) + i;
-    ulonglong2 x = *reinterpret_cast<const ulonglong2 *>(src), y = *reinterpret_cast<const ulonglong2 *>(src + half);
-    if (sr.reduce_in[which]) {  // gathered key-switch digit: residues of another modulus (Bfv+Keys.swift:168-172)
-        x.x = barrett64(x.x, p, S.mu1), x.y = barrett64(x.y, p, S.mu1);
-        y.x = barrett64(y.x, p, S.mu1), y.y = barrett64(y.y, p, S.mu1);
+    for (int64_t poly = blockIdx.z; poly < polys; poly += gridDim.z) {  // grid z is capped at 65535
+        const u64 *src = in + poly * sr.src_poly_stride + ((int64_t)sr.src_row[which] << logn) + i;
+        u64 *dst = out + (((poly * sr.rows_per_poly) + sr.row[which]) << logn) + i;
+        ulonglong2 x = *reinterpret_cast<const ulonglong2 *>(src), y = *reinterpret_cast<const ulonglong2 *>(src + half);
+        if (sr.reduce_in[which]) {  // gathered key-switch digit: residues of another modulus (Bfv+Keys.swift:168-172)
+            x.x = barrett64(x.x, p, S.mu1), x.y = barrett64(x.y, p, S.mu1);
+            y.x = barrett64(y.x, p, S.mu1), y.y = barrett64(y.y, p, S.mu1);
+        }
+        const u64 v0 = shoup_mul(y.x, w.x, w.y, p), v1 = shoup_mul(y.y, w.x, w.y, p);
+        *reinterpret_cast<ulonglong2 *>(dst) = make_ulonglong2(add_mod(x.x, v0, p), add_mod(x.y, v1, p));
+        *reinterpret_cast<ulonglong2 *>(dst + half) = make_ulonglong2(sub_mod(x.x, v0, p), sub_mod(x.y, v1, p));
     }
-    const u64 v0 = shoup_mul(y.x, w.x, w.y, p), v1 = shoup_mul(y.y, w.x, w.y, p);
-    *reinterpret_cast<ulonglong2 *>(dst) = make_ulonglong2(add_mod(x.x, v0, p), add_mod(x.y, v1, p));
-    *reinterpret_cast<ulonglong2 *>(dst + half) = make_ulonglong2(sub_mod(x.x, v0, p), sub_mod(x.y, v1, p));
 }
 __global__ void __launch_bounds__(256) ntt_merge_inverse_kernel(u64 *__restrict__ data, const ModSlot *__restrict__ slots,
                                                                const __grid_constant__ SplitRows sr, int polys, int logn,
                                                                int scale_mode) {
     const int64_t n = (int64_t)1 << logn, half = n >> 1;
     const int which = blockIdx.y;
-    const int64_t poly = blockIdx.z;
     const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;
     if (i >= half) return;
     const ModSlot &S = slots[sr.slot[which]];
     const u64 p = S.p;
     const ModSlot::InvScale sc = S.inv_scale[scale_mode];
-    u64 *row = data + (((poly * sr.rows_per_poly) + sr.row[which]) << logn) + i;
-    const ulonglong2 x = *reinterpret_cast<const ulonglong2 *>(row), y = *reinterpret_cast<const ulonglong2 *>(row + half);
-    // (x + y) N^-1 and (x - y) N^-1 psi^-(N/2), each times the scaling of scale_mode (PolyRq+Ntt.swift:416-419)
-    *reinterpret_cast<ulonglong2 *>(row) =
-        make_ulonglong2(shoup_mul(x.x + y.x, sc.c0, sc.c0p, p), shoup_mul(x.y + y.y, sc.c0, sc.c0p, p));
-    *reinterpret_cast<ulonglong2 *>(row + half) =
-        make_ulonglong2(shoup_mul(x.x - y.x + p, sc.c1, sc.c1p, p), shoup_mul(x.y - y.y + p, sc.c1, sc.c1p, p));
+    for (int64_t poly = blockIdx.z; poly < polys; poly += gridDim.z) {  // grid z is capped at 65535
+        u64 *row = data + (((poly * sr.rows_per_poly) + sr.row[which]) << logn) + i;
+        const ulonglong2 x = *reinterpret_cast<const ulonglong2 *>(row), y = *reinterpret_cast<const ulonglong2 *>(row + half);
+        // (x + y) N^-1 and (x - y) N^-1 psi^-(N/2), each times the scaling of scale_mode (PolyRq+Ntt.swift:416-419)
+        *reinterpret_cast<ulonglong2 *>(row) =
+            make_ulonglong2(shoup_mul(x.x + y.x, sc.c0, sc.c0p, p), shoup_mul(x.y + y.y, sc.c0, sc.c0p, p));
+        *reinterpret_cast<ulonglong2 *>(row + half) =
+            make_ulonglong2(shoup_mul(x.x - y.x + p, sc.c1, sc.c1p, p), shoup_mul(x.y - y.y + p, sc.c1, sc.c1p, p));
+    }
 }
 
 template <bool INVERSE>
@@ -695,7 +697,8 @@ static cudaError_t launch_split(const Context &ctx, const NttRowMap &map, const 
             rl.flags[j] = (unsigned char)((full.flags[i] & 7) | (INVERSE ? 16 : 0));
         }
     }
-    const dim3 egrid((unsigned)((ctx.n / 4 + 255) / 256), (unsigned)full.count, (unsigned)polys);
+    // the split and merge kernels loop over the polynomials past grid z's limit
+    const dim3 egrid((unsigned)((ctx.n / 4 + 255) / 256), (unsigned)full.count, (unsigned)std::min(polys, 65535));
     if (!INVERSE) {
         ++g_kernel_launches;
         ntt_split_forward_kernel<<<egrid, 256, 0, stream>>>(in, out, ctx.d_slots, sr, polys, ctx.logn);
