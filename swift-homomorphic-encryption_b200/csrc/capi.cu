@@ -1,8 +1,10 @@
 // capi.cu -- the C ABI declared in include/hecuda.h.  No torch types, no exceptions across the boundary.
 //
-// Host-pointer entry points run a chunked, double-buffered pipeline (two workspaces on two streams) so that the
-// H2D copy of chunk k+1, the kernels of chunk k and the D2H copy of chunk k-1 overlap when the caller's buffers are
-// pinned.  Device-pointer entry points enqueue on the caller's stream and do not synchronize.
+// Each batched operation is described once (a Batched: per-item buffer sizes, chunk sizes and a body that runs a run of
+// items on the device) and run three ways.  Host-pointer entry points run it through a pipeline of three workspaces on
+// three streams, so that the H2D copy of stage k+1, the kernels of stage k and the D2H copy of stage k-1 overlap when
+// the caller's buffers are pinned; the hecuda_u32_ entry points run the same pipeline on uint32 host buffers.
+// Device-pointer entry points enqueue on the caller's stream and do not synchronize.
 #include "../../include/hecuda.h"
 
 #include <cuda_runtime.h>
@@ -15,6 +17,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -203,43 +206,78 @@ size_t inner_product_scratch_words(const Context &c, int64_t pairs) {
 
 namespace {
 
-// The u32 entry points (Bfv<UInt32> contexts) run the same bodies: the calling thread marks its host buffers as uint32
-// for the duration of the call and the pipeline widens after the H2D copy / narrows before the D2H copy.
-thread_local bool tl_io32 = false;
-struct Io32Scope {
-    Io32Scope() { tl_io32 = true; }
-    ~Io32Scope() { tl_io32 = false; }
+// Host buffers of uint64 words, or of uint32 words in the hecuda_u32_ entry points (Bfv<UInt32> contexts): the host
+// pipeline widens those after the H2D copy and narrows the output before the D2H copy.
+enum class Words { u64, u32 };
+
+constexpr int kPipelineDepth = 3;              // host pipeline stages in flight, each on its own stream
+constexpr int64_t kMinStages = 16;             // a batch of 64 or more runs in at least this many stages of >= 16 items
+constexpr size_t kStageWords = 4 * 1024 * 1024;  // per-stage budget of the operations not sized by h->chunk
+constexpr int64_t kWholeBatch = INT64_MAX;     // items per device launch of the operations that launch once
+
+// items per stage when the largest per-item buffer is `words`
+int64_t stage_items(size_t budget, size_t words) { return std::max<int64_t>(1, (int64_t)(budget / words)); }
+
+// One run of items [first, first + items) of a Batched: in[i] and out point at item `first`, scratch holds
+// items x scratch_words.
+struct Chunk {
+    u64 *scratch;
+    int64_t first, items;
+    const u64 *const *in;
+    u64 *out;
+    cudaStream_t stream;
 };
 
-// Generic double-buffered host pipeline: for each chunk, copy inputs in, run `body`, copy outputs out.
-struct HostIo {
-    const u64 *src;  // host
-    size_t words_per_item;
+// One batched operation.  Items lie back to back in every input and in the output; operands shared by every item
+// are uploaded once by the caller and captured by the body.
+struct Batched {
+    const char *name;  // in the device entry points' errors
+    struct Io {
+        const void *p;  // host (uint64 or uint32 words) or device buffer
+        size_t words;   // per item
+    };
+    std::vector<Io> in;
+    void *out;
+    size_t out_words, scratch_words;  // per item
+    int64_t per_launch;               // items per device launch
+    int64_t stage_hint;               // items per host pipeline stage, before host_pipeline's clamp
+    std::function<cudaError_t(const Chunk &)> body;
 };
-template <class Body>
-int32_t host_pipeline(const hecuda_context *h, int64_t batch, int64_t chunk_hint, size_t scratch_words_per_item,
-                      const std::vector<HostIo> &inputs, u64 *host_out, size_t out_words_per_item, Body body) {
+
+// On the caller's device buffers and stream: per_launch items per body call, no host synchronisation, stream-ordered
+// scratch (graph-capturable), nothing launched for an empty batch.
+int32_t run_device(const Batched &op, int64_t batch, cudaStream_t s) {
     if (batch == 0) return HECUDA_OK;
-    // `depth` stages in flight, each on its own stream: H2D of stage k+1.., kernels of stage k, D2H of stage k-1
-    static const int depth = [] {
-        const char *env = std::getenv("HECUDA_PIPELINE_DEPTH");
-        const int d = env ? std::atoi(env) : 3;
-        return d < 1 ? 1 : (d > 8 ? 8 : d);
-    }();
-    static const int64_t min_stages = [] {
-        const char *env = std::getenv("HECUDA_PIPELINE_STAGES");
-        const long long v = env ? std::atoll(env) : 16;
-        return (int64_t)(v < 1 ? 1 : v);
-    }();
+    const int64_t chunk = std::min(op.per_launch, batch);
+    u64 *scratch = nullptr;
+    if (op.scratch_words) CK(cudaMallocAsync(&scratch, op.scratch_words * (size_t)chunk * sizeof(u64), s));
+    std::vector<const u64 *> in(op.in.size());
+    cudaError_t e = cudaSuccess;
+    for (int64_t done = 0; e == cudaSuccess && done < batch; done += chunk) {
+        for (size_t i = 0; i < in.size(); ++i) in[i] = static_cast<const u64 *>(op.in[i].p) + op.in[i].words * (size_t)done;
+        e = op.body({scratch, done, std::min(chunk, batch - done), in.data(),
+                     static_cast<u64 *>(op.out) + op.out_words * (size_t)done, s});
+    }
+    if (e != cudaSuccess) {
+        if (scratch) cudaFreeAsync(scratch, s);
+        return cuda_fail(e, op.name);
+    }
+    if (scratch) CK(cudaFreeAsync(scratch, s));
+    return HECUDA_OK;
+}
+
+// On host buffers: for each stage, copy the inputs in, run the body, copy the output out.
+int32_t host_pipeline(const hecuda_context *h, const Batched &op, int64_t batch, Words words) {
+    if (batch == 0) return HECUDA_OK;
     std::vector<std::unique_ptr<WsGuard>> guards;
     std::vector<Workspace *> ws;
-    for (int i = 0; i < depth; ++i) {
+    for (int i = 0; i < kPipelineDepth; ++i) {
         guards.emplace_back(new WsGuard(h));
         if (!guards.back()->w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
         ws.push_back(guards.back()->w);
     }
-    int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(chunk_hint, batch));
-    if (batch >= 64) chunk = std::min<int64_t>(chunk, std::max<int64_t>(16, (batch + min_stages - 1) / min_stages));
+    int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(op.stage_hint, batch));
+    if (batch >= 64) chunk = std::min<int64_t>(chunk, std::max<int64_t>(16, (batch + kMinStages - 1) / kMinStages));
     // On any early return, earlier stages may still have copies into / out of the caller's buffers in flight on the
     // other streams: wait for all of them so the caller may free or reuse its buffers as soon as it sees the error.
     struct DrainOnExit {
@@ -248,53 +286,68 @@ int32_t host_pipeline(const hecuda_context *h, int64_t batch, int64_t chunk_hint
             for (Workspace *w : ws) wait_stream(w->stream);
         }
     } drain{ws};
+    const bool io32 = words == Words::u32;
     int k = 0;
     for (int64_t done = 0; done < batch; done += chunk, ++k) {
-        Workspace &w = *ws[k % depth];
+        Workspace &w = *ws[k % kPipelineDepth];
         const int64_t items = std::min<int64_t>(chunk, batch - done);
-        // Work on one workspace is ordered by its stream; buffers only ever grow (first `depth` iterations).
-        // slot 0 = kernel scratch, slot 4 = staged inputs (back to back), slot 5 = staged output
+        // Work on one workspace is ordered by its stream; buffers only ever grow (first kPipelineDepth stages).
         size_t in_words = 0;
-        for (const HostIo &io : inputs) in_words += io.words_per_item * (size_t)items;
-        const bool io32 = tl_io32;
-        const size_t out_words = out_words_per_item * (size_t)items;
-        CK(w.reserve(0, scratch_words_per_item * (size_t)items));
-        CK(w.reserve(4, in_words));
-        CK(w.reserve(5, out_words));
-        if (io32) {  // slots 6 / 7: the uint32 images (each input starts on a 16-byte boundary)
-            CK(w.reserve(6, in_words / 2 + inputs.size() * 2 + 2));
-            CK(w.reserve(7, out_words / 2 + 2));
+        for (const Batched::Io &io : op.in) in_words += io.words * (size_t)items;
+        const size_t out_words = op.out_words * (size_t)items;
+        CK(w.scratch.reserve(op.scratch_words * (size_t)items));
+        CK(w.in.reserve(in_words));
+        CK(w.out.reserve(out_words));
+        if (io32) {  // each input's uint32 image starts on a 16-byte boundary
+            CK(w.in32.reserve(in_words / 2 + op.in.size() * 2 + 2));
+            CK(w.out32.reserve(out_words / 2 + 2));
         }
         std::vector<const u64 *> d_in;
         size_t off = 0, off32 = 0;
-        for (const HostIo &io : inputs) {
-            const size_t words = io.words_per_item * (size_t)items;
+        for (const Batched::Io &io : op.in) {
+            const size_t n = io.words * (size_t)items, first = io.words * (size_t)done;
             if (io32) {
-                u32 *raw = reinterpret_cast<u32 *>(w.buf[6]) + off32;
-                CK(cudaMemcpyAsync(raw, reinterpret_cast<const u32 *>(io.src) + io.words_per_item * (size_t)done,
-                                   words * sizeof(u32), cudaMemcpyHostToDevice, w.stream));
-                CK(launch_widen(raw, w.buf[4] + off, (int64_t)words, w.stream));
-                off32 += (words + 3) & ~(size_t)3;
+                u32 *raw = reinterpret_cast<u32 *>(w.in32.p) + off32;
+                CK(cudaMemcpyAsync(raw, static_cast<const u32 *>(io.p) + first, n * sizeof(u32), cudaMemcpyHostToDevice,
+                                   w.stream));
+                CK(launch_widen(raw, w.in.p + off, (int64_t)n, w.stream));
+                off32 += (n + 3) & ~(size_t)3;
             } else {
-                CK(cudaMemcpyAsync(w.buf[4] + off, io.src + io.words_per_item * (size_t)done, words * sizeof(u64),
+                CK(cudaMemcpyAsync(w.in.p + off, static_cast<const u64 *>(io.p) + first, n * sizeof(u64),
                                    cudaMemcpyHostToDevice, w.stream));
             }
-            d_in.push_back(w.buf[4] + off);
-            off += words;
+            d_in.push_back(w.in.p + off);
+            off += n;
         }
-        cudaError_t e = body(w, d_in, w.buf[5], items);
+        cudaError_t e = op.body({w.scratch.p, done, items, d_in.data(), w.out.p, w.stream});
         if (e != cudaSuccess) return cuda_fail(e, "kernel launch");
+        const size_t first = op.out_words * (size_t)done;
         if (io32) {
-            CK(launch_narrow(w.buf[5], reinterpret_cast<u32 *>(w.buf[7]), (int64_t)out_words, w.stream));
-            CK(cudaMemcpyAsync(reinterpret_cast<u32 *>(host_out) + out_words_per_item * (size_t)done, w.buf[7],
-                               out_words * sizeof(u32), cudaMemcpyDeviceToHost, w.stream));
+            u32 *out32 = reinterpret_cast<u32 *>(w.out32.p);
+            CK(launch_narrow(w.out.p, out32, (int64_t)out_words, w.stream));
+            CK(cudaMemcpyAsync(static_cast<u32 *>(op.out) + first, out32, out_words * sizeof(u32), cudaMemcpyDeviceToHost,
+                               w.stream));
         } else {
-            CK(cudaMemcpyAsync(host_out + out_words_per_item * (size_t)done, w.buf[5], out_words * sizeof(u64),
-                               cudaMemcpyDeviceToHost, w.stream));
+            CK(cudaMemcpyAsync(static_cast<u64 *>(op.out) + first, w.out.p, out_words * sizeof(u64), cudaMemcpyDeviceToHost,
+                               w.stream));
         }
     }
     for (Workspace *w : ws) CK(wait_stream(w->stream));
     return HECUDA_OK;
+}
+
+// Where a batched entry point runs its operation: on device buffers on the caller's stream, or through the host
+// pipeline on host buffers of `words`.
+struct Target {
+    bool device;
+    cudaStream_t stream;
+    Words words;
+};
+constexpr Target kHost64{false, nullptr, Words::u64}, kHost32{false, nullptr, Words::u32};
+Target on_stream(void *stream) { return {true, (cudaStream_t)stream, Words::u64}; }
+
+int32_t run(const hecuda_context *h, const Batched &op, int64_t batch, Target t) {
+    return t.device ? run_device(op, batch, t.stream) : host_pipeline(h, op, batch, t.words);
 }
 
 }  // namespace
@@ -491,142 +544,96 @@ int32_t hecuda_context_root_tables(const hecuda_context *h, uint64_t modulus, ui
 
 // ---------------------------------------------------------------- NTT
 
-static int32_t ntt_device(const hecuda_context *h, int32_t base, uint64_t *data, int32_t rows, int64_t polys,
-                          void *stream, bool inverse) {
+// forward or inverse NTT, in place, of items of `rows` rows
+static Batched ntt_op(const Context &c, const NttRowMap &map, void *data, int64_t rows, bool inverse) {
+    const size_t words = (size_t)rows * c.n;
+    return {"ntt launch", {{data, words}}, data, words, 0, kWholeBatch, stage_items(kStageWords, words),
+            [&c, map, rows, inverse](const Chunk &x) {
+                return inverse ? launch_ntt_inverse(c, map, x.in[0], x.out, x.items * rows, kScalePlain, x.stream)
+                               : launch_ntt_forward(c, map, x.in[0], x.out, x.items * rows, x.stream);
+            }};
+}
+static int32_t ntt(const hecuda_context *h, int32_t base, void *data, int32_t rows, int64_t polys, bool inverse, Target t) {
     int32_t rc = check_ctx(h);
     if (rc) return rc;
     if (polys < 0 || (!data && polys)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid data / poly_count");
     NttRowMap map;
     std::string err;
     if (!make_map(*h->ctx, base, rows, map, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
-    cudaError_t e = inverse ? launch_ntt_inverse(*h->ctx, map, (u64 *)data, (u64 *)data, polys * rows, kScalePlain,
-                                                 (cudaStream_t)stream)
-                            : launch_ntt_forward(*h->ctx, map, (u64 *)data, (u64 *)data, polys * rows,
-                                                 (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "ntt launch");
-    return HECUDA_OK;
+    return run(h, ntt_op(*h->ctx, map, data, rows, inverse), polys, t);
 }
 int32_t hecuda_ntt_forward_device(const hecuda_context *h, int32_t base, uint64_t *data, int32_t rows, int64_t polys,
                                   void *stream) {
-    return ntt_device(h, base, data, rows, polys, stream, false);
+    return ntt(h, base, data, rows, polys, false, on_stream(stream));
 }
 int32_t hecuda_ntt_inverse_device(const hecuda_context *h, int32_t base, uint64_t *data, int32_t rows, int64_t polys,
                                   void *stream) {
-    return ntt_device(h, base, data, rows, polys, stream, true);
-}
-
-static int32_t ntt_host(const hecuda_context *h, const NttRowMap &map, uint64_t *data, size_t words_per_item,
-                        int64_t items, int64_t rows_per_item, bool inverse) {
-    const Context &c = *h->ctx;
-    std::vector<HostIo> in = {{(const u64 *)data, words_per_item}};
-    // NTT items are single polynomials: stage ~32 MB per pipeline step
-    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / std::max<size_t>(1, words_per_item)));
-    return host_pipeline(h, items, chunk, 0, in, (u64 *)data, words_per_item,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t n_items) {
-                             return inverse ? launch_ntt_inverse(c, map, d_in[0], d_out, n_items * rows_per_item, kScalePlain,
-                                                                 w.stream)
-                                            : launch_ntt_forward(c, map, d_in[0], d_out, n_items * rows_per_item,
-                                                                 w.stream);
-                         });
+    return ntt(h, base, data, rows, polys, true, on_stream(stream));
 }
 int32_t hecuda_ntt_forward(const hecuda_context *h, int32_t base, uint64_t *data, int32_t rows, int64_t polys) {
-    int32_t rc = check_ctx(h);
-    if (rc) return rc;
-    if (polys < 0 || (!data && polys)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid data / poly_count");
-    NttRowMap map;
-    std::string err;
-    if (!make_map(*h->ctx, base, rows, map, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
-    return ntt_host(h, map, data, (size_t)rows * h->ctx->n, polys, rows, false);
+    return ntt(h, base, data, rows, polys, false, kHost64);
 }
 int32_t hecuda_ntt_inverse(const hecuda_context *h, int32_t base, uint64_t *data, int32_t rows, int64_t polys) {
-    int32_t rc = check_ctx(h);
-    if (rc) return rc;
-    if (polys < 0 || (!data && polys)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid data / poly_count");
-    NttRowMap map;
-    std::string err;
-    if (!make_map(*h->ctx, base, rows, map, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
-    return ntt_host(h, map, data, (size_t)rows * h->ctx->n, polys, rows, true);
+    return ntt(h, base, data, rows, polys, true, kHost64);
 }
 // Stage-level BEHZ entry points over the reference's [Q, Bsk] (RnsTool.swift:324-331, 453-456), Coeff format.
-int32_t hecuda_rnstool_lift_q_to_qbsk(const hecuda_context *h, const uint64_t *polys, uint64_t *out, int64_t count) {
+static int32_t lift_or_floor(const hecuda_context *h, const void *polys, void *out, int64_t count, bool lift, Words words) {
     int32_t rc = check_ctx(h);
     if (rc) return rc;
     if (count < 0 || ((!polys || !out) && count)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid buffers / poly_count");
     const Context &c = *h->ctx;
-    const size_t in_words = (size_t)c.L * c.n, out_words = (size_t)(2 * c.L + 1) * c.n;
-    std::vector<HostIo> in = {{(const u64 *)polys, in_words}};
-    return host_pipeline(h, count, std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / out_words)), 0, in, (u64 *)out, out_words,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t n_items) {
-                             return launch_lift(c, d_in[0], nullptr, 1, d_out, n_items, w.stream, /*reference_base=*/true);
-                         });
+    const size_t q_words = (size_t)c.L * c.n, qbsk_words = (size_t)(2 * c.L + 1) * c.n;
+    return host_pipeline(h,
+                         {lift ? "lift" : "floor", {{polys, lift ? q_words : qbsk_words}}, out, lift ? qbsk_words : q_words, 0,
+                          kWholeBatch, stage_items(kStageWords, qbsk_words),
+                          [&](const Chunk &x) {
+                              return lift ? launch_lift(c, x.in[0], nullptr, 1, x.out, x.items, x.stream, /*reference_base=*/true)
+                                          : launch_floor(c, x.in[0], x.out, x.items, x.stream, /*reference_base=*/true);
+                          }},
+                         count, words);
+}
+int32_t hecuda_rnstool_lift_q_to_qbsk(const hecuda_context *h, const uint64_t *polys, uint64_t *out, int64_t count) {
+    return lift_or_floor(h, polys, out, count, true, Words::u64);
 }
 int32_t hecuda_rnstool_floor_qbsk_to_q(const hecuda_context *h, const uint64_t *polys, uint64_t *out, int64_t count) {
-    int32_t rc = check_ctx(h);
-    if (rc) return rc;
-    if (count < 0 || ((!polys || !out) && count)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid buffers / poly_count");
-    const Context &c = *h->ctx;
-    const size_t in_words = (size_t)(2 * c.L + 1) * c.n, out_words = (size_t)c.L * c.n;
-    std::vector<HostIo> in = {{(const u64 *)polys, in_words}};
-    return host_pipeline(h, count, std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / in_words)), 0, in, (u64 *)out, out_words,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t n_items) {
-                             return launch_floor(c, d_in[0], d_out, n_items, w.stream, /*reference_base=*/true);
-                         });
+    return lift_or_floor(h, polys, out, count, false, Words::u64);
 }
 
-static int32_t ntt_rows_host(const hecuda_context *h, uint64_t modulus, uint64_t *data, int64_t rows, bool inverse) {
+static int32_t ntt_rows(const hecuda_context *h, uint64_t modulus, uint64_t *data, int64_t rows, bool inverse) {
     int32_t rc = check_ctx(h);
     if (rc) return rc;
     if (rows < 0 || (!data && rows)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid data / row_count");
     const int s = h->ctx->find_slot(modulus);
     if (s < 0) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidPolyContext: modulus is not part of this context");
-    return ntt_host(h, h->ctx->map_single(s), data, (size_t)h->ctx->n, rows, 1, inverse);
+    return host_pipeline(h, ntt_op(*h->ctx, h->ctx->map_single(s), data, 1, inverse), rows, Words::u64);
 }
 int32_t hecuda_ntt_forward_rows(const hecuda_context *h, uint64_t modulus, uint64_t *data, int64_t rows) {
-    return ntt_rows_host(h, modulus, data, rows, false);
+    return ntt_rows(h, modulus, data, rows, false);
 }
 int32_t hecuda_ntt_inverse_rows(const hecuda_context *h, uint64_t modulus, uint64_t *data, int64_t rows) {
-    return ntt_rows_host(h, modulus, data, rows, true);
+    return ntt_rows(h, modulus, data, rows, true);
 }
 
 // ---------------------------------------------------------------- multiply
 
+static int32_t bfv_multiply(const hecuda_context *h, const void *lhs, const void *rhs, void *out, int64_t batch, Target t) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (batch < 0 || (batch && (!lhs || !rhs || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: null buffer");
+    const Context &c = *h->ctx;
+    const size_t in_words = (size_t)2 * c.L * c.n;
+    return run(h,
+               {"multiply", {{lhs, in_words}, {rhs, in_words}}, out, (size_t)3 * c.L * c.n, multiply_scratch_words(c), h->chunk,
+                h->chunk, [&](const Chunk &x) { return multiply_chunk(c, x.scratch, x.in[0], x.in[1], x.out, x.items, x.stream); }},
+               batch, t);
+}
 int32_t hecuda_bfv_multiply_device(const hecuda_context *h, const uint64_t *lhs, const uint64_t *rhs, uint64_t *out,
                                    int64_t batch, void *stream) {
-    int32_t rc = check_ctx(h);
-    if (rc) return rc;
-    if (batch < 0 || (batch && (!lhs || !rhs || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: null buffer");
-    if (batch == 0) return HECUDA_OK;
-    const Context &c = *h->ctx;
-    const size_t in_words = (size_t)2 * c.L * c.n, out_words = (size_t)3 * c.L * c.n;
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, batch));
-    cudaStream_t s = (cudaStream_t)stream;
-    u64 *scratch = nullptr;  // stream-ordered scratch: no host synchronization, graph-capturable
-    CK(cudaMallocAsync(&scratch, multiply_scratch_words(c) * (size_t)chunk * sizeof(u64), s));
-    for (int64_t done = 0; done < batch; done += chunk) {
-        const int64_t items = std::min<int64_t>(chunk, batch - done);
-        cudaError_t e = multiply_chunk(c, scratch, (const u64 *)lhs + in_words * done, (const u64 *)rhs + in_words * done,
-                                       (u64 *)out + out_words * done, items, s);
-        if (e != cudaSuccess) {
-            cudaFreeAsync(scratch, s);
-            return cuda_fail(e, "multiply");
-        }
-    }
-    CK(cudaFreeAsync(scratch, s));
-    return HECUDA_OK;
+    return bfv_multiply(h, lhs, rhs, out, batch, on_stream(stream));
 }
-
 int32_t hecuda_bfv_multiply(const hecuda_context *h, const uint64_t *lhs, const uint64_t *rhs, uint64_t *out,
                             int64_t batch) {
-    int32_t rc = check_ctx(h);
-    if (rc) return rc;
-    if (batch < 0 || (batch && (!lhs || !rhs || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: null buffer");
-    const Context &c = *h->ctx;
-    const size_t in_words = (size_t)2 * c.L * c.n, out_words = (size_t)3 * c.L * c.n;
-    std::vector<HostIo> in = {{(const u64 *)lhs, in_words}, {(const u64 *)rhs, in_words}};
-    return host_pipeline(h, batch, h->chunk, multiply_scratch_words(c), in, (u64 *)out, out_words,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return multiply_chunk(c, w.buf[0], d_in[0], d_in[1], d_out, items, w.stream);
-                         });
+    return bfv_multiply(h, lhs, rhs, out, batch, kHost64);
 }
 
 // ---------------------------------------------------------------- evaluation key
@@ -683,105 +690,96 @@ int32_t hecuda_evk_device_buffer(hecuda_evk *k, void **device_ptr, uint64_t *byt
 
 // ---------------------------------------------------------------- relinearize / mod switch
 
-static int32_t check_relin(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct3, int32_t l, uint64_t *out,
-                           int64_t batch) {
+// The key checks of the key-switching operations: a key (with its relinearization key when `relin`) made for `h`.
+static int32_t check_key(const hecuda_context *h, const hecuda_evk *k, bool relin) {
     int32_t rc = check_ctx(h);
     if (rc) return rc;
-    if (!k || !k->loaded) return fail(HECUDA_ERR_MISSING_KEY, "missingRelinearizationKey");
+    if (!k || (relin && !k->loaded))
+        return fail(HECUDA_ERR_MISSING_KEY, relin ? "missingRelinearizationKey" : "missingGaloisKey");
     if (k->owner != h) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidContext: evaluation key belongs to another context");
+    return HECUDA_OK;
+}
+static int32_t check_moduli(const hecuda_context *h, int32_t l) {
     if (l < 1 || l > h->ctx->L) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: moduli_count out of range");
+    return HECUDA_OK;
+}
+
+static int32_t check_relin(const hecuda_context *h, const hecuda_evk *k, const void *ct3, int32_t l, const void *out,
+                           int64_t batch) {
+    int32_t rc = check_key(h, k, true);
+    if (rc || (rc = check_moduli(h, l))) return rc;
     if (batch < 0 || (batch && (!ct3 || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: null buffer");
     return HECUDA_OK;
 }
 
+static int32_t bfv_relinearize(const hecuda_context *h, const hecuda_evk *k, const void *ct3, int32_t l, void *out,
+                               int64_t batch, Target t) {
+    int32_t rc = check_relin(h, k, ct3, l, out, batch);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    return run(h,
+               {"relinearize", {{ct3, (size_t)3 * l * c.n}}, out, (size_t)2 * l * c.n, relinearize_scratch_words(c, l), h->chunk,
+                h->chunk,
+                [&](const Chunk &x) { return relinearize_chunk(c, x.scratch, k->d_relin, x.in[0], l, x.out, x.items, x.stream); }},
+               batch, t);
+}
 int32_t hecuda_bfv_relinearize_device(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct3, int32_t l,
                                       uint64_t *out, int64_t batch, void *stream) {
-    int32_t rc = check_relin(h, k, ct3, l, out, batch);
-    if (rc) return rc;
-    if (batch == 0) return HECUDA_OK;
-    const Context &c = *h->ctx;
-    const size_t in_words = (size_t)3 * l * c.n, out_words = (size_t)2 * l * c.n;
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, batch));
-    cudaStream_t s = (cudaStream_t)stream;
-    u64 *scratch = nullptr;
-    CK(cudaMallocAsync(&scratch, relinearize_scratch_words(c, l) * (size_t)chunk * sizeof(u64), s));
-    for (int64_t done = 0; done < batch; done += chunk) {
-        const int64_t items = std::min<int64_t>(chunk, batch - done);
-        cudaError_t e = relinearize_chunk(c, scratch, k->d_relin, (const u64 *)ct3 + in_words * done, l,
-                                          (u64 *)out + out_words * done, items, s);
-        if (e != cudaSuccess) {
-            cudaFreeAsync(scratch, s);
-            return cuda_fail(e, "relinearize");
-        }
-    }
-    CK(cudaFreeAsync(scratch, s));
-    return HECUDA_OK;
+    return bfv_relinearize(h, k, ct3, l, out, batch, on_stream(stream));
 }
-
 int32_t hecuda_bfv_relinearize(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct3, int32_t l,
                                uint64_t *out, int64_t batch) {
-    int32_t rc = check_relin(h, k, ct3, l, out, batch);
-    if (rc) return rc;
-    const Context &c = *h->ctx;
-    std::vector<HostIo> in = {{(const u64 *)ct3, (size_t)3 * l * c.n}};
-    return host_pipeline(h, batch, h->chunk, relinearize_scratch_words(c, l), in, (u64 *)out, (size_t)2 * l * c.n,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return relinearize_chunk(c, w.buf[0], k->d_relin, d_in[0], l, d_out, items, w.stream);
-                         });
+    return bfv_relinearize(h, k, ct3, l, out, batch, kHost64);
 }
 
-static int32_t check_ms(const hecuda_context *h, const uint64_t *ct, int32_t polys, int32_t l, uint64_t *out,
-                        int64_t batch) {
+static int32_t bfv_mod_switch_down(const hecuda_context *h, const void *ct, int32_t polys, int32_t l, void *out, int64_t batch,
+                                   Target t) {
     int32_t rc = check_ctx(h);
     if (rc) return rc;
     if (polys < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: poly_count");
     if (l < 2 || l > h->ctx->L)
         return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidPolyContext: modSwitchDown needs a next context (2 <= moduli_count <= L)");
     if (batch < 0 || (batch && (!ct || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: null buffer");
-    return HECUDA_OK;
+    const Context &c = *h->ctx;
+    const size_t in_words = (size_t)polys * l * c.n;
+    return run(h,
+               {"mod_switch", {{ct, in_words}}, out, (size_t)polys * (l - 1) * c.n, 0, kWholeBatch, stage_items(kStageWords, in_words),
+                [&](const Chunk &x) { return launch_mod_switch(c, x.in[0], l, x.out, x.items * polys, x.stream); }},
+               batch, t);
 }
-
 int32_t hecuda_bfv_mod_switch_down_device(const hecuda_context *h, const uint64_t *ct, int32_t polys, int32_t l,
                                           uint64_t *out, int64_t batch, void *stream) {
-    int32_t rc = check_ms(h, ct, polys, l, out, batch);
-    if (rc) return rc;
-    cudaError_t e = launch_mod_switch(*h->ctx, (const u64 *)ct, l, (u64 *)out, batch * polys, (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "mod_switch");
-    return HECUDA_OK;
+    return bfv_mod_switch_down(h, ct, polys, l, out, batch, on_stream(stream));
 }
-
 int32_t hecuda_bfv_mod_switch_down(const hecuda_context *h, const uint64_t *ct, int32_t polys, int32_t l, uint64_t *out,
                                    int64_t batch) {
-    int32_t rc = check_ms(h, ct, polys, l, out, batch);
-    if (rc) return rc;
-    const Context &c = *h->ctx;
-    std::vector<HostIo> in = {{(const u64 *)ct, (size_t)polys * l * c.n}};
-    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / ((size_t)polys * l * c.n)));
-    return host_pipeline(h, batch, chunk, 0, in, (u64 *)out, (size_t)polys * (l - 1) * c.n,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return launch_mod_switch(c, d_in[0], l, d_out, items * polys, w.stream);
-                         });
+    return bfv_mod_switch_down(h, ct, polys, l, out, batch, kHost64);
 }
-
 
 // ---------------------------------------------------------------- relinearize -> modSwitchDown, fused
 // Bfv.relinearize then Bfv.modSwitchDown on a batch in one pass (BASELINE config 3): the relinearized ciphertext stays
 // in HBM, 2 x (l-1) rows per ciphertext come back.
-int32_t hecuda_bfv_relinearize_mod_switch_down(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct3, int32_t l,
-                                               uint64_t *out, int64_t batch) {
+static int32_t relinearize_mod_switch_down(const hecuda_context *h, const hecuda_evk *k, const void *ct3, int32_t l, void *out,
+                                           int64_t batch, Words words) {
     int32_t rc = check_relin(h, k, ct3, l, out, batch);
     if (rc) return rc;
     if (l < 2) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidPolyContext: modSwitchDown needs a next context (moduli_count >= 2)");
     const Context &c = *h->ctx;
-    const size_t relin_words = (size_t)2 * l * c.n;
-    std::vector<HostIo> in = {{(const u64 *)ct3, (size_t)3 * l * c.n}};
-    return host_pipeline(h, batch, h->chunk, relinearize_scratch_words(c, l) + relin_words, in, (u64 *)out, (size_t)2 * (l - 1) * c.n,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             u64 *relin = w.buf[0] + relinearize_scratch_words(c, l) * (size_t)items;
-                             cudaError_t e = relinearize_chunk(c, w.buf[0], k->d_relin, d_in[0], l, relin, items, w.stream);
-                             if (e != cudaSuccess) return e;
-                             return launch_mod_switch(c, relin, l, d_out, items * 2, w.stream);
-                         });
+    const size_t ks_words = relinearize_scratch_words(c, l);
+    return host_pipeline(h,
+                         {"relinearize_mod_switch_down", {{ct3, (size_t)3 * l * c.n}}, out, (size_t)2 * (l - 1) * c.n,
+                          ks_words + (size_t)2 * l * c.n, h->chunk, h->chunk,
+                          [&](const Chunk &x) {
+                              u64 *relin = x.scratch + ks_words * (size_t)x.items;
+                              cudaError_t e = relinearize_chunk(c, x.scratch, k->d_relin, x.in[0], l, relin, x.items, x.stream);
+                              if (e != cudaSuccess) return e;
+                              return launch_mod_switch(c, relin, l, x.out, x.items * 2, x.stream);
+                          }},
+                         batch, words);
+}
+int32_t hecuda_bfv_relinearize_mod_switch_down(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct3, int32_t l,
+                                               uint64_t *out, int64_t batch) {
+    return relinearize_mod_switch_down(h, k, ct3, l, out, batch, Words::u64);
 }
 
 // ---------------------------------------------------------------- multiply -> relinearize (-> modSwitchDown), fused
@@ -804,52 +802,31 @@ static cudaError_t mul_relin_chunk(const Context &c, u64 *scratch, const u64 *ke
     if (mod_switch) return launch_mod_switch(c, relin, c.L, out, items * 2, s);
     return cudaSuccess;
 }
-static int32_t check_mul_relin(const hecuda_context *h, const hecuda_evk *k, const void *lhs, const void *rhs, const void *out,
-                               int32_t mod_switch, int64_t batch) {
-    int32_t rc = check_ctx(h);
+static int32_t bfv_multiply_relinearize(const hecuda_context *h, const hecuda_evk *k, const void *lhs, const void *rhs,
+                                        int32_t mod_switch, void *out, int64_t batch, Target t) {
+    int32_t rc = check_key(h, k, true);
     if (rc) return rc;
-    if (!k || !k->loaded) return fail(HECUDA_ERR_MISSING_KEY, "missingRelinearizationKey");
-    if (k->owner != h) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidContext: evaluation key belongs to another context");
     if (mod_switch && h->ctx->L < 2)
         return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidPolyContext: modSwitchDown needs a next context (L >= 2)");
     if (batch < 0 || (batch && (!lhs || !rhs || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: null buffer");
-    return HECUDA_OK;
+    const Context &c = *h->ctx;
+    const size_t in_words = (size_t)2 * c.L * c.n, out_words = (size_t)2 * (c.L - (mod_switch ? 1 : 0)) * c.n;
+    const int64_t chunk = std::max<int64_t>(1, h->chunk / 2);
+    return run(h,
+               {"multiply_relinearize", {{lhs, in_words}, {rhs, in_words}}, out, out_words, mul_relin_scratch_words(c), chunk, chunk,
+                [&](const Chunk &x) {
+                    return mul_relin_chunk(c, x.scratch, k->d_relin, x.in[0], x.in[1], mod_switch != 0, x.out, x.items, x.stream);
+                }},
+               batch, t);
 }
 int32_t hecuda_bfv_multiply_relinearize_device(const hecuda_context *h, const hecuda_evk *k, const uint64_t *lhs,
                                                const uint64_t *rhs, int32_t mod_switch, uint64_t *out, int64_t batch,
                                                void *stream) {
-    int32_t rc = check_mul_relin(h, k, lhs, rhs, out, mod_switch, batch);
-    if (rc || batch == 0) return rc;
-    const Context &c = *h->ctx;
-    const size_t in_words = (size_t)2 * c.L * c.n, out_words = (size_t)2 * (c.L - (mod_switch ? 1 : 0)) * c.n;
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk / 2, batch));
-    cudaStream_t s = (cudaStream_t)stream;
-    u64 *scratch = nullptr;
-    CK(cudaMallocAsync(&scratch, mul_relin_scratch_words(c) * (size_t)chunk * sizeof(u64), s));
-    for (int64_t done = 0; done < batch; done += chunk) {
-        const int64_t items = std::min<int64_t>(chunk, batch - done);
-        cudaError_t e = mul_relin_chunk(c, scratch, k->d_relin, (const u64 *)lhs + in_words * done, (const u64 *)rhs + in_words * done,
-                                        mod_switch != 0, (u64 *)out + out_words * done, items, s);
-        if (e != cudaSuccess) {
-            cudaFreeAsync(scratch, s);
-            return cuda_fail(e, "multiply_relinearize");
-        }
-    }
-    CK(cudaFreeAsync(scratch, s));
-    return HECUDA_OK;
+    return bfv_multiply_relinearize(h, k, lhs, rhs, mod_switch, out, batch, on_stream(stream));
 }
 int32_t hecuda_bfv_multiply_relinearize(const hecuda_context *h, const hecuda_evk *k, const uint64_t *lhs, const uint64_t *rhs,
                                         int32_t mod_switch, uint64_t *out, int64_t batch) {
-    int32_t rc = check_mul_relin(h, k, lhs, rhs, out, mod_switch, batch);
-    if (rc) return rc;
-    const Context &c = *h->ctx;
-    const size_t in_words = (size_t)2 * c.L * c.n, out_words = (size_t)2 * (c.L - (mod_switch ? 1 : 0)) * c.n;
-    std::vector<HostIo> in = {{(const u64 *)lhs, in_words}, {(const u64 *)rhs, in_words}};
-    return host_pipeline(h, batch, std::max<int64_t>(1, h->chunk / 2), mul_relin_scratch_words(c), in, (u64 *)out, out_words,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return mul_relin_chunk(c, w.buf[0], k->d_relin, d_in[0], d_in[1], mod_switch != 0, d_out, items,
-                                                    w.stream);
-                         });
+    return bfv_multiply_relinearize(h, k, lhs, rhs, mod_switch, out, batch, kHost64);
 }
 
 // ---------------------------------------------------------------- Galois (SURVEY.md 8f rank 1)
@@ -981,59 +958,35 @@ int32_t hecuda_evk_create_serialized(const hecuda_context *h, const uint8_t *rel
     return HECUDA_OK;
 }
 
-static int32_t check_galois(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct, int32_t l, uint32_t element,
-                            uint64_t *out, int64_t batch, const u64 **key) {
-    int32_t rc = check_ctx(h);
+static int32_t bfv_apply_galois(const hecuda_context *h, const hecuda_evk *k, const void *ct, int32_t l, uint32_t element,
+                                void *out, int64_t batch, Target t) {
+    int32_t rc = check_key(h, k, false);
     if (rc) return rc;
-    if (!k) return fail(HECUDA_ERR_MISSING_KEY, "missingGaloisKey");
-    if (k->owner != h) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidContext: evaluation key belongs to another context");
     if (!valid_galois_element(element, h->ctx->n)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid Galois element");
-    if (l < 1 || l > h->ctx->L) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: moduli_count out of range");
+    if ((rc = check_moduli(h, l))) return rc;
     if (batch < 0 || (batch && (!ct || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: null buffer");
-    hecuda_evk *km = const_cast<hecuda_evk *>(k);
-    std::lock_guard<std::mutex> g(km->mu);
-    auto it = km->galois.find(element);
-    if (it == km->galois.end()) return fail(HECUDA_ERR_MISSING_KEY, "missingGaloisElement: " + std::to_string(element));
-    *key = it->second;
-    return HECUDA_OK;
-}
-
-int32_t hecuda_bfv_apply_galois_device(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct, int32_t l,
-                                       uint32_t element, uint64_t *out, int64_t batch, void *stream) {
     const u64 *key = nullptr;
-    int32_t rc = check_galois(h, k, ct, l, element, out, batch, &key);
-    if (rc) return rc;
-    if (batch == 0) return HECUDA_OK;
+    {
+        hecuda_evk *km = const_cast<hecuda_evk *>(k);
+        std::lock_guard<std::mutex> g(km->mu);
+        auto it = km->galois.find(element);
+        if (it == km->galois.end()) return fail(HECUDA_ERR_MISSING_KEY, "missingGaloisElement: " + std::to_string(element));
+        key = it->second;
+    }
     const Context &c = *h->ctx;
     const size_t words = (size_t)2 * l * c.n;
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(h->chunk, batch));
-    cudaStream_t s = (cudaStream_t)stream;
-    u64 *scratch = nullptr;
-    CK(cudaMallocAsync(&scratch, galois_scratch_words(c, l) * (size_t)chunk * sizeof(u64), s));
-    for (int64_t done = 0; done < batch; done += chunk) {
-        const int64_t items = std::min<int64_t>(chunk, batch - done);
-        cudaError_t e = apply_galois_chunk(c, scratch, key, (const u64 *)ct + words * done, l, element,
-                                           (u64 *)out + words * done, items, s);
-        if (e != cudaSuccess) {
-            cudaFreeAsync(scratch, s);
-            return cuda_fail(e, "applyGalois");
-        }
-    }
-    CK(cudaFreeAsync(scratch, s));
-    return HECUDA_OK;
+    return run(h,
+               {"applyGalois", {{ct, words}}, out, words, galois_scratch_words(c, l), h->chunk, h->chunk,
+                [&](const Chunk &x) { return apply_galois_chunk(c, x.scratch, key, x.in[0], l, element, x.out, x.items, x.stream); }},
+               batch, t);
 }
-
+int32_t hecuda_bfv_apply_galois_device(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct, int32_t l,
+                                       uint32_t element, uint64_t *out, int64_t batch, void *stream) {
+    return bfv_apply_galois(h, k, ct, l, element, out, batch, on_stream(stream));
+}
 int32_t hecuda_bfv_apply_galois(const hecuda_context *h, const hecuda_evk *k, const uint64_t *ct, int32_t l,
                                 uint32_t element, uint64_t *out, int64_t batch) {
-    const u64 *key = nullptr;
-    int32_t rc = check_galois(h, k, ct, l, element, out, batch, &key);
-    if (rc) return rc;
-    const Context &c = *h->ctx;
-    std::vector<HostIo> in = {{(const u64 *)ct, (size_t)2 * l * c.n}};
-    return host_pipeline(h, batch, h->chunk, galois_scratch_words(c, l), in, (u64 *)out, (size_t)2 * l * c.n,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return apply_galois_chunk(c, w.buf[0], key, d_in[0], l, element, d_out, items, w.stream);
-                         });
+    return bfv_apply_galois(h, k, ct, l, element, out, batch, kHost64);
 }
 
 int32_t hecuda_poly_apply_galois(const hecuda_context *h, int32_t base, int32_t eval_format, const uint64_t *in,
@@ -1047,14 +1000,14 @@ int32_t hecuda_poly_apply_galois(const hecuda_context *h, int32_t base, int32_t 
     if (!make_map(*h->ctx, base, rows, map, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
     const Context &c = *h->ctx;
     const size_t words = (size_t)rows * c.n;
-    std::vector<HostIo> hin = {{(const u64 *)in, words}};
-    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / words));
-    return host_pipeline(h, polys, chunk, 0, hin, (u64 *)out, words,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return eval_format ? launch_galois_eval(c, rows, element, d_in[0], d_out, items, w.stream)
-                                                : launch_galois_coeff(c, map, element, d_in[0], (int64_t)words, d_out,
-                                                                      (int64_t)words, items, w.stream);
-                         });
+    return host_pipeline(h,
+                         {"poly_apply_galois", {{in, words}}, out, words, 0, kWholeBatch, stage_items(kStageWords, words),
+                          [&](const Chunk &x) {
+                              return eval_format ? launch_galois_eval(c, rows, element, x.in[0], x.out, x.items, x.stream)
+                                                 : launch_galois_coeff(c, map, element, x.in[0], (int64_t)words, x.out,
+                                                                       (int64_t)words, x.items, x.stream);
+                          }},
+                         polys, Words::u64);
 }
 
 // ---------------------------------------------------------------- lazy ct x pt inner product (SURVEY.md 8f rank 2)
@@ -1071,16 +1024,24 @@ static int32_t check_ip(const hecuda_context *h, const uint64_t *cts, int32_t po
     return HECUDA_OK;
 }
 
+// the query ciphertexts `cts` and the presence flags are device buffers here, shared by every output row
+static Batched inner_product_plaintexts_op(const Context &c, const u64 *cts, int32_t polys, int32_t l, int64_t terms,
+                                           const void *pts, const unsigned char *present, void *out) {
+    const size_t pt_words = (size_t)terms * l * c.n;
+    return {"inner_product", {{pts, pt_words}}, out, (size_t)polys * l * c.n, 0, kWholeBatch,
+            stage_items(8 * kStageWords, pt_words), [&c, cts, polys, l, terms, present](const Chunk &x) {
+                return launch_inner_product_plain(c, cts, polys, l, terms, x.in[0], present ? present + x.first * terms : nullptr,
+                                                  x.out, x.items, x.stream);
+            }};
+}
 int32_t hecuda_bfv_inner_product_plaintexts_device(const hecuda_context *h, const uint64_t *cts, int32_t polys,
                                                    int32_t l, int64_t terms, const uint64_t *pts,
                                                    const uint8_t *present, uint64_t *out, int64_t out_count,
                                                    void *stream) {
     int32_t rc = check_ip(h, cts, polys, l, terms, pts, out, out_count);
     if (rc) return rc;
-    cudaError_t e = launch_inner_product_plain(*h->ctx, (const u64 *)cts, polys, l, terms, (const u64 *)pts, present,
-                                               (u64 *)out, out_count, (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "inner_product");
-    return HECUDA_OK;
+    return run_device(inner_product_plaintexts_op(*h->ctx, (const u64 *)cts, polys, l, terms, pts, present, out), out_count,
+                      (cudaStream_t)stream);
 }
 
 int32_t hecuda_bfv_inner_product_plaintexts(const hecuda_context *h, const uint64_t *cts, int32_t polys, int32_t l,
@@ -1105,46 +1066,31 @@ int32_t hecuda_bfv_inner_product_plaintexts(const hecuda_context *h, const uint6
         cudaFree(d_present);
         return cuda_fail(e, "inner_product upload");
     }
-    const size_t pt_words = (size_t)terms * l * c.n;
-    std::vector<HostIo> in = {{(const u64 *)pts, pt_words}};
-    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)32 * 1024 * 1024 / pt_words));
-    int64_t done_items = 0;  // host_pipeline calls the body in order, one chunk at a time
-    rc = host_pipeline(h, out_count, chunk, 0, in, (u64 *)out, (size_t)polys * l * c.n,
-                       [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                           const unsigned char *pr = d_present ? d_present + done_items * terms : nullptr;
-                           done_items += items;
-                           return launch_inner_product_plain(c, d_cts, polys, l, terms, d_in[0], pr, d_out, items, w.stream);
-                       });
-    cudaDeviceSynchronize();
+    rc = host_pipeline(h, inner_product_plaintexts_op(c, d_cts, polys, l, terms, pts, d_present, out), out_count, Words::u64);
     cudaFree(d_cts);
     cudaFree(d_present);
     return rc;
 }
 
-int32_t hecuda_plaintext_to_eval_device(const hecuda_context *h, const uint64_t *plain, int32_t l, uint64_t *out,
-                                        int64_t count, void *stream) {
-    int32_t rc = check_ctx(h);
-    if (rc) return rc;
-    if (l < 1 || l > h->ctx->L) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidPolyContext: moduli_count out of range");
-    if (count < 0 || (count && (!plain || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null buffer");
-    cudaError_t e = launch_plaintext_to_eval(*h->ctx, (const u64 *)plain, l, (u64 *)out, count, (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "plaintext_to_eval");
-    return HECUDA_OK;
-}
-
-int32_t hecuda_plaintext_to_eval(const hecuda_context *h, const uint64_t *plain, int32_t l, uint64_t *out,
-                                 int64_t count) {
+static int32_t plaintext_to_eval(const hecuda_context *h, const void *plain, int32_t l, void *out, int64_t count, Target t) {
     int32_t rc = check_ctx(h);
     if (rc) return rc;
     if (l < 1 || l > h->ctx->L) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidPolyContext: moduli_count out of range");
     if (count < 0 || (count && (!plain || !out))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null buffer");
     const Context &c = *h->ctx;
-    std::vector<HostIo> in = {{(const u64 *)plain, (size_t)c.n}};
-    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / ((size_t)l * c.n)));
-    return host_pipeline(h, count, chunk, 0, in, (u64 *)out, (size_t)l * c.n,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return launch_plaintext_to_eval(c, d_in[0], l, d_out, items, w.stream);
-                         });
+    const size_t out_words = (size_t)l * c.n;
+    return run(h,
+               {"plaintext_to_eval", {{plain, (size_t)c.n}}, out, out_words, 0, kWholeBatch, stage_items(kStageWords, out_words),
+                [&](const Chunk &x) { return launch_plaintext_to_eval(c, x.in[0], l, x.out, x.items, x.stream); }},
+               count, t);
+}
+int32_t hecuda_plaintext_to_eval_device(const hecuda_context *h, const uint64_t *plain, int32_t l, uint64_t *out,
+                                        int64_t count, void *stream) {
+    return plaintext_to_eval(h, plain, l, out, count, on_stream(stream));
+}
+int32_t hecuda_plaintext_to_eval(const hecuda_context *h, const uint64_t *plain, int32_t l, uint64_t *out,
+                                 int64_t count) {
+    return plaintext_to_eval(h, plain, l, out, count, kHost64);
 }
 
 // ---------------------------------------------------------------- plaintext side: SIMD encode / decode, ct +- pt
@@ -1167,9 +1113,9 @@ int32_t need_simd(const hecuda_context *h) {
     return HECUDA_OK;
 }
 
-// encodingDataOutOfBounds (Encoding.swift:147-156): host buffers of uint64 (or uint32 inside a hecuda_u32_ call)
-bool host_values_below(const void *p, size_t count, u64 t) {
-    if (tl_io32) {
+// encodingDataOutOfBounds (Encoding.swift:147-156) on host buffers
+bool host_values_below(const void *p, size_t count, u64 t, Words words) {
+    if (words == Words::u32) {
         const uint32_t *v = static_cast<const uint32_t *>(p);
         return std::all_of(v, v + count, [t](uint32_t x) { return x < t; });
     }
@@ -1218,126 +1164,106 @@ int64_t simd_chunk(const Context &c) { return std::max<int64_t>(1, ((int64_t)1 <
 
 extern "C" {
 
+static int32_t bfv_encode_simd(const hecuda_context *h, const void *values, int32_t value_count, int32_t l, void *out,
+                               int64_t count, Target t) {
+    int32_t rc = check_encode(h, values, value_count, l, out, count);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    if (!t.device && !host_values_below(values, (size_t)count * value_count, c.t, t.words))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "encodingDataOutOfBounds: values must be below the plaintext modulus");
+    std::vector<Batched::Io> in;
+    if (value_count) in.push_back({values, (size_t)value_count});
+    const size_t out_words = (size_t)(l ? l : 1) * c.n;
+    return run(h,
+               {"encodeSimd", in, out, out_words, simd_scratch_words(c, true, l), simd_chunk(c), stage_items(kStageWords, out_words),
+                [&](const Chunk &x) {
+                    return launch_encode_simd(c, value_count ? x.in[0] : nullptr, value_count, l, x.out, x.scratch, x.items, x.stream);
+                }},
+               count, t);
+}
 int32_t hecuda_bfv_encode_simd_device(const hecuda_context *h, const uint64_t *values, int32_t value_count,
                                       int32_t moduli_count, uint64_t *out, int64_t count, void *stream) {
-    int32_t rc = check_encode(h, values, value_count, moduli_count, out, count);
-    if (rc || count == 0) return rc;
-    const Context &c = *h->ctx;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int64_t chunk = std::min<int64_t>(simd_chunk(c), count);
-    const size_t scratch_words = simd_scratch_words(c, true, moduli_count) * (size_t)chunk;
-    u64 *scratch = nullptr;
-    if (scratch_words) CK(cudaMallocAsync(&scratch, scratch_words * sizeof(u64), s));
-    const int64_t out_words = (int64_t)(moduli_count ? moduli_count : 1) * c.n;
-    cudaError_t e = cudaSuccess;
-    for (int64_t done = 0; e == cudaSuccess && done < count; done += chunk)
-        e = launch_encode_simd(c, (const u64 *)values + done * value_count, value_count, moduli_count,
-                               (u64 *)out + done * out_words, scratch, std::min<int64_t>(chunk, count - done), s);
-    if (scratch) cudaFreeAsync(scratch, s);
-    return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "encodeSimd");
+    return bfv_encode_simd(h, values, value_count, moduli_count, out, count, on_stream(stream));
 }
-
 int32_t hecuda_bfv_encode_simd(const hecuda_context *h, const uint64_t *values, int32_t value_count, int32_t moduli_count,
                                uint64_t *out, int64_t count) {
-    int32_t rc = check_encode(h, values, value_count, moduli_count, out, count);
-    if (rc) return rc;
-    const Context &c = *h->ctx;
-    if (!host_values_below(values, (size_t)count * value_count, c.t))
-        return fail(HECUDA_ERR_INVALID_ARGUMENT, "encodingDataOutOfBounds: values must be below the plaintext modulus");
-    const int l = moduli_count;
-    std::vector<HostIo> in;
-    if (value_count) in.push_back({(const u64 *)values, (size_t)value_count});
-    const size_t out_words = (size_t)(l ? l : 1) * c.n;
-    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / out_words));
-    return host_pipeline(h, count, chunk, simd_scratch_words(c, true, l), in, (u64 *)out, out_words,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return launch_encode_simd(c, d_in.empty() ? nullptr : d_in[0], value_count, l, d_out, w.buf[0],
-                                                       items, w.stream);
-                         });
+    return bfv_encode_simd(h, values, value_count, moduli_count, out, count, kHost64);
 }
 
+static int32_t bfv_decode_simd(const hecuda_context *h, const void *plaintexts, int32_t l, void *values, int64_t count,
+                               Target t) {
+    int32_t rc = check_decode(h, plaintexts, l, values, count);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    const size_t in_words = (size_t)(l ? l : 1) * c.n;
+    return run(h,
+               {"decodeSimd", {{plaintexts, in_words}}, values, (size_t)c.n, simd_scratch_words(c, false, l), simd_chunk(c),
+                stage_items(kStageWords, in_words),
+                [&](const Chunk &x) { return launch_decode_simd(c, x.in[0], l, x.out, x.scratch, x.items, x.stream); }},
+               count, t);
+}
 int32_t hecuda_bfv_decode_simd_device(const hecuda_context *h, const uint64_t *plaintexts, int32_t moduli_count,
                                       uint64_t *values, int64_t count, void *stream) {
-    int32_t rc = check_decode(h, plaintexts, moduli_count, values, count);
-    if (rc || count == 0) return rc;
-    const Context &c = *h->ctx;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int64_t chunk = std::min<int64_t>(simd_chunk(c), count);
-    u64 *scratch = nullptr;
-    CK(cudaMallocAsync(&scratch, simd_scratch_words(c, false, moduli_count) * (size_t)chunk * sizeof(u64), s));
-    const int64_t in_words = (int64_t)(moduli_count ? moduli_count : 1) * c.n;
-    cudaError_t e = cudaSuccess;
-    for (int64_t done = 0; e == cudaSuccess && done < count; done += chunk)
-        e = launch_decode_simd(c, (const u64 *)plaintexts + done * in_words, moduli_count, (u64 *)values + done * c.n, scratch,
-                               std::min<int64_t>(chunk, count - done), s);
-    cudaFreeAsync(scratch, s);
-    return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "decodeSimd");
+    return bfv_decode_simd(h, plaintexts, moduli_count, values, count, on_stream(stream));
 }
-
 int32_t hecuda_bfv_decode_simd(const hecuda_context *h, const uint64_t *plaintexts, int32_t moduli_count, uint64_t *values,
                                int64_t count) {
-    int32_t rc = check_decode(h, plaintexts, moduli_count, values, count);
-    if (rc) return rc;
-    const Context &c = *h->ctx;
-    const int l = moduli_count;
-    const size_t in_words = (size_t)(l ? l : 1) * c.n;
-    std::vector<HostIo> in = {{(const u64 *)plaintexts, in_words}};
-    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / in_words));
-    return host_pipeline(h, count, chunk, simd_scratch_words(c, false, l), in, (u64 *)values, (size_t)c.n,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return launch_decode_simd(c, d_in[0], l, d_out, w.buf[0], items, w.stream);
-                         });
+    return bfv_decode_simd(h, plaintexts, moduli_count, values, count, kHost64);
 }
 
+static int32_t bfv_plaintext_translate(const hecuda_context *h, const void *ct, int32_t poly_count, int32_t l,
+                                       const void *plaintexts, int64_t plaintext_count, int32_t op, void *out, int64_t batch,
+                                       Target t) {
+    int32_t rc = check_translate(h, ct, poly_count, l, plaintexts, plaintext_count, op, out, batch);
+    if (rc || batch == 0) return rc;
+    const Context &c = *h->ctx;
+    const bool broadcast = plaintext_count == 1;
+    const size_t ct_words = (size_t)poly_count * l * c.n;
+    std::vector<Batched::Io> in = {{ct, ct_words}};
+    const u64 *pt = static_cast<const u64 *>(plaintexts);  // the shared plaintext of a broadcast, on the device
+    u64 *d_pt = nullptr;
+    if (!t.device) {
+        if (!host_values_below(plaintexts, (size_t)plaintext_count * c.n, c.t, t.words))
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "encodingDataOutOfBounds: plaintext coefficients must be below t");
+        if (broadcast) {  // uploaded once
+            std::vector<u64> wide(c.n);
+            if (t.words == Words::u32) std::copy((const uint32_t *)plaintexts, (const uint32_t *)plaintexts + c.n, wide.begin());
+            else std::copy(pt, pt + c.n, wide.begin());
+            CK(cudaMalloc(&d_pt, sizeof(u64) * (size_t)c.n));
+            cudaError_t e = upload(d_pt, wide.data(), sizeof(u64) * (size_t)c.n);
+            if (e != cudaSuccess) {
+                cudaFree(d_pt);
+                return cuda_fail(e, "plaintext upload");
+            }
+            pt = d_pt;
+        }
+    }
+    if (!broadcast) in.push_back({plaintexts, (size_t)c.n});
+    rc = run(h,
+             {"plaintextTranslate", in, out, ct_words, 0, kWholeBatch, stage_items(kStageWords, ct_words),
+              [&](const Chunk &x) {
+                  return launch_plaintext_translate(c, x.in[0], poly_count, l, broadcast ? pt : x.in[1], broadcast, op, x.out,
+                                                    x.items, x.stream);
+              }},
+             batch, t);
+    if (d_pt) cudaFree(d_pt);
+    return rc;
+}
 int32_t hecuda_bfv_plaintext_translate_device(const hecuda_context *h, const uint64_t *ct, int32_t poly_count,
                                               int32_t moduli_count, const uint64_t *plaintexts, int64_t plaintext_count,
                                               int32_t op, uint64_t *out, int64_t batch, void *stream) {
-    int32_t rc = check_translate(h, ct, poly_count, moduli_count, plaintexts, plaintext_count, op, out, batch);
-    if (rc) return rc;
-    cudaError_t e = launch_plaintext_translate(*h->ctx, (const u64 *)ct, poly_count, moduli_count, (const u64 *)plaintexts,
-                                               plaintext_count == 1, op, (u64 *)out, batch, (cudaStream_t)stream);
-    return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "plaintextTranslate");
+    return bfv_plaintext_translate(h, ct, poly_count, moduli_count, plaintexts, plaintext_count, op, out, batch,
+                                   on_stream(stream));
 }
-
 int32_t hecuda_bfv_plaintext_translate(const hecuda_context *h, const uint64_t *ct, int32_t poly_count, int32_t moduli_count,
                                        const uint64_t *plaintexts, int64_t plaintext_count, int32_t op, uint64_t *out,
                                        int64_t batch) {
-    int32_t rc = check_translate(h, ct, poly_count, moduli_count, plaintexts, plaintext_count, op, out, batch);
-    if (rc || batch == 0) return rc;
-    const Context &c = *h->ctx;
-    if (!host_values_below(plaintexts, (size_t)plaintext_count * c.n, c.t))
-        return fail(HECUDA_ERR_INVALID_ARGUMENT, "encodingDataOutOfBounds: plaintext coefficients must be below t");
-    const bool broadcast = plaintext_count == 1;
-    const int l = moduli_count;
-    const size_t ct_words = (size_t)poly_count * l * c.n;
-    std::vector<HostIo> in = {{(const u64 *)ct, ct_words}};
-    u64 *d_pt = nullptr;  // the shared plaintext, uploaded once
-    if (broadcast) {
-        std::vector<u64> pt(c.n);
-        if (tl_io32) std::copy((const uint32_t *)plaintexts, (const uint32_t *)plaintexts + c.n, pt.begin());
-        else std::copy(plaintexts, plaintexts + c.n, pt.begin());
-        CK(cudaMalloc(&d_pt, sizeof(u64) * (size_t)c.n));
-        cudaError_t e = upload(d_pt, pt.data(), sizeof(u64) * (size_t)c.n);
-        if (e != cudaSuccess) {
-            cudaFree(d_pt);
-            return cuda_fail(e, "plaintext upload");
-        }
-    } else {
-        in.push_back({(const u64 *)plaintexts, (size_t)c.n});
-    }
-    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / ct_words));
-    rc = host_pipeline(h, batch, chunk, 0, in, (u64 *)out, ct_words,
-                       [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                           return launch_plaintext_translate(c, d_in[0], poly_count, l, broadcast ? d_pt : d_in[1], broadcast,
-                                                             op, d_out, items, w.stream);
-                       });
-    if (d_pt) cudaFree(d_pt);
-    return rc;
+    return bfv_plaintext_translate(h, ct, poly_count, moduli_count, plaintexts, plaintext_count, op, out, batch, kHost64);
 }
 
 // ---------------------------------------------------------------- ct x ct inner product (SURVEY.md 8f rank 2)
 
-static int32_t check_ipc(const hecuda_context *h, const uint64_t *lhs, const uint64_t *rhs, uint64_t *out, int64_t pairs,
+static int32_t check_ipc(const hecuda_context *h, const void *lhs, const void *rhs, const void *out, int64_t pairs,
                          int64_t groups) {
     int32_t rc = check_ctx(h);
     if (rc) return rc;
@@ -1347,42 +1273,26 @@ static int32_t check_ipc(const hecuda_context *h, const uint64_t *lhs, const uin
     return HECUDA_OK;
 }
 
-int32_t hecuda_bfv_inner_product_device(const hecuda_context *h, const uint64_t *lhs, const uint64_t *rhs, uint64_t *out,
-                                        int64_t pairs, int64_t groups, void *stream) {
-    int32_t rc = check_ipc(h, lhs, rhs, out, pairs, groups);
-    if (rc) return rc;
-    if (groups == 0) return HECUDA_OK;
-    const Context &c = *h->ctx;
-    const size_t in_words = (size_t)pairs * 2 * c.L * c.n, out_words = (size_t)3 * c.L * c.n;
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(std::max<int64_t>(1, h->chunk / pairs), groups));
-    cudaStream_t s = (cudaStream_t)stream;
-    u64 *scratch = nullptr;
-    CK(cudaMallocAsync(&scratch, inner_product_scratch_words(c, pairs) * (size_t)chunk * sizeof(u64), s));
-    for (int64_t done = 0; done < groups; done += chunk) {
-        const int64_t g = std::min<int64_t>(chunk, groups - done);
-        cudaError_t e = inner_product_chunk(c, scratch, (const u64 *)lhs + in_words * done, (const u64 *)rhs + in_words * done,
-                                            pairs, (u64 *)out + out_words * done, g, s);
-        if (e != cudaSuccess) {
-            cudaFreeAsync(scratch, s);
-            return cuda_fail(e, "innerProduct");
-        }
-    }
-    CK(cudaFreeAsync(scratch, s));
-    return HECUDA_OK;
-}
-
-int32_t hecuda_bfv_inner_product(const hecuda_context *h, const uint64_t *lhs, const uint64_t *rhs, uint64_t *out,
-                                 int64_t pairs, int64_t groups) {
+static int32_t bfv_inner_product(const hecuda_context *h, const void *lhs, const void *rhs, void *out, int64_t pairs,
+                                 int64_t groups, Target t) {
     int32_t rc = check_ipc(h, lhs, rhs, out, pairs, groups);
     if (rc) return rc;
     const Context &c = *h->ctx;
     const size_t in_words = (size_t)pairs * 2 * c.L * c.n;
-    std::vector<HostIo> in = {{(const u64 *)lhs, in_words}, {(const u64 *)rhs, in_words}};
-    const int64_t chunk = std::max<int64_t>(1, h->chunk / pairs);
-    return host_pipeline(h, groups, chunk, inner_product_scratch_words(c, pairs), in, (u64 *)out, (size_t)3 * c.L * c.n,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t g) {
-                             return inner_product_chunk(c, w.buf[0], d_in[0], d_in[1], pairs, d_out, g, w.stream);
-                         });
+    const int64_t chunk = std::max<int64_t>(1, h->chunk / pairs);  // groups
+    return run(h,
+               {"innerProduct", {{lhs, in_words}, {rhs, in_words}}, out, (size_t)3 * c.L * c.n, inner_product_scratch_words(c, pairs),
+                chunk, chunk,
+                [&](const Chunk &x) { return inner_product_chunk(c, x.scratch, x.in[0], x.in[1], pairs, x.out, x.items, x.stream); }},
+               groups, t);
+}
+int32_t hecuda_bfv_inner_product_device(const hecuda_context *h, const uint64_t *lhs, const uint64_t *rhs, uint64_t *out,
+                                        int64_t pairs, int64_t groups, void *stream) {
+    return bfv_inner_product(h, lhs, rhs, out, pairs, groups, on_stream(stream));
+}
+int32_t hecuda_bfv_inner_product(const hecuda_context *h, const uint64_t *lhs, const uint64_t *rhs, uint64_t *out,
+                                 int64_t pairs, int64_t groups) {
+    return bfv_inner_product(h, lhs, rhs, out, pairs, groups, kHost64);
 }
 
 int32_t hecuda_poly_multiply_power_of_x(const hecuda_context *h, int32_t base, const uint64_t *in, uint64_t *out,
@@ -1395,12 +1305,10 @@ int32_t hecuda_poly_multiply_power_of_x(const hecuda_context *h, int32_t base, c
     if (!make_map(*h->ctx, base, rows, map, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
     const Context &c = *h->ctx;
     const size_t words = (size_t)rows * c.n;
-    std::vector<HostIo> hin = {{(const u64 *)in, words}};
-    const int64_t chunk = std::max<int64_t>(1, (int64_t)((size_t)4 * 1024 * 1024 / words));
-    return host_pipeline(h, polys, chunk, 0, hin, (u64 *)out, words,
-                         [&](Workspace &w, const std::vector<const u64 *> &d_in, u64 *d_out, int64_t items) {
-                             return launch_multiply_power_of_x(c, map, power, d_in[0], d_out, items, w.stream);
-                         });
+    return host_pipeline(h,
+                         {"multiply_power_of_x", {{in, words}}, out, words, 0, kWholeBatch, stage_items(kStageWords, words),
+                          [&](const Chunk &x) { return launch_multiply_power_of_x(c, map, power, x.in[0], x.out, x.items, x.stream); }},
+                         polys, Words::u64);
 }
 
 uint64_t hecuda_kernel_launch_count(void) { return g_kernel_launches.load(); }
@@ -1416,22 +1324,15 @@ static int32_t need_word32(const hecuda_context *h) {
 }
 int32_t hecuda_u32_ntt_forward(const hecuda_context *h, int32_t base, uint32_t *data, int32_t rows, int64_t polys) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_ntt_forward(h, base, reinterpret_cast<uint64_t *>(data), rows, polys);
+    return rc ? rc : ntt(h, base, data, rows, polys, false, kHost32);
 }
 int32_t hecuda_u32_ntt_inverse(const hecuda_context *h, int32_t base, uint32_t *data, int32_t rows, int64_t polys) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_ntt_inverse(h, base, reinterpret_cast<uint64_t *>(data), rows, polys);
+    return rc ? rc : ntt(h, base, data, rows, polys, true, kHost32);
 }
 int32_t hecuda_u32_bfv_multiply(const hecuda_context *h, const uint32_t *lhs, const uint32_t *rhs, uint32_t *out, int64_t batch) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_multiply(h, reinterpret_cast<const uint64_t *>(lhs), reinterpret_cast<const uint64_t *>(rhs),
-                               reinterpret_cast<uint64_t *>(out), batch);
+    return rc ? rc : bfv_multiply(h, lhs, rhs, out, batch, kHost32);
 }
 int32_t hecuda_u32_evk_create(const hecuda_context *h, const uint32_t *relin_key, hecuda_evk **out) {
     int32_t rc = need_word32(h);
@@ -1445,32 +1346,22 @@ int32_t hecuda_u32_evk_create(const hecuda_context *h, const uint32_t *relin_key
 int32_t hecuda_u32_bfv_relinearize(const hecuda_context *h, const hecuda_evk *evk, const uint32_t *ct3, int32_t l, uint32_t *out,
                                    int64_t batch) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_relinearize(h, evk, reinterpret_cast<const uint64_t *>(ct3), l, reinterpret_cast<uint64_t *>(out), batch);
+    return rc ? rc : bfv_relinearize(h, evk, ct3, l, out, batch, kHost32);
 }
 int32_t hecuda_u32_bfv_mod_switch_down(const hecuda_context *h, const uint32_t *ct, int32_t polys, int32_t l, uint32_t *out,
                                        int64_t batch) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_mod_switch_down(h, reinterpret_cast<const uint64_t *>(ct), polys, l, reinterpret_cast<uint64_t *>(out), batch);
+    return rc ? rc : bfv_mod_switch_down(h, ct, polys, l, out, batch, kHost32);
 }
 int32_t hecuda_u32_bfv_multiply_relinearize(const hecuda_context *h, const hecuda_evk *evk, const uint32_t *lhs, const uint32_t *rhs,
                                             int32_t mod_switch, uint32_t *out, int64_t batch) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_multiply_relinearize(h, evk, reinterpret_cast<const uint64_t *>(lhs), reinterpret_cast<const uint64_t *>(rhs),
-                                           mod_switch, reinterpret_cast<uint64_t *>(out), batch);
+    return rc ? rc : bfv_multiply_relinearize(h, evk, lhs, rhs, mod_switch, out, batch, kHost32);
 }
 int32_t hecuda_u32_bfv_relinearize_mod_switch_down(const hecuda_context *h, const hecuda_evk *evk, const uint32_t *ct3, int32_t l,
                                                    uint32_t *out, int64_t batch) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_relinearize_mod_switch_down(h, evk, reinterpret_cast<const uint64_t *>(ct3), l,
-                                                  reinterpret_cast<uint64_t *>(out), batch);
+    return rc ? rc : relinearize_mod_switch_down(h, evk, ct3, l, out, batch, Words::u32);
 }
 int32_t hecuda_u32_evk_set_galois_key(hecuda_evk *evk, uint32_t element, const uint32_t *key) {
     if (!evk || !key) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
@@ -1482,55 +1373,36 @@ int32_t hecuda_u32_evk_set_galois_key(hecuda_evk *evk, uint32_t element, const u
 int32_t hecuda_u32_bfv_apply_galois(const hecuda_context *h, const hecuda_evk *evk, const uint32_t *ct, int32_t l, uint32_t element,
                                     uint32_t *out, int64_t batch) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_apply_galois(h, evk, reinterpret_cast<const uint64_t *>(ct), l, element, reinterpret_cast<uint64_t *>(out), batch);
+    return rc ? rc : bfv_apply_galois(h, evk, ct, l, element, out, batch, kHost32);
 }
 int32_t hecuda_u32_bfv_inner_product(const hecuda_context *h, const uint32_t *lhs, const uint32_t *rhs, uint32_t *out, int64_t pairs,
                                      int64_t groups) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_inner_product(h, reinterpret_cast<const uint64_t *>(lhs), reinterpret_cast<const uint64_t *>(rhs),
-                                    reinterpret_cast<uint64_t *>(out), pairs, groups);
+    return rc ? rc : bfv_inner_product(h, lhs, rhs, out, pairs, groups, kHost32);
 }
 int32_t hecuda_u32_rnstool_lift_q_to_qbsk(const hecuda_context *h, const uint32_t *polys, uint32_t *out, int64_t count) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_rnstool_lift_q_to_qbsk(h, reinterpret_cast<const uint64_t *>(polys), reinterpret_cast<uint64_t *>(out), count);
+    return rc ? rc : lift_or_floor(h, polys, out, count, true, Words::u32);
 }
 int32_t hecuda_u32_rnstool_floor_qbsk_to_q(const hecuda_context *h, const uint32_t *polys, uint32_t *out, int64_t count) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_rnstool_floor_qbsk_to_q(h, reinterpret_cast<const uint64_t *>(polys), reinterpret_cast<uint64_t *>(out), count);
+    return rc ? rc : lift_or_floor(h, polys, out, count, false, Words::u32);
 }
 int32_t hecuda_u32_bfv_encode_simd(const hecuda_context *h, const uint32_t *values, int32_t value_count, int32_t moduli_count,
                                    uint32_t *out, int64_t count) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_encode_simd(h, reinterpret_cast<const uint64_t *>(values), value_count, moduli_count,
-                                  reinterpret_cast<uint64_t *>(out), count);
+    return rc ? rc : bfv_encode_simd(h, values, value_count, moduli_count, out, count, kHost32);
 }
 int32_t hecuda_u32_bfv_decode_simd(const hecuda_context *h, const uint32_t *plaintexts, int32_t moduli_count, uint32_t *values,
                                    int64_t count) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_decode_simd(h, reinterpret_cast<const uint64_t *>(plaintexts), moduli_count,
-                                  reinterpret_cast<uint64_t *>(values), count);
+    return rc ? rc : bfv_decode_simd(h, plaintexts, moduli_count, values, count, kHost32);
 }
 int32_t hecuda_u32_bfv_plaintext_translate(const hecuda_context *h, const uint32_t *ct, int32_t poly_count, int32_t moduli_count,
                                            const uint32_t *plaintexts, int64_t plaintext_count, int32_t op, uint32_t *out,
                                            int64_t batch) {
     int32_t rc = need_word32(h);
-    if (rc) return rc;
-    Io32Scope scope;
-    return hecuda_bfv_plaintext_translate(h, reinterpret_cast<const uint64_t *>(ct), poly_count, moduli_count,
-                                          reinterpret_cast<const uint64_t *>(plaintexts), plaintext_count, op,
-                                          reinterpret_cast<uint64_t *>(out), batch);
+    return rc ? rc : bfv_plaintext_translate(h, ct, poly_count, moduli_count, plaintexts, plaintext_count, op, out, batch, kHost32);
 }
 
 }  // extern "C"

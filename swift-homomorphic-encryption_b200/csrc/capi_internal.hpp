@@ -41,27 +41,33 @@ inline cudaError_t fill(void *dst, int value, size_t bytes) {
     return e != cudaSuccess ? e : cudaStreamSynchronize(cudaStreamLegacy);
 }
 
-// Scratch for one in-flight chunk.  Grows on demand, never shrinks.
+// A device buffer that grows on demand and never shrinks.
+struct GrowBuffer {
+    u64 *p = nullptr;
+    size_t cap = 0;  // words
+    cudaError_t reserve(size_t words) {
+        if (cap >= words) return cudaSuccess;
+        if (p) {
+            cudaError_t e = cudaFree(p);
+            if (e != cudaSuccess) return e;
+            p = nullptr;
+            cap = 0;
+        }
+        cudaError_t e = cudaMalloc(&p, words * sizeof(u64));
+        if (e == cudaSuccess) cap = words;
+        return e;
+    }
+};
+
+// A stream and what one in-flight stage of the host pipeline (capi.cu) stages through it.
 struct Workspace {
     cudaStream_t stream = nullptr;
     bool owns_stream = false;
-    u64 *buf[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    size_t cap[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    cudaError_t reserve(int i, size_t words) {
-        if (cap[i] >= words) return cudaSuccess;
-        if (buf[i]) {
-            cudaError_t e = cudaFree(buf[i]);
-            if (e != cudaSuccess) return e;
-            buf[i] = nullptr;
-            cap[i] = 0;
-        }
-        cudaError_t e = cudaMalloc(&buf[i], words * sizeof(u64));
-        if (e == cudaSuccess) cap[i] = words;
-        return e;
-    }
+    GrowBuffer scratch, in, out;  // kernel scratch, staged inputs (back to back), staged output
+    GrowBuffer in32, out32;       // the uint32 images of `in` and `out` when the host buffers hold uint32 words
     void release() {
-        for (int i = 0; i < 8; ++i)
-            if (buf[i]) cudaFree(buf[i]);
+        for (GrowBuffer *b : {&scratch, &in, &out, &in32, &out32})
+            if (b->p) cudaFree(b->p);
         if (owns_stream && stream) cudaStreamDestroy(stream);
     }
 };
