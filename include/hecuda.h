@@ -666,6 +666,53 @@ int32_t hecuda_bfv_decrypt(const hecuda_context *ctx, const uint64_t *secret_key
                            int32_t poly_count, int32_t moduli_count, uint64_t scaling_factor, uint64_t *plaintexts,
                            int64_t batch);
 
+/* ---- client side: secret keys, encryption, evaluation keys, noise budgets (uint64_t only) ----
+ * Every random polynomial comes from a NistAes128Ctr(seed:) stream (the generator of hecuda_poly_random_from_seed), one
+ * stream per polynomial, keyed by a 32-byte seed the caller supplies.  The reference draws `a` the same way and the
+ * secret and the error from SystemRandomNumberGenerator (Bfv+Keys.swift:20-26, Bfv+Encrypt.swift:150-181); here their
+ * seeds must come from a cryptographically secure source (the Python layer uses secrets.token_bytes) and must never be
+ * reused or revealed.  Each stream maps to coefficients byte for byte as the reference maps its generator:
+ *   secret  PolyRq.randomizeTernary (PolyRq+Randomize.swift:87-104): coefficient j takes a little-endian UInt64 and a
+ *           UInt32 (stream bytes 12j..12j+11), (u64 << 32 | u32) mod 3, minus 1 modulo every q_i;
+ *   error   randomizeCenteredBinomialDistribution (:120-160) at ErrorStdDev.stdDev32 (sigma = 3.2, k = 21): coefficient j
+ *           takes two little-endian UInt64 (bytes 16j..16j+15), each masked to k bits, popcount(first) - popcount(second);
+ *   a       PolyRq.random (:49-81), sampled in Eval format as hecuda_poly_random_from_seed.
+ * Device copies of the secret key, s^2, s(X^g), the errors and the error seeds are zeroized before they are freed.
+ *
+ * hecuda_bfv_generate_secret_key = Bfv.generateSecretKey (Bfv+Keys.swift:20-26): seeds count x 32 -> secret_keys count x
+ * K x N, SecretKey.poly in Eval format over all K coefficient moduli (K = L + 1, or 1 for a single modulus).
+ * hecuda_bfv_encrypt = Bfv.encrypt (Bfv+Encrypt.swift:64-72: encryptZero :141-181, then plaintextTranslate(.Add)
+ * :75-139) at the top level: secret_key K x N (Eval); plaintexts batch x N Coeff values < t; a_seeds, error_seeds batch x
+ * 32 -> ciphertexts batch x 2 x L x N (Coeff) = (-(INTT(a s) + e) + Delta m + adjust, INTT(a)).  A value >= t:
+ * HECUDA_ERR_INVALID_ARGUMENT.
+ * hecuda_bfv_encrypt_seeded: the same ciphertexts in the .seeded(poly0:seed:) wire form (SerializedCiphertext.swift:41-60):
+ * poly0 batch x hecuda_poly_serialized_byte_count(ctx, HECUDA_BASE_Q, L, 0) bytes; the seed is a_seeds[i].  This is what
+ * hecuda_ciphertext_expand_seeded and the _clients_wire calls read.
+ * hecuda_evk_generate = Bfv.generateEvaluationKey (Bfv+Keys.swift:30-65, _generateKeySwitchKey :67-103): for each key,
+ * key ciphertext i is encryptZero over [q_0..q_{L-1}, q_ks] in Eval with (q_ks mod q_i) currentKey[i] added to row i of
+ * poly0; currentKey = s^2 for the relinearization key (has_relin != 0), s(X^g) for each element g (Galois.swift:151-166).
+ * a_seeds and error_seeds: (has_relin + element_count) x L x 32 bytes, in hecuda_evk_create_serialized's order (the
+ * relinearization key, then elements[]).  *out is an ordinary evaluation key.  wire_poly0 (nullable): the keys' poly0 in
+ * hecuda_evk_create_serialized's layout, so that (wire_poly0, a_seeds) loads the same key there.  Errors as
+ * hecuda_evk_create_serialized, plus HECUDA_ERR_MISSING_KEY for a null secret key and HECUDA_ERR_INVALID_ARGUMENT for null
+ * seeds; on error *out is NULL and nothing was launched.
+ * hecuda_bfv_noise_budget = Bfv.noiseBudgetEval / noiseBudgetCoeff (Bfv+Decrypt.swift:116-185): ciphertexts batch x
+ * poly_count x moduli_count x N (Coeff, or Eval with eval_format != 0; poly_count 2 or 3, any level) -> budgets[batch] =
+ * log2(qDouble / (2 norm)), norm = the largest centred |[t (c0 + c1 s (+ c2 s^2))]_q| as a Double (round to nearest),
+ * qDouble the running product of Double(q_i); +inf for a zero norm.
+ * WARNING (Bfv+Decrypt.swift:111-112): a noise budget must never be forwarded to any other party.  Sharing it acts as an
+ * oracle that can be used to recover the secret key. */
+int32_t hecuda_bfv_generate_secret_key(const hecuda_context *ctx, const uint8_t *seeds, uint64_t *secret_keys, int64_t count);
+int32_t hecuda_bfv_encrypt(const hecuda_context *ctx, const uint64_t *secret_key, const uint64_t *plaintexts,
+                           const uint8_t *a_seeds, const uint8_t *error_seeds, uint64_t *ciphertexts, int64_t batch);
+int32_t hecuda_bfv_encrypt_seeded(const hecuda_context *ctx, const uint64_t *secret_key, const uint64_t *plaintexts,
+                                  const uint8_t *a_seeds, const uint8_t *error_seeds, uint8_t *poly0, int64_t batch);
+int32_t hecuda_evk_generate(const hecuda_context *ctx, const uint64_t *secret_key, int32_t has_relin, const uint32_t *elements,
+                            int32_t element_count, const uint8_t *a_seeds, const uint8_t *error_seeds, hecuda_evk **out,
+                            uint8_t *wire_poly0);
+int32_t hecuda_bfv_noise_budget(const hecuda_context *ctx, const uint64_t *secret_key, const uint64_t *ciphertexts,
+                                int32_t poly_count, int32_t moduli_count, int32_t eval_format, double *budgets, int64_t batch);
+
 /* Bookkeeping for bench.py: number of kernel launches issued by this library in the calling process so far. */
 uint64_t hecuda_kernel_launch_count(void);
 

@@ -166,6 +166,12 @@ cudaError_t expand_seeded_device(const Context &c, int l, const unsigned char *d
 // count x 32; ciphertext i's 2 x K x N words go to d_dst[i] (a device table of pointers into evaluation keys)
 cudaError_t expand_seeded_keys_device(const Context &c, const unsigned char *d_poly0, const unsigned char *d_seeds,
                                       u64 *const *d_dst, int64_t count, cudaStream_t s);
+// NistAes128Ctr streams (drbg.cu): the AES tables, then for every 32-byte seed the round keys (segments x 44 words) and
+// counters V (segments x 2 words) of its first `segments` 4096-byte segments; free_chains zeroizes the round keys.
+cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, unsigned int **d_rk, u64 **d_ctr,
+                        cudaStream_t s);
+void free_chains(unsigned int *d_rk, u64 *d_ctr, int segments, int64_t batch, cudaStream_t s);
+cudaError_t drbg_tables(const unsigned char **sbox, const unsigned int **te0);
 cudaError_t inner_product_chunk(const Context &c, u64 *scratch, const u64 *lhs, const u64 *rhs, int64_t pairs, u64 *out,
                                 int64_t groups, cudaStream_t s);
 // `tables` MulPir databases from entry bytes already on the device (pir.cu; used by keyword_pir.cu)

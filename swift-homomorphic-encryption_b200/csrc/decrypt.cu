@@ -6,6 +6,9 @@
 // c_0 + c_1 s + c_2 s^2 in Eval format, inverse NTT, then per coefficient: scale by gamma*t, exact base conversion to
 // {t, gamma} (the sums are reduced modulo the small moduli, so any summation order gives the reference's residues),
 // the gamma-centred correction, and the final multiplication by gamma^-1 * scalingFactor mod t.
+#include <cmath>
+#include <vector>
+
 #include "capi_internal.hpp"
 #include "hostmath.hpp"
 #include "modarith.cuh"
@@ -121,6 +124,131 @@ cudaError_t decrypt_chunk(const Context &c, const DecryptConsts &dc, u64 *scratc
     return cudaGetLastError();
 }
 
+// ---------------------------------------------------------------- noise budget
+// Bfv.noiseBudgetEval (Bfv+Decrypt.swift:116-174): v = c_0 + c_1 s (+ c_2 s^2) by dot_secret_kernel, the inverse NTT,
+// then per coefficient the CRT composition of [v t]_{q_i} into a multi-word integer in [0, q) (RnsTool.crtCompose),
+// its centred absolute value against (q + 1) / 2, and the maximum over the ciphertext.  The host turns the maximum into
+// log2(qDouble / (2 norm)).
+constexpr int kNormThreads = 256;
+
+struct NoiseConsts {
+    int l;              // rows = words of q (every q_i < 2^64)
+    u64 q[kMaxL];
+    u64 t_mod[kMaxL];   // t mod q_i
+    u64 inv_punctured[kMaxL];  // (q / q_i)^-1 mod q_i
+};
+
+// a > b over `w` words (little-endian)
+__device__ __forceinline__ bool wide_greater(const u64 *a, const u64 *b, int w) {
+    for (int i = w - 1; i >= 0; --i)
+        if (a[i] != b[i]) return a[i] > b[i];
+    return false;
+}
+
+// one CTA per ciphertext; big = [q / q_i for each i][q][(q + 1) / 2], l words each; out: items x l words
+__global__ void __launch_bounds__(kNormThreads) noise_norm_kernel(const u64 *__restrict__ v, const u64 *__restrict__ big,
+                                                                 const __grid_constant__ NoiseConsts c, int n, u64 *__restrict__ out) {
+    __shared__ u64 warp_best[kNormThreads / 32][kMaxL];
+    const int W = c.l;
+    const u64 *q = big + (size_t)W * W, *half = q + W;
+    const long long item = blockIdx.x;
+    u64 best[kMaxL], acc[kMaxL + 1], other[kMaxL];
+    for (int w = 0; w < W; ++w) best[w] = 0;
+    for (int e = threadIdx.x; e < n; e += blockDim.x) {
+        for (int w = 0; w <= W; ++w) acc[w] = 0;
+        for (int i = 0; i < W; ++i) {
+            const u64 x = v[(item * W + i) * (long long)n + e];
+            const u64 y = mulmod_dev(mulmod_dev(x, c.t_mod[i], c.q[i]), c.inv_punctured[i], c.q[i]);
+            const u64 *punct = big + (size_t)i * W;
+            u64 carry = 0;
+            for (int w = 0; w < W; ++w) {
+                const u128 prod = (u128)y * punct[w] + acc[w] + carry;
+                acc[w] = (u64)prod;
+                carry = (u64)(prod >> 64);
+            }
+            acc[W] += carry;
+        }
+        // the sum is below l q: subtract q until it is in [0, q)
+        while (acc[W] || !wide_greater(q, acc, W)) {
+            u64 borrow = 0;
+            for (int w = 0; w < W; ++w) {
+                const u64 d = acc[w] - q[w] - borrow;
+                borrow = (acc[w] < q[w] || (acc[w] == q[w] && borrow)) ? 1 : 0;
+                acc[w] = d;
+            }
+            acc[W] -= borrow;
+        }
+        if (wide_greater(acc, half, W)) {  // q - coeff
+            u64 borrow = 0;
+            for (int w = 0; w < W; ++w) {
+                const u64 d = q[w] - acc[w] - borrow;
+                borrow = (q[w] < acc[w] || (q[w] == acc[w] && borrow)) ? 1 : 0;
+                acc[w] = d;
+            }
+        }
+        if (wide_greater(acc, best, W))
+            for (int w = 0; w < W; ++w) best[w] = acc[w];
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+        for (int w = 0; w < W; ++w) other[w] = __shfl_down_sync(0xffffffffu, best[w], off);
+        if (wide_greater(other, best, W))
+            for (int w = 0; w < W; ++w) best[w] = other[w];
+    }
+    const int warp = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0)
+        for (int w = 0; w < W; ++w) warp_best[warp][w] = best[w];
+    __syncthreads();
+    if (threadIdx.x) return;
+    for (int k = 1; k < (int)(blockDim.x >> 5); ++k)
+        if (wide_greater(warp_best[k], best, W))
+            for (int w = 0; w < W; ++w) best[w] = warp_best[k][w];
+    for (int w = 0; w < W; ++w) out[item * W + w] = best[w];
+}
+
+// x (w little-endian words) as a Double, rounded to nearest (ties to even) like Double(_:) of a wide integer
+double wide_to_double(const u64 *x, int w) {
+    int top = w - 1;
+    while (top >= 0 && !x[top]) --top;
+    if (top < 0) return 0.0;
+    if (top == 0) return (double)x[0];
+    const int lz = __builtin_clzll(x[top]);
+    u64 m = lz ? (x[top] << lz) | (x[top - 1] >> (64 - lz)) : x[top];  // the leading 64 bits
+    bool sticky = lz ? (x[top - 1] << lz) != 0 : false;
+    for (int i = top - 2; i >= 0 && !sticky; --i) sticky = x[i] != 0;
+    if (sticky) m |= 1;  // far below the rounding bit of the 53-bit result: only breaks ties
+    return std::ldexp((double)m, 64 * top - lz);
+}
+
+// big = [q / q_i for each i][q][(q + 1) / 2] as l-word integers
+std::vector<u64> noise_big_constants(const u64 *q, int l) {
+    std::vector<u64> big((size_t)(l + 2) * l, 0);
+    auto mul_small = [&](u64 *x, u64 m) {
+        u64 carry = 0;
+        for (int w = 0; w < l; ++w) {
+            const unsigned __int128 p = (unsigned __int128)x[w] * m + carry;
+            x[w] = (u64)p;
+            carry = (u64)(p >> 64);
+        }
+    };
+    for (int i = 0; i < l; ++i) {
+        u64 *p = &big[(size_t)i * l];
+        p[0] = 1;
+        for (int j = 0; j < l; ++j)
+            if (j != i) mul_small(p, q[j]);
+    }
+    u64 *prod = &big[(size_t)l * l], *half = prod + l;
+    prod[0] = 1;
+    for (int j = 0; j < l; ++j) mul_small(prod, q[j]);
+    unsigned carry = 1;  // (q + 1) >> 1
+    for (int w = 0; w < l; ++w) {
+        const u64 s = prod[w] + carry;
+        carry = (carry && s == 0) ? 1 : 0;
+        half[w] = s;
+    }
+    for (int w = 0; w < l; ++w) half[w] = (half[w] >> 1) | (w + 1 < l ? half[w + 1] << 63 : (u64)carry << 63);
+    return big;
+}
+
 }  // namespace
 
 extern "C" {
@@ -173,6 +301,85 @@ int32_t hecuda_bfv_decrypt(const hecuda_context *h, const uint64_t *secret_key, 
     cudaFree(d_sk);
     if (e == cudaSuccess) e = e2;
     return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "decrypt");
+}
+
+int32_t hecuda_bfv_noise_budget(const hecuda_context *h, const uint64_t *secret_key, const uint64_t *ciphertexts, int32_t polys,
+                                int32_t l, int32_t eval_format, double *budgets, int64_t batch) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    if (!secret_key) return fail(HECUDA_ERR_MISSING_KEY, "null secret key");
+    if (polys < 2 || polys > 3) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: poly_count must be 2 or 3");
+    if (l < 1 || l > c.L) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: moduli_count out of range");
+    if (batch < 0 || (batch && (!ciphertexts || !budgets))) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidCiphertext: null buffer");
+    if (batch == 0) return HECUDA_OK;
+    const DecryptConsts dc = make_consts(c, l, 1);
+    NoiseConsts nc;
+    nc.l = l;
+    for (int i = 0; i < l; ++i) {
+        nc.q[i] = dc.q[i];
+        nc.t_mod[i] = c.t % dc.q[i];
+        nc.inv_punctured[i] = dc.inv_punctured[i];
+    }
+    const std::vector<u64> big = noise_big_constants(dc.q, l);
+    const int64_t n = c.n;
+    const size_t in_words = (size_t)polys * l * n;
+    const int64_t cap = std::min<int64_t>(batch, std::max<int64_t>(1, (int64_t)((size_t)64 * 1024 * 1024 / in_words)));
+    std::vector<u64> norms((size_t)batch * l);
+    WsGuard g(h);
+    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    cudaStream_t s = g.w->stream;
+    u64 *d_sk = nullptr, *d_big = nullptr, *d_in = nullptr, *d_ev = nullptr, *d_dot = nullptr, *d_norm = nullptr;
+    cudaError_t e = cudaMallocAsync((void **)&d_sk, (size_t)l * n * sizeof(u64), s);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_big, big.size() * sizeof(u64), s);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_in, in_words * cap * sizeof(u64), s);
+    if (e == cudaSuccess && !eval_format) e = cudaMallocAsync((void **)&d_ev, in_words * cap * sizeof(u64), s);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_dot, (size_t)l * n * cap * sizeof(u64), s);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_norm, (size_t)l * cap * sizeof(u64), s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_sk, secret_key, (size_t)l * n * sizeof(u64), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_big, big.data(), big.size() * sizeof(u64), cudaMemcpyHostToDevice, s);
+    const NttRowMap map = c.map_q(l);
+    const int threads = n >= 256 ? 256 : (n < 32 ? 32 : (int)n);
+    const unsigned gx = (unsigned)((n + threads - 1) / threads);
+    for (int64_t done = 0; e == cudaSuccess && done < batch; done += cap) {
+        const int64_t items = std::min<int64_t>(cap, batch - done);
+        e = cudaMemcpyAsync(d_in, ciphertexts + in_words * done, in_words * items * sizeof(u64), cudaMemcpyHostToDevice, s);
+        const u64 *ev = d_in;
+        if (e == cudaSuccess && !eval_format) {  // noiseBudgetCoeff = noiseBudgetEval of convertToEvalFormat (:181-185)
+            e = launch_ntt_forward(c, map, d_in, d_ev, items * polys * l, s);
+            ev = d_ev;
+        }
+        for (int64_t first = 0; e == cudaSuccess && first < items;) {
+            const int64_t part = std::min<int64_t>(items - first, 65535);
+            ++g_kernel_launches;
+            dot_secret_kernel<<<dim3(gx, (unsigned)l, (unsigned)part), threads, 0, s>>>(ev + first * polys * l * n, d_sk,
+                                                                                       d_dot + first * l * n, dc, (int)n, polys);
+            e = cudaGetLastError();
+            first += part;
+        }
+        if (e == cudaSuccess) e = launch_ntt_inverse(c, map, d_dot, d_dot, items * l, kScalePlain, s);
+        if (e == cudaSuccess) {
+            ++g_kernel_launches;
+            noise_norm_kernel<<<(unsigned)items, kNormThreads, 0, s>>>(d_dot, d_big, nc, (int)n, d_norm);
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess)
+            e = cudaMemcpyAsync(norms.data() + (size_t)l * done, d_norm, (size_t)l * items * sizeof(u64), cudaMemcpyDeviceToHost, s);
+    }
+    if (d_sk) cudaMemsetAsync(d_sk, 0, (size_t)l * n * sizeof(u64), s);  // zeroize the key copy
+    if (d_dot) cudaMemsetAsync(d_dot, 0, (size_t)l * n * cap * sizeof(u64), s);  // v = m Delta + noise: secret too
+    for (void *p : {(void *)d_sk, (void *)d_big, (void *)d_in, (void *)d_ev, (void *)d_dot, (void *)d_norm})
+        if (p) cudaFreeAsync(p, s);
+    const cudaError_t e2 = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = e2;
+    if (e != cudaSuccess) return cuda_fail(e, "noise_budget");
+    double q_double = 1.0;  // vTimesT.moduli.map { Double($0) }.reduce(1.0, *)
+    for (int i = 0; i < l; ++i) q_double *= (double)dc.q[i];
+    for (int64_t b = 0; b < batch; ++b) {
+        const double norm = wide_to_double(norms.data() + (size_t)l * b, l);
+        budgets[b] = norm == 0.0 ? HUGE_VAL : std::log2(q_double / (2 * norm));
+    }
+    return HECUDA_OK;
 }
 
 }  // extern "C"

@@ -137,6 +137,11 @@ __global__ void __launch_bounds__(kSegmentBlocks) key_expand_kernel(const u32w *
     out[(long long)c.rows * n + k] = (u64)((((u128)hi << 64) | lo) % c.p[row]);
 }
 
+}  // namespace
+
+namespace hecuda {
+namespace api {
+
 // The AES tables, then every seed's chain: (round keys, V) of each of its `segments` segments into *d_rk / *d_ctr, both
 // allocated on `s` and released by free_chains.
 cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, u32w **d_rk, u64 **d_ctr, cudaStream_t s) {
@@ -165,6 +170,17 @@ void free_chains(u32w *d_rk, u64 *d_ctr, int segments, int64_t batch, cudaStream
     }
     if (d_ctr) cudaFreeAsync(d_ctr, s);
 }
+
+// Device addresses of the AES tables drbg_chains uploads, for kernels in other translation units that read a stream
+cudaError_t drbg_tables(const unsigned char **sbox, const u32w **te0) {
+    cudaError_t e = cudaGetSymbolAddress((void **)sbox, c_sbox);
+    return e == cudaSuccess ? cudaGetSymbolAddress((void **)te0, c_te0) : e;
+}
+
+}  // namespace api
+}  // namespace hecuda
+
+namespace {
 
 cudaError_t random_polys_device(const Context &c, int l, const unsigned char *d_seeds, u64 *d_out, int64_t batch,
                                 cudaStream_t s) {

@@ -99,6 +99,21 @@ cudaError_t launch_inner_product_plain_clients(const Context &ctx, const u64 *ct
 cudaError_t launch_plaintext_to_eval(const Context &ctx, const u64 *plain, int l, u64 *out, int64_t count,
                                      cudaStream_t stream);
 
+#ifdef __CUDACC__
+// floor(([Q_l]_t m + tThreshold) / t) for m < t (context.hpp, TranslateConsts): the rounding term of plaintextTranslate,
+// shared by the translate kernel (plaintext.cu) and the encryption epilogue (client.cu)
+__device__ __forceinline__ u64 translate_adjust(u64 m, const TranslateConsts &c) {
+    const u64 quot = mulhi64(m, c.q_mod_t_p);
+    u64 r = m * c.q_mod_t - quot * c.t;  // [Q_l]_t m - quot t in [0, 2t)
+    u64 fl = quot;
+    if (r >= c.t) {
+        r -= c.t;
+        ++fl;
+    }
+    return fl + (r + c.t_threshold >= c.t ? 1 : 0);
+}
+#endif
+
 // ---- the plaintext side of Bfv (plaintext.cu); the context must support SIMD encoding for encode / decode
 // encodeSimd (+ convertToEvalFormat when l >= 1): values count x value_count (< t) -> out count x N (Coeff, l = 0) or
 // count x l x N (Eval).  decodeSimd / decodeEval: plain count x N (l = 0) or count x l x N -> values count x N.

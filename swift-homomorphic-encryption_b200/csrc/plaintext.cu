@@ -22,18 +22,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int64_t kMaxGridY = 65535;
 
-// floor(([Q_l]_t m + tThreshold) / t) for m < t (context.hpp, TranslateConsts)
-__device__ __forceinline__ u64 translate_adjust(u64 m, const TranslateConsts &c) {
-    const u64 quot = mulhi64(m, c.q_mod_t_p);
-    u64 r = m * c.q_mod_t - quot * c.t;  // [Q_l]_t m - quot t in [0, 2t)
-    u64 fl = quot;
-    if (r >= c.t) {
-        r -= c.t;
-        ++fl;
-    }
-    return fl + (r + c.t_threshold >= c.t ? 1 : 0);
-}
-
 template <int OP>
 __device__ __forceinline__ u64 translate_one(u64 x, u64 v, u64 q) {
     if (OP == HECUDA_PLAINTEXT_ADD) return add_mod(x, v, q);

@@ -15,6 +15,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import secrets
 
 import numpy as np
 
@@ -159,6 +160,11 @@ SYMBOLS = {
     "hecuda_poly_random_from_seed": (C.c_int32, [_VP, _VP, C.c_int32, _VP, C.c_int64]),
     "hecuda_ciphertext_expand_seeded": (C.c_int32, [_VP, _VP, _VP, C.c_int32, _VP, C.c_int64]),
     "hecuda_bfv_decrypt": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int32, C.c_uint64, _VP, C.c_int64]),
+    "hecuda_bfv_generate_secret_key": (C.c_int32, [_VP, _VP, _VP, C.c_int64]),
+    "hecuda_bfv_encrypt": (C.c_int32, [_VP, _VP, _VP, _VP, _VP, _VP, C.c_int64]),
+    "hecuda_bfv_encrypt_seeded": (C.c_int32, [_VP, _VP, _VP, _VP, _VP, _VP, C.c_int64]),
+    "hecuda_evk_generate": (C.c_int32, [_VP, _VP, C.c_int32, _VP, C.c_int32, _VP, _VP, C.POINTER(_VP), _VP]),
+    "hecuda_bfv_noise_budget": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int32, C.c_int32, _VP, C.c_int64]),
     "hecuda_poly_add": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int32, C.c_int64]),
     "hecuda_poly_add_device": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int32, C.c_int64, _VP]),
     "hecuda_poly_sub": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int32, C.c_int64]),
@@ -369,6 +375,40 @@ class Context:
         return roots, inv
 
 
+def _seeds(count: int, seeds=None) -> np.ndarray:
+    """`count` 32-byte NistAes128Ctr seeds: the caller's, or fresh ones from the operating system's CSPRNG."""
+    if seeds is None:
+        return np.frombuffer(secrets.token_bytes(32 * count) or b"\0" * 32, dtype=np.uint8)[:32 * count].reshape(count, 32).copy()
+    if isinstance(seeds, (bytes, bytearray)):
+        seeds = np.frombuffer(bytes(seeds), dtype=np.uint8)
+    sd = np.array(seeds, dtype=np.uint8, copy=True).reshape(-1, 32)  # a copy: the error seeds are zeroized after use
+    if sd.shape[0] != count:
+        raise HeError(-1, f"expected {count} seeds of 32 bytes, got {sd.shape[0]}")
+    return sd
+
+
+def _secret_poly(secretKey) -> np.ndarray:
+    return _host(secretKey.poly if isinstance(secretKey, SecretKey) else secretKey)
+
+
+class SecretKey:
+    """SecretKey<Bfv<UInt64>> (Keys.swift:20-60): `poly` is SecretKey.poly, (K, N) in Eval format over every coefficient
+    modulus (K = L + 1, or 1 for a single modulus).  Never leaves the client."""
+
+    def __init__(self, context: Context, poly):
+        self.context, self.poly = context, _host(poly)
+
+    @classmethod
+    def generate(cls, context: Context, seed=None) -> "SecretKey":
+        """Bfv.generateSecretKey (Bfv+Keys.swift:20-26) on the device: randomizeTernary over a NistAes128Ctr stream keyed by
+        `seed` (32 bytes; by default fresh from secrets.token_bytes), then the forward NTT."""
+        sd = _seeds(1, seed)
+        K = context.L + 1 if len(context.coefficientModuli) > 1 else 1
+        out = np.empty((1, K, context.degree), dtype=np.uint64)
+        _check(load_library().hecuda_bfv_generate_secret_key(context._h, _ptr(sd), _ptr(out), 1))
+        return cls(context, out[0])
+
+
 class EvaluationKey:
     """EvaluationKey<Bfv<UInt64>> holding the relinearization key (Keys.swift:66-99,222)."""
 
@@ -422,6 +462,37 @@ class EvaluationKey:
         key = cls.__new__(cls)
         key.context, key.galoisElements, key._h = context, elements, h
         return key
+
+    @classmethod
+    def generate(cls, context: Context, config, secretKey, wire: bool = False, aSeeds=None, errorSeeds=None):
+        """Bfv.generateEvaluationKey (Bfv+Keys.swift:30-103) on the device (hecuda_evk_generate).  config: an
+        EvaluationKeyConfig (galoisElements, hasRelinearizationKey).  Seeds: (keys x L, 32) uint8 in the order of
+        fromSerialized (the relinearization key, then galoisElements), fresh from secrets.token_bytes by default.
+        wire=True also returns the seeded wire form as fromSerialized's keyword arguments:
+        (key, {"relinPoly0", "relinSeeds", "galois": {element: (poly0, seeds)}})."""
+        L = context.L
+        elements = [int(e) for e in dict.fromkeys(config.galoisElements)]  # the reference skips repeated elements
+        relin = bool(config.hasRelinearizationKey)
+        count = (int(relin) + len(elements)) * L
+        a = _seeds(count, aSeeds)
+        err = _seeds(count, errorSeeds)
+        elems = np.ascontiguousarray(elements, dtype=np.uint32)
+        size = Bfv.serializationByteCount(context, L + 1, base=BASE_KEYSWITCH)
+        poly0 = np.empty((count, size), dtype=np.uint8) if wire else None
+        h = C.c_void_p()
+        _check(load_library().hecuda_evk_generate(context._h, _ptr(_secret_poly(secretKey)), int(relin),
+                                                  _ptr(elems) if elements else None, len(elements), _ptr(a), _ptr(err),
+                                                  C.byref(h), _ptr(poly0) if wire else None))
+        err[:] = 0
+        key = cls.__new__(cls)
+        key.context, key.galoisElements, key._h = context, elements, h
+        if not wire:
+            return key
+        first = L if relin else 0
+        form = {"relinPoly0": poly0[:L] if relin else None, "relinSeeds": a[:L] if relin else None,
+                "galois": {e: (poly0[first + j * L:first + (j + 1) * L], a[first + j * L:first + (j + 1) * L])
+                           for j, e in enumerate(elements)}}
+        return key, form
 
     def setGaloisKey(self, element: int, key):
         """GaloisKey.keys[element] (Keys.swift:150-163): (L, 2, L+1, N) uint64, Eval format."""
@@ -739,15 +810,56 @@ class Bfv:
         """PolyRq *= [T] (PolyRq.swift:232-245): one reduced scalar per RNS row."""
         return Bfv._elementwise("mul_scalars", context, poly, np.asarray(scalars, dtype=np.uint64), base)
 
+    minNoiseBudget = 0.0  # Bfv.minNoiseBudget (Bfv.swift:41-43)
+
+    @staticmethod
+    def encrypt(context: Context, secretKey, plaintexts, seeded: bool = False, aSeeds=None, errorSeeds=None):
+        """Bfv.encrypt (Bfv+Encrypt.swift:64-181) of (batch, N) Coeff plaintexts (values < t) at the top level, on the
+        device.  Seeds (batch, 32) uint8 default to fresh ones from secrets.token_bytes.  Returns (batch, 2, L, N) Coeff
+        ciphertexts, or with seeded=True the .seeded(poly0:seed:) wire form (poly0 (batch, B) uint8, a-seeds (batch, 32))."""
+        pts = _host(plaintexts).reshape(-1, context.degree)
+        batch = pts.shape[0]
+        a = _seeds(batch, aSeeds)
+        err = _seeds(batch, errorSeeds)
+        sk = _secret_poly(secretKey)
+        lib = load_library()
+        if seeded:
+            out = np.empty((batch, Bfv.serializationByteCount(context, context.L)), dtype=np.uint8)
+            _check(lib.hecuda_bfv_encrypt_seeded(context._h, _ptr(sk), _ptr(pts), _ptr(a), _ptr(err), _ptr(out), batch))
+            err[:] = 0
+            return out, a
+        out = np.empty((batch, 2, context.L, context.degree), dtype=np.uint64)
+        _check(lib.hecuda_bfv_encrypt(context._h, _ptr(sk), _ptr(pts), _ptr(a), _ptr(err), _ptr(out), batch))
+        err[:] = 0
+        return out
+
+    @staticmethod
+    def noiseBudget(context: Context, secretKey, ciphertexts, evalFormat: bool = False):
+        """Bfv.noiseBudgetCoeff / noiseBudgetEval (Bfv+Decrypt.swift:116-185) with variableTime: (batch, polys, l, N) ->
+        (batch,) float64; one (polys, l, N) ciphertext -> float.  inf for a noiseless ciphertext.
+        Warning: the noise budget must never be forwarded to another party; it acts as an oracle for the secret key."""
+        cts = _host(ciphertexts)
+        single = cts.ndim == 3
+        if single:
+            cts = cts[None]
+        batch, polys, l, n = cts.shape
+        sk = _secret_poly(secretKey)
+        if sk.size < l * n:
+            raise HeError(-1, "invalidContext: secret key has too few rows")
+        out = np.empty(batch, dtype=np.float64)
+        _check(load_library().hecuda_bfv_noise_budget(context._h, _ptr(sk), _ptr(cts), polys, l, 1 if evalFormat else 0,
+                                                      _ptr(out), batch))
+        return float(out[0]) if single else out
+
     @staticmethod
     def decrypt(context: Context, ciphertexts, secretKey, scalingFactor: int = 1) -> np.ndarray:
         """Bfv.decryptCoeff (Bfv+Decrypt.swift:21-41): (batch, polys, l, N) Coeff ciphertexts -> (batch, N) coefficients < t.
-        secretKey: SecretKey.poly, (L+1, N) in Eval format."""
+        secretKey: a SecretKey, or SecretKey.poly, (L+1, N) in Eval format."""
         cts = _host(ciphertexts)
         if cts.ndim == 3:
             cts = cts[None]
         batch, polys, l, n = cts.shape
-        sk = _host(secretKey)
+        sk = _secret_poly(secretKey)
         if sk.size < l * n:
             raise HeError(-1, "invalidContext: secret key has too few rows")
         out = np.empty((batch, n), dtype=np.uint64)

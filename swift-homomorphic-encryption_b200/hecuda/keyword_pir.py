@@ -7,6 +7,8 @@ Names and argument meaning follow Sources/PrivateInformationRetrieval/KeywordPir
     KeywordDatabase, ShardingFunction, Sharding    KeywordDatabase.swift
     KeywordPirConfig, KeywordPirParameter          KeywordPirProtocol.swift:19-114
     KeywordPirServer.process / computeResponse     KeywordPirProtocol.swift:137-276
+    KeywordPirClient                               KeywordPirProtocol.swift:280-392
+    KeywordDatabase.validateShard                  KeywordDatabase.swift:557-630
 
 Keyword hashing, candidate indices and bucket serialization run on the device; the cuckoo placement runs on the host
 inside libhecuda (csrc/cuckoo.hpp) because the table depends on the order of its random draws.  The table's buckets
@@ -19,14 +21,15 @@ index, CuckooTable.insertLoop expands and drops the pair in hand; here that pair
 from __future__ import annotations
 
 import ctypes as C
+import struct
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from . import Context, EvaluationKey, _check, _ptr, load_library
-from .pir import IndexPirConfig, IndexPirParameter, MulPir, MulPirServer, PirError, PirKeyCompressionStrategy, PirWire, \
-    ProcessedDatabase, bytesPerPlaintext
+from . import Context, EvaluationKey, SecretKey, _check, _ptr, load_library
+from .pir import IndexPirConfig, IndexPirParameter, MulPir, MulPirClient, MulPirServer, PirError, PirKeyCompressionStrategy, \
+    PirWire, ProcessedDatabase, ShardValidationResult, _validate, bytesPerPlaintext
 
 MAX_SLOT_COUNT = 255  # HashBucket.maxSlotCount
 RNG_COUNTER, RNG_SPLITMIX64 = 0, 1  # HECUDA_CUCKOO_RNG_*
@@ -84,6 +87,39 @@ class HashKeyword:
         """HashKeyword.hashIndices (HashBucket.swift:221-235) of one keyword."""
         return [int(i) for i in HashKeyword.hashIndicesOfHashes(HashKeyword.hashes([keyword]), bucketCount,
                                                                  hashFunctionCount)[0]]
+
+
+class HashBucket:
+    """HashBucket (HashBucket.swift): a serialized bucket is a slot count, then per slot the keyword hash (UInt64), the
+    value length (UInt16), both little-endian, and the value."""
+
+    @staticmethod
+    def deserialize(raw: bytes) -> List[Tuple[int, bytes]]:
+        """HashBucket(deserialize:) -> [(keyword hash, value)]; PirError("corruptedData...") on a short buffer."""
+        if not raw:
+            raise PirError("corruptedData: Serialized HashBucket shouldn't be empty.")
+        count, offset, slots = raw[0], 1, []
+        for _ in range(count):
+            if len(raw) < offset + 10:
+                raise PirError("corruptedData: Serialized HashBucketEntry should at least have a keyword hash and a value size.")
+            keyword_hash, size = struct.unpack_from("<QH", raw, offset)
+            offset += 10
+            if offset + size > len(raw):
+                raise PirError("corruptedData: HashBucketEntry buffer has less data than expected")
+            slots.append((keyword_hash, bytes(raw[offset:offset + size])))
+            offset += size
+        return slots
+
+    @staticmethod
+    def serializedSize(slots: Sequence[Tuple[int, bytes]]) -> int:
+        return 1 + sum(10 + len(value) for _, value in slots)
+
+    @staticmethod
+    def find(slots: Sequence[Tuple[int, bytes]], keywordHash: int) -> Optional[bytes]:
+        for slot_hash, value in slots:
+            if slot_hash == keywordHash:
+                return value
+        return None
 
 
 # ------------------------------------------------------------------------------------------------ cuckoo table
@@ -344,6 +380,51 @@ class ProcessedKeywordDatabase:
         self.table.close()
 
 
+class KeywordPirClient:
+    """KeywordPirClient<MulPirClient> (KeywordPirProtocol.swift:280-392), on the device."""
+
+    def __init__(self, keywordParameter: KeywordPirParameter, pirParameter: IndexPirParameter, context: Context):
+        self.keywordParameter, self.context = keywordParameter, context
+        self.indexPirClient = MulPirClient(pirParameter, context)
+
+    def _indices(self, keyword: bytes) -> List[int]:
+        return HashKeyword.hashIndices(bytes(keyword), self.indexPirClient.parameter.entryCount,
+                                       self.keywordParameter.hashFunctionCount)
+
+    def generateEvaluationKey(self, secretKey: SecretKey) -> EvaluationKey:
+        return self.indexPirClient.generateEvaluationKey(secretKey)
+
+    def generateQuery(self, keyword: bytes, secretKey: SecretKey) -> np.ndarray:
+        """KeywordPirClient.generateQuery (:326-334): an index query at the keyword's hashIndices, one per table."""
+        return self.indexPirClient.generateQuery(self._indices(keyword), secretKey)
+
+    def decrypt(self, response, keyword: bytes, secretKey: SecretKey) -> Optional[bytes]:
+        """KeywordPirClient.decrypt (:343-359): the value stored with the keyword in one of its buckets, or None."""
+        keyword_hash = int(HashKeyword.hashes([bytes(keyword)])[0])
+        for raw in self.indexPirClient.decrypt(response, self._indices(keyword), secretKey):
+            value = HashBucket.find(HashBucket.deserialize(raw), keyword_hash)
+            if value is not None:
+                return value
+        return None
+
+    def countEntriesInResponse(self, response, secretKey: SecretKey) -> int:
+        """KeywordPirClient.countEntriesInResponse (:376-391): the slots of every bucket found in the replies' bytes."""
+        found = 0
+        for data in self.indexPirClient.decryptFull(response, secretKey):
+            offset = 0
+            while offset < len(data):
+                try:
+                    slots = HashBucket.deserialize(data[offset:])
+                except PirError:
+                    break
+                found += len(slots)
+                offset += HashBucket.serializedSize(slots)
+        return found
+
+    def noiseBudget(self, response, secretKey: SecretKey) -> float:
+        return self.indexPirClient.noiseBudget(response, secretKey)
+
+
 class KeywordPirServer:
     """KeywordPirServer<MulPirServer> (KeywordPirProtocol.swift:137-276)."""
 
@@ -400,3 +481,11 @@ class KeywordPirServer:
     def computeResponsesWire(self, queryPoly0, querySeeds, evaluationKeys: Sequence[EvaluationKey]):
         return PirWire.computeResponses(self.indexPirServer, queryPoly0, querySeeds, evaluationKeys, self.hashFunctionCount)
 
+    def validate(self, row: KeywordValuePair, trials: int = 1) -> ShardValidationResult:
+        """KeywordDatabase.validateShard (KeywordDatabase.swift:557-630): row = (keyword, value).  Every step runs on the
+        device; raises PirError("Insufficient noise budget") or PirError("Incorrect PIR response") when a trial's reply
+        does not decrypt to the value."""
+        keyword, value = bytes(row[0]), bytes(row[1])
+        client = KeywordPirClient(self.processed.keywordPirParameter, self.indexPirParameter, self.context)
+        return _validate(trials, client, self.computeResponse, lambda sk: client.generateQuery(keyword, sk),
+                         lambda response, sk: client.decrypt(response, keyword, sk), value, client.countEntriesInResponse)

@@ -8,20 +8,25 @@ Names and argument meaning follow Sources/PrivateInformationRetrieval/IndexPir:
     MulPirServer.process / computeResponse       MulPir.swift:412-556, PirUtil.swift:490-568
     PirUtil.expand                               PirUtil.swift:321-355
 
-Only the server side lives here (the client's encrypt / decrypt are SURVEY.md 8f rank 4).  The database stays resident in
-HBM (`ProcessedDatabase`); `computeResponse` is one C-ABI call per query.  No CPU fallback: everything that touches
-ciphertexts or plaintext polynomials runs in libhecuda.
+    MulPirClient                                 MulPir.swift:119-290, PirUtil.swift:361-404
+    ProcessedDatabaseWithParameters.validate     IndexPirProtocol.swift:420-484
+
+The database stays resident in HBM (`ProcessedDatabase`); `computeResponse` is one C-ABI call per query.  The client
+(key generation, query encryption, decryption, noise budgets) runs on the device too, so a processed database can be
+validated the way the reference's PIRProcessDatabase does.  No CPU fallback: everything that touches ciphertexts or
+plaintext polynomials runs in libhecuda.
 """
 from __future__ import annotations
 
 import ctypes as C
+import time
 from dataclasses import dataclass, field
 from enum import Enum
-from typing import List, Optional, Sequence
+from typing import Any, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import Context, EvaluationKey, HeError, _check, _host, _ptr, load_library
+from . import Bfv, Context, EvaluationKey, HeError, SecretKey, _check, _host, _ptr, load_library
 
 
 class PirKeyCompressionStrategy(str, Enum):
@@ -380,6 +385,143 @@ class PirUtil:
         return out
 
 
+class MulPirClient:
+    """MulPirClient<PirUtil<Bfv<UInt64>>> (MulPir.swift:119-290): evaluation keys, queries and reply decryption, on the
+    device."""
+
+    def __init__(self, parameter: IndexPirParameter, context: Context):
+        self.parameter, self.context = parameter, context
+
+    @property
+    def evaluationKeyConfig(self) -> EvaluationKeyConfig:
+        return self.parameter.evaluationKeyConfig
+
+    @property
+    def entryChunksPerPlaintext(self) -> int:
+        per_plaintext, encoded = bytesPerPlaintext(self.context), self.parameter.encodedEntrySize
+        return per_plaintext // encoded if per_plaintext >= encoded else 1
+
+    def generateEvaluationKey(self, secretKey: SecretKey) -> EvaluationKey:
+        """MulPirClient.generateEvaluationKey (MulPir.swift:171-174)."""
+        return EvaluationKey.generate(self.context, self.evaluationKeyConfig, secretKey)
+
+    def computeCoordinates(self, index: int) -> List[int]:
+        """MulPirClient.computeCoordinates (MulPir.swift:181-193)."""
+        if not 0 <= index < self.parameter.entryCount:
+            raise PirError(f"invalidIndex(index: {index}, numberOfEntries: {self.parameter.entryCount})")
+        plaintext_index = index // self.entryChunksPerPlaintext
+        product = int(np.prod(self.parameter.dimensions, dtype=np.int64))
+        coordinates = []
+        for size in self.parameter.dimensions:
+            product //= size
+            coordinate = plaintext_index // product
+            plaintext_index -= coordinate * product
+            coordinates.append(coordinate)
+        return coordinates
+
+    def generateQuery(self, indices: Sequence[int], secretKey: SecretKey) -> np.ndarray:
+        """MulPirClient.generateQuery (MulPir.swift:201-218) with PirUtil.compressBinaryInputs (PirUtil.swift:361-404):
+        Query.ciphertexts as (count, 2, L, N) Coeff."""
+        ctx, dims = self.context, self.parameter.dimensions
+        accumulated, positions = 0, []
+        for index in indices:
+            coordinates = self.computeCoordinates(int(index))
+            for dim, size in enumerate(dims):
+                positions.append(accumulated + coordinates[dim])
+                accumulated += size
+        t, n = ctx.plaintextModulus, ctx.degree
+        remaining, processed, plaintexts = self.parameter.expandedQueryCount * len(indices), 0, []
+        while remaining > 0:
+            count = min(remaining, n)
+            raw = np.zeros(n, dtype=np.uint64)  # compressInputsForOneCiphertext: 2^-ceilLog2(count) mod t at the positions
+            inverse = pow(pow(2, _ceil_log2(count), t), -1, t)
+            for position in positions:
+                if processed <= position < processed + count:
+                    raw[position - processed] = inverse
+            plaintexts.append(raw)
+            processed += count
+            remaining -= count
+        return Bfv.encrypt(ctx, secretKey, np.stack(plaintexts))
+
+    def decryptFull(self, response, secretKey: SecretKey) -> List[bytes]:
+        """MulPirClient.decryptFull: every reply's bytes.  response: (replies, chunkCount, 2, 1, N)."""
+        ctx = self.context
+        cts = _host(response)
+        replies = cts.shape[0]
+        plain = Bfv.decrypt(ctx, cts.reshape(-1, 2, cts.shape[-2], ctx.degree), secretKey).reshape(replies, -1, ctx.degree)
+        bits = ctx.plaintextModulus.bit_length() - 1
+        return [b"".join(CoefficientPacking.coefficientsToBytes(p, bits) for p in reply) for reply in plain]
+
+    def decrypt(self, response, indices: Sequence[int], secretKey: SecretKey) -> List[bytes]:
+        """MulPirClient.decrypt (MulPir.swift:245-275): decrypt, coefficient decode, bytes, the entry's range and its
+        entry-size prefix."""
+        cts = _host(response)
+        if cts.shape[0] != len(indices):
+            raise PirError(f"invalidResponse(replyCount: {cts.shape[0]}, expected: {len(indices)})")
+        encoded, width = self.parameter.encodedEntrySize, self.parameter.entrySizeEncodingWidth
+        out = []
+        for data, index in zip(self.decryptFull(cts, secretKey), indices):
+            position = int(index) % self.entryChunksPerPlaintext
+            entry = data[position * encoded:(position + 1) * encoded]
+            if self.parameter.encodingEntrySize:
+                entry = entry[width:][:int.from_bytes(entry[:width], "little")]
+            out.append(entry)
+        return out
+
+    def noiseBudget(self, response, secretKey: SecretKey) -> float:
+        """Response.noiseBudget(using:variableTime:) (IndexPirProtocol.swift:742-747): the least budget of its ciphertexts.
+        Must not be shared with another party."""
+        cts = _host(response)
+        if cts.size == 0:
+            return -float("inf")
+        return float(np.min(Bfv.noiseBudget(self.context, secretKey, cts.reshape(-1, 2, cts.shape[-2], self.context.degree))))
+
+
+@dataclass
+class ShardValidationResult:
+    """ShardValidationResult (IndexPirProtocol.swift): the first trial's key and query, the last response, the least
+    noise budget over the trials, each trial's response time (seconds) and entries per response."""
+
+    evaluationKey: Any
+    query: Any
+    response: np.ndarray
+    noiseBudget: float
+    computeTimes: List[float]
+    entryCountPerResponse: List[int]
+    decryptedRow: Optional[bytes] = None  # the last trial's decrypted value (equal to the row's)
+
+
+def _validate(trials: int, client, server_response, generate_query, decrypt, value: bytes, count_entries) -> ShardValidationResult:
+    """The trial loop shared by the index and keyword validations (IndexPirProtocol.swift:420-484,
+    KeywordDatabase.swift:557-630): a fresh secret key, evaluation key and query per trial, the response timed, its noise
+    budget, and its decryption compared with the row."""
+    if trials <= 0:
+        raise PirError(f"Invalid trialsPerShard: {trials}")
+    ctx = client.context
+    first_key = first_query = response = None
+    min_budget, times, counts = float("inf"), [], []
+    for trial in range(trials):
+        secret_key = SecretKey.generate(ctx)
+        key = client.generateEvaluationKey(secret_key)
+        query = generate_query(secret_key)
+        start = time.perf_counter()
+        response = server_response(query, key)
+        times.append(time.perf_counter() - start)
+        budget = client.noiseBudget(response, secret_key)
+        min_budget = min(min_budget, budget)
+        decrypted = decrypt(response, secret_key)
+        if decrypted != value:
+            if budget < Bfv.minNoiseBudget:
+                raise PirError("Insufficient noise budget")
+            raise PirError("Incorrect PIR response")
+        counts.append(count_entries(response, secret_key))
+        if trial == 0:
+            first_key, first_query = key, query
+        else:
+            key.close()
+    return ShardValidationResult(first_key, first_query, response, min_budget, times, counts, decrypted)
+
+
 class MulPirServer:
     """MulPirServer<PirUtil<Bfv<UInt64>>> (MulPir.swift:292-426)."""
 
@@ -491,3 +633,13 @@ class MulPirServer:
             ctx._h, key_handles, len(keys), handles, len(self.databases), dims, len(self.parameter.dimensions),
             self.chunkCount, _ptr(cts), cts.size // (words * len(keys)), indicesCount, _ptr(out)))
         return out
+
+    def validate(self, row: Tuple[int, bytes], trials: int = 1) -> ShardValidationResult:
+        """ProcessedDatabaseWithParameters.validate(row:trials:) (IndexPirProtocol.swift:420-484) against the first
+        database: row = (index, value).  Every step runs on the device; raises PirError("Insufficient noise budget") or
+        PirError("Incorrect PIR response") when a trial's reply does not decrypt to the value."""
+        index, value = int(row[0]), bytes(row[1])
+        client = MulPirClient(self.parameter, self.context)
+        return _validate(trials, client, lambda query, key: self.computeResponse(query, key),
+                         lambda sk: client.generateQuery([index], sk),
+                         lambda response, sk: client.decrypt(response, [index], sk)[0], value, lambda response, sk: 1)
