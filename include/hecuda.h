@@ -713,6 +713,52 @@ int32_t hecuda_evk_generate(const hecuda_context *ctx, const uint64_t *secret_ke
 int32_t hecuda_bfv_noise_budget(const hecuda_context *ctx, const uint64_t *secret_key, const uint64_t *ciphertexts,
                                 int32_t poly_count, int32_t moduli_count, int32_t eval_format, double *budgets, int64_t batch);
 
+/* hecuda_evk_copy: a device-to-device copy of `evk` (its relinearization key and every Galois key) owned by `ctx`, as
+ * the reference uses one evaluation key generated on contexts[0] with every plaintext modulus (PrivateNearestNeighborSearch/
+ * Client.swift:137-146: BFV keys do not depend on t).  Refused (HECUDA_ERR_INVALID_ARGUMENT) unless N, the word size
+ * and the coefficient moduli, in order and including the key-switching modulus, are identical.  The copy is
+ * independent of `evk` (either may be destroyed first).  On error *out is NULL and nothing is launched. */
+int32_t hecuda_evk_copy(const hecuda_evk *evk, const hecuda_context *ctx, hecuda_evk **out);
+
+/* ---- PNNS client and float database processing (uint64_t only) ----
+ * Array2d.normalizedScaledAndRounded (PrivateNearestNeighborSearch/Util.swift:74-89) in Swift Float arithmetic: per
+ * row, the squares summed left to right in float32, a correctly rounded square root, then for each value
+ * (value * Float(scaling_factor)) / norm rounded twice and .toNearestOrAwayFromZero into Int64; a zero-norm row is 0.
+ * Every operation is rounded on its own (no FMA contraction).  Where Swift traps -- a non-finite input, a value outside
+ * Int64, or (without reduce) outside [-floor(t/2), floor((t-1)/2)] -- the call returns HECUDA_ERR_INVALID_ARGUMENT.
+ *
+ * hecuda_pnns_matrices_create_from_vectors = Database.process (ProcessedDatabase.swift:194-229) for the .diagonal
+ * packing: vectors row_count x column_count floats, row-major; one matrix per context (ctxs[0 .. plaintext_count), all
+ * with the same N), each the handle hecuda_pnns_matrix_create_from_values builds from the normalised values with
+ * reduce = (plaintext_count > 1) (:213-214).  The floats cross PCIe once and are normalised once.  On error every out[k]
+ * is NULL and nothing stays allocated.
+ *
+ * hecuda_pnns_query_generate = Client.generateQuery for one context (Client.swift:73-91): normalise, pack .denseRow
+ * (PlaintextMatrix.swift:341-413) into ceil(rows / (N / nextPow2(cols))) SIMD plaintexts, encode, encrypt
+ * (hecuda_bfv_encrypt: secret_key K x N Eval, a_seeds / error_seeds one 32-byte seed per ciphertext), all on the device.
+ * reduce: Modulus.reduce instead of centeredToRemainder (the reference reduces when there are several plaintext
+ * moduli).  Exactly one of ciphertexts (count x 2 x L x N, Coeff) and poly0 (count x byteCount(L rows), the
+ * .seeded(poly0:seed: a_seeds[i]) wire form) is non-null.  A non-finite input, column_count outside 1 .. N/2, or a
+ * scaling factor whose values cannot fit the plaintext map is refused before anything is launched.
+ *
+ * hecuda_pnns_decrypt_distances = Client.decrypt (Client.swift:99-127): replies[k] is the .denseColumn response matrix of
+ * context k (reply_count x 2 x moduli_count x N, Coeff; reply_count as the reference packs matrix_rows x query_rows
+ * values).  Per context: the decryption dot product and scale-and-round (hecuda_bfv_decrypt), SIMD decode; then one
+ * kernel: unpackDenseColumn (PlaintextMatrix.swift:515-555), CrtComposer.compose (CrtComposer.swift:76-97),
+ * remainderToCentered over prod t and Float(signed) / (Float(s) * Float(s)).  distances: matrix_rows x query_rows float,
+ * row-major (MatrixMultiplication.swift:291-293).  The contexts must differ only in t; refused: 2 prod t above UInt64.max
+ * with several moduli (composeMaxIntermediateValue), plaintext moduli that are not pairwise distinct, more than 8
+ * contexts.  The device copy of the secret key is zeroized before it is freed. */
+int32_t hecuda_pnns_matrices_create_from_vectors(const hecuda_context *const *ctxs, int32_t plaintext_count, const float *vectors,
+                                                 int64_t row_count, int64_t column_count, int64_t scaling_factor,
+                                                 int32_t baby_step, int32_t giant_step, hecuda_pnns_matrix **out);
+int32_t hecuda_pnns_query_generate(const hecuda_context *ctx, const uint64_t *secret_key, const float *vectors, int64_t row_count,
+                                   int64_t column_count, int64_t scaling_factor, int32_t reduce, const uint8_t *a_seeds,
+                                   const uint8_t *error_seeds, uint64_t *ciphertexts, uint8_t *poly0);
+int32_t hecuda_pnns_decrypt_distances(const hecuda_context *const *ctxs, int32_t plaintext_count, const uint64_t *secret_key,
+                                      const uint64_t *const *replies, int64_t reply_count, int32_t moduli_count,
+                                      int64_t matrix_rows, int64_t query_rows, int64_t scaling_factor, float *distances);
+
 /* Bookkeeping for bench.py: number of kernel launches issued by this library in the calling process so far. */
 uint64_t hecuda_kernel_launch_count(void);
 

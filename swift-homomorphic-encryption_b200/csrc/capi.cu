@@ -679,6 +679,40 @@ int32_t hecuda_evk_destroy(hecuda_evk *k) {
     delete k;
     return HECUDA_OK;
 }
+int32_t hecuda_evk_copy(const hecuda_evk *key, const hecuda_context *h, hecuda_evk **out) {
+    if (!out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (!key || !key->owner) return fail(HECUDA_ERR_MISSING_KEY, "null evaluation key");
+    const Context &a = *key->owner->ctx, &b = *h->ctx;
+    // BFV keys do not depend on t: the key is valid wherever N, the word size and every coefficient modulus agree
+    if (a.n != b.n || a.word_bits != b.word_bits || a.q != b.q || a.q_ks != b.q_ks)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidContext: the key's context differs in N, word size or coefficient moduli");
+    hecuda_evk *k = nullptr;
+    if ((rc = hecuda_evk_create_empty(h, &k))) return rc;
+    hecuda_evk *src = const_cast<hecuda_evk *>(key);
+    cudaError_t e;
+    {
+        std::lock_guard<std::mutex> lock(src->mu);
+        e = cudaMemcpy(k->d_relin, src->d_relin, k->words * sizeof(u64), cudaMemcpyDeviceToDevice);
+        for (auto it = src->galois.begin(); e == cudaSuccess && it != src->galois.end(); ++it) {
+            u64 *d = nullptr;
+            if ((e = cudaMalloc(&d, k->words * sizeof(u64))) != cudaSuccess) break;
+            k->galois[it->first] = d;
+            e = cudaMemcpy(d, it->second, k->words * sizeof(u64), cudaMemcpyDeviceToDevice);
+        }
+        k->loaded = src->loaded;
+    }
+    // the copy is read on other non-blocking streams: publish it once the legacy-stream copies are done (see upload())
+    if (e == cudaSuccess) e = cudaStreamSynchronize(cudaStreamLegacy);
+    if (e != cudaSuccess) {
+        hecuda_evk_destroy(k);
+        return cuda_fail(e, "evk_copy");
+    }
+    *out = k;
+    return HECUDA_OK;
+}
 int32_t hecuda_evk_device_buffer(hecuda_evk *k, void **device_ptr, uint64_t *bytes) {
     if (!k || !device_ptr || !bytes) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
     *device_ptr = k->d_relin;

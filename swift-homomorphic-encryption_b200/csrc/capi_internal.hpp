@@ -179,5 +179,21 @@ int32_t pir_databases_from_device_entries(const hecuda_context *h, const unsigne
                                           const uint64_t *d_offsets, int64_t per_table, int tables, int64_t entry_size,
                                           const int32_t *dims, int32_t dim_count, hecuda_pir_database **out);
 
+// Bfv.encrypt of `batch` plaintexts already on the device (client.cu): d_sk L x N (Eval), d_pt batch x N (< t), seeds
+// batch x 32 each -> d_c0 batch x L x N (Coeff) and d_c1 = d_c0 + batch x L x N (Coeff with c1_coeff, else Eval)
+cudaError_t encrypt_plaintexts_device(const Context &c, const u64 *d_sk, const u64 *d_pt, const unsigned char *d_a_seeds,
+                                      const unsigned char *d_e_seeds, u64 *d_c0, u64 *d_c1, bool c1_coeff, int64_t batch,
+                                      cudaStream_t s);
+// Bfv.decryptCoeff of `items` ciphertexts of polys x l x N on the device (decrypt.cu) -> out items x N (< t); scratch:
+// decrypt_scratch_words per item
+size_t decrypt_scratch_words(const Context &c, int polys, int l);
+cudaError_t decrypt_device(const Context &c, const u64 *d_sk, const u64 *d_ct, int polys, int l, u64 *scratch, u64 *out,
+                           int64_t items, cudaStream_t s);
+// The host-side refusals of a float front end (pnns_client.cu): a null or non-finite vector value, a negative scaling
+// factor, or one whose scaled values cannot fit the plaintext map (Int64 with `reduce`, else the centred range mod t).
+// scan: look for non-finite values on the host (else the device's normalisation flags them)
+int32_t check_float_vectors(const float *vectors, int64_t rows, int64_t cols, int64_t scaling_factor, u64 t, bool reduce,
+                            bool scan);
+
 }  // namespace api
 }  // namespace hecuda

@@ -349,6 +349,18 @@ int32_t encrypt(const hecuda_context *h, const uint64_t *sk, const uint64_t *pt,
 
 }  // namespace
 
+namespace hecuda {
+namespace api {
+
+cudaError_t encrypt_plaintexts_device(const Context &c, const u64 *d_sk, const u64 *d_pt, const unsigned char *d_a_seeds,
+                                      const unsigned char *d_e_seeds, u64 *d_c0, u64 *d_c1, bool c1_coeff, int64_t batch,
+                                      cudaStream_t s) {
+    return encrypt_device(c, d_sk, d_pt, d_a_seeds, d_e_seeds, d_c0, d_c1, c1_coeff, batch, s);
+}
+
+}  // namespace api
+}  // namespace hecuda
+
 extern "C" {
 
 int32_t hecuda_bfv_generate_secret_key(const hecuda_context *h, const uint8_t *seeds, uint64_t *secret_keys, int64_t count) {

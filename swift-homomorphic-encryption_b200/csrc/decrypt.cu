@@ -251,6 +251,19 @@ std::vector<u64> noise_big_constants(const u64 *q, int l) {
 
 }  // namespace
 
+namespace hecuda {
+namespace api {
+
+size_t decrypt_scratch_words(const Context &c, int polys, int l) { return ((size_t)polys * l + l) * c.n; }
+
+cudaError_t decrypt_device(const Context &c, const u64 *d_sk, const u64 *d_ct, int polys, int l, u64 *scratch, u64 *out,
+                           int64_t items, cudaStream_t s) {
+    return decrypt_chunk(c, make_consts(c, l, 1), scratch, d_sk, d_ct, polys, out, items, s);
+}
+
+}  // namespace api
+}  // namespace hecuda
+
 extern "C" {
 
 int32_t hecuda_bfv_decrypt(const hecuda_context *h, const uint64_t *secret_key, const uint64_t *ciphertexts, int32_t polys,

@@ -177,6 +177,11 @@ cudaError_t launch_pir_pack(const procdb::PirShape &s, int n, int64_t first, int
 cudaError_t launch_pnns_diagonal(const Context &ctx, const procdb::PnnsShape &s, const int64_t *values, bool reduce,
                                  bool resident, int64_t first, int64_t items, u64 *out, int *bad, cudaStream_t stream);
 
+// Array2d.normalizedScaledAndRounded (pnns_client.cu): vectors rows x cols floats (on the device) -> norms[rows] and
+// values rows x cols Int64 (0 for a zero-norm row); a non-finite input or a value outside Int64 sets *bad
+cudaError_t launch_pnns_normalize(const float *vectors, int64_t rows, int64_t cols, int64_t scaling_factor, float *norms,
+                                  int64_t *values, int *bad, cudaStream_t stream);
+
 // divideAndRoundQLast over polys x l x N -> polys x (l-1) x N
 cudaError_t launch_mod_switch(const Context &ctx, const u64 *in, int l, u64 *out, int64_t polys, cudaStream_t stream);
 

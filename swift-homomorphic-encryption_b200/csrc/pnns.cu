@@ -605,21 +605,17 @@ int32_t check_steps(const Context &c, int64_t dimension, int32_t baby_step, int3
 }
 
 // PlaintextMatrix.init(signedValues:) + diagonalPlaintexts (PlaintextMatrix.swift:155-190, 417-482) on the default
-// stream: uploads the row-major values once, then SIMD-encodes `count` plaintexts slab by slab (in slot order when
+// stream from row-major values already on the device: SIMD-encodes `count` plaintexts slab by slab (in slot order when
 // `resident`), handing each slab's coefficients to sink(first, items, d_coeff).  Frees its buffers before it returns;
 // HECUDA_ERR_INVALID_ARGUMENT when a value is outside centeredToRemainder's range and `reduce` is off.
 template <class Sink>
-int32_t pnns_encode_slabs(const Context &c, const procdb::PnnsShape &shape, const int64_t *values, bool reduce,
+int32_t pnns_encode_slabs(const Context &c, const procdb::PnnsShape &shape, const int64_t *d_values, bool reduce,
                           bool resident, int64_t count, Sink sink) {
-    const size_t value_bytes = (size_t)shape.rows * shape.cols * sizeof(int64_t);
     const int64_t slab = coefficient_slab(c);
-    int64_t *d_values = nullptr;
     int *d_bad = nullptr;
     u64 *d_coeff = nullptr;
     int bad = 0;
-    cudaError_t e = cudaMalloc(&d_values, value_bytes);
-    if (e == cudaSuccess) e = upload(d_values, values, value_bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&d_bad, sizeof(int));
+    cudaError_t e = cudaMalloc(&d_bad, sizeof(int));
     if (e == cudaSuccess) e = fill(d_bad, 0, sizeof(int));
     if (e == cudaSuccess) e = cudaMalloc(&d_coeff, (size_t)std::min(slab, count) * c.n * sizeof(u64));
     for (int64_t done = 0; e == cudaSuccess && done < count; done += slab) {
@@ -630,10 +626,69 @@ int32_t pnns_encode_slabs(const Context &c, const procdb::PnnsShape &shape, cons
     if (e == cudaSuccess) e = cudaMemcpy(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost);
     cudaFree(d_coeff);
     cudaFree(d_bad);
-    cudaFree(d_values);
     if (e != cudaSuccess) return cuda_fail(e, "pnns diagonal packing");
     if (bad)  // Scalar.centeredToRemainder's precondition (Scalar.swift:85-87)
         return fail(HECUDA_ERR_INVALID_ARGUMENT, "signed value outside [-floor(t/2), floor((t-1)/2)]; pass reduce to reduce mod t");
+    return HECUDA_OK;
+}
+
+// pnns_encode_slabs from host values: uploads them once
+template <class Sink>
+int32_t pnns_encode_slabs_host(const Context &c, const procdb::PnnsShape &shape, const int64_t *values, bool reduce,
+                               bool resident, int64_t count, Sink sink) {
+    const size_t value_bytes = (size_t)shape.rows * shape.cols * sizeof(int64_t);
+    int64_t *d_values = nullptr;
+    cudaError_t e = cudaMalloc(&d_values, value_bytes);
+    if (e == cudaSuccess) e = upload(d_values, values, value_bytes);
+    if (e != cudaSuccess) {
+        cudaFree(d_values);
+        return cuda_fail(e, "pnns diagonal packing");
+    }
+    const int32_t rc = pnns_encode_slabs(c, shape, d_values, reduce, resident, count, sink);
+    cudaFree(d_values);
+    return rc;
+}
+
+// The resident matrix of hecuda_pnns_matrix_create_from_values from row-major signed values on the device; the shape
+// has passed check_values.  On error *out stays NULL and nothing stays allocated.
+int32_t matrix_from_device_values(const hecuda_context *h, const procdb::PnnsShape &shape, const int64_t *d_values,
+                                  bool reduce, hecuda_pnns_matrix **out) {
+    const Context &c = *h->ctx;
+    const size_t row_words = (size_t)c.L * c.n;
+    const int32_t baby_step = shape.baby, giant_step = shape.giant;
+    const int64_t slots = shape.results * giant_step * baby_step;
+    hecuda_pnns_matrix *m = new (std::nothrow) hecuda_pnns_matrix();
+    if (!m) return fail(HECUDA_ERR_CUDA, "out of host memory");
+    m->owner = h;
+    m->row_count = shape.rows;
+    m->column_count = shape.cols;
+    m->result_count = shape.results;
+    m->baby = baby_step;
+    m->giant = giant_step;
+    m->dimension = shape.dimension;
+    // slot (r, g, j) holds diagonal baby * g + j of chunk r; slots past the padded dimension are absent (all zero)
+    std::vector<unsigned char> present((size_t)slots, 0);
+    for (int64_t slot = 0; slot < slots; ++slot) present[(size_t)slot] = slot % ((int64_t)giant_step * baby_step) < shape.dimension;
+    cudaError_t e = cudaMalloc(&m->d_plain, row_words * slots * sizeof(u64));
+    if (e == cudaSuccess) e = cudaMalloc(&m->d_present, (size_t)slots);
+    if (e == cudaSuccess) e = upload(m->d_present, present.data(), (size_t)slots);
+    if (e != cudaSuccess) {
+        hecuda_pnns_matrix_destroy(m);
+        return cuda_fail(e, "pnns matrix from values");
+    }
+    // Plaintext.convertToEvalFormat (MatrixMultiplication.swift:206-208), one slab of slots at a time
+    int32_t rc = pnns_encode_slabs(c, shape, d_values, reduce, true, slots, [&](int64_t first, int64_t items, const u64 *d) {
+        return launch_plaintext_to_eval(c, d, c.L, m->d_plain + row_words * first, items, nullptr);
+    });
+    if (rc == HECUDA_OK) {
+        e = cudaStreamSynchronize(nullptr);
+        if (e != cudaSuccess) rc = cuda_fail(e, "pnns matrix from values");
+    }
+    if (rc) {
+        hecuda_pnns_matrix_destroy(m);
+        return rc;
+    }
+    *out = m;
     return HECUDA_OK;
 }
 
@@ -669,7 +724,7 @@ int32_t hecuda_pnns_diagonal_plaintexts(const hecuda_context *h, const int64_t *
     if (rc) return rc;
     if (!out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
     const Context &c = *h->ctx;
-    return pnns_encode_slabs(c, shape, values, reduce != 0, false, (int64_t)shape.dimension * shape.results,
+    return pnns_encode_slabs_host(c, shape, values, reduce != 0, false, (int64_t)shape.dimension * shape.results,
                              [&](int64_t first, int64_t items, const u64 *d) {
                                  return cudaMemcpy(out + (size_t)first * c.n, d, (size_t)items * c.n * sizeof(u64),
                                                    cudaMemcpyDeviceToHost);
@@ -684,42 +739,62 @@ int32_t hecuda_pnns_matrix_create_from_values(const hecuda_context *h, const int
     procdb::PnnsShape shape;
     int32_t rc = check_values(h, values, row_count, column_count, baby_step, giant_step, true, shape);
     if (rc) return rc;
-    const Context &c = *h->ctx;
-    const size_t row_words = (size_t)c.L * c.n;
-    const int64_t slots = shape.results * giant_step * baby_step;
-    hecuda_pnns_matrix *m = new (std::nothrow) hecuda_pnns_matrix();
-    if (!m) return fail(HECUDA_ERR_CUDA, "out of host memory");
-    m->owner = h;
-    m->row_count = row_count;
-    m->column_count = column_count;
-    m->result_count = shape.results;
-    m->baby = baby_step;
-    m->giant = giant_step;
-    m->dimension = shape.dimension;
-    // slot (r, g, j) holds diagonal baby * g + j of chunk r; slots past the padded dimension are absent (all zero)
-    std::vector<unsigned char> present((size_t)slots, 0);
-    for (int64_t slot = 0; slot < slots; ++slot) present[(size_t)slot] = slot % ((int64_t)giant_step * baby_step) < shape.dimension;
-    cudaError_t e = cudaMalloc(&m->d_plain, row_words * slots * sizeof(u64));
-    if (e == cudaSuccess) e = cudaMalloc(&m->d_present, (size_t)slots);
-    if (e == cudaSuccess) e = upload(m->d_present, present.data(), (size_t)slots);
-    if (e != cudaSuccess) {
-        hecuda_pnns_matrix_destroy(m);
-        return cuda_fail(e, "pnns matrix from values");
+    const size_t value_bytes = (size_t)row_count * column_count * sizeof(int64_t);
+    int64_t *d_values = nullptr;
+    cudaError_t e = cudaMalloc(&d_values, value_bytes);
+    if (e == cudaSuccess) e = upload(d_values, values, value_bytes);
+    rc = e == cudaSuccess ? matrix_from_device_values(h, shape, d_values, reduce != 0, out) : cuda_fail(e, "pnns matrix from values");
+    cudaFree(d_values);
+    return rc;
+}
+
+int32_t hecuda_pnns_matrices_create_from_vectors(const hecuda_context *const *ctxs, int32_t plaintext_count, const float *vectors,
+                                                 int64_t row_count, int64_t column_count, int64_t scaling_factor,
+                                                 int32_t baby_step, int32_t giant_step, hecuda_pnns_matrix **out) {
+    if (!out || !ctxs || plaintext_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument or no context");
+    for (int32_t k = 0; k < plaintext_count; ++k) out[k] = nullptr;
+    // For a single plaintext modulus, reduction isn't necessary (ProcessedDatabase.swift:213-214)
+    const bool reduce = plaintext_count > 1;
+    std::vector<procdb::PnnsShape> shapes((size_t)plaintext_count);
+    int32_t rc;
+    for (int32_t k = 0; k < plaintext_count; ++k) {
+        // check_values only needs a non-null values pointer here; the float vectors stand in for it
+        if ((rc = check_values(ctxs[k], (const int64_t *)(const void *)vectors, row_count, column_count, baby_step, giant_step,
+                               true, shapes[(size_t)k])))
+            return rc;
+        if (ctxs[k]->ctx->n != ctxs[0]->ctx->n)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongEncryptionParameters: the contexts differ in N");
+        if ((rc = check_float_vectors(vectors, row_count, column_count, scaling_factor, ctxs[k]->ctx->t, reduce, false))) return rc;
     }
-    // Plaintext.convertToEvalFormat (MatrixMultiplication.swift:206-208), one slab of slots at a time
-    rc = pnns_encode_slabs(c, shape, values, reduce != 0, true, slots, [&](int64_t first, int64_t items, const u64 *d) {
-        return launch_plaintext_to_eval(c, d, c.L, m->d_plain + row_words * first, items, nullptr);
-    });
-    if (rc == HECUDA_OK) {
-        e = cudaStreamSynchronize(nullptr);
-        if (e != cudaSuccess) rc = cuda_fail(e, "pnns matrix from values");
-    }
-    if (rc) {
-        hecuda_pnns_matrix_destroy(m);
-        return rc;
-    }
-    *out = m;
-    return HECUDA_OK;
+    const size_t values = (size_t)row_count * column_count;
+    float *d_vec = nullptr, *d_norm = nullptr;
+    int64_t *d_values = nullptr;
+    int *d_bad = nullptr;
+    int bad = 0;
+    // the float rows cross PCIe once and are normalised once; every context packs the same device-resident values
+    cudaError_t e = cudaMalloc(&d_vec, values * sizeof(float));
+    if (e == cudaSuccess) e = cudaMalloc(&d_norm, (size_t)row_count * sizeof(float));
+    if (e == cudaSuccess) e = cudaMalloc(&d_values, values * sizeof(int64_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_bad, sizeof(int));
+    if (e == cudaSuccess) e = upload(d_vec, vectors, values * sizeof(float));
+    if (e == cudaSuccess) e = fill(d_bad, 0, sizeof(int));
+    if (e == cudaSuccess) e = launch_pnns_normalize(d_vec, row_count, column_count, scaling_factor, d_norm, d_values, d_bad, nullptr);
+    if (e == cudaSuccess) e = cudaMemcpy(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost);
+    cudaFree(d_vec);
+    cudaFree(d_norm);
+    cudaFree(d_bad);
+    rc = e != cudaSuccess ? cuda_fail(e, "pnns vectors normalisation")
+         : bad            ? fail(HECUDA_ERR_INVALID_ARGUMENT, "a vector value is not finite or a scaled value leaves Int64")
+                          : HECUDA_OK;
+    for (int32_t k = 0; rc == HECUDA_OK && k < plaintext_count; ++k)
+        rc = matrix_from_device_values(ctxs[k], shapes[(size_t)k], d_values, reduce, &out[k]);
+    cudaFree(d_values);
+    if (rc)
+        for (int32_t k = 0; k < plaintext_count; ++k) {
+            hecuda_pnns_matrix_destroy(out[k]);
+            out[k] = nullptr;
+        }
+    return rc;
 }
 
 int32_t hecuda_pnns_matrix_device_buffer(hecuda_pnns_matrix *m, void **device_ptr, uint64_t *bytes) {

@@ -5,6 +5,8 @@
 //   CoefficientPacking.bytesToCoefficients                                  HomomorphicEncryption/CoefficientPacking.swift
 //   PlaintextMatrix.init(signedValues:) + diagonalPlaintexts                PlaintextMatrix.swift:155-190, 417-482
 #pragma once
+#include <math.h>
+
 #include <cstdint>
 
 #ifdef __CUDACC__
@@ -161,6 +163,142 @@ PDB_HD uint64_t pnns_signed_value(long long x, uint64_t t, bool reduce, bool &ba
     }
     if (x > (m - 1) / 2 || x < -(m / 2)) bad = true;
     return x < 0 ? (uint64_t)(x + m) : (uint64_t)x;
+}
+
+// ---- PNNS client ----------------------------------------------------------------------------------------------------
+// Array2d.normalizedScaledAndRounded (PrivateNearestNeighborSearch/Util.swift:74-89) in Swift Float arithmetic: every
+// operation rounded on its own (no contraction into an FMA, whatever the compiler flags), the squares summed left to
+// right, a correctly rounded square root, (value * s) / norm as two roundings, then .toNearestOrAwayFromZero.
+#ifdef __CUDA_ARCH__
+#define PNNS_FMUL(a, b) __fmul_rn(a, b)
+#define PNNS_FADD(a, b) __fadd_rn(a, b)
+#define PNNS_FDIV(a, b) __fdiv_rn(a, b)
+#define PNNS_FSQRT(a) __fsqrt_rn(a)
+#else
+// the host build that replays these helpers compiles with -ffp-contract=off; a volatile keeps each step rounded anyway
+PDB_HD float pnns_round_step(float x) {
+    volatile float v = x;
+    return v;
+}
+#define PNNS_FMUL(a, b) pnns_round_step((a) * (b))
+#define PNNS_FADD(a, b) pnns_round_step((a) + (b))
+#define PNNS_FDIV(a, b) pnns_round_step((a) / (b))
+#define PNNS_FSQRT(a) sqrtf(a)
+#endif
+
+// row.map { $0 * $0 }.reduce(0, +).squareRoot(): the sum is sequential on purpose -- a reordered sum changes the norm
+PDB_HD float pnns_row_norm(const float *row, long long cols) {
+    float sum = 0.0f;
+    for (long long k = 0; k < cols; ++k) sum = PNNS_FADD(sum, PNNS_FMUL(row[k], row[k]));
+    return PNNS_FSQRT(sum);
+}
+
+// V((value * scalingFactor / norm).rounded()) with V = Int64; 0 for a zero norm.  `bad` is set where Swift traps: a
+// non-finite input (its row's values are NaN) or a rounded value outside Int64.
+PDB_HD long long pnns_scaled_value(float value, float scale, float norm, bool &bad) {
+    if (!isfinite(value)) {
+        bad = true;
+        return 0;
+    }
+    if (norm == 0.0f) return 0;
+    const float r = roundf(PNNS_FDIV(PNNS_FMUL(value, scale), norm));
+    if (!(r >= -9223372036854775808.0f && r < 9223372036854775808.0f)) {  // also NaN
+        bad = true;
+        return 0;
+    }
+    return (long long)r;
+}
+
+PDB_HD long long pnns_next_pow2(long long v) {
+    long long p = 1;
+    while (p < v) p <<= 1;
+    return p;
+}
+
+// PlaintextMatrix.denseRowPlaintexts (PlaintextMatrix.swift:341-413) for `rows` rows of `cols` values: SIMD slot `slot`
+// (0 .. N) of plaintext `p` -> index of the row-major value it holds, -1 for a zero.  Rows take nextPow2(cols) slots
+// each, N / nextPow2(cols) rows per plaintext (the SIMD-row padding of :386-388 never applies, as nextPow2(cols)
+// divides N / 2).  The last plaintext's k rows are padded to a power of two within their SIMD row and repeated to
+// fill N slots (:396-408): [0, P) repeated when they fit in one SIMD row, else the first SIMD row then the second's
+// P slots repeated.  The same formula covers full plaintexts (k = N / nextPow2(cols), P = N / 2).
+PDB_HD long long pnns_dense_row_element(long long rows, long long cols, int logn, long long p, long long slot) {
+    const long long n = 1ll << logn, half = n >> 1, width = pnns_next_pow2(cols), per = n / width;
+    const long long left = rows - p * per, k = left < per ? left : per;
+    const long long len = k * width;
+    long long at;
+    if (len <= half) {
+        at = slot % pnns_next_pow2(len);
+    } else {
+        at = slot < half ? slot : half + (slot - half) % pnns_next_pow2(len - half);
+    }
+    const long long j = at / width, c = at - j * width;
+    return j < k && c < cols ? (p * per + j) * cols + c : -1;
+}
+
+// ciphertexts of a .denseRow matrix: ceil(rows / (N / nextPow2(cols)))
+PDB_HD long long pnns_dense_row_count(long long rows, long long cols, int logn) {
+    const long long per = (1ll << logn) / pnns_next_pow2(cols);
+    return (rows + per - 1) / per;
+}
+
+// PlaintextMatrix.unpackDenseColumn (PlaintextMatrix.swift:515-556) of a rows x cols .denseColumn matrix: element
+// (r, c) of the row-major result is column-major value c * rows + r, which plaintext `p` holds at SIMD slot `slot`.
+// With 2 * (N/2 / rows) > 1 columns per plaintext, each SIMD row holds rows * (N/2 / rows) values; otherwise a column
+// takes ceil(rows / N) plaintexts.
+PDB_HD void pnns_dense_column_slot(long long rows, long long cols, int logn, long long r, long long c, long long &p,
+                                   long long &slot) {
+    const long long n = 1ll << logn, half = n >> 1;
+    const long long m = c * rows + r;
+    if (2 * (half / rows) > 1) {
+        const long long per_row = rows * (half / rows);
+        p = m / (2 * per_row);
+        const long long w = m - p * 2 * per_row;
+        slot = w < per_row ? w : half + (w - per_row);
+    } else {
+        const long long per_column = (rows + n - 1) / n;
+        p = c * per_column + r / n;
+        slot = r % n;
+    }
+    (void)cols;
+}
+
+// plaintexts of a rows x cols .denseColumn matrix (the replies mulTranspose(matrix:) returns)
+PDB_HD long long pnns_dense_column_count(long long rows, long long cols, int logn) {
+    const long long n = 1ll << logn, half = n >> 1;
+    if (2 * (half / rows) > 1) {
+        const long long per = 2 * rows * (half / rows);
+        return (rows * cols + per - 1) / per;
+    }
+    return cols * ((rows + n - 1) / n);
+}
+
+// Plaintext CRT over t_0 .. t_{k-1} (CrtComposer.compose, CrtComposer.swift:76-97), remainderToCentered over T = prod t_i
+// and Float(signed) / (Float(s) * Float(s)) (Client.swift:110-117).  x[i] < t[i]; inv[i] = (T / t_i)^-1 mod t_i,
+// punct[i] = T / t_i; T below 2^63 when k > 1 (composeMaxIntermediateValue = 2T), so the modular sum never wraps.
+struct PnnsCrt {
+    int count;
+    uint64_t t[8], inv[8], punct[8];
+    uint64_t product;
+};
+PDB_HD long long pnns_crt_signed(const PnnsCrt &c, const uint64_t *x) {
+    uint64_t acc = 0;
+    for (int i = 0; i < c.count; ++i) {
+        const uint64_t tmp = (uint64_t)((unsigned __int128)x[i] * c.inv[i] % c.t[i]);
+        const uint64_t add = tmp * c.punct[i];  // < T
+        acc += add;
+        if (acc >= c.product) acc -= c.product;
+    }
+    // UInt64.remainderToCentered (Scalar.swift): x > (T - 1) / 2 ? x - T : x
+    return acc > (c.product - 1) / 2 ? (long long)(acc - c.product) : (long long)acc;
+}
+PDB_HD float pnns_distance(long long v, long long scaling_factor) {
+#ifdef __CUDA_ARCH__
+    const float s = __ll2float_rn(scaling_factor);
+    return __fdiv_rn(__ll2float_rn(v), __fmul_rn(s, s));
+#else
+    const float s = (float)scaling_factor;
+    return PNNS_FDIV((float)v, PNNS_FMUL(s, s));
+#endif
 }
 
 }  // namespace procdb

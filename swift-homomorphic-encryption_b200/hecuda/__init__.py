@@ -165,6 +165,12 @@ SYMBOLS = {
     "hecuda_bfv_encrypt_seeded": (C.c_int32, [_VP, _VP, _VP, _VP, _VP, _VP, C.c_int64]),
     "hecuda_evk_generate": (C.c_int32, [_VP, _VP, C.c_int32, _VP, C.c_int32, _VP, _VP, C.POINTER(_VP), _VP]),
     "hecuda_bfv_noise_budget": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int32, C.c_int32, _VP, C.c_int64]),
+    "hecuda_evk_copy": (C.c_int32, [_VP, _VP, C.POINTER(_VP)]),
+    "hecuda_pnns_matrices_create_from_vectors": (C.c_int32, [C.POINTER(_VP), C.c_int32, _VP, C.c_int64, C.c_int64, C.c_int64,
+                                                             C.c_int32, C.c_int32, C.POINTER(_VP)]),
+    "hecuda_pnns_query_generate": (C.c_int32, [_VP, _VP, _VP, C.c_int64, C.c_int64, C.c_int64, C.c_int32, _VP, _VP, _VP, _VP]),
+    "hecuda_pnns_decrypt_distances": (C.c_int32, [C.POINTER(_VP), C.c_int32, _VP, C.POINTER(_VP), C.c_int64, C.c_int32,
+                                                  C.c_int64, C.c_int64, C.c_int64, _VP]),
     "hecuda_poly_add": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int32, C.c_int64]),
     "hecuda_poly_add_device": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int32, C.c_int64, _VP]),
     "hecuda_poly_sub": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int32, C.c_int64]),
@@ -494,6 +500,23 @@ class EvaluationKey:
                            for j, e in enumerate(elements)}}
         return key, form
 
+    def forContext(self, context: Context) -> "EvaluationKey":
+        """This key for another context that differs only in the plaintext modulus (hecuda_evk_copy): BFV keys do not
+        depend on t, so the reference uses one key generated on contexts[0] with every plaintext modulus
+        (PrivateNearestNeighborSearch/Client.swift:137-146).  The device copy is made once per context, kept on this
+        key and freed with it; the key itself is returned for its own context."""
+        if context is self.context:
+            return self
+        copies = self.__dict__.setdefault("_copies", {})
+        key = copies.get(id(context))
+        if key is None:
+            h = C.c_void_p()
+            _check(load_library().hecuda_evk_copy(self._h, context._h, C.byref(h)))
+            key = EvaluationKey.__new__(EvaluationKey)
+            key.context, key.galoisElements, key._h = context, list(self.galoisElements), h
+            copies[id(context)] = key
+        return key
+
     def setGaloisKey(self, element: int, key):
         """GaloisKey.keys[element] (Keys.swift:150-163): (L, 2, L+1, N) uint64, Eval format."""
         k = _host(key)
@@ -517,6 +540,8 @@ class EvaluationKey:
         return p.value, n.value
 
     def close(self):
+        for key in self.__dict__.pop("_copies", {}).values():
+            key.close()
         if getattr(self, "_h", None) is not None:
             load_library().hecuda_evk_destroy(self._h)
             self._h = None

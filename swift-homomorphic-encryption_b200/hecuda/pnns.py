@@ -16,6 +16,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 from dataclasses import dataclass
+from typing import Any
 
 import numpy as np
 
@@ -516,3 +517,397 @@ def denseRowVector(context, vector) -> np.ndarray:
     while len(packed) < n:
         packed += repeat
     return SimdEncoder(n, t).encode(np.array(packed[:n], dtype=np.uint64))[0]
+
+
+# ------------------------------------------------------------------------------------------------ client and server
+# Client, Server, Database and ProcessedDatabase of PrivateNearestNeighborSearch (Client.swift, Server.swift,
+# Database.swift, ProcessedDatabase.swift, Config.swift) over one context per plaintext modulus.  Float vectors are
+# normalised, scaled and rounded on the device in Swift Float arithmetic; queries are packed, encoded and encrypted
+# there (hecuda_pnns_query_generate), and replies decrypted, decoded, CRT-composed and turned into float distances
+# (hecuda_pnns_decrypt_distances).
+
+COSINE_SIMILARITY = "cosineSimilarity"  # DistanceMetric.cosineSimilarity, the only metric
+
+
+@dataclass(frozen=True)
+class EncryptionParameters:
+    """The parts of EncryptionParameters a PNNS configuration compares contexts against."""
+
+    polyDegree: int
+    plaintextModulus: int
+    coefficientModuli: tuple
+
+    @staticmethod
+    def ofContext(context: Context) -> "EncryptionParameters":
+        return EncryptionParameters(context.degree, context.plaintextModulus, tuple(context.coefficientModuli))
+
+
+class MatrixMultiplication:
+    @staticmethod
+    def evaluationKeyConfig(plaintextMatrixDimensions: MatrixDimensions, maxQueryCount: int, degree: int):
+        """MatrixMultiplication.evaluationKeyConfig (MatrixMultiplication.swift:76-116) united with
+        CiphertextMatrix.extractDenseRowConfig (CiphertextMatrix.swift:224-243)."""
+        from .pir import EvaluationKeyConfig
+        simd_columns = degree // 2
+        bsgs = BabyStepGiantStep.forVectorDimension(plaintextMatrixDimensions.columnCount)
+        rot = GaloisElement.rotatingColumns
+        elements = [rot(-1, degree), rot(-bsgs.babyStep, degree), GaloisElement.swappingRows(degree)]
+        if simd_columns // plaintextMatrixDimensions.rowCount > 1:
+            elements.append(rot(1, degree))
+            if simd_columns > 16:
+                elements.append(rot(16, degree))
+            if simd_columns > 256:
+                elements.append(rot(256, degree))
+        if maxQueryCount != 1:
+            width = _next_power_of_two(plaintextMatrixDimensions.columnCount)
+            if width != simd_columns:
+                elements.append(rot(width, degree))
+        return EvaluationKeyConfig(list(dict.fromkeys(elements)), False)
+
+
+class ClientConfig:
+    """ClientConfig (Config.swift:50-136).  encryptionParameters: the first context's EncryptionParameters; one more
+    set per extra plaintext modulus, identical but for t."""
+
+    def __init__(self, encryptionParameters: EncryptionParameters, scalingFactor: int, vectorDimension: int,
+                 evaluationKeyConfig, distanceMetric: str = COSINE_SIMILARITY, extraPlaintextModuli=(),
+                 queryPacking: str = "denseRow"):
+        p = encryptionParameters
+        self.encryptionParameters = [p] + [EncryptionParameters(p.polyDegree, int(t), p.coefficientModuli)
+                                           for t in extraPlaintextModuli]
+        self.scalingFactor = int(scalingFactor)
+        self.queryPacking = queryPacking
+        self.vectorDimension = int(vectorDimension)
+        self.evaluationKeyConfig = evaluationKeyConfig
+        self.distanceMetric = distanceMetric
+        self.extraPlaintextModuli = [int(t) for t in extraPlaintextModuli]
+
+    @property
+    def plaintextModuli(self):
+        return [p.plaintextModulus for p in self.encryptionParameters]
+
+    @staticmethod
+    def maxScalingFactor(distanceMetric: str, vectorDimension: int, plaintextModuli) -> int:
+        """ClientConfig.maxScalingFactor (Config.swift:112-120) in Float: floor(sqrt((t - 1) / 2) - sqrt(d) / 2) with
+        t the Float product of the moduli."""
+        if distanceMetric != COSINE_SIMILARITY:
+            raise PnnsError(f"wrongDistanceMetric(got: {distanceMetric}, expected: {COSINE_SIMILARITY})")
+        f = np.float32
+        t = f(1)
+        for m in plaintextModuli:
+            t = f(t * f(int(m)))
+        value = f(np.sqrt(f(f(t - f(1)) / f(2)))) - f(f(np.sqrt(f(int(vectorDimension)))) / f(2))
+        return int(np.floor(f(value)))
+
+    def validateContexts(self, contexts):
+        """ClientConfig.validateContexts (Config.swift:125-135)."""
+        if len(contexts) != len(self.encryptionParameters):
+            raise PnnsError(f"wrongContextsCount(got: {len(contexts)}, expected: {len(self.encryptionParameters)})")
+        for context, params in zip(contexts, self.encryptionParameters):
+            got = EncryptionParameters.ofContext(context)
+            if got != params:
+                raise PnnsError(f"wrongEncryptionParameters(got: {got}, expected: {params})")
+
+
+class ServerConfig:
+    """ServerConfig (Config.swift:138-204): the client's configuration and the database's .diagonal packing."""
+
+    def __init__(self, clientConfig: ClientConfig, babyStepGiantStep: BabyStepGiantStep = None):
+        self.clientConfig = clientConfig
+        self.babyStepGiantStep = babyStepGiantStep or BabyStepGiantStep.forVectorDimension(clientConfig.vectorDimension)
+
+    def __getattr__(self, name):  # scalingFactor, plaintextModuli, distanceMetric, vectorDimension, ...
+        if name == "clientConfig":
+            raise AttributeError(name)
+        return getattr(self.clientConfig, name)
+
+    def validateContexts(self, contexts):
+        self.clientConfig.validateContexts(contexts)
+
+
+def _check_metric(metric: str):
+    if metric != COSINE_SIMILARITY:
+        raise PnnsError(f"wrongDistanceMetric(got: {metric}, expected: {COSINE_SIMILARITY})")
+
+
+def _float_rows(vectors) -> np.ndarray:
+    v = np.ascontiguousarray(np.asarray(vectors, dtype=np.float32))
+    return v.reshape(1, -1) if v.ndim == 1 else v
+
+
+@dataclass
+class DatabaseRow:
+    """DatabaseRow (Database.swift): an identifier, optional metadata bytes and the vector."""
+
+    entryId: int
+    entryMetadata: bytes
+    vector: list
+
+
+@dataclass
+class Database:
+    rows: list
+
+
+@dataclass
+class Query:
+    """Query (PnnsProtocol.swift:18-27): one dense-row ciphertext matrix per plaintext modulus, each (count, 2, L, N)
+    Coeff, or with `wire` each the .seeded form (poly0 (count, B) uint8, seeds (count, 32) uint8)."""
+
+    ciphertextMatrices: list
+    dimensions: MatrixDimensions
+    wire: bool = False
+
+
+@dataclass
+class Response:
+    """Response (PnnsProtocol.swift:30-52): one dense-column ciphertext matrix per plaintext modulus of `dimensions`
+    (database rows x query rows), each (count, 2, l, N) Coeff or PnnsWire reply bytes (bytes (count, B0 + B1), skips)."""
+
+    ciphertextMatrices: list
+    dimensions: MatrixDimensions
+    entryIds: list = None
+    entryMetadatas: list = None
+
+    def _ciphertexts(self, contexts):
+        from . import Bfv
+        out = []
+        for ctx, m in zip(contexts, self.ciphertextMatrices):
+            if isinstance(m, tuple):  # PnnsWire reply bytes, skipLSBsForDecryption
+                data, skips = m
+                data = np.asarray(data, dtype=np.uint8).reshape(-1, np.asarray(data).shape[-1])
+                b0 = Bfv.serializationByteCount(ctx, 1, skips[0])
+                poly0 = Bfv.load(ctx, np.ascontiguousarray(data[:, :b0]), 1, skips[0])
+                poly1 = Bfv.load(ctx, np.ascontiguousarray(data[:, b0:]), 1, skips[1])
+                m = np.stack([poly0, poly1], axis=1)
+            out.append(np.ascontiguousarray(np.asarray(m, dtype=np.uint64)))
+        return out
+
+    def noiseBudget(self, contexts, secretKey) -> float:
+        """Response.noiseBudget (PnnsProtocol.swift:98-102): the least budget over the matrices, each under its own
+        context's t.  Must never be forwarded to another party."""
+        from . import Bfv
+        budgets = [float(np.min(Bfv.noiseBudget(ctx, secretKey, cts)))
+                   for ctx, cts in zip(contexts, self._ciphertexts(contexts))]
+        return min(budgets) if budgets else -math.inf
+
+
+@dataclass
+class DatabaseDistances:
+    """DatabaseDistances (PnnsProtocol.swift:55-77): float32 distances (database rows x query rows)."""
+
+    distances: np.ndarray
+    entryIds: list
+    entryMetadatas: list
+
+
+class Client:
+    """Client (Client.swift:20-147) over one context per plaintext modulus."""
+
+    def __init__(self, config: ClientConfig, contexts):
+        _check_metric(config.distanceMetric)
+        config.validateContexts(contexts)
+        ts = config.plaintextModuli
+        if len(set(ts)) != len(ts):
+            raise PnnsError("plaintext moduli must be pairwise distinct")
+        self.config, self.contexts = config, list(contexts)
+
+    @property
+    def evaluationKeyConfig(self):
+        return self.config.evaluationKeyConfig
+
+    def generateSecretKey(self, seed=None):
+        from . import SecretKey
+        return SecretKey.generate(self.contexts[0], seed)
+
+    def generateEvaluationKey(self, secretKey):
+        """On contexts[0], used with every plaintext modulus (Client.swift:137-146)."""
+        return EvaluationKey.generate(self.contexts[0], self.evaluationKeyConfig, secretKey)
+
+    def generateQuery(self, vectors, secretKey, wire: bool = False, aSeeds=None, errorSeeds=None) -> Query:
+        """Client.generateQuery (Client.swift:73-91) on the device: one encrypted .denseRow matrix per context, the values
+        reduced mod t when there are several (hecuda_pnns_query_generate).  Seeds: per context, (count, 32) uint8 each,
+        fresh from secrets.token_bytes by default."""
+        from . import Bfv, _secret_poly, _seeds
+        v = _float_rows(vectors)
+        rows, cols = v.shape
+        dims = MatrixDimensions(rows, cols)
+        sk = _secret_poly(secretKey)
+        reduce = 1 if len(self.contexts) > 1 else 0
+        out = []
+        for k, ctx in enumerate(self.contexts):
+            count = CiphertextMatrix.ciphertextCount(ctx.degree, dims) if cols <= ctx.degree // 2 else 1
+            a = _seeds(count, None if aSeeds is None else aSeeds[k])
+            err = _seeds(count, None if errorSeeds is None else errorSeeds[k])
+            if wire:
+                poly0 = np.empty((count, Bfv.serializationByteCount(ctx, ctx.L)), dtype=np.uint8)
+                cts = None
+            else:
+                cts = np.empty((count, 2, ctx.L, ctx.degree), dtype=np.uint64)
+                poly0 = None
+            rc = load_library().hecuda_pnns_query_generate(
+                ctx._h, _ptr(sk), v.ctypes.data_as(C.c_void_p), rows, cols, self.config.scalingFactor, reduce, _ptr(a),
+                _ptr(err), _ptr(cts) if cts is not None else None, _ptr(poly0) if poly0 is not None else None)
+            err[:] = 0
+            _check(rc)
+            out.append((poly0, a) if wire else cts)
+        return Query(out, dims, wire)
+
+    def decrypt(self, response: Response, secretKey) -> DatabaseDistances:
+        """Client.decrypt (Client.swift:99-127) on the device (hecuda_pnns_decrypt_distances): float32 distances,
+        database rows x query rows."""
+        from . import _secret_poly
+        if not response.ciphertextMatrices:
+            raise PnnsError("emptyCiphertextArray")
+        if len(response.ciphertextMatrices) != len(self.contexts):
+            raise PnnsError(f"wrongCiphertextMatrixCount(got: {len(response.ciphertextMatrices)}, expected: {len(self.contexts)})")
+        cts = response._ciphertexts(self.contexts)
+        count, polys, l, n = cts[0].shape
+        if polys != 2 or any(c.shape != cts[0].shape for c in cts):
+            raise HeError(-1, "invalidCiphertext: every matrix must hold the same number of 2 x l x N ciphertexts")
+        sk = _secret_poly(secretKey)
+        dims = response.dimensions
+        out = np.empty((dims.rowCount, dims.columnCount), dtype=np.float32)
+        ctxs = (C.c_void_p * len(self.contexts))(*[c._h.value for c in self.contexts])
+        replies = (C.c_void_p * len(cts))(*[c.ctypes.data for c in cts])
+        _check(load_library().hecuda_pnns_decrypt_distances(ctxs, len(self.contexts), _ptr(sk), replies, count, l,
+                                                           dims.rowCount, dims.columnCount, self.config.scalingFactor,
+                                                           out.ctypes.data_as(C.c_void_p)))
+        return DatabaseDistances(out, response.entryIds, response.entryMetadatas)
+
+
+@dataclass
+class ValidationResult:
+    """ValidationResult (ProcessedDatabase.swift:147-184): the first trial's key and query, the last response, its
+    distances (first trial), the least noise budget and each trial's response time in seconds."""
+
+    evaluationKey: Any
+    query: Query
+    response: Response
+    databaseDistances: DatabaseDistances
+    noiseBudget: float
+    computeTimes: list
+
+
+class ProcessedDatabase:
+    """ProcessedDatabase (ProcessedDatabase.swift): its contexts, one resident .diagonal matrix per context, the entry
+    identifiers and metadata."""
+
+    def __init__(self, contexts, plaintextMatrices, entryIds, entryMetadatas, serverConfig: ServerConfig):
+        self.contexts, self.plaintextMatrices = list(contexts), list(plaintextMatrices)
+        self.entryIds, self.entryMetadatas, self.serverConfig = list(entryIds), list(entryMetadatas), serverConfig
+
+    @classmethod
+    def processOnDevice(cls, database: Database, serverConfig: ServerConfig, contexts) -> "ProcessedDatabase":
+        """Database.process (ProcessedDatabase.swift:194-229) on the device (hecuda_pnns_matrices_create_from_vectors):
+        the float rows cross PCIe once, are normalised, scaled and rounded once, and packed into one resident Eval
+        matrix per context, reduced mod t when there are several."""
+        _check_metric(serverConfig.distanceMetric)
+        serverConfig.validateContexts(contexts)
+        if not database.rows:
+            raise PnnsError("emptyDatabase")
+        vectors = _float_rows([row.vector for row in database.rows])
+        rows, cols = vectors.shape
+        dims = MatrixDimensions(rows, cols)
+        bsgs = serverConfig.babyStepGiantStep
+        handles = (C.c_void_p * len(contexts))()
+        ctxs = (C.c_void_p * len(contexts))(*[c._h.value for c in contexts])
+        _check(load_library().hecuda_pnns_matrices_create_from_vectors(
+            ctxs, len(contexts), vectors.ctypes.data_as(C.c_void_p), rows, cols, serverConfig.scalingFactor, bsgs.babyStep,
+            bsgs.giantStep, handles))
+        matrices = []
+        for ctx, h in zip(contexts, handles):
+            m = PlaintextMatrix.__new__(PlaintextMatrix)
+            m.context, m.dimensions, m.babyStepGiantStep, m._h = ctx, dims, bsgs, C.c_void_p(h)
+            m.resultCiphertextCount = -(-rows // ctx.degree)
+            matrices.append(m)
+        has_metadata = any(len(row.entryMetadata) for row in database.rows)
+        return cls(contexts, matrices, [row.entryId for row in database.rows],
+                   [bytes(row.entryMetadata) for row in database.rows] if has_metadata else [], serverConfig)
+
+    def validate(self, queryVectors, trials: int = 1) -> ValidationResult:
+        """ProcessedDatabase.validate (ProcessedDatabase.swift:91-143), every step on the device."""
+        import time
+        from . import Bfv
+        if trials <= 0:
+            raise PnnsError(f"validationError(Invalid trialsPerShard: {trials})")
+        v = _float_rows(queryVectors)
+        if v.shape[1] != self.serverConfig.vectorDimension:
+            raise PnnsError(f"validationError(Wrong vector dimension {v.shape[1]}, expected {self.serverConfig.vectorDimension})")
+        server = Server(self)
+        client = Client(self.serverConfig.clientConfig, self.contexts)
+        first_key = first_query = response = distances = None
+        min_budget, times = math.inf, []
+        for trial in range(trials):
+            secret_key = client.generateSecretKey()
+            key = client.generateEvaluationKey(secret_key)
+            query = client.generateQuery(v, secret_key)
+            start = time.perf_counter()
+            response = server.computeResponse(query, key)
+            times.append(time.perf_counter() - start)
+            budget = response.noiseBudget(self.contexts, secret_key)
+            if budget < Bfv.minNoiseBudget:
+                raise PnnsError("validationError(Insufficient noise budget)")
+            decrypted = client.decrypt(response, secret_key)
+            min_budget = min(min_budget, budget)
+            if trial == 0:
+                first_key, first_query, distances = key, query, decrypted
+            else:
+                key.close()
+        return ValidationResult(first_key, first_query, response, distances, min_budget, times)
+
+    def close(self):
+        for m in self.plaintextMatrices:
+            m.close()
+
+
+class Server:
+    """Server (Server.swift:19-89) over a processed database, one matrix per plaintext modulus."""
+
+    def __init__(self, database: ProcessedDatabase):
+        _check_metric(database.serverConfig.distanceMetric)
+        self.database = database
+
+    @property
+    def contexts(self):
+        return self.database.contexts
+
+    def _check(self, query: Query):
+        expected = len(self.database.plaintextMatrices)
+        if len(query.ciphertextMatrices) != expected:
+            raise PnnsError(f"invalidQuery(wrongCiphertextMatrixCount(got: {len(query.ciphertextMatrices)}, expected: {expected}))")
+
+    def computeResponse(self, query: Query, evaluationKey: EvaluationKey) -> Response:
+        """Server.computeResponse (Server.swift:61-88): mulTranspose(matrix:) and modSwitchDownToSingle per matrix, the
+        key copied to contexts 1 and up (EvaluationKey.forContext)."""
+        return self.computeResponses([query], [evaluationKey])[0]
+
+    def computeResponses(self, queries, evaluationKeys) -> list:
+        """computeResponse for many clients, each with its own key: one PlaintextMatrix.computeResponses call (or its
+        wire form for wire queries) per matrix."""
+        queries, keys = list(queries), list(evaluationKeys)
+        for q in queries:
+            self._check(q)
+        if not queries or len(queries) != len(keys):
+            raise PnnsError("one evaluation key per query")
+        dims = queries[0].dimensions
+        if any(q.dimensions != dims or q.wire != queries[0].wire for q in queries):
+            raise PnnsError("every query must have the same dimensions and form")
+        per_matrix = []
+        for k, m in enumerate(self.database.plaintextMatrices):
+            ctx_keys = [key.forContext(m.context) for key in keys]
+            if queries[0].wire:
+                poly0 = np.stack([q.ciphertextMatrices[k][0] for q in queries])
+                seeds = np.stack([q.ciphertextMatrices[k][1] for q in queries])
+                replies, skips = PnnsWire.computeResponses(m, poly0, seeds, dims, ctx_keys)
+                per_matrix.append([(replies[c], skips) for c in range(len(queries))])
+            else:
+                cts = np.stack([q.ciphertextMatrices[k] for q in queries])
+                if len(queries) == 1:
+                    replies = m.mulTransposeMatrix(cts[0], dims, ctx_keys[0], modSwitchDownToSingle=True)[None]
+                else:
+                    replies = m.computeResponses(cts, dims, ctx_keys)
+                per_matrix.append([replies[c] for c in range(len(queries))])
+        out_dims = MatrixDimensions(self.database.plaintextMatrices[0].dimensions.rowCount, dims.rowCount)
+        return [Response([per_matrix[k][c] for k in range(len(per_matrix))], out_dims, list(self.database.entryIds),
+                         list(self.database.entryMetadatas)) for c in range(len(queries))]
