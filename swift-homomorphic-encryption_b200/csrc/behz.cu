@@ -390,30 +390,26 @@ static ColTiles col_tiles(int64_t n, int64_t polys, int cols) {
     return tl;
 }
 
-// a lift / floor launch: one CTA per tile
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_tiles(void (*kernel)(KArgs...), const ColTiles &tl, cudaStream_t stream, Args... args) {
-    if (tl.count == 0) return cudaSuccess;
-    if (tl.count > 0x7fffffffLL) return cudaErrorInvalidConfiguration;  // gridDim.x
-    ++g_kernel_launches;
-    kernel<<<(unsigned)tl.count, kThreads, 0, stream>>>(args..., tl);
-    return cudaGetLastError();
-}
-
 template <bool H, bool Q_ROWS>
 static cudaError_t launch_lift_tiles(const Context &ctx, const u64 *lhs, const u64 *rhs, int pin_shift, u64 *ext,
                                      int64_t polys_out, const LiftConsts &consts, cudaStream_t stream) {
     cudaError_t e;
-    HE_DISPATCH_L(ctx.L, (e = launch_tiles(lift_kernel<LL, H, Q_ROWS>, col_tiles(ctx.n, polys_out, BehzCols<LL>::value),
-                                           stream, lhs, rhs, pin_shift, ext, consts, (int)ctx.n)));
+    ColTiles tl;
+    HE_DISPATCH_L(ctx.L, (tl = col_tiles(ctx.n, polys_out, BehzCols<LL>::value),
+                          e = tl.count > 0x7fffffffLL ? cudaErrorInvalidConfiguration  // one CTA per tile: gridDim.x
+                                                    : launch(lift_kernel<LL, H, Q_ROWS>, (unsigned)tl.count, kThreads, 0,
+                                                             stream, lhs, rhs, pin_shift, ext, consts, (int)ctx.n, tl)));
     return e;
 }
 template <bool H, bool Q_SCALED>
 static cudaError_t launch_floor_tiles(const Context &ctx, const u64 *in, u64 *out, int64_t polys,
                                       const FloorConsts &consts, cudaStream_t stream) {
     cudaError_t e;
-    HE_DISPATCH_L(ctx.L, (e = launch_tiles(floor_kernel<LL, H, Q_SCALED>, col_tiles(ctx.n, polys, BehzCols<LL>::value),
-                                           stream, in, out, consts, (int)ctx.n)));
+    ColTiles tl;
+    HE_DISPATCH_L(ctx.L, (tl = col_tiles(ctx.n, polys, BehzCols<LL>::value),
+                          e = tl.count > 0x7fffffffLL ? cudaErrorInvalidConfiguration  // one CTA per tile: gridDim.x
+                                                    : launch(floor_kernel<LL, H, Q_SCALED>, (unsigned)tl.count, kThreads, 0,
+                                                             stream, in, out, consts, (int)ctx.n, tl)));
     return e;
 }
 
@@ -432,15 +428,15 @@ static cudaError_t launch_lift_generic(const Context &ctx, const u64 *in, int po
     // the z dimension must divide exactly: launch in slabs of y = 32768 polys, then the remainder
     while (polys > 0) {
         int64_t slab = polys >= 32768 ? (polys / 32768) * 32768 : polys;
-        ++g_kernel_launches;
-        lift_generic_kernel<<<poly_grid(ctx.n, slab), kThreads, 0, stream>>>(in, polys_in, ext, ext_polys, out_poly_offset,
-                                                                              consts, (int)ctx.n, q_rows);
+        const cudaError_t e = launch(lift_generic_kernel, poly_grid(ctx.n, slab), kThreads, 0, stream, in, polys_in, ext,
+                                     ext_polys, out_poly_offset, consts, (int)ctx.n, q_rows);
+        if (e != cudaSuccess) return e;
         // advance whole items only (32768 is even and polys_in is 1 or 2)
         in += slab * pstride_in;
         ext += (slab / polys_in) * (int64_t)ext_polys * (q_rows ? 2 * ctx.L + 1 : ctx.L + 1) * ctx.n;
         polys -= slab;
     }
-    return cudaGetLastError();
+    return cudaSuccess;
 }
 
 cudaError_t launch_lift(const Context &ctx, const u64 *lhs, const u64 *rhs, int polys_in, u64 *ext, int64_t items,
@@ -457,9 +453,9 @@ cudaError_t launch_lift(const Context &ctx, const u64 *lhs, const u64 *rhs, int 
     }
     const int64_t polys_out = items * ops * polys_in;
     const int pin_shift = polys_in == 2 ? 1 : 0;
-    auto launch = consts.h_primes ? (q_rows ? launch_lift_tiles<true, true> : launch_lift_tiles<true, false>)
-                                  : (q_rows ? launch_lift_tiles<false, true> : launch_lift_tiles<false, false>);
-    return launch(ctx, lhs, rhs, pin_shift, ext, polys_out, consts, stream);
+    auto lift_tiles = consts.h_primes ? (q_rows ? launch_lift_tiles<true, true> : launch_lift_tiles<true, false>)
+                                      : (q_rows ? launch_lift_tiles<false, true> : launch_lift_tiles<false, false>);
+    return lift_tiles(ctx, lhs, rhs, pin_shift, ext, polys_out, consts, stream);
 }
 
 cudaError_t launch_tensor(const Context &ctx, const u64 *ext, u64 *ten, int64_t items, cudaStream_t stream,
@@ -477,14 +473,10 @@ cudaError_t launch_tensor(const Context &ctx, const u64 *ext, u64 *ten, int64_t 
     for (int r = 0; r < tc.R; ++r) any_h |= tc.h[r] != 0;
     auto k = any_h ? tensor_kernel<2, true> : tensor_kernel<2, false>;  // N >= 2: two columns per thread
     const unsigned gx = (unsigned)((ctx.n / 2 + kThreads - 1) / kThreads);
-    for (int64_t done = 0; done < items;) {  // gridDim.z <= 65535
-        const int64_t chunk = (items - done) > 65535 ? 65535 : (items - done);
+    return for_each_part(items, [&](int64_t done, int64_t chunk) {
         dim3 grid(gx ? gx : 1, (unsigned)tc.R, (unsigned)chunk);
-        ++g_kernel_launches;
-        k<<<grid, kThreads, 0, stream>>>(ext + done * 4 * tc.R * ctx.n, ten + done * 3 * tc.R * ctx.n, tc, (int)ctx.n);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(k, grid, kThreads, 0, stream, ext + done * 4 * tc.R * ctx.n, ten + done * 3 * tc.R * ctx.n, tc, (int)ctx.n);
+    });
 }
 
 cudaError_t launch_tensor_sum(const Context &ctx, const u64 *ext, u64 *ten, int64_t pairs, int64_t groups,
@@ -509,15 +501,11 @@ cudaError_t launch_tensor_sum(const Context &ctx, const u64 *ext, u64 *ten, int6
     const u128 cap = (((u128)1) << 127) / per_pair;
     tc.max_pairs = cap < 1 ? 1 : (cap > (u128)0x7fffffffLL ? 0x7fffffffLL : (long long)cap);
     const unsigned gx = (unsigned)((ctx.n / 2 + kThreads - 1) / kThreads);
-    for (int64_t done = 0; done < groups;) {
-        const int64_t chunk = (groups - done) > 65535 ? 65535 : (groups - done);
+    return for_each_part(groups, [&](int64_t done, int64_t chunk) {
         dim3 grid(gx ? gx : 1, (unsigned)tc.R, (unsigned)chunk);
-        ++g_kernel_launches;
-        tensor_sum_kernel<<<grid, kThreads, 0, stream>>>(ext + done * pairs * 4 * tc.R * ctx.n, ten + done * 3 * tc.R * ctx.n,
-                                                         tc, (int)ctx.n, pairs);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(tensor_sum_kernel, grid, kThreads, 0, stream, ext + done * pairs * 4 * tc.R * ctx.n,
+                      ten + done * 3 * tc.R * ctx.n, tc, (int)ctx.n, pairs);
+    });
 }
 
 bool floor_takes_scaled_q(const Context &ctx) { return ctx.L <= 16; }
@@ -527,21 +515,21 @@ cudaError_t launch_floor(const Context &ctx, const u64 *in, u64 *out, int64_t po
     if (polys == 0) return cudaSuccess;
     const FloorConsts &consts = reference_base ? ctx.floor : ctx.floor_mul;
     if (ctx.L <= 16) {
-        auto launch = consts.h_primes ? (q_scaled ? launch_floor_tiles<true, true> : launch_floor_tiles<true, false>)
-                                      : (q_scaled ? launch_floor_tiles<false, true> : launch_floor_tiles<false, false>);
-        return launch(ctx, in, out, polys, consts, stream);
+        auto floor_tiles = consts.h_primes ? (q_scaled ? launch_floor_tiles<true, true> : launch_floor_tiles<true, false>)
+                                           : (q_scaled ? launch_floor_tiles<false, true> : launch_floor_tiles<false, false>);
+        return floor_tiles(ctx, in, out, polys, consts, stream);
     }
     if (q_scaled) return cudaErrorInvalidValue;  // floor_takes_scaled_q
     const int R = 2 * ctx.L + 1;
     while (polys > 0) {
         int64_t slab = polys >= 32768 ? (polys / 32768) * 32768 : polys;
-        ++g_kernel_launches;
-        floor_generic_kernel<<<poly_grid(ctx.n, slab), kThreads, 0, stream>>>(in, out, consts, (int)ctx.n);
+        const cudaError_t e = launch(floor_generic_kernel, poly_grid(ctx.n, slab), kThreads, 0, stream, in, out, consts, (int)ctx.n);
+        if (e != cudaSuccess) return e;
         in += slab * (int64_t)R * ctx.n;
         out += slab * (int64_t)ctx.L * ctx.n;
         polys -= slab;
     }
-    return cudaGetLastError();
+    return cudaSuccess;
 }
 
 }  // namespace hecuda

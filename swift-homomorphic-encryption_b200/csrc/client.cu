@@ -203,20 +203,6 @@ struct Streams {
     }
 };
 
-// launch `body(first, part)` over [0, count) in parts of at most 65535 (grid y)
-template <class F>
-cudaError_t over_grid_y(int64_t count, F body) {
-    for (int64_t done = 0; done < count;) {
-        const int64_t part = std::min<int64_t>(count - done, 65535);
-        ++g_kernel_launches;
-        body(done, part);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-        done += part;
-    }
-    return cudaSuccess;
-}
-
 // Device buffers of one call, on one stream; the ones marked secret are zeroized before they are freed.
 struct Allocs {
     cudaStream_t s;
@@ -272,18 +258,18 @@ cudaError_t encrypt_device(const Context &c, const u64 *d_sk, const u64 *d_pt, c
     if (e == cudaSuccess) e = es.make(d_e_seeds, segments_for(8LL * words * n), batch, s);
     const unsigned gx = (unsigned)((L * (long long)n + kThreads - 1) / kThreads), gn = (unsigned)((n + kThreads - 1) / kThreads);
     if (e == cudaSuccess)
-        e = over_grid_y(batch, [&](int64_t first, int64_t part) {
-            uniform_times_secret_kernel<<<dim3(gx, (unsigned)part), kThreads, 0, s>>>(
-                as.rk + (size_t)first * as.segments * kRoundKeyWords, as.ctr + (size_t)first * as.segments * 2, as.segments, tb, rc,
-                d_sk, d_c0 + (size_t)first * L * n, d_c1 + (size_t)first * L * n, n);
+        e = for_each_part(batch, [&](int64_t first, int64_t part) {
+            return launch(uniform_times_secret_kernel, dim3(gx, (unsigned)part), kThreads, 0, s,
+                          as.rk + (size_t)first * as.segments * kRoundKeyWords, as.ctr + (size_t)first * as.segments * 2,
+                          as.segments, tb, rc, d_sk, d_c0 + (size_t)first * L * n, d_c1 + (size_t)first * L * n, n);
         });
     // c0 and c1 are adjacent: one inverse NTT over both (c0 alone when only poly0 is wanted)
     if (e == cudaSuccess) e = launch_ntt_inverse(c, map, d_c0, d_c0, batch * L * (c1_coeff ? 2 : 1), kScalePlain, s);
     if (e == cudaSuccess)
-        e = over_grid_y(batch, [&](int64_t first, int64_t part) {
-            encrypt_epilogue_kernel<<<dim3(gn, (unsigned)part), kThreads, 0, s>>>(
-                es.rk + (size_t)first * es.segments * kRoundKeyWords, es.ctr + (size_t)first * es.segments * 2, es.segments, tb,
-                c.translate[L], words, mask, d_pt + (size_t)first * n, d_c0 + (size_t)first * L * n, n);
+        e = for_each_part(batch, [&](int64_t first, int64_t part) {
+            return launch(encrypt_epilogue_kernel, dim3(gn, (unsigned)part), kThreads, 0, s,
+                          es.rk + (size_t)first * es.segments * kRoundKeyWords, es.ctr + (size_t)first * es.segments * 2,
+                          es.segments, tb, c.translate[L], words, mask, d_pt + (size_t)first * n, d_c0 + (size_t)first * L * n, n);
         });
     return e;
 }
@@ -388,10 +374,10 @@ int32_t hecuda_bfv_generate_secret_key(const hecuda_context *h, const uint8_t *s
         Streams st;
         if (e == cudaSuccess) e = st.make(d_seeds, segments_for((long long)kTernaryBytes * n), count, s);
         if (e == cudaSuccess)
-            e = over_grid_y(count, [&](int64_t first, int64_t part) {
-                ternary_kernel<<<dim3((unsigned)((n + kThreads - 1) / kThreads), (unsigned)part), kThreads, 0, s>>>(
-                    st.rk + (size_t)first * st.segments * kRoundKeyWords, st.ctr + (size_t)first * st.segments * 2, st.segments, tb,
-                    rcs, d_sk + (size_t)first * rows * n, n);
+            e = for_each_part(count, [&](int64_t first, int64_t part) {
+                return launch(ternary_kernel, dim3((unsigned)((n + kThreads - 1) / kThreads), (unsigned)part), kThreads, 0, s,
+                              st.rk + (size_t)first * st.segments * kRoundKeyWords, st.ctr + (size_t)first * st.segments * 2,
+                              st.segments, tb, rcs, d_sk + (size_t)first * rows * n, n);
             });
         if (e == cudaSuccess) e = launch_ntt_forward(c, map, d_sk, d_sk, count * rows, s);
         if (e == cudaSuccess) e = cudaMemcpyAsync(secret_keys, d_sk, words * sizeof(u64), cudaMemcpyDeviceToHost, s);
@@ -474,9 +460,7 @@ int32_t hecuda_evk_generate(const hecuda_context *h, const uint64_t *secret_key,
             // currentKey of every key: s * s (generateRelinearizationKey, :58-65), s.applyGalois(element:) (:40-44)
             u64 *cur = d_cur;
             if (e == cudaSuccess && has_relin) {
-                ++g_kernel_launches;
-                square_kernel<<<(unsigned)((key_words + kThreads - 1) / kThreads), kThreads, 0, s>>>(d_sk, cur, rcs, n);
-                e = cudaGetLastError();
+                e = launch(square_kernel, (unsigned)((key_words + kThreads - 1) / kThreads), kThreads, 0, s, d_sk, cur, rcs, n);
                 cur += key_words;
             }
             for (int32_t j = 0; e == cudaSuccess && j < element_count; ++j, cur += key_words)
@@ -490,19 +474,20 @@ int32_t hecuda_evk_generate(const hecuda_context *h, const uint64_t *secret_key,
                 Streams es;
                 if (e == cudaSuccess) e = es.make(d_es, segments_for(8LL * words * n), count, s);
                 if (e == cudaSuccess)
-                    e = over_grid_y(count, [&](int64_t first, int64_t part) {
-                        cbd_kernel<<<dim3((unsigned)((n + kThreads - 1) / kThreads), (unsigned)part), kThreads, 0, s>>>(
-                            es.rk + (size_t)first * es.segments * kRoundKeyWords, es.ctr + (size_t)first * es.segments * 2, es.segments,
-                            tb, rcs, words, mask, d_e + key_words * first, n);
+                    e = for_each_part(count, [&](int64_t first, int64_t part) {
+                        return launch(cbd_kernel, dim3((unsigned)((n + kThreads - 1) / kThreads), (unsigned)part), kThreads, 0, s,
+                                      es.rk + (size_t)first * es.segments * kRoundKeyWords,
+                                      es.ctr + (size_t)first * es.segments * 2, es.segments, tb, rcs, words, mask,
+                                      d_e + key_words * first, n);
                     });
             }
             if (e == cudaSuccess) e = launch_ntt_forward(c, map, d_e, d_e, count * K, s);
             Streams as;
             if (e == cudaSuccess) e = as.make(d_as, segments_for(16LL * K * n), count, s);
             if (e == cudaSuccess)
-                e = over_grid_y(count, [&](int64_t first, int64_t part) {
-                    key_switch_key_kernel<<<dim3((unsigned)((key_words + kThreads - 1) / kThreads), (unsigned)part), kThreads, 0, s>>>(
-                        as.rk, as.ctr, as.segments, tb, rcs, c.L, d_sk, d_cur, d_e, d_dst, n, first);
+                e = for_each_part(count, [&](int64_t first, int64_t part) {
+                    return launch(key_switch_key_kernel, dim3((unsigned)((key_words + kThreads - 1) / kThreads), (unsigned)part),
+                                  kThreads, 0, s, as.rk, as.ctr, as.segments, tb, rcs, c.L, d_sk, d_cur, d_e, d_dst, n, first);
                 });
             if (e == cudaSuccess && wire_poly0) {
                 const size_t b = (size_t)serialized_poly_bytes(cc);

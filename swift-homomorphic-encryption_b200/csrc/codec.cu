@@ -75,16 +75,12 @@ long long serialized_poly_bytes(const CodecConsts &c) { return c.byte_offset[c.r
 
 cudaError_t launch_poly_load(const Context &ctx, const CodecConsts &c, int skip, const unsigned char *bytes, u64 *out,
                              int64_t polys, cudaStream_t stream) {
-    const int threads = ctx.n >= 256 ? 256 : (ctx.n < 32 ? 32 : (int)ctx.n);
-    for (int64_t done = 0; done < polys;) {
-        const int64_t chunk = (polys - done) > 65535 ? 65535 : (polys - done);
+    const int threads = coeff_threads(ctx.n);
+    return for_each_part(polys, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((ctx.n + threads - 1) / threads), (unsigned)c.rows, (unsigned)chunk);
-        ++g_kernel_launches;
-        poly_load_kernel<<<grid, threads, 0, stream>>>(bytes + done * c.byte_offset[c.rows], out + done * c.rows * ctx.n, c,
-                                                       (int)ctx.n, skip);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(poly_load_kernel, grid, threads, 0, stream, bytes + done * c.byte_offset[c.rows],
+                      out + done * c.rows * ctx.n, c, (int)ctx.n, skip);
+    });
 }
 
 // coefficients -> bytes, 8 output bytes per thread (rows whose byte count and offset are multiples of 8: N >= 64)
@@ -121,21 +117,11 @@ cudaError_t launch_poly_serialize(const Context &ctx, const CodecConsts &c, int 
         widest = std::max(widest, c.byte_offset[r + 1] - c.byte_offset[r]);
         words = words && (c.byte_offset[r] & 7) == 0 && (c.byte_offset[r + 1] & 7) == 0;
     }
-    for (int64_t done = 0; done < polys;) {
-        const int64_t chunk = (polys - done) > 65535 ? 65535 : (polys - done);
-        ++g_kernel_launches;
-        if (words) {
-            dim3 grid((unsigned)((widest / 8 + 255) / 256), (unsigned)c.rows, (unsigned)chunk);
-            poly_serialize_words_kernel<<<grid, 256, 0, stream>>>(in + done * c.rows * ctx.n, bytes + done * c.byte_offset[c.rows],
-                                                                  c, (int)ctx.n, skip);
-        } else {
-            dim3 grid((unsigned)((widest + 255) / 256), (unsigned)c.rows, (unsigned)chunk);
-            poly_serialize_kernel<<<grid, 256, 0, stream>>>(in + done * c.rows * ctx.n, bytes + done * c.byte_offset[c.rows], c,
-                                                            (int)ctx.n, skip);
-        }
-        done += chunk;
-    }
-    return cudaGetLastError();
+    return for_each_part(polys, [&](int64_t done, int64_t chunk) {
+        dim3 grid((unsigned)(((words ? widest / 8 : widest) + 255) / 256), (unsigned)c.rows, (unsigned)chunk);
+        return launch(words ? poly_serialize_words_kernel : poly_serialize_kernel, grid, 256, 0, stream,
+                      in + done * c.rows * ctx.n, bytes + done * c.byte_offset[c.rows], c, (int)ctx.n, skip);
+    });
 }
 
 }  // namespace hecuda

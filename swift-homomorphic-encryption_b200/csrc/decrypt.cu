@@ -104,24 +104,18 @@ cudaError_t decrypt_chunk(const Context &c, const DecryptConsts &dc, u64 *scratc
     const NttRowMap map = c.map_q(l);
     cudaError_t e;
     if ((e = launch_ntt_forward(c, map, ct, ev, items * polys * l, s)) != cudaSuccess) return e;
-    const int threads = n >= 256 ? 256 : (n < 32 ? 32 : (int)n);
+    const int threads = coeff_threads(n);
     const unsigned gx = (unsigned)((n + threads - 1) / threads);
-    for (int64_t done = 0; done < items;) {
-        const int64_t part = std::min<int64_t>(items - done, 65535);
-        ++g_kernel_launches;
-        dot_secret_kernel<<<dim3(gx, (unsigned)l, (unsigned)part), threads, 0, s>>>(ev + done * polys * l * n, sk,
-                                                                                   dot + done * l * n, dc, (int)n, polys);
-        done += part;
-    }
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    e = for_each_part(items, [&](int64_t done, int64_t part) {
+        return launch(dot_secret_kernel, dim3(gx, (unsigned)l, (unsigned)part), threads, 0, s, ev + done * polys * l * n, sk,
+                      dot + done * l * n, dc, (int)n, polys);
+    });
+    if (e != cudaSuccess) return e;
     if ((e = launch_ntt_inverse(c, map, dot, dot, items * l, kScalePlain, s)) != cudaSuccess) return e;
-    for (int64_t done = 0; done < items;) {
-        const int64_t part = std::min<int64_t>(items - done, 65535);
-        ++g_kernel_launches;
-        scale_and_round_kernel<<<dim3(gx, (unsigned)part), threads, 0, s>>>(dot + done * l * n, out + done * n, dc, (int)n);
-        done += part;
-    }
-    return cudaGetLastError();
+    return for_each_part(items, [&](int64_t done, int64_t part) {
+        return launch(scale_and_round_kernel, dim3(gx, (unsigned)part), threads, 0, s, dot + done * l * n, out + done * n, dc,
+                      (int)n);
+    });
 }
 
 // ---------------------------------------------------------------- noise budget
@@ -352,7 +346,7 @@ int32_t hecuda_bfv_noise_budget(const hecuda_context *h, const uint64_t *secret_
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_sk, secret_key, (size_t)l * n * sizeof(u64), cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_big, big.data(), big.size() * sizeof(u64), cudaMemcpyHostToDevice, s);
     const NttRowMap map = c.map_q(l);
-    const int threads = n >= 256 ? 256 : (n < 32 ? 32 : (int)n);
+    const int threads = coeff_threads(n);
     const unsigned gx = (unsigned)((n + threads - 1) / threads);
     for (int64_t done = 0; e == cudaSuccess && done < batch; done += cap) {
         const int64_t items = std::min<int64_t>(cap, batch - done);
@@ -362,20 +356,13 @@ int32_t hecuda_bfv_noise_budget(const hecuda_context *h, const uint64_t *secret_
             e = launch_ntt_forward(c, map, d_in, d_ev, items * polys * l, s);
             ev = d_ev;
         }
-        for (int64_t first = 0; e == cudaSuccess && first < items;) {
-            const int64_t part = std::min<int64_t>(items - first, 65535);
-            ++g_kernel_launches;
-            dot_secret_kernel<<<dim3(gx, (unsigned)l, (unsigned)part), threads, 0, s>>>(ev + first * polys * l * n, d_sk,
-                                                                                       d_dot + first * l * n, dc, (int)n, polys);
-            e = cudaGetLastError();
-            first += part;
-        }
+        if (e == cudaSuccess)
+            e = for_each_part(items, [&](int64_t first, int64_t part) {
+                return launch(dot_secret_kernel, dim3(gx, (unsigned)l, (unsigned)part), threads, 0, s,
+                              ev + first * polys * l * n, d_sk, d_dot + first * l * n, dc, (int)n, polys);
+            });
         if (e == cudaSuccess) e = launch_ntt_inverse(c, map, d_dot, d_dot, items * l, kScalePlain, s);
-        if (e == cudaSuccess) {
-            ++g_kernel_launches;
-            noise_norm_kernel<<<(unsigned)items, kNormThreads, 0, s>>>(d_dot, d_big, nc, (int)n, d_norm);
-            e = cudaGetLastError();
-        }
+        if (e == cudaSuccess) e = launch(noise_norm_kernel, (unsigned)items, kNormThreads, 0, s, d_dot, d_big, nc, (int)n, d_norm);
         if (e == cudaSuccess)
             e = cudaMemcpyAsync(norms.data() + (size_t)l * done, d_norm, (size_t)l * items * sizeof(u64), cudaMemcpyDeviceToHost, s);
     }

@@ -14,8 +14,6 @@
 // kernel that also unpacks poly0 and writes both polys into the key buffers.
 // AES is FIPS-197 written from the specification (S-box, ShiftRows, MixColumns over GF(2^8)); the reference gets it
 // from swift-crypto.  Pinned by the reference's NIST vectors through the oracle (tests/test_oracle_drbg.py).
-#include <algorithm>
-
 #include "capi_internal.hpp"
 #include "drbg.cuh"
 #include "modarith.cuh"
@@ -77,15 +75,10 @@ __global__ void __launch_bounds__(64) drbg_chain_kernel(const unsigned char *__r
     }
 }
 
-struct FillConsts {
-    int rows;
-    u64 p[kMaxRows];
-};
-
 // one CTA per segment, one thread per 16-byte block = per coefficient (randomizeUniform, PolyRq+Randomize.swift:58-80)
 __global__ void __launch_bounds__(kSegmentBlocks) drbg_fill_kernel(const u32w *__restrict__ round_keys,
                                                                    const u64 *__restrict__ counters, u64 *__restrict__ out,
-                                                                   const __grid_constant__ FillConsts c, int n, int segments) {
+                                                                   const __grid_constant__ RowModuli c, int n, int segments) {
     __shared__ unsigned char sbox[256];
     __shared__ u32w te0[256];
     __shared__ u32w rk[kRoundKeyWords];
@@ -113,7 +106,7 @@ __global__ void __launch_bounds__(kSegmentBlocks) drbg_fill_kernel(const u32w *_
 __global__ void __launch_bounds__(kSegmentBlocks) key_expand_kernel(const u32w *__restrict__ round_keys,
                                                                     const u64 *__restrict__ counters,
                                                                     const unsigned char *__restrict__ poly0,
-                                                                    u64 *const *__restrict__ dst, const __grid_constant__ FillConsts c,
+                                                                    u64 *const *__restrict__ dst, const __grid_constant__ RowModuli c,
                                                                     const __grid_constant__ CodecConsts cc, int n, int segments) {
     __shared__ unsigned char sbox[256];
     __shared__ u32w te0[256];
@@ -155,11 +148,7 @@ cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batc
     if (e != cudaSuccess) return e;
     e = cudaMallocAsync((void **)d_rk, (size_t)batch * segments * kRoundKeyWords * sizeof(u32w), s);
     if (e == cudaSuccess) e = cudaMallocAsync((void **)d_ctr, (size_t)batch * segments * 2 * sizeof(u64), s);
-    if (e == cudaSuccess) {
-        ++g_kernel_launches;
-        drbg_chain_kernel<<<(unsigned)((batch + 31) / 32), 64, 0, s>>>(d_seeds, *d_rk, *d_ctr, segments, batch);
-        e = cudaGetLastError();
-    }
+    if (e == cudaSuccess) e = launch(drbg_chain_kernel, (unsigned)((batch + 31) / 32), 64, 0, s, d_seeds, *d_rk, *d_ctr, segments, batch);
     return e;
 }
 
@@ -188,18 +177,13 @@ cudaError_t random_polys_device(const Context &c, int l, const unsigned char *d_
     u32w *d_rk = nullptr;
     u64 *d_ctr = nullptr;
     cudaError_t e = drbg_chains(d_seeds, segments, batch, &d_rk, &d_ctr, s);
-    FillConsts fc;
-    fc.rows = l;
-    for (int r = 0; r < l; ++r) fc.p[r] = c.slots[c.slot_q(r)].dev.p;
-    for (int64_t done = 0; e == cudaSuccess && done < batch;) {
-        const int64_t part = std::min<int64_t>(batch - done, 65535);
-        ++g_kernel_launches;
-        drbg_fill_kernel<<<dim3((unsigned)segments, (unsigned)part), kSegmentBlocks, 0, s>>>(
-            d_rk + (size_t)done * segments * kRoundKeyWords, d_ctr + (size_t)done * segments * 2, d_out + (size_t)done * l * c.n, fc,
-            (int)c.n, segments);
-        e = cudaGetLastError();
-        done += part;
-    }
+    const RowModuli fc = row_moduli(c, c.map_q(l));
+    if (e == cudaSuccess)
+        e = for_each_part(batch, [&](int64_t done, int64_t part) {
+            return launch(drbg_fill_kernel, dim3((unsigned)segments, (unsigned)part), kSegmentBlocks, 0, s,
+                          d_rk + (size_t)done * segments * kRoundKeyWords, d_ctr + (size_t)done * segments * 2,
+                          d_out + (size_t)done * l * c.n, fc, (int)c.n, segments);
+        });
     free_chains(d_rk, d_ctr, segments, batch, s);
     return e;
 }
@@ -250,18 +234,13 @@ cudaError_t expand_seeded_keys_device(const Context &c, const unsigned char *d_p
     u32w *d_rk = nullptr;
     u64 *d_ctr = nullptr;
     cudaError_t e = drbg_chains(d_seeds, segments, count, &d_rk, &d_ctr, s);
-    FillConsts fc;
-    fc.rows = rows;
-    for (int r = 0; r < rows; ++r) fc.p[r] = c.slots[map.slot[r]].dev.p;
-    for (int64_t done = 0; e == cudaSuccess && done < count;) {
-        const int64_t part = std::min<int64_t>(count - done, 65535);
-        ++g_kernel_launches;
-        key_expand_kernel<<<dim3((unsigned)segments, (unsigned)part), kSegmentBlocks, 0, s>>>(
-            d_rk + (size_t)done * segments * kRoundKeyWords, d_ctr + (size_t)done * segments * 2,
-            d_poly0 + (size_t)done * serialized_poly_bytes(cc), d_dst + done, fc, cc, (int)c.n, segments);
-        e = cudaGetLastError();
-        done += part;
-    }
+    const RowModuli fc = row_moduli(c, map);
+    if (e == cudaSuccess)
+        e = for_each_part(count, [&](int64_t done, int64_t part) {
+            return launch(key_expand_kernel, dim3((unsigned)segments, (unsigned)part), kSegmentBlocks, 0, s,
+                          d_rk + (size_t)done * segments * kRoundKeyWords, d_ctr + (size_t)done * segments * 2,
+                          d_poly0 + (size_t)done * serialized_poly_bytes(cc), d_dst + done, fc, cc, (int)c.n, segments);
+        });
     free_chains(d_rk, d_ctr, segments, count, s);
     return e;
 }

@@ -65,24 +65,18 @@ cudaError_t launch_elementwise(const Context &ctx, const NttRowMap &map, int op,
         c.mu_lo[r] = S.mu_lo;
         c.scalar[r] = scalars ? scalars[r] : 0;
     }
-    const int threads = ctx.n >= 512 ? 256 : (ctx.n < 64 ? 32 : (int)(ctx.n / 2));
+    const int threads = coeff_threads(ctx.n / 2);
     const unsigned gx = (unsigned)(((ctx.n + 1) / 2 + threads - 1) / threads);
-    for (int64_t done = 0; done < polys;) {
-        const int64_t chunk = std::min<int64_t>(polys - done, 65535);
+    auto kernel = op == kAdd ? elementwise_kernel<kAdd>
+                : op == kSub ? elementwise_kernel<kSub>
+                : op == kMul ? elementwise_kernel<kMul>
+                : op == kNeg ? elementwise_kernel<kNeg>
+                             : elementwise_kernel<kScalar>;
+    return for_each_part(polys, [&](int64_t done, int64_t chunk) {
         dim3 grid(gx, (unsigned)c.rows, (unsigned)chunk);
-        u64 *l = lhs + done * c.rows * ctx.n;
-        const u64 *r = rhs ? rhs + done * c.rows * ctx.n : nullptr;
-        ++g_kernel_launches;
-        switch (op) {
-            case kAdd: elementwise_kernel<kAdd><<<grid, threads, 0, s>>>(l, r, c, (int)ctx.n); break;
-            case kSub: elementwise_kernel<kSub><<<grid, threads, 0, s>>>(l, r, c, (int)ctx.n); break;
-            case kMul: elementwise_kernel<kMul><<<grid, threads, 0, s>>>(l, r, c, (int)ctx.n); break;
-            case kNeg: elementwise_kernel<kNeg><<<grid, threads, 0, s>>>(l, r, c, (int)ctx.n); break;
-            default: elementwise_kernel<kScalar><<<grid, threads, 0, s>>>(l, r, c, (int)ctx.n); break;
-        }
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(kernel, grid, threads, 0, s, lhs + done * c.rows * ctx.n, rhs ? rhs + done * c.rows * ctx.n : nullptr, c,
+                      (int)ctx.n);
+    });
 }
 
 int32_t run(const hecuda_context *h, int32_t base, int op, uint64_t *lhs, const uint64_t *rhs, const uint64_t *scalars,
@@ -194,15 +188,11 @@ __global__ void __launch_bounds__(256) narrow_kernel(const u64 *__restrict__ in,
 }
 cudaError_t launch_widen(const u32 *in, u64 *out, int64_t words, cudaStream_t stream) {
     if (words == 0) return cudaSuccess;
-    ++g_kernel_launches;
-    widen_kernel<<<(unsigned)((words + 1023) / 1024), 256, 0, stream>>>(in, out, words);
-    return cudaGetLastError();
+    return launch(widen_kernel, (unsigned)((words + 1023) / 1024), 256, 0, stream, in, out, words);
 }
 cudaError_t launch_narrow(const u64 *in, u32 *out, int64_t words, cudaStream_t stream) {
     if (words == 0) return cudaSuccess;
-    ++g_kernel_launches;
-    narrow_kernel<<<(unsigned)((words + 1023) / 1024), 256, 0, stream>>>(in, out, words);
-    return cudaGetLastError();
+    return launch(narrow_kernel, (unsigned)((words + 1023) / 1024), 256, 0, stream, in, out, words);
 }
 
 }  // namespace hecuda

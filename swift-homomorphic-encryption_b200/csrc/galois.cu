@@ -9,14 +9,9 @@
 
 namespace hecuda {
 
-struct GaloisConsts {
-    int rows;
-    u64 p[kMaxRows];
-};
-
 __global__ void __launch_bounds__(256) galois_coeff_kernel(const u64 *__restrict__ in, int64_t in_poly_stride,
                                                           u64 *__restrict__ out, int64_t out_poly_stride,
-                                                          const __grid_constant__ GaloisConsts c, int logn,
+                                                          const __grid_constant__ RowModuli c, int logn,
                                                           unsigned g_inv) {
     const int n = 1 << logn;
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -44,7 +39,7 @@ __global__ void __launch_bounds__(256) galois_eval_kernel(const u64 *__restrict_
 
 // PolyRq<Coeff>.multiplyPowerOfX (PolyRq.swift:398-422) as a gather: out[c] = +-in[(c - s) mod N], s = power mod 2N
 __global__ void __launch_bounds__(256) monomial_kernel(const u64 *__restrict__ in, u64 *__restrict__ out,
-                                                      const __grid_constant__ GaloisConsts c, int logn, unsigned s) {
+                                                      const __grid_constant__ RowModuli c, int logn, unsigned s) {
     const int n = 1 << logn;
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n) return;
@@ -58,22 +53,16 @@ __global__ void __launch_bounds__(256) monomial_kernel(const u64 *__restrict__ i
 cudaError_t launch_multiply_power_of_x(const Context &ctx, const NttRowMap &map, long long power, const u64 *in, u64 *out,
                                        int64_t polys, cudaStream_t stream) {
     if (polys == 0) return cudaSuccess;
-    GaloisConsts c;
-    c.rows = map.rows_per_poly;
-    for (int r = 0; r < c.rows; ++r) c.p[r] = ctx.slots[map.slot[r]].dev.p;
+    const RowModuli c = row_moduli(ctx, map);
     const long long two_n = 2 * ctx.n;
     long long s = power % two_n;
     if (s < 0) s += two_n;
-    const int threads = ctx.n >= 256 ? 256 : (ctx.n < 32 ? 32 : (int)ctx.n);
-    for (int64_t done = 0; done < polys;) {
-        const int64_t chunk = (polys - done) > 65535 ? 65535 : (polys - done);
+    const int threads = coeff_threads(ctx.n);
+    return for_each_part(polys, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((ctx.n + threads - 1) / threads), (unsigned)c.rows, (unsigned)chunk);
-        ++g_kernel_launches;
-        monomial_kernel<<<grid, threads, 0, stream>>>(in + done * c.rows * ctx.n, out + done * c.rows * ctx.n, c, ctx.logn,
-                                                      (unsigned)s);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(monomial_kernel, grid, threads, 0, stream, in + done * c.rows * ctx.n, out + done * c.rows * ctx.n, c,
+                      ctx.logn, (unsigned)s);
+    });
 }
 
 static unsigned inverse_mod_pow2(unsigned g, unsigned two_n) {  // g odd
@@ -86,35 +75,25 @@ cudaError_t launch_galois_coeff(const Context &ctx, const NttRowMap &map, unsign
                                 int64_t in_poly_stride, u64 *out, int64_t out_poly_stride, int64_t polys,
                                 cudaStream_t stream) {
     if (polys == 0) return cudaSuccess;
-    GaloisConsts c;
-    c.rows = map.rows_per_poly;
-    for (int r = 0; r < c.rows; ++r) c.p[r] = ctx.slots[map.slot[r]].dev.p;
+    const RowModuli c = row_moduli(ctx, map);
     const unsigned g_inv = inverse_mod_pow2(element, 2u * (unsigned)ctx.n);
-    const int threads = ctx.n >= 256 ? 256 : (ctx.n < 32 ? 32 : (int)ctx.n);
-    for (int64_t done = 0; done < polys;) {
-        const int64_t chunk = (polys - done) > 65535 ? 65535 : (polys - done);
+    const int threads = coeff_threads(ctx.n);
+    return for_each_part(polys, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((ctx.n + threads - 1) / threads), (unsigned)c.rows, (unsigned)chunk);
-        ++g_kernel_launches;
-        galois_coeff_kernel<<<grid, threads, 0, stream>>>(in + done * in_poly_stride, in_poly_stride,
-                                                          out + done * out_poly_stride, out_poly_stride, c, ctx.logn, g_inv);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(galois_coeff_kernel, grid, threads, 0, stream, in + done * in_poly_stride, in_poly_stride,
+                      out + done * out_poly_stride, out_poly_stride, c, ctx.logn, g_inv);
+    });
 }
 
 cudaError_t launch_galois_eval(const Context &ctx, int rows, unsigned element, const u64 *in, u64 *out, int64_t polys,
                                cudaStream_t stream) {
     if (polys == 0) return cudaSuccess;
-    const int threads = ctx.n >= 256 ? 256 : (ctx.n < 32 ? 32 : (int)ctx.n);
-    for (int64_t done = 0; done < polys;) {
-        const int64_t chunk = (polys - done) > 65535 ? 65535 : (polys - done);
+    const int threads = coeff_threads(ctx.n);
+    return for_each_part(polys, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((ctx.n + threads - 1) / threads), (unsigned)rows, (unsigned)chunk);
-        ++g_kernel_launches;
-        galois_eval_kernel<<<grid, threads, 0, stream>>>(in + done * rows * ctx.n, out + done * rows * ctx.n, rows, ctx.logn,
-                                                         element);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(galois_eval_kernel, grid, threads, 0, stream, in + done * rows * ctx.n, out + done * rows * ctx.n, rows,
+                      ctx.logn, element);
+    });
 }
 
 }  // namespace hecuda

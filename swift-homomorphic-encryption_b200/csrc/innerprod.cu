@@ -105,17 +105,13 @@ cudaError_t launch_inner_product_plain(const Context &ctx, const u64 *cts, int n
         {inner_product_plain_kernel<1, false>, inner_product_plain_kernel<1, true>},
         {inner_product_plain_kernel<2, false>, inner_product_plain_kernel<2, true>},
         {inner_product_plain_kernel<3, false>, inner_product_plain_kernel<3, true>}};
-    for (int64_t done = 0; done < out_count;) {
-        const int64_t chunk = (out_count - done) > 65535 ? 65535 : (out_count - done);
+    return for_each_part(out_count, [&](int64_t done, int64_t chunk) {
         dim3 grid(gx ? gx : 1, (unsigned)l, (unsigned)chunk);
         const u64 *pt = pts + done * terms * l * ctx.n;
         const unsigned char *pr = present ? present + done * terms : nullptr;
         u64 *o = out + done * npoly * l * ctx.n;
-        ++g_kernel_launches;
-        kernels[npoly - 1][pr != nullptr]<<<grid, 128, 0, stream>>>(cts, pt, pr, o, c, (int)ctx.n, terms);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(kernels[npoly - 1][pr != nullptr], grid, 128, 0, stream, cts, pt, pr, o, c, (int)ctx.n, terms);
+    });
 }
 
 // ---- the same scan for moduli below 2^31 (the reference's default PIR parameters, 27 / 28 / 28 bits): the database
@@ -213,17 +209,13 @@ cudaError_t launch_inner_product_plain_small(const Context &ctx, const u64 *cts,
         {inner_product_plain_small_kernel<1, false>, inner_product_plain_small_kernel<1, true>},
         {inner_product_plain_small_kernel<2, false>, inner_product_plain_small_kernel<2, true>},
         {inner_product_plain_small_kernel<3, false>, inner_product_plain_small_kernel<3, true>}};
-    for (int64_t done = 0; done < out_count;) {
-        const int64_t chunk = (out_count - done) > 65535 ? 65535 : (out_count - done);
+    return for_each_part(out_count, [&](int64_t done, int64_t chunk) {
         dim3 grid(gx ? gx : 1, (unsigned)l, (unsigned)chunk);
         const u32 *pt = pts + done * terms * l * ctx.n;
         const unsigned char *pr = present ? present + done * terms : nullptr;
         u64 *o = out + done * npoly * l * ctx.n;
-        ++g_kernel_launches;
-        kernels[npoly - 1][pr != nullptr]<<<grid, 128, 0, stream>>>(cts, pt, pr, o, c, (int)ctx.n, terms);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(kernels[npoly - 1][pr != nullptr], grid, 128, 0, stream, cts, pt, pr, o, c, (int)ctx.n, terms);
+    });
 }
 
 // ---- both scans for several clients' 2-poly queries against the same database rows (hecuda_mulpir_compute_response_
@@ -395,25 +387,18 @@ cudaError_t launch_inner_product_plain_clients(const Context &ctx, const u64 *ct
     const unsigned tiles = (unsigned)((clients + kScanClientTile - 1) / kScanClientTile);
     const unsigned gx = (unsigned)coeff_blocks * tiles;
     const int block = 64;
-    const int64_t max_rows = (int64_t)65535 * kScanRowTile;
-    for (int64_t done = 0; done < out_count;) {
-        const int64_t rows = (out_count - done) > max_rows ? max_rows : (out_count - done);
+    return for_each_part(out_count, [&](int64_t done, int64_t rows) {  // grid z counts row tiles
         dim3 grid(gx ? gx : 1, (unsigned)l, (unsigned)((rows + kScanRowTile - 1) / kScanRowTile));
         const unsigned char *pr = present ? present + done * terms : nullptr;
         u64 *o = out + done * 2 * l * ctx.n;
-        ++g_kernel_launches;
-        if (pts32) {
-            const u32 *pt = pts32 + done * terms * l * ctx.n;
-            (pr ? inner_product_plain_small_clients_kernel<true> : inner_product_plain_small_clients_kernel<false>)
-                <<<grid, block, 0, stream>>>(cts, client_stride, clients, pt, pr, o, out_client_stride, rows, cs, (int)ctx.n, terms);
-        } else {
-            const u64 *pt = pts + done * terms * l * ctx.n;
-            (pr ? inner_product_plain_clients_kernel<true> : inner_product_plain_clients_kernel<false>)
-                <<<grid, block, 0, stream>>>(cts, client_stride, clients, pt, pr, o, out_client_stride, rows, cw, (int)ctx.n, terms);
-        }
-        done += rows;
-    }
-    return cudaGetLastError();
+        if (pts32)
+            return launch(pr ? inner_product_plain_small_clients_kernel<true> : inner_product_plain_small_clients_kernel<false>,
+                          grid, block, 0, stream, cts, client_stride, clients, pts32 + done * terms * l * ctx.n, pr, o,
+                          out_client_stride, rows, cs, (int)ctx.n, terms);
+        return launch(pr ? inner_product_plain_clients_kernel<true> : inner_product_plain_clients_kernel<false>, grid, block, 0,
+                      stream, cts, client_stride, clients, pts + done * terms * l * ctx.n, pr, o, out_client_stride, rows, cw,
+                      (int)ctx.n, terms);
+    }, kMaxGridYZ * kScanRowTile);
 }
 
 // Plaintext.convertToEvalFormat, Plaintext.swift:149-171: centered lift mod each q_r (the forward NTT follows)
@@ -436,15 +421,12 @@ cudaError_t launch_plaintext_to_eval(const Context &ctx, const u64 *plain, int l
     c.l = l;
     c.max_terms = 0;
     for (int r = 0; r < l; ++r) c.p[r] = ctx.slots[ctx.slot_q(r)].dev.p;
-    const int threads = ctx.n >= 256 ? 256 : (ctx.n < 32 ? 32 : (int)ctx.n);
-    for (int64_t done = 0; done < count;) {
-        const int64_t chunk = (count - done) > 65535 ? 65535 : (count - done);
+    const int threads = coeff_threads(ctx.n);
+    cudaError_t e = for_each_part(count, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((ctx.n + threads - 1) / threads), (unsigned)l, (unsigned)chunk);
-        ++g_kernel_launches;
-        plaintext_lift_kernel<<<grid, threads, 0, stream>>>(plain + done * ctx.n, out + done * l * ctx.n, c, ctx.t, (int)ctx.n);
-        done += chunk;
-    }
-    cudaError_t e = cudaGetLastError();
+        return launch(plaintext_lift_kernel, grid, threads, 0, stream, plain + done * ctx.n, out + done * l * ctx.n, c, ctx.t,
+                      (int)ctx.n);
+    });
     if (e != cudaSuccess) return e;
     return launch_ntt_forward(ctx, ctx.map_q(l), out, out, count * l, stream);
 }

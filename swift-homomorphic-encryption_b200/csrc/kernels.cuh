@@ -2,8 +2,10 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <string>
+#include <utility>
 
 #include "context.hpp"
 #include "process_db.cuh"
@@ -11,6 +13,44 @@
 namespace hecuda {
 
 extern std::atomic<unsigned long long> g_kernel_launches;  // every <<<>>> issued by this library
+
+// ---- launching.  Every kernel outside the NTT files (ntt_simple.cu, ntt_fast.cu/.cuh) is launched through `launch`,
+// so hecuda_kernel_launch_count counts it.
+constexpr int64_t kMaxGridYZ = 65535;  // the largest gridDim.y / gridDim.z
+
+// block size of a kernel with one thread per coefficient of an n-coefficient row: n clamped to 32 .. 256
+inline int coeff_threads(int64_t n) { return n >= 256 ? 256 : (n < 32 ? 32 : (int)n); }
+
+// one counted launch: kernel<<<grid, block, smem, stream>>>(args...), then the launch's error
+template <typename... KArgs, typename... Args>
+cudaError_t launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args &&...args) {
+    ++g_kernel_launches;
+    kernel<<<grid, block, smem, stream>>>(std::forward<Args>(args)...);
+    return cudaGetLastError();
+}
+
+// body(first, part) for consecutive parts [first, first + part) of [0, count), part <= limit, until one returns an
+// error: a batch that a kernel puts in grid y or z is launched in parts of at most kMaxGridYZ
+template <typename Body>
+cudaError_t for_each_part(int64_t count, Body &&body, int64_t limit = kMaxGridYZ) {
+    for (int64_t first = 0; first < count; first += limit) {
+        const cudaError_t e = body(first, std::min(limit, count - first));
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
+// the modulus of each of a polynomial's rows under `map`, for a kernel's parameter block
+struct RowModuli {
+    int rows;
+    u64 p[kMaxRows];
+};
+inline RowModuli row_moduli(const Context &ctx, const NttRowMap &map) {
+    RowModuli m;
+    m.rows = map.rows_per_poly;
+    for (int r = 0; r < m.rows; ++r) m.p[r] = ctx.slots[map.slot[r]].dev.p;
+    return m;
+}
 
 // ---- negacyclic NTT over rows (ntt.cu).  data: rows x N, row r uses slot map.slot[r % map.rows_per_poly].
 // Forward: natural order in -> bit-reversed out (PolyRq+Ntt.swift:237-319); inverse is its inverse (:379-483).

@@ -98,8 +98,6 @@ __global__ void __launch_bounds__(256) mod_switch_kernel(const u64 *__restrict__
     divround_column(in + poly * c.l * n + coeff, nullptr, out + poly * (c.l - 1) * n + coeff, c, n);
 }
 
-static inline int pick_threads(int64_t n) { return n >= 256 ? 256 : (n < 32 ? 32 : (int)n); }
-
 cudaError_t launch_ks_mac(const Context &ctx, const u64 *dig, const u64 *key, int l, u64 *prod, int64_t items,
                           cudaStream_t stream, const KsKeyTable *keys) {
     if (items == 0) return cudaSuccess;
@@ -115,38 +113,27 @@ cudaError_t launch_ks_mac(const Context &ctx, const u64 *dig, const u64 *key, in
     if (keys && keys->items_per_client < 1) return cudaErrorInvalidValue;
     KsKeyTable table = keys ? *keys : KsKeyTable{};
     const unsigned gx = (unsigned)((ctx.n / 2 + 127) / 128);
-    for (int64_t done = 0; done < items;) {
-        const int64_t chunk = (items - done) > 65535 ? 65535 : (items - done);
+    return for_each_part(items, [&](int64_t done, int64_t chunk) {
         dim3 grid(gx ? gx : 1, (unsigned)(l + 1), (unsigned)chunk);
-        ++g_kernel_launches;
         const u64 *d = dig + done * (l + 1) * l * ctx.n;
         u64 *o = prod + done * 2 * (l + 1) * ctx.n;
-        if (keys) {
-            table.item0 = keys->item0 + done;
-            ks_mac_kernel<true><<<grid, 128, 0, stream>>>(d, nullptr, o, c, (int)ctx.n, table);
-        } else {
-            ks_mac_kernel<false><<<grid, 128, 0, stream>>>(d, key, o, c, (int)ctx.n, table);
-        }
-        done += chunk;
-    }
-    return cudaGetLastError();
+        if (!keys) return launch(ks_mac_kernel<false>, grid, 128, 0, stream, d, key, o, c, (int)ctx.n, table);
+        table.item0 = keys->item0 + done;
+        return launch(ks_mac_kernel<true>, grid, 128, 0, stream, d, nullptr, o, c, (int)ctx.n, table);
+    });
 }
 
 cudaError_t launch_ks_finish(const Context &ctx, const u64 *prod, const u64 *base, int64_t base_item_stride, int base_mask,
                              int l, u64 *out, int64_t items, cudaStream_t stream) {
     if (items == 0) return cudaSuccess;
-    const int threads = pick_threads(ctx.n);
+    const int threads = coeff_threads(ctx.n);
     const DivRoundConsts &c = ctx.ks_divround[l];
-    for (int64_t done = 0; done < items;) {
-        const int64_t chunk = (items - done) > 65535 ? 65535 : (items - done);
+    return for_each_part(items, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((ctx.n + threads - 1) / threads), 2, (unsigned)chunk);
-        ++g_kernel_launches;
-        ks_finish_kernel<<<grid, threads, 0, stream>>>(prod + done * 2 * (l + 1) * ctx.n,
-                                                       base ? base + done * base_item_stride : nullptr, base_item_stride, base_mask,
-                                                       out + done * 2 * l * ctx.n, c, ctx.n);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(ks_finish_kernel, grid, threads, 0, stream, prod + done * 2 * (l + 1) * ctx.n,
+                      base ? base + done * base_item_stride : nullptr, base_item_stride, base_mask, out + done * 2 * l * ctx.n,
+                      c, ctx.n);
+    });
 }
 
 cudaError_t launch_mod_switch(const Context &ctx, const u64 *in, int l, u64 *out, int64_t polys, cudaStream_t stream) {
@@ -154,9 +141,7 @@ cudaError_t launch_mod_switch(const Context &ctx, const u64 *in, int l, u64 *out
     if (total == 0) return cudaSuccess;
     if (l < 2 || l > ctx.L) return cudaErrorInvalidValue;
     const unsigned blocks = (unsigned)((total + 255) / 256);
-    ++g_kernel_launches;
-    mod_switch_kernel<<<blocks, 256, 0, stream>>>(in, out, ctx.ms_divround[l], ctx.n, total);
-    return cudaGetLastError();
+    return launch(mod_switch_kernel, blocks, 256, 0, stream, in, out, ctx.ms_divround[l], ctx.n, total);
 }
 
 }  // namespace hecuda

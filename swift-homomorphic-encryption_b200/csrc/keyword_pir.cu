@@ -84,25 +84,19 @@ unsigned grid_for(long long items, long long per_block) { return (unsigned)((ite
 
 cudaError_t launch_keyword_hash(const unsigned char *d_keywords, const uint64_t *d_offsets, int64_t count, uint64_t *d_hashes) {
     if (count == 0) return cudaSuccess;
-    ++g_kernel_launches;
-    keyword_hash_kernel<<<grid_for(count, kThreads), kThreads>>>(d_keywords, d_offsets, count, d_hashes);
-    return cudaGetLastError();
+    return launch(keyword_hash_kernel, grid_for(count, kThreads), kThreads, 0, 0, d_keywords, d_offsets, count, d_hashes);
 }
 
 cudaError_t launch_hash_indices(const uint64_t *d_hashes, int64_t count, int64_t bucket_count, int h, int64_t *d_out) {
     if (count == 0) return cudaSuccess;
-    ++g_kernel_launches;
-    hash_indices_kernel<<<grid_for(count, kThreads), kThreads>>>(d_hashes, count, bucket_count, h, d_out);
-    return cudaGetLastError();
+    return launch(hash_indices_kernel, grid_for(count, kThreads), kThreads, 0, 0, d_hashes, count, bucket_count, h, d_out);
 }
 
 // Bucket bytes into d_out (table->offsets.back() bytes) on the default stream
 cudaError_t launch_bucket_serialize(const hecuda_cuckoo_table *t, unsigned char *d_out) {
     if (t->bucket_count == 0) return cudaSuccess;
-    ++g_kernel_launches;
-    bucket_serialize_kernel<<<grid_for(t->bucket_count * 32, kThreads), kThreads>>>(
-        t->bucket_count, t->d_row_ptr, t->d_ids, t->d_hashes, t->d_values, t->d_value_offsets, t->d_offsets, d_out);
-    return cudaGetLastError();
+    return launch(bucket_serialize_kernel, grid_for(t->bucket_count * 32, kThreads), kThreads, 0, 0, t->bucket_count, t->d_row_ptr,
+                  t->d_ids, t->d_hashes, t->d_values, t->d_value_offsets, t->d_offsets, d_out);
 }
 
 int32_t have_device() {

@@ -36,21 +36,11 @@ struct hecuda_pir_database {
 
 namespace {
 
-struct RowConsts {
-    int rows;
-    u64 p[kMaxRows];
-};
-
 // one node of an expansion level: where its two children go
 struct ExpandStep {
     int dst0, dst1;
     unsigned flags;  // 1: p0 is a leaf (goes to `out`), 2: p0 doubled, 4: p1 is a leaf, 8: p1 doubled
 };
-
-__device__ __forceinline__ u64 add_mod(u64 a, u64 b, u64 p) {
-    const u64 s = a + b;
-    return s >= p ? s - p : s;
-}
 
 // expandCiphertextForOneStep after the Galois step (PirUtil.swift:230-235) for every node of a level:
 //   p0 = c1 + ct,  p1 = multiplyPowerOfX(ct - c1, -2^(logStep-1))   [gather form of PolyRq.swift:398-422]
@@ -59,7 +49,7 @@ __device__ __forceinline__ u64 add_mod(u64 a, u64 b, u64 p) {
 __global__ void __launch_bounds__(256) expand_combine_kernel(const u64 *__restrict__ cur, const u64 *__restrict__ c1,
                                                             u64 *__restrict__ next, u64 *__restrict__ out,
                                                             const ExpandStep *__restrict__ steps,
-                                                            const __grid_constant__ RowConsts c, int logn, unsigned s,
+                                                            const __grid_constant__ RowModuli c, int logn, unsigned s,
                                                             int64_t item0, int nodes, int64_t next_cts, int64_t out_cts) {
     const int n = 1 << logn;
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -82,14 +72,6 @@ __global__ void __launch_bounds__(256) expand_combine_kernel(const u64 *__restri
     if (st.flags & 8u) d = add_mod(d, d, p);
     ((st.flags & 1u) ? out : next)[(int64_t)st.dst0 * ct_words + (int64_t)pr * n + e] = sum;
     ((st.flags & 4u) ? out : next)[(int64_t)st.dst1 * ct_words + (int64_t)pr * n + e] = d;
-}
-
-RowConsts row_consts(const Context &c, int l) {
-    RowConsts rc;
-    const NttRowMap map = c.map_q(l);
-    rc.rows = l;
-    for (int r = 0; r < l; ++r) rc.p[r] = c.slots[map.slot[r]].dev.p;
-    return rc;
 }
 
 int ceil_log2(int64_t x) {
@@ -298,8 +280,8 @@ int32_t expand_device(const hecuda_context *h, const hecuda_evk *const *keys, in
     CK(tmp.alloc(&c1_buf[0], level_words));
     CK(tmp.alloc(&c1_buf[1], level_words));
     CK(tmp.alloc(&scratch, galois_scratch_words(c, l) * (size_t)chunk));
-    const RowConsts rc = row_consts(c, l);
-    const int threads = n >= 256 ? 256 : (n < 32 ? 32 : (int)n);
+    const RowModuli rc = row_moduli(c, c.map_q(l));
+    const int threads = coeff_threads(n);
     // the active roots are a prefix of each input (only the last one can be a single output); a level's nodes must be
     // contiguous over all clients, so several clients' roots are gathered when a single-output root sits between them
     const u64 *cur = d_in;
@@ -330,15 +312,12 @@ int32_t expand_device(const hecuda_context *h, const hecuda_evk *const *keys, in
         flip ^= 1;
         const int64_t next_nodes = li + 1 < plan.levels.size() ? plan.levels[li + 1].nodes : 0;
         const unsigned shift = (unsigned)(2 * n) - (1u << (level.log_step - 1));  // -2^(logStep-1) mod 2N
-        for (int64_t done = 0; done < total;) {
-            const int64_t items = std::min<int64_t>(total - done, 65535);
+        const cudaError_t e = for_each_part(total, [&](int64_t done, int64_t items) {
             dim3 grid((unsigned)((n + threads - 1) / threads), (unsigned)(2 * l), (unsigned)items);
-            ++g_kernel_launches;
-            expand_combine_kernel<<<grid, threads, 0, s>>>(cur, c1, next, d_out, d_steps + level.step_offset, rc, c.logn, shift,
-                                                           done, (int)level.nodes, next_nodes, output_count);
-            done += items;
-        }
-        CK(cudaGetLastError());
+            return launch(expand_combine_kernel, grid, threads, 0, s, cur, c1, next, d_out, d_steps + level.step_offset, rc, c.logn,
+                          shift, done, (int)level.nodes, next_nodes, output_count);
+        });
+        if (e != cudaSuccess) return cuda_fail(e, "expand: combine");
         cur = next;
     }
     return HECUDA_OK;

@@ -8,7 +8,6 @@
 //
 // The encode / decode pipelines are compositions of one gather kernel (writes coalesced) and the row NTT kernels on the
 // plaintext modulus' slot (Context::slot_t); the translate is one coefficient-wise kernel.  All enqueue on one stream.
-#include <algorithm>
 #include <cstdint>
 
 #include "../../include/hecuda.h"
@@ -20,7 +19,6 @@ namespace hecuda {
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int64_t kMaxGridY = 65535;
 
 template <int OP>
 __device__ __forceinline__ u64 translate_one(u64 x, u64 v, u64 q) {
@@ -129,42 +127,30 @@ __global__ void __launch_bounds__(kThreads) uncenter_kernel(u64 *data, u64 thres
     data[i] = x >= threshold ? x - increment : x;
 }
 
-int threads_for(int64_t n) { return n >= kThreads ? kThreads : (n < 32 ? 32 : (int)n); }
-
 }  // namespace
 
-// at most 65535 rows per call when N = 2^15 (the split path puts rows in grid z)
+// at most kMaxGridYZ rows per call when N = 2^15 (the split path puts rows in grid z)
 cudaError_t ntt_single(const Context &ctx, int slot, bool inverse, const u64 *in, u64 *out, int64_t rows, cudaStream_t s) {
-    const int64_t step = ctx.logn >= fast::kSplitLogN ? kMaxGridY : rows;
     const NttRowMap map = ctx.map_single(slot);
-    for (int64_t done = 0; done < rows;) {
-        const int64_t part = std::min<int64_t>(step, rows - done);
-        cudaError_t e = inverse ? launch_ntt_inverse(ctx, map, in + done * ctx.n, out + done * ctx.n, part, kScalePlain, s)
-                                : launch_ntt_forward(ctx, map, in + done * ctx.n, out + done * ctx.n, part, s);
-        if (e != cudaSuccess) return e;
-        done += part;
-    }
-    return cudaSuccess;
+    return for_each_part(rows, [&](int64_t done, int64_t part) {
+        return inverse ? launch_ntt_inverse(ctx, map, in + done * ctx.n, out + done * ctx.n, part, kScalePlain, s)
+                       : launch_ntt_forward(ctx, map, in + done * ctx.n, out + done * ctx.n, part, s);
+    }, ctx.logn >= fast::kSplitLogN ? kMaxGridYZ : rows);
 }
 
 namespace {
 
 cudaError_t launch_simd_gather(const Context &ctx, bool encode, const u64 *in, int value_count, u64 *out, int64_t count,
                                cudaStream_t s) {
-    const int threads = threads_for(ctx.n);
+    const int threads = coeff_threads(ctx.n);
     const unsigned gx = (unsigned)((ctx.n + threads - 1) / threads);
-    for (int64_t done = 0; done < count;) {
-        const int64_t part = std::min<int64_t>(kMaxGridY, count - done);
-        ++g_kernel_launches;
+    return for_each_part(count, [&](int64_t done, int64_t part) {
         if (encode)
-            simd_encode_kernel<<<dim3(gx, (unsigned)part), threads, 0, s>>>(in + done * value_count, value_count,
-                                                                           ctx.d_simd_inverse, out + done * ctx.n, (int)ctx.n);
-        else
-            simd_decode_kernel<<<dim3(gx, (unsigned)part), threads, 0, s>>>(in + done * ctx.n, ctx.d_simd_matrix,
-                                                                           out + done * ctx.n, (int)ctx.n);
-        done += part;
-    }
-    return cudaGetLastError();
+            return launch(simd_encode_kernel, dim3(gx, (unsigned)part), threads, 0, s, in + done * value_count, value_count,
+                          ctx.d_simd_inverse, out + done * ctx.n, (int)ctx.n);
+        return launch(simd_decode_kernel, dim3(gx, (unsigned)part), threads, 0, s, in + done * ctx.n, ctx.d_simd_matrix,
+                      out + done * ctx.n, (int)ctx.n);
+    });
 }
 
 }  // namespace
@@ -198,10 +184,9 @@ cudaError_t launch_decode_simd(const Context &ctx, const u64 *plain, int l, u64 
             return e;
         if ((e = ntt_single(ctx, ctx.slot_q(0), true, scratch, scratch, count, s)) != cudaSuccess) return e;
         const long long words = (long long)count * ctx.n;
-        ++g_kernel_launches;
-        uncenter_kernel<<<(unsigned)((words + kThreads - 1) / kThreads), kThreads, 0, s>>>(
-            scratch, (ctx.t + 1) / 2, ctx.q[0] - ctx.t, words);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if ((e = launch(uncenter_kernel, (unsigned)((words + kThreads - 1) / kThreads), kThreads, 0, s, scratch,
+                        (ctx.t + 1) / 2, ctx.q[0] - ctx.t, words)) != cudaSuccess)
+            return e;
         if ((e = ntt_single(ctx, ctx.slot_t(), false, scratch, scratch, count, s)) != cudaSuccess) return e;
     }
     return launch_simd_gather(ctx, false, scratch, 0, values, count, s);
@@ -215,27 +200,19 @@ cudaError_t launch_plaintext_translate(const Context &ctx, const u64 *ct, int po
     const TranslateConsts &c = ctx.translate[l];
     const int rest = op == HECUDA_PLAINTEXT_SUB_FROM ? 2 : (out != ct ? 1 : 0);
     const bool vec = (((uintptr_t)ct | (uintptr_t)out | (uintptr_t)pt) & 15) == 0;
-    const int threads = threads_for(ctx.n / 2);
+    const int threads = coeff_threads(ctx.n / 2);
     const unsigned gx = (unsigned)((ctx.n / 2 + threads - 1) / threads);
     const long long pt_stride = broadcast ? 0 : ctx.n;
     const int64_t ct_words = (int64_t)polys * l * ctx.n;
-    for (int64_t done = 0; done < batch;) {
-        const int64_t part = std::min<int64_t>(kMaxGridY, batch - done);
-        const dim3 grid(gx, (unsigned)part);
-        const u64 *src = ct + done * ct_words;
-        u64 *dst = out + done * ct_words;
-        const u64 *p = pt + done * pt_stride;
-        ++g_kernel_launches;
-#define HE_TRANSLATE(OP)                                                                                                   \
-    if (vec) plaintext_translate_kernel<OP, true><<<grid, threads, 0, s>>>(src, dst, p, pt_stride, polys, rest, c, (int)ctx.n); \
-    else plaintext_translate_kernel<OP, false><<<grid, threads, 0, s>>>(src, dst, p, pt_stride, polys, rest, c, (int)ctx.n);
-        if (op == HECUDA_PLAINTEXT_ADD) { HE_TRANSLATE(HECUDA_PLAINTEXT_ADD) }
-        else if (op == HECUDA_PLAINTEXT_SUB) { HE_TRANSLATE(HECUDA_PLAINTEXT_SUB) }
-        else { HE_TRANSLATE(HECUDA_PLAINTEXT_SUB_FROM) }
-#undef HE_TRANSLATE
-        done += part;
-    }
-    return cudaGetLastError();
+    // [op][vec]
+    static void (*const kernels[3][2])(const u64 *, u64 *, const u64 *, long long, int, int, TranslateConsts, int) = {
+        {plaintext_translate_kernel<HECUDA_PLAINTEXT_ADD, false>, plaintext_translate_kernel<HECUDA_PLAINTEXT_ADD, true>},
+        {plaintext_translate_kernel<HECUDA_PLAINTEXT_SUB, false>, plaintext_translate_kernel<HECUDA_PLAINTEXT_SUB, true>},
+        {plaintext_translate_kernel<HECUDA_PLAINTEXT_SUB_FROM, false>, plaintext_translate_kernel<HECUDA_PLAINTEXT_SUB_FROM, true>}};
+    return for_each_part(batch, [&](int64_t done, int64_t part) {
+        return launch(kernels[op][vec], dim3(gx, (unsigned)part), threads, 0, s, ct + done * ct_words, out + done * ct_words,
+                      pt + done * pt_stride, pt_stride, polys, rest, c, (int)ctx.n);
+    });
 }
 
 }  // namespace hecuda

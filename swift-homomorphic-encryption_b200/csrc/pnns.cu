@@ -33,11 +33,6 @@ namespace {
 
 static_assert(HECUDA_PNNS_CLIENT_GROUP == kKeyTableSize, "one key-table entry per client of a group");
 
-struct RowConsts {
-    int rows;
-    u64 p[kMaxRows];
-};
-
 // Where the items of an accumulate live: they form clients of `per_client` items each, and item k of client j is the
 // ciphertext at acc + j * acc_client + k * (2 x rows x N) and at src + j * src_client + k * src_stride (all in words).
 struct AccLayout {
@@ -48,7 +43,7 @@ struct AccLayout {
 // modes (optional, per item): 0 = leave acc alone, 1 = copy, 2 = add; without modes every item uses `add`
 __global__ void __launch_bounds__(256) accumulate_kernel(u64 *__restrict__ acc, const u64 *__restrict__ src,
                                                         const __grid_constant__ AccLayout lay, long long item0,
-                                                        const __grid_constant__ RowConsts c, int n, int add,
+                                                        const __grid_constant__ RowModuli c, int n, int add,
                                                         const signed char *__restrict__ modes) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n) return;
@@ -73,30 +68,18 @@ __global__ void __launch_bounds__(256) accumulate_kernel(u64 *__restrict__ acc, 
     }
 }
 
-RowConsts row_consts(const Context &c, int l) {
-    RowConsts rc;
-    const NttRowMap map = c.map_q(l);
-    rc.rows = l;
-    for (int r = 0; r < l; ++r) rc.p[r] = c.slots[map.slot[r]].dev.p;
-    return rc;
-}
-
 // acc[k] (+)= src[k * src_item_stride] for k < items; per_client > 0 splits the items into clients (AccLayout)
 cudaError_t launch_accumulate(const Context &c, int l, u64 *acc, const u64 *src, int64_t src_item_stride, int64_t items,
                               bool add, cudaStream_t s, const signed char *modes = nullptr, int64_t per_client = 0,
                               int64_t src_client_stride = 0, int64_t acc_client_stride = 0) {
-    const RowConsts rc = row_consts(c, l);
+    const RowModuli rc = row_moduli(c, c.map_q(l));
     const AccLayout lay{per_client > 0 ? per_client : std::max<int64_t>(items, 1), src_item_stride, src_client_stride,
                         acc_client_stride};
-    const int threads = c.n >= 256 ? 256 : (c.n < 32 ? 32 : (int)c.n);
-    for (int64_t done = 0; done < items;) {
-        const int64_t chunk = std::min<int64_t>(items - done, 65535);
+    const int threads = coeff_threads(c.n);
+    return for_each_part(items, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((c.n + threads - 1) / threads), (unsigned)(2 * l), (unsigned)chunk);
-        ++g_kernel_launches;
-        accumulate_kernel<<<grid, threads, 0, s>>>(acc, src, lay, done, rc, (int)c.n, add ? 1 : 0, modes);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(accumulate_kernel, grid, threads, 0, s, acc, src, lay, done, rc, (int)c.n, add ? 1 : 0, modes);
+    });
 }
 
 struct MaskConsts {
@@ -135,17 +118,12 @@ cudaError_t launch_mask_product(const Context &c, const u64 *ct_eval, int64_t ct
         mc.mu_hi[r] = S.mu_hi;
         mc.mu_lo[r] = S.mu_lo;
     }
-    const int threads = c.n >= 256 ? 256 : (c.n < 32 ? 32 : (int)c.n);
-    const int64_t items = rows_per_client * clients;
-    for (int64_t done = 0; done < items;) {
-        const int64_t chunk = std::min<int64_t>(items - done, 65535);
+    const int threads = coeff_threads(c.n);
+    return for_each_part(rows_per_client * clients, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((c.n + threads - 1) / threads), (unsigned)(2 * c.L), (unsigned)chunk);
-        ++g_kernel_launches;
-        mask_product_kernel<<<grid, threads, 0, s>>>(ct_eval, mask_eval, index, y, mc, (int)c.n, (int)rows_per_client,
-                                                     ct_count, done);
-        done += chunk;
-    }
-    return cudaGetLastError();
+        return launch(mask_product_kernel, grid, threads, 0, s, ct_eval, mask_eval, index, y, mc, (int)c.n, (int)rows_per_client,
+                      ct_count, done);
+    });
 }
 
 // GaloisElement.rotatingColumns(by:degree:) (PolyRq/Galois.swift:195-212)

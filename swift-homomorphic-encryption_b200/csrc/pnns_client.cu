@@ -127,14 +127,10 @@ namespace hecuda {
 cudaError_t launch_pnns_normalize(const float *vectors, int64_t rows, int64_t cols, int64_t scaling_factor, float *norms,
                                   int64_t *values, int *bad, cudaStream_t s) {
     if (rows == 0) return cudaSuccess;
-    ++g_kernel_launches;
-    row_norm_kernel<<<blocks(rows), kThreads, 0, s>>>(vectors, (long long)rows, (long long)cols, norms);
-    cudaError_t e = cudaGetLastError();
+    const cudaError_t e = launch(row_norm_kernel, blocks(rows), kThreads, 0, s, vectors, (long long)rows, (long long)cols, norms);
     if (e != cudaSuccess) return e;
-    ++g_kernel_launches;
-    scaled_value_kernel<<<blocks(rows * cols), kThreads, 0, s>>>(vectors, norms, (long long)rows, (long long)cols,
-                                                                  (float)scaling_factor, (long long *)values, bad);
-    return cudaGetLastError();
+    return launch(scaled_value_kernel, blocks(rows * cols), kThreads, 0, s, vectors, norms, (long long)rows, (long long)cols,
+                  (float)scaling_factor, (long long *)values, bad);
 }
 
 namespace api {
@@ -172,7 +168,7 @@ int32_t hecuda_pnns_query_generate(const hecuda_context *h, const uint64_t *secr
         return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
     if ((rc = check_float_vectors(vectors, row_count, column_count, scaling_factor, c.t, reduce != 0, true))) return rc;
     const int64_t count = procdb::pnns_dense_row_count(row_count, column_count, c.logn);
-    if (count > 65535) return fail(HECUDA_ERR_INVALID_ARGUMENT, "too many query rows");
+    if (count > kMaxGridYZ) return fail(HECUDA_ERR_INVALID_ARGUMENT, "too many query rows");  // grid y of dense_row_kernel
     const int L = c.L;
     const int64_t n = c.n;
     const size_t poly_words = (size_t)L * n, values = (size_t)row_count * column_count;
@@ -200,12 +196,9 @@ int32_t hecuda_pnns_query_generate(const hecuda_context *h, const uint64_t *secr
         if (e == cudaSuccess) e = cudaMemcpyAsync(d_vec, vectors, values * sizeof(float), cudaMemcpyHostToDevice, s);
         if (e == cudaSuccess) e = cudaMemsetAsync(d_bad, 0, sizeof(int), s);
         if (e == cudaSuccess) e = launch_pnns_normalize(d_vec, row_count, column_count, scaling_factor, d_norm, d_vals, d_bad, s);
-        if (e == cudaSuccess) {
-            ++g_kernel_launches;
-            dense_row_kernel<<<dim3(blocks(n), (unsigned)count), kThreads, 0, s>>>(
-                (const long long *)d_vals, row_count, column_count, c.logn, c.t, reduce, c.d_simd_inverse, d_pt, d_bad);
-            e = cudaGetLastError();
-        }
+        if (e == cudaSuccess)
+            e = launch(dense_row_kernel, dim3(blocks(n), (unsigned)count), kThreads, 0, s, (const long long *)d_vals, row_count,
+                       column_count, c.logn, c.t, reduce, c.d_simd_inverse, d_pt, d_bad);
         // encodeSimd's inverse NTT mod t (Encoding.swift:206-214)
         if (e == cudaSuccess) e = ntt_single(c, c.slot_t(), true, d_pt, d_pt, count, s);
         // a value Swift would trap on refuses the call before anything is encrypted or returned
@@ -303,9 +296,7 @@ int32_t hecuda_pnns_decrypt_distances(const hecuda_context *const *ctxs, int32_t
         }
         if (e == cudaSuccess) {
             const DistanceArgs a{matrix_rows, query_rows, reply_count, scaling_factor, c.logn, crt};
-            ++g_kernel_launches;
-            distance_kernel<<<blocks((long long)total), kThreads, 0, s>>>(d_dec, a, d_out);
-            e = cudaGetLastError();
+            e = launch(distance_kernel, blocks((long long)total), kThreads, 0, s, d_dec, a, d_out);
         }
         if (e == cudaSuccess) e = cudaMemcpyAsync(distances, d_out, total * sizeof(float), cudaMemcpyDeviceToHost, s);
     }

@@ -1,8 +1,6 @@
 // process_db.cu -- the server's own data into plaintexts on the device: MulPirServer.process's packing and
 // PlaintextMatrix(signedValues:)'s .diagonal packing with its SIMD encoding.  The index arithmetic is in
 // process_db.cuh; these kernels only apply it.  Both enqueue on one stream.
-#include <algorithm>
-
 #include "kernels.cuh"
 
 namespace hecuda {
@@ -10,7 +8,6 @@ namespace hecuda {
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int64_t kMaxGridY = 65535;
 
 // One CTA per plaintext: every thread extracts its coefficients straight from the entry bytes; a block-wide OR says
 // whether the plaintext is non-nil (MulPir.swift:480, 536: an all-zero plaintext is nil).
@@ -65,28 +62,20 @@ __global__ void __launch_bounds__(kThreads) pnns_gather_kernel(const long long *
 cudaError_t launch_pir_pack(const procdb::PirShape &s, int n, int64_t first, int64_t items, u64 *out,
                             unsigned char *present, cudaStream_t stream) {
     if (items == 0) return cudaSuccess;
-    const int threads = std::max(32, std::min(kThreads, n));
-    ++g_kernel_launches;
-    pir_pack_kernel<<<(unsigned)items, threads, 0, stream>>>(s, n, (long long)first, out, present);
-    return cudaGetLastError();
+    return launch(pir_pack_kernel, (unsigned)items, coeff_threads(n), 0, stream, s, n, (long long)first, out, present);
 }
 
 cudaError_t launch_pnns_diagonal(const Context &ctx, const procdb::PnnsShape &s, const int64_t *values, bool reduce,
                                  bool resident, int64_t first, int64_t items, u64 *out, int *bad, cudaStream_t stream) {
     if (items == 0) return cudaSuccess;
     if (!ctx.simd) return cudaErrorInvalidValue;
-    const int threads = std::max(32, (int)std::min<int64_t>(kThreads, ctx.n));
+    const int threads = coeff_threads(ctx.n);
     const unsigned gx = (unsigned)((ctx.n + threads - 1) / threads);
-    for (int64_t done = 0; done < items;) {
-        const int64_t part = std::min(kMaxGridY, items - done);
-        ++g_kernel_launches;
-        pnns_gather_kernel<<<dim3(gx, (unsigned)part), threads, 0, stream>>>(
-            (const long long *)values, s, ctx.t, reduce ? 1 : 0, resident ? 1 : 0, ctx.d_simd_inverse,
-            (long long)(first + done), out + done * ctx.n, bad);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-        done += part;
-    }
+    const cudaError_t e = for_each_part(items, [&](int64_t done, int64_t part) {
+        return launch(pnns_gather_kernel, dim3(gx, (unsigned)part), threads, 0, stream, (const long long *)values, s, ctx.t,
+                      reduce ? 1 : 0, resident ? 1 : 0, ctx.d_simd_inverse, (long long)(first + done), out + done * ctx.n, bad);
+    });
+    if (e != cudaSuccess) return e;
     // encodeSimd's inverse NTT mod t (Encoding.swift:206-214)
     return ntt_single(ctx, ctx.slot_t(), true, out, out, items, stream);
 }
