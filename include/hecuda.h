@@ -412,6 +412,30 @@ int32_t hecuda_keyword_pir_databases_create(const hecuda_context *ctx, const hec
                                             int64_t entry_size, const int32_t *dims, int32_t dim_count,
                                             hecuda_pir_database **out);
 
+/* ---- Symmetric keyword PIR: SymmetricPir/SymmetricPirDatabase.swift, config OPRF_P384_AES_GCM_192_NONCE_96_TAG_128 ----
+ * The OPRF is RFC 9497 in VOPRF mode over P384-SHA384 (swift-crypto's P384._VOPRF): HashToGroup is RFC 9380
+ * P384_XMD:SHA-384_SSWU_RO_ with DST "HashToGroup-" || contextString, contextString = "OPRFV1-" || 0x01 || "-P384-SHA384"
+ * as RFC 9497 writes it.  The secret key is 48 big-endian bytes k with 0 < k < n (OprfPrivateKey(rawRepresentation:)).
+ * These calls need no context.  Refused with HECUDA_ERR_INVALID_ARGUMENT and no kernel launched: null pointers, a
+ * negative count, decreasing offsets, a key outside [1, n - 1], and an OPRF input (keyword) over 65535 bytes (its length
+ * is hashed as I2OSP(len, 2)).  A count of 0 launches nothing.  The device copies of the key's recoding and of each
+ * row's OPRF output are zeroized before they are freed. */
+#define HECUDA_OPRF_KEY_BYTES 48
+#define HECUDA_OPRF_ELEMENT_BYTES 49
+#define HECUDA_OPRF_OUTPUT_BYTES 48
+/* SymmetricPirConfig.clientConfig().serverPublicKey (SymmetricPirDatabase.swift:176-183): k G, SEC1 compressed. */
+int32_t hecuda_oprf_public_key(const uint8_t *secret_key, uint8_t *public_key /* 49 */);
+/* OprfPrivateKey.evaluate (RFC 9497 3.3.1 Evaluate) of every input, one device thread each: outputs[i] =
+ * SHA-384(I2OSP(len, 2) || input || I2OSP(49, 2) || k HashToGroup(input) || "Finalize"). */
+int32_t hecuda_oprf_evaluate(const uint8_t *secret_key, const uint8_t *inputs, const uint64_t *offsets, int64_t count,
+                             uint8_t *outputs /* 48 * count */);
+/* KeywordDatabase.symmetricPIRProcess(database:config:) (SymmetricPirDatabase.swift:193-211): with h the OPRF output of
+ * keyword i, keywords_out[i] = h[0:16] and value i becomes AES.GCM.seal(value, key h[24:48], nonce h[0:12]) as ciphertext
+ * || 16-byte tag, at values_out + value_offsets[i] + 16 i (value_offsets[count] + 16 count bytes in all). */
+int32_t hecuda_symmetric_pir_process(const uint8_t *secret_key, const uint8_t *keywords, const uint64_t *keyword_offsets,
+                                     const uint8_t *values, const uint64_t *value_offsets, int64_t count,
+                                     uint8_t *keywords_out /* 16 * count */, uint8_t *values_out);
+
 /* PirUtil.expand(ciphertexts:outputCount:using:) -- IndexPir/PirUtil.swift:321-355 (expandCiphertext :249-304,
  * expandCiphertextForOneStep :204-236).  ciphertexts: ciphertext_count x 2 x L x N (Coeff); out: output_count x 2 x L x N,
  * output i encrypting the constant polynomial whose constant is coefficient i of the inputs (x 2^ceilLog2(count)).

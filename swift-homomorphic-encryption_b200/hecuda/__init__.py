@@ -114,6 +114,9 @@ SYMBOLS = {
     "hecuda_cuckoo_table_serialize_buckets": (C.c_int32, [_VP, _VP, C.c_uint64, _VP]),
     "hecuda_cuckoo_table_destroy": (C.c_int32, [_VP]),
     "hecuda_keyword_pir_databases_create": (C.c_int32, [_VP, _VP, C.c_int64, _VP, C.c_int32, _VP]),
+    "hecuda_oprf_public_key": (C.c_int32, [_VP, _VP]),
+    "hecuda_oprf_evaluate": (C.c_int32, [_VP, _VP, _VP, C.c_int64, _VP]),
+    "hecuda_symmetric_pir_process": (C.c_int32, [_VP, _VP, _VP, _VP, _VP, C.c_int64, _VP, _VP]),
     "hecuda_mulpir_expand": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP]),
     "hecuda_mulpir_expand_device": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP, _VP]),
     "hecuda_mulpir_compute_response": (C.c_int32, [_VP, _VP, C.POINTER(_VP), C.c_int32, C.POINTER(C.c_int32), C.c_int32,

@@ -9,6 +9,7 @@ Names and argument meaning follow Sources/PrivateInformationRetrieval/KeywordPir
     KeywordPirServer.process / computeResponse     KeywordPirProtocol.swift:137-276
     KeywordPirClient                               KeywordPirProtocol.swift:280-392
     KeywordDatabase.validateShard                  KeywordDatabase.swift:557-630
+    KeywordDatabase.symmetricPIRProcess            SymmetricPir/SymmetricPirDatabase.swift:186-211 (hecuda.symmetric_pir)
 
 Keyword hashing, candidate indices and bucket serialization run on the device; the cuckoo placement runs on the host
 inside libhecuda (csrc/cuckoo.hpp) because the table depends on the order of its random draws.  The table's buckets
@@ -28,8 +29,10 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 
 from . import Context, EvaluationKey, SecretKey, _check, _ptr, load_library
+from . import symmetric_pir
 from .pir import IndexPirConfig, IndexPirParameter, MulPir, MulPirClient, MulPirServer, PirError, PirKeyCompressionStrategy, \
     PirWire, ProcessedDatabase, ShardValidationResult, _validate, bytesPerPlaintext
+from .symmetric_pir import SymmetricPirClientConfig, SymmetricPirConfig
 
 MAX_SLOT_COUNT = 255  # HashBucket.maxSlotCount
 RNG_COUNTER, RNG_SPLITMIX64 = 0, 1  # HECUDA_CUCKOO_RNG_*
@@ -315,13 +318,18 @@ class Sharding:
 
 
 class KeywordDatabase:
-    """KeywordDatabase (KeywordDatabase.swift:388-435): rows split into shards by their device-computed keyword hashes.
-    shards: shard id (str) -> [(keyword, value)] in row order."""
+    """KeywordDatabase (KeywordDatabase.swift:388-437): rows split into shards by their device-computed keyword hashes.
+    shards: shard id (str) -> [(keyword, value)] in row order.  With a symmetricPirConfig the rows are first replaced by
+    symmetricPIRProcess's (keyword', sealed value) rows, and those are sharded; the shard count still comes from the row
+    count."""
 
     def __init__(self, rows: Sequence[KeywordValuePair], sharding: Sharding,
-                 shardingFunction: ShardingFunction = ShardingFunction.sha256):
+                 shardingFunction: ShardingFunction = ShardingFunction.sha256,
+                 symmetricPirConfig: Optional[SymmetricPirConfig] = None):
         rows = [(bytes(k), bytes(v)) for k, v in rows]
         count = sharding.shardCountFor(len(rows))
+        if symmetricPirConfig is not None:
+            rows = KeywordDatabase.symmetricPIRProcess(rows, symmetricPirConfig)
         indices = shardingFunction.shardIndices(HashKeyword.hashes([k for k, _ in rows]), count) if rows else []
         shards: Dict[str, Dict[bytes, bytes]] = {}
         for (keyword, value), index in zip(rows, indices):
@@ -331,6 +339,12 @@ class KeywordDatabase:
                                f"newValue: {list(value)})")
             shard[keyword] = value
         self.shards = {sid: list(rows.items()) for sid, rows in shards.items()}
+
+    @staticmethod
+    def symmetricPIRProcess(database: Sequence[KeywordValuePair], config: SymmetricPirConfig) -> List[KeywordValuePair]:
+        """KeywordDatabase.symmetricPIRProcess(database:config:) (SymmetricPirDatabase.swift:193-211), every row on the
+        device: (keyword, value) -> (OPRF output[0:16], AES-GCM-192 ciphertext || tag)."""
+        return symmetric_pir.symmetricPIRProcess(database, config)
 
 
 # ------------------------------------------------------------------------------------------------ keyword PIR
@@ -352,6 +366,7 @@ class KeywordPirConfig:
     keyCompression: PirKeyCompressionStrategy
     useMaxSerializedBucketSize: bool = False
     shardingFunction: ShardingFunction = ShardingFunction.sha256
+    symmetricPirClientConfig: Optional[SymmetricPirClientConfig] = None
 
     def __post_init__(self):
         if self.dimensionCount not in (1, 2):
@@ -373,6 +388,7 @@ class ProcessedKeywordDatabase:
     pirParameter: IndexPirParameter
     keywordPirParameter: KeywordPirParameter
     table: CuckooTable
+    symmetricPirConfig: Optional[SymmetricPirConfig] = None  # as ProcessedDatabaseWithParameters keeps it
 
     def close(self):
         for db in self.databases:
@@ -439,10 +455,13 @@ class KeywordPirServer:
 
     @staticmethod
     def processOnDevice(database: Sequence[KeywordValuePair], config: KeywordPirConfig, context: Context,
-                        rng: Rng = Rng.splitMix64()) -> ProcessedKeywordDatabase:
+                        rng: Rng = Rng.splitMix64(),
+                        symmetricPirConfig: Optional[SymmetricPirConfig] = None) -> ProcessedKeywordDatabase:
         """KeywordPirServer.process (KeywordPirProtocol.swift:191-247): the cuckoo table, its IndexPirParameter
         (entryCount = bucketsPerTable, batchSize = hashFunctionCount, no entry-size encoding) and one MulPir database per
-        table, built from the serialized buckets without them leaving the device."""
+        table, built from the serialized buckets without them leaving the device.  The database is taken as given: a
+        symmetric PIR database is one KeywordDatabase.symmetricPIRProcess has already processed, and symmetricPirConfig
+        is only stored with the result."""
         cuckoo = config.cuckooTableConfig
         table = CuckooTable(context, cuckoo, database, rng)
         try:
@@ -463,7 +482,7 @@ class KeywordPirServer:
             raise
         count = -(-parameter.encodedEntrySize // bytesPerPlaintext(context)) * int(np.prod(parameter.dimensions))
         databases = [ProcessedDatabase._adopt(context, C.c_void_p(h), count) for h in handles]
-        return ProcessedKeywordDatabase(databases, parameter, config.parameter, table)
+        return ProcessedKeywordDatabase(databases, parameter, config.parameter, table, symmetricPirConfig)
 
     def computeResponse(self, query, evaluationKey: EvaluationKey) -> np.ndarray:
         """computeResponse(to:using:): MulPir over the hashFunctionCount tables with indicesCount = hashFunctionCount.
