@@ -435,6 +435,22 @@ int32_t hecuda_oprf_evaluate(const uint8_t *secret_key, const uint8_t *inputs, c
 int32_t hecuda_symmetric_pir_process(const uint8_t *secret_key, const uint8_t *keywords, const uint64_t *keyword_offsets,
                                      const uint8_t *values, const uint64_t *value_offsets, int64_t count,
                                      uint8_t *keywords_out /* 16 * count */, uint8_t *values_out);
+/* OprfServer.computeResponse(query:) (SymmetricPir/SymmetricPirProtocol.swift:39-59), swift-crypto's
+ * P384._VOPRF.PrivateKey.evaluate: RFC 9497 3.3.2 BlindEvaluate with the 2.2.1 DLEQ proof (ComputeCompositesFast) over
+ * one element, for each of `count` blinded elements, one device thread each.  responses[i] = SerializeElement(k B_i) ||
+ * I2OSP(c, 48) || I2OSP(s, 48), the layout BlindEvaluation(rawRepresentation:) takes (ApplicationProtobuf/
+ * PirConversion.swift:358-377).  The proof nonce is r = OS2IP(expand_message_xmd(I2OSP(k, 48) || seed || Ser(B_i),
+ * "HECUDA-ProofNonce-" || contextString, 72)) mod n instead of the RFC's random draw: a verifier accepts any r in
+ * [1, n - 1], and equal (k, B) give equal proofs whatever the seed, so a repeated seed cannot reuse r under two
+ * challenges.  A query that is not a valid SEC1-compressed point (prefix 2 or 3, x < p, on the curve) gets status[i] = 1
+ * and 145 zero bytes; the others are answered.  Refused with no kernel launched: null pointers, count < 0 and a key
+ * outside [1, n - 1]. */
+#define HECUDA_OPRF_PROOF_BYTES 96
+#define HECUDA_OPRF_RESPONSE_BYTES 145 /* evaluated element || c || s */
+#define HECUDA_OPRF_SEED_BYTES 32
+int32_t hecuda_oprf_blind_evaluate(const uint8_t *secret_key, const uint8_t *blinded_elements /* count x 49 */,
+                                   int64_t count, const uint8_t *seed /* 32 */,
+                                   uint8_t *responses /* count x 145 */, uint8_t *status /* count: 0 ok, 1 invalid */);
 
 /* PirUtil.expand(ciphertexts:outputCount:using:) -- IndexPir/PirUtil.swift:321-355 (expandCiphertext :249-304,
  * expandCiphertextForOneStep :204-236).  ciphertexts: ciphertext_count x 2 x L x N (Coeff); out: output_count x 2 x L x N,

@@ -1,16 +1,20 @@
 // p384.cuh -- the P-384 field and group (SEC 2, FIPS 186-5) as __host__ __device__ functions, for symmetric_pir.cu's
-// OPRF evaluation; tests/emu replays them against oracle/oprf_oracle.py.
+// OPRF evaluation and OPRF server; tests/emu replays them against oracle/oprf_oracle.py.
 //
 //   Field   12 x 32-bit little-endian limbs in Montgomery form, R = 2^384.  p = 2^384 - 2^128 - 2^96 + 2^32 - 1 is
 //           -1 mod 2^32, so the per-word Montgomery factor -p^-1 mod 2^32 is 1 and each reduction step's multiplier
 //           is the low word itself.  Every function returns a value below p.
+//   Scalars mod n through the same Montgomery code with n's own factor -n^-1 mod 2^32 (ModN), kept as plain integers.
 //   Group   Jacobian coordinates (x = X/Z^2, y = Y/Z^3, the identity has Z = 0), a = -3 doubling (dbl-2001-b) and
 //           the general addition (add-2007-bl).
 //   Hashing RFC 9380 P384_XMD:SHA-384_SSWU_RO_: expand_message_xmd with SHA-384, hash_to_field (L = 72, count 2),
 //           the straight-line simplified SWU of its appendix F.2 with Z = -12 and sqrt_ratio for p = 3 mod 4, and the
 //           sum of the two mapped points (cofactor 1).
-//   Scalar  k * P for a scalar shared by every thread: the host recodes k once into 96 signed odd 4-bit digits
-//           (recode_scalar), so the ladder is a fixed sequence of 4 doublings and one table addition per digit.
+//   Scalar  k * P over 96 signed odd 4-bit digits (recode_scalar): a fixed sequence of 4 doublings and one table
+//           addition per digit.  scalar_mul indexes the table directly, for the key every thread shares (recoded
+//           once on the host) and for public scalars; scalar_mul_ct reads it without secret-dependent addresses or
+//           branches, for a secret scalar of one thread.
+//   VOPRF   RFC 9497 BlindEvaluate with the DLEQ proof over one element (blind_evaluate_composite, generate_proof).
 #pragma once
 #include <cstdint>
 
@@ -67,9 +71,14 @@ struct Point {
     X(kPMinus2, 0xfffffffdu, 0x00000000u, 0x00000000u, 0xffffffffu, 0xfffffffeu, 0xffffffffu, 0xffffffffu,             \
       0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu)                                                 \
     X(kSqrtRatioC1, 0x3fffffffu, 0x00000000u, 0xc0000000u, 0xbfffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu,         \
-      0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0x3fffffffu)
+      0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0x3fffffffu)                                                 \
+    X(kSqrtExp, 0x40000000u, 0x00000000u, 0xc0000000u, 0xbfffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu,             \
+      0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0x3fffffffu)                                                 \
+    X(kNR2, 0x19b409a9u, 0x2d319b24u, 0xdf1aa419u, 0xff3d81e5u, 0xfcb82947u, 0xbc3e483au, 0x4aab1cc5u, 0xd40d4917u,    \
+      0x28266895u, 0x3fb05b7au, 0x2b39bf21u, 0x0c84ee01u)
 // p and n are plain integers; kOne .. kGy are in Montgomery form (x R mod p): R, R^2, R^3, b, a = -3, Z = -12,
-// sqrt(-Z) = sqrt(12) and the generator; kPMinus2 and kSqrtRatioC1 = (p - 3) / 4 are exponents.
+// sqrt(-Z) = sqrt(12) and the generator; kPMinus2, kSqrtRatioC1 = (p - 3) / 4 and kSqrtExp = (p + 1) / 4 are
+// exponents; kNR2 = R^2 mod n.
 
 #ifdef __CUDACC__
 #define HECUDA_P384_DEVICE(name, ...) static __constant__ Fe name##Device = {{__VA_ARGS__}};
@@ -86,10 +95,22 @@ HECUDA_P384_CONSTANTS(HECUDA_P384_HOST)
 #define P384_CONST(name) name##Host
 #endif
 
-// ---------------------------------------------------------------- field
-// r = t - p if t (with carry word `top`) >= p, else t
+// ---------------------------------------------------------------- field and scalars
+// The two moduli share one Montgomery code: ModP for the field, ModN for scalars mod the group order.  kM0 is the
+// per-word factor -m^-1 mod 2^32; it is 1 for p, so p's reduction step multiplies by the low word itself.
+struct ModP {
+    static constexpr uint32_t kM0 = 1;
+    P384_HD static const Fe &m() { return P384_CONST(kP); }
+};
+struct ModN {
+    static constexpr uint32_t kM0 = 0xe88fdc45u;
+    P384_HD static const Fe &m() { return P384_CONST(kN); }
+};
+
+// r = t - m if t (with carry word `top`) >= m, else t
+template <class M>
 P384_HD void reduce_once(Fe &r, const uint32_t t[kLimbs], uint32_t top) {
-    const Fe &p = P384_CONST(kP);
+    const Fe &p = M::m();
     uint32_t d[kLimbs];
     uint64_t borrow = 0;
     for (int i = 0; i < kLimbs; ++i) {
@@ -97,10 +118,12 @@ P384_HD void reduce_once(Fe &r, const uint32_t t[kLimbs], uint32_t top) {
         d[i] = (uint32_t)s;
         borrow = (s >> 32) & 1;
     }
-    const uint32_t keep = (uint32_t)0 - (uint32_t)(borrow & (uint64_t)(top == 0));  // all ones: t < p
+    const uint32_t keep = (uint32_t)0 - (uint32_t)(borrow & (uint64_t)(top == 0));  // all ones: t < m
     for (int i = 0; i < kLimbs; ++i) r.v[i] = (t[i] & keep) | (d[i] & ~keep);
 }
 
+// a + b mod m for a, b < m
+template <class M>
 P384_HD void add(Fe &r, const Fe &a, const Fe &b) {
     uint32_t t[kLimbs];
     uint64_t c = 0;
@@ -109,11 +132,14 @@ P384_HD void add(Fe &r, const Fe &a, const Fe &b) {
         t[i] = (uint32_t)c;
         c >>= 32;
     }
-    reduce_once(r, t, (uint32_t)c);
+    reduce_once<M>(r, t, (uint32_t)c);
 }
+P384_HD void add(Fe &r, const Fe &a, const Fe &b) { add<ModP>(r, a, b); }
 
+// a - b mod m for a, b < m
+template <class M>
 P384_HD void sub(Fe &r, const Fe &a, const Fe &b) {
-    const Fe &p = P384_CONST(kP);
+    const Fe &p = M::m();
     uint32_t t[kLimbs];
     uint64_t borrow = 0;
     for (int i = 0; i < kLimbs; ++i) {
@@ -121,7 +147,7 @@ P384_HD void sub(Fe &r, const Fe &a, const Fe &b) {
         t[i] = (uint32_t)s;
         borrow = (s >> 32) & 1;
     }
-    const uint32_t mask = (uint32_t)0 - (uint32_t)borrow;  // add p back after a borrow
+    const uint32_t mask = (uint32_t)0 - (uint32_t)borrow;  // add m back after a borrow
     uint64_t c = 0;
     for (int i = 0; i < kLimbs; ++i) {
         c += (uint64_t)t[i] + (p.v[i] & mask);
@@ -129,15 +155,17 @@ P384_HD void sub(Fe &r, const Fe &a, const Fe &b) {
         c >>= 32;
     }
 }
+P384_HD void sub(Fe &r, const Fe &a, const Fe &b) { sub<ModP>(r, a, b); }
 
 P384_HD void neg(Fe &r, const Fe &a) {
     Fe zero = {};
     sub(r, zero, a);
 }
 
-// a b R^-1 mod p by CIOS; a may be any value below 2^384 and b below p
+// a b R^-1 mod m by CIOS; a may be any value below 2^384 and b below m
+template <class M>
 P384_HD void mul(Fe &r, const Fe &a, const Fe &b) {
-    const Fe &p = P384_CONST(kP);
+    const Fe &p = M::m();
     uint32_t t[kLimbs + 2] = {};
     for (int i = 0; i < kLimbs; ++i) {
         const uint32_t bi = b.v[i];
@@ -149,7 +177,7 @@ P384_HD void mul(Fe &r, const Fe &a, const Fe &b) {
         c = (uint64_t)t[kLimbs] + (c >> 32);
         t[kLimbs] = (uint32_t)c;
         t[kLimbs + 1] = (uint32_t)(c >> 32);
-        const uint32_t m = t[0];  // t[0] * (-p^-1 mod 2^32), and -p^-1 = 1
+        const uint32_t m = t[0] * M::kM0;
         c = (uint64_t)m * p.v[0] + t[0];
         for (int j = 1; j < kLimbs; ++j) {
             c = (uint64_t)m * p.v[j] + t[j] + (c >> 32);
@@ -159,8 +187,9 @@ P384_HD void mul(Fe &r, const Fe &a, const Fe &b) {
         t[kLimbs - 1] = (uint32_t)c;
         t[kLimbs] = t[kLimbs + 1] + (uint32_t)(c >> 32);
     }
-    reduce_once(r, t, t[kLimbs]);
+    reduce_once<M>(r, t, t[kLimbs]);
 }
+P384_HD void mul(Fe &r, const Fe &a, const Fe &b) { mul<ModP>(r, a, b); }
 
 P384_HD void sqr(Fe &r, const Fe &a) { mul(r, a, a); }
 
@@ -243,17 +272,47 @@ P384_HD void to_bytes(unsigned char *be, const Fe &a) {
     for (int i = 0; i < kScalarBytes; ++i) be[i] = (unsigned char)(a.v[kLimbs - 1 - i / 4] >> (24 - 8 * (i & 3)));
 }
 
-// A 72-byte big-endian integer mod p, in Montgomery form: hi 2^384 + lo -> hi R^3 R^-1 + lo R^2 R^-1 = (hi 2^384 + lo) R
-P384_HD void from_bytes72(Fe &r, const unsigned char be[72]) {
-    Fe hi = {}, lo, a, b;
+// A 72-byte big-endian integer as hi 2^384 + lo
+P384_HD void split_bytes72(Fe &hi, Fe &lo, const unsigned char be[72]) {
+    hi = Fe{};
     for (int i = 0; i < 6; ++i) {
         const unsigned char *q = be + 4 * (5 - i);
         hi.v[i] = ((uint32_t)q[0] << 24) | ((uint32_t)q[1] << 16) | ((uint32_t)q[2] << 8) | q[3];
     }
     from_bytes(lo, be + 24);
+}
+
+// A 72-byte big-endian integer mod p, in Montgomery form: hi 2^384 + lo -> hi R^3 R^-1 + lo R^2 R^-1 = (hi 2^384 + lo) R
+P384_HD void from_bytes72(Fe &r, const unsigned char be[72]) {
+    Fe hi, lo, a, b;
+    split_bytes72(hi, lo, be);
     mul(a, hi, P384_CONST(kR3));
     mul(b, lo, P384_CONST(kR2));
     add(r, a, b);
+}
+
+// The same integer mod n as a plain integer (HashToScalar's reduction): hi R^2 R^-1 = hi 2^384 mod n, and lo < 2^384 <
+// 2n needs one conditional subtraction
+P384_HD void from_bytes72_mod_n(Fe &r, const unsigned char be[72]) {
+    Fe hi, lo, a, b;
+    split_bytes72(hi, lo, be);
+    mul<ModN>(a, hi, P384_CONST(kNR2));
+    reduce_once<ModN>(b, lo.v, 0);
+    add<ModN>(r, a, b);
+}
+
+// a b mod n for plain a < 2^384 and b < n: (a R^2 R^-1) b R^-1
+P384_HD void mul_mod_n(Fe &r, const Fe &a, const Fe &b) {
+    Fe t;
+    mul<ModN>(t, a, P384_CONST(kNR2));
+    mul<ModN>(r, t, b);
+}
+
+// a < b for plain integers, without a branch
+P384_HD bool less_than(const Fe &a, const Fe &b) {
+    uint64_t borrow = 0;
+    for (int i = 0; i < kLimbs; ++i) borrow = (((uint64_t)a.v[i] - b.v[i] - borrow) >> 32) & 1;
+    return borrow != 0;
 }
 
 // ---------------------------------------------------------------- group
@@ -354,16 +413,42 @@ P384_HD bool to_affine(Fe &x, Fe &y, const Point &p) {
 
 // SEC1 compressed encoding, 49 bytes (RFC 9497 SerializeElement); the identity (never produced by a valid key and a
 // hashed input, except with negligible probability) encodes as 49 zero bytes
-P384_HD void compress(unsigned char out[kElementBytes], const Point &p) {
-    Fe x, y, xp, yp;
-    if (!to_affine(x, y, p)) {
-        for (int i = 0; i < kElementBytes; ++i) out[i] = 0;
-        return;
-    }
+P384_HD void compress_affine(unsigned char out[kElementBytes], const Fe &x, const Fe &y) {
+    Fe xp, yp;
     from_mont(xp, x);
     from_mont(yp, y);
     out[0] = (unsigned char)(2 | (yp.v[0] & 1));
     to_bytes(out + 1, xp);
+}
+
+P384_HD void compress(unsigned char out[kElementBytes], const Point &p) {
+    Fe x, y;
+    if (!to_affine(x, y, p)) {
+        for (int i = 0; i < kElementBytes; ++i) out[i] = 0;
+        return;
+    }
+    compress_affine(out, x, y);
+}
+
+// RFC 9497 DeserializeElement: SEC1 compressed with prefix 2 or 3, x < p and x^3 - 3x + b a square; false otherwise.
+// The encoding is public, so this branches on it.  r = (x, y, 1) in Montgomery form.
+P384_HD bool decompress(Point &r, const unsigned char in[kElementBytes]) {
+    if (in[0] != 2 && in[0] != 3) return false;
+    Fe x, y2, y, t;
+    from_bytes(x, in + 1);
+    if (!less_than(x, P384_CONST(kP))) return false;
+    to_mont(r.x, x);
+    sqr(t, r.x);
+    add(t, t, P384_CONST(kA));
+    mul(y2, t, r.x);
+    add(y2, y2, P384_CONST(kB));
+    pow_fixed(y, y2, P384_CONST(kSqrtExp));  // p = 3 mod 4
+    sqr(t, y);
+    if (!equal(t, y2)) return false;
+    from_mont(t, y);
+    if ((t.v[0] & 1) != (in[0] & 1u)) neg(y, y);  // y = 0 has no point: the group's order is odd
+    r.y = y, r.z = P384_CONST(kOne);
+    return true;
 }
 
 // ---------------------------------------------------------------- hash to curve
@@ -404,30 +489,42 @@ P384_HD bool map_to_curve(Point &r, const Fe &u) {
     return gx1_square;
 }
 
-// expand_message_xmd(msg, DST, 144) with SHA-384 (RFC 9380 5.3.1), DST = HashToGroup-contextString
-P384_HD void expand_message_xmd(unsigned char out[144], const unsigned char *msg, long long len) {
-    const unsigned char *dst = (const unsigned char *)HECUDA_OPRF_HASH_TO_GROUP_DST;
-    sha512::Sha384 s;
+// expand_message_xmd(msg, DST, len_in_bytes) with SHA-384 (RFC 9380 5.3.1), in two halves so that a caller can stream
+// msg into the hasher: xmd_begin absorbs Z_pad, the caller absorbs msg, xmd_finish writes len_in_bytes (<= 255 * 48)
+// bytes to out.  DST is at most 255 bytes.
+P384_HD void xmd_begin(sha512::Sha384 &s) {
     s.init();
     s.zeros(128);  // Z_pad
-    s.bytes(msg, len);
-    s.byte(0), s.byte(144), s.byte(0);  // I2OSP(len_in_bytes, 2) || I2OSP(0, 1)
-    s.bytes(dst, kHashToGroupDstBytes), s.byte(kHashToGroupDstBytes);
-    unsigned char b0[48];
+}
+
+P384_HD void xmd_finish(unsigned char *out, int len_in_bytes, sha512::Sha384 &s, const char *dst_chars, int dst_len) {
+    const unsigned char *dst = (const unsigned char *)dst_chars;
+    s.byte((uint32_t)len_in_bytes >> 8), s.byte((uint32_t)len_in_bytes), s.byte(0);  // I2OSP(len, 2) || I2OSP(0, 1)
+    s.bytes(dst, dst_len), s.byte((uint32_t)dst_len);
+    unsigned char b0[48], bi[48];
     s.finish(b0);
-    for (int i = 1; i <= 3; ++i) {
+    for (int i = 1; 48 * (i - 1) < len_in_bytes; ++i) {
         s.init();
-        for (int j = 0; j < 48; ++j) s.byte(i == 1 ? b0[j] : (unsigned char)(b0[j] ^ out[48 * (i - 2) + j]));
-        s.byte(i);
-        s.bytes(dst, kHashToGroupDstBytes), s.byte(kHashToGroupDstBytes);
-        s.finish(out + 48 * (i - 1));
+        for (int j = 0; j < 48; ++j) s.byte(i == 1 ? b0[j] : (unsigned char)(b0[j] ^ bi[j]));
+        s.byte((uint32_t)i);
+        s.bytes(dst, dst_len), s.byte((uint32_t)dst_len);
+        s.finish(bi);
+        for (int j = 0; j < 48 && 48 * (i - 1) + j < len_in_bytes; ++j) out[48 * (i - 1) + j] = bi[j];
     }
+}
+
+P384_HD void expand_message_xmd(unsigned char *out, int len_in_bytes, const unsigned char *msg, long long len,
+                                const char *dst, int dst_len) {
+    sha512::Sha384 s;
+    xmd_begin(s);
+    s.bytes(msg, len);
+    xmd_finish(out, len_in_bytes, s, dst, dst_len);
 }
 
 // HashToGroup(msg): hash_to_field (two 72-byte field elements), map both, add
 P384_HD void hash_to_group(Point &r, const unsigned char *msg, long long len) {
     unsigned char uniform[144];
-    expand_message_xmd(uniform, msg, len);
+    expand_message_xmd(uniform, 144, msg, len, HECUDA_OPRF_HASH_TO_GROUP_DST, kHashToGroupDstBytes);
     Fe u0, u1;
     from_bytes72(u0, uniform);
     from_bytes72(u1, uniform + 72);
@@ -439,28 +536,22 @@ P384_HD void hash_to_group(Point &r, const unsigned char *msg, long long len) {
 
 // ---------------------------------------------------------------- scalar multiplication
 // 0 < k < n for a plain 384-bit k
-P384_HD bool scalar_valid(const Fe &k) {
-    if (is_zero(k)) return false;
-    const Fe &n = P384_CONST(kN);
-    for (int i = kLimbs - 1; i >= 0; --i)
-        if (k.v[i] != n.v[i]) return k.v[i] < n.v[i];
-    return false;
-}
+P384_HD bool scalar_valid(const Fe &k) { return !is_zero(k) && less_than(k, P384_CONST(kN)); }
 
-// The recoding of a valid k, done once on the host: k is made odd (k' = n - k and flip = 1 when k is even, since n is
-// odd), then k' = sum d_i 16^i with 96 odd digits |d_i| <= 15, d_95 > 0 (regular signed windows).  digits[96] = flip.
+// The recoding of a k in [0, n - 1]: k is made odd (k' = n - k and flip = 1 when k is even, since n is odd), then
+// k' = sum d_i 16^i with 96 odd digits |d_i| <= 15, d_95 > 0 (regular signed windows).  digits[96] = flip.  No branch
+// or address depends on k, so a thread can recode its own secret scalar; the shared key is recoded once on the host.
 P384_HD void recode_scalar(const Fe &k, signed char digits[kDigits + 1]) {
     const Fe &n = P384_CONST(kN);
-    Fe w = k;
-    const int flip = (k.v[0] & 1) == 0;
-    if (flip) {
-        uint64_t borrow = 0;
-        for (int i = 0; i < kLimbs; ++i) {
-            const uint64_t s = (uint64_t)n.v[i] - k.v[i] - borrow;
-            w.v[i] = (uint32_t)s;
-            borrow = (s >> 32) & 1;
-        }
+    Fe w, nk;
+    const uint32_t flip = (k.v[0] & 1) ^ 1;
+    uint64_t borrow = 0;
+    for (int i = 0; i < kLimbs; ++i) {
+        const uint64_t s = (uint64_t)n.v[i] - k.v[i] - borrow;
+        nk.v[i] = (uint32_t)s;
+        borrow = (s >> 32) & 1;
     }
+    select(w, flip != 0, nk, k);
     for (int d = 0; d < kDigits - 1; ++d) {
         const int digit = (int)(w.v[0] & 31) - 16;
         digits[d] = (signed char)digit;
@@ -502,6 +593,43 @@ P384_HD void scalar_mul(Point &r, const Point &p, const signed char *digits) {
     r = acc;
 }
 
+// q = sign(digit) table[(|digit| - 1) / 2] for an odd digit, reading all eight entries and negating with a mask
+P384_HD void lookup_ct(Point &q, const Point table[kTable], int digit) {
+    const int sign = digit >> 31;  // -1 or 0
+    const int index = (((digit ^ sign) - sign) - 1) >> 1;
+    q = table[0];
+    for (int i = 1; i < kTable; ++i) {
+        const bool hit = i == index;
+        select(q.x, hit, table[i].x, q.x);
+        select(q.y, hit, table[i].y, q.y);
+        select(q.z, hit, table[i].z, q.z);
+    }
+    Fe ny;
+    neg(ny, q.y);
+    select(q.y, sign != 0, ny, q.y);
+}
+
+// k P for a secret scalar of this thread alone (the proof nonce), recoded on the device: scalar_mul's operation
+// sequence, with every table read through lookup_ct and the final flip applied with a mask, so no branch and no memory
+// address depends on k.  add()'s identity and equal-inputs branches remain; a uniformly random k reaches them only if
+// a partial sum of the ladder is the identity or +-(the entry being added), which has negligible probability.
+P384_HD void scalar_mul_ct(Point &r, const Point &p, const signed char digits[kDigits + 1]) {
+    Point table[kTable], twice, acc, q;
+    table[0] = p;
+    dbl(twice, p);
+    for (int i = 1; i < kTable; ++i) add(table[i], table[i - 1], twice);
+    lookup_ct(acc, table, digits[kDigits - 1]);
+    for (int d = kDigits - 2; d >= 0; --d) {
+        for (int s = 0; s < kWindow; ++s) dbl(acc, acc);
+        lookup_ct(q, table, digits[d]);
+        add(acc, acc, q);
+    }
+    Fe ny;
+    neg(ny, acc.y);
+    select(acc.y, digits[kDigits] != 0, ny, acc.y);
+    r = acc;
+}
+
 P384_HD void generator(Point &g) {
     g.x = P384_CONST(kGx), g.y = P384_CONST(kGy), g.z = P384_CONST(kOne);
 }
@@ -523,6 +651,133 @@ P384_HD void oprf_evaluate(unsigned char out[kOutputBytes], const signed char *d
     s.bytes(issued, kElementBytes);
     s.bytes((const unsigned char *)"Finalize", 8);
     s.finish(out);
+}
+
+// ---------------------------------------------------------------- VOPRF BlindEvaluate with the DLEQ proof
+// RFC 9497 3.3.2 BlindEvaluate and 2.2.1 GenerateProof with ComputeCompositesFast, for a proof over one element, as
+// swift-crypto's P384._VOPRF.PrivateKey.evaluate returns it: Ser(k B) || I2OSP(c, 48) || I2OSP(s, 48).  A query is
+// answered in two halves, blind_evaluate_composite then generate_proof, with the composite M passed between them.
+#define HECUDA_OPRF_HASH_TO_SCALAR_DST "HashToScalar-" HECUDA_OPRF_CONTEXT_STRING
+#define HECUDA_OPRF_SEED_DST "Seed-" HECUDA_OPRF_CONTEXT_STRING
+#define HECUDA_OPRF_PROOF_NONCE_DST "HECUDA-ProofNonce-" HECUDA_OPRF_CONTEXT_STRING  // see proof_nonce
+constexpr int kHashToScalarDstBytes = (int)sizeof(HECUDA_OPRF_HASH_TO_SCALAR_DST) - 1;  // 33
+constexpr int kSeedDstBytes = (int)sizeof(HECUDA_OPRF_SEED_DST) - 1;                    // 25
+constexpr int kProofNonceDstBytes = (int)sizeof(HECUDA_OPRF_PROOF_NONCE_DST) - 1;       // 38
+constexpr int kSeedBytes = 48, kNonceSeedBytes = 32, kProofBytes = 96;
+constexpr int kResponseBytes = kElementBytes + kProofBytes;  // 145
+
+P384_HD void i2osp2(sha512::Sha384 &s, int v) { s.byte((uint32_t)v >> 8), s.byte((uint32_t)v); }
+
+// HashToScalar(msg): hash_to_field(msg, 1) with modulus n, L = 72 and DST "HashToScalar-" || contextString, for a msg
+// the caller absorbed after xmd_begin
+P384_HD void hash_to_scalar_finish(Fe &r, sha512::Sha384 &s) {
+    unsigned char u[72];
+    xmd_finish(u, 72, s, HECUDA_OPRF_HASH_TO_SCALAR_DST, kHashToScalarDstBytes);
+    from_bytes72_mod_n(r, u);
+}
+
+// ComputeCompositesFast's seed for bm = SerializeElement(k G): SHA-384(I2OSP(49, 2) || bm || I2OSP(25, 2) || "Seed-"
+// || contextString), the same for every query under one key
+P384_HD void composite_seed(unsigned char seed[kSeedBytes], const unsigned char bm[kElementBytes]) {
+    sha512::Sha384 s;
+    s.init();
+    i2osp2(s, kElementBytes);
+    s.bytes(bm, kElementBytes);
+    i2osp2(s, kSeedDstBytes);
+    s.bytes((const unsigned char *)HECUDA_OPRF_SEED_DST, kSeedDstBytes);
+    s.finish(seed);
+}
+
+// d0 = HashToScalar(I2OSP(48, 2) || seed || I2OSP(0, 2) || I2OSP(49, 2) || Ser(B) || I2OSP(49, 2) || Ser(D) ||
+// "Composite")
+P384_HD void composite_scalar(Fe &d0, const unsigned char seed[kSeedBytes], const unsigned char blinded[kElementBytes],
+                              const unsigned char evaluated[kElementBytes]) {
+    sha512::Sha384 s;
+    xmd_begin(s);
+    i2osp2(s, kSeedBytes);
+    s.bytes(seed, kSeedBytes);
+    i2osp2(s, 0);
+    i2osp2(s, kElementBytes);
+    s.bytes(blinded, kElementBytes);
+    i2osp2(s, kElementBytes);
+    s.bytes(evaluated, kElementBytes);
+    s.bytes((const unsigned char *)"Composite", 9);
+    hash_to_scalar_finish(d0, s);
+}
+
+// The first half: B = DeserializeElement(query), evaluated = Ser(D) with D = k B, and M = d0 B in affine Montgomery
+// coordinates (mx, my).  A valid query is its own Ser(B): x < p and the prefix's parity bit make the encoding unique.
+// d0 is public, so M uses scalar_mul.  False for an invalid query, and for M the identity (d0 = 0, negligible).
+P384_HD bool blind_evaluate_composite(unsigned char evaluated[kElementBytes], Fe &mx, Fe &my,
+                                      const unsigned char query[kElementBytes], const signed char *k_digits,
+                                      const unsigned char seed[kSeedBytes]) {
+    Point b, p;
+    if (!decompress(b, query)) return false;
+    scalar_mul(p, b, k_digits);
+    compress(evaluated, p);
+    Fe d0;
+    composite_scalar(d0, seed, query, evaluated);
+    signed char digits[kDigits + 1];
+    recode_scalar(d0, digits);
+    scalar_mul(p, b, digits);
+    return to_affine(mx, my, p);
+}
+
+// The proof nonce r = OS2IP(expand_message_xmd(I2OSP(k, 48) || seed32 || Ser(B), "HECUDA-ProofNonce-" ||
+// contextString, 72)) mod n.  RFC 9497 draws r at random, and any r in [1, n - 1] gives a proof that a verifier accepts.
+// Reusing one r under two different challenges reveals k = (s1 - s2) / (c2 - c1); deriving r from (k, B), hedged with
+// the caller's seed32, makes a repeated seed harmless, since equal (k, B) give equal challenges.
+P384_HD void proof_nonce(Fe &r, const Fe &k, const unsigned char seed32[kNonceSeedBytes],
+                         const unsigned char query[kElementBytes]) {
+    unsigned char kb[kScalarBytes], u[72];
+    to_bytes(kb, k);
+    sha512::Sha384 s;
+    xmd_begin(s);
+    s.bytes(kb, kScalarBytes);
+    s.bytes(seed32, kNonceSeedBytes);
+    s.bytes(query, kElementBytes);
+    xmd_finish(u, 72, s, HECUDA_OPRF_PROOF_NONCE_DST, kProofNonceDstBytes);
+    from_bytes72_mod_n(r, u);
+}
+
+// The second half, GenerateProof: Z = k M, t2 = r G, t3 = r M, c = HashToScalar(I2OSP(49, 2) || bm || I2OSP(49, 2) ||
+// Ser(M) || I2OSP(49, 2) || Ser(Z) || I2OSP(49, 2) || Ser(t2) || I2OSP(49, 2) || Ser(t3) || "Challenge") and
+// s = r - c k mod n, written as proof = I2OSP(c, 48) || I2OSP(s, 48).  k is plain, in [1, n - 1], with its recoding
+// k_digits; r in [1, n - 1] is secret and differs per thread, so t2 and t3 run through scalar_mul_ct.
+P384_HD void generate_proof(unsigned char proof[kProofBytes], const signed char *k_digits, const Fe &k,
+                            const unsigned char bm[kElementBytes], const Fe &mx, const Fe &my, const Fe &r) {
+    sha512::Sha384 s;
+    xmd_begin(s);
+    unsigned char e[kElementBytes];
+    i2osp2(s, kElementBytes);
+    s.bytes(bm, kElementBytes);
+    compress_affine(e, mx, my);
+    i2osp2(s, kElementBytes);
+    s.bytes(e, kElementBytes);
+    Point m, g, p;
+    m.x = mx, m.y = my, m.z = P384_CONST(kOne);
+    scalar_mul(p, m, k_digits);
+    compress(e, p);
+    i2osp2(s, kElementBytes);
+    s.bytes(e, kElementBytes);
+    signed char digits[kDigits + 1];
+    recode_scalar(r, digits);
+    generator(g);
+    scalar_mul_ct(p, g, digits);
+    compress(e, p);
+    i2osp2(s, kElementBytes);
+    s.bytes(e, kElementBytes);
+    scalar_mul_ct(p, m, digits);
+    compress(e, p);
+    i2osp2(s, kElementBytes);
+    s.bytes(e, kElementBytes);
+    s.bytes((const unsigned char *)"Challenge", 9);
+    Fe c, ck;
+    hash_to_scalar_finish(c, s);
+    mul_mod_n(ck, c, k);
+    sub<ModN>(ck, r, ck);
+    to_bytes(proof, c);
+    to_bytes(proof + kScalarBytes, ck);
 }
 
 #undef P384_CONST

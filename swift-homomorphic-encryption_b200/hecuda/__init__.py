@@ -117,6 +117,7 @@ SYMBOLS = {
     "hecuda_oprf_public_key": (C.c_int32, [_VP, _VP]),
     "hecuda_oprf_evaluate": (C.c_int32, [_VP, _VP, _VP, C.c_int64, _VP]),
     "hecuda_symmetric_pir_process": (C.c_int32, [_VP, _VP, _VP, _VP, _VP, C.c_int64, _VP, _VP]),
+    "hecuda_oprf_blind_evaluate": (C.c_int32, [_VP, _VP, C.c_int64, _VP, _VP, _VP]),
     "hecuda_mulpir_expand": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP]),
     "hecuda_mulpir_expand_device": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP, _VP]),
     "hecuda_mulpir_compute_response": (C.c_int32, [_VP, _VP, C.POINTER(_VP), C.c_int32, C.POINTER(C.c_int32), C.c_int32,

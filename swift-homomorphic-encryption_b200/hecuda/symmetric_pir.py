@@ -4,15 +4,17 @@ Names follow Sources/PrivateInformationRetrieval/SymmetricPir/SymmetricPirDataba
 
     SymmetricPirConfigType, SymmetricPirClientConfig, SymmetricPirConfig   :21-184
     KeywordDatabase.symmetricPIRProcess                                    :186-211 (hecuda.keyword_pir)
+    OprfServer                        SymmetricPir/SymmetricPirProtocol.swift:39-59
 
 The OPRF is RFC 9497 in VOPRF mode over P384-SHA384 (swift-crypto's P384._VOPRF), evaluated on the device one thread
-per row; the rows' AES-GCM-192 sealing runs there too.
+per row; the rows' AES-GCM-192 sealing runs there too, and so do the server's answers to clients' blinded queries.
 """
 from __future__ import annotations
 
 import enum
+import secrets
 from dataclasses import dataclass
-from typing import List, Sequence, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -20,6 +22,7 @@ from . import _check, _ptr, load_library
 from .pir import PirError
 
 OPRF_KEY_BYTES, OPRF_ELEMENT_BYTES, OPRF_OUTPUT_BYTES = 48, 49, 48  # HECUDA_OPRF_*
+OPRF_RESPONSE_BYTES, OPRF_SEED_BYTES = 145, 32
 
 
 def _concatenate(blobs: Sequence[bytes]):
@@ -129,3 +132,44 @@ def symmetricPIRProcess(database: Sequence[Tuple[bytes, bytes]], config: Symmetr
                                                        _ptr(values_out)))
     kw, raw = keywords_out.tobytes(), values_out.tobytes()
     return [(kw[16 * i:16 * (i + 1)], raw[int(voff[i]) + tag * i:int(voff[i + 1]) + tag * (i + 1)]) for i in range(count)]
+
+
+class OprfServer:
+    """OprfServer (SymmetricPirProtocol.swift:39-59): answers clients' blinded OPRF queries on the device with RFC 9497
+    BlindEvaluate and its DLEQ proof.  A response is the 145 bytes swift-crypto's BlindEvaluation(rawRepresentation:)
+    takes: the evaluated element, then the proof's c and s.
+
+    `seed` (32 bytes, random by default) hedges the proof nonce, which is derived from the key and the query: the
+    same seed gives the same response, and no seed can make two different challenges share a nonce."""
+
+    def __init__(self, symmetricPirConfig: SymmetricPirConfig):
+        if symmetricPirConfig.configType is not SymmetricPirConfigType.OPRF_P384_AES_GCM_192_NONCE_96_TAG_128:
+            raise PirError(f"invalidSymmetricPirConfig(symmetricPirConfig: {symmetricPirConfig})")
+        self._key = _key(symmetricPirConfig.oprfSecretKey)
+
+    def computeResponse(self, query: bytes, seed: Optional[bytes] = None) -> bytes:
+        """computeResponse(query:): PirError when the query is not a valid compressed P-384 point."""
+        response = self.computeResponses([query], seed)[0]
+        if response is None:
+            raise PirError("invalidOprfQuery: not a valid SEC1-compressed P-384 element")
+        return response
+
+    def computeResponses(self, queries: Sequence[bytes], seed: Optional[bytes] = None) -> List[Optional[bytes]]:
+        """One response per query in one device call; None where a query is invalid, including a wrong length."""
+        seed = secrets.token_bytes(OPRF_SEED_BYTES) if seed is None else bytes(seed)
+        if len(seed) != OPRF_SEED_BYTES:
+            raise PirError(f"OPRF proof seed must be {OPRF_SEED_BYTES} bytes, got {len(seed)}")
+        queries = [bytes(q) for q in queries]
+        sized = [i for i, q in enumerate(queries) if len(q) == OPRF_ELEMENT_BYTES]
+        count = len(sized)
+        blinded = np.frombuffer(b"".join(queries[i] for i in sized) or b"\0", dtype=np.uint8)
+        responses = np.zeros((max(count, 1), OPRF_RESPONSE_BYTES), dtype=np.uint8)
+        status = np.ones(max(count, 1), dtype=np.uint8)
+        _check(load_library().hecuda_oprf_blind_evaluate(_ptr(self._key), _ptr(blinded), count,
+                                                         _ptr(np.frombuffer(seed, dtype=np.uint8)), _ptr(responses),
+                                                         _ptr(status)))
+        out: List[Optional[bytes]] = [None] * len(queries)
+        for j, i in enumerate(sized):
+            if status[j] == 0:
+                out[i] = responses[j].tobytes()
+        return out
