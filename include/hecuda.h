@@ -452,6 +452,53 @@ int32_t hecuda_oprf_blind_evaluate(const uint8_t *secret_key, const uint8_t *bli
                                    int64_t count, const uint8_t *seed /* 32 */,
                                    uint8_t *responses /* count x 145 */, uint8_t *status /* count: 0 ok, 1 invalid */);
 
+/* ---- SimplePIR: Sources/PrivateInformationRetrieval/SimplePir/ ----
+ * SimplePirServer<Scalar> with Scalar = UInt32 (word_bits 32) or UInt64 (word_bits 64): requests, responses, the hint and
+ * the processed database cross the boundary as little-endian words of that width.  These calls need no context; the
+ * hint's single-modulus context over nttFriendlyMod (the smallest NTT prime of ct + 1 bits for degree N,
+ * SimplePirContext.swift:78-81) is built inside hecuda_simple_pir_process.  The processed database DB' is columnSize (M)
+ * x databaseColumns (K) and stays on the device as ceil(pt / 8) planes of u8 digits.  Every parameter the reference
+ * derives is rechecked before anything is allocated (SimplePir.swift:47-79, :144-155): N a power of two, ct > pt,
+ * entriesPerColumn == 1 || chunksPerEntry == 1, positive sizes -> HECUDA_ERR_INVALID_ARGUMENT; ct + 1 above word_bits
+ * (generatePrimes fails there), nttFriendlyMod >= 2^62 (ct > 61) or N > 2^15 -> HECUDA_ERR_UNSUPPORTED.  Null pointers
+ * and negative counts are refused with no kernel launched.  The security bound maxLog2CoefficientModulus
+ * (EncryptionParameters.swift:192-219) is checked by the Python layer (hecuda.simple_pir.SimplePirEncryptionParams). */
+typedef struct hecuda_simple_pir_database hecuda_simple_pir_database; /* SimplePirServer's processedDatabase, resident */
+typedef struct hecuda_simple_pir_params {                            /* SimplePirParameters (SimplePir.swift:95-160) */
+    int32_t plaintext_modulus_bits;  /* pt */
+    int32_t ciphertext_modulus_bits; /* ct */
+    int64_t lattice_dimension;       /* N */
+    int64_t entry_size;              /* entrySizeInBytes */
+    int64_t entries_per_column;
+    int64_t chunks_per_entry;
+    int64_t database_columns;        /* K */
+    int32_t word_bits;               /* 32 or 64: the Scalar type */
+} hecuda_simple_pir_params;
+/* SimplePirServer.process(database:encryptionParams:seed:) (SimplePir+Database.swift:252-290) after computingParams
+ * (:208-243): entries entry_count x entry_size bytes; seed 32 bytes (params.seed).  Entry e's bytesToCoefficients at pt
+ * bits go to e * paddedEntrySize of the K x M matrix, which is transposed to DB' (M x K) and kept on the device as *out.
+ * hint (M x N words) = DB' . A mod nttFriendlyMod, A the stacked negacyclic matrices of the aPolyCount = ceil(K / N)
+ * polynomials PolyRq.random draws from NistAes128Ctr(seed) (:177-206); computed through the NTT without materialising A.
+ * Refused: entry_count < 1, or entries that do not fit K x M (HECUDA_ERR_INVALID_ARGUMENT). */
+int32_t hecuda_simple_pir_process(const uint8_t *entries, int64_t entry_count, const hecuda_simple_pir_params *params,
+                                  const uint8_t *seed, void *hint, hecuda_simple_pir_database **out);
+/* SimplePirServer(processedDatabase:hint:params:) (SimplePir+Server.swift:24-29): processed is DB', M x K words.  A value
+ * >= 2^pt is refused with HECUDA_ERR_INVALID_ARGUMENT (the digit planes hold pt bits; process never produces one). */
+int32_t hecuda_simple_pir_database_create(const void *processed, const hecuda_simple_pir_params *params,
+                                          hecuda_simple_pir_database **out);
+/* SimplePirDatabase.database (for save(to:), SimplePir+Database.swift:95-121): DB' as M x K words. */
+int32_t hecuda_simple_pir_database_export(const hecuda_simple_pir_database *database, void *processed);
+int32_t hecuda_simple_pir_database_destroy(hecuda_simple_pir_database *database);
+/* SimplePirServer.computeResponse(to:) (SimplePir+Server.swift:31-38, Array2d.multiply(transposing:mask:),
+ * SimplePir+Precompute.swift:51-114) for `count` requests at once: requests count x chunksPerEntry x K words, responses
+ * count x chunksPerEntry x M words, response i = transpose((DB' . request_i^T) mod 2^ct).  Request bits at or above ct do
+ * not change the result, as in the reference.  The _device variant follows the conventions above (stream order,
+ * stream-ordered scratch, graph capture, 16-byte alignment). */
+int32_t hecuda_simple_pir_compute_response(const hecuda_simple_pir_database *database, const void *requests, int64_t count,
+                                           void *responses);
+int32_t hecuda_simple_pir_compute_response_device(const hecuda_simple_pir_database *database, const void *requests,
+                                                  int64_t count, void *responses, void *stream);
+
 /* PirUtil.expand(ciphertexts:outputCount:using:) -- IndexPir/PirUtil.swift:321-355 (expandCiphertext :249-304,
  * expandCiphertextForOneStep :204-236).  ciphertexts: ciphertext_count x 2 x L x N (Coeff); out: output_count x 2 x L x N,
  * output i encrypting the constant polynomial whose constant is coefficient i of the inputs (x 2^ceilLog2(count)).

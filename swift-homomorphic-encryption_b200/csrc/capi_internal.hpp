@@ -172,6 +172,10 @@ cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batc
                         cudaStream_t s);
 void free_chains(unsigned int *d_rk, u64 *d_ctr, int segments, int64_t batch, cudaStream_t s);
 cudaError_t drbg_tables(const unsigned char **sbox, const unsigned int **te0);
+// PolyRq.random mod p of `polys` degree-n polynomials from the one stream of the 32-byte d_seed (coefficient k of
+// polynomial j is the stream's (jN + k)-th 128-bit word mod p), stored as sigma(a) = a(x^-1) (simple_pir.cuh)
+cudaError_t random_sigma_polys_device(const unsigned char *d_seed, u64 p, int64_t n, int64_t polys, u64 *d_out,
+                                      cudaStream_t s);
 cudaError_t inner_product_chunk(const Context &c, u64 *scratch, const u64 *lhs, const u64 *rhs, int64_t pairs, u64 *out,
                                 int64_t groups, cudaStream_t s);
 // `tables` MulPir databases from entry bytes already on the device (pir.cu; used by keyword_pir.cu)

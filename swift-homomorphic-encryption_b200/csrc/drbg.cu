@@ -17,6 +17,7 @@
 #include "capi_internal.hpp"
 #include "drbg.cuh"
 #include "modarith.cuh"
+#include "simple_pir.cuh"
 
 using namespace hecuda;
 using namespace hecuda::api;
@@ -33,6 +34,17 @@ __device__ __forceinline__ void load_tables(unsigned char *sbox, u32w *te0) {
         te0[i] = c_te0[i];
     }
     __syncthreads();
+}
+
+// The 128-bit word of this thread's block (counter V + 1 + threadIdx.x) of a segment whose (V hi, V lo) is at ctr:
+// UInt128(littleEndianBytes:) of the 16 output bytes, byte i of the block being bits 8i.. of the value
+__device__ __forceinline__ u128 segment_word(const u32w *rk, const u64 *ctr, const u32w *te0, const unsigned char *sbox) {
+    u32w blk[4];
+    counter_block(ctr[0], ctr[1], 1 + (u64)threadIdx.x, blk);
+    encrypt_block(blk, rk, te0, sbox);
+    const u64 lo = (u64)__byte_perm(blk[0], 0, 0x0123) | ((u64)__byte_perm(blk[1], 0, 0x0123) << 32);
+    const u64 hi = (u64)__byte_perm(blk[2], 0, 0x0123) | ((u64)__byte_perm(blk[3], 0, 0x0123) << 32);
+    return ((u128)hi << 64) | lo;
 }
 
 // two lanes per seed walk its chain of segments: both expand the current key, lane p encrypts counter block V + 1 + p,
@@ -88,14 +100,26 @@ __global__ void __launch_bounds__(kSegmentBlocks) drbg_fill_kernel(const u32w *_
     load_tables(sbox, te0);
     const long long k = (long long)s * kSegmentBlocks + threadIdx.x;
     if (k >= (long long)c.rows * n) return;
-    u32w blk[4];
-    counter_block(counters[2 * ((size_t)b * segments + s)], counters[2 * ((size_t)b * segments + s) + 1], 1 + (u64)threadIdx.x, blk);
-    encrypt_block(blk, rk, te0, sbox);
-    // UInt128(littleEndianBytes:) of the 16 output bytes: byte i of the block is bits 8i.. of the value
-    const u64 lo = (u64)__byte_perm(blk[0], 0, 0x0123) | ((u64)__byte_perm(blk[1], 0, 0x0123) << 32);
-    const u64 hi = (u64)__byte_perm(blk[2], 0, 0x0123) | ((u64)__byte_perm(blk[3], 0, 0x0123) << 32);
     const int row = (int)(k / n);
-    out[(size_t)b * c.rows * n + k] = (u64)((((u128)hi << 64) | lo) % c.p[row]);
+    out[(size_t)b * c.rows * n + k] = (u64)(segment_word(rk, counters + 2 * ((size_t)b * segments + s), te0, sbox) % c.p[row]);
+}
+
+// PolyRq.random over one modulus for `total` = polys x N coefficients of one stream (SimplePirContext
+// .generateAPolynomials, SimplePir+Database.swift:181-184), stored as sigma(a) = a(x^-1) (simple_pir.cuh)
+__global__ void __launch_bounds__(kSegmentBlocks) drbg_sigma_fill_kernel(const u32w *__restrict__ round_keys,
+                                                                         const u64 *__restrict__ counters, u64 *__restrict__ out,
+                                                                         u64 p, long long n, long long total) {
+    __shared__ unsigned char sbox[256];
+    __shared__ u32w te0[256];
+    __shared__ u32w rk[kRoundKeyWords];
+    const int s = blockIdx.x;
+    if (threadIdx.x < kRoundKeyWords) rk[threadIdx.x] = round_keys[(size_t)s * kRoundKeyWords + threadIdx.x];
+    load_tables(sbox, te0);
+    const long long k = (long long)s * kSegmentBlocks + threadIdx.x;
+    if (k >= total) return;
+    const u64 v = (u64)(segment_word(rk, counters + 2 * (size_t)s, te0, sbox) % p);
+    const long long poly = k / n, i = k - poly * n;
+    out[poly * n + spir::sigma_index(i, n)] = spir::sigma_value(v, i, p);
 }
 
 // EvaluationKey(deserialize:) of seeded key-switching ciphertexts (SerializedCiphertext.swift:53-60 with Format = Eval):
@@ -117,17 +141,13 @@ __global__ void __launch_bounds__(kSegmentBlocks) key_expand_kernel(const u32w *
     load_tables(sbox, te0);
     const long long k = (long long)s * kSegmentBlocks + threadIdx.x;
     if (k >= (long long)c.rows * n) return;
-    u32w blk[4];
-    counter_block(counters[2 * ((size_t)b * segments + s)], counters[2 * ((size_t)b * segments + s) + 1], 1 + (u64)threadIdx.x, blk);
-    encrypt_block(blk, rk, te0, sbox);
-    const u64 lo = (u64)__byte_perm(blk[0], 0, 0x0123) | ((u64)__byte_perm(blk[1], 0, 0x0123) << 32);
-    const u64 hi = (u64)__byte_perm(blk[2], 0, 0x0123) | ((u64)__byte_perm(blk[3], 0, 0x0123) << 32);
+    const u128 word = segment_word(rk, counters + 2 * ((size_t)b * segments + s), te0, sbox);
     const int row = (int)(k / n);
     const long long i = k - (long long)row * n;
     const unsigned char *src = poly0 + b * cc.byte_offset[cc.rows] + cc.byte_offset[row];
     u64 *out = dst[b];
     out[k] = codec_unpack(src, cc.byte_offset[row + 1] - cc.byte_offset[row], cc.width[row], i);
-    out[(long long)c.rows * n + k] = (u64)((((u128)hi << 64) | lo) % c.p[row]);
+    out[(long long)c.rows * n + k] = (u64)(word % c.p[row]);
 }
 
 }  // namespace
@@ -158,6 +178,22 @@ void free_chains(u32w *d_rk, u64 *d_ctr, int segments, int64_t batch, cudaStream
         cudaFreeAsync(d_rk, s);
     }
     if (d_ctr) cudaFreeAsync(d_ctr, s);
+}
+
+// PolyRq.random mod p for `polys` polynomials of degree n from the one NistAes128Ctr stream of the 32-byte d_seed,
+// written as sigma(a) (drbg_sigma_fill_kernel) to d_out (polys x n)
+cudaError_t random_sigma_polys_device(const unsigned char *d_seed, u64 p, int64_t n, int64_t polys, u64 *d_out,
+                                      cudaStream_t s) {
+    const int64_t total = polys * n;
+    const int segments = (int)((total * 16 + kSegmentBytes - 1) / kSegmentBytes);
+    u32w *d_rk = nullptr;
+    u64 *d_ctr = nullptr;
+    cudaError_t e = drbg_chains(d_seed, segments, 1, &d_rk, &d_ctr, s);
+    if (e == cudaSuccess)
+        e = launch(drbg_sigma_fill_kernel, (unsigned)segments, kSegmentBlocks, 0, s, d_rk, d_ctr, d_out, p, (long long)n,
+                   (long long)total);
+    free_chains(d_rk, d_ctr, segments, 1, s);
+    return e;
 }
 
 // Device addresses of the AES tables drbg_chains uploads, for kernels in other translation units that read a stream

@@ -118,6 +118,12 @@ SYMBOLS = {
     "hecuda_oprf_evaluate": (C.c_int32, [_VP, _VP, _VP, C.c_int64, _VP]),
     "hecuda_symmetric_pir_process": (C.c_int32, [_VP, _VP, _VP, _VP, _VP, C.c_int64, _VP, _VP]),
     "hecuda_oprf_blind_evaluate": (C.c_int32, [_VP, _VP, C.c_int64, _VP, _VP, _VP]),
+    "hecuda_simple_pir_process": (C.c_int32, [_VP, C.c_int64, _VP, _VP, _VP, C.POINTER(_VP)]),
+    "hecuda_simple_pir_database_create": (C.c_int32, [_VP, _VP, C.POINTER(_VP)]),
+    "hecuda_simple_pir_database_export": (C.c_int32, [_VP, _VP]),
+    "hecuda_simple_pir_database_destroy": (C.c_int32, [_VP]),
+    "hecuda_simple_pir_compute_response": (C.c_int32, [_VP, _VP, C.c_int64, _VP]),
+    "hecuda_simple_pir_compute_response_device": (C.c_int32, [_VP, _VP, C.c_int64, _VP, _VP]),
     "hecuda_mulpir_expand": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP]),
     "hecuda_mulpir_expand_device": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP, _VP]),
     "hecuda_mulpir_compute_response": (C.c_int32, [_VP, _VP, C.POINTER(_VP), C.c_int32, C.POINTER(C.c_int32), C.c_int32,
