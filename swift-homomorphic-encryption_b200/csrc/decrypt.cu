@@ -199,20 +199,6 @@ __global__ void __launch_bounds__(kNormThreads) noise_norm_kernel(const u64 *__r
     for (int w = 0; w < W; ++w) out[item * W + w] = best[w];
 }
 
-// x (w little-endian words) as a Double, rounded to nearest (ties to even) like Double(_:) of a wide integer
-double wide_to_double(const u64 *x, int w) {
-    int top = w - 1;
-    while (top >= 0 && !x[top]) --top;
-    if (top < 0) return 0.0;
-    if (top == 0) return (double)x[0];
-    const int lz = __builtin_clzll(x[top]);
-    u64 m = lz ? (x[top] << lz) | (x[top - 1] >> (64 - lz)) : x[top];  // the leading 64 bits
-    bool sticky = lz ? (x[top - 1] << lz) != 0 : false;
-    for (int i = top - 2; i >= 0 && !sticky; --i) sticky = x[i] != 0;
-    if (sticky) m |= 1;  // far below the rounding bit of the 53-bit result: only breaks ties
-    return std::ldexp((double)m, 64 * top - lz);
-}
-
 // big = [q / q_i for each i][q][(q + 1) / 2] as l-word integers
 std::vector<u64> noise_big_constants(const u64 *q, int l) {
     std::vector<u64> big((size_t)(l + 2) * l, 0);
@@ -376,7 +362,7 @@ int32_t hecuda_bfv_noise_budget(const hecuda_context *h, const uint64_t *secret_
     double q_double = 1.0;  // vTimesT.moduli.map { Double($0) }.reduce(1.0, *)
     for (int i = 0; i < l; ++i) q_double *= (double)dc.q[i];
     for (int64_t b = 0; b < batch; ++b) {
-        const double norm = wide_to_double(norms.data() + (size_t)l * b, l);
+        const double norm = host::wide_to_double(norms.data() + (size_t)l * b, l);
         budgets[b] = norm == 0.0 ? HUGE_VAL : std::log2(q_double / (2 * norm));
     }
     return HECUDA_OK;

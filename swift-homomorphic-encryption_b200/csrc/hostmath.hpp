@@ -8,6 +8,7 @@
 // but is an independent implementation (exact 128-bit `%` arithmetic, deterministic root search); the parity
 // tests compare its outputs with the oracle's.
 #pragma once
+#include <cmath>
 #include <cstdint>
 #include <vector>
 
@@ -119,6 +120,22 @@ inline u64 punctured_mod(const u64 *m, int n, int skip, u64 p) {
     return r;
 }
 inline u64 shoup_factor(u64 w, u64 p) { return (u64)(((u128)w << 64) / p); }
+
+// x (w little-endian words) as a double, rounded to nearest with ties to even, like Double(_:) of a wide integer (the
+// noise budget's infinity norm, Bfv+Decrypt.swift:137-146).  The leading 64 bits convert with one rounding; every bit
+// below them only decides ties, so it is folded into bit 0, far below the rounding bit of the 53-bit result.
+inline double wide_to_double(const u64 *x, int w) {
+    int top = w - 1;
+    while (top >= 0 && !x[top]) --top;
+    if (top < 0) return 0.0;
+    if (top == 0) return (double)x[0];
+    const int lz = __builtin_clzll(x[top]);
+    u64 m = lz ? (x[top] << lz) | (x[top - 1] >> (64 - lz)) : x[top];  // the leading 64 bits
+    bool sticky = lz ? (x[top - 1] << lz) != 0 : x[top - 1] != 0;      // the bits of x[top - 1] below them
+    for (int i = top - 2; i >= 0 && !sticky; --i) sticky = x[i] != 0;
+    if (sticky) m |= 1;
+    return std::ldexp((double)m, 64 * top - lz);
+}
 
 }  // namespace host
 }  // namespace hecuda
