@@ -498,6 +498,39 @@ int32_t hecuda_simple_pir_compute_response(const hecuda_simple_pir_database *dat
                                            void *responses);
 int32_t hecuda_simple_pir_compute_response_device(const hecuda_simple_pir_database *database, const void *requests,
                                                   int64_t count, void *responses, void *stream);
+/* Sharded SimplePIR, as the SimplePIRProcessDatabase tool deploys it (Sources/SimplePIRProcessDatabase/main.swift:
+ * 158-253).  DatabaseMap.shardDatabase (SimplePir/DatabaseMap.swift:82-110) cuts entry i, bytes [offsets[i],
+ * offsets[i + 1]) of values, into ceil(size / chunk_size) chunks, each zero-padded to chunk_size, and puts chunk c on
+ * row chunk_locations[2 j + 1] of shard chunk_locations[2 j], with j counting chunks entry-major (DatabaseMap's
+ * ChunkLocation(shardIndex, index)).  The caller chooses the locations; the library draws no permutation.  Each shard
+ * is then processed as hecuda_simple_pir_process would process its rows: params[s] (shard_count of them, from
+ * computingParams over the shard's row count and chunk_size) and seeds[32 s .. 32 s + 32).  out[s] gets shard s's
+ * resident database; hints gets every shard's hint, shard after shard, each M_s x N words.  The values cross PCIe once
+ * and the shards' rows are gathered on the device.  Refused with HECUDA_ERR_INVALID_ARGUMENT before anything is
+ * allocated or launched: null pointers, entry_count < 0, shard_count < 1, chunk_size < 1, decreasing offsets,
+ * locations that are not a permutation of every shard's rows, a shard with no rows, params[s].entry_size !=
+ * chunk_size, databaseColumns that do not match the shard's row count, and shards whose pt, ct, N or word_bits
+ * differ; and every refusal of hecuda_simple_pir_process's parameters. */
+int32_t hecuda_simple_pir_process_shards(const uint8_t *values, const uint64_t *offsets /* entry_count + 1 */,
+                                         int64_t entry_count, int64_t chunk_size, int32_t shard_count,
+                                         const int64_t *chunk_locations /* chunks x 2 */,
+                                         const hecuda_simple_pir_params *params, const uint8_t *seeds /* 32 x shards */,
+                                         void *hints, hecuda_simple_pir_database **out /* shard_count */);
+/* computeResponse on every shard for `count` clients (SimplePirClientForAllShards.query, SimplePir+Shards.swift:
+ * 47-173, sends requests_per_shard = ShardMap.chunksPerShard requests to every shard).  requests are client-major: a
+ * client's block is shard 0's requests_per_shard x chunksPerEntry_0 x K_0 words, then shard 1's, and so on; responses
+ * follow the same order with M_s in place of K_s.  Each response equals hecuda_simple_pir_compute_response's.  One call
+ * makes one scratch allocation, one memset, one digit-split and one response launch per group of at most 32 shards,
+ * and one finish launch, whatever the shard count.  Refused with no kernel launched: null pointers, shard_count < 1,
+ * requests_per_shard < 1, count < 0, and shards that differ in ct or word_bits or live on different devices.
+ * count == 0 launches nothing.  The _device variant follows the conventions above. */
+int32_t hecuda_simple_pir_compute_response_shards(const hecuda_simple_pir_database *const *shards, int32_t shard_count,
+                                                  int64_t requests_per_shard, const void *requests, int64_t count,
+                                                  void *responses);
+int32_t hecuda_simple_pir_compute_response_shards_device(const hecuda_simple_pir_database *const *shards,
+                                                         int32_t shard_count, int64_t requests_per_shard,
+                                                         const void *requests, int64_t count, void *responses,
+                                                         void *stream);
 
 /* PirUtil.expand(ciphertexts:outputCount:using:) -- IndexPir/PirUtil.swift:321-355 (expandCiphertext :249-304,
  * expandCiphertextForOneStep :204-236).  ciphertexts: ciphertext_count x 2 x L x N (Coeff); out: output_count x 2 x L x N,

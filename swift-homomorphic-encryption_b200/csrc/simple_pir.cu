@@ -5,7 +5,10 @@
 //   SimplePirServer.process               SimplePir/SimplePir+Database.swift:252-290
 //   SimplePirContext.generateAPolynomials / materializeAMatrix   :177-206
 //   SimplePirServer(processedDatabase:hint:params:), computeResponse   SimplePir+Server.swift:24-38
+//   DatabaseMap.shardDatabase + per-shard process   SimplePir/DatabaseMap.swift:82-110, SimplePIRProcessDatabase/main.swift:158-253
+//   every shard's responses for SimplePirClientForAllShards   SimplePir/SimplePir+Shards.swift:47-173
 #include <algorithm>
+#include <climits>
 #include <vector>
 
 #include "capi_internal.hpp"
@@ -74,6 +77,26 @@ __global__ void __launch_bounds__(kThreads) pack_entries_kernel(const procdb::Pi
         long long e = -1, k = 0;
         if (r < g.m && c0 + b < g.k) spir::db_source(r, c0 + b, g.m, padded_entry, entry_scalars, s.entry_count, e, k);
         v[b] = e < 0 ? 0 : procdb::pir_coefficient(s, procdb::PirPiece{e, 0, s.entry_size}, k);
+    }
+    store_digits(planes, g.plane_bytes, g.planes, spir::a_offset(r, c0, g.col_tiles), v);
+}
+
+// pack_entries_kernel for one shard: its row e is the chunk row_source[e] = {entry, chunk} of the raw entries
+__global__ void __launch_bounds__(kThreads) pack_shard_kernel(const procdb::PirShape s, const Geometry g, long long padded_entry,
+                                                              long long entry_scalars, long long rows,
+                                                              const long long *__restrict__ row_source, long long chunk_size,
+                                                              unsigned char *__restrict__ planes) {
+    const long long padded_rows = g.row_tiles * spir::kTileRows;
+    const long long t = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (t >= padded_rows * g.col_tiles * (spir::kTileCols / 4)) return;
+    const long long r = t % padded_rows, c0 = t / padded_rows * 4;
+    u64 v[4];
+#pragma unroll
+    for (int b = 0; b < 4; ++b) {
+        long long e = -1, k = 0;
+        if (r < g.m && c0 + b < g.k) spir::db_source(r, c0 + b, g.m, padded_entry, entry_scalars, rows, e, k);
+        v[b] = e < 0 ? 0
+                     : procdb::pir_coefficient(s, spir::shard_piece(s, row_source[2 * e], row_source[2 * e + 1], chunk_size), k);
     }
     store_digits(planes, g.plane_bytes, g.planes, spir::a_offset(r, c0, g.col_tiles), v);
 }
@@ -150,18 +173,16 @@ struct ResponseArgs {
     int ct;
 };
 
-// Warp w of a CTA owns row tiles (blockIdx.x * kWarps + w) * 2 + {0, 1} and query tiles query_tile0 + blockIdx.y * 2 +
-// {0, 1}, over the K range of blockIdx.z.  For every slice of <= kSliceTiles tiles and every plane i, the s32 sums of
-// each live (i, j) pair are accumulated by the MMA and then widened into the 64-bit sums; the K ranges' sums meet in
-// acc (mod 2^64, so the order of the atomic adds does not matter).
-template <int D>
-__global__ void __launch_bounds__(kWarps * 32) response_kernel(const ResponseArgs a, long long query_tile0, u64 *__restrict__ acc) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long long rt0 = ((long long)blockIdx.x * kWarps + warp) * kWarpRowTiles;
-    if (rt0 * spir::kTileRows >= a.m) return;  // padding rows only; the kernel has no block-wide barrier
-    const long long qt0 = query_tile0 + (long long)blockIdx.y * kCtaQueryTiles;
-    const long long kt_begin = (long long)blockIdx.z * a.split_tiles;
-    const long long kt_end = min(a.col_tiles, kt_begin + a.split_tiles);
+static_assert(spir::kCtaRows == kWarps * kWarpRowTiles * spir::kTileRows, "simple_pir.cuh's CTA rows");
+static_assert(spir::kCtaQueries == kCtaQueryTiles * spir::kTileQueries, "simple_pir.cuh's CTA queries");
+
+// One warp's share of a response CTA: row tiles rt0 + {0, 1} against query tiles qt0 + {0, 1} over the K tiles
+// [kt_begin, kt_end).  For every slice of <= kSliceTiles tiles and every plane i, the s32 sums of each live (i, j) pair
+// are accumulated by the MMA and then widened into the 64-bit sums, which are atomically added at at(query, row) for
+// every row < a.m and query < a.q.
+template <int D, typename At>
+__device__ __forceinline__ void response_warp(const ResponseArgs &a, long long rt0, long long qt0, long long kt_begin,
+                                              long long kt_end, int lane, At at) {
     u64 wide[kWarpRowTiles][kCtaQueryTiles][4];
 #pragma unroll
     for (int mt = 0; mt < kWarpRowTiles; ++mt)
@@ -221,9 +242,99 @@ __global__ void __launch_bounds__(kWarps * 32) response_kernel(const ResponseArg
                 const long long row = (rt0 + mt) * spir::kTileRows + g + (e >> 1) * 8;
                 const long long query = (qt0 + nt) * spir::kTileQueries + tq + (e & 1);
                 if (row < a.m && query < a.q)
-                    atomicAdd(reinterpret_cast<unsigned long long *>(acc + query * a.m + row),
-                              (unsigned long long)wide[mt][nt][e]);
+                    atomicAdd(reinterpret_cast<unsigned long long *>(at(query, row)), (unsigned long long)wide[mt][nt][e]);
             }
+}
+
+// Warp w of a CTA owns row tiles (blockIdx.x * kWarps + w) * 2 + {0, 1} and query tiles query_tile0 + blockIdx.y * 2 +
+// {0, 1}, over the K range of blockIdx.z; the K ranges' sums meet in acc (mod 2^64, so the order of the atomic adds
+// does not matter).
+template <int D>
+__global__ void __launch_bounds__(kWarps * 32) response_kernel(const ResponseArgs a, long long query_tile0, u64 *__restrict__ acc) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long rt0 = ((long long)blockIdx.x * kWarps + warp) * kWarpRowTiles;
+    if (rt0 * spir::kTileRows >= a.m) return;  // padding rows only; the kernel has no block-wide barrier
+    const long long qt0 = query_tile0 + (long long)blockIdx.y * kCtaQueryTiles;
+    const long long kt_begin = (long long)blockIdx.z * a.split_tiles;
+    const long long kt_end = min(a.col_tiles, kt_begin + a.split_tiles);
+    response_warp<D>(a, rt0, qt0, kt_begin, kt_end, lane,
+                     [&](long long query, long long row) { return acc + query * a.m + row; });
+}
+
+// ---- grouped responses over shards (simple_pir.cuh, "grouped responses").  Requests and responses are client-major:
+// client c's block holds, for each shard s in order, requests_per_shard x chunksPerEntry_s rows of K_s request words
+// (M_s response words).  Query q of shard s is row q % qpc of client q / qpc's part of shard s.  The accumulators use
+// the responses' layout, so one finish_kernel serves every shard.
+constexpr int kMaxShards = 32;  // shards per launch: their descriptors travel in the kernel parameters
+
+struct ShardDesc {
+    const unsigned char *planes;
+    unsigned char *digits;  // the shard's request digit planes
+    size_t plane_bytes;
+    long long m, k, q;       // DB' rows and columns, queries (count x qpc)
+    long long split_tiles;   // 32-column tiles per K range
+    long long qpc;           // queries per client: requests_per_shard x chunksPerEntry
+    long long in_off, out_off;  // the shard's first word in a client's request / response block
+};
+
+struct ShardGroup {
+    int count, planes, ct;
+    long long in_block, out_block;  // words per client, over every shard of the call
+    long long split_threads;        // split_shards_kernel threads of the group
+    long long item_begin[kMaxShards], split_begin[kMaxShards];
+    ShardDesc shard[kMaxShards];
+};
+static_assert(sizeof(ShardGroup) < 4096, "the grouped kernels' parameters must stay under 4 KB");
+
+__device__ __forceinline__ long long col_tiles_of(long long k) { return (k + spir::kTileCols - 1) / spir::kTileCols; }
+__device__ __forceinline__ long long digit_plane_of(const ShardDesc &d) {
+    return (d.q + spir::kCtaQueries - 1) / spir::kCtaQueries * spir::kCtaQueries * col_tiles_of(d.k) * spir::kTileCols;
+}
+
+// split_requests_kernel for every shard of the group: thread (shard, query, four columns)
+template <typename W>
+__global__ void __launch_bounds__(kThreads) split_shards_kernel(const W *__restrict__ req, const ShardGroup g) {
+    const long long t = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (t >= g.split_threads) return;
+    const int s = spir::item_shard(g.split_begin, g.count, t);
+    const ShardDesc &d = g.shard[s];
+    const long long col_tiles = col_tiles_of(d.k), quads = col_tiles * (spir::kTileCols / 4);
+    const long long local = t - g.split_begin[s], c0 = local % quads * 4, row = local / quads;
+    u64 w[4] = {0, 0, 0, 0};
+    if (row < d.q) {
+        const W *src = req + row / d.qpc * g.in_block + d.in_off + row % d.qpc * d.k;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) w[b] = c0 + b < d.k ? (u64)src[c0 + b] : 0;
+    }
+    const long long at = spir::b_offset(row, c0, col_tiles), plane = digit_plane_of(d);
+    for (int j = 0; j < spir::digits(g.ct); ++j) {
+        unsigned digit = 0;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) digit |= spir::query_digit(w[b], g.ct, j) << (8 * b);
+        *reinterpret_cast<unsigned *>(d.digits + j * plane + at) = digit;
+    }
+}
+
+// response_kernel over the group's flat work items: CTA blockIdx.x is one (shard, row CTA, query-tile pair, K range)
+template <int D>
+__global__ void __launch_bounds__(kWarps * 32) response_shards_kernel(const ShardGroup g, u64 *__restrict__ acc) {
+    const long long item = blockIdx.x;
+    const int s = spir::item_shard(g.item_begin, g.count, item);
+    const ShardDesc &d = g.shard[s];
+    const long long col_tiles = col_tiles_of(d.k);
+    const spir::ItemShape shape{(d.m + spir::kCtaRows - 1) / spir::kCtaRows, (d.q + spir::kCtaQueries - 1) / spir::kCtaQueries,
+                                d.split_tiles, 0};
+    long long row_cta, pair, kt_begin, kt_end;
+    spir::decode_item(shape, col_tiles, item - g.item_begin[s], row_cta, pair, kt_begin, kt_end);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long rt0 = (row_cta * kWarps + warp) * kWarpRowTiles;
+    if (rt0 * spir::kTileRows >= d.m) return;  // padding rows only; the kernel has no block-wide barrier
+    const long long qt0 = pair * kCtaQueryTiles;
+    const ResponseArgs a{d.planes, d.plane_bytes, g.planes, d.digits, digit_plane_of(d), col_tiles, d.m, d.q,
+                         d.split_tiles, g.ct};
+    response_warp<D>(a, rt0, qt0, kt_begin, kt_end, lane, [&](long long query, long long row) {
+        return acc + query / d.qpc * g.out_block + d.out_off + query % d.qpc * d.m + row;
+    });
 }
 
 // responses[q][r] = acc[q][r] mod 2^ct in the reference's scalar width (query q = request * chunksPerEntry + chunk)
@@ -403,6 +514,129 @@ int32_t check_response(const hecuda_simple_pir_database *db, const void *req, in
     if (count > (1ll << 40) / std::max<int64_t>(1, db->params.chunks_per_entry * std::max(db->k, db->m)))
         return fail(HECUDA_ERR_INVALID_ARGUMENT, "too many requests for one call");
     return select_device(db->device);
+}
+
+template <int D>
+cudaError_t launch_response_shards(const ShardGroup &g, long long items, u64 *acc, cudaStream_t s) {
+    return launch(response_shards_kernel<D>, (unsigned)items, kWarps * 32, 0, s, g, acc);
+}
+
+// the grouped computeResponse for `count` clients already on the device, enqueued on s: one scratch allocation, one
+// memset, a split and a response launch per group of <= kMaxShards shards, one finish
+template <typename W>
+cudaError_t response_shards_device(const hecuda_simple_pir_database *const *shards, int shard_count, int64_t per_shard,
+                                   const W *d_req, int64_t count, W *d_out, cudaStream_t s) {
+    const int ct = shards[0]->params.ciphertext_modulus_bits, digits = spir::digits(ct);
+    int dev = 0, sms = 1;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    std::vector<ShardDesc> desc(shard_count);
+    std::vector<long long> items(shard_count), split_threads(shard_count);
+    std::vector<size_t> digit_at(shard_count);
+    long long in_block = 0, out_block = 0, ctas = 0;
+    for (int i = 0; i < shard_count; ++i) {
+        const hecuda_simple_pir_database &db = *shards[i];
+        ShardDesc &d = desc[i];
+        d.planes = db.d_planes;
+        d.plane_bytes = db.plane_bytes;
+        d.m = db.m;
+        d.k = db.k;
+        d.qpc = per_shard * db.params.chunks_per_entry;
+        d.q = count * d.qpc;
+        d.in_off = in_block;
+        d.out_off = out_block;
+        in_block += d.qpc * db.k;
+        out_block += d.qpc * db.m;
+        ctas += spir::base_ctas(db.m, d.q);
+    }
+    const size_t acc_bytes = (size_t)count * out_block * sizeof(u64);
+    size_t scratch = acc_bytes;  // the accumulators, then each shard's digit planes (multiples of 512 bytes)
+    for (int i = 0; i < shard_count; ++i) {
+        ShardDesc &d = desc[i];
+        const spir::ItemShape shape = spir::item_shape(d.m, shards[i]->col_tiles, d.q, ctas, sms, kMinSplitTiles);
+        d.split_tiles = shape.split_tiles;
+        items[i] = spir::item_count(shape);
+        const long long q_pad = shape.pairs * spir::kCtaQueries;
+        split_threads[i] = q_pad * shards[i]->col_tiles * (spir::kTileCols / 4);
+        digit_at[i] = scratch;
+        scratch += (size_t)q_pad * shards[i]->col_tiles * spir::kTileCols * digits;
+    }
+    unsigned char *d_scratch = nullptr;
+    cudaError_t e = cudaMallocAsync((void **)&d_scratch, scratch, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_scratch, 0, acc_bytes, s);
+    u64 *acc = reinterpret_cast<u64 *>(d_scratch);
+    for (int first = 0, end = 0; e == cudaSuccess && first < shard_count; first = end) {
+        end = spir::group_end(items.data(), first, shard_count, kMaxShards, INT_MAX);
+        ShardGroup g{};
+        g.count = end - first;
+        g.planes = shards[0]->planes;
+        g.ct = ct;
+        g.in_block = in_block;
+        g.out_block = out_block;
+        long long group_items = 0;
+        for (int j = 0; j < g.count; ++j) {
+            g.shard[j] = desc[first + j];
+            g.shard[j].digits = d_scratch + digit_at[first + j];
+            g.item_begin[j] = group_items;
+            g.split_begin[j] = g.split_threads;
+            group_items += items[first + j];
+            g.split_threads += split_threads[first + j];
+        }
+        e = launch(split_shards_kernel<W>, blocks_for(g.split_threads), kThreads, 0, s, d_req, g);
+        if (e != cudaSuccess) break;
+        switch (digits) {
+            case 1: e = launch_response_shards<1>(g, group_items, acc, s); break;
+            case 2: e = launch_response_shards<2>(g, group_items, acc, s); break;
+            case 3: e = launch_response_shards<3>(g, group_items, acc, s); break;
+            case 4: e = launch_response_shards<4>(g, group_items, acc, s); break;
+            case 5: e = launch_response_shards<5>(g, group_items, acc, s); break;
+            case 6: e = launch_response_shards<6>(g, group_items, acc, s); break;
+            case 7: e = launch_response_shards<7>(g, group_items, acc, s); break;
+            default: e = launch_response_shards<8>(g, group_items, acc, s); break;
+        }
+    }
+    if (e == cudaSuccess)
+        e = launch(finish_kernel<W>, blocks_for(count * out_block), kThreads, 0, s, (const u64 *)acc, (long long)(count * out_block),
+                   ct, d_out);
+    if (d_scratch) cudaFreeAsync(d_scratch, s);
+    return e;
+}
+
+// words of one client's requests (in) and responses (out) over every shard
+void client_words(const hecuda_simple_pir_database *const *shards, int shard_count, int64_t per_shard, size_t &in,
+                  size_t &out) {
+    in = out = 0;
+    for (int i = 0; i < shard_count; ++i) {
+        in += (size_t)per_shard * shards[i]->params.chunks_per_entry * shards[i]->k;
+        out += (size_t)per_shard * shards[i]->params.chunks_per_entry * shards[i]->m;
+    }
+}
+
+int32_t check_shards(const hecuda_simple_pir_database *const *shards, int32_t shard_count, int64_t per_shard,
+                     const void *req, int64_t count, const void *out) {
+    if (!shards || shard_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "no shards");
+    if (per_shard < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "requests_per_shard must be positive");
+    if (count < 0) return fail(HECUDA_ERR_INVALID_ARGUMENT, "negative client count");
+    if (count && (!req || !out)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null buffer");
+    for (int i = 0; i < shard_count; ++i) {
+        const hecuda_simple_pir_database *db = shards[i];
+        if (!db) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null shard");
+        if (db->params.ciphertext_modulus_bits != shards[0]->params.ciphertext_modulus_bits ||
+            db->params.word_bits != shards[0]->params.word_bits)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "shards differ in ciphertextModulusBits or word_bits");
+        if (db->device != shards[0]->device) return fail(HECUDA_ERR_INVALID_ARGUMENT, "shards on different devices");
+        const int64_t limit = (1ll << 40) / std::max<int64_t>(1, db->params.chunks_per_entry * std::max(db->k, db->m));
+        if (per_shard > limit || count > limit / per_shard)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "too many requests for one call");
+    }
+    return select_device(shards[0]->device);
+}
+
+// A shard's params against its rows: databaseColumns as computingParams derives it from entryCount = rows
+bool columns_match(const hecuda_simple_pir_params &p, int64_t rows) {
+    const int64_t epc = p.entries_per_column;
+    return epc == 1 ? p.database_columns == rows * p.chunks_per_entry
+                    : p.database_columns == std::max<int64_t>((rows + epc - 1) / epc, 1);
 }
 
 }  // namespace
@@ -588,6 +822,155 @@ int32_t hecuda_simple_pir_compute_response(const hecuda_simple_pir_database *db,
         cudaStreamDestroy(s);
     }
     return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "simple_pir_compute_response");
+}
+
+int32_t hecuda_simple_pir_process_shards(const uint8_t *values, const uint64_t *offsets, int64_t entry_count,
+                                         int64_t chunk_size, int32_t shard_count, const int64_t *chunk_locations,
+                                         const hecuda_simple_pir_params *params, const uint8_t *seeds, void *hints,
+                                         hecuda_simple_pir_database **out) {
+    if (!out || !values || !offsets || !chunk_locations || !params || !seeds || !hints)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (entry_count < 0 || shard_count < 1 || chunk_size < 1)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "entry_count, shard_count and chunk_size must be positive");
+    for (int s = 0; s < shard_count; ++s) out[s] = nullptr;
+    for (int64_t i = 0; i < entry_count; ++i)
+        if (offsets[i + 1] < offsets[i]) return fail(HECUDA_ERR_INVALID_ARGUMENT, "offsets must not decrease");
+    std::vector<Derived> d(shard_count);
+    for (int s = 0; s < shard_count; ++s) {
+        const int32_t rc = derive(params + s, d[s]);
+        if (rc) return rc;
+        const hecuda_simple_pir_params &p = params[s], &p0 = params[0];
+        if (p.entry_size != chunk_size) return fail(HECUDA_ERR_INVALID_ARGUMENT, "a shard's entry_size is not chunk_size");
+        if (p.plaintext_modulus_bits != p0.plaintext_modulus_bits || p.ciphertext_modulus_bits != p0.ciphertext_modulus_bits ||
+            p.lattice_dimension != p0.lattice_dimension || p.word_bits != p0.word_bits)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "shards differ in pt, ct, N or word_bits");
+    }
+    std::vector<long long> row_begin(shard_count + 1), row_source;
+    {
+        int64_t chunks = 0;
+        for (int64_t i = 0; i < entry_count; ++i) chunks += (int64_t)((offsets[i + 1] - offsets[i] + chunk_size - 1) / chunk_size);
+        row_source.resize(2 * chunks);
+    }
+    if (!spir::shard_rows(offsets, entry_count, chunk_size, chunk_locations, shard_count, row_begin.data(), row_source.data()))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "chunk locations are not a permutation of every shard's rows, or a shard is empty");
+    for (int s = 0; s < shard_count; ++s)
+        if (!columns_match(params[s], row_begin[s + 1] - row_begin[s]))
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "a shard's params do not match its row count");
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(HECUDA_ERR_NO_DEVICE, "no CUDA device: libhecuda has no CPU fallback");
+    std::string err;
+    Context *ctx = Context::create(params[0].lattice_dimension, &d[0].p, 1, 2, err, 64);
+    if (!ctx) return fail(HECUDA_ERR_UNSUPPORTED, err);
+    const int64_t n = params[0].lattice_dimension;
+    const bool wide = params[0].word_bits == 64;
+    const size_t value_bytes = entry_count ? offsets[entry_count] : 0;
+    int64_t most_rows = 0;
+    for (int s = 0; s < shard_count; ++s) most_rows = std::max(most_rows, d[s].m);
+    cudaStream_t st = nullptr;
+    unsigned char *d_values = nullptr, *d_seeds = nullptr;
+    uint64_t *d_offsets = nullptr;
+    long long *d_rows = nullptr;
+    u64 *d_hint = nullptr;
+    u32 *d_hint32 = nullptr;
+    cudaError_t e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_values, std::max<size_t>(1, value_bytes), st);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_offsets, (entry_count + 1) * sizeof(uint64_t), st);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_rows, row_source.size() * sizeof(long long), st);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_seeds, (size_t)shard_count * 32, st);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_hint, (size_t)most_rows * n * sizeof(u64), st);
+    if (e == cudaSuccess && !wide) e = cudaMallocAsync((void **)&d_hint32, (size_t)most_rows * n * sizeof(u32), st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_values, values, value_bytes, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_offsets, offsets, (entry_count + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_rows, row_source.data(), row_source.size() * sizeof(long long), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_seeds, seeds, (size_t)shard_count * 32, cudaMemcpyHostToDevice, st);
+    procdb::PirShape ps{};
+    ps.entries = d_values;
+    ps.offsets = d_offsets;
+    ps.entry_count = entry_count;
+    ps.entry_size = chunk_size;
+    ps.encoded = chunk_size;
+    ps.bits = params[0].plaintext_modulus_bits;
+    unsigned char *hint_out = (unsigned char *)hints;
+    for (int s = 0; e == cudaSuccess && s < shard_count; ++s) {
+        hecuda_simple_pir_database *db = new_database(params[s], d[s]);
+        if (!db) {
+            e = cudaErrorMemoryAllocation;
+            break;
+        }
+        out[s] = db;
+        e = cudaMalloc(&db->d_planes, db->plane_bytes * db->planes);
+        const Geometry g = d[s].g;
+        if (e == cudaSuccess)
+            e = launch(pack_shard_kernel, blocks_for(g.row_tiles * spir::kTileRows * g.col_tiles * (spir::kTileCols / 4)),
+                       kThreads, 0, st, ps, g, (long long)d[s].padded_entry, (long long)d[s].entry_scalars,
+                       (long long)(row_begin[s + 1] - row_begin[s]), (const long long *)d_rows + 2 * row_begin[s],
+                       (long long)chunk_size, db->d_planes);
+        if (e == cudaSuccess) e = compute_hint(*ctx, *db, d_seeds + 32 * s, d_hint, st);
+        const size_t words = (size_t)d[s].m * n;
+        if (e == cudaSuccess && !wide) e = launch_narrow(d_hint, d_hint32, (int64_t)words, st);
+        if (e == cudaSuccess)
+            e = cudaMemcpyAsync(hint_out, wide ? (const void *)d_hint : (const void *)d_hint32, words * (wide ? 8 : 4),
+                                cudaMemcpyDeviceToHost, st);
+        hint_out += words * (wide ? 8 : 4);
+    }
+    for (void *p : {(void *)d_values, (void *)d_offsets, (void *)d_rows, (void *)d_seeds, (void *)d_hint, (void *)d_hint32})
+        if (p) cudaFreeAsync(p, st);
+    if (st) {
+        const cudaError_t e2 = cudaStreamSynchronize(st);
+        if (e == cudaSuccess) e = e2;
+        cudaStreamDestroy(st);
+    }
+    delete ctx;
+    if (e != cudaSuccess) {
+        for (int s = 0; s < shard_count; ++s) {
+            hecuda_simple_pir_database_destroy(out[s]);
+            out[s] = nullptr;
+        }
+        return cuda_fail(e, "simple_pir_process_shards");
+    }
+    return HECUDA_OK;
+}
+
+int32_t hecuda_simple_pir_compute_response_shards_device(const hecuda_simple_pir_database *const *shards, int32_t shard_count,
+                                                         int64_t requests_per_shard, const void *requests, int64_t count,
+                                                         void *responses, void *stream) {
+    int32_t rc = check_shards(shards, shard_count, requests_per_shard, requests, count, responses);
+    if (rc || count == 0) return rc;
+    const cudaStream_t s = (cudaStream_t)stream;
+    const cudaError_t e =
+        shards[0]->params.word_bits == 64
+            ? response_shards_device(shards, shard_count, requests_per_shard, (const u64 *)requests, count, (u64 *)responses, s)
+            : response_shards_device(shards, shard_count, requests_per_shard, (const u32 *)requests, count, (u32 *)responses, s);
+    return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "simple_pir_compute_response_shards_device");
+}
+
+int32_t hecuda_simple_pir_compute_response_shards(const hecuda_simple_pir_database *const *shards, int32_t shard_count,
+                                                  int64_t requests_per_shard, const void *requests, int64_t count,
+                                                  void *responses) {
+    int32_t rc = check_shards(shards, shard_count, requests_per_shard, requests, count, responses);
+    if (rc || count == 0) return rc;
+    const size_t word = shards[0]->params.word_bits / 8;
+    size_t in_words = 0, out_words = 0;
+    client_words(shards, shard_count, requests_per_shard, in_words, out_words);
+    const size_t in_bytes = (size_t)count * in_words * word, out_bytes = (size_t)count * out_words * word;
+    cudaStream_t s = nullptr;
+    void *d_in = nullptr, *d_out = nullptr;
+    cudaError_t e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMallocAsync(&d_in, in_bytes, s);
+    if (e == cudaSuccess) e = cudaMallocAsync(&d_out, out_bytes, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_in, requests, in_bytes, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess)
+        e = word == 8 ? response_shards_device(shards, shard_count, requests_per_shard, (const u64 *)d_in, count, (u64 *)d_out, s)
+                      : response_shards_device(shards, shard_count, requests_per_shard, (const u32 *)d_in, count, (u32 *)d_out, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(responses, d_out, out_bytes, cudaMemcpyDeviceToHost, s);
+    for (void *p : {d_in, d_out})
+        if (p) cudaFreeAsync(p, s);
+    if (s) {
+        const cudaError_t e2 = cudaStreamSynchronize(s);
+        if (e == cudaSuccess) e = e2;
+        cudaStreamDestroy(s);
+    }
+    return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "simple_pir_compute_response_shards");
 }
 
 }  // extern "C"

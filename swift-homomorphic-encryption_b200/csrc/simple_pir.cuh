@@ -1,9 +1,12 @@
 // simple_pir.cuh -- the arithmetic and index maps of the SimplePIR kernels (simple_pir.cu).  Every function is __host__
-// __device__, so tests/emu/simple_pir_emulate.cu replays exactly what the kernels compute on the CPU.
+// __device__, so tests/emu/simple_pir_emulate.cu and tests/emu/simple_pir_shards_emulate.cu replay exactly what the
+// kernels compute on the CPU.
 //
 //   SimplePirServer.process            SimplePir/SimplePir+Database.swift:252-290
 //   SimplePirServer.computeResponse    SimplePir/SimplePir+Server.swift:31-38, Array2d.multiply(transposing:mask:)
 //                                      SimplePir+Precompute.swift:51-114
+//   DatabaseMap.shardDatabase          SimplePir/DatabaseMap.swift:82-110
+//   grouped responses over shards      SimplePir/SimplePir+Shards.swift:47-173 (one request set per shard and client)
 //
 // The response is (DB' . request^T) mod 2^ct with DB' (M x K) below 2^pt and request words of any width.  Both sides
 // are split into u8 digits: DB' into ceil(pt / 8) planes, requests (masked to ct bits first) into ceil(ct / 8) digits.
@@ -13,6 +16,8 @@
 // multiple of 2^ct and is skipped.  Masking the 64-bit sum to ct <= 61 bits gives the reference's wrapped product.
 #pragma once
 #include <cstdint>
+
+#include "process_db.cuh"
 
 #ifdef __CUDACC__
 #define SPIR_HD __host__ __device__ __forceinline__
@@ -77,6 +82,110 @@ SPIR_HD void db_source(long long r, long long c, long long m, long long padded_e
 // sigma(a) = a(x^-1) in Coeff form: sigma(a)_0 = a_0, sigma(a)_{N-i} = -a_i.  Coefficient i of a lands at sigma_index.
 SPIR_HD long long sigma_index(long long i, long long n) { return i ? n - i : 0; }
 SPIR_HD uint64_t sigma_value(uint64_t v, long long i, uint64_t p) { return (i && v) ? p - v : v; }
+
+// ---- sharding: DatabaseMap.shardDatabase (SimplePir/DatabaseMap.swift:82-110)
+// Entry e is cut into ceil(size / chunk_size) chunks; chunk c is bytes [c * chunk_size, (c + 1) * chunk_size) of the
+// entry, zero-padded to chunk_size.  The caller's chunk locations (shard, index), entry-major, place every chunk on one
+// row of one shard.  shard_rows inverts them: row_source[row_begin[s] + index] = {entry, chunk}, with row_begin the
+// prefix of the shards' row counts (shard_count + 1).  Returns false, leaving row_source partly written, unless the
+// locations are a permutation of every shard's rows and no shard is empty.
+inline bool shard_rows(const uint64_t *offsets, long long entry_count, long long chunk_size, const int64_t *locations,
+                       int shard_count, long long *row_begin, long long *row_source) {
+    for (int s = 0; s <= shard_count; ++s) row_begin[s] = 0;
+    long long chunks = 0;
+    for (long long e = 0; e < entry_count; ++e) {
+        const long long n = (long long)((offsets[e + 1] - offsets[e] + chunk_size - 1) / chunk_size);
+        for (long long c = 0; c < n; ++c, ++chunks) {
+            const int64_t s = locations[2 * chunks];
+            if (s < 0 || s >= shard_count) return false;
+            ++row_begin[s + 1];
+        }
+    }
+    for (int s = 0; s < shard_count; ++s) {
+        if (row_begin[s + 1] == 0) return false;
+        row_begin[s + 1] += row_begin[s];
+    }
+    for (long long r = 0; r < chunks; ++r) row_source[2 * r] = -1;
+    chunks = 0;
+    for (long long e = 0; e < entry_count; ++e) {
+        const long long n = (long long)((offsets[e + 1] - offsets[e] + chunk_size - 1) / chunk_size);
+        for (long long c = 0; c < n; ++c, ++chunks) {
+            const int64_t s = locations[2 * chunks], i = locations[2 * chunks + 1];
+            if (i < 0 || i >= row_begin[s + 1] - row_begin[s] || row_source[2 * (row_begin[s] + i)] >= 0) return false;
+            row_source[2 * (row_begin[s] + i)] = e;
+            row_source[2 * (row_begin[s] + i) + 1] = c;
+        }
+    }
+    return true;
+}
+
+// A shard's row {entry, chunk} as the bytes of the entry it holds: the chunk's bytes, shorter than chunk_size for the
+// entry's last chunk; bytesToCoefficients reads the missing bytes as the zero padding shardDatabase appends.
+SPIR_HD procdb::PirPiece shard_piece(const procdb::PirShape &s, long long entry, long long chunk, long long chunk_size) {
+    const long long start = chunk * chunk_size, left = procdb::pir_entry_length(s, entry) - start;
+    return procdb::PirPiece{entry, start, left < chunk_size ? left : chunk_size};
+}
+
+// ---- grouped responses over shards: one launch answers the queries of up to kMaxShards shards.  Its CTAs are a flat
+// list of work items; shard s owns items [item_begin[s], item_begin[s] + item_count) of the launch, ordered as
+// response_kernel's grid (row-CTA fastest, then query-tile pair, then K range).  A CTA covers kCtaRows rows and
+// kCtaQueries queries.
+constexpr int kCtaRows = 128, kCtaQueries = 16;
+
+struct ItemShape {
+    long long row_ctas, pairs;  // ceil(M / kCtaRows), padded queries / kCtaQueries
+    long long split_tiles;      // 32-column tiles per K range
+    long long splits;           // K ranges
+};
+
+SPIR_HD long long base_ctas(long long m, long long q) {
+    return (m + kCtaRows - 1) / kCtaRows * ((q + kCtaQueries - 1) / kCtaQueries);
+}
+// The K split of one shard when the shards of the call make `ctas` CTAs before splitting: as response_kernel's, ranges
+// until the launch covers the SMs about four times over, each of at least min_split_tiles tiles.
+SPIR_HD ItemShape item_shape(long long m, long long col_tiles, long long q, long long ctas, int sm_count,
+                             int min_split_tiles) {
+    ItemShape s;
+    s.row_ctas = (m + kCtaRows - 1) / kCtaRows;
+    s.pairs = (q + kCtaQueries - 1) / kCtaQueries;
+    long long splits = (4ll * sm_count + ctas - 1) / ctas;
+    const long long most = col_tiles / min_split_tiles;
+    splits = splits < 1 ? 1 : splits;
+    splits = splits < most ? splits : (most < 1 ? 1 : most);
+    s.split_tiles = (col_tiles + splits - 1) / splits;
+    s.splits = (col_tiles + s.split_tiles - 1) / s.split_tiles;
+    return s;
+}
+SPIR_HD long long item_count(const ItemShape &s) { return s.row_ctas * s.pairs * s.splits; }
+
+// The shards [first, end) of one launch: at most max_shards, and at most max_items items unless one shard alone has more
+// (the caller refuses that).  items[s] = item_count of shard s.
+SPIR_HD int group_end(const long long *items, int first, int shard_count, int max_shards, long long max_items) {
+    int end = first + 1;
+    long long total = items[first];
+    while (end < shard_count && end - first < max_shards && total + items[end] <= max_items) total += items[end++];
+    return end;
+}
+
+// Item `item` of a launch whose shards start at item_begin[0..count) (ascending, item_begin[0] = 0) -> its shard, row
+// CTA, query-tile pair and K range [k_begin, k_end) in 32-column tiles.
+SPIR_HD int item_shard(const long long *item_begin, int count, long long item) {
+    int lo = 0, hi = count - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) / 2;
+        if (item_begin[mid] <= item) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+SPIR_HD void decode_item(const ItemShape &s, long long col_tiles, long long local, long long &row_cta, long long &pair,
+                         long long &k_begin, long long &k_end) {
+    row_cta = local % s.row_ctas;
+    const long long t = local / s.row_ctas;
+    pair = t % s.pairs;
+    k_begin = t / s.pairs * s.split_tiles;
+    k_end = k_begin + s.split_tiles < col_tiles ? k_begin + s.split_tiles : col_tiles;
+}
 
 }  // namespace spir
 }  // namespace hecuda

@@ -7,6 +7,9 @@ Names follow Sources/PrivateInformationRetrieval/SimplePir/:
     SimplePirServer(processedDatabase:hint:params:)         SimplePir+Server.swift:24-29
     SimplePirServer.computeResponse                         SimplePir+Server.swift:31-38
     Array2d.save / init(from:)                              SimplePir+Database.swift:36-121
+    DatabaseMap, DatabaseMap.shardDatabase                  SimplePir/DatabaseMap.swift:18-110
+    ShardMap                                                SimplePir/SimplePir+Shards.swift:18-45
+    SimplePIRProcessDatabase's sharding and file names      Sources/SimplePIRProcessDatabase/main.swift:158-253
 
 The processed database stays on the device as u8 digit planes; responses are integer tensor-core products there.
 `scalar` is the reference's Scalar type: np.uint32 (UInt32) or np.uint64 (UInt64).
@@ -258,3 +261,244 @@ class SimplePirServer:
         """Device buffers (torch data_ptr()): enqueue on `stream` without synchronising."""
         _check(load_library().hecuda_simple_pir_compute_response_device(self.database._h, C.c_void_p(requests_ptr), count,
                                                                         C.c_void_p(responses_ptr), C.c_void_p(stream)))
+
+
+# ---- sharding (DatabaseMap.swift, SimplePir+Shards.swift, SimplePIRProcessDatabase/main.swift:158-253)
+@dataclass(frozen=True)
+class ChunkLocation:
+    shardIndex: int
+    index: int
+
+
+@dataclass(frozen=True)
+class DatabaseMapEntry:  # DatabaseMap.Entry
+    originalIndex: int
+    size: int
+    chunks: tuple
+
+
+def _raw_entries(entries):
+    """(originalIndex, bytes) pairs or an entryCount x entrySize uint8 matrix -> (original indices, values, uint64
+    offsets with entryCount + 1 elements)."""
+    if isinstance(entries, np.ndarray):
+        raw = np.ascontiguousarray(entries, dtype=np.uint8)
+        if raw.ndim != 2:
+            raise PirError("entries must be a 2-D uint8 array or (originalIndex, bytes) pairs")
+        count, size = raw.shape
+        return (np.arange(count, dtype=np.int64), raw.reshape(-1),
+                np.arange(count + 1, dtype=np.uint64) * np.uint64(size))
+    pairs = list(entries)
+    index = np.array([int(i) for i, _ in pairs], dtype=np.int64)
+    values = [np.frombuffer(bytes(v), dtype=np.uint8) for _, v in pairs]
+    offsets = np.zeros(len(values) + 1, dtype=np.uint64)
+    offsets[1:] = np.cumsum([len(v) for v in values], dtype=np.uint64)
+    flat = np.concatenate(values) if values else np.zeros(0, dtype=np.uint8)
+    return index, flat, offsets
+
+
+def _chunk_locations(sizes: np.ndarray, shard_count: int, chunk_size: int, rng) -> np.ndarray:
+    """shardDatabase's placement, vectorised: each entry draws its own permutation of the shards (one row of
+    rng.permuted), chunk c goes to shard perm[c % shardCount] at the next free row.  -> chunks x 2 int64, entry-major."""
+    counts = (sizes.astype(np.int64) + chunk_size - 1) // chunk_size
+    perms = rng.permuted(np.tile(np.arange(shard_count, dtype=np.int64), (len(sizes), 1)), axis=1)
+    entry = np.repeat(np.arange(len(sizes)), counts)
+    chunk = np.arange(int(counts.sum())) - np.repeat(np.cumsum(counts) - counts, counts)
+    shard = perms[entry, chunk % shard_count] if len(entry) else np.zeros(0, dtype=np.int64)
+    order = np.argsort(shard, kind="stable")  # rows of a shard in entry-major order
+    first = np.searchsorted(shard[order], np.arange(shard_count))
+    index = np.empty_like(shard)
+    index[order] = np.arange(len(shard)) - first[shard[order]]
+    return np.ascontiguousarray(np.stack([shard, index], axis=1), dtype=np.int64)
+
+
+class DatabaseMap:
+    """DatabaseMap: entries (originalIndex, size, chunks of ChunkLocation(shardIndex, index)) and chunkSize.  The
+    chunk locations are kept as one chunks x 2 array (entry-major); `entries` builds the reference's view of them."""
+
+    def __init__(self, originalIndices, sizes, locations, chunkSize: int):
+        self.originalIndices = np.asarray(originalIndices, dtype=np.int64)
+        self.sizes = np.asarray(sizes, dtype=np.int64)
+        self.chunkLocations = np.ascontiguousarray(locations, dtype=np.int64).reshape(-1, 2)
+        self.chunkSize = chunkSize
+
+    @property
+    def entries(self) -> tuple:
+        bounds = np.concatenate([[0], np.cumsum((self.sizes + self.chunkSize - 1) // self.chunkSize)])
+        locs = [ChunkLocation(int(s), int(i)) for s, i in self.chunkLocations]
+        return tuple(DatabaseMapEntry(int(self.originalIndices[e]), int(self.sizes[e]), tuple(locs[bounds[e]:bounds[e + 1]]))
+                     for e in range(len(self.sizes)))
+
+    def __eq__(self, other):
+        return (isinstance(other, DatabaseMap) and self.chunkSize == other.chunkSize and
+                np.array_equal(self.originalIndices, other.originalIndices) and np.array_equal(self.sizes, other.sizes)
+                and np.array_equal(self.chunkLocations, other.chunkLocations))
+
+    @staticmethod
+    def shardDatabase(entries, shardCount: int, chunkSize: int, rng=None):
+        """DatabaseMap.shardDatabase(entries:shardCount:chunkSize:) on the host -> (databaseMap, shards), each shard a
+        rows x chunkSize uint8 matrix.  rng (numpy Generator) draws the permutations; the reference's draws from
+        SystemRandomNumberGenerator cannot be reproduced."""
+        if shardCount < 1 or chunkSize < 1:
+            raise PirError("shardCount and chunkSize must be positive")
+        index, values, offsets = _raw_entries(entries)
+        sizes = np.diff(offsets).astype(np.int64)
+        locations = _chunk_locations(sizes, shardCount, chunkSize, rng or np.random.default_rng())
+        rows = np.bincount(locations[:, 0], minlength=shardCount)
+        shards = [np.zeros((int(r), chunkSize), dtype=np.uint8) for r in rows]
+        if len(sizes) and np.all(sizes == sizes[0]):  # equal sizes: every entry's zero-padded chunks at once
+            per = -(-int(sizes[0]) // chunkSize)
+            padded = np.zeros((len(sizes), per * chunkSize), dtype=np.uint8)
+            padded[:, :sizes[0]] = values.reshape(len(sizes), -1)
+            chunks = padded.reshape(-1, chunkSize)
+            for s in range(shardCount):
+                mine = locations[:, 0] == s
+                shards[s][locations[mine, 1]] = chunks[mine]
+        else:
+            chunk = 0
+            for e in range(len(sizes)):
+                start = int(offsets[e])
+                for c in range(0, int(sizes[e]), chunkSize):
+                    s, i = locations[chunk]
+                    piece = values[start + c:start + min(c + chunkSize, int(sizes[e]))]
+                    shards[s][i, :len(piece)] = piece
+                    chunk += 1
+        return DatabaseMap(index, sizes, locations, chunkSize), shards
+
+
+class ShardMap:
+    """ShardMap(databaseMap:): shardCount counts the shards that hold a chunk; chunksPerShard = ceil(maximumChunkCount
+    / shardCount)."""
+
+    def __init__(self, databaseMap: DatabaseMap):
+        self.mapping = {e.originalIndex: e for e in databaseMap.entries}
+        self.shardCount = len({c.shardIndex for e in self.mapping.values() for c in e.chunks})
+        self.maximumChunkCount = max((len(e.chunks) for e in self.mapping.values()), default=0)
+        self.chunkSize = databaseMap.chunkSize
+        self.chunksPerShard = -(-self.maximumChunkCount // self.shardCount) if self.shardCount else 0
+
+    def __getitem__(self, originalIndex: int) -> Optional[DatabaseMapEntry]:
+        return self.mapping.get(originalIndex)
+
+
+def _handles(databases) -> C.Array:
+    return (C.c_void_p * len(databases))(*[d._h.value if isinstance(d._h, C.c_void_p) else d._h for d in databases])
+
+
+class SimplePirShardedServer:
+    """One SimplePirServer per shard, answered together: computeResponses sends every client's requests to every shard
+    in one grouped device pass.  process shards and processes raw entries on the device, as the
+    SimplePIRProcessDatabase tool does."""
+
+    def __init__(self, databases: Sequence[SimplePirDatabase], hints: Sequence[np.ndarray],
+                 params: Sequence[SimplePirParameters], scalar=np.uint64, databaseMap: Optional[DatabaseMap] = None):
+        self.scalar = np.dtype(scalar)
+        _word_bits(self.scalar)
+        if not (len(databases) == len(hints) == len(params)) or not databases:
+            raise PirError("one database, hint and params per shard")
+        self.databases, self.hints, self.params = list(databases), list(hints), list(params)
+        self.databaseMap = databaseMap
+        self._h = _handles(self.databases)
+
+    @property
+    def shardCount(self) -> int:
+        return len(self.databases)
+
+    @staticmethod
+    def process(entries, encryptionParams: SimplePirEncryptionParams, shardCount: int, chunkSize: Optional[int] = None,
+                seed: Optional[bytes] = None, scalar=np.uint64, rng=None) -> "SimplePirShardedServer":
+        """entries: (originalIndex, bytes) pairs or an entryCount x entrySize uint8 matrix.  chunkSize None is the
+        tool's ceil(largest entry / shardCount); seed None draws one seed per shard, given bytes seed every shard."""
+        bits = _word_bits(scalar)
+        if shardCount < 1:
+            raise PirError("shardCount must be positive")
+        index, values, offsets = _raw_entries(entries)
+        sizes = np.diff(offsets).astype(np.int64)
+        if chunkSize is None:
+            chunkSize = -(-int(sizes.max(initial=0)) // shardCount)
+        if chunkSize < 1:
+            raise PirError("chunkSize must be positive")
+        locations = _chunk_locations(sizes, shardCount, chunkSize, rng or np.random.default_rng())
+        rows = np.bincount(locations[:, 0], minlength=shardCount)
+        if seed is not None and len(seed) != SEED_BYTES:
+            raise PirError(f"seed must be {SEED_BYTES} bytes")
+        params = [SimplePirParameters.computingParams(encryptionParams, max(int(r), 1), chunkSize, seed) for r in rows]
+        hints = [np.empty((p.columnSize, p.latticeDimension), dtype=scalar) for p in params]
+        hint_buf = np.empty(sum(h.size for h in hints), dtype=scalar)
+        seeds = np.frombuffer(b"".join(p.seed for p in params), dtype=np.uint8).copy()
+        cparams = (_Params * shardCount)(*[p._c(bits) for p in params])
+        handles = (C.c_void_p * shardCount)()
+        values = values if values.size else np.zeros(1, dtype=np.uint8)
+        _check(load_library().hecuda_simple_pir_process_shards(
+            _ptr(values), _ptr(offsets), len(sizes), chunkSize, shardCount, _ptr(locations),
+            cparams, _ptr(seeds), _ptr(hint_buf), handles))
+        at = 0
+        for h in hints:
+            h[...] = hint_buf[at:at + h.size].reshape(h.shape)
+            at += h.size
+        databases = [SimplePirDatabase(C.c_void_p(handles[i]), params[i], scalar) for i in range(shardCount)]
+        return SimplePirShardedServer(databases, hints, params, scalar, DatabaseMap(index, sizes, locations, chunkSize))
+
+    def _words(self, requests_per_shard: int):
+        inw = [requests_per_shard * p.chunksPerEntry * p.databaseColumns for p in self.params]
+        outw = [requests_per_shard * p.chunksPerEntry * p.columnSize for p in self.params]
+        return inw, outw
+
+    def computeResponses(self, requests, requests_per_shard: Optional[int] = None):
+        """requests: one entry per client, each a list of shardCount arrays requests_per_shard x chunksPerEntry_s x K_s
+        (SimplePirClientForAllShards.query, flattened) -> the same nesting with columnSize_s in place of K_s.  A 2-D
+        array count x words (client-major blocks) with requests_per_shard given returns count x response words."""
+        flat = isinstance(requests, np.ndarray)
+        if flat:
+            if requests_per_shard is None:
+                raise PirError("a flat request array needs requests_per_shard")
+            r = np.ascontiguousarray(requests, dtype=self.scalar)
+        else:
+            requests = list(requests)
+            if not requests:
+                return []
+            requests_per_shard = len(requests[0][0])
+            blocks = []
+            for client in requests:
+                if len(client) != self.shardCount:
+                    raise PirError(f"a client must send requests to all {self.shardCount} shards")
+                for s, (q, p) in enumerate(zip(client, self.params)):
+                    q = np.asarray(q, dtype=self.scalar)
+                    if q.shape != (requests_per_shard, p.chunksPerEntry, p.databaseColumns):
+                        raise PirError(f"shard {s}: requests must be {requests_per_shard} x {p.chunksPerEntry} x "
+                                       f"{p.databaseColumns}, got {q.shape}")
+                    blocks.append(q.reshape(-1))
+            r = np.concatenate(blocks).reshape(len(requests), -1)
+        inw, outw = self._words(requests_per_shard)
+        if r.ndim != 2 or r.shape[1] != sum(inw):
+            raise PirError(f"requests must be count x {sum(inw)} words")
+        out = np.empty((r.shape[0], sum(outw)), dtype=self.scalar)
+        _check(load_library().hecuda_simple_pir_compute_response_shards(self._h, self.shardCount, requests_per_shard,
+                                                                        _ptr(r), r.shape[0], _ptr(out)))
+        if flat:
+            return out
+        bounds = np.concatenate([[0], np.cumsum(outw)])
+        return [[out[c, bounds[s]:bounds[s + 1]].reshape(requests_per_shard, p.chunksPerEntry, p.columnSize)
+                 for s, p in enumerate(self.params)] for c in range(out.shape[0])]
+
+    def computeResponsesDevice(self, requests_ptr: int, requests_per_shard: int, count: int, responses_ptr: int,
+                               stream: int = 0):
+        """Device buffers in the flat client-major layout: enqueue on `stream` without synchronising."""
+        _check(load_library().hecuda_simple_pir_compute_response_shards_device(
+            self._h, self.shardCount, requests_per_shard, C.c_void_p(requests_ptr), count, C.c_void_p(responses_ptr),
+            C.c_void_p(stream)))
+
+    def save(self, prefix: str):
+        """The tool's files: prefix-i.bin (processed database) and prefix-i.hint.bin for every shard i."""
+        for i, (db, hint) in enumerate(zip(self.databases, self.hints)):
+            db.save(f"{prefix}-{i}.bin")
+            save_array2d(hint, f"{prefix}-{i}.hint.bin")
+
+    @staticmethod
+    def load(prefix: str, params: Sequence[SimplePirParameters], scalar=np.uint64) -> "SimplePirShardedServer":
+        databases = [SimplePirDatabase.load(f"{prefix}-{i}.bin", p, scalar) for i, p in enumerate(params)]
+        hints = [load_array2d(f"{prefix}-{i}.hint.bin", scalar) for i in range(len(params))]
+        return SimplePirShardedServer(databases, hints, params, scalar)
+
+    def close(self):
+        for db in self.databases:
+            db.close()
