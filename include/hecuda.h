@@ -58,9 +58,11 @@ enum {
     HECUDA_BASE_Q_BSK = 1,     /* [q_0..q_{L-1}, Bsk], rows = 2L+1               (RnsTool.swift:228-233) */
     HECUDA_BASE_KEYSWITCH = 2, /* q_0..q_{rows-2}, q_ks                          (Context.swift:114-127) */
     HECUDA_BASE_Q_AUX = 3      /* [q_0..q_{L-1}, aux], rows = 2L+1: the base hecuda_bfv_multiply computes in.  Its
-                                  auxiliary primes are below 2^55 when BEHZ's exactness conditions allow (they do for
-                                  every predefined parameter set), else they are Bsk; the product does not depend on the
-                                  choice (csrc/context.cu).  HECUDA_AUX_BASE=reference in the environment forces Bsk. */
+                                  auxiliary primes are below 2^30 or 2^55 when BEHZ's exactness conditions for one product
+                                  allow, else they are Bsk (as for n_8192_logq_3x55_logt_42, whose t is too large); the
+                                  product does not depend on the choice (csrc/context.cu).  hecuda_bfv_inner_product uses
+                                  this base only while its pair count keeps the sum exact in it, and Bsk above that.
+                                  HECUDA_AUX_BASE=reference in the environment forces Bsk. */
 };
 
 int32_t hecuda_version(void);

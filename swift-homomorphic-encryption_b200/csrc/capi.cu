@@ -180,22 +180,25 @@ cudaError_t apply_galois_chunk(const Context &c, u64 *scratch, const u64 *key, c
 }
 
 // Bfv.innerProduct(_:_:) (Bfv.swift:315-361): sum of the tensor products of `pairs` ciphertext pairs in [Q, Bsk],
-// then ONE dropExtendedBase -- instead of `pairs` full multiplies.
+// then ONE dropExtendedBase -- instead of `pairs` full multiplies.  The sum grows with `pairs`; past aux_max_pairs it
+// would wrap in the auxiliary base (context.cu), so it runs over the reference's Bsk, as the reference does.  The floor's
+// folded Q-row scaling (kScaleTMontFloor) lives in the Q slots' inverse twiddles and is the same for either base.
 cudaError_t inner_product_chunk(const Context &c, u64 *scratch, const u64 *lhs, const u64 *rhs, int64_t pairs,
                                        u64 *out, int64_t groups, cudaStream_t s) {
     const int R = 2 * c.L + 1;
     const size_t poly_words = (size_t)R * c.n;
     const int64_t items = groups * pairs;
     u64 *ext = scratch, *ten = scratch + 4 * poly_words * items;
-    const NttRowMap map = c.map_qaux();
+    const bool bsk = pairs > c.aux_max_pairs;
+    const NttRowMap map = bsk ? c.map_qbsk() : c.map_qaux();
     cudaError_t e;
     const bool scaled = floor_takes_scaled_q(c);
-    if ((e = launch_lift(c, lhs, rhs, 2, ext, items, s)) != cudaSuccess) return e;
+    if ((e = launch_lift(c, lhs, rhs, 2, ext, items, s, bsk)) != cudaSuccess) return e;
     if ((e = launch_ntt_forward(c, map, ext, ext, items * 4 * R, s)) != cudaSuccess) return e;
-    if ((e = launch_tensor_sum(c, ext, ten, pairs, groups, s)) != cudaSuccess) return e;
+    if ((e = launch_tensor_sum(c, ext, ten, pairs, groups, s, bsk)) != cudaSuccess) return e;
     if ((e = launch_ntt_inverse(c, map, ten, ten, groups * 3 * R, scaled ? kScaleTMontFloor : kScaleTMont, s)) != cudaSuccess)
         return e;
-    return launch_floor(c, ten, out, groups * 3, s, false, scaled);
+    return launch_floor(c, ten, out, groups * 3, s, bsk, scaled);
 }
 size_t inner_product_scratch_words(const Context &c, int64_t pairs) {
     return (size_t)(4 * pairs + 3) * (2 * c.L + 1) * c.n;

@@ -3,6 +3,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -163,8 +164,11 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
     // below 2^55, whose NTT rows never need a conditional subtraction (ntt_fast.cuh, NARROW class), instead of the
     // reference's 61-bit Bsk; the reference base stays available for the stage-level entry points.  The 55-bit primes
     // are the smallest of the form h 2^32 + 1: their butterflies (NARROW-H) and Montgomery reductions (mont_reduce_h)
-    // need fewer multiplies.  Conditions checked:
+    // need fewer multiplies.  Conditions checked, each with one bit to spare in the log2 test below:
     //   q * B_aux > 8 N q^2   (D is represented exactly),   B_aux(L primes) * m_sk > 16 t N q   (F survives SK)
+    // They bound ONE tensor product.  The ct x ct inner product floors the sum of `pairs` products once, so D and F
+    // grow by that factor: aux_max_pairs is the largest P for which both still hold with log2(P) added to their right-hand
+    // sides, and longer inner products run over Bsk instead (capi.cu inner_product_chunk).
     c->aux = c->bsk;
     {
         const char *env = std::getenv("HECUDA_AUX_BASE");
@@ -189,9 +193,14 @@ Context *Context::create(int64_t n, const u64 *coeff_moduli, int nmod, u64 t, st
                 log_aux += std::log2((double)pick[j]);
                 if ((int)j < L) log_aux_l += std::log2((double)pick[j]);
             }
-            const bool enough = (int)pick.size() == L + 1 && log_aux >= log_q + log_n + 4 &&
-                                log_aux_l + std::log2((double)pick.back()) >= log_t + log_n + log_q + 5;
-            if (enough) c->aux = pick;
+            if ((int)pick.size() != L + 1) continue;
+            const double slack_d = log_aux - (log_q + log_n + 4);
+            const double slack_f = log_aux_l + std::log2((double)pick.back()) - (log_t + log_n + log_q + 5);
+            const double slack = std::min(slack_d, slack_f);
+            if (slack >= 0) {
+                c->aux = pick;
+                c->aux_max_pairs = slack >= 62 ? INT64_MAX : (int64_t)std::floor(std::exp2(slack));
+            }
         }
     }
     c->aux_is_reference = c->aux == c->bsk;

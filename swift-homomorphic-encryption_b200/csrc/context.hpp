@@ -155,6 +155,8 @@ class Context {
     std::vector<u64> bsk;  // L+1 primes: the reference's BEHZ base (RnsTool.swift:30-33)
     std::vector<u64> aux;  // L+1 primes: the base ct x ct multiply actually computes in (context.cu); == bsk when
     bool aux_is_reference = true;  // the conditions for the faster base do not hold (or HECUDA_AUX_BASE=reference)
+    // the most tensor products one floor may sum over aux (ct x ct inner product); larger sums run over Bsk
+    int64_t aux_max_pairs = INT64_MAX;
     std::vector<HostSlot> slots;  // L q's, L+1 bsk, 1 q_ks, then L+1 aux (when different from bsk), then t (SIMD)
     ModSlot *d_slots = nullptr;   // device array: the slots, then (N = 2^15 only) 2 virtual half-transform slots per slot
     int split_slot_base = 0;      // index of the first virtual slot (slot s, half h -> split_slot_base + 2 s + h)
