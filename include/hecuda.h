@@ -475,6 +475,7 @@ typedef struct hecuda_simple_pir_params {                            /* SimplePi
     int64_t chunks_per_entry;
     int64_t database_columns;        /* K */
     int32_t word_bits;               /* 32 or 64: the Scalar type */
+    double error_std_dev;            /* errorStdDev: read by the client calls only (3.2 or 6.4 in the reference) */
 } hecuda_simple_pir_params;
 /* SimplePirServer.process(database:encryptionParams:seed:) (SimplePir+Database.swift:252-290) after computingParams
  * (:208-243): entries entry_count x entry_size bytes; seed 32 bytes (params.seed).  Entry e's bytesToCoefficients at pt
@@ -533,6 +534,47 @@ int32_t hecuda_simple_pir_compute_response_shards_device(const hecuda_simple_pir
                                                          int32_t shard_count, int64_t requests_per_shard,
                                                          const void *requests, int64_t count, void *responses,
                                                          void *stream);
+
+/* SimplePIR's client (SimplePirClient with DefaultQueryGenerator, SimplePir+Client.swift, SimplePir+Precompute.swift).
+ * hecuda_simple_pir_client_create: DefaultQueryGenerator.init (SimplePir+Precompute.swift:328-334) from the hint (M x N
+ * words), params and seed (32 bytes, params.seed): the aPolyCount polynomials PolyRq.random draws from
+ * NistAes128Ctr(seed) (generateAPolynomials, SimplePir+Database.swift:177-184) stay on the device in Eval format, and the
+ * hint as ceil((ct + 1) / 8) u8 digit planes.  Refused with HECUDA_ERR_INVALID_ARGUMENT: every refusal of
+ * hecuda_simple_pir_process's parameters, null pointers, a hint word >= nttFriendlyMod, errorStdDev not in (0, 16).
+ * The AES tables are uploaded here, so the _device calls below stay stream-ordered and graph-capturable. */
+typedef struct hecuda_simple_pir_client hecuda_simple_pir_client;
+int32_t hecuda_simple_pir_client_create(const void *hint /* M x N words */, const hecuda_simple_pir_params *params,
+                                        const uint8_t *seed /* 32, params.seed */, hecuda_simple_pir_client **out);
+int32_t hecuda_simple_pir_client_destroy(hecuda_simple_pir_client *client);
+/* PrecomputedQueries.WithoutIndices.init (SimplePir+Precompute.swift:199-227; generateSecretPolys, noiselessSample and
+ * encryptZero, SimplePir+Client.swift:20-82) for `count` queries, each drawn from two 32-byte seeds (count x 32 each)
+ * in place of the reference's SystemRandomNumberGenerator and rng: secret i < chunksPerEntry, coefficient j is stream
+ * coefficient i N + j of PolyRq.randomizeTernary over NistAes128Ctr(secret seed) (12 bytes each, -1 stored as p - 1);
+ * error (i, c) is stream coefficient i K + c of Array2d.randomCenteredBinomialDistribution over NistAes128Ctr(error seed)
+ * (Array2d.swift:382-429).  queries: count x chunksPerEntry x K words, the modSwitched sample divideAndRound(p -> 2^ct)
+ * plus the error, masked to ct bits; with indices (count, nullable) each query is WithQueryIndices.queries, delta =
+ * 2^(ct - pt) added at column (index chunksPerEntry + i) / entriesPerColumn (add(index:), :241-256).  results: count x
+ * chunksPerEntry x M words = S . hint^T mod p as Array2d.multiply(transposing:modulus:) (:122-188) computes it: the sum
+ * in the scalar's double width with wrapping adds, then mod p, so results where that sum wraps are the reference's, not
+ * the exact product.  Refused with no kernel launched: null pointers, count < 0, an index < 0 or whose column reaches K
+ * (host variant), more than 2^40 / (chunksPerEntry max(K, M)) queries.  count == 0 launches nothing.  The _device
+ * variant takes device buffers (indices too, unchecked) and follows the conventions above. */
+int32_t hecuda_simple_pir_client_precompute(const hecuda_simple_pir_client *client, const uint8_t *secret_seeds,
+                                            const uint8_t *error_seeds, const int64_t *indices, int64_t count,
+                                            void *queries, void *results);
+int32_t hecuda_simple_pir_client_precompute_device(const hecuda_simple_pir_client *client, const uint8_t *secret_seeds,
+                                                   const uint8_t *error_seeds, const int64_t *indices, int64_t count,
+                                                   void *queries, void *results, void *stream);
+/* SimplePirClient.decrypt (SimplePir+Client.swift:111-121) after prepareResponse and integrate (SimplePir+Precompute.swift:
+ * 280-311) for `count` responses (count x chunksPerEntry x M words) with the results precompute wrote for them and their
+ * indices (count): extractEntries of both at the index, ((r - s + delta / 2) & mask) >> (ct - pt), coefficientsToBytes
+ * at pt bits, the first entrySizeInBytes bytes -> entries (count x entrySizeInBytes).  Refusals as precompute's, indices
+ * required. */
+int32_t hecuda_simple_pir_client_decrypt(const hecuda_simple_pir_client *client, const void *responses, const void *results,
+                                         const int64_t *indices, int64_t count, uint8_t *entries);
+int32_t hecuda_simple_pir_client_decrypt_device(const hecuda_simple_pir_client *client, const void *responses,
+                                                const void *results, const int64_t *indices, int64_t count,
+                                                uint8_t *entries, void *stream);
 
 /* PirUtil.expand(ciphertexts:outputCount:using:) -- IndexPir/PirUtil.swift:321-355 (expandCiphertext :249-304,
  * expandCiphertextForOneStep :204-236).  ciphertexts: ciphertext_count x 2 x L x N (Coeff); out: output_count x 2 x L x N,

@@ -171,11 +171,22 @@ cudaError_t expand_seeded_keys_device(const Context &c, const unsigned char *d_p
 cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, unsigned int **d_rk, u64 **d_ctr,
                         cudaStream_t s);
 void free_chains(unsigned int *d_rk, u64 *d_ctr, int segments, int64_t batch, cudaStream_t s);
+// drbg_chains in two steps: the AES tables (synchronises s), then the chains alone (stream-ordered and graph-capturable
+// once the tables are on the device)
+cudaError_t drbg_upload_tables(cudaStream_t s);
+cudaError_t drbg_chains_uploaded(const unsigned char *d_seeds, int segments, int64_t batch, unsigned int **d_rk, u64 **d_ctr,
+                                 cudaStream_t s);
 cudaError_t drbg_tables(const unsigned char **sbox, const unsigned int **te0);
 // PolyRq.random mod p of `polys` degree-n polynomials from the one stream of the 32-byte d_seed (coefficient k of
 // polynomial j is the stream's (jN + k)-th 128-bit word mod p), stored as sigma(a) = a(x^-1) (simple_pir.cuh)
 cudaError_t random_sigma_polys_device(const unsigned char *d_seed, u64 p, int64_t n, int64_t polys, u64 *d_out,
                                       cudaStream_t s);
+// the same polynomials as a itself (SimplePirContext.generateAPolynomials for the client)
+cudaError_t random_polys_one_modulus_device(const unsigned char *d_seed, u64 p, int64_t n, int64_t polys, bool sigma,
+                                            u64 *d_out, cudaStream_t s);
+// SimplePirParameters' checks and derived sizes (simple_pir.cu): DB' is m x k (columnSize x databaseColumns), an entry
+// is entry_scalars coefficients, p = nttFriendlyMod
+int32_t simple_pir_derive(const hecuda_simple_pir_params *params, int64_t &m, int64_t &k, int64_t &entry_scalars, u64 &p);
 cudaError_t inner_product_chunk(const Context &c, u64 *scratch, const u64 *lhs, const u64 *rhs, int64_t pairs, u64 *out,
                                 int64_t groups, cudaStream_t s);
 // `tables` MulPir databases from entry bytes already on the device (pir.cu; used by keyword_pir.cu)

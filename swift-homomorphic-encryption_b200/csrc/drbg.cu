@@ -105,10 +105,11 @@ __global__ void __launch_bounds__(kSegmentBlocks) drbg_fill_kernel(const u32w *_
 }
 
 // PolyRq.random over one modulus for `total` = polys x N coefficients of one stream (SimplePirContext
-// .generateAPolynomials, SimplePir+Database.swift:181-184), stored as sigma(a) = a(x^-1) (simple_pir.cuh)
-__global__ void __launch_bounds__(kSegmentBlocks) drbg_sigma_fill_kernel(const u32w *__restrict__ round_keys,
-                                                                         const u64 *__restrict__ counters, u64 *__restrict__ out,
-                                                                         u64 p, long long n, long long total) {
+// .generateAPolynomials, SimplePir+Database.swift:181-184), stored as a, or as sigma(a) = a(x^-1) (simple_pir.cuh)
+__global__ void __launch_bounds__(kSegmentBlocks) drbg_one_modulus_fill_kernel(const u32w *__restrict__ round_keys,
+                                                                               const u64 *__restrict__ counters,
+                                                                               u64 *__restrict__ out, u64 p, long long n,
+                                                                               long long total, bool sigma) {
     __shared__ unsigned char sbox[256];
     __shared__ u32w te0[256];
     __shared__ u32w rk[kRoundKeyWords];
@@ -119,7 +120,10 @@ __global__ void __launch_bounds__(kSegmentBlocks) drbg_sigma_fill_kernel(const u
     if (k >= total) return;
     const u64 v = (u64)(segment_word(rk, counters + 2 * (size_t)s, te0, sbox) % p);
     const long long poly = k / n, i = k - poly * n;
-    out[poly * n + spir::sigma_index(i, n)] = spir::sigma_value(v, i, p);
+    if (sigma)
+        out[poly * n + spir::sigma_index(i, n)] = spir::sigma_value(v, i, p);
+    else
+        out[k] = v;
 }
 
 // EvaluationKey(deserialize:) of seeded key-switching ciphertexts (SerializedCiphertext.swift:53-60 with Format = Eval):
@@ -157,16 +161,24 @@ namespace api {
 
 // The AES tables, then every seed's chain: (round keys, V) of each of its `segments` segments into *d_rk / *d_ctr, both
 // allocated on `s` and released by free_chains.
-cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, u32w **d_rk, u64 **d_ctr, cudaStream_t s) {
+cudaError_t drbg_upload_tables(cudaStream_t s) {
     unsigned char sbox[256];
     u32w te0[256];
     make_tables(sbox, te0);
     cudaError_t e = cudaMemcpyToSymbolAsync(c_sbox, sbox, sizeof(sbox), 0, cudaMemcpyHostToDevice, s);  // per device, cheap
     if (e == cudaSuccess) e = cudaMemcpyToSymbolAsync(c_te0, te0, sizeof(te0), 0, cudaMemcpyHostToDevice, s);
     if (e != cudaSuccess) return e;
-    e = cudaStreamSynchronize(s);  // the tables live on this stack frame
-    if (e != cudaSuccess) return e;
-    e = cudaMallocAsync((void **)d_rk, (size_t)batch * segments * kRoundKeyWords * sizeof(u32w), s);
+    return cudaStreamSynchronize(s);  // the tables live on this stack frame
+}
+
+cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, u32w **d_rk, u64 **d_ctr, cudaStream_t s) {
+    const cudaError_t e = drbg_upload_tables(s);
+    return e == cudaSuccess ? drbg_chains_uploaded(d_seeds, segments, batch, d_rk, d_ctr, s) : e;
+}
+
+cudaError_t drbg_chains_uploaded(const unsigned char *d_seeds, int segments, int64_t batch, u32w **d_rk, u64 **d_ctr,
+                                 cudaStream_t s) {
+    cudaError_t e = cudaMallocAsync((void **)d_rk, (size_t)batch * segments * kRoundKeyWords * sizeof(u32w), s);
     if (e == cudaSuccess) e = cudaMallocAsync((void **)d_ctr, (size_t)batch * segments * 2 * sizeof(u64), s);
     if (e == cudaSuccess) e = launch(drbg_chain_kernel, (unsigned)((batch + 31) / 32), 64, 0, s, d_seeds, *d_rk, *d_ctr, segments, batch);
     return e;
@@ -181,19 +193,24 @@ void free_chains(u32w *d_rk, u64 *d_ctr, int segments, int64_t batch, cudaStream
 }
 
 // PolyRq.random mod p for `polys` polynomials of degree n from the one NistAes128Ctr stream of the 32-byte d_seed,
-// written as sigma(a) (drbg_sigma_fill_kernel) to d_out (polys x n)
-cudaError_t random_sigma_polys_device(const unsigned char *d_seed, u64 p, int64_t n, int64_t polys, u64 *d_out,
-                                      cudaStream_t s) {
+// written as a (sigma false) or sigma(a) (drbg_one_modulus_fill_kernel) to d_out (polys x n)
+cudaError_t random_polys_one_modulus_device(const unsigned char *d_seed, u64 p, int64_t n, int64_t polys, bool sigma,
+                                            u64 *d_out, cudaStream_t s) {
     const int64_t total = polys * n;
     const int segments = (int)((total * 16 + kSegmentBytes - 1) / kSegmentBytes);
     u32w *d_rk = nullptr;
     u64 *d_ctr = nullptr;
     cudaError_t e = drbg_chains(d_seed, segments, 1, &d_rk, &d_ctr, s);
     if (e == cudaSuccess)
-        e = launch(drbg_sigma_fill_kernel, (unsigned)segments, kSegmentBlocks, 0, s, d_rk, d_ctr, d_out, p, (long long)n,
-                   (long long)total);
+        e = launch(drbg_one_modulus_fill_kernel, (unsigned)segments, kSegmentBlocks, 0, s, d_rk, d_ctr, d_out, p,
+                   (long long)n, (long long)total, sigma);
     free_chains(d_rk, d_ctr, segments, 1, s);
     return e;
+}
+
+cudaError_t random_sigma_polys_device(const unsigned char *d_seed, u64 p, int64_t n, int64_t polys, u64 *d_out,
+                                      cudaStream_t s) {
+    return random_polys_one_modulus_device(d_seed, p, n, polys, true, d_out, s);
 }
 
 // Device addresses of the AES tables drbg_chains uploads, for kernels in other translation units that read a stream

@@ -118,6 +118,21 @@ PDB_HD uint64_t pir_coefficient(const PirShape &s, const PirPiece &p, long long 
     return (uint64_t)(acc >> (8 * bytes - shift - s.bits)) & mask;
 }
 
+// coefficientsToBytes (CoefficientPacking.swift:141-217), the inverse map: byte b is bits [8b, 8b + 8) of the big-endian
+// bit stream of `count` coefficients of `bits` bits each (coefficient(i) < 2^bits), zero past the last coefficient.
+template <typename Coefficient>
+PDB_HD unsigned coefficients_byte(Coefficient coefficient, long long count, int bits, long long b) {
+    unsigned out = 0;
+    long long cached = -1;
+    uint64_t c = 0;
+    for (int k = 0; k < 8; ++k) {
+        const long long bit = 8 * b + k, i = bit / bits;
+        if (i != cached && i < count) c = coefficient(i), cached = i;
+        out = (out << 1) | (i < count ? (unsigned)(c >> (bits - 1 - (int)(bit - i * bits))) & 1u : 0u);
+    }
+    return out;
+}
+
 // ---- PNNS ---------------------------------------------------------------------------------------------------------
 // A row-major rows x cols matrix in .diagonal packing: dimension = nextPow2(cols) diagonals of `results` =
 // ceil(rows / N) chunks each, diagonal d's chunks rotated by floor(d / baby) * baby in both SIMD half-rows.

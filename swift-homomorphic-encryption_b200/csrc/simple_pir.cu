@@ -155,12 +155,7 @@ __global__ void __launch_bounds__(kThreads) split_requests_kernel(const W *__res
     }
 }
 
-__device__ __forceinline__ void mma_u8(int (&c)[4], const uint4 &a, const uint2 &b) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-        : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
-        : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y));
-}
+using spir::mma_u8;
 
 struct ResponseArgs {
     const unsigned char *planes;
@@ -640,6 +635,20 @@ bool columns_match(const hecuda_simple_pir_params &p, int64_t rows) {
 }
 
 }  // namespace
+
+namespace hecuda {
+namespace api {
+
+int32_t simple_pir_derive(const hecuda_simple_pir_params *params, int64_t &m, int64_t &k, int64_t &entry_scalars, u64 &p) {
+    Derived d;
+    const int32_t rc = derive(params, d);
+    if (rc) return rc;
+    m = d.m, k = d.k, entry_scalars = d.entry_scalars, p = d.p;
+    return HECUDA_OK;
+}
+
+}  // namespace api
+}  // namespace hecuda
 
 extern "C" {
 

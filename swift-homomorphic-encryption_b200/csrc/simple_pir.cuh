@@ -1,6 +1,6 @@
 // simple_pir.cuh -- the arithmetic and index maps of the SimplePIR kernels (simple_pir.cu).  Every function is __host__
-// __device__, so tests/emu/simple_pir_emulate.cu and tests/emu/simple_pir_shards_emulate.cu replay exactly what the
-// kernels compute on the CPU.
+// __device__, so tests/emu/simple_pir_emulate.cu, simple_pir_shards_emulate.cu and simple_pir_client_emulate.cu replay
+// exactly what the kernels (simple_pir.cu, simple_pir_client.cu) compute on the CPU.
 //
 //   SimplePirServer.process            SimplePir/SimplePir+Database.swift:252-290
 //   SimplePirServer.computeResponse    SimplePir/SimplePir+Server.swift:31-38, Array2d.multiply(transposing:mask:)
@@ -68,6 +68,17 @@ SPIR_HD long long b_offset(long long q, long long c, long long col_tiles) {
     const int lane = (int)(q % kTileQueries) * 4 + ((cc & 15) >> 2);
     return tile * 256 + lane * 8 + (cc >> 4) * 4 + (cc & 3);
 }
+
+#ifdef __CUDACC__
+// The warp-level u8 x u8 -> s32 MMA of the response kernels and the client's results product: c += a (16 x 32 A
+// fragment, a_offset layout) . b (32 x 8 B fragment, b_offset layout)
+__device__ __forceinline__ void mma_u8(int (&c)[4], const uint4 &a, const uint2 &b) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+        : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+        : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y));
+}
+#endif
 
 // The processed database before its transpose is row-major K x M with entry e's coefficients at e * padded_entry
 // (:262-280); DB'[r][c] is its element c * M + r.  -> (entry, coefficient index), or entry = -1 for a zero.
@@ -185,6 +196,62 @@ SPIR_HD void decode_item(const ItemShape &s, long long col_tiles, long long loca
     pair = t % s.pairs;
     k_begin = t / s.pairs * s.split_tiles;
     k_end = k_begin + s.split_tiles < col_tiles ? k_begin + s.split_tiles : col_tiles;
+}
+
+// ---- the client (simple_pir_client.cu): PrecomputedQueries.WithoutIndices.init, add(index:), integrate
+//   generateSecretPolys / noiselessSample / encryptZero / extractEntries   SimplePir+Client.swift:20-95
+//   Array2d.multiply(transposing:modulus:)                                  SimplePir+Precompute.swift:122-188
+//   Array2d.divideAndRound, randomCenteredBinomialDistribution              Array2d.swift:382-429, 489-514
+// A query's secret seed draws its chunksPerEntry ternary polynomials one after another from one stream; its error seed
+// draws the 1 x (chunksPerEntry K) error array, which is then read as chunksPerEntry x K.  -> stream coefficient index.
+SPIR_HD long long secret_coefficient(long long i, long long j, long long n) { return i * n + j; }
+SPIR_HD long long error_coefficient(long long i, long long c, long long k) { return i * k + c; }
+// add(index:): the column of query row i (< chunksPerEntry) that gets delta = 2^(ct - pt)
+SPIR_HD long long delta_column(long long index, long long i, long long cpe, long long epc) { return (index * cpe + i) / epc; }
+// extractEntries: element t (< chunkSize) of row i of the extracted cpe x chunkSize array, as an offset into one query's
+// cpe x M array (responses or resultsWithoutResponse)
+SPIR_HD long long extract_offset(long long index, long long i, long long t, long long cpe, long long epc, long long m,
+                                 long long chunk) {
+    return i * m + (index * cpe + i) % epc * chunk + t;
+}
+
+typedef unsigned __int128 spir_u128;
+SPIR_HD uint64_t mulhi(uint64_t a, uint64_t b) { return (uint64_t)(((spir_u128)a * b) >> 64); }
+// floor(x / p) for any 128-bit x with the quotient below 2^64, and x mod p: Barrett with mu = floor(2^128 / p) = (mu_hi,
+// mu_lo) (p < 2^63, not a power of two) gives the low word of a quotient at most 2 below the true one, then corrections
+SPIR_HD uint64_t div_mod(spir_u128 x, uint64_t p, uint64_t mu_hi, uint64_t mu_lo, uint64_t &rem) {
+    const uint64_t lo = (uint64_t)x, hi = (uint64_t)(x >> 64);
+    const spir_u128 mid = (spir_u128)mulhi(lo, mu_lo) + (uint64_t)(lo * mu_hi) + (uint64_t)(hi * mu_lo);
+    uint64_t q = hi * mu_hi + mulhi(lo, mu_hi) + mulhi(hi, mu_lo) + (uint64_t)(mid >> 64);
+    uint64_t r = lo - q * p;  // the true remainder plus at most 2p, below 2^64
+    for (int i = 0; i < 2; ++i)
+        if (r >= p) r -= p, ++q;
+    rem = r;
+    return q;
+}
+// divideAndRound(initialMod: p, newMod: 2^ct) of x < p: floor((x 2^ct + floor(p / 2)) / p) mod 2^ct, exactly
+SPIR_HD uint64_t divide_and_round(uint64_t x, uint64_t p, uint64_t mu_hi, uint64_t mu_lo, int ct) {
+    uint64_t rem;
+    return div_mod(((spir_u128)x << ct) + (p >> 1), p, mu_hi, mu_lo, rem) & low_mask(ct);
+}
+// resultsWithoutResponse = S . hint^T mod p, with the secrets stored mod p (-1 as p - 1) and the reference's sum taken
+// in T.DoubleWidth with &+= (2 word_bits bits, wrapping).  With hint words split into u8 digits h = sum_d h_d 2^(8d)
+// and P_d, Nn_d the digit-d sums over the secret's +1 and -1 positions, the reference's sum is
+// U = sum_d (P_d + (p - 1) Nn_d) 2^(8d) mod 2^(2 word_bits).  results_add adds plane d's term mod 2^128 (a multiple of
+// 2^(2 word_bits)); results_word takes U mod p.
+SPIR_HD spir_u128 results_add(spir_u128 acc, uint32_t pos, uint32_t neg, int d, uint64_t p) {
+    return acc + (((spir_u128)pos + (spir_u128)(p - 1) * neg) << (8 * d));
+}
+SPIR_HD uint64_t results_word(spir_u128 acc, int word_bits, uint64_t p, uint64_t mu_hi, uint64_t mu_lo) {
+    if (word_bits == 32) acc = (uint64_t)acc;
+    uint64_t rem;
+    div_mod(acc, p, mu_hi, mu_lo, rem);
+    return rem;
+}
+// integrate: ((response - result + delta / 2) & mask) >> (ct - pt), in the scalar's wrapping arithmetic (the mask keeps
+// ct < word_bits bits, so 64-bit wrapping gives the same value)
+SPIR_HD uint64_t integrate(uint64_t response, uint64_t result, int pt, int ct) {
+    return ((response - result + ((1ull << (ct - pt)) >> 1)) & low_mask(ct)) >> (ct - pt);
 }
 
 }  // namespace spir

@@ -129,6 +129,12 @@ SYMBOLS = {
     "hecuda_simple_pir_compute_response_shards": (C.c_int32, [_VP, C.c_int32, C.c_int64, _VP, C.c_int64, _VP]),
     "hecuda_simple_pir_compute_response_shards_device": (C.c_int32, [_VP, C.c_int32, C.c_int64, _VP, C.c_int64, _VP,
                                                                      _VP]),
+    "hecuda_simple_pir_client_create": (C.c_int32, [_VP, _VP, _VP, C.POINTER(_VP)]),
+    "hecuda_simple_pir_client_destroy": (C.c_int32, [_VP]),
+    "hecuda_simple_pir_client_precompute": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int64, _VP, _VP]),
+    "hecuda_simple_pir_client_precompute_device": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int64, _VP, _VP, _VP]),
+    "hecuda_simple_pir_client_decrypt": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int64, _VP]),
+    "hecuda_simple_pir_client_decrypt_device": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int64, _VP, _VP]),
     "hecuda_mulpir_expand": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP]),
     "hecuda_mulpir_expand_device": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int64, _VP, _VP]),
     "hecuda_mulpir_compute_response": (C.c_int32, [_VP, _VP, C.POINTER(_VP), C.c_int32, C.POINTER(C.c_int32), C.c_int32,

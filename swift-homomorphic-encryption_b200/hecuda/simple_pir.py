@@ -9,6 +9,10 @@ Names follow Sources/PrivateInformationRetrieval/SimplePir/:
     Array2d.save / init(from:)                              SimplePir+Database.swift:36-121
     DatabaseMap, DatabaseMap.shardDatabase                  SimplePir/DatabaseMap.swift:18-110
     ShardMap                                                SimplePir/SimplePir+Shards.swift:18-45
+    DefaultQueryGenerator, PrecomputedQueries               SimplePir/SimplePir+Precompute.swift:191-356
+    SimplePirClient                                         SimplePir/SimplePir+Client.swift:98-127
+    SimplePirClientForAllShards                             SimplePir/SimplePir+Shards.swift:47-173
+    SimplePirServer.validate / SimplePirShardedServer.validate   verifyProcessing, SimplePIRProcessDatabase/main.swift:260-348
     SimplePIRProcessDatabase's sharding and file names      Sources/SimplePIRProcessDatabase/main.swift:158-253
 
 The processed database stays on the device as u8 digit planes; responses are integer tensor-core products there.
@@ -20,6 +24,8 @@ import ctypes as C
 import math
 import secrets
 import struct
+import time
+from collections import deque
 from dataclasses import dataclass, field
 from typing import Optional, Sequence
 
@@ -39,7 +45,8 @@ _MAX_LOG2_Q_STDDEV64 = {1 << 11: 42}
 class _Params(C.Structure):  # hecuda_simple_pir_params
     _fields_ = [("plaintext_modulus_bits", C.c_int32), ("ciphertext_modulus_bits", C.c_int32),
                 ("lattice_dimension", C.c_int64), ("entry_size", C.c_int64), ("entries_per_column", C.c_int64),
-                ("chunks_per_entry", C.c_int64), ("database_columns", C.c_int64), ("word_bits", C.c_int32)]
+                ("chunks_per_entry", C.c_int64), ("database_columns", C.c_int64), ("word_bits", C.c_int32),
+                ("error_std_dev", C.c_double)]
 
 
 @dataclass(frozen=True)
@@ -123,7 +130,8 @@ class SimplePirParameters:
 
     def _c(self, word_bits: int) -> _Params:
         return _Params(self.plaintextModulusBits, self.ciphertextModulusBits, self.latticeDimension, self.entrySizeInBytes,
-                       self.entriesPerColumn, self.chunksPerEntry, self.databaseColumns, word_bits)
+                       self.entriesPerColumn, self.chunksPerEntry, self.databaseColumns, word_bits,
+                       self.encryptionParams.errorStdDev)
 
 
 def _word_bits(scalar) -> int:
@@ -502,3 +510,282 @@ class SimplePirShardedServer:
     def close(self):
         for db in self.databases:
             db.close()
+
+
+# ---- the client (SimplePir+Client.swift, SimplePir+Precompute.swift:191-356, SimplePir+Shards.swift:47-173)
+def _seeds(seeds, count: int) -> np.ndarray:
+    """count x 32 seed bytes; None draws them with secrets.token_bytes."""
+    raw = b"".join(secrets.token_bytes(SEED_BYTES) for _ in range(count)) if seeds is None else b"".join(bytes(s) for s in seeds)
+    if len(raw) != count * SEED_BYTES:
+        raise PirError(f"need {count} seeds of {SEED_BYTES} bytes")
+    return np.frombuffer(raw, dtype=np.uint8).copy()
+
+
+@dataclass
+class WithPreparedResponse:
+    """PrecomputedQueries.WithPreparedResponse: the query's results (chunksPerEntry x columnSize) and index; the
+    extractEntries gather runs on the device with the decryption."""
+    resultsWithoutResponse: np.ndarray
+    index: int
+
+
+@dataclass
+class WithQueryIndices:
+    """PrecomputedQueries.WithQueryIndices: the request (chunksPerEntry x databaseColumns) for `index`."""
+    queries: np.ndarray
+    resultsWithoutResponse: np.ndarray
+    index: int
+
+    def prepareResponse(self) -> WithPreparedResponse:
+        return WithPreparedResponse(self.resultsWithoutResponse, self.index)
+
+
+@dataclass
+class WithoutIndices:
+    """PrecomputedQueries.WithoutIndices: an encrypted zero query and its resultsWithoutResponse."""
+    queriesWithoutIndices: np.ndarray
+    resultsWithoutResponse: np.ndarray
+    params: SimplePirParameters
+
+    def add(self, index: int) -> WithQueryIndices:
+        """add(index:) (SimplePir+Precompute.swift:241-256): delta at one column per chunk, in numpy."""
+        p = self.params
+        ct, pt = p.ciphertextModulusBits, p.plaintextModulusBits
+        q = self.queriesWithoutIndices.copy()
+        dtype = q.dtype.type
+        for i in range(p.chunksPerEntry):
+            col = (index * p.chunksPerEntry + i) // p.entriesPerColumn
+            q[i, col] = dtype((int(q[i, col]) + (1 << (ct - pt))) & ((1 << ct) - 1))
+        return WithQueryIndices(q, self.resultsWithoutResponse, index)
+
+
+class PrecomputedQueries:
+    WithoutIndices = WithoutIndices
+    WithQueryIndices = WithQueryIndices
+    WithPreparedResponse = WithPreparedResponse
+
+
+class DefaultQueryGenerator:
+    """DefaultQueryGenerator (SimplePir+Precompute.swift:321-356) on the device: the a-polynomials (Eval) and the hint
+    stay resident; addPrecomputedQueries(count) is one device call."""
+
+    def __init__(self, params: SimplePirParameters, hint, scalar=np.uint64, errorStdDev: Optional[float] = None):
+        self.scalar = np.dtype(scalar)
+        bits = _word_bits(self.scalar)
+        self.params = params
+        hint = np.ascontiguousarray(np.asarray(hint, dtype=self.scalar))
+        if hint.shape != (params.columnSize, params.latticeDimension):
+            raise PirError(f"hint must be {params.columnSize} x {params.latticeDimension}, got {hint.shape}")
+        if len(params.seed) != SEED_BYTES:
+            raise PirError(f"seed must be {SEED_BYTES} bytes")
+        cp = params._c(bits)
+        cp.error_std_dev = params.encryptionParams.errorStdDev if errorStdDev is None else errorStdDev
+        seed = np.frombuffer(params.seed, dtype=np.uint8).copy()
+        self._h = C.c_void_p()
+        _check(load_library().hecuda_simple_pir_client_create(_ptr(hint), C.byref(cp), _ptr(seed), C.byref(self._h)))
+        self.unusedRequests = deque()
+        self.addPrecomputedQueries()
+
+    def precompute(self, count: int, indices=None, secretSeeds=None, errorSeeds=None):
+        """count queries in one call -> (queries count x chunksPerEntry x K, results count x chunksPerEntry x M);
+        with indices, WithQueryIndices.queries."""
+        p = self.params
+        q = np.empty((count, p.chunksPerEntry, p.databaseColumns), dtype=self.scalar)
+        r = np.empty((count, p.chunksPerEntry, p.columnSize), dtype=self.scalar)
+        ss, es = _seeds(secretSeeds, count), _seeds(errorSeeds, count)
+        idx = None if indices is None else np.ascontiguousarray(indices, dtype=np.int64)
+        if idx is not None and idx.shape != (count,):
+            raise PirError("one index per query")
+        _check(load_library().hecuda_simple_pir_client_precompute(self._h, _ptr(ss), _ptr(es),
+                                                                  None if idx is None else _ptr(idx), count, _ptr(q), _ptr(r)))
+        return q, r
+
+    def addPrecomputedQueries(self, count: int = 1):
+        q, r = self.precompute(count)
+        self.unusedRequests.extend(WithoutIndices(q[i], r[i], self.params) for i in range(count))
+
+    def nextPrecomputedQueries(self) -> WithoutIndices:
+        if self.unusedRequests:
+            return self.unusedRequests.popleft()
+        q, r = self.precompute(1)
+        return WithoutIndices(q[0], r[0], self.params)
+
+    def close(self):
+        if self._h is not None:
+            load_library().hecuda_simple_pir_client_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class SimplePirClient:
+    """SimplePirClient<DefaultQueryGenerator> (SimplePir+Client.swift:98-127) with batched forms."""
+
+    def __init__(self, queryGenerator: DefaultQueryGenerator):
+        self.queryGenerator = queryGenerator
+        self.params, self.scalar = queryGenerator.params, queryGenerator.scalar
+
+    def query(self, at: int) -> WithQueryIndices:
+        return self.queryGenerator.nextPrecomputedQueries().add(at)
+
+    def queries(self, indices, secretSeeds=None, errorSeeds=None):
+        """One precompute call with the deltas added on the device -> [WithQueryIndices]."""
+        indices = [int(i) for i in indices]
+        q, r = self.queryGenerator.precompute(len(indices), indices, secretSeeds, errorSeeds)
+        return [WithQueryIndices(q[i], r[i], ix) for i, ix in enumerate(indices)]
+
+    def decryptMany(self, responses, results, indices) -> np.ndarray:
+        """count responses (count x chunksPerEntry x columnSize) -> count x entrySizeInBytes bytes, one device call."""
+        p = self.params
+        resp = np.ascontiguousarray(np.asarray(responses, dtype=self.scalar)).reshape(-1, p.chunksPerEntry, p.columnSize)
+        res = np.ascontiguousarray(np.asarray(results, dtype=self.scalar)).reshape(resp.shape)
+        idx = np.ascontiguousarray(indices, dtype=np.int64).reshape(-1)
+        if idx.shape[0] != resp.shape[0]:
+            raise PirError("one index per response")
+        out = np.empty((resp.shape[0], p.entrySizeInBytes), dtype=np.uint8)
+        _check(load_library().hecuda_simple_pir_client_decrypt(self.queryGenerator._h, _ptr(resp), _ptr(res), _ptr(idx),
+                                                               resp.shape[0], _ptr(out)))
+        return out
+
+    def decrypt(self, responses, with_: WithPreparedResponse, at: int) -> bytes:
+        return self.decryptMany(responses[None], with_.resultsWithoutResponse[None], [at])[0].tobytes()
+
+    def precomputeDevice(self, secret_seeds_ptr: int, error_seeds_ptr: int, indices_ptr: Optional[int], count: int,
+                         queries_ptr: int, results_ptr: int, stream: int = 0):
+        """Device buffers (torch data_ptr()): enqueue on `stream` without synchronising."""
+        _check(load_library().hecuda_simple_pir_client_precompute_device(
+            self.queryGenerator._h, C.c_void_p(secret_seeds_ptr), C.c_void_p(error_seeds_ptr),
+            None if indices_ptr is None else C.c_void_p(indices_ptr), count, C.c_void_p(queries_ptr),
+            C.c_void_p(results_ptr), C.c_void_p(stream)))
+
+    def decryptDevice(self, responses_ptr: int, results_ptr: int, indices_ptr: int, count: int, entries_ptr: int,
+                      stream: int = 0):
+        _check(load_library().hecuda_simple_pir_client_decrypt_device(
+            self.queryGenerator._h, C.c_void_p(responses_ptr), C.c_void_p(results_ptr), C.c_void_p(indices_ptr), count,
+            C.c_void_p(entries_ptr), C.c_void_p(stream)))
+
+
+class SimplePirClientForAllShards:
+    """SimplePirClientForAllShards (SimplePir+Shards.swift:47-173): one SimplePirClient per shard."""
+
+    def __init__(self, databaseMap, clients: Sequence[SimplePirClient]):
+        self.shardMap = databaseMap if isinstance(databaseMap, ShardMap) else ShardMap(databaseMap)
+        self.clients = list(clients)
+        if self.shardMap.shardCount != len(self.clients):
+            raise PirError(f"validationError: Mismatching shard count {self.shardMap.shardCount} and number of clients "
+                           f"{len(self.clients)}")
+
+    @property
+    def queriesPerShard(self) -> int:
+        return self.shardMap.chunksPerShard
+
+    def _rows(self, index: int):
+        rows = [[] for _ in self.clients]
+        entry = self.shardMap[index]
+        if entry is not None:
+            for c in entry.chunks:
+                rows[c.shardIndex].append(c.index)
+        return [r + [0] * (self.shardMap.chunksPerShard - len(r)) for r in rows]
+
+    def query(self, index: int):
+        """query(for:): per shard chunksPerShard WithQueryIndices (the entry's rows, then row 0), one precompute call
+        per shard; an absent index makes the same calls with the same shapes."""
+        return [client.queries(rows) for client, rows in zip(self.clients, self._rows(index))]
+
+    def queriesMany(self, indices):
+        """query(for:) for many clients at once -> (count x words requests in the client-major layout
+        SimplePirShardedServer.computeResponses(..., requests_per_shard) reads, the per-shard [WithQueryIndices] lists)."""
+        per = self.shardMap.chunksPerShard
+        rows = [self._rows(int(i)) for i in indices]
+        shards = [self.clients[s].queries([r for client in rows for r in client[s]]) for s in range(len(self.clients))]
+        flat = np.stack([np.concatenate([np.stack([w.queries for w in shards[s][c * per:(c + 1) * per]]).reshape(-1)
+                                         for s in range(len(self.clients))]) for c in range(len(rows))])
+        return flat, [[shards[s][c * per:(c + 1) * per] for s in range(len(self.clients))] for c in range(len(rows))]
+
+    def decrypt(self, responses, index: int, queries) -> Optional[bytes]:
+        """decrypt(responses:for:with:): every query of every shard is decrypted (one device call per shard), then the
+        reference's fixed-work chunk selection; None for an index the map does not hold."""
+        if len(responses) != len(self.clients) or len(queries) != len(self.clients):
+            raise PirError("validationError: one response and query list per shard")
+        plain = []
+        for client, rs, qs in zip(self.clients, responses, queries):
+            if len(rs) != len(qs):
+                raise PirError("validationError: response count does not match query count")
+            plain.append(client.decryptMany(np.stack([np.asarray(r) for r in rs]),
+                                            np.stack([q.resultsWithoutResponse for q in qs]), [q.index for q in qs]))
+        entry = self.shardMap[index]
+        chunks = entry.chunks if entry is not None else ()
+        out = b""
+        for c in range(self.shardMap.maximumChunkCount):
+            real = c < len(chunks)
+            shard, row = (chunks[c].shardIndex, chunks[c].index) if real else (0, 0)
+            at = 0
+            for i, q in enumerate(queries[shard]):
+                at = i if q.index == row else at
+            out += plain[shard][at][:self.shardMap.chunkSize].tobytes()
+        return None if entry is None else out[:entry.size]
+
+
+def _validate(trial, trials: int, index: int, expected: bytes):
+    """verifyProcessing (SimplePIRProcessDatabase/main.swift:260-348): `trials` fresh queries for `index`."""
+    times, value = [], None
+    for _ in range(trials):
+        start = time.perf_counter()
+        value = trial()
+        times.append(time.perf_counter() - start)
+        if value != bytes(expected):
+            raise PirError(f"Verification failed for index {index}")
+    return times, value
+
+
+def _server_validate(self, row, trials: int = 1, errorStdDev: Optional[float] = None):
+    """Query, answer and decrypt entry `row` = (index, expected bytes) with a device client built from the hint; raise
+    PirError on a mismatch.  -> (seconds per round trip, decrypted bytes)."""
+    index, expected = row
+    client = SimplePirClient(DefaultQueryGenerator(self.params, self.hint, self.scalar, errorStdDev))
+
+    def trial():
+        q = client.queries([index])[0]
+        response = self.computeResponse(q.queries)
+        return client.decrypt(response, q.prepareResponse(), index)
+
+    try:
+        return _validate(trial, trials, index, expected)
+    finally:
+        client.queryGenerator.close()
+
+
+def _sharded_validate(self, row, databaseMap: Optional[DatabaseMap] = None, trials: int = 1,
+                      errorStdDev: Optional[float] = None):
+    """verifyProcessing for sharded databases: entry `row` = (originalIndex, expected bytes) through one device client
+    per shard built from its hint and the all-shards client; raise PirError on a mismatch.  -> (seconds per round
+    trip, decrypted bytes)."""
+    index, expected = row
+    database_map = databaseMap if databaseMap is not None else self.databaseMap
+    if database_map is None:
+        raise PirError("validate needs the databaseMap")
+    clients = [SimplePirClient(DefaultQueryGenerator(p, h, self.scalar, errorStdDev)) for p, h in zip(self.params, self.hints)]
+    all_shards = SimplePirClientForAllShards(database_map, clients)
+    per = all_shards.queriesPerShard
+
+    def trial():
+        flat, queries = all_shards.queriesMany([index])
+        out = self.computeResponses(flat, requests_per_shard=per)[0]
+        bounds = np.concatenate([[0], np.cumsum(self._words(per)[1])])
+        responses = [out[bounds[s]:bounds[s + 1]].reshape(per, p.chunksPerEntry, p.columnSize)
+                     for s, p in enumerate(self.params)]
+        return all_shards.decrypt(responses, index, queries[0])
+
+    try:
+        return _validate(trial, trials, index, expected)
+    finally:
+        for c in clients:
+            c.queryGenerator.close()
+
+
+SimplePirServer.validate = _server_validate
+SimplePirShardedServer.validate = _sharded_validate
