@@ -316,6 +316,35 @@ int32_t hecuda_pir_database_device_buffer(hecuda_pir_database *db, void **device
  * when it was created without flags).  capacity >= the database's plaintext count. */
 int32_t hecuda_pir_database_present(const hecuda_pir_database *db, uint8_t *out, int64_t capacity);
 
+/* Processed databases in the reference's file format -- ProcessedDatabase.serialize() / save(to:) and
+ * ProcessedDatabase(from:context:) (IndexPir/IndexPirProtocol.swift:286-378): a version byte (1), plaintextCount as a
+ * little-endian UInt32, then per plaintext a tag byte, 0 for nil or 1 followed by PolyRq.serialize() of the Eval
+ * plaintext over every ciphertext modulus (ceil(log2 q_i) bits per coefficient, rows in order).  A keyword-PIR shard is
+ * one such stream: its tables' plaintexts concatenated in table order (KeywordPir/KeywordPirProtocol.swift:161-171,
+ * 230-239).  Whole plaintexts cross PCIe in chunks of at most 64 MB through two device staging buffers, and are unpacked
+ * into (or packed from) the resident rows on the device; a caller buffer that is pinned (hecuda_host_alloc,
+ * hecuda_host_register) is copied directly, a pageable one through pinned staging.  Peak device memory is the databases
+ * and 2 x 64 MB.  A Bfv<UInt32> context reads and writes the same bytes.
+ * hecuda_pir_databases_create_serialized: `byte_count` bytes -> `database_count` databases of plaintextCount /
+ * database_count plaintexts each (1 for index PIR, hashFunctionCount for keyword PIR), out[t] word for word what
+ * hecuda_pir_database_create builds from the same Eval plaintexts and flags.  Bytes after the last plaintext are ignored,
+ * as the reference ignores them.  Refused with HECUDA_ERR_INVALID_ARGUMENT, every out[t] NULL and nothing left allocated:
+ * a version other than 1 (invalidDatabaseSerializationVersion), a tag other than 0 or 1
+ * (invalidDatabaseSerializationPlaintextTag), a header, tag or plaintext past the end or a plaintextCount that cannot
+ * fit the buffer (corruptedData; the reference traps), no plaintexts (emptyDatabase), a plaintextCount that
+ * database_count does not divide (invalidDatabasePlaintextCount), and -- checked on the device -- a residue >= its
+ * modulus q_i (corruptedData, naming the plaintext and row; the reference accepts it, but the lazy accumulators of the
+ * scans assume canonical residues).  Every refusal except the last launches no kernel.
+ * hecuda_pir_databases_serialized_byte_count / _serialize: the serialization of `database_count` databases of one
+ * context concatenated (one header over all of their plaintexts).  Refused: null pointers, databases of different
+ * contexts, more than 2^32 - 1 plaintexts, only nil plaintexts (emptyDatabase), and a capacity below the size. */
+int32_t hecuda_pir_databases_create_serialized(const hecuda_context *ctx, const uint8_t *bytes, uint64_t byte_count,
+                                               int32_t database_count, hecuda_pir_database **out);
+int32_t hecuda_pir_databases_serialized_byte_count(const hecuda_pir_database *const *databases, int32_t database_count,
+                                                   uint64_t *bytes);
+int32_t hecuda_pir_databases_serialize(const hecuda_pir_database *const *databases, int32_t database_count, uint8_t *out,
+                                       uint64_t capacity, uint64_t *written);
+
 /* MulPirServer.process(database:with:using:) -- IndexPir/MulPir.swift:433-556 (processPackEntries,
  * processSplitLargeEntries, CoefficientPacking.bytesToCoefficients with floor(log2 t) bits per coefficient) on the
  * device.  entries: the concatenated entry bytes; offsets: entry_count + 1 byte offsets (entry i = [offsets[i],

@@ -15,39 +15,53 @@
 namespace hecuda {
 
 
+// offset of polynomial `poly`'s rows in `bytes` under `at` (-1: a nil plaintext)
+__device__ __forceinline__ long long poly_bytes_offset(const CodecConsts &c, const PolyLayout &at, int64_t poly) {
+    return at.tag ? tagged_rows_offset(at.tag + at.first, at.base, poly) : poly * c.byte_offset[c.rows];
+}
+
 // bytes -> coefficients: one thread per coefficient
-__global__ void __launch_bounds__(256) poly_load_kernel(const unsigned char *__restrict__ bytes, u64 *__restrict__ out,
-                                                       const __grid_constant__ CodecConsts c, int n, int skip) {
+template <typename Word>
+__global__ void __launch_bounds__(256) poly_load_kernel(const unsigned char *__restrict__ bytes, Word *__restrict__ out,
+                                                       const __grid_constant__ CodecConsts c, int n, int skip,
+                                                       const __grid_constant__ PolyLayout at) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int row = blockIdx.y;
     const int64_t poly = blockIdx.z;
+    const long long offset = poly_bytes_offset(c, at, poly);
+    if (at.present && row == 0 && i == 0) at.present[poly] = offset >= 0;
+    Word *dst = out + (poly * c.rows + row) * n + i;
+    if (offset < 0) {
+        *dst = 0;
+        return;
+    }
     const long long row_bytes = c.byte_offset[row + 1] - c.byte_offset[row];
-    const unsigned char *src = bytes + poly * c.byte_offset[c.rows] + c.byte_offset[row];
-    out[(poly * c.rows + row) * n + i] = codec_unpack(src, row_bytes, c.width[row], i) << skip;
+    const u64 v = codec_unpack(bytes + offset + c.byte_offset[row], row_bytes, c.width[row], i) << skip;
+    if (at.bad && v >= c.modulus[row]) atomicMin(at.bad, (unsigned long long)(at.first + poly) * c.rows + row);
+    *dst = (Word)v;
+}
+
+// the tag byte of a tagged stream's plaintext, written by the first thread of its first row
+__device__ __forceinline__ void write_tag(unsigned char *bytes, const PolyLayout &at, int64_t poly, long long offset, long long j) {
+    if (at.tag && blockIdx.y == 0 && j == 0) bytes[at.tag[at.first + poly] - at.base] = offset >= 0;
 }
 
 // coefficients -> bytes: one thread per output byte
-__global__ void __launch_bounds__(256) poly_serialize_kernel(const u64 *__restrict__ in, unsigned char *__restrict__ bytes,
-                                                            const __grid_constant__ CodecConsts c, int n, int skip) {
+template <typename Word>
+__global__ void __launch_bounds__(256) poly_serialize_kernel(const Word *__restrict__ in, unsigned char *__restrict__ bytes,
+                                                            const __grid_constant__ CodecConsts c, int n, int skip,
+                                                            const __grid_constant__ PolyLayout at) {
     const int row = blockIdx.y;
     const int64_t poly = blockIdx.z;
     const long long row_bytes = c.byte_offset[row + 1] - c.byte_offset[row];
     const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= row_bytes) return;
-    const int w = c.width[row];
-    const u64 mask = w >= 64 ? ~0ull : ((1ull << w) - 1);
-    const u64 *src = in + (poly * c.rows + row) * n;
-    const long long lo_bit = 8 * j, hi_bit = lo_bit + 8;
-    unsigned value = 0;
-    for (long long coeff = lo_bit / w; coeff < n && coeff * w < hi_bit; ++coeff) {
-        const long long begin = coeff * w, end = begin + w;
-        const long long lo = begin > lo_bit ? begin : lo_bit, hi = end < hi_bit ? end : hi_bit;
-        const u64 v = (src[coeff] >> skip) & mask;
-        const unsigned field = (unsigned)((v >> (end - hi)) & ((1ull << (hi - lo)) - 1));
-        value |= field << (hi_bit - hi);
-    }
-    bytes[poly * c.byte_offset[c.rows] + c.byte_offset[row] + j] = (unsigned char)value;
+    const long long offset = poly_bytes_offset(c, at, poly);
+    write_tag(bytes, at, poly, offset, j);
+    if (offset < 0) return;
+    const u64 value = codec_pack(in + (poly * c.rows + row) * n, n, c.width[row], skip, 8 * j, 8);
+    bytes[offset + c.byte_offset[row] + j] = (unsigned char)value;
 }
 
 static int ceil_log2_u64(u64 q) {  // T.ceilLog2
@@ -67,62 +81,94 @@ bool codec_consts(const Context &ctx, const NttRowMap &map, int skip, CodecConst
         }
         c.width[r] = bits - skip;
         c.byte_offset[r + 1] = c.byte_offset[r] + ((long long)ctx.n * c.width[r] + 7) / 8;
+        c.modulus[r] = ctx.slots[map.slot[r]].dev.p;
     }
     return true;
 }
 
 long long serialized_poly_bytes(const CodecConsts &c) { return c.byte_offset[c.rows]; }
 
-cudaError_t launch_poly_load(const Context &ctx, const CodecConsts &c, int skip, const unsigned char *bytes, u64 *out,
-                             int64_t polys, cudaStream_t stream) {
+// `at` for the polynomials from `done` on: a tagged layout moves its first plaintext, the default one its pointers
+PolyLayout layout_from(const PolyLayout &at, int64_t done) {
+    PolyLayout part = at;
+    part.first += done;
+    if (part.present) part.present += done;
+    return part;
+}
+
+template <typename Word>
+cudaError_t launch_poly_load(const Context &ctx, const CodecConsts &c, int skip, const unsigned char *bytes, Word *out,
+                             int64_t polys, cudaStream_t stream, const PolyLayout &layout) {
     const int threads = coeff_threads(ctx.n);
     return for_each_part(polys, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((ctx.n + threads - 1) / threads), (unsigned)c.rows, (unsigned)chunk);
-        return launch(poly_load_kernel, grid, threads, 0, stream, bytes + done * c.byte_offset[c.rows],
-                      out + done * c.rows * ctx.n, c, (int)ctx.n, skip);
+        return launch(poly_load_kernel<Word>, grid, threads, 0, stream, layout.tag ? bytes : bytes + done * c.byte_offset[c.rows],
+                      out + done * c.rows * ctx.n, c, (int)ctx.n, skip, layout_from(layout, done));
     });
 }
 
-// coefficients -> bytes, 8 output bytes per thread (rows whose byte count and offset are multiples of 8: N >= 64)
-__global__ void __launch_bounds__(256) poly_serialize_words_kernel(const u64 *__restrict__ in, unsigned char *__restrict__ bytes,
-                                                                  const __grid_constant__ CodecConsts c, int n, int skip) {
+// coefficients -> bytes, 8 output bytes per thread (rows whose byte count and offset are multiples of 8: N >= 64).
+// A tagged stream's rows start one byte after their tag, so mostly off an 8-byte boundary: the 8 bytes then go out in
+// the widest stores that the rows' alignment allows, the same for every thread of the block.
+template <typename Word>
+__global__ void __launch_bounds__(256) poly_serialize_words_kernel(const Word *__restrict__ in, unsigned char *__restrict__ bytes,
+                                                                  const __grid_constant__ CodecConsts c, int n, int skip,
+                                                                  const __grid_constant__ PolyLayout at) {
     const int row = blockIdx.y;
     const int64_t poly = blockIdx.z;
     const long long row_words = (c.byte_offset[row + 1] - c.byte_offset[row]) >> 3;
     const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= row_words) return;
-    const int w = c.width[row];
-    const u64 mask = w >= 64 ? ~0ull : ((1ull << w) - 1);
-    const u64 *src = in + (poly * c.rows + row) * n;
-    const long long lo_bit = 64 * j, hi_bit = lo_bit + 64;
-    u64 value = 0;  // big-endian bit stream: stream bit lo_bit is the MSB of `value`
-    for (long long coeff = lo_bit / w; coeff < n && coeff * w < hi_bit; ++coeff) {
-        const long long begin = coeff * w, end = begin + w;
-        const long long lo = begin > lo_bit ? begin : lo_bit, hi = end < hi_bit ? end : hi_bit;
-        const int bits = (int)(hi - lo);
-        const u64 v = (src[coeff] >> skip) & mask;
-        const u64 field = (v >> (end - hi)) & (bits >= 64 ? ~0ull : ((1ull << bits) - 1));
-        value |= bits >= 64 ? field : field << (hi_bit - hi);
-    }
+    const long long offset = poly_bytes_offset(c, at, poly);
+    write_tag(bytes, at, poly, offset, j);
+    if (offset < 0) return;
+    // big-endian bit stream: stream bit 64 j is the MSB of the value
+    const u64 value = codec_pack(in + (poly * c.rows + row) * n, n, c.width[row], skip, 64 * j, 64);
     // store most significant byte first
     const u64 swapped = __byte_perm((unsigned)(value >> 32), 0, 0x0123) | ((u64)__byte_perm((unsigned)value, 0, 0x0123) << 32);
-    *reinterpret_cast<u64 *>(bytes + poly * c.byte_offset[c.rows] + c.byte_offset[row] + 8 * j) = swapped;
+    unsigned char *dst = bytes + offset + c.byte_offset[row] + 8 * j;
+    switch (reinterpret_cast<uintptr_t>(dst) & 7) {
+    case 0:
+        *reinterpret_cast<u64 *>(dst) = swapped;
+        break;
+    case 4:
+        for (int k = 0; k < 2; ++k) reinterpret_cast<unsigned *>(dst)[k] = (unsigned)(swapped >> (32 * k));
+        break;
+    case 2:
+    case 6:
+        for (int k = 0; k < 4; ++k) reinterpret_cast<unsigned short *>(dst)[k] = (unsigned short)(swapped >> (16 * k));
+        break;
+    default:
+        for (int k = 0; k < 8; ++k) dst[k] = (unsigned char)(swapped >> (8 * k));
+    }
 }
 
-cudaError_t launch_poly_serialize(const Context &ctx, const CodecConsts &c, int skip, const u64 *in, unsigned char *bytes,
-                                  int64_t polys, cudaStream_t stream) {
+template <typename Word>
+cudaError_t launch_poly_serialize(const Context &ctx, const CodecConsts &c, int skip, const Word *in, unsigned char *bytes,
+                                  int64_t polys, cudaStream_t stream, const PolyLayout &layout) {
     long long widest = 0;
-    bool words = (reinterpret_cast<uintptr_t>(bytes) & 7) == 0 && (c.byte_offset[c.rows] & 7) == 0;
+    // a tagged stream's rows are at least byte aligned; a plain one's must sit on 8-byte boundaries
+    bool words = layout.tag || ((reinterpret_cast<uintptr_t>(bytes) & 7) == 0 && (c.byte_offset[c.rows] & 7) == 0);
     for (int r = 0; r < c.rows; ++r) {
         widest = std::max(widest, c.byte_offset[r + 1] - c.byte_offset[r]);
         words = words && (c.byte_offset[r] & 7) == 0 && (c.byte_offset[r + 1] & 7) == 0;
     }
     return for_each_part(polys, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)(((words ? widest / 8 : widest) + 255) / 256), (unsigned)c.rows, (unsigned)chunk);
-        return launch(words ? poly_serialize_words_kernel : poly_serialize_kernel, grid, 256, 0, stream,
-                      in + done * c.rows * ctx.n, bytes + done * c.byte_offset[c.rows], c, (int)ctx.n, skip);
+        return launch(words ? poly_serialize_words_kernel<Word> : poly_serialize_kernel<Word>, grid, 256, 0, stream,
+                      in + done * c.rows * ctx.n, layout.tag ? bytes : bytes + done * c.byte_offset[c.rows], c, (int)ctx.n,
+                      skip, layout_from(layout, done));
     });
 }
+
+template cudaError_t launch_poly_load<u64>(const Context &, const CodecConsts &, int, const unsigned char *, u64 *, int64_t,
+                                           cudaStream_t, const PolyLayout &);
+template cudaError_t launch_poly_load<u32>(const Context &, const CodecConsts &, int, const unsigned char *, u32 *, int64_t,
+                                           cudaStream_t, const PolyLayout &);
+template cudaError_t launch_poly_serialize<u64>(const Context &, const CodecConsts &, int, const u64 *, unsigned char *,
+                                                int64_t, cudaStream_t, const PolyLayout &);
+template cudaError_t launch_poly_serialize<u32>(const Context &, const CodecConsts &, int, const u32 *, unsigned char *,
+                                                int64_t, cudaStream_t, const PolyLayout &);
 
 }  // namespace hecuda
 

@@ -175,9 +175,10 @@ struct CodecConsts {
     int rows;
     int width[kMaxRows];                  // serialized bits per coefficient of each row
     long long byte_offset[kMaxRows + 1];  // of each row inside one serialized polynomial
+    u64 modulus[kMaxRows];                // of each row (a checked load refuses residues >= it)
 };
 // field i of one row: the `w` bits at bit i * w of the big-endian stream of the row's `row_bytes` bytes at `src`
-__device__ __forceinline__ u64 codec_unpack(const unsigned char *__restrict__ src, long long row_bytes, int w, long long i) {
+HE_HD u64 codec_unpack(const unsigned char *__restrict__ src, long long row_bytes, int w, long long i) {
     const long long bit = i * w;
     const long long first = bit >> 3;
     const int shift = (int)(bit & 7);
@@ -190,21 +191,58 @@ __device__ __forceinline__ u64 codec_unpack(const unsigned char *__restrict__ sr
     const u64 mask = w >= 64 ? ~0ull : ((1ull << w) - 1);
     return (u64)(acc >> (72 - shift - w)) & mask;
 }
+// the inverse: bits [lo_bit, lo_bit + span) (span <= 64) of the big-endian stream of one row's n coefficients at `src`
+// (each shifted right by `skip` and cut to `w` bits), stream bit lo_bit as bit span - 1 of the result
+template <typename Word>
+HE_HD u64 codec_pack(const Word *__restrict__ src, int n, int w, int skip, long long lo_bit, int span) {
+    const u64 mask = w >= 64 ? ~0ull : ((1ull << w) - 1);
+    const long long hi_bit = lo_bit + span;
+    u64 value = 0;
+    for (long long coeff = lo_bit / w; coeff < n && coeff * w < hi_bit; ++coeff) {
+        const long long begin = coeff * w, end = begin + w;
+        const long long lo = begin > lo_bit ? begin : lo_bit, hi = end < hi_bit ? end : hi_bit;
+        const int bits = (int)(hi - lo);
+        const u64 v = ((u64)src[coeff] >> skip) & mask;
+        const u64 field = (v >> (end - hi)) & (bits >= 64 ? ~0ull : ((1ull << bits) - 1));
+        value |= bits >= 64 ? field : field << (hi_bit - hi);
+    }
+    return value;
+}
+// Where each polynomial's bytes are.  Default: polynomial p at p * serialized_poly_bytes.  With `tag`: a processed
+// database's stream (IndexPirProtocol.swift:336-378) staged from byte `base` of the file, in which plaintext `first` + p
+// has its tag byte at tag[first + p] and, unless it is nil, its rows right after it; tag[first + p + 1] is where the
+// next one starts.  A load then writes present[p], writes zero rows for a nil plaintext, and atomically lowers *bad to
+// (first + p) * rows + row where a residue is >= its modulus; a serialization writes the tag byte too.
+struct PolyLayout {
+    const long long *tag = nullptr;
+    long long base = 0, first = 0;
+    unsigned char *present = nullptr;
+    unsigned long long *bad = nullptr;
+};
+// offset from `base` of the rows of plaintext p of a tagged stream (tag[] as in PolyLayout), or -1 for a nil plaintext
+HE_HD long long tagged_rows_offset(const long long *tag, long long base, long long p) {
+    return tag[p + 1] - tag[p] > 1 ? tag[p] + 1 - base : -1;
+}
 bool codec_consts(const Context &ctx, const NttRowMap &map, int skip, CodecConsts &c, std::string &err);
 long long serialized_poly_bytes(const CodecConsts &c);
-cudaError_t launch_poly_load(const Context &ctx, const CodecConsts &c, int skip, const unsigned char *bytes, u64 *out,
-                             int64_t polys, cudaStream_t stream);
-cudaError_t launch_poly_serialize(const Context &ctx, const CodecConsts &c, int skip, const u64 *in, unsigned char *bytes,
-                                  int64_t polys, cudaStream_t stream);
+// bytes -> rows of `Word` (uint64, or uint32 when every modulus is below 2^32)
+template <typename Word>
+cudaError_t launch_poly_load(const Context &ctx, const CodecConsts &c, int skip, const unsigned char *bytes, Word *out,
+                             int64_t polys, cudaStream_t stream, const PolyLayout &layout = PolyLayout{});
+template <typename Word>
+cudaError_t launch_poly_serialize(const Context &ctx, const CodecConsts &c, int skip, const Word *in, unsigned char *bytes,
+                                  int64_t polys, cudaStream_t stream, const PolyLayout &layout = PolyLayout{});
 
 // uint32 <-> uint64 residues at the boundary of a Bfv<UInt32> context (elementwise.cu); both buffers 16-byte aligned
 cudaError_t launch_widen(const u32 *in, u64 *out, int64_t words, cudaStream_t stream);
 cudaError_t launch_narrow(const u64 *in, u32 *out, int64_t words, cudaStream_t stream);
 
 // ---- the server's data into plaintexts (process_db.cu; index maps in process_db.cuh)
+// The device staging budget of the database pipelines: 64 MB per slab
+constexpr int64_t kSlabBytes = (int64_t)64 << 20;
 // Plaintexts per slab when a database is packed and converted to Eval piecewise: <= 64 MB of coefficients
 inline int64_t coefficient_slab(const Context &ctx) {
-    const int64_t per = (int64_t)((size_t)8 * 1024 * 1024 / ctx.n);
+    const int64_t per = kSlabBytes / (int64_t)(sizeof(u64) * ctx.n);
     return per > 1 ? per : 1;
 }
 // MulPirServer.process: plaintexts first .. first + items of the database `s` (entries / offsets on the device) ->

@@ -21,6 +21,7 @@
 #include <set>
 
 #include "capi_internal.hpp"
+#include "database_io.hpp"
 #include "wire_codec.hpp"
 
 using namespace hecuda;
@@ -909,6 +910,150 @@ int32_t pir_databases_from_device_entries(const hecuda_context *h, const unsigne
 }  // namespace api
 }  // namespace hecuda
 
+// ---------------------------------------------------------------- saving and loading processed databases
+// ProcessedDatabase.serialize / init(from:context:) (IndexPirProtocol.swift:286-378).  The host walks the tags
+// (database_io.hpp); whole plaintexts then cross PCIe in chunks of at most one 64 MB slab through two device staging
+// buffers, one stream each, so that chunk k + 1's copy runs under chunk k's kernel.  The kernels (codec.cu) unpack
+// straight into the resident rows, or pack straight from them.
+namespace {
+
+// A caller's buffer that is pinned from its first to its last byte (hecuda_host_alloc, hecuda_host_register) is copied
+// from directly; a pageable one goes through pinned staging.
+bool host_pinned(const void *p, size_t bytes) {
+    for (const char *at : {(const char *)p, (const char *)p + bytes - 1}) {
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, at) != cudaSuccess) {
+            cudaGetLastError();
+            return false;
+        }
+        if (a.type != cudaMemoryTypeHost) return false;
+    }
+    return true;
+}
+
+// The pipeline's buffers: two pooled workspaces, each a stream and a device staging buffer (its staged-input buffer,
+// which stays with the workspace for later calls), and for a pageable caller buffer a pinned buffer per stream with the
+// event after which it may be reused.  The streams are synchronized before this is destroyed.
+struct DbStaging {
+    WsGuard g0, g1;
+    cudaStream_t stream[2];
+    unsigned char *dev[2] = {nullptr, nullptr}, *host[2] = {nullptr, nullptr};
+    cudaEvent_t copied[2] = {nullptr, nullptr};
+    explicit DbStaging(const hecuda_context *h) : g0(h), g1(h) {
+        stream[0] = g0.w ? g0.w->stream : nullptr;
+        stream[1] = g1.w ? g1.w->stream : nullptr;
+    }
+    cudaError_t init(size_t bytes, bool pageable) {
+        if (!g0.w || !g1.w) return cudaErrorMemoryAllocation;
+        Workspace *w[2] = {g0.w, g1.w};
+        for (int b = 0; b < 2; ++b) {
+            cudaError_t e = w[b]->in.reserve((bytes + sizeof(u64) - 1) / sizeof(u64));
+            dev[b] = (unsigned char *)w[b]->in.p;
+            if (e == cudaSuccess && pageable) e = cudaHostAlloc(&host[b], bytes, cudaHostAllocDefault);
+            if (e == cudaSuccess && pageable) e = cudaEventCreateWithFlags(&copied[b], cudaEventDisableTiming);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    }
+    ~DbStaging() {
+        for (int b = 0; b < 2; ++b) {
+            if (host[b]) cudaFreeHost(host[b]);
+            if (copied[b]) cudaEventDestroy(copied[b]);
+        }
+    }
+};
+
+// one chunk of the pipeline: plaintexts of the stream, the first of which is plaintext `local` of database `db`
+struct DbChunk {
+    int db;
+    int64_t local;
+    dbio::Chunk chunk;
+};
+
+// the chunks of databases of counts[t] plaintexts each, concatenated in the stream, and the largest chunk's bytes
+std::vector<DbChunk> plan_db_chunks(const std::vector<long long> &tag, const std::vector<int64_t> &counts, long long &widest) {
+    std::vector<DbChunk> plan;
+    widest = 1;
+    int64_t first = 0;
+    for (size_t t = 0; t < counts.size(); first += counts[t++])
+        for (const dbio::Chunk &ch : dbio::plan_chunks(tag, first, first + counts[t], kSlabBytes)) {
+            plan.push_back({(int)t, ch.first - first, ch});
+            widest = std::max(widest, tag[(size_t)(ch.first + ch.count)] - tag[(size_t)ch.first]);
+        }
+    return plan;
+}
+
+// resident rows of a database, whichever word type it keeps
+struct ResidentRows {
+    u64 *p64;
+    u32 *p32;
+    size_t row_words;
+    template <class F>
+    cudaError_t with(int64_t first, F f) const {
+        return p32 ? f(p32 + row_words * first) : f(p64 + row_words * first);
+    }
+};
+ResidentRows resident_rows(const Context &c, const hecuda_pir_database *db) {
+    return {db->d_plain, db->d_plain32, (size_t)c.L * c.n};
+}
+
+std::string corrupted(const std::string &what) { return "corruptedData(" + what + ")"; }
+
+int32_t load_refusal(const dbio::TagWalk &w, uint64_t byte_count, long long plaintext_bytes) {
+    const std::string size = std::to_string(byte_count) + "-byte buffer";
+    switch (w.error) {
+    case dbio::TagWalk::kVersion:
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidDatabaseSerializationVersion(serializationVersion: " +
+                                                     std::to_string(w.value) + ", expected: " + std::to_string(dbio::kVersion) + ")");
+    case dbio::TagWalk::kTag:
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidDatabaseSerializationPlaintextTag(tag: " + std::to_string(w.value) +
+                                                     ") of plaintext " + std::to_string(w.at));
+    default:
+        if (w.at < 0 && w.count == 0)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, corrupted("the header runs past the end of the " + size));
+        if (w.at < 0)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, corrupted("plaintextCount " + std::to_string(w.count) + " cannot fit the " + size));
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, corrupted("plaintext " + std::to_string(w.at) + " (" +
+                                                           std::to_string(plaintext_bytes) + " bytes after its tag) runs past the end of the " + size));
+    }
+}
+
+// The checks shared by the byte count and the serialization, and the tag offset of every plaintext of the
+// concatenated databases.  Copies the presence flags to the host; launches nothing.
+int32_t serialization_plan(const hecuda_pir_database *const *dbs, int32_t database_count, CodecConsts &cc,
+                           std::vector<long long> &tag) {
+    if (!dbs || database_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument / no databases");
+    long long total = 0;
+    for (int32_t i = 0; i < database_count; ++i) {
+        if (!dbs[i]) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null database");
+        if (dbs[i]->owner != dbs[0]->owner)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidContext: the databases belong to different contexts");
+        total += dbs[i]->count;
+    }
+    int32_t rc = check_ctx(dbs[0]->owner);
+    if (rc) return rc;
+    if (total > dbio::kMaxCount)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "a serialized database holds at most 2^32 - 1 plaintexts (UInt32 plaintextCount), not " +
+                                                     std::to_string(total));
+    const Context &c = *dbs[0]->owner->ctx;
+    std::string err;
+    if (!codec_consts(c, c.map_q(c.L), 0, cc, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+    std::vector<unsigned char> present((size_t)total);
+    long long at = 0;
+    for (int32_t i = 0; i < database_count; ++i) {
+        if (dbs[i]->d_present)
+            CK(cudaMemcpy(present.data() + at, dbs[i]->d_present, (size_t)dbs[i]->count, cudaMemcpyDeviceToHost));
+        else
+            memset(present.data() + at, 1, (size_t)dbs[i]->count);
+        at += dbs[i]->count;
+    }
+    if (std::find(present.begin(), present.end(), 1) == present.end()) return fail(HECUDA_ERR_INVALID_ARGUMENT, "emptyDatabase");
+    dbio::tag_offsets(present.data(), total, serialized_poly_bytes(cc), tag);
+    return HECUDA_OK;
+}
+
+}  // namespace
+
 extern "C" {
 
 int32_t hecuda_pir_process_entries(const hecuda_context *h, const uint8_t *entries, const uint64_t *offsets,
@@ -1042,6 +1187,167 @@ int32_t hecuda_pir_database_present(const hecuda_pir_database *db, uint8_t *out,
         return HECUDA_OK;
     }
     CK(cudaMemcpy(out, db->d_present, (size_t)db->count, cudaMemcpyDeviceToHost));
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pir_databases_create_serialized(const hecuda_context *h, const uint8_t *bytes, uint64_t byte_count,
+                                               int32_t database_count, hecuda_pir_database **out) {
+    if (!out || database_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument / no databases");
+    for (int32_t t = 0; t < database_count; ++t) out[t] = nullptr;
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (!bytes) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null buffer");
+    const Context &c = *h->ctx;
+    CodecConsts cc;
+    std::string err;
+    if (!codec_consts(c, c.map_q(c.L), 0, cc, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+    const long long plaintext_bytes = serialized_poly_bytes(cc);
+    std::vector<long long> tag;
+    const dbio::TagWalk walk = dbio::walk_tags(bytes, (long long)std::min<uint64_t>(byte_count, INT64_MAX), plaintext_bytes, tag);
+    if (walk.error != dbio::TagWalk::kOk) return load_refusal(walk, byte_count, plaintext_bytes);
+    if (walk.count == 0) return fail(HECUDA_ERR_INVALID_ARGUMENT, "emptyDatabase: no plaintexts to load");
+    if (walk.count % database_count)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidDatabasePlaintextCount(plaintextCount: " + std::to_string(walk.count) +
+                                                     ", expected: a multiple of " + std::to_string(database_count) + ")");
+    const int64_t per_db = walk.count / database_count;
+    long long widest = 0;
+    const std::vector<DbChunk> plan = plan_db_chunks(tag, std::vector<int64_t>((size_t)database_count, per_db), widest);
+    const bool pinned = host_pinned(bytes, (size_t)tag.back());
+    const bool narrow = inner_product_plain_small_supported(c, c.L);
+    const size_t rows_words = (size_t)c.L * c.n * per_db;
+
+    DbStaging st(h);
+    if (!st.g0.w || !st.g1.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    const cudaStream_t *streams = st.stream;
+    std::vector<hecuda_pir_database *> dbs;
+    long long *d_tag = nullptr;
+    unsigned long long *d_bad = nullptr, bad = ~0ull;
+    cudaError_t e = cudaSuccess;
+    for (int32_t t = 0; t < database_count && e == cudaSuccess; ++t) {
+        hecuda_pir_database *db = new (std::nothrow) hecuda_pir_database();
+        if (!db) {
+            e = cudaErrorMemoryAllocation;
+            break;
+        }
+        db->owner = h;
+        db->count = per_db;
+        dbs.push_back(db);
+        e = narrow ? cudaMalloc(&db->d_plain32, rows_words * sizeof(u32)) : cudaMalloc(&db->d_plain, rows_words * sizeof(u64));
+        if (e == cudaSuccess) e = cudaMalloc(&db->d_present, (size_t)per_db);
+    }
+    if (e == cudaSuccess) e = cudaMalloc(&d_tag, tag.size() * sizeof(long long));
+    if (e == cudaSuccess) e = upload(d_tag, tag.data(), tag.size() * sizeof(long long));
+    if (e == cudaSuccess) e = cudaMalloc(&d_bad, sizeof(unsigned long long));
+    if (e == cudaSuccess) e = fill(d_bad, 0xff, sizeof(unsigned long long));
+    if (e == cudaSuccess) e = st.init((size_t)widest, !pinned);
+    for (size_t k = 0; k < plan.size() && e == cudaSuccess; ++k) {
+        const int b = (int)(k & 1);
+        const dbio::Chunk &ch = plan[k].chunk;
+        const long long base = tag[(size_t)ch.first], size = tag[(size_t)(ch.first + ch.count)] - base;
+        const unsigned char *src = bytes + base;
+        if (!pinned) {  // the pinned buffer is free once the copy two chunks back has finished
+            if (k >= 2) e = cudaEventSynchronize(st.copied[b]);
+            if (e != cudaSuccess) break;
+            memcpy(st.host[b], src, (size_t)size);
+            src = st.host[b];
+        }
+        e = cudaMemcpyAsync(st.dev[b], src, (size_t)size, cudaMemcpyHostToDevice, streams[b]);
+        if (e == cudaSuccess && !pinned) e = cudaEventRecord(st.copied[b], streams[b]);
+        hecuda_pir_database *db = dbs[(size_t)plan[k].db];
+        const PolyLayout at{d_tag, base, ch.first, db->d_present + plan[k].local, d_bad};
+        if (e == cudaSuccess)
+            e = resident_rows(c, db).with(plan[k].local, [&](auto *rows) {
+                return launch_poly_load(c, cc, 0, st.dev[b], rows, ch.count, streams[b], at);
+            });
+    }
+    for (int b = 0; b < 2; ++b) {
+        const cudaError_t e2 = cudaStreamSynchronize(streams[b]);
+        if (e == cudaSuccess) e = e2;
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost);
+    cudaFree(d_tag);
+    cudaFree(d_bad);
+    if (e == cudaSuccess && bad == ~0ull) {
+        for (int32_t t = 0; t < database_count; ++t) out[t] = dbs[(size_t)t];
+        return HECUDA_OK;
+    }
+    for (hecuda_pir_database *db : dbs) hecuda_pir_database_destroy(db);
+    if (e != cudaSuccess) return cuda_fail(e, "pir databases from serialized bytes");
+    const int row = (int)(bad % (unsigned long long)c.L);
+    return fail(HECUDA_ERR_INVALID_ARGUMENT, corrupted("plaintext " + std::to_string(bad / (unsigned long long)c.L) + ", row " +
+                                                       std::to_string(row) + ": a residue is not below q_" + std::to_string(row) +
+                                                       " = " + std::to_string(cc.modulus[row])));
+}
+
+int32_t hecuda_pir_databases_serialized_byte_count(const hecuda_pir_database *const *dbs, int32_t database_count,
+                                                   uint64_t *bytes) {
+    if (!bytes) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    CodecConsts cc;
+    std::vector<long long> tag;
+    int32_t rc = serialization_plan(dbs, database_count, cc, tag);
+    if (rc) return rc;
+    *bytes = (uint64_t)tag.back();
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pir_databases_serialize(const hecuda_pir_database *const *dbs, int32_t database_count, uint8_t *out,
+                                       uint64_t capacity, uint64_t *written) {
+    if (!out || !written) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *written = 0;
+    CodecConsts cc;
+    std::vector<long long> tag;
+    int32_t rc = serialization_plan(dbs, database_count, cc, tag);
+    if (rc) return rc;
+    const uint64_t size = (uint64_t)tag.back();
+    if (capacity < size)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "capacity " + std::to_string(capacity) + " below the serialized size " +
+                                                     std::to_string(size));
+    const hecuda_context *h = dbs[0]->owner;
+    const Context &c = *h->ctx;
+    const long long count = (long long)tag.size() - 1;
+    out[0] = (uint8_t)dbio::kVersion;
+    for (int k = 0; k < 4; ++k) out[1 + k] = (uint8_t)(count >> (8 * k));
+    std::vector<int64_t> counts((size_t)database_count);
+    for (int32_t t = 0; t < database_count; ++t) counts[(size_t)t] = dbs[t]->count;
+    long long widest = 0;
+    const std::vector<DbChunk> plan = plan_db_chunks(tag, counts, widest);
+    const bool pinned = host_pinned(out, (size_t)size);
+    DbStaging st(h);
+    if (!st.g0.w || !st.g1.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    const cudaStream_t *streams = st.stream;
+    long long *d_tag = nullptr;
+    cudaError_t e = cudaMalloc(&d_tag, tag.size() * sizeof(long long));
+    if (e == cudaSuccess) e = upload(d_tag, tag.data(), tag.size() * sizeof(long long));
+    if (e == cudaSuccess) e = st.init((size_t)widest, !pinned);
+    // a pageable `out`: chunk k's pinned bytes are copied out once chunk k + 1 is enqueued
+    auto drain = [&](size_t k) {
+        const dbio::Chunk &ch = plan[k].chunk;
+        const long long base = tag[(size_t)ch.first];
+        cudaError_t e2 = cudaEventSynchronize(st.copied[k & 1]);
+        if (e2 == cudaSuccess) memcpy(out + base, st.host[k & 1], (size_t)(tag[(size_t)(ch.first + ch.count)] - base));
+        return e2;
+    };
+    for (size_t k = 0; k < plan.size() && e == cudaSuccess; ++k) {
+        const int b = (int)(k & 1);
+        const dbio::Chunk &ch = plan[k].chunk;
+        const long long base = tag[(size_t)ch.first], bytes = tag[(size_t)(ch.first + ch.count)] - base;
+        const PolyLayout at{d_tag, base, ch.first, nullptr, nullptr};
+        e = resident_rows(c, dbs[plan[k].db]).with(plan[k].local, [&](const auto *rows) {
+            return launch_poly_serialize(c, cc, 0, rows, st.dev[b], ch.count, streams[b], at);
+        });
+        if (e == cudaSuccess)
+            e = cudaMemcpyAsync(pinned ? out + base : st.host[b], st.dev[b], (size_t)bytes, cudaMemcpyDeviceToHost, streams[b]);
+        if (e == cudaSuccess && !pinned) e = cudaEventRecord(st.copied[b], streams[b]);
+        if (e == cudaSuccess && !pinned && k >= 1) e = drain(k - 1);
+    }
+    if (e == cudaSuccess && !pinned && !plan.empty()) e = drain(plan.size() - 1);
+    for (int b = 0; b < 2; ++b) {
+        const cudaError_t e2 = cudaStreamSynchronize(streams[b]);
+        if (e == cudaSuccess) e = e2;
+    }
+    cudaFree(d_tag);
+    if (e != cudaSuccess) return cuda_fail(e, "pir databases serialize");
+    *written = size;
     return HECUDA_OK;
 }
 

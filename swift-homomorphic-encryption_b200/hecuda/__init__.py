@@ -102,6 +102,9 @@ SYMBOLS = {
     "hecuda_pir_database_destroy": (C.c_int32, [_VP]),
     "hecuda_pir_database_device_buffer": (C.c_int32, [_VP, C.POINTER(_VP), C.POINTER(C.c_uint64)]),
     "hecuda_pir_database_present": (C.c_int32, [_VP, _VP, C.c_int64]),
+    "hecuda_pir_databases_create_serialized": (C.c_int32, [_VP, _VP, C.c_uint64, C.c_int32, C.POINTER(_VP)]),
+    "hecuda_pir_databases_serialized_byte_count": (C.c_int32, [C.POINTER(_VP), C.c_int32, C.POINTER(C.c_uint64)]),
+    "hecuda_pir_databases_serialize": (C.c_int32, [C.POINTER(_VP), C.c_int32, _VP, C.c_uint64, C.POINTER(C.c_uint64)]),
     "hecuda_pir_process_entries": (C.c_int32, [_VP, _VP, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, C.c_int32, _VP, _VP,
                                                C.c_int64]),
     "hecuda_pir_database_create_from_entries": (C.c_int32, [_VP, _VP, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, C.c_int32,

@@ -31,7 +31,7 @@ import numpy as np
 from . import Context, EvaluationKey, SecretKey, _check, _ptr, load_library
 from . import symmetric_pir
 from .pir import IndexPirConfig, IndexPirParameter, MulPir, MulPirClient, MulPirServer, PirError, PirKeyCompressionStrategy, \
-    PirWire, ProcessedDatabase, ShardValidationResult, _validate, bytesPerPlaintext
+    PirWire, ProcessedDatabase, ShardValidationResult, _save_databases, _validate, bytesPerPlaintext
 from .symmetric_pir import SymmetricPirClientConfig, SymmetricPirConfig
 
 MAX_SLOT_COUNT = 255  # HashBucket.maxSlotCount
@@ -387,13 +387,28 @@ class ProcessedKeywordDatabase:
     databases: List[ProcessedDatabase]
     pirParameter: IndexPirParameter
     keywordPirParameter: KeywordPirParameter
-    table: CuckooTable
+    table: Optional[CuckooTable]  # None for a database loaded from its serialization
     symmetricPirConfig: Optional[SymmetricPirConfig] = None  # as ProcessedDatabaseWithParameters keeps it
+
+    def save(self, path) -> None:
+        """The shard's ProcessedDatabase.save(to:) (KeywordPirProtocol.swift:230-239): the tables' plaintexts
+        concatenated in table order, serialized on the device."""
+        _save_databases(self.databases, path)
+
+    @staticmethod
+    def load(path, context: Context, pirParameter: IndexPirParameter, keywordPirParameter: KeywordPirParameter,
+             symmetricPirConfig: Optional[SymmetricPirConfig] = None) -> "ProcessedKeywordDatabase":
+        """A saved shard (ProcessedDatabase(from:context:)) cut into hashFunctionCount tables as
+        KeywordPirServer.init(context:processed:) does (KeywordPirProtocol.swift:161-171), without its cuckoo table.
+        The parameters are the caller's: the reference keeps them in a separate protobuf file."""
+        databases = ProcessedDatabase.load(context, path, keywordPirParameter.hashFunctionCount)
+        return ProcessedKeywordDatabase(databases, pirParameter, keywordPirParameter, None, symmetricPirConfig)
 
     def close(self):
         for db in self.databases:
             db.close()
-        self.table.close()
+        if self.table is not None:
+            self.table.close()
 
 
 class KeywordPirClient:

@@ -19,6 +19,7 @@ plaintext polynomials runs in libhecuda.
 from __future__ import annotations
 
 import ctypes as C
+import os
 import time
 from dataclasses import dataclass, field
 from enum import Enum
@@ -278,6 +279,35 @@ class ProcessedDatabase:
         _check(load_library().hecuda_pir_database_present(self._h, _ptr(out), self.count))
         return out
 
+    def serializationByteCount(self) -> int:
+        """ProcessedDatabase.serializationByteCount() (IndexPirProtocol.swift:336-348); HeError("emptyDatabase") when
+        every plaintext is nil."""
+        return _serialized_byte_count([self])
+
+    def serialize(self) -> bytes:
+        """ProcessedDatabase.serialize() (IndexPirProtocol.swift:360-378), packed on the device: the version byte, the
+        little-endian UInt32 plaintext count, then per plaintext a tag (0 nil, 1 present) and its Eval rows."""
+        return _serialize_databases([self]).tobytes()
+
+    def save(self, path) -> None:
+        """ProcessedDatabase.save(to:) (IndexPirProtocol.swift:350-355), written straight into the file's pages."""
+        _save_databases([self], path)
+
+    @staticmethod
+    def load(context: Context, source, tableCount: int = 1) -> List["ProcessedDatabase"]:
+        """ProcessedDatabase(from:context:) (IndexPirProtocol.swift:286-334) unpacked on the device, cut into
+        `tableCount` databases of equal size (1 for index PIR; hashFunctionCount for a keyword-PIR shard,
+        KeywordPirProtocol.swift:161-171).  source: bytes, a uint8 array, or a path, which is read through np.memmap so
+        that a file larger than a host buffer streams.  Raises HeError with the reference's error name when the bytes are
+        refused, and also where the reference would accept a residue >= its modulus or trap on a truncated buffer."""
+        data = _source_bytes(source)
+        handles = (C.c_void_p * max(1, tableCount))()
+        buffer = data if data.size else np.zeros(1, dtype=np.uint8)  # an empty source still has an address
+        _check(load_library().hecuda_pir_databases_create_serialized(context._h, _ptr(buffer), data.size, tableCount,
+                                                                     handles))
+        count = int.from_bytes(data[1:5].tobytes(), "little") // tableCount
+        return [ProcessedDatabase._adopt(context, C.c_void_p(h), count) for h in handles[:tableCount]]
+
     def close(self):
         if getattr(self, "_h", None) is not None:
             load_library().hecuda_pir_database_destroy(self._h)
@@ -288,6 +318,49 @@ class ProcessedDatabase:
             self.close()
         except Exception:
             pass
+
+
+def _source_bytes(source) -> np.ndarray:
+    """The bytes of a serialized database as a uint8 array; a path is mapped, not read."""
+    if isinstance(source, (str, os.PathLike)):
+        return np.memmap(source, dtype=np.uint8, mode="r") if os.path.getsize(source) else np.zeros(0, dtype=np.uint8)
+    if isinstance(source, (bytes, bytearray, memoryview)):
+        return np.frombuffer(source, dtype=np.uint8)
+    return np.ascontiguousarray(np.asarray(source, dtype=np.uint8)).reshape(-1)
+
+
+def _handles(databases: Sequence[ProcessedDatabase]):
+    return (C.c_void_p * len(databases))(*[db._h for db in databases])
+
+
+def _serialized_byte_count(databases: Sequence[ProcessedDatabase]) -> int:
+    size = C.c_uint64(0)
+    _check(load_library().hecuda_pir_databases_serialized_byte_count(_handles(databases), len(databases), C.byref(size)))
+    return size.value
+
+
+def _serialize_into(databases: Sequence[ProcessedDatabase], out: np.ndarray) -> None:
+    written = C.c_uint64(0)
+    _check(load_library().hecuda_pir_databases_serialize(_handles(databases), len(databases), _ptr(out), out.size,
+                                                         C.byref(written)))
+
+
+def _serialize_databases(databases: Sequence[ProcessedDatabase]) -> np.ndarray:
+    """The databases' plaintexts serialized as one ProcessedDatabase, in order (a keyword-PIR shard's layout)."""
+    out = np.empty(_serialized_byte_count(databases), dtype=np.uint8)
+    _serialize_into(databases, out)
+    return out
+
+
+def _save_databases(databases: Sequence[ProcessedDatabase], path) -> None:
+    out = np.memmap(path, dtype=np.uint8, mode="w+", shape=(_serialized_byte_count(databases),))
+    try:
+        _serialize_into(databases, out)
+        out.flush()
+    except Exception:
+        del out
+        os.remove(path)
+        raise
 
 
 def _entry_arguments(database: Sequence[bytes], parameter: IndexPirParameter):
@@ -535,6 +608,18 @@ class MulPirServer:
     @property
     def chunkCount(self) -> int:
         return -(-self.parameter.encodedEntrySize // bytesPerPlaintext(self.context))
+
+    @staticmethod
+    def load(path, parameter: IndexPirParameter, context: Context) -> "MulPirServer":
+        """A server over the processed database saved at `path` (ProcessedDatabase(from:context:),
+        IndexPirProtocol.swift:286-334); PirError("invalidDatabasePlaintextCount...") when it does not fit `parameter`."""
+        databases = ProcessedDatabase.load(context, path)
+        try:
+            return MulPirServer(parameter, context, databases)
+        except Exception:
+            for db in databases:
+                db.close()
+            raise
 
     @staticmethod
     def process(database: Sequence[bytes], context: Context, parameter: IndexPirParameter) -> ProcessedDatabase:
