@@ -113,30 +113,31 @@ def encrypt(n: int, moduli, t: int, sk, plain, a_seed: bytes, e_seed: bytes) -> 
     return translate_add(n, moduli, t, encrypt_zero(n, moduli, sk, a_seed, e_seed), plain)
 
 
-def key_switch_key(n: int, ct_moduli, q_ks: int, current_key, sk, a_seeds, e_seeds) -> np.ndarray:
+def key_switch_key(n: int, ct_moduli, q_ks: int, current_key, sk, a_seeds, e_seeds, rows=None) -> np.ndarray:
     """_generateKeySwitchKey (Bfv+Keys.swift:67-103) -> (L, 2, K, N) Eval: key ciphertext i = forwardNtt(encryptZero over
-    [q_0..q_{L-1}, q_ks]) with (q_ks mod q_i) currentKey[i] added to row i of poly0."""
+    [q_0..q_{L-1}, q_ks]) with (q_ks mod q_i) currentKey[i] added to row i of poly0.  rows: only the key ciphertexts i
+    in `rows`, in that order ((len(rows), 2, K, N)); each has its own seeds, so they equal those of the whole key."""
     ks = [int(q) for q in ct_moduli] + [int(q_ks)]
     out = []
-    for i, q in enumerate(ct_moduli):
+    for i in (range(len(ct_moduli)) if rows is None else rows):
         ct = encrypt_zero(n, ks, sk, a_seeds[i], e_seeds[i])
         ev = np.stack([O.ntt_forward(n, ks, ct[p]) for p in range(2)])
-        q = int(q)
+        q = int(ct_moduli[i])
         ev[0, i] = (ev[0, i].astype(object) + (int(q_ks) % q) * np.asarray(current_key)[i].astype(object)) % q
         out.append(ev)
     return np.stack(out)
 
 
-def generate_evaluation_key(n: int, ct_moduli, q_ks: int, sk, has_relin: bool, elements, a_seeds, e_seeds):
+def generate_evaluation_key(n: int, ct_moduli, q_ks: int, sk, has_relin: bool, elements, a_seeds, e_seeds, rows=None):
     """Bfv.generateEvaluationKey (Bfv+Keys.swift:30-65) with seeds in hecuda_evk_generate's order (the relinearization
-    key, then the elements, L per key) -> (relinearization key or None, {element: key})."""
+    key, then the elements, L per key) -> (relinearization key or None, {element: key}); rows as in key_switch_key."""
     L = len(ct_moduli)
     ks = [int(q) for q in ct_moduli] + [int(q_ks)]
     sk = np.asarray(sk)
     keys, used = [], 0
     currents = ([_mul(sk, sk, ks)] if has_relin else []) + [O.galois_eval(n, L + 1, g, sk) for g in elements]
     for current in currents:
-        keys.append(key_switch_key(n, ct_moduli, q_ks, current, sk, a_seeds[used:used + L], e_seeds[used:used + L]))
+        keys.append(key_switch_key(n, ct_moduli, q_ks, current, sk, a_seeds[used:used + L], e_seeds[used:used + L], rows))
         used += L
     relin = keys.pop(0) if has_relin else None
     return relin, dict(zip(elements, keys))

@@ -247,8 +247,18 @@ def _negacyclic_at(a, b, k: int) -> int:
 def tensor_at(q, lhs_ct, rhs_ct, coeffs, word_bits: int = 64) -> list[list[int]]:
     """The tensor product D = lift(lhs_ct) (x) lift(rhs_ct) of one (2, L, N) ciphertext pair, as integers, at `coeffs`:
     [[D0[k] for k in coeffs], [D1[k] ...], [D2[k] ...]]."""
-    y = [np.array([lift_value(v, q, word_bits) for v in _crt(lhs_ct[p], q)], dtype=object) for p in range(2)]
-    z = [np.array([lift_value(v, q, word_bits) for v in _crt(rhs_ct[p], q)], dtype=object) for p in range(2)]
+    lifts = {}  # aligned operands hold two values per polynomial: lift each distinct value once
+
+    def lift(res):
+        out = []
+        for v in _crt(res, q):
+            if v not in lifts:
+                lifts[v] = lift_value(v, q, word_bits)
+            out.append(lifts[v])
+        return np.array(out, dtype=object)
+
+    y = [lift(lhs_ct[p]) for p in range(2)]
+    z = [lift(rhs_ct[p]) for p in range(2)]
     return [[_negacyclic_at(y[0], z[0], k) for k in coeffs],
             [_negacyclic_at(y[0], z[1], k) + _negacyclic_at(y[1], z[0], k) for k in coeffs],
             [_negacyclic_at(y[1], z[1], k) for k in coeffs]]

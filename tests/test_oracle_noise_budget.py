@@ -63,3 +63,21 @@ def test_secret_key_is_ternary(params):
     for i, q in enumerate(moduli):
         assert set(int(v) for v in coeff[i]) <= {0, 1, int(q) - 1}
     assert np.array_equal(coeff[0] == 0, coeff[2] == 0)
+
+
+def test_evaluation_key_rows_are_those_of_the_whole_key():
+    """generate_evaluation_key(rows=...) computes only some key ciphertexts; each has its own seeds, so they are the
+    same rows of the whole key."""
+    n = 64
+    moduli = orc.generate_primes([40, 40, 41], False, n)
+    L = len(moduli) - 1
+    sk = co.generate_secret_key(n, moduli, bytes(range(32)))
+    a = [bytes([i]) * 32 for i in range(3 * L)]
+    e = [bytes([100 + i]) * 32 for i in range(3 * L)]
+    relin, galois = co.generate_evaluation_key(n, moduli[:L], moduli[L], sk, True, [3, 2 * n - 1], a, e)
+    for rows in ([1], [L - 1, 0]):
+        part_relin, part_galois = co.generate_evaluation_key(n, moduli[:L], moduli[L], sk, True, [3, 2 * n - 1], a, e,
+                                                             rows)
+        assert np.array_equal(part_relin, relin[rows])
+        for el in (3, 2 * n - 1):
+            assert np.array_equal(part_galois[el], galois[el][rows])
