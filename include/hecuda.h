@@ -483,6 +483,36 @@ int32_t hecuda_oprf_blind_evaluate(const uint8_t *secret_key, const uint8_t *bli
                                    int64_t count, const uint8_t *seed /* 32 */,
                                    uint8_t *responses /* count x 145 */, uint8_t *status /* count: 0 ok, 1 invalid */);
 
+/* ---- The OPRF client: OprfClient (SymmetricPir/SymmetricPirProtocol.swift:62-133), one device thread per query ----
+ * swift-crypto's P384._VOPRF.PublicKey.blind and .finalize (RFC 9497 3.3.2 Blind and Finalize, with 2.2.2 VerifyProof
+ * over one element), and the AES-GCM-192 open of a retrieved entry.  Blinds are 48 big-endian bytes r with 0 < r < n,
+ * drawn by the caller.  These calls need no context.  Refused with HECUDA_ERR_INVALID_ARGUMENT and no kernel launched:
+ * null pointers, a negative count, decreasing offsets and an OPRF input over 65535 bytes.  A count of 0 launches nothing
+ * once the arguments pass.  The device copies of the blinds, the OPRF outputs and the opened values are zeroized before
+ * they are freed. */
+/* queryContext(at:) (:98-104): queries[i] = SerializeElement(r_i HashToGroup(input_i)) and status[i] = 0, or 49 zero
+ * bytes and status[i] = 1 when r_i is not in [1, n - 1]. */
+int32_t hecuda_oprf_blind(const uint8_t *inputs, const uint64_t *offsets, int64_t count,
+                          const uint8_t *blinds /* count x 48 */, uint8_t *queries /* count x 49 */,
+                          uint8_t *status /* count */);
+/* parse(oprfResponse:with:) (:106-117), RFC 9497 VOPRF Finalize of each query: verify the response's proof against the
+ * server's public key and the query, unblind the evaluated element D as N = r^-1 D, and outputs[i] = SHA-384(I2OSP(len,
+ * 2) || input || I2OSP(49, 2) || Ser(N) || "Finalize").  status[i]: 0 verified and written; 1 response rejected (D not
+ * a valid encoding, c >= n or s >= n, or the challenge does not match); 2 context invalid (the blind not in [1, n - 1]
+ * or the query not a valid encoding).  A non-zero status writes 48 zero bytes.  A public key that is not a valid
+ * SEC1-compressed point is refused with HECUDA_ERR_INVALID_ARGUMENT. */
+int32_t hecuda_oprf_finalize(const uint8_t *public_key /* 49 */, const uint8_t *inputs, const uint64_t *offsets,
+                             int64_t count, const uint8_t *blinds /* count x 48 */, const uint8_t *queries /* count x 49 */,
+                             const uint8_t *responses /* count x 145 */, uint8_t *outputs /* count x 48 */,
+                             uint8_t *status /* count */);
+/* decrypt(encryptedEntry:with:) (:119-132): entry i is sealed[sealed_offsets[i] : sealed_offsets[i + 1]], ciphertext ||
+ * 16-byte tag, opened with AES.GCM.open under key h[24:48] and nonce h[0:12] of oprf_outputs[i].  values has the layout
+ * of sealed (sealed_offsets[count] bytes): entry i's plaintext at values[sealed_offsets[i] : sealed_offsets[i + 1] - 16]
+ * and zeros in its last 16 bytes, status[i] = 0.  When the tag does not match, or the entry is shorter than 16 bytes,
+ * status[i] = 1 and all of entry i's bytes in values are zero; no unauthenticated plaintext is written. */
+int32_t hecuda_symmetric_pir_open(const uint8_t *oprf_outputs /* count x 48 */, const uint8_t *sealed,
+                                  const uint64_t *sealed_offsets, int64_t count, uint8_t *values, uint8_t *status);
+
 /* ---- SimplePIR: Sources/PrivateInformationRetrieval/SimplePir/ ----
  * SimplePirServer<Scalar> with Scalar = UInt32 (word_bits 32) or UInt64 (word_bits 64): requests, responses, the hint and
  * the processed database cross the boundary as little-endian words of that width.  These calls need no context; the

@@ -100,5 +100,47 @@ HE_HD void seal(const u32w *rk, const u32w *te0, const unsigned char *sbox, cons
     }
 }
 
+// AES.GCM.open(ciphertext || tag, key, nonce) without associated data: in = ciphertext (len bytes), tag = the 16
+// received bytes.  The tag is recomputed over the ciphertext and compared with every byte read (no early exit); only
+// then is the ciphertext decrypted, with seal's counter blocks, and out gets the plaintext if the tags match and len
+// zero bytes if not.  Returns whether they matched.
+HE_HD bool open(const u32w *rk, const u32w *te0, const unsigned char *sbox, const unsigned char nonce[12],
+                const unsigned char *in, long long len, const unsigned char tag[16], unsigned char *out) {
+    u32w blk[4] = {0, 0, 0, 0};
+    encrypt_block(blk, rk, kRounds192, te0, sbox);
+    const u64 hh = ((u64)blk[0] << 32) | blk[1], hl = ((u64)blk[2] << 32) | blk[3];  // H = E(0^128)
+    const u32w n0 = ((u32w)nonce[0] << 24) | ((u32w)nonce[1] << 16) | ((u32w)nonce[2] << 8) | nonce[3];
+    const u32w n1 = ((u32w)nonce[4] << 24) | ((u32w)nonce[5] << 16) | ((u32w)nonce[6] << 8) | nonce[7];
+    const u32w n2 = ((u32w)nonce[8] << 24) | ((u32w)nonce[9] << 16) | ((u32w)nonce[10] << 8) | nonce[11];
+    u64 sh = 0, sl = 0;  // GHASH state
+    for (long long at = 0; at < len; at += 16) {
+        unsigned char c[16];
+        const int take = len - at < 16 ? (int)(len - at) : 16;
+        for (int j = 0; j < 16; ++j) c[j] = j < take ? in[at + j] : 0;  // zero-padded
+        sh ^= load_be64(c), sl ^= load_be64(c + 8);
+        gf_mul(sh, sl, hh, hl);
+    }
+    sl ^= (u64)len * 8;
+    gf_mul(sh, sl, hh, hl);
+    u32w j0[4] = {n0, n1, n2, 1};
+    encrypt_block(j0, rk, kRounds192, te0, sbox);
+    unsigned diff = 0;
+    for (int j = 0; j < 16; ++j) {
+        const u64 s = j < 8 ? sh >> (56 - 8 * j) : sl >> (56 - 8 * (j - 8));
+        diff |= (unsigned char)(s ^ (j0[j >> 2] >> (24 - 8 * (j & 3)))) ^ tag[j];
+    }
+    const bool ok = diff == 0;
+    const unsigned char keep = (unsigned char)(0 - (unsigned)ok);
+    u32w counter = 1;
+    for (long long at = 0; at < len; at += 16) {
+        ++counter;
+        u32w ks[4] = {n0, n1, n2, counter};
+        encrypt_block(ks, rk, kRounds192, te0, sbox);
+        const int take = len - at < 16 ? (int)(len - at) : 16;
+        for (int j = 0; j < take; ++j) out[at + j] = (unsigned char)((in[at + j] ^ (ks[j >> 2] >> (24 - 8 * (j & 3)))) & keep);
+    }
+    return ok;
+}
+
 }  // namespace gcm
 }  // namespace hecuda

@@ -1,5 +1,6 @@
 // p384.cuh -- the P-384 field and group (SEC 2, FIPS 186-5) as __host__ __device__ functions, for symmetric_pir.cu's
-// OPRF evaluation and OPRF server; tests/emu replays them against oracle/oprf_oracle.py.
+// OPRF evaluation and OPRF server and oprf_client.cu's OPRF client; tests/emu replays them against
+// oracle/oprf_oracle.py.
 //
 //   Field   12 x 32-bit little-endian limbs in Montgomery form, R = 2^384.  p = 2^384 - 2^128 - 2^96 + 2^32 - 1 is
 //           -1 mod 2^32, so the per-word Montgomery factor -p^-1 mod 2^32 is 1 and each reduction step's multiplier
@@ -14,7 +15,8 @@
 //           addition per digit.  scalar_mul indexes the table directly, for the key every thread shares (recoded
 //           once on the host) and for public scalars; scalar_mul_ct reads it without secret-dependent addresses or
 //           branches, for a secret scalar of one thread.
-//   VOPRF   RFC 9497 BlindEvaluate with the DLEQ proof over one element (blind_evaluate_composite, generate_proof).
+//   VOPRF   RFC 9497 BlindEvaluate with the DLEQ proof over one element (blind_evaluate_composite, generate_proof),
+//           and the client's Blind, VerifyProof and Finalize (blind, verify_proof, unblind_finalize).
 #pragma once
 #include <cstdint>
 
@@ -75,10 +77,14 @@ struct Point {
     X(kSqrtExp, 0x40000000u, 0x00000000u, 0xc0000000u, 0xbfffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu,             \
       0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0x3fffffffu)                                                 \
     X(kNR2, 0x19b409a9u, 0x2d319b24u, 0xdf1aa419u, 0xff3d81e5u, 0xfcb82947u, 0xbc3e483au, 0x4aab1cc5u, 0xd40d4917u,    \
-      0x28266895u, 0x3fb05b7au, 0x2b39bf21u, 0x0c84ee01u)
+      0x28266895u, 0x3fb05b7au, 0x2b39bf21u, 0x0c84ee01u)                                                              \
+    X(kNOne, 0x333ad68du, 0x1313e695u, 0xb74f5885u, 0xa7e5f24du, 0x0bc8d220u, 0x389cb27eu, 0x00000000u, 0x00000000u,   \
+      0x00000000u, 0x00000000u, 0x00000000u, 0x00000000u)                                                              \
+    X(kNMinus2, 0xccc52971u, 0xecec196au, 0x48b0a77au, 0x581a0db2u, 0xf4372ddfu, 0xc7634d81u, 0xffffffffu,             \
+      0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu)
 // p and n are plain integers; kOne .. kGy are in Montgomery form (x R mod p): R, R^2, R^3, b, a = -3, Z = -12,
 // sqrt(-Z) = sqrt(12) and the generator; kPMinus2, kSqrtRatioC1 = (p - 3) / 4 and kSqrtExp = (p + 1) / 4 are
-// exponents; kNR2 = R^2 mod n.
+// exponents; kNR2 = R^2 mod n and kNOne = R mod n; kNMinus2 = n - 2 is an exponent.
 
 #ifdef __CUDACC__
 #define HECUDA_P384_DEVICE(name, ...) static __constant__ Fe name##Device = {{__VA_ARGS__}};
@@ -98,13 +104,16 @@ HECUDA_P384_CONSTANTS(HECUDA_P384_HOST)
 // ---------------------------------------------------------------- field and scalars
 // The two moduli share one Montgomery code: ModP for the field, ModN for scalars mod the group order.  kM0 is the
 // per-word factor -m^-1 mod 2^32; it is 1 for p, so p's reduction step multiplies by the low word itself.
+// one() is R mod m, the Montgomery form of 1.
 struct ModP {
     static constexpr uint32_t kM0 = 1;
     P384_HD static const Fe &m() { return P384_CONST(kP); }
+    P384_HD static const Fe &one() { return P384_CONST(kOne); }
 };
 struct ModN {
     static constexpr uint32_t kM0 = 0xe88fdc45u;
     P384_HD static const Fe &m() { return P384_CONST(kN); }
+    P384_HD static const Fe &one() { return P384_CONST(kNOne); }
 };
 
 // r = t - m if t (with carry word `top`) >= m, else t
@@ -218,19 +227,22 @@ P384_HD void from_mont(Fe &r, const Fe &a) {
     mul(r, a, one);
 }
 
-// a^e for a public exponent e (a plain integer), by fixed 4-bit windows
+// a^e mod m for a in Montgomery form and a public exponent e (a plain integer), by fixed 4-bit windows.  Only the
+// exponent's digits choose a branch or a table entry, so a may be secret.
+template <class M>
 P384_HD void pow_fixed(Fe &r, const Fe &a, const Fe &e) {
     Fe table[16];
-    table[0] = P384_CONST(kOne);
+    table[0] = M::one();
     table[1] = a;
-    for (int i = 2; i < 16; ++i) mul(table[i], table[i - 1], a);
-    r = P384_CONST(kOne);
+    for (int i = 2; i < 16; ++i) mul<M>(table[i], table[i - 1], a);
+    r = M::one();
     for (int w = kDigits - 1; w >= 0; --w) {
-        for (int s = 0; s < 4; ++s) sqr(r, r);
+        for (int s = 0; s < 4; ++s) mul<M>(r, r, r);
         const uint32_t nibble = (e.v[w >> 3] >> (4 * (w & 7))) & 15;
-        if (nibble) mul(r, r, table[nibble]);
+        if (nibble) mul<M>(r, r, table[nibble]);
     }
 }
+P384_HD void pow_fixed(Fe &r, const Fe &a, const Fe &e) { pow_fixed<ModP>(r, a, e); }
 
 P384_HD void inv(Fe &r, const Fe &a) { pow_fixed(r, a, P384_CONST(kPMinus2)); }
 
@@ -306,6 +318,16 @@ P384_HD void mul_mod_n(Fe &r, const Fe &a, const Fe &b) {
     Fe t;
     mul<ModN>(t, a, P384_CONST(kNR2));
     mul<ModN>(r, t, b);
+}
+
+// a^-1 mod n for a plain a in [1, n - 1] (0 for a = 0), as a^(n - 2) (Fermat) in Montgomery form: a R -> a^-1 R -> a^-1.
+// a may be secret: pow_fixed branches on the public exponent only.
+P384_HD void inv_mod_n(Fe &r, const Fe &a) {
+    Fe am, t, one = {};
+    one.v[0] = 1;
+    mul<ModN>(am, a, P384_CONST(kNR2));
+    pow_fixed<ModN>(t, am, P384_CONST(kNMinus2));
+    mul<ModN>(r, t, one);
 }
 
 // a < b for plain integers, without a branch
@@ -634,15 +656,9 @@ P384_HD void generator(Point &g) {
     g.x = P384_CONST(kGx), g.y = P384_CONST(kGy), g.z = P384_CONST(kOne);
 }
 
-// RFC 9497 Evaluate's output for one input: SHA-384(I2OSP(len, 2) || input || I2OSP(49, 2) || k HashToGroup(input) ||
-// "Finalize"); len < 2^16
-P384_HD void oprf_evaluate(unsigned char out[kOutputBytes], const signed char *digits, const unsigned char *input,
-                           long long len) {
-    Point e, z;
-    hash_to_group(e, input, len);
-    scalar_mul(z, e, digits);
-    unsigned char issued[kElementBytes];
-    compress(issued, z);
+// RFC 9497 Finalize's hash: SHA-384(I2OSP(len, 2) || input || I2OSP(49, 2) || issued || "Finalize"); len < 2^16
+P384_HD void finalize_hash(unsigned char out[kOutputBytes], const unsigned char *input, long long len,
+                           const unsigned char issued[kElementBytes]) {
     sha512::Sha384 s;
     s.init();
     s.byte((uint32_t)(len >> 8)), s.byte((uint32_t)len);
@@ -651,6 +667,17 @@ P384_HD void oprf_evaluate(unsigned char out[kOutputBytes], const signed char *d
     s.bytes(issued, kElementBytes);
     s.bytes((const unsigned char *)"Finalize", 8);
     s.finish(out);
+}
+
+// RFC 9497 Evaluate's output for one input: finalize_hash of Ser(k HashToGroup(input))
+P384_HD void oprf_evaluate(unsigned char out[kOutputBytes], const signed char *digits, const unsigned char *input,
+                           long long len) {
+    Point e, z;
+    hash_to_group(e, input, len);
+    scalar_mul(z, e, digits);
+    unsigned char issued[kElementBytes];
+    compress(issued, z);
+    finalize_hash(out, input, len, issued);
 }
 
 // ---------------------------------------------------------------- VOPRF BlindEvaluate with the DLEQ proof
@@ -778,6 +805,90 @@ P384_HD void generate_proof(unsigned char proof[kProofBytes], const signed char 
     sub<ModN>(ck, r, ck);
     to_bytes(proof, c);
     to_bytes(proof + kScalarBytes, ck);
+}
+
+// ---------------------------------------------------------------- VOPRF client: Blind, VerifyProof, Finalize
+// RFC 9497 3.3.2 for one element, as swift-crypto's P384._VOPRF.PublicKey.blind and .finalize run it.  The blind r is
+// the client's secret, so r B and r^-1 D go through scalar_mul_ct and r^-1 through inv_mod_n; the proof's scalars and
+// every point of the verification are public, so VerifyProof uses scalar_mul.
+
+// Blind: query = Ser(r HashToGroup(input)) for a plain r in [1, n - 1]
+P384_HD void blind(unsigned char query[kElementBytes], const Fe &r, const unsigned char *input, long long len) {
+    Point e, b;
+    hash_to_group(e, input, len);
+    signed char digits[kDigits + 1];
+    recode_scalar(r, digits);
+    scalar_mul_ct(b, e, digits);
+    compress(query, b);
+}
+
+// The challenge's element: I2OSP(49, 2) || Ser(p)
+P384_HD void absorb_element(sha512::Sha384 &s, const Point &p) {
+    unsigned char e[kElementBytes];
+    compress(e, p);
+    i2osp2(s, kElementBytes);
+    s.bytes(e, kElementBytes);
+}
+
+// VerifyProof (2.2.2) over one element with ComputeComposites: pk_ser = Ser(pkS) and seed = composite_seed(pk_ser) are
+// per key, B and D the decoded query and evaluated element, their encodings `blinded` and `evaluated`, and proof = c ||
+// s.  c, s < n; d0 = composite_scalar(seed, Ser(B), Ser(D)); M = d0 B and Z = d0 D; t2 = s G + c pkS and t3 = s M + c Z;
+// true when HashToScalar(Ser(pkS), Ser(M), Z, t2, t3 framed || "Challenge") is c.  The six products run through one
+// scalar_mul in a loop, so a kernel holds one copy of the ladder.
+P384_HD bool verify_proof(const Point &pk, const unsigned char pk_ser[kElementBytes],
+                          const unsigned char seed[kSeedBytes], const Point &b, const unsigned char blinded[kElementBytes],
+                          const Point &d, const unsigned char evaluated[kElementBytes],
+                          const unsigned char proof[kProofBytes]) {
+    Fe c, s, d0;
+    from_bytes(c, proof);
+    from_bytes(s, proof + kScalarBytes);
+    if (!less_than(c, P384_CONST(kN)) || !less_than(s, P384_CONST(kN))) return false;
+    composite_scalar(d0, seed, blinded, evaluated);
+    // products: M = d0 B, Z = d0 D, s G, c pkS, s M, c Z
+    Point base[6], prod[6];
+    Fe k[6] = {d0, d0, s, c, s, c};
+    base[0] = b, base[1] = d;
+    generator(base[2]);
+    base[3] = pk;
+#ifdef __CUDA_ARCH__
+#pragma unroll 1
+#endif
+    for (int j = 0; j < 6; ++j) {
+        if (j == 4) base[4] = prod[0], base[5] = prod[1];
+        signed char digits[kDigits + 1];
+        recode_scalar(k[j], digits);
+        scalar_mul(prod[j], base[j], digits);
+    }
+    Point t2, t3;
+    add(t2, prod[2], prod[3]);
+    add(t3, prod[4], prod[5]);
+    sha512::Sha384 h;
+    xmd_begin(h);
+    i2osp2(h, kElementBytes);
+    h.bytes(pk_ser, kElementBytes);
+    const Point *framed[4] = {&prod[0], &prod[1], &t2, &t3};
+#ifdef __CUDA_ARCH__
+#pragma unroll 1
+#endif
+    for (int j = 0; j < 4; ++j) absorb_element(h, *framed[j]);
+    h.bytes((const unsigned char *)"Challenge", 9);
+    Fe expected;
+    hash_to_scalar_finish(expected, h);
+    return equal(expected, c);
+}
+
+// Finalize after a verified proof: N = r^-1 D for the plain blind r in [1, n - 1], then finalize_hash(input, Ser(N))
+P384_HD void unblind_finalize(unsigned char out[kOutputBytes], const Fe &r, const Point &d, const unsigned char *input,
+                              long long len) {
+    Fe ri;
+    inv_mod_n(ri, r);
+    signed char digits[kDigits + 1];
+    recode_scalar(ri, digits);
+    Point u;
+    scalar_mul_ct(u, d, digits);
+    unsigned char issued[kElementBytes];
+    compress(issued, u);
+    finalize_hash(out, input, len, issued);
 }
 
 #undef P384_CONST

@@ -23,16 +23,17 @@
 
 #include "aes_gcm.cuh"
 #include "capi_internal.hpp"
+#include "oprf_host.hpp"
 #include "p384.cuh"
 
 using namespace hecuda;
 using namespace hecuda::api;
+using namespace hecuda::api::oprf_host;
 
 namespace {
 
 constexpr int kThreads = 128;
 constexpr int kRecodingBytes = p384::kDigits + 1;  // 96 digits, then the flip flag
-constexpr long long kMaxInputBytes = 65535;         // I2OSP(len(input), 2)
 constexpr int kKeywordBytes = 16, kNonceBytes = 12, kAesKeyOffset = 24, kTagBytes = 16;
 
 __constant__ unsigned char c_sbox[256];
@@ -212,11 +213,6 @@ cudaError_t upload_aes_tables() {
     return e == cudaSuccess ? cudaMemcpyToSymbol(c_te0, te0, sizeof(te0)) : e;
 }
 
-void wipe(void *p, size_t bytes) {  // a host copy of key material
-    volatile unsigned char *q = (volatile unsigned char *)p;
-    for (size_t i = 0; i < bytes; ++i) q[i] = 0;
-}
-
 // The key as OprfPrivateKey(rawRepresentation:) takes it: 48 big-endian bytes, 0 < k < n; recoded into `recoding`
 int32_t recode_key(const uint8_t *secret_key, signed char recoding[kRecodingBytes]) {
     if (!secret_key) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null OPRF secret key");
@@ -226,39 +222,6 @@ int32_t recode_key(const uint8_t *secret_key, signed char recoding[kRecodingByte
     if (valid) p384::recode_scalar(k, recoding);
     wipe(&k, sizeof(k));
     return valid ? HECUDA_OK : fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid OPRF secret key: not in [1, n - 1] for P-384");
-}
-
-// offsets[0..count] must not decrease; `longest` gets the longest row
-int32_t check_rows(const uint64_t *offsets, int64_t count, const char *what, uint64_t &longest) {
-    longest = 0;
-    for (int64_t i = 0; i < count; ++i) {
-        if (offsets[i + 1] < offsets[i]) return fail(HECUDA_ERR_INVALID_ARGUMENT, std::string(what) + " offsets must not decrease");
-        longest = std::max<uint64_t>(longest, offsets[i + 1] - offsets[i]);
-    }
-    return HECUDA_OK;
-}
-
-int32_t check_inputs(const uint8_t *inputs, const uint64_t *offsets, int64_t count, const char *what) {
-    if (!inputs || !offsets || count < 0) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument / negative count");
-    uint64_t longest = 0;
-    const int32_t rc = check_rows(offsets, count, what, longest);
-    if (rc) return rc;
-    if (longest > (uint64_t)kMaxInputBytes)
-        return fail(HECUDA_ERR_INVALID_ARGUMENT, std::string(what) + " longer than 65535 bytes (OPRF inputs carry a 2-byte length)");
-    return HECUDA_OK;
-}
-
-int32_t have_device() {
-    int dev = -1;
-    if (cudaGetDevice(&dev) != cudaSuccess) return fail(HECUDA_ERR_NO_DEVICE, "no CUDA device: libhecuda has no CPU fallback");
-    return HECUDA_OK;
-}
-
-template <class T>
-cudaError_t upload_new(T **dst, const void *src, size_t bytes) {
-    cudaError_t e = cudaMalloc(dst, std::max<size_t>(bytes, 1));
-    if (e == cudaSuccess && bytes) e = upload(*dst, src, bytes);
-    return e;
 }
 
 // Device buffers of one call; the key's recoding and plain copy and the OPRF outputs are zeroized before they are freed.

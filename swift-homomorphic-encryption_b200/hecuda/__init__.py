@@ -121,6 +121,9 @@ SYMBOLS = {
     "hecuda_oprf_evaluate": (C.c_int32, [_VP, _VP, _VP, C.c_int64, _VP]),
     "hecuda_symmetric_pir_process": (C.c_int32, [_VP, _VP, _VP, _VP, _VP, C.c_int64, _VP, _VP]),
     "hecuda_oprf_blind_evaluate": (C.c_int32, [_VP, _VP, C.c_int64, _VP, _VP, _VP]),
+    "hecuda_oprf_blind": (C.c_int32, [_VP, _VP, C.c_int64, _VP, _VP, _VP]),
+    "hecuda_oprf_finalize": (C.c_int32, [_VP, _VP, _VP, C.c_int64, _VP, _VP, _VP, _VP, _VP]),
+    "hecuda_symmetric_pir_open": (C.c_int32, [_VP, _VP, _VP, C.c_int64, _VP, _VP]),
     "hecuda_simple_pir_process": (C.c_int32, [_VP, C.c_int64, _VP, _VP, _VP, C.POINTER(_VP)]),
     "hecuda_simple_pir_database_create": (C.c_int32, [_VP, _VP, C.POINTER(_VP)]),
     "hecuda_simple_pir_database_export": (C.c_int32, [_VP, _VP]),

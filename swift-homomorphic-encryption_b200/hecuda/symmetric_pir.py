@@ -5,9 +5,12 @@ Names follow Sources/PrivateInformationRetrieval/SymmetricPir/SymmetricPirDataba
     SymmetricPirConfigType, SymmetricPirClientConfig, SymmetricPirConfig   :21-184
     KeywordDatabase.symmetricPIRProcess                                    :186-211 (hecuda.keyword_pir)
     OprfServer                        SymmetricPir/SymmetricPirProtocol.swift:39-59
+    OprfClient, ParsedOprfOutput      SymmetricPir/SymmetricPirProtocol.swift:62-133
+    OprfQueryContext (.query)         SymmetricPir/SymmetricPirProtocol.swift:20-36
 
 The OPRF is RFC 9497 in VOPRF mode over P384-SHA384 (swift-crypto's P384._VOPRF), evaluated on the device one thread
-per row; the rows' AES-GCM-192 sealing runs there too, and so do the server's answers to clients' blinded queries.
+per row; the rows' AES-GCM-192 sealing runs there too, and so do the server's answers to clients' blinded queries and
+the client's blinding, proof verification, finalization and opening of retrieved entries.
 """
 from __future__ import annotations
 
@@ -23,6 +26,8 @@ from .pir import PirError
 
 OPRF_KEY_BYTES, OPRF_ELEMENT_BYTES, OPRF_OUTPUT_BYTES = 48, 49, 48  # HECUDA_OPRF_*
 OPRF_RESPONSE_BYTES, OPRF_SEED_BYTES = 145, 32
+# the order n of P-384's group: blinds are drawn from [1, n - 1]
+P384_ORDER = 0xffffffffffffffffffffffffffffffffffffffffffffffffc7634d81f4372ddf581a0db248b0a77aecec196accc52973
 
 
 def _concatenate(blobs: Sequence[bytes]):
@@ -173,3 +178,139 @@ class OprfServer:
             if status[j] == 0:
                 out[i] = responses[j].tobytes()
         return out
+
+
+@dataclass(frozen=True, repr=False)
+class OprfQueryContext:
+    """OprfQueryContext (swift-crypto's P384._VOPRF.BlindedInput): the keyword, its secret blind r and the query
+    Ser(r HashToGroup(keyword)) to send to the server (the `query` extension, SymmetricPirProtocol.swift:31-36).  repr
+    never shows the blind."""
+
+    keyword: bytes
+    blind: int
+    query: bytes
+
+    def __repr__(self) -> str:
+        return f"OprfQueryContext(keyword: {self.keyword!r}, blind: ****, query: {self.query.hex()})"
+
+
+@dataclass(frozen=True, repr=False)
+class ParsedOprfOutput:
+    """OprfClient.ParsedOprfOutput (:64-82): the finalized OPRF output split into the oblivious keyword (its first 16
+    bytes), the entry's nonce (its first 12) and the entry's AES key (its last 24).  repr never shows the key."""
+
+    obliviousKeyword: bytes
+    nonce: bytes
+    secretKey: bytes
+
+    @classmethod
+    def fromOprfOutput(cls, oprfOutput: bytes, configType: SymmetricPirConfigType) -> "ParsedOprfOutput":
+        oprfOutput = bytes(oprfOutput)
+        return cls(oprfOutput[:configType.obliviousKeywordSize], oprfOutput[:configType.nonceSize],
+                   oprfOutput[len(oprfOutput) - configType.entryEncryptionKeySize:])
+
+    def __repr__(self) -> str:
+        return f"ParsedOprfOutput(obliviousKeyword: {self.obliviousKeyword.hex()}, nonce: {self.nonce.hex()}, secretKey: ****)"
+
+
+class OprfClient:
+    """OprfClient (SymmetricPirProtocol.swift:62-133) on the device: blinding, the server's proof check, unblinding and
+    finalization, and the AES-GCM open of retrieved entries, each one device call for a whole list."""
+
+    def __init__(self, symmetricPirClientConfig: SymmetricPirClientConfig):
+        config = symmetricPirClientConfig
+        if config.configType is not SymmetricPirConfigType.OPRF_P384_AES_GCM_192_NONCE_96_TAG_128:
+            raise PirError(f"invalidSymmetricPirConfig(symmetricPirConfig: {config})")
+        key = bytes(config.serverPublicKey)
+        if len(key) != OPRF_ELEMENT_BYTES:
+            raise PirError(f"invalid OPRF public key: {len(key)} bytes, expected {OPRF_ELEMENT_BYTES}")
+        self._publicKey = np.frombuffer(key, dtype=np.uint8)
+        self.configType = config.configType
+        lib = load_library()
+        none = np.zeros(1, dtype=np.uint64)  # a finalize of no queries checks the key and launches nothing
+        if lib.hecuda_oprf_finalize(_ptr(self._publicKey), _ptr(none), _ptr(none), 0, _ptr(none), _ptr(none),
+                                    _ptr(none), _ptr(none), _ptr(none)) != 0:
+            raise PirError("invalid OPRF public key: " + (lib.hecuda_last_error() or b"").decode())
+
+    def queryContext(self, keyword: bytes) -> OprfQueryContext:
+        """queryContext(at:) (:98-104) with a fresh random blind."""
+        return self.queryContexts([keyword])[0]
+
+    def queryContexts(self, keywords: Sequence[bytes], blinds: Optional[Sequence[int]] = None) -> List[OprfQueryContext]:
+        """One context per keyword in one device call.  `blinds` (integers in [1, n - 1]) defaults to fresh draws from
+        `secrets`; PirError for a blind outside that range."""
+        keywords = [bytes(k) for k in keywords]
+        if blinds is None:
+            blinds = [1 + secrets.randbelow(P384_ORDER - 1) for _ in keywords]
+        blinds = [int(r) for r in blinds]
+        if len(blinds) != len(keywords):
+            raise PirError(f"{len(blinds)} blinds for {len(keywords)} keywords")
+        if any(not 0 < r < P384_ORDER for r in blinds):
+            raise PirError("invalid OPRF blind: not in [1, n - 1]")
+        data, offsets = _concatenate(keywords)
+        count = len(keywords)
+        packed = np.frombuffer(b"".join(r.to_bytes(OPRF_KEY_BYTES, "big") for r in blinds) or b"\0", dtype=np.uint8)
+        queries = np.zeros((max(count, 1), OPRF_ELEMENT_BYTES), dtype=np.uint8)
+        status = np.ones(max(count, 1), dtype=np.uint8)
+        _check(load_library().hecuda_oprf_blind(_ptr(data), _ptr(offsets), count, _ptr(packed), _ptr(queries),
+                                                _ptr(status)))
+        return [OprfQueryContext(k, r, queries[i].tobytes()) for i, (k, r) in enumerate(zip(keywords, blinds))]
+
+    def parse(self, response: bytes, context: OprfQueryContext) -> ParsedOprfOutput:
+        """parse(oprfResponse:with:) (:106-117): PirError when the response does not verify."""
+        parsed = self.parseMany([response], [context])[0]
+        if parsed is None:
+            raise PirError("invalidOprfResponse: the server's proof does not verify")
+        return parsed
+
+    def parseMany(self, responses: Sequence[bytes], contexts: Sequence[OprfQueryContext]) -> List[Optional[ParsedOprfOutput]]:
+        """One parsed output per response in one device call; None where a response is rejected, including a wrong
+        length."""
+        responses = [bytes(r) for r in responses]
+        if len(responses) != len(contexts):
+            raise PirError(f"{len(responses)} responses for {len(contexts)} query contexts")
+        sized = [i for i, r in enumerate(responses) if len(r) == OPRF_RESPONSE_BYTES]
+        count = len(sized)
+        data, offsets = _concatenate([contexts[i].keyword for i in sized])
+        blinds = np.frombuffer(b"".join(contexts[i].blind.to_bytes(OPRF_KEY_BYTES, "big") for i in sized) or b"\0",
+                               dtype=np.uint8)
+        queries = np.frombuffer(b"".join(bytes(contexts[i].query) for i in sized) or b"\0", dtype=np.uint8)
+        packed = np.frombuffer(b"".join(responses[i] for i in sized) or b"\0", dtype=np.uint8)
+        outputs = np.zeros((max(count, 1), OPRF_OUTPUT_BYTES), dtype=np.uint8)
+        status = np.ones(max(count, 1), dtype=np.uint8)
+        _check(load_library().hecuda_oprf_finalize(_ptr(self._publicKey), _ptr(data), _ptr(offsets), count, _ptr(blinds),
+                                                   _ptr(queries), _ptr(packed), _ptr(outputs), _ptr(status)))
+        out: List[Optional[ParsedOprfOutput]] = [None] * len(responses)
+        for j, i in enumerate(sized):
+            if status[j] == 0:
+                out[i] = ParsedOprfOutput.fromOprfOutput(outputs[j].tobytes(), self.configType)
+        return out
+
+    def decrypt(self, encryptedEntry: bytes, parsed: ParsedOprfOutput) -> bytes:
+        """decrypt(encryptedEntry:with:) (:119-132): PirError when the entry does not authenticate."""
+        value = self.decryptMany([encryptedEntry], [parsed])[0]
+        if value is None:
+            raise PirError("authenticationFailure: the entry does not open under its OPRF output")
+        return value
+
+    def decryptMany(self, encryptedEntries: Sequence[bytes], parsedOutputs: Sequence[ParsedOprfOutput]) -> List[Optional[bytes]]:
+        """Every entry opened in one device call; None where an entry does not authenticate or is shorter than a tag."""
+        entries = [bytes(e) for e in encryptedEntries]
+        if len(entries) != len(parsedOutputs):
+            raise PirError(f"{len(entries)} entries for {len(parsedOutputs)} parsed outputs")
+        count = len(entries)
+        sealed, offsets = _concatenate(entries)
+        config = self.configType
+        if any(len(p.nonce) != config.nonceSize or len(p.secretKey) != config.entryEncryptionKeySize
+               for p in parsedOutputs):
+            raise PirError("a parsed OPRF output has the wrong nonce or key size")
+        # the device reads the nonce at h[0:12] and the key at h[24:48] of each OPRF output h
+        outputs = np.frombuffer(b"".join(p.nonce + bytes(12) + p.secretKey for p in parsedOutputs) or b"\0",
+                                dtype=np.uint8)
+        values = np.zeros(max(int(offsets[-1]), 1), dtype=np.uint8)
+        status = np.ones(max(count, 1), dtype=np.uint8)
+        _check(load_library().hecuda_symmetric_pir_open(_ptr(outputs), _ptr(sealed), _ptr(offsets), count, _ptr(values),
+                                                        _ptr(status)))
+        tag = config.tagSize
+        raw = values.tobytes()
+        return [raw[int(offsets[i]):int(offsets[i + 1]) - tag] if status[i] == 0 else None for i in range(count)]
