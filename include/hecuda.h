@@ -755,6 +755,98 @@ int32_t hecuda_pnns_matrix_device_buffer(hecuda_pnns_matrix *matrix, void **devi
  * the padded dimension (an absent plaintext).  capacity >= result_count * giant * baby. */
 int32_t hecuda_pnns_matrix_present(const hecuda_pnns_matrix *matrix, uint8_t *out, int64_t capacity);
 
+/* ---- PNNS processed databases and configurations in the reference's protobuf format ----
+ * apple.swift_homomorphic_encryption.pnns.v1.SerializedProcessedDatabase (proto3 binary): the plaintext matrices, one
+ * per plaintext modulus, each plaintext PolyRq.serialize() of its L Eval rows; the entry identifiers and metadata; the
+ * ServerConfig.  Saves are byte for byte what SwiftProtobuf writes (fields in field-number order, proto3 zero scalars
+ * omitted, repeated scalars packed).  Loads accept any conforming encoding: fields in any order, unknown fields of wire
+ * types 0, 1, 2 and 5, repeated scalars packed or not.  Refused: groups, varints over 10 bytes, lengths that run past
+ * the buffer, a singular message field given twice, and a wrong wire type for a known field.
+ *
+ * hecuda_pnns_server_config holds a ServerConfig (or, with database_packing = 0, a ClientConfig).  Enumerations keep
+ * their protobuf numbers: error_std_dev 0 = stdDev32 (3.2), 1 = stdDev64 (6.4); security_level 0 = unchecked
+ * (SECURITY_LEVEL_UNSPECIFIED), 1 = quantum128; he_scheme 0 = unspecified, 1 = BFV, 2 = BGV; distance_metric 0 =
+ * cosineSimilarity; a packing 0 = unset, 1 = denseRow, 2 = diagonal (with its BabyStepGiantStep), 3 = denseColumn.  A
+ * message with more coefficient moduli, extra plaintext moduli or Galois elements than the arrays hold is
+ * HECUDA_ERR_UNSUPPORTED. */
+#define HECUDA_PNNS_MAX_COEFFICIENT_MODULI 32    /* the reference's own limit */
+#define HECUDA_PNNS_MAX_EXTRA_PLAINTEXT_MODULI 7 /* 8 plaintext moduli: hecuda_pnns_decrypt_distances' limit */
+#define HECUDA_PNNS_MAX_GALOIS_ELEMENTS 64
+typedef struct hecuda_pnns_server_config {
+    /* ClientConfig.encryption_parameters (v1.EncryptionParameters); coefficient_moduli include the key-switching one */
+    uint64_t poly_degree;
+    uint64_t plaintext_modulus;
+    int32_t coefficient_moduli_count;
+    int32_t error_std_dev;
+    uint64_t coefficient_moduli[HECUDA_PNNS_MAX_COEFFICIENT_MODULI];
+    int32_t security_level;
+    int32_t he_scheme;
+    /* the rest of ClientConfig */
+    uint64_t scaling_factor;
+    int32_t query_packing;
+    uint32_t query_vector_dimension, query_baby_step, query_giant_step; /* query_packing = 2 only */
+    uint32_t vector_dimension;
+    int32_t galois_element_count;
+    uint32_t galois_elements[HECUDA_PNNS_MAX_GALOIS_ELEMENTS];
+    int32_t distance_metric;
+    int32_t extra_plaintext_moduli_count;
+    uint64_t extra_plaintext_moduli[HECUDA_PNNS_MAX_EXTRA_PLAINTEXT_MODULI];
+    /* ServerConfig.database_packing */
+    int32_t database_packing;
+    uint32_t database_vector_dimension, database_baby_step, database_giant_step; /* database_packing = 2 only */
+} hecuda_pnns_server_config;
+
+/* A ServerConfig message (hecuda_pnns_server_config_*) or a ClientConfig message (hecuda_pnns_client_config_*) on its
+ * own, as the reference's tools write them beside a database.  Parsing refuses what ServerConfig / ClientConfig.native()
+ * refuses, by the reference's error names: unsetField (no client_config / encryption_parameters), unsetOneof (a packing
+ * with no type), unrecognizedEnumValue, invalidScheme (BGV).  Serializing writes `*written` bytes to `out`; with out =
+ * NULL it only sets *written to the size.  HECUDA_ERR_INVALID_ARGUMENT when capacity is below it. */
+int32_t hecuda_pnns_server_config_parse(const uint8_t *bytes, uint64_t byte_count, hecuda_pnns_server_config *out);
+int32_t hecuda_pnns_server_config_serialize(const hecuda_pnns_server_config *config, uint8_t *out, uint64_t capacity,
+                                            uint64_t *written);
+int32_t hecuda_pnns_client_config_parse(const uint8_t *bytes, uint64_t byte_count, hecuda_pnns_server_config *out);
+int32_t hecuda_pnns_client_config_serialize(const hecuda_pnns_server_config *config, uint8_t *out, uint64_t capacity,
+                                            uint64_t *written);
+
+/* What a SerializedProcessedDatabase holds, from one walk of its framing (no payload is read, nothing is allocated on
+ * the device): its ServerConfig, the number of plaintext matrices and their row and column counts (the same for every
+ * matrix, or HECUDA_ERR_INVALID_ARGUMENT), the entry-identifier count, and the metadata count and total bytes.
+ * hecuda_pnns_database_entries copies the identifiers (id_capacity >= their count) and the metadata: entry k's bytes are
+ * metadata[metadata_offsets[k] .. metadata_offsets[k + 1]) (offsets_capacity >= count + 1).  Null buffers are skipped. */
+int32_t hecuda_pnns_database_describe(const uint8_t *bytes, uint64_t byte_count, hecuda_pnns_server_config *config,
+                                      int32_t *matrix_count, int64_t *row_count, int64_t *column_count,
+                                      int64_t *entry_id_count, int64_t *metadata_count, uint64_t *metadata_bytes);
+int32_t hecuda_pnns_database_entries(const uint8_t *bytes, uint64_t byte_count, uint64_t *entry_ids, int64_t id_capacity,
+                                     uint8_t *metadata, uint64_t metadata_capacity, uint64_t *metadata_offsets,
+                                     int64_t offsets_capacity);
+
+/* ProcessedDatabase(from:contexts:) (ProcessedDatabase.swift:56-75) for its plaintext matrices, unpacked on the device:
+ * out[k] is the matrix of plaintext modulus k over ctxs[k], word for word the handle hecuda_pnns_matrix_create(
+ * eval_format = 1, ...) builds from the same plaintexts (the same resident words, flags, result count and steps).
+ * count must equal 1 + the config's extra plaintext moduli (wrongContextsCount) and every context the config's
+ * parameters (wrongEncryptionParameters); every matrix must be .diagonal (HECUDA_ERR_UNSUPPORTED otherwise), hold
+ * nextPow2(num_columns) * ceil(num_rows / N) plaintexts (wrongPlaintextCount), each of exactly L serialized rows, with
+ * steps hecuda_pnns_matrix_create accepts.  All of it is checked before anything is allocated.  Whole plaintexts cross
+ * PCIe in chunks of at most 64 MB, through pinned staging unless `bytes` is pinned.  Residues >= their modulus are
+ * refused (the reference accepts them), naming the matrix, plaintext and row.  On error every out[k] is NULL and nothing
+ * stays allocated. */
+int32_t hecuda_pnns_matrices_create_serialized(const hecuda_context *const *ctxs, int32_t count, const uint8_t *bytes,
+                                               uint64_t byte_count, hecuda_pnns_matrix **out);
+/* ProcessedDatabase.serialize() (ProcessedDatabase.swift:81-88) followed by proto().serializedData(): matrices[k] of
+ * plaintext modulus k, the entry identifiers, the metadata (entry k at metadata[metadata_offsets[k] ..
+ * metadata_offsets[k + 1]); metadata_count 0 for none), and `config`, whose parameters must match the matrices'
+ * contexts and whose database packing must be the matrices' .diagonal steps.  The plaintexts are packed on the device
+ * with their framing, so each chunk leaves as one contiguous range of the file.  *written = the byte count. */
+int32_t hecuda_pnns_database_serialized_byte_count(const hecuda_pnns_matrix *const *matrices, int32_t count,
+                                                   const uint64_t *entry_ids, int64_t entry_id_count,
+                                                   const uint8_t *metadata, const uint64_t *metadata_offsets,
+                                                   int64_t metadata_count, const hecuda_pnns_server_config *config,
+                                                   uint64_t *bytes);
+int32_t hecuda_pnns_database_serialize(const hecuda_pnns_matrix *const *matrices, int32_t count, const uint64_t *entry_ids,
+                                       int64_t entry_id_count, const uint8_t *metadata, const uint64_t *metadata_offsets,
+                                       int64_t metadata_count, const hecuda_pnns_server_config *config, uint8_t *out,
+                                       uint64_t capacity, uint64_t *written);
+
 /* PlaintextMatrix.mulTranspose(vector:using:) -- MatrixMultiplication.swift:131-226, for `batch` dense-row query
  * ciphertexts (batch x 2 x L x N, Coeff) that share `evk`: babyStep-1 rotateColumns(by: -1), forward NTTs, one
  * ct x pt inner product per (result ciphertext, giant step), rotateColumnsAndSum(by: -babyStep)

@@ -139,6 +139,53 @@ struct WsGuard {
 
 int32_t check_ctx(const hecuda_context *h);
 
+// ---- the staging of the processed-database pipelines (saving and loading PIR and PNNS databases)
+// A caller's buffer that is pinned from its first to its last byte (hecuda_host_alloc, hecuda_host_register) is copied
+// from directly; a pageable one goes through pinned staging.
+inline bool host_pinned(const void *p, size_t bytes) {
+    for (const char *at : {(const char *)p, (const char *)p + bytes - 1}) {
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, at) != cudaSuccess) {
+            cudaGetLastError();
+            return false;
+        }
+        if (a.type != cudaMemoryTypeHost) return false;
+    }
+    return true;
+}
+
+// The pipeline's buffers: two pooled workspaces, each a stream and a device staging buffer (its staged-input buffer,
+// which stays with the workspace for later calls), and for a pageable caller buffer a pinned buffer per stream with the
+// event after which it may be reused.  The streams are synchronized before this is destroyed.
+struct DbStaging {
+    WsGuard g0, g1;
+    cudaStream_t stream[2];
+    unsigned char *dev[2] = {nullptr, nullptr}, *host[2] = {nullptr, nullptr};
+    cudaEvent_t copied[2] = {nullptr, nullptr};
+    explicit DbStaging(const hecuda_context *h) : g0(h), g1(h) {
+        stream[0] = g0.w ? g0.w->stream : nullptr;
+        stream[1] = g1.w ? g1.w->stream : nullptr;
+    }
+    cudaError_t init(size_t bytes, bool pageable) {
+        if (!g0.w || !g1.w) return cudaErrorMemoryAllocation;
+        Workspace *w[2] = {g0.w, g1.w};
+        for (int b = 0; b < 2; ++b) {
+            cudaError_t e = w[b]->in.reserve((bytes + sizeof(u64) - 1) / sizeof(u64));
+            dev[b] = (unsigned char *)w[b]->in.p;
+            if (e == cudaSuccess && pageable) e = cudaHostAlloc(&host[b], bytes, cudaHostAllocDefault);
+            if (e == cudaSuccess && pageable) e = cudaEventCreateWithFlags(&copied[b], cudaEventDisableTiming);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    }
+    ~DbStaging() {
+        for (int b = 0; b < 2; ++b) {
+            if (host[b]) cudaFreeHost(host[b]);
+            if (copied[b]) cudaEventDestroy(copied[b]);
+        }
+    }
+};
+
 // Wait for a stream from a host thread: yields the CPU (an event created with cudaEventBlockingSync, one per thread)
 // instead of spinning in cudaStreamSynchronize.
 cudaError_t wait_stream(cudaStream_t s);

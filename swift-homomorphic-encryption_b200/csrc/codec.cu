@@ -17,7 +17,12 @@ namespace hecuda {
 
 // offset of polynomial `poly`'s rows in `bytes` under `at` (-1: a nil plaintext)
 __device__ __forceinline__ long long poly_bytes_offset(const CodecConsts &c, const PolyLayout &at, int64_t poly) {
-    return at.tag ? tagged_rows_offset(at.tag + at.first, at.base, poly) : poly * c.byte_offset[c.rows];
+    return at.tag ? tagged_rows_offset(at.tag + at.first, at.base, poly, at.frame) : poly * c.byte_offset[c.rows];
+}
+
+// the resident polynomial that plaintext `poly` of the layout is
+__device__ __forceinline__ int64_t resident_poly(const PolyLayout &at, int64_t poly) {
+    return at.slot ? at.slot[at.first + poly] : poly;
 }
 
 // bytes -> coefficients: one thread per coefficient
@@ -31,7 +36,7 @@ __global__ void __launch_bounds__(256) poly_load_kernel(const unsigned char *__r
     const int64_t poly = blockIdx.z;
     const long long offset = poly_bytes_offset(c, at, poly);
     if (at.present && row == 0 && i == 0) at.present[poly] = offset >= 0;
-    Word *dst = out + (poly * c.rows + row) * n + i;
+    Word *dst = out + (resident_poly(at, poly) * c.rows + row) * n + i;
     if (offset < 0) {
         *dst = 0;
         return;
@@ -42,9 +47,15 @@ __global__ void __launch_bounds__(256) poly_load_kernel(const unsigned char *__r
     *dst = (Word)v;
 }
 
-// the tag byte of a tagged stream's plaintext, written by the first thread of its first row
+// the framing of a tagged stream's plaintext (a nil plaintext's: its 0 tag), written by the first thread of its first row
 __device__ __forceinline__ void write_tag(unsigned char *bytes, const PolyLayout &at, int64_t poly, long long offset, long long j) {
-    if (at.tag && blockIdx.y == 0 && j == 0) bytes[at.tag[at.first + poly] - at.base] = offset >= 0;
+    if (!at.tag || blockIdx.y != 0 || j != 0) return;
+    unsigned char *dst = bytes + at.tag[at.first + poly] - at.base;
+    if (offset < 0) {
+        *dst = 0;
+        return;
+    }
+    for (int k = 0; k < at.frame; ++k) dst[k] = at.frame_bytes[k];
 }
 
 // coefficients -> bytes: one thread per output byte
@@ -60,7 +71,7 @@ __global__ void __launch_bounds__(256) poly_serialize_kernel(const Word *__restr
     const long long offset = poly_bytes_offset(c, at, poly);
     write_tag(bytes, at, poly, offset, j);
     if (offset < 0) return;
-    const u64 value = codec_pack(in + (poly * c.rows + row) * n, n, c.width[row], skip, 8 * j, 8);
+    const u64 value = codec_pack(in + (resident_poly(at, poly) * c.rows + row) * n, n, c.width[row], skip, 8 * j, 8);
     bytes[offset + c.byte_offset[row] + j] = (unsigned char)value;
 }
 
@@ -89,6 +100,7 @@ bool codec_consts(const Context &ctx, const NttRowMap &map, int skip, CodecConst
 long long serialized_poly_bytes(const CodecConsts &c) { return c.byte_offset[c.rows]; }
 
 // `at` for the polynomials from `done` on: a tagged layout moves its first plaintext, the default one its pointers
+// (with slots, the rows' pointer stays where it is: the slots are indices into it)
 PolyLayout layout_from(const PolyLayout &at, int64_t done) {
     PolyLayout part = at;
     part.first += done;
@@ -103,13 +115,14 @@ cudaError_t launch_poly_load(const Context &ctx, const CodecConsts &c, int skip,
     return for_each_part(polys, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)((ctx.n + threads - 1) / threads), (unsigned)c.rows, (unsigned)chunk);
         return launch(poly_load_kernel<Word>, grid, threads, 0, stream, layout.tag ? bytes : bytes + done * c.byte_offset[c.rows],
-                      out + done * c.rows * ctx.n, c, (int)ctx.n, skip, layout_from(layout, done));
+                      out + (layout.slot ? 0 : done * c.rows * ctx.n), c, (int)ctx.n, skip, layout_from(layout, done));
     });
 }
 
 // coefficients -> bytes, 8 output bytes per thread (rows whose byte count and offset are multiples of 8: N >= 64).
-// A tagged stream's rows start one byte after their tag, so mostly off an 8-byte boundary: the 8 bytes then go out in
-// the widest stores that the rows' alignment allows, the same for every thread of the block.
+// A tagged stream's rows start right after their framing (a tag byte, or a PNNS file's protobuf keys and lengths), so
+// mostly off an 8-byte boundary: the 8 bytes then go out in the widest stores that the rows' alignment allows, the same
+// for every thread of the block.
 template <typename Word>
 __global__ void __launch_bounds__(256) poly_serialize_words_kernel(const Word *__restrict__ in, unsigned char *__restrict__ bytes,
                                                                   const __grid_constant__ CodecConsts c, int n, int skip,
@@ -123,7 +136,7 @@ __global__ void __launch_bounds__(256) poly_serialize_words_kernel(const Word *_
     write_tag(bytes, at, poly, offset, j);
     if (offset < 0) return;
     // big-endian bit stream: stream bit 64 j is the MSB of the value
-    const u64 value = codec_pack(in + (poly * c.rows + row) * n, n, c.width[row], skip, 64 * j, 64);
+    const u64 value = codec_pack(in + (resident_poly(at, poly) * c.rows + row) * n, n, c.width[row], skip, 64 * j, 64);
     // store most significant byte first
     const u64 swapped = __byte_perm((unsigned)(value >> 32), 0, 0x0123) | ((u64)__byte_perm((unsigned)value, 0, 0x0123) << 32);
     unsigned char *dst = bytes + offset + c.byte_offset[row] + 8 * j;
@@ -156,7 +169,7 @@ cudaError_t launch_poly_serialize(const Context &ctx, const CodecConsts &c, int 
     return for_each_part(polys, [&](int64_t done, int64_t chunk) {
         dim3 grid((unsigned)(((words ? widest / 8 : widest) + 255) / 256), (unsigned)c.rows, (unsigned)chunk);
         return launch(words ? poly_serialize_words_kernel<Word> : poly_serialize_kernel<Word>, grid, 256, 0, stream,
-                      in + done * c.rows * ctx.n, layout.tag ? bytes : bytes + done * c.byte_offset[c.rows], c, (int)ctx.n,
+                      in + (layout.slot ? 0 : done * c.rows * ctx.n), layout.tag ? bytes : bytes + done * c.byte_offset[c.rows], c, (int)ctx.n,
                       skip, layout_from(layout, done));
     });
 }

@@ -209,19 +209,27 @@ HE_HD u64 codec_pack(const Word *__restrict__ src, int n, int w, int skip, long 
     return value;
 }
 // Where each polynomial's bytes are.  Default: polynomial p at p * serialized_poly_bytes.  With `tag`: a processed
-// database's stream (IndexPirProtocol.swift:336-378) staged from byte `base` of the file, in which plaintext `first` + p
-// has its tag byte at tag[first + p] and, unless it is nil, its rows right after it; tag[first + p + 1] is where the
-// next one starts.  A load then writes present[p], writes zero rows for a nil plaintext, and atomically lowers *bad to
-// (first + p) * rows + row where a residue is >= its modulus; a serialization writes the tag byte too.
+// database's stream staged from byte `base` of the file, in which plaintext `first` + p has `frame` bytes of framing at
+// tag[first + p] and, unless it is nil, its rows right after them; tag[first + p + 1] is where the next one starts.
+// A PIR file (IndexPirProtocol.swift:336-378) frames each plaintext with its tag byte (frame 1: 1 present, 0 nil); a
+// PNNS file (SerializedProcessedDatabase) with its protobuf keys and lengths, the same bytes for every plaintext of a
+// matrix (a load, which walked them on the host, passes the rows' own offsets with frame 0).  A load then writes
+// present[p], writes zero rows for a nil plaintext, and atomically lowers *bad to (first + p) * rows + row where a
+// residue is >= its modulus; a serialization writes the framing too (frame_bytes, or a 0 tag for a nil plaintext).
+// With `slot`, plaintext first + p is resident polynomial slot[first + p] of the rows passed, instead of polynomial p.
+constexpr int kMaxFrame = 24;  // two keys and two 10-byte varints at most
 struct PolyLayout {
     const long long *tag = nullptr;
     long long base = 0, first = 0;
     unsigned char *present = nullptr;
     unsigned long long *bad = nullptr;
+    const long long *slot = nullptr;
+    int frame = 1;
+    unsigned char frame_bytes[kMaxFrame] = {1};
 };
 // offset from `base` of the rows of plaintext p of a tagged stream (tag[] as in PolyLayout), or -1 for a nil plaintext
-HE_HD long long tagged_rows_offset(const long long *tag, long long base, long long p) {
-    return tag[p + 1] - tag[p] > 1 ? tag[p] + 1 - base : -1;
+HE_HD long long tagged_rows_offset(const long long *tag, long long base, long long p, int frame = 1) {
+    return tag[p + 1] - tag[p] > frame ? tag[p] + frame - base : -1;
 }
 bool codec_consts(const Context &ctx, const NttRowMap &map, int skip, CodecConsts &c, std::string &err);
 long long serialized_poly_bytes(const CodecConsts &c);

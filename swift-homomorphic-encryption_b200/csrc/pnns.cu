@@ -977,3 +977,479 @@ int32_t hecuda_pnns_compute_response_clients_wire(const hecuda_context *h, const
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------- saving and loading processed databases
+// SerializedProcessedDatabase (ProcessedDatabase.swift:56-88, PnnsConversion.swift).  The host walks or places the
+// protobuf framing (pnns_database_io.hpp); whole plaintexts then cross PCIe in chunks of at most one 64 MB slab
+// through the two-workspace pipeline of the PIR files (pir.cu), and the codec kernels (codec.cu) unpack each plaintext
+// straight into its resident slot, or pack it from there together with its framing.
+#include "database_io.hpp"
+#include "pnns_database_io.hpp"
+
+namespace {
+
+int32_t io_fail(const pnnsio::Error &e) { return fail(e.code, e.what); }
+
+std::string moduli_text(const std::vector<u64> &m) {
+    std::string s = "[";
+    for (size_t k = 0; k < m.size(); ++k) s += (k ? ", " : "") + std::to_string(m[k]);
+    return s + "]";
+}
+
+// ServerConfig.validateContexts (Config.swift:125-135): one context per plaintext modulus, each with the config's
+// degree, coefficient moduli (the key-switching one included) and its plaintext modulus
+int32_t validate_contexts(const hecuda_context *const *ctxs, int32_t count, const hecuda_pnns_server_config &cfg) {
+    const int32_t expected = 1 + cfg.extra_plaintext_moduli_count;
+    if (count != expected)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongContextsCount(got: " + std::to_string(count) + ", expected: " +
+                                                     std::to_string(expected) + ")");
+    const std::vector<u64> want(cfg.coefficient_moduli, cfg.coefficient_moduli + cfg.coefficient_moduli_count);
+    for (int32_t k = 0; k < count; ++k) {
+        int32_t rc = check_ctx(ctxs[k]);
+        if (rc) return rc;
+        const Context &c = *ctxs[k]->ctx;
+        std::vector<u64> got = c.q;
+        if (c.has_ks) got.push_back(c.q_ks);
+        const u64 t = k ? cfg.extra_plaintext_moduli[k - 1] : cfg.plaintext_modulus;
+        if ((u64)c.n != cfg.poly_degree || c.t != t || got != want)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT,
+                        "wrongEncryptionParameters(context " + std::to_string(k) + ": got N = " + std::to_string(c.n) +
+                            ", t = " + std::to_string(c.t) + ", moduli " + moduli_text(got) + "; expected N = " +
+                            std::to_string(cfg.poly_degree) + ", t = " + std::to_string(t) + ", moduli " + moduli_text(want) + ")");
+    }
+    return HECUDA_OK;
+}
+
+// A resident .diagonal matrix's shape, as hecuda_pnns_matrix_create checks it
+struct DiagonalShape {
+    int64_t dimension = 0, results = 0, count = 0, slots = 0;
+    int32_t baby = 0, giant = 0;
+};
+int32_t diagonal_shape(const Context &c, int64_t rows, int64_t cols, uint32_t baby, uint32_t giant, DiagonalShape &s) {
+    int32_t rc = check_dimensions(c, rows, cols, s.dimension);
+    if (rc) return rc;
+    s.baby = (int32_t)baby, s.giant = (int32_t)giant;
+    if ((int64_t)baby != s.baby || (int64_t)giant != s.giant) s.baby = s.giant = -1;
+    if ((rc = check_steps(c, s.dimension, s.baby, s.giant))) return rc;
+    if (!c.simd) return fail(HECUDA_ERR_UNSUPPORTED, "simdEncodingNotSupported");
+    s.results = (rows + c.n - 1) / c.n;
+    s.count = s.dimension * s.results;
+    s.slots = s.results * s.giant * s.baby;
+    return HECUDA_OK;
+}
+
+// plaintext index resultCount * (j + babyStep * g) + r  ->  slot (r, g, j), as hecuda_pnns_matrix_create places them
+std::vector<long long> file_slots(const DiagonalShape &s) {
+    std::vector<long long> slot((size_t)s.count);
+    for (int64_t p = 0; p < s.count; ++p) {
+        const int64_t r = p % s.results, d = p / s.results;
+        slot[(size_t)p] = (r * s.giant + d / s.baby) * s.baby + d % s.baby;
+    }
+    return slot;
+}
+
+// The chunks of every matrix, in file order: (matrix, chunk of its plaintexts), and the largest chunk's bytes
+struct MatrixChunk {
+    int matrix;
+    dbio::Chunk chunk;
+};
+std::vector<MatrixChunk> plan_matrix_chunks(const std::vector<std::vector<long long>> &tags, long long &widest) {
+    std::vector<MatrixChunk> plan;
+    widest = 1;
+    for (size_t k = 0; k < tags.size(); ++k)
+        for (const dbio::Chunk &ch : dbio::plan_chunks(tags[k], 0, (long long)tags[k].size() - 1, kSlabBytes)) {
+            plan.push_back({(int)k, ch});
+            widest = std::max(widest, tags[k][(size_t)(ch.first + ch.count)] - tags[k][(size_t)ch.first]);
+        }
+    return plan;
+}
+
+// Device copies of each matrix's framing offsets and slot map
+struct DeviceMaps {
+    std::vector<long long *> tag, slot;
+    ~DeviceMaps() {
+        for (long long *p : tag) cudaFree(p);
+        for (long long *p : slot) cudaFree(p);
+    }
+    cudaError_t add(const std::vector<long long> &t, const std::vector<long long> &s) {
+        tag.push_back(nullptr);
+        slot.push_back(nullptr);
+        cudaError_t e = cudaMalloc(&tag.back(), t.size() * sizeof(long long));
+        if (e == cudaSuccess) e = upload(tag.back(), t.data(), t.size() * sizeof(long long));
+        if (e == cudaSuccess) e = cudaMalloc(&slot.back(), std::max<size_t>(s.size(), 1) * sizeof(long long));
+        if (e == cudaSuccess && !s.empty()) e = upload(slot.back(), s.data(), s.size() * sizeof(long long));
+        return e;
+    }
+};
+
+// The checks shared by the byte count and the serialization, and where everything goes.  Launches nothing.
+int32_t serialization_placement(const hecuda_pnns_matrix *const *ms, int32_t count, const uint64_t *ids, int64_t id_count,
+                                const uint8_t *metadata, const uint64_t *metadata_offsets, int64_t metadata_count,
+                                const hecuda_pnns_server_config *cfg, pnnsio::Placement &pl, std::vector<DiagonalShape> &shapes,
+                                std::vector<CodecConsts> &cc) {
+    if (!ms || count < 1 || !cfg) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument / no matrices");
+    if (id_count < 0 || metadata_count < 0 || (id_count && !ids) || (metadata_count && !metadata_offsets))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "null or negative entry buffers");
+    for (int64_t k = 0; k < metadata_count; ++k)
+        if (metadata_offsets[k + 1] < metadata_offsets[k])
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "metadata offsets must not decrease");
+    if (metadata_count && metadata_offsets[metadata_count] > metadata_offsets[0] && !metadata)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "null metadata");
+    pnnsio::Error e;
+    if (!pnnsio::check_config(*cfg, true, e)) return io_fail(e);
+    if (cfg->database_packing != pnnsio::kDiagonal)
+        return fail(HECUDA_ERR_UNSUPPORTED, "databasePacking: only .diagonal matrices are resident here");
+    std::vector<const hecuda_context *> ctxs((size_t)count);
+    for (int32_t k = 0; k < count; ++k) {
+        if (!ms[k]) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null matrix");
+        ctxs[(size_t)k] = ms[k]->owner;
+    }
+    int32_t rc = validate_contexts(ctxs.data(), count, *cfg);
+    if (rc) return rc;
+    std::vector<pnnsio::MatrixShape> placed;
+    for (int32_t k = 0; k < count; ++k) {
+        const hecuda_pnns_matrix *m = ms[k];
+        const Context &c = *m->owner->ctx;
+        if (m->row_count != ms[0]->row_count || m->column_count != ms[0]->column_count)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "the matrices differ in shape");
+        if ((uint32_t)m->baby != cfg->database_baby_step || (uint32_t)m->giant != cfg->database_giant_step)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongMatrixPacking: the config's babyStep / giantStep are not the matrix's");
+        shapes.emplace_back();
+        if ((rc = diagonal_shape(c, m->row_count, m->column_count, (uint32_t)m->baby, (uint32_t)m->giant, shapes.back()))) return rc;
+        cc.emplace_back();
+        std::string err;
+        if (!codec_consts(c, c.map_q(c.L), 0, cc.back(), err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+        placed.push_back({m->row_count, m->column_count, shapes.back().count, serialized_poly_bytes(cc.back())});
+    }
+    pl = pnnsio::place_database(placed, ids, id_count, metadata, metadata_offsets, metadata_count, *cfg);
+    return HECUDA_OK;
+}
+
+// A standalone config message: its bytes into `out`, or only their count with out = NULL
+int32_t write_message(const pnnsio::Bytes &bytes, uint8_t *out, uint64_t capacity, uint64_t *written) {
+    if (!out) {
+        *written = bytes.size();
+        return HECUDA_OK;
+    }
+    if (capacity < bytes.size())
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "capacity " + std::to_string(capacity) + " below the serialized size " +
+                                                     std::to_string(bytes.size()));
+    memcpy(out, bytes.data(), bytes.size());
+    *written = bytes.size();
+    return HECUDA_OK;
+}
+
+long long clamp_size(uint64_t byte_count) { return (long long)std::min<uint64_t>(byte_count, INT64_MAX); }
+
+}  // namespace
+
+extern "C" {
+
+int32_t hecuda_pnns_server_config_parse(const uint8_t *bytes, uint64_t byte_count, hecuda_pnns_server_config *out) {
+    if (!out || (!bytes && byte_count)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    hecuda_pnns_server_config c{};
+    pnnsio::Error e;
+    if (!pnnsio::parse_server_config(bytes, 0, clamp_size(byte_count), c, e)) return io_fail(e);
+    *out = c;
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pnns_client_config_parse(const uint8_t *bytes, uint64_t byte_count, hecuda_pnns_server_config *out) {
+    if (!out || (!bytes && byte_count)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    hecuda_pnns_server_config c{};
+    pnnsio::Error e;
+    if (!pnnsio::parse_client_config(bytes, 0, clamp_size(byte_count), c, e)) return io_fail(e);
+    *out = c;
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pnns_server_config_serialize(const hecuda_pnns_server_config *config, uint8_t *out, uint64_t capacity,
+                                            uint64_t *written) {
+    if (!config || !written) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *written = 0;
+    pnnsio::Error e;
+    if (!pnnsio::check_config(*config, true, e)) return io_fail(e);
+    return write_message(pnnsio::encode_server_config(*config), out, capacity, written);
+}
+
+int32_t hecuda_pnns_client_config_serialize(const hecuda_pnns_server_config *config, uint8_t *out, uint64_t capacity,
+                                            uint64_t *written) {
+    if (!config || !written) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *written = 0;
+    pnnsio::Error e;
+    if (!pnnsio::check_config(*config, false, e)) return io_fail(e);
+    return write_message(pnnsio::encode_client_config(*config), out, capacity, written);
+}
+
+int32_t hecuda_pnns_database_describe(const uint8_t *bytes, uint64_t byte_count, hecuda_pnns_server_config *config,
+                                      int32_t *matrix_count, int64_t *row_count, int64_t *column_count,
+                                      int64_t *entry_id_count, int64_t *metadata_count, uint64_t *metadata_bytes) {
+    if (!config || !matrix_count || !row_count || !column_count || !entry_id_count || !metadata_count || !metadata_bytes ||
+        (!bytes && byte_count))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    pnnsio::Database db;
+    pnnsio::Error e;
+    if (!pnnsio::walk_database(bytes, clamp_size(byte_count), db, e)) return io_fail(e);
+    for (const pnnsio::Matrix &m : db.matrices)
+        if (m.rows != db.matrices[0].rows || m.cols != db.matrices[0].cols)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "the plaintext matrices differ in num_rows / num_columns");
+    *config = db.config;
+    *matrix_count = (int32_t)db.matrices.size();
+    *row_count = db.matrices.empty() ? 0 : db.matrices[0].rows;
+    *column_count = db.matrices.empty() ? 0 : db.matrices[0].cols;
+    *entry_id_count = (int64_t)db.entry_ids.size();
+    *metadata_count = (int64_t)db.metadata_bytes.size();
+    uint64_t total = 0;
+    for (long long b : db.metadata_bytes) total += (uint64_t)b;
+    *metadata_bytes = total;
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pnns_database_entries(const uint8_t *bytes, uint64_t byte_count, uint64_t *entry_ids, int64_t id_capacity,
+                                     uint8_t *metadata, uint64_t metadata_capacity, uint64_t *metadata_offsets,
+                                     int64_t offsets_capacity) {
+    if (!bytes && byte_count) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    pnnsio::Database db;
+    pnnsio::Error e;
+    if (!pnnsio::walk_database(bytes, clamp_size(byte_count), db, e)) return io_fail(e);
+    if (entry_ids) {
+        if (id_capacity < (int64_t)db.entry_ids.size()) return fail(HECUDA_ERR_INVALID_ARGUMENT, "id_capacity below the entry count");
+        std::copy(db.entry_ids.begin(), db.entry_ids.end(), entry_ids);
+    }
+    uint64_t total = 0;
+    for (long long b : db.metadata_bytes) total += (uint64_t)b;
+    if (metadata_offsets && offsets_capacity < (int64_t)db.metadata_bytes.size() + 1)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "offsets_capacity below the metadata count + 1");
+    if (metadata && metadata_capacity < total) return fail(HECUDA_ERR_INVALID_ARGUMENT, "metadata_capacity below the metadata bytes");
+    uint64_t at = 0;
+    for (size_t k = 0; k < db.metadata_bytes.size(); ++k) {
+        if (metadata_offsets) metadata_offsets[k] = at;
+        if (metadata) memcpy(metadata + at, bytes + db.metadata_at[k], (size_t)db.metadata_bytes[k]);
+        at += (uint64_t)db.metadata_bytes[k];
+    }
+    if (metadata_offsets) metadata_offsets[db.metadata_bytes.size()] = at;
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pnns_matrices_create_serialized(const hecuda_context *const *ctxs, int32_t count, const uint8_t *bytes,
+                                               uint64_t byte_count, hecuda_pnns_matrix **out) {
+    if (!out || !ctxs || count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument or no context");
+    for (int32_t k = 0; k < count; ++k) out[k] = nullptr;
+    if (!bytes && byte_count) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null buffer");
+    // every check before anything is allocated
+    pnnsio::Database db;
+    pnnsio::Error e;
+    if (!pnnsio::walk_database(bytes, clamp_size(byte_count), db, e)) return io_fail(e);
+    int32_t rc = validate_contexts(ctxs, count, db.config);
+    if (rc) return rc;
+    if ((int32_t)db.matrices.size() != count)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidDatabase: " + std::to_string(db.matrices.size()) +
+                                                     " plaintext matrices for " + std::to_string(count) + " plaintext moduli");
+    if (db.config.database_packing != pnnsio::kDiagonal)
+        return fail(HECUDA_ERR_UNSUPPORTED, "databasePacking: only .diagonal matrices are resident here");
+    std::vector<DiagonalShape> shapes((size_t)count);
+    std::vector<CodecConsts> cc((size_t)count);
+    std::vector<std::vector<long long>> tags((size_t)count);
+    for (int32_t k = 0; k < count; ++k) {
+        const pnnsio::Matrix &m = db.matrices[(size_t)k];
+        const Context &c = *ctxs[k]->ctx;
+        const std::string which = "matrix " + std::to_string(k);
+        if (m.packing != pnnsio::kDiagonal)
+            return fail(HECUDA_ERR_UNSUPPORTED, which + ": only .diagonal matrices are resident here");
+        DiagonalShape &s = shapes[(size_t)k];
+        if ((rc = diagonal_shape(c, m.rows, m.cols, m.bsgs[1], m.bsgs[2], s))) return rc;
+        if ((int64_t)m.poly_at.size() != s.count)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongPlaintextCount(got: " + std::to_string(m.poly_at.size()) +
+                                                         ", expected: " + std::to_string(s.count) + ") in " + which);
+        std::string err;
+        if (!codec_consts(c, c.map_q(c.L), 0, cc[(size_t)k], err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+        const long long poly_bytes = serialized_poly_bytes(cc[(size_t)k]);
+        for (size_t p = 0; p < m.poly_bytes.size(); ++p)
+            if (m.poly_bytes[p] != poly_bytes)
+                return fail(HECUDA_ERR_INVALID_ARGUMENT, "corruptedData(" + which + ", plaintext " + std::to_string(p) + ": " +
+                                                             std::to_string(m.poly_bytes[p]) + " bytes of poly, expected " +
+                                                             std::to_string(poly_bytes) + " for " + std::to_string(c.L) + " rows)");
+        // the rows' own offsets (frame 0); the last plaintext ends its matrix's stream
+        tags[(size_t)k] = m.poly_at;
+        tags[(size_t)k].push_back(m.poly_at.back() + poly_bytes);
+    }
+    long long widest = 0;
+    const std::vector<MatrixChunk> plan = plan_matrix_chunks(tags, widest);
+    long long last = 0;
+    for (const std::vector<long long> &t : tags) last = std::max(last, t.back());
+    const bool pinned = host_pinned(bytes, (size_t)last);
+
+    DbStaging st(ctxs[0]);
+    if (!st.g0.w || !st.g1.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    std::vector<hecuda_pnns_matrix *> ms;
+    DeviceMaps maps;
+    unsigned long long *d_bad = nullptr;
+    std::vector<unsigned long long> bad((size_t)count, ~0ull);
+    cudaError_t err = cudaSuccess;
+    for (int32_t k = 0; k < count && err == cudaSuccess; ++k) {
+        const Context &c = *ctxs[k]->ctx;
+        const DiagonalShape &s = shapes[(size_t)k];
+        hecuda_pnns_matrix *m = new (std::nothrow) hecuda_pnns_matrix();
+        if (!m) {
+            err = cudaErrorMemoryAllocation;
+            break;
+        }
+        ms.push_back(m);
+        m->owner = ctxs[k];
+        m->row_count = db.matrices[(size_t)k].rows;
+        m->column_count = db.matrices[(size_t)k].cols;
+        m->result_count = s.results;
+        m->baby = s.baby;
+        m->giant = s.giant;
+        m->dimension = (int)s.dimension;
+        // slots past the padded dimension are absent: zero rows, flag 0
+        std::vector<unsigned char> present((size_t)s.slots);
+        for (int64_t slot = 0; slot < s.slots; ++slot) present[(size_t)slot] = slot % ((int64_t)s.giant * s.baby) < s.dimension;
+        const size_t words = (size_t)c.L * c.n * s.slots;
+        err = cudaMalloc(&m->d_plain, words * sizeof(u64));
+        if (err == cudaSuccess) err = fill(m->d_plain, 0, words * sizeof(u64));
+        if (err == cudaSuccess) err = cudaMalloc(&m->d_present, (size_t)s.slots);
+        if (err == cudaSuccess) err = upload(m->d_present, present.data(), (size_t)s.slots);
+        if (err == cudaSuccess) err = maps.add(tags[(size_t)k], file_slots(s));
+    }
+    if (err == cudaSuccess) err = cudaMalloc(&d_bad, (size_t)count * sizeof(unsigned long long));
+    if (err == cudaSuccess) err = fill(d_bad, 0xff, (size_t)count * sizeof(unsigned long long));
+    if (err == cudaSuccess) err = st.init((size_t)widest, !pinned);
+    for (size_t k = 0; k < plan.size() && err == cudaSuccess; ++k) {
+        const int b = (int)(k & 1), mi = plan[k].matrix;
+        const dbio::Chunk &ch = plan[k].chunk;
+        const std::vector<long long> &tag = tags[(size_t)mi];
+        const long long base = tag[(size_t)ch.first], size = tag[(size_t)(ch.first + ch.count)] - base;
+        const unsigned char *src = bytes + base;
+        if (!pinned) {  // the pinned buffer is free once the copy two chunks back has finished
+            if (k >= 2) err = cudaEventSynchronize(st.copied[b]);
+            if (err != cudaSuccess) break;
+            memcpy(st.host[b], src, (size_t)size);
+            src = st.host[b];
+        }
+        err = cudaMemcpyAsync(st.dev[b], src, (size_t)size, cudaMemcpyHostToDevice, st.stream[b]);
+        if (err == cudaSuccess && !pinned) err = cudaEventRecord(st.copied[b], st.stream[b]);
+        PolyLayout at;
+        at.tag = maps.tag[(size_t)mi];
+        at.base = base;
+        at.first = ch.first;
+        at.bad = d_bad + mi;
+        at.slot = maps.slot[(size_t)mi];
+        at.frame = 0;
+        if (err == cudaSuccess)
+            err = launch_poly_load(*ctxs[mi]->ctx, cc[(size_t)mi], 0, st.dev[b], ms[(size_t)mi]->d_plain, ch.count, st.stream[b], at);
+    }
+    for (int b = 0; b < 2; ++b) {
+        const cudaError_t e2 = cudaStreamSynchronize(st.stream[b]);
+        if (err == cudaSuccess) err = e2;
+    }
+    if (err == cudaSuccess) err = cudaMemcpy(bad.data(), d_bad, (size_t)count * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
+    cudaFree(d_bad);
+    const auto first_bad = std::find_if(bad.begin(), bad.end(), [](unsigned long long v) { return v != ~0ull; });
+    if (err == cudaSuccess && first_bad == bad.end()) {
+        for (int32_t k = 0; k < count; ++k) out[k] = ms[(size_t)k];
+        return HECUDA_OK;
+    }
+    for (hecuda_pnns_matrix *m : ms) hecuda_pnns_matrix_destroy(m);
+    if (err != cudaSuccess) return cuda_fail(err, "pnns matrices from serialized bytes");
+    const int mi = (int)(first_bad - bad.begin());
+    const int L = ctxs[mi]->ctx->L;
+    const int row = (int)(*first_bad % (unsigned long long)L);
+    return fail(HECUDA_ERR_INVALID_ARGUMENT, "corruptedData(matrix " + std::to_string(mi) + ", plaintext " +
+                                                 std::to_string(*first_bad / (unsigned long long)L) + ", row " +
+                                                 std::to_string(row) + ": a residue is not below q_" + std::to_string(row) +
+                                                 " = " + std::to_string(cc[(size_t)mi].modulus[row]) + ")");
+}
+
+int32_t hecuda_pnns_database_serialized_byte_count(const hecuda_pnns_matrix *const *matrices, int32_t count,
+                                                   const uint64_t *entry_ids, int64_t entry_id_count,
+                                                   const uint8_t *metadata, const uint64_t *metadata_offsets,
+                                                   int64_t metadata_count, const hecuda_pnns_server_config *config,
+                                                   uint64_t *bytes) {
+    if (!bytes) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    pnnsio::Placement pl;
+    std::vector<DiagonalShape> shapes;
+    std::vector<CodecConsts> cc;
+    int32_t rc = serialization_placement(matrices, count, entry_ids, entry_id_count, metadata, metadata_offsets,
+                                         metadata_count, config, pl, shapes, cc);
+    if (rc) return rc;
+    *bytes = (uint64_t)pl.size;
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pnns_database_serialize(const hecuda_pnns_matrix *const *matrices, int32_t count, const uint64_t *entry_ids,
+                                       int64_t entry_id_count, const uint8_t *metadata, const uint64_t *metadata_offsets,
+                                       int64_t metadata_count, const hecuda_pnns_server_config *config, uint8_t *out,
+                                       uint64_t capacity, uint64_t *written) {
+    if (!out || !written) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    *written = 0;
+    pnnsio::Placement pl;
+    std::vector<DiagonalShape> shapes;
+    std::vector<CodecConsts> cc;
+    int32_t rc = serialization_placement(matrices, count, entry_ids, entry_id_count, metadata, metadata_offsets,
+                                         metadata_count, config, pl, shapes, cc);
+    if (rc) return rc;
+    if (capacity < (uint64_t)pl.size)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "capacity " + std::to_string(capacity) + " below the serialized size " +
+                                                     std::to_string(pl.size));
+    // the bytes around the plaintexts come from the host
+    for (const pnnsio::MatrixPlacement &mp : pl.matrices) {
+        memcpy(out + mp.head_at, mp.head.data(), mp.head.size());
+        memcpy(out + mp.tag.back(), mp.tail.data(), mp.tail.size());
+    }
+    memcpy(out + pl.rest_at, pl.rest.data(), pl.rest.size());
+    std::vector<std::vector<long long>> tags;
+    for (const pnnsio::MatrixPlacement &mp : pl.matrices) tags.push_back(mp.tag);
+    long long widest = 0;
+    const std::vector<MatrixChunk> plan = plan_matrix_chunks(tags, widest);
+    const bool pinned = host_pinned(out, (size_t)pl.size);
+    DbStaging st(matrices[0]->owner);
+    if (!st.g0.w || !st.g1.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    DeviceMaps maps;
+    cudaError_t e = cudaSuccess;
+    for (int32_t k = 0; k < count && e == cudaSuccess; ++k) e = maps.add(tags[(size_t)k], file_slots(shapes[(size_t)k]));
+    if (e == cudaSuccess) e = st.init((size_t)widest, !pinned);
+    auto range = [&](size_t k, long long &base) {
+        const dbio::Chunk &ch = plan[k].chunk;
+        const std::vector<long long> &tag = tags[(size_t)plan[k].matrix];
+        base = tag[(size_t)ch.first];
+        return tag[(size_t)(ch.first + ch.count)] - base;
+    };
+    // a pageable `out`: chunk k's pinned bytes are copied out once chunk k + 1 is enqueued
+    auto drain = [&](size_t k) {
+        long long base = 0;
+        const long long size = range(k, base);
+        cudaError_t e2 = cudaEventSynchronize(st.copied[k & 1]);
+        if (e2 == cudaSuccess) memcpy(out + base, st.host[k & 1], (size_t)size);
+        return e2;
+    };
+    for (size_t k = 0; k < plan.size() && e == cudaSuccess; ++k) {
+        const int b = (int)(k & 1), mi = plan[k].matrix;
+        const pnnsio::MatrixPlacement &mp = pl.matrices[(size_t)mi];
+        long long base = 0;
+        const long long size = range(k, base);
+        PolyLayout at;
+        at.tag = maps.tag[(size_t)mi];
+        at.base = base;
+        at.first = plan[k].chunk.first;
+        at.slot = maps.slot[(size_t)mi];
+        at.frame = (int)mp.frame.size();
+        std::copy(mp.frame.begin(), mp.frame.end(), at.frame_bytes);
+        e = launch_poly_serialize(*matrices[mi]->owner->ctx, cc[(size_t)mi], 0, (const u64 *)matrices[mi]->d_plain, st.dev[b],
+                                  plan[k].chunk.count, st.stream[b], at);
+        if (e == cudaSuccess)
+            e = cudaMemcpyAsync(pinned ? out + base : st.host[b], st.dev[b], (size_t)size, cudaMemcpyDeviceToHost, st.stream[b]);
+        if (e == cudaSuccess && !pinned) e = cudaEventRecord(st.copied[b], st.stream[b]);
+        if (e == cudaSuccess && !pinned && k >= 1) e = drain(k - 1);
+    }
+    if (e == cudaSuccess && !pinned && !plan.empty()) e = drain(plan.size() - 1);
+    for (int b = 0; b < 2; ++b) {
+        const cudaError_t e2 = cudaStreamSynchronize(st.stream[b]);
+        if (e == cudaSuccess) e = e2;
+    }
+    if (e != cudaSuccess) return cuda_fail(e, "pnns database serialize");
+    *written = (uint64_t)pl.size;
+    return HECUDA_OK;
+}
+
+}  // extern "C"

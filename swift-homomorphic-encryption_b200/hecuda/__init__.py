@@ -166,6 +166,19 @@ SYMBOLS = {
                                                           C.POINTER(_VP)]),
     "hecuda_pnns_matrix_device_buffer": (C.c_int32, [_VP, C.POINTER(_VP), C.POINTER(C.c_uint64)]),
     "hecuda_pnns_matrix_present": (C.c_int32, [_VP, _VP, C.c_int64]),
+    "hecuda_pnns_server_config_parse": (C.c_int32, [_VP, C.c_uint64, _VP]),
+    "hecuda_pnns_server_config_serialize": (C.c_int32, [_VP, _VP, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "hecuda_pnns_client_config_parse": (C.c_int32, [_VP, C.c_uint64, _VP]),
+    "hecuda_pnns_client_config_serialize": (C.c_int32, [_VP, _VP, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "hecuda_pnns_database_describe": (C.c_int32, [_VP, C.c_uint64, _VP, C.POINTER(C.c_int32), C.POINTER(C.c_int64),
+                                                  C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                                  C.POINTER(C.c_uint64)]),
+    "hecuda_pnns_database_entries": (C.c_int32, [_VP, C.c_uint64, _VP, C.c_int64, _VP, C.c_uint64, _VP, C.c_int64]),
+    "hecuda_pnns_matrices_create_serialized": (C.c_int32, [C.POINTER(_VP), C.c_int32, _VP, C.c_uint64, C.POINTER(_VP)]),
+    "hecuda_pnns_database_serialized_byte_count": (C.c_int32, [C.POINTER(_VP), C.c_int32, _VP, C.c_int64, _VP, _VP,
+                                                               C.c_int64, _VP, C.POINTER(C.c_uint64)]),
+    "hecuda_pnns_database_serialize": (C.c_int32, [C.POINTER(_VP), C.c_int32, _VP, C.c_int64, _VP, _VP, C.c_int64, _VP,
+                                                   _VP, C.c_uint64, C.POINTER(C.c_uint64)]),
     "hecuda_pnns_mul_transpose_vector": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int64, C.c_int32, _VP]),
     "hecuda_pnns_mul_transpose_vector_device": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int64, C.c_int32, _VP, _VP]),
     "hecuda_pnns_mul_transpose_matrix": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int32, C.c_int32, C.POINTER(C.c_int32), _VP,
@@ -224,6 +237,10 @@ SYMBOLS = {
 }
 
 PLAINTEXT_ADD, PLAINTEXT_SUB, PLAINTEXT_SUB_FROM = 0, 1, 2  # HECUDA_PLAINTEXT_* (plaintextTranslate ops)
+# EncryptionParameters.maxLog2CoefficientModulus (EncryptionParameters.swift:192-219) for .quantum128: the largest
+# log2 of the coefficient modulus per degree, for error standard deviation 3.2 and (at N = 2048 only) 6.4
+_MAX_LOG2_Q_STDDEV32 = {1 << 10: 21, 1 << 11: 41, 1 << 12: 83, 1 << 13: 165, 1 << 14: 330, 1 << 15: 660}
+_MAX_LOG2_Q_STDDEV64 = {1 << 11: 42}
 
 _lib = None
 

@@ -571,7 +571,11 @@ class ClientConfig:
 
     def __init__(self, encryptionParameters: EncryptionParameters, scalingFactor: int, vectorDimension: int,
                  evaluationKeyConfig, distanceMetric: str = COSINE_SIMILARITY, extraPlaintextModuli=(),
-                 queryPacking: str = "denseRow"):
+                 queryPacking="denseRow", errorStdDev: float = 3.2, securityLevel: str = "unchecked"):
+        """queryPacking: "denseRow", "denseColumn" or a BabyStepGiantStep (.diagonal).  errorStdDev: 3.2 (.stdDev32) or
+        6.4 (.stdDev64); securityLevel: "unchecked" or "quantum128", which EncryptionParameters.init checks
+        (EncryptionParameters.swift:139-145): insecureEncryptionParameters when log2 of the coefficient modulus exceeds
+        the bound for the degree."""
         p = encryptionParameters
         self.encryptionParameters = [p] + [EncryptionParameters(p.polyDegree, int(t), p.coefficientModuli)
                                            for t in extraPlaintextModuli]
@@ -581,6 +585,17 @@ class ClientConfig:
         self.evaluationKeyConfig = evaluationKeyConfig
         self.distanceMetric = distanceMetric
         self.extraPlaintextModuli = [int(t) for t in extraPlaintextModuli]
+        self.errorStdDev, self.securityLevel = float(errorStdDev), securityLevel
+        _check_security(p, self.errorStdDev, securityLevel)
+
+    def serialize(self) -> bytes:
+        """The ClientConfig protobuf message (PnnsConversion.swift: ClientConfig.proto()), as SwiftProtobuf writes it."""
+        return _serialize_config(load_library().hecuda_pnns_client_config_serialize, _config_struct(self))
+
+    @staticmethod
+    def deserialize(data) -> "ClientConfig":
+        """ClientConfig.native() of a ClientConfig protobuf message, with the reference's refusals."""
+        return _client_config(_parse_config(load_library().hecuda_pnns_client_config_parse, data))
 
     @property
     def plaintextModuli(self):
@@ -623,6 +638,135 @@ class ServerConfig:
 
     def validateContexts(self, contexts):
         self.clientConfig.validateContexts(contexts)
+
+    def serialize(self) -> bytes:
+        """The ServerConfig protobuf message (PnnsConversion.swift: ServerConfig.proto()), as SwiftProtobuf writes it."""
+        return _serialize_config(load_library().hecuda_pnns_server_config_serialize,
+                                 _config_struct(self.clientConfig, self.babyStepGiantStep))
+
+    @staticmethod
+    def deserialize(data) -> "ServerConfig":
+        """ServerConfig.native() of a ServerConfig protobuf message.  Its database packing must be .diagonal, the only
+        one resident here (HeError, unsupported, otherwise)."""
+        return _server_config(_parse_config(load_library().hecuda_pnns_server_config_parse, data))
+
+
+# ---- the configuration messages: hecuda_pnns_server_config, filled and read here; the protobuf bytes are the library's
+_MAX_MODULI, _MAX_EXTRA, _MAX_GALOIS = 32, 7, 64  # HECUDA_PNNS_MAX_*
+_PACKINGS = {"denseRow": 1, "diagonal": 2, "denseColumn": 3}
+_ERR_UNSUPPORTED = -2  # HECUDA_ERR_UNSUPPORTED
+
+
+class _ConfigStruct(C.Structure):  # hecuda_pnns_server_config
+    _fields_ = [("poly_degree", C.c_uint64), ("plaintext_modulus", C.c_uint64), ("coefficient_moduli_count", C.c_int32),
+                ("error_std_dev", C.c_int32), ("coefficient_moduli", C.c_uint64 * _MAX_MODULI),
+                ("security_level", C.c_int32), ("he_scheme", C.c_int32), ("scaling_factor", C.c_uint64),
+                ("query_packing", C.c_int32), ("query_vector_dimension", C.c_uint32), ("query_baby_step", C.c_uint32),
+                ("query_giant_step", C.c_uint32), ("vector_dimension", C.c_uint32), ("galois_element_count", C.c_int32),
+                ("galois_elements", C.c_uint32 * _MAX_GALOIS), ("distance_metric", C.c_int32),
+                ("extra_plaintext_moduli_count", C.c_int32), ("extra_plaintext_moduli", C.c_uint64 * _MAX_EXTRA),
+                ("database_packing", C.c_int32), ("database_vector_dimension", C.c_uint32),
+                ("database_baby_step", C.c_uint32), ("database_giant_step", C.c_uint32)]
+
+
+def _check_security(params: EncryptionParameters, errorStdDev: float, securityLevel: str):
+    from . import _MAX_LOG2_Q_STDDEV32, _MAX_LOG2_Q_STDDEV64
+    if errorStdDev not in (3.2, 6.4):
+        raise PnnsError(f"invalidEncryptionParameters: errorStdDev must be 3.2 (.stdDev32) or 6.4 (.stdDev64), got {errorStdDev}")
+    if securityLevel == "unchecked":
+        return
+    if securityLevel != "quantum128":
+        raise PnnsError(f"invalidEncryptionParameters: securityLevel must be 'unchecked' or 'quantum128', got {securityLevel!r}")
+    table = _MAX_LOG2_Q_STDDEV64 if errorStdDev == 6.4 else _MAX_LOG2_Q_STDDEV32
+    if params.polyDegree not in table:
+        raise PnnsError(f"invalidEncryptionParameters: no quantum128 bound for degree {params.polyDegree}, "
+                        f"errorStdDev {errorStdDev}")
+    log2q = np.float32(0)
+    for q in params.coefficientModuli:  # Float arithmetic, as the reference sums it
+        log2q = np.float32(log2q + np.log2(np.float32(q)))
+    if log2q > np.float32(table[params.polyDegree]):
+        raise PnnsError(f"insecureEncryptionParameters: log2(q) = {float(log2q):.2f} exceeds {table[params.polyDegree]} "
+                        f"for degree {params.polyDegree}")
+
+
+def _set_packing(s, prefix: str, packing):
+    if isinstance(packing, BabyStepGiantStep):
+        setattr(s, prefix + "_packing", 2)
+        setattr(s, prefix + "_vector_dimension", packing.vectorDimension)
+        setattr(s, prefix + "_baby_step", packing.babyStep)
+        setattr(s, prefix + "_giant_step", packing.giantStep)
+    elif packing in ("denseRow", "denseColumn"):
+        setattr(s, prefix + "_packing", _PACKINGS[packing])
+    else:
+        raise PnnsError(f"unknown packing {packing!r}")
+
+
+def _packing(s, prefix: str):
+    kind = getattr(s, prefix + "_packing")
+    if kind == 2:
+        return BabyStepGiantStep(getattr(s, prefix + "_vector_dimension"), getattr(s, prefix + "_baby_step"),
+                                 getattr(s, prefix + "_giant_step"))
+    return {1: "denseRow", 3: "denseColumn"}[kind]
+
+
+def _config_struct(config: ClientConfig, databasePacking: BabyStepGiantStep = None) -> _ConfigStruct:
+    _check_metric(config.distanceMetric)
+    _check_security(config.encryptionParameters[0], config.errorStdDev, config.securityLevel)
+    p = config.encryptionParameters[0]
+    galois = list(config.evaluationKeyConfig.galoisElements)
+    if len(p.coefficientModuli) > _MAX_MODULI or len(config.extraPlaintextModuli) > _MAX_EXTRA or len(galois) > _MAX_GALOIS:
+        raise HeError(_ERR_UNSUPPORTED, "a configuration with more moduli or Galois elements than hecuda_pnns_server_config holds")
+    s = _ConfigStruct()
+    s.poly_degree, s.plaintext_modulus = p.polyDegree, p.plaintextModulus
+    s.coefficient_moduli_count = len(p.coefficientModuli)
+    s.coefficient_moduli[:len(p.coefficientModuli)] = [int(q) for q in p.coefficientModuli]
+    s.error_std_dev = 1 if config.errorStdDev == 6.4 else 0
+    s.security_level = 1 if config.securityLevel == "quantum128" else 0
+    s.he_scheme = 1  # BFV
+    s.scaling_factor = config.scalingFactor
+    _set_packing(s, "query", config.queryPacking)
+    s.vector_dimension = config.vectorDimension
+    s.galois_element_count = len(galois)
+    s.galois_elements[:len(galois)] = [int(g) for g in galois]
+    s.distance_metric = 0  # cosineSimilarity
+    s.extra_plaintext_moduli_count = len(config.extraPlaintextModuli)
+    s.extra_plaintext_moduli[:len(config.extraPlaintextModuli)] = config.extraPlaintextModuli
+    if databasePacking is not None:
+        _set_packing(s, "database", databasePacking)
+    return s
+
+
+def _client_config(s: _ConfigStruct) -> ClientConfig:
+    from .pir import EvaluationKeyConfig
+    params = EncryptionParameters(int(s.poly_degree), int(s.plaintext_modulus),
+                                  tuple(int(q) for q in s.coefficient_moduli[:s.coefficient_moduli_count]))
+    return ClientConfig(params, int(s.scaling_factor), int(s.vector_dimension),
+                        EvaluationKeyConfig([int(g) for g in s.galois_elements[:s.galois_element_count]], False),
+                        COSINE_SIMILARITY, [int(t) for t in s.extra_plaintext_moduli[:s.extra_plaintext_moduli_count]],
+                        _packing(s, "query"), 6.4 if s.error_std_dev == 1 else 3.2,
+                        "quantum128" if s.security_level == 1 else "unchecked")
+
+
+def _server_config(s: _ConfigStruct) -> ServerConfig:
+    packing = _packing(s, "database")
+    if not isinstance(packing, BabyStepGiantStep):
+        raise HeError(_ERR_UNSUPPORTED, f"databasePacking .{packing}: only .diagonal matrices are resident here")
+    return ServerConfig(_client_config(s), packing)
+
+
+def _parse_config(parse, data) -> _ConfigStruct:
+    buf = np.frombuffer(bytes(data) or b"\0", dtype=np.uint8)
+    s = _ConfigStruct()
+    _check(parse(_ptr(buf), len(bytes(data)), C.byref(s)))
+    return s
+
+
+def _serialize_config(serialize, s: _ConfigStruct) -> bytes:
+    size = C.c_uint64(0)
+    _check(serialize(C.byref(s), None, 0, C.byref(size)))
+    out = np.empty(max(1, size.value), dtype=np.uint8)
+    _check(serialize(C.byref(s), _ptr(out), out.size, C.byref(size)))
+    return out[:size.value].tobytes()
 
 
 def _check_metric(metric: str):
@@ -706,6 +850,8 @@ class Client:
 
     def __init__(self, config: ClientConfig, contexts):
         _check_metric(config.distanceMetric)
+        if config.errorStdDev != 3.2:
+            raise HeError(_ERR_UNSUPPORTED, f"errorStdDev {config.errorStdDev}: the device samples errors at 3.2 only")
         config.validateContexts(contexts)
         ts = config.plaintextModuli
         if len(set(ts)) != len(ts):
@@ -824,6 +970,89 @@ class ProcessedDatabase:
         has_metadata = any(len(row.entryMetadata) for row in database.rows)
         return cls(contexts, matrices, [row.entryId for row in database.rows],
                    [bytes(row.entryMetadata) for row in database.rows] if has_metadata else [], serverConfig)
+
+    def _entries(self):
+        ids = np.ascontiguousarray(np.asarray(self.entryIds, dtype=np.uint64)).reshape(-1)
+        meta = [bytes(m) for m in self.entryMetadatas]
+        offsets = np.zeros(len(meta) + 1, dtype=np.uint64)
+        offsets[1:] = np.cumsum([len(m) for m in meta], dtype=np.uint64)
+        blob = np.frombuffer(b"".join(meta) or b"\0", dtype=np.uint8)
+        config = _config_struct(self.serverConfig.clientConfig, self.serverConfig.babyStepGiantStep)
+        handles = (C.c_void_p * len(self.plaintextMatrices))(*[m._h.value for m in self.plaintextMatrices])
+        return (handles, len(self.plaintextMatrices), _ptr(ids) if ids.size else None, ids.size, _ptr(blob), _ptr(offsets),
+                len(meta), C.byref(config)), (ids, blob, offsets, config)
+
+    def serializationByteCount(self) -> int:
+        """The byte count of serialize()."""
+        args, keep = self._entries()
+        size = C.c_uint64(0)
+        _check(load_library().hecuda_pnns_database_serialized_byte_count(*args, C.byref(size)))
+        return size.value
+
+    def _serialize_into(self, out: np.ndarray):
+        args, keep = self._entries()
+        written = C.c_uint64(0)
+        _check(load_library().hecuda_pnns_database_serialize(*args, _ptr(out), out.size, C.byref(written)))
+
+    def serialize(self) -> bytes:
+        """ProcessedDatabase.serialize().proto().serializedData() (ProcessedDatabase.swift:81-88): the
+        SerializedProcessedDatabase protobuf message, byte for byte as SwiftProtobuf writes it.  The plaintexts are
+        packed on the device with their framing (hecuda_pnns_database_serialize)."""
+        out = np.empty(self.serializationByteCount(), dtype=np.uint8)
+        self._serialize_into(out)
+        return out.tobytes()
+
+    def save(self, path) -> None:
+        """serialize(), written straight into the file's pages (the reference's `.binpb` file)."""
+        import os
+        out = np.memmap(path, dtype=np.uint8, mode="w+", shape=(self.serializationByteCount(),))
+        try:
+            self._serialize_into(out)
+            out.flush()
+        except Exception:
+            del out
+            os.remove(path)
+            raise
+
+    @classmethod
+    def load(cls, source, contexts=None) -> "ProcessedDatabase":
+        """ProcessedDatabase(from:contexts:) (ProcessedDatabase.swift:56-75) of a SerializedProcessedDatabase, unpacked on
+        the device (hecuda_pnns_matrices_create_serialized).  source: bytes, a uint8 array, or a path, which is mapped
+        with np.memmap.  Without contexts, one Context per encryption parameters set of the config is created.  Raises
+        HeError with the reference's error names; also where the reference would accept a residue >= its modulus or
+        trap on a truncated buffer."""
+        from .pir import _source_bytes
+        data = _source_bytes(source)
+        buf = data if data.size else np.zeros(1, dtype=np.uint8)
+        lib = load_library()
+        config = _ConfigStruct()
+        matrices, rows, cols, id_count, meta_count = C.c_int32(0), C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        meta_bytes = C.c_uint64(0)
+        _check(lib.hecuda_pnns_database_describe(_ptr(buf), data.size, C.byref(config), C.byref(matrices), C.byref(rows),
+                                                 C.byref(cols), C.byref(id_count), C.byref(meta_count), C.byref(meta_bytes)))
+        serverConfig = _server_config(config)
+        if contexts is None:
+            p = serverConfig.encryptionParameters[0]
+            contexts = [Context(p.polyDegree, list(p.coefficientModuli), t) for t in serverConfig.plaintextModuli]
+        contexts = list(contexts)
+        serverConfig.validateContexts(contexts)
+        handles = (C.c_void_p * len(contexts))()
+        ctxs = (C.c_void_p * len(contexts))(*[c._h.value for c in contexts])
+        _check(lib.hecuda_pnns_matrices_create_serialized(ctxs, len(contexts), _ptr(buf), data.size, handles))
+        ids = np.empty(max(1, id_count.value), dtype=np.uint64)
+        blob = np.empty(max(1, meta_bytes.value), dtype=np.uint8)
+        offsets = np.empty(meta_count.value + 1, dtype=np.uint64)
+        _check(lib.hecuda_pnns_database_entries(_ptr(buf), data.size, _ptr(ids), ids.size, _ptr(blob), blob.size,
+                                                _ptr(offsets), offsets.size))
+        dims = MatrixDimensions(rows.value, cols.value)
+        out = []
+        for ctx, h in zip(contexts, handles):
+            m = PlaintextMatrix.__new__(PlaintextMatrix)
+            m.context, m.dimensions, m.babyStepGiantStep, m._h = ctx, dims, serverConfig.babyStepGiantStep, C.c_void_p(h)
+            m.resultCiphertextCount = -(-rows.value // ctx.degree)
+            out.append(m)
+        metadatas = [blob[int(offsets[k]):int(offsets[k + 1])].tobytes() for k in range(meta_count.value)]
+        return cls(contexts, out, [int(v) for v in ids[:id_count.value]], metadatas, serverConfig)
 
     def validate(self, queryVectors, trials: int = 1) -> ValidationResult:
         """ProcessedDatabase.validate (ProcessedDatabase.swift:91-143), every step on the device."""

@@ -31,15 +31,11 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from . import _check, _ptr, load_library
+from . import _MAX_LOG2_Q_STDDEV32, _MAX_LOG2_Q_STDDEV64, _check, _ptr, load_library
 from .pir import PirError
 
 SEED_BYTES = 32  # NistAes128Ctr.SeedCount
 
-# EncryptionParameters.maxLog2CoefficientModulus (EncryptionParameters.swift:192-219) for .quantum128: the largest
-# log2 of the coefficient modulus per degree, for error standard deviation 3.2 and (at N = 2048 only) 6.4
-_MAX_LOG2_Q_STDDEV32 = {1 << 10: 21, 1 << 11: 41, 1 << 12: 83, 1 << 13: 165, 1 << 14: 330, 1 << 15: 660}
-_MAX_LOG2_Q_STDDEV64 = {1 << 11: 42}
 
 
 class _Params(C.Structure):  # hecuda_simple_pir_params
