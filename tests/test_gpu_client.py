@@ -16,17 +16,13 @@ from hecuda import pir, pnns
 from oracle import client_oracle as co
 from oracle import oracle as orc
 from oracle import pir_oracle as opir
-from test_gpu_evk_wire import read_device
+from rlwe_shapes import read_device, seed
 
 Q8192 = [36028797018652673, 36028797017571329, 36028797017456641, 36028797017276417]  # bench.py C2 moduli
 T_C2 = 557057
 PIR_MODULI = [134176769, 268369921, 268361729]  # n_4096_logq_27_28_28 (EncryptionParameters.swift:346-367)
 PARAMS = [(4096, Q8192, T_C2), (8192, Q8192, T_C2), (4096, PIR_MODULI, 17)]
 IDS = ["n4096-c2", "n8192-c2", "n4096-pir"]
-
-
-def seed(i: int) -> bytes:
-    return random.Random(i).randbytes(32)
 
 
 @pytest.fixture(scope="module", params=PARAMS, ids=IDS)

@@ -15,21 +15,12 @@ import hecuda
 from hecuda import pir
 from oracle import oracle as orc
 from oracle import pir_oracle as opir
+from rlwe_shapes import read_device
 from test_gpu_pir_clients import CONFIGS, GROUP, Setup
 
 TEST_MODULI_BITS = [55, 52, 62, 58]  # TestUtils.testCoefficientModuli for UInt64 (TestUtilities.swift:312-317)
 PIR_MODULI = [134176769, 268369921, 268361729]  # n_4096_logq_27_28_28 (EncryptionParameters.swift:357-367)
 ERR_INVALID_ARGUMENT, ERR_UNSUPPORTED, ERR_MISSING_KEY = -1, -2, -5  # HECUDA_ERR_*
-
-
-def read_device(ptr, nbytes):
-    """Copy `nbytes` of device memory at `ptr` to the host as uint64 words."""
-    import torch
-
-    class Buffer:
-        __cuda_array_interface__ = {"shape": (nbytes // 8,), "typestr": "<i8", "data": (ptr, False), "version": 2}
-
-    return torch.as_tensor(Buffer(), device="cuda").cpu().numpy().view(np.uint64)
 
 
 def seeded_keys(o, key_seed, rng, elements, galois_seed):

@@ -34,11 +34,10 @@ from oracle import client_oracle as co  # noqa: E402
 from oracle import drbg_oracle as drbg  # noqa: E402
 from oracle import oracle as orc  # noqa: E402
 from oracle import pir_oracle as opir  # noqa: E402
+from rlwe_shapes import (MID, NARROW, NARROW_H, SMALL, WIDE, keyed_elements, mixed_moduli, modulus_class,  # noqa: E402
+                         read_device, seed)
 from test_gpu_batched_entry_points import chunk_env, stages  # noqa: E402
 from test_gpu_behz_bounds import both_signs, check_floor, check_multiply  # noqa: E402
-from test_gpu_client import seed  # noqa: E402
-from test_gpu_evk_wire import read_device  # noqa: E402
-from test_gpu_lazy_bounds import NARROW, NARROW_H, MID, SMALL, WIDE, mixed_moduli, modulus_class  # noqa: E402
 from test_lazy_bounds_model import max_lazy_product_count  # noqa: E402
 
 N14, N15 = 1 << 14, 1 << 15
@@ -56,12 +55,6 @@ def shape_moduli(name):
         return N15, orc.generate_primes([55] * 12, False, N15)
     assert name == "D15-mixed"
     return N15, mixed_moduli(N15)
-
-
-def keyed_elements(n):
-    """The Galois elements of every shape's evaluation key: rotate by 1, rotate by -N/4, swap rows."""
-    return [orc.galois_element_rotating_columns(1, n), orc.galois_element_rotating_columns(-(n // 4), n),
-            orc.galois_element_swapping_rows(n)]
 
 
 class Shape:

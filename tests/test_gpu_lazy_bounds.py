@@ -15,6 +15,7 @@ import hecuda
 from hecuda import pir
 from oracle import oracle as orc
 from oracle import pir_oracle as opir
+from rlwe_shapes import MID, NARROW, NARROW_H, SMALL, WIDE, mixed_moduli, modulus_class
 from test_lazy_bounds_model import (U128, constant_target, first_window_sum, ip_plain_model, ks_mac_reduces_high_word,
                                     ks_mac_wraps_without_high_reduction, ks_model, max_lazy_product_count,
                                     saturated_key, tensor_sum_cap)
@@ -299,29 +300,6 @@ def test_mulpir_scan_past_max_terms(bits, entries, entry_size, t, double_bits, c
 
 
 # ------------------------------------------------------------------------------------------------ NTT classes
-SMALL, NARROW, NARROW_H, MID, WIDE = "small", "narrow", "narrow-h", "mid", "wide"
-
-
-def modulus_class(p):
-    """The NTT's butterfly class of a modulus: <= 30 bits, 31-55 (h 2^32 + 1 apart), 56-61, 62."""
-    bits = p.bit_length()
-    if bits <= 30:
-        return SMALL
-    if bits <= 55:
-        return NARROW_H if p % (1 << 32) == 1 else NARROW
-    return MID if bits <= 61 else WIDE
-
-
-def mixed_moduli(n):
-    """[q_0..q_5, q_ks] spanning every class, the 62-bit modulus first so that it is gathered into narrower key-switching
-    rows: 62, 30, 55, h 2^32 + 1, 31, 61 bits, then a 56-bit key-switching modulus."""
-    q = orc.generate_primes([62, 30, 55], False, n)
-    h = (1 << 50) + 1
-    while not orc.is_prime(h) or h in q:
-        h += 1 << 32
-    return q + [h] + orc.generate_primes([31, 61, 56], False, n)
-
-
 def edge_inputs(moduli, n, seed, batch_extra=1):
     """(4 + batch_extra, rows, N): all p - 1, alternating 0 / p - 1, a delta, and uniform rows."""
     rows = len(moduli)
