@@ -149,10 +149,20 @@ def rotate_columns_and_sum(ctx, cts: list, step: int, galois_keys: dict):
     return acc
 
 
-def mul_transpose_vector(ctx: O.Context, plaintexts: list, row_count: int, bsgs: BabyStepGiantStep, ct, galois_keys: dict):
+def plaintexts_to_eval(ctx: O.Context, plaintexts: list, l: int = 0) -> np.ndarray:
+    """The diagonal packing's Coeff plaintexts in Eval format over the first l moduli: (count, l, N)."""
+    return np.stack([ctx.plaintext_to_eval(p, l) for p in plaintexts])
+
+
+def mul_transpose_vector(ctx: O.Context, plaintexts: list, row_count: int, bsgs: BabyStepGiantStep, ct, galois_keys: dict,
+                         eval_rows=None):
     """PlaintextMatrix.mulTranspose(vector:using:) (MatrixMultiplication.swift:131-226).  plaintexts: the diagonal
-    packing in Coeff format; ct: dense-row ciphertext (2, L, N) Coeff.  Returns resultCiphertextCount ciphertexts."""
+    packing in Coeff format; ct: dense-row ciphertext (2, L, N) Coeff.  Returns resultCiphertextCount ciphertexts.
+    eval_rows: optionally the same plaintexts already in Eval format over the ciphertext's moduli (plaintexts_to_eval),
+    so that many calls over one matrix convert it once; `plaintexts` is then not read."""
     n, L = ctx.n, ct.shape[-2]
+    if eval_rows is not None:
+        assert eval_rows.shape[1:] == (L, n)
     states, state = [], ct
     for step in range(bsgs.baby_step):
         states.append(state)
@@ -166,7 +176,10 @@ def mul_transpose_vector(ctx: O.Context, plaintexts: list, row_count: int, bsgs:
         for g in range(bsgs.giant_step):
             count = min(len(states), bsgs.vector_dimension - bsgs.baby_step * g)
             indices = [result_count * (j + bsgs.baby_step * g) + r for j in range(count)]
-            rows = np.stack([ctx.plaintext_to_eval(plaintexts[i], L) for i in indices])
+            if eval_rows is None:
+                rows = np.stack([ctx.plaintext_to_eval(plaintexts[i], L) for i in indices])
+            else:
+                rows = eval_rows[indices]
             ip = ctx.inner_product_plain(rotated[:count], rows[None], None, threads=1)[0]
             to_add.append(np.stack([O.ntt_inverse(n, ctx.q[:L], ip[p]) for p in range(2)]))
         out.append(rotate_columns_and_sum(ctx, to_add, -bsgs.baby_step, galois_keys))

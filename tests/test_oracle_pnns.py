@@ -57,6 +57,9 @@ def test_mul_transpose_vector_is_matrix_vector_product(n, t, bits, rows, cols):
     ct = ctx.encrypt(12, sk, pn.dense_row_vector(ctx, vector))
     result = pn.mul_transpose_vector(ctx, plaintexts, rows, bsgs, ct, keys)
     assert len(result) == pn.dividing_ceil(rows, n)
+    # the Eval rows converted once give the same ciphertexts (and `plaintexts` is then not read)
+    converted = pn.mul_transpose_vector(ctx, None, rows, bsgs, ct, keys, eval_rows=pn.plaintexts_to_eval(ctx, plaintexts))
+    assert all(np.array_equal(a, b) for a, b in zip(converted, result)) and len(converted) == len(result)
     expected = [sum(a * b for a, b in zip(row, vector)) % t for row in matrix]
     got = []
     for ct_out in result:
