@@ -212,6 +212,28 @@ int32_t hecuda_evk_galois_device_buffer(hecuda_evk *evk, uint32_t element, void 
 int32_t hecuda_evk_create_serialized(const hecuda_context *ctx, const uint8_t *relin_poly0, const uint8_t *relin_seeds,
                                      const uint32_t *elements, int32_t element_count, const uint8_t *galois_poly0,
                                      const uint8_t *galois_seeds, hecuda_evk **out);
+/* Many clients' seeded evaluation keys in one call: hecuda_evk_create_serialized for key_count clients that share one
+ * EvaluationKeyConfig (a relinearization key for all or for none, the same elements[]).  With C = (has_relin +
+ * element_count) x L key ciphertexts per key, client j's poly0[j] is C x B bytes and seeds[j] C x 32 bytes, the
+ * relinearization key first and then elements[] in order (hecuda_evk_create_serialized's relin and Galois arrays back
+ * to back).  Each client's bytes stay in the caller's own buffer.  out[j] is an ordinary, independent evaluation key;
+ * the handles may be destroyed in any order, each freeing its own device memory.  A key is one device allocation that
+ * holds its relinearization key (allocated even when has_relin is 0) and its Galois keys.
+ * On the device: one upload of every seed and one DRBG chain launch over all key_count x C seeds, then per group of at
+ * most HECUDA_EVK_LOAD_GROUP keys an upload of the group's poly0 bytes and one expansion launch; the next group's
+ * upload overlaps the current group's expansion.  A group also holds at most HECUDA_EVK_LOAD_GROUP_BYTES of poly0 bytes
+ * (but at least one key), which bounds the staging of contexts with large keys.  So a call makes 1 + groups kernel
+ * launches whatever element_count is, and none when C = 0.  Each poly0[j] is one copy: by DMA directly when it is
+ * pinned (hecuda_host_alloc, hecuda_host_register), through the driver's pinned staging when it is pageable.  The call
+ * returns once every key is written.  Errors as hecuda_evk_create_serialized, plus HECUDA_ERR_INVALID_ARGUMENT for
+ * key_count < 1, null out, and (when C > 0) null poly0 / seeds or a null poly0[j] / seeds[j] ("client <j>: null
+ * argument").  Every argument is checked before anything is allocated or launched; on any error every out[j] is NULL
+ * and nothing is left allocated. */
+#define HECUDA_EVK_LOAD_GROUP 16
+#define HECUDA_EVK_LOAD_GROUP_BYTES (64ull << 20)
+int32_t hecuda_evk_create_serialized_many(const hecuda_context *ctx, int32_t key_count, int32_t has_relin,
+                                          const uint32_t *elements, int32_t element_count, const uint8_t *const *poly0,
+                                          const uint8_t *const *seeds, hecuda_evk **out);
 /* Bfv.applyGalois(ciphertext:element:using:) -- Bfv/Bfv.swift:174-198 (rotateColumns / swapRows call this with
  * GaloisElement.rotatingColumns / swappingRows, HeScheme.swift:1463-1478).  ct, out: batch x 2 x l x N (Coeff). */
 int32_t hecuda_bfv_apply_galois(const hecuda_context *ctx, const hecuda_evk *evk, const uint64_t *ct,

@@ -676,9 +676,12 @@ int32_t hecuda_evk_create(const hecuda_context *h, const uint64_t *relin_key, he
 int32_t hecuda_evk_destroy(hecuda_evk *k) {
     if (!k) return HECUDA_OK;
     if (k->owner) pir_graphs_purge(const_cast<hecuda_context *>(k->owner), k);
-    if (k->d_relin) cudaFree(k->d_relin);
-    for (auto &kv : k->galois) cudaFree(kv.second);
-    for (hecuda::u64 *p : k->retired) cudaFree(p);
+    if (k->d_block) cudaFree(k->d_block);
+    if (k->owns(k->d_relin)) cudaFree(k->d_relin);
+    for (auto &kv : k->galois)
+        if (k->owns(kv.second)) cudaFree(kv.second);
+    for (hecuda::u64 *p : k->retired)
+        if (k->owns(p)) cudaFree(p);
     delete k;
     return HECUDA_OK;
 }
@@ -915,9 +918,131 @@ int32_t hecuda_evk_galois_device_buffer(hecuda_evk *k, uint32_t element, void **
     return HECUDA_OK;
 }
 
-// EvaluationKey(deserialize:context:) (SerializedKeys.swift:141-157) with every key ciphertext .seeded: one DRBG chain
-// pass over all the key's seeds, then one fused kernel that writes poly0 and poly1 of every ciphertext into the key's
-// device buffers (drbg.cu).
+// EvaluationKey(deserialize:context:) (SerializedKeys.swift:141-157) with every key ciphertext .seeded, for one client
+// or many with one EvaluationKeyConfig.  One DRBG chain pass over every seed of the call, then per group of keys the
+// upload of their poly0 bytes and one fused kernel that writes poly0 and poly1 of every ciphertext into the keys'
+// device buffers (drbg.cu); groups alternate between two streams, so a group's upload overlaps the previous group's
+// expansion.
+
+static int32_t check_key_elements(const Context &c, const uint32_t *elements, int32_t element_count) {
+    std::vector<uint32_t> sorted(elements, elements + element_count);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint32_t e : sorted)
+        if (!valid_galois_element(e, c.n)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid Galois element " + std::to_string(e));
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "repeated Galois element " + std::to_string(*std::adjacent_find(sorted.begin(), sorted.end())));
+    return HECUDA_OK;
+}
+
+// One client's wire bytes as two runs of key ciphertexts: [0] the relinearization key's, [1] the Galois keys'.
+// one_buffer: poly0[1] continues poly0[0] in one allocation (a copy must not span two allocations, even adjacent ones).
+struct KeyWire {
+    const uint8_t *poly0[2], *seeds[2];
+    bool one_buffer;
+};
+
+// The device side of load_serialized_keys: cts[p] ciphertexts in run p of every client; ciphertext i of client j
+// (in the order of its runs) lands at dst[j x per_key + i].
+static cudaError_t expand_serialized_keys(const hecuda_context *h, size_t poly_bytes, const int64_t cts[2], int32_t count,
+                                          const KeyWire *wire, const std::vector<u64 *> &dst) {
+    const Context &c = *h->ctx;
+    const int64_t per_key = cts[0] + cts[1], total = per_key * count;
+    const size_t key_bytes = poly_bytes * per_key;
+    const int32_t group = (int32_t)std::max<uint64_t>(
+        1, std::min<uint64_t>(HECUDA_EVK_LOAD_GROUP, HECUDA_EVK_LOAD_GROUP_BYTES / key_bytes));
+    std::vector<unsigned char> seeds((size_t)total * 32);
+    for (int32_t j = 0; j < count; ++j)
+        for (int p = 0; p < 2; ++p)
+            if (cts[p]) memcpy(seeds.data() + 32 * (j * per_key + (p ? cts[0] : 0)), wire[j].seeds[p], 32 * (size_t)cts[p]);
+    DbStaging st(h);
+    if (!st.g0.w || !st.g1.w) return cudaErrorMemoryAllocation;
+    const cudaStream_t s0 = st.stream[0];
+    const int segments = key_segments(c);
+    unsigned char *d_seeds = nullptr;
+    u64 **d_dst = nullptr;
+    unsigned int *d_rk = nullptr;
+    u64 *d_ctr = nullptr;
+    cudaEvent_t chained = nullptr;
+    cudaError_t e = st.init(key_bytes * std::min(group, count), false);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&chained, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_seeds, seeds.size(), s0);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_dst, sizeof(u64 *) * total, s0);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_seeds, seeds.data(), seeds.size(), cudaMemcpyHostToDevice, s0);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_dst, dst.data(), sizeof(u64 *) * total, cudaMemcpyHostToDevice, s0);
+    if (e == cudaSuccess) e = drbg_chains(d_seeds, segments, total, &d_rk, &d_ctr, s0);
+    if (e == cudaSuccess) e = cudaEventRecord(chained, s0);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(st.stream[1], chained, 0);
+    for (int32_t first = 0, g = 0; first < count && e == cudaSuccess; first += group, ++g) {
+        const int b = g & 1;
+        const int32_t keys = std::min(group, count - first);
+        // the group's poly0 bytes into st.dev[b], key after key: one copy per client buffer.  A pinned buffer is copied
+        // by DMA directly; a pageable one through the driver's pinned staging, which returns once the bytes are staged,
+        // so the host moves on to the next group while this group's expansion runs on the other stream.
+        for (int32_t j = first; j < first + keys && e == cudaSuccess; ++j) {
+            unsigned char *at = st.dev[b] + key_bytes * (j - first);
+            if (wire[j].one_buffer) {
+                e = cudaMemcpyAsync(at, wire[j].poly0[0], key_bytes, cudaMemcpyHostToDevice, st.stream[b]);
+                continue;
+            }
+            for (int p = 0; p < 2 && e == cudaSuccess; at += poly_bytes * cts[p++])
+                if (cts[p]) e = cudaMemcpyAsync(at, wire[j].poly0[p], poly_bytes * cts[p], cudaMemcpyHostToDevice, st.stream[b]);
+        }
+        if (e == cudaSuccess)
+            e = expand_key_ciphertexts(c, d_rk, d_ctr, first * per_key, keys * per_key, st.dev[b], d_dst, st.stream[b]);
+    }
+    // the chains are zeroized and freed once both streams' expansions have read them; the keys are read on other
+    // non-blocking streams, so return once they are written (see upload())
+    cudaError_t e2 = wait_stream(st.stream[1]);
+    if (e == cudaSuccess) e = e2;
+    free_chains(d_rk, d_ctr, segments, total, s0);
+    for (void *p : {(void *)d_seeds, (void *)d_dst})
+        if (p) cudaFreeAsync(p, s0);
+    e2 = wait_stream(s0);
+    if (e == cudaSuccess) e = e2;
+    if (chained) cudaEventDestroy(chained);
+    return e;
+}
+
+// `count` clients' keys of one config, every argument already checked: one allocation per key, then the expansion.
+// On error nothing is left allocated and out[] is untouched.
+static int32_t load_serialized_keys(const hecuda_context *h, uint64_t poly_bytes, int32_t count, bool relin,
+                                    const uint32_t *elements, int32_t element_count, const KeyWire *wire, hecuda_evk **out) {
+    const Context &c = *h->ctx;
+    const size_t words = (size_t)c.L * 2 * (c.L + 1) * c.n, ct_words = words / c.L;
+    const int64_t cts[2] = {relin ? c.L : 0, (int64_t)element_count * c.L};
+    std::vector<hecuda_evk *> keys;
+    // ciphertext i of a key lands at key + i x 2 x K x N: its relinearization key, then galois[elements[e]]
+    std::vector<u64 *> dst;
+    dst.reserve((size_t)(cts[0] + cts[1]) * count);
+    cudaError_t e = cudaSuccess;
+    for (int32_t j = 0; j < count && e == cudaSuccess; ++j) {
+        hecuda_evk *k = new (std::nothrow) hecuda_evk();
+        if (!k) {
+            e = cudaErrorMemoryAllocation;
+            break;
+        }
+        keys.push_back(k);
+        k->owner = h;
+        k->words = words;
+        k->block_words = words * (1 + (size_t)element_count);  // d_relin is allocated even without a relinearization key
+        if ((e = cudaMalloc(&k->d_block, k->block_words * sizeof(u64))) != cudaSuccess) break;
+        k->d_relin = k->d_block;
+        for (int32_t g = relin ? -1 : 0; g < element_count; ++g) {
+            u64 *key = k->d_block + words * (1 + g);
+            if (g >= 0) k->galois[elements[g]] = key;
+            for (int i = 0; i < c.L; ++i) dst.push_back(key + ct_words * i);
+        }
+        k->loaded = relin;
+    }
+    if (e == cudaSuccess && !dst.empty()) e = expand_serialized_keys(h, (size_t)poly_bytes, cts, count, wire, dst);
+    if (e != cudaSuccess) {
+        for (hecuda_evk *k : keys) hecuda_evk_destroy(k);
+        return cuda_fail(e, "evk_create_serialized");
+    }
+    std::copy(keys.begin(), keys.end(), out);
+    return HECUDA_OK;
+}
+
 int32_t hecuda_evk_create_serialized(const hecuda_context *h, const uint8_t *relin_poly0, const uint8_t *relin_seeds,
                                      const uint32_t *elements, int32_t element_count, const uint8_t *galois_poly0,
                                      const uint8_t *galois_seeds, hecuda_evk **out) {
@@ -932,67 +1057,39 @@ int32_t hecuda_evk_create_serialized(const hecuda_context *h, const uint8_t *rel
         return fail(HECUDA_ERR_INVALID_ARGUMENT, "relin_poly0 and relin_seeds must both be given or both be null");
     if (element_count < 0 || (element_count > 0 && (!elements || !galois_poly0 || !galois_seeds)))
         return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
-    std::vector<uint32_t> sorted(elements, elements + element_count);
-    std::sort(sorted.begin(), sorted.end());
-    for (uint32_t e : sorted)
-        if (!valid_galois_element(e, c.n)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalid Galois element " + std::to_string(e));
-    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
-        return fail(HECUDA_ERR_INVALID_ARGUMENT, "repeated Galois element " + std::to_string(*std::adjacent_find(sorted.begin(), sorted.end())));
+    if ((rc = check_key_elements(c, elements, element_count))) return rc;
     uint64_t poly_bytes = 0;
     if ((rc = hecuda_poly_serialized_byte_count(h, HECUDA_BASE_KEYSWITCH, c.L + 1, 0, &poly_bytes))) return rc;
-    const bool relin = relin_poly0 != nullptr;
-    const int64_t count = (int64_t)(relin + element_count) * c.L;  // key ciphertexts
-    hecuda_evk *k = nullptr;
-    if ((rc = hecuda_evk_create_empty(h, &k))) return rc;
-    // ciphertext i of key j lands at key_j + i x 2 x K x N: the relinearization key, then galois[elements[e]]
-    std::vector<u64 *> dst;
-    dst.reserve((size_t)count);
-    const size_t ct_words = k->words / c.L;
-    cudaError_t e = cudaSuccess;
-    for (int32_t j = -1; j < element_count && e == cudaSuccess; ++j) {
-        u64 *key = nullptr;
-        if (j < 0) {
-            if (!relin) continue;
-            key = k->d_relin;
-        } else if ((e = cudaMalloc(&key, k->words * sizeof(u64))) == cudaSuccess) {
-            k->galois[elements[j]] = key;
-        }
-        for (int i = 0; key && i < c.L; ++i) dst.push_back(key + ct_words * i);
+    const KeyWire wire{{relin_poly0, galois_poly0}, {relin_seeds, galois_seeds}, false};
+    return load_serialized_keys(h, poly_bytes, 1, relin_poly0 != nullptr, elements, element_count, &wire, out);
+}
+
+int32_t hecuda_evk_create_serialized_many(const hecuda_context *h, int32_t key_count, int32_t has_relin,
+                                          const uint32_t *elements, int32_t element_count, const uint8_t *const *poly0,
+                                          const uint8_t *const *seeds, hecuda_evk **out) {
+    if (!out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (key_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "key_count " + std::to_string(key_count) + ": expected at least 1");
+    std::fill(out, out + key_count, nullptr);
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    if (!c.has_ks)
+        return fail(HECUDA_ERR_UNSUPPORTED, "unsupportedHeOperation: a single coefficient modulus leaves no key-switching modulus");
+    if (element_count < 0) return fail(HECUDA_ERR_INVALID_ARGUMENT, "element_count " + std::to_string(element_count) + " < 0");
+    if (element_count > 0 && !elements) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if ((rc = check_key_elements(c, elements, element_count))) return rc;
+    uint64_t poly_bytes = 0;
+    if ((rc = hecuda_poly_serialized_byte_count(h, HECUDA_BASE_KEYSWITCH, c.L + 1, 0, &poly_bytes))) return rc;
+    const bool relin = has_relin != 0;
+    const bool any = relin || element_count > 0;
+    if (any && (!poly0 || !seeds)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    const size_t relin_cts = relin ? (size_t)c.L : 0;
+    std::vector<KeyWire> wire((size_t)key_count, KeyWire{{nullptr, nullptr}, {nullptr, nullptr}, true});
+    for (int32_t j = 0; any && j < key_count; ++j) {
+        if (!poly0[j] || !seeds[j]) return fail(HECUDA_ERR_INVALID_ARGUMENT, "client " + std::to_string(j) + ": null argument");
+        wire[(size_t)j] = KeyWire{{poly0[j], poly0[j] + poly_bytes * relin_cts}, {seeds[j], seeds[j] + 32 * relin_cts}, true};
     }
-    if (e == cudaSuccess && count > 0) {
-        WsGuard g(h);
-        if (!g.w) {
-            hecuda_evk_destroy(k);
-            return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
-        }
-        cudaStream_t s = g.w->stream;
-        const size_t relin_cts = relin ? (size_t)c.L : 0, galois_cts = (size_t)element_count * c.L;
-        unsigned char *d_poly0 = nullptr, *d_seeds = nullptr;
-        u64 **d_dst = nullptr;
-        e = cudaMallocAsync((void **)&d_poly0, poly_bytes * count, s);
-        if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_seeds, (size_t)32 * count, s);
-        if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_dst, sizeof(u64 *) * count, s);
-        if (e == cudaSuccess && relin) e = cudaMemcpyAsync(d_poly0, relin_poly0, poly_bytes * relin_cts, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess && relin) e = cudaMemcpyAsync(d_seeds, relin_seeds, 32 * relin_cts, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess && galois_cts)
-            e = cudaMemcpyAsync(d_poly0 + poly_bytes * relin_cts, galois_poly0, poly_bytes * galois_cts, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess && galois_cts)
-            e = cudaMemcpyAsync(d_seeds + 32 * relin_cts, galois_seeds, 32 * galois_cts, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_dst, dst.data(), sizeof(u64 *) * count, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess) e = expand_seeded_keys_device(c, d_poly0, d_seeds, d_dst, count, s);
-        for (void *p : {(void *)d_poly0, (void *)d_seeds, (void *)d_dst})
-            if (p) cudaFreeAsync(p, s);
-        // the keys are read on other non-blocking streams: return once the kernel has written them (see upload())
-        const cudaError_t e2 = wait_stream(s);
-        if (e == cudaSuccess) e = e2;
-    }
-    if (e != cudaSuccess) {
-        hecuda_evk_destroy(k);
-        return cuda_fail(e, "evk_create_serialized");
-    }
-    k->loaded = relin;
-    *out = k;
-    return HECUDA_OK;
+    return load_serialized_keys(h, poly_bytes, key_count, relin, elements, element_count, wire.data(), out);
 }
 
 static int32_t bfv_apply_galois(const hecuda_context *h, const hecuda_evk *k, const void *ct, int32_t l, uint32_t element,

@@ -122,6 +122,11 @@ struct hecuda_evk {
     bool loaded = false;
     std::map<uint32_t, hecuda::u64 *> galois;  // GaloisKey.keys: element -> key-switch key (Keys.swift:150-163), same layout
     std::vector<hecuda::u64 *> retired;        // replaced Galois keys, kept until destroy (in-flight kernels may read them)
+    // hecuda_evk_create_serialized(_many): one allocation holding d_relin and the loaded Galois keys.  Pointers into it
+    // are freed with it, never on their own; d_relin, galois and retired entries outside it are separate allocations.
+    hecuda::u64 *d_block = nullptr;
+    size_t block_words = 0;
+    bool owns(const hecuda::u64 *p) const { return p && !(p >= d_block && p < d_block + block_words); }
     std::mutex mu;
 };
 
@@ -209,10 +214,13 @@ cudaError_t apply_galois_chunk(const Context &c, u64 *scratch, const u64 *key, c
                                u64 *out, int64_t items, cudaStream_t s, const KsKeyTable *keys = nullptr);
 cudaError_t expand_seeded_device(const Context &c, int l, const unsigned char *d_poly0, const unsigned char *d_seeds, u64 *d_out,
                                  int64_t batch, cudaStream_t s);
-// `count` seeded key-switching ciphertexts (K = L + 1 rows, Eval): d_poly0 count x byteCount(K rows) bytes, d_seeds
-// count x 32; ciphertext i's 2 x K x N words go to d_dst[i] (a device table of pointers into evaluation keys)
-cudaError_t expand_seeded_keys_device(const Context &c, const unsigned char *d_poly0, const unsigned char *d_seeds,
-                                      u64 *const *d_dst, int64_t count, cudaStream_t s);
+// Seeded key-switching ciphertexts (K = L + 1 rows, Eval) in two steps: drbg_chains over their seeds with
+// key_segments(c) segments each, then ciphertexts [first, first + count) from those chains: d_poly0 holds their
+// count x byteCount(K rows) bytes, and ciphertext i's 2 x K x N words go to d_dst[i] (a device table of pointers into
+// evaluation keys)
+int key_segments(const Context &c);
+cudaError_t expand_key_ciphertexts(const Context &c, const unsigned int *d_rk, const u64 *d_ctr, int64_t first, int64_t count,
+                                   const unsigned char *d_poly0, u64 *const *d_dst, cudaStream_t s);
 // NistAes128Ctr streams (drbg.cu): the AES tables, then for every 32-byte seed the round keys (segments x 44 words) and
 // counters V (segments x 2 words) of its first `segments` 4096-byte segments; free_chains zeroizes the round keys.
 cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, unsigned int **d_rk, u64 **d_ctr,

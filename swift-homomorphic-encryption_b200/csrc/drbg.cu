@@ -276,26 +276,24 @@ cudaError_t expand_seeded_device(const Context &c, int l, const unsigned char *d
     return e;
 }
 
-cudaError_t expand_seeded_keys_device(const Context &c, const unsigned char *d_poly0, const unsigned char *d_seeds,
-                                      u64 *const *d_dst, int64_t count, cudaStream_t s) {
+int key_segments(const Context &c) {
+    return (int)(((size_t)(c.L + 1) * c.n * 16 + kSegmentBytes - 1) / kSegmentBytes);
+}
+
+cudaError_t expand_key_ciphertexts(const Context &c, const u32w *d_rk, const u64 *d_ctr, int64_t first, int64_t count,
+                                   const unsigned char *d_poly0, u64 *const *d_dst, cudaStream_t s) {
     const NttRowMap map = c.map_ks(c.L);  // row K-1 is q_ks
     CodecConsts cc;
     std::string err;
     if (!codec_consts(c, map, 0, cc, err)) return cudaErrorInvalidValue;
-    const int rows = c.L + 1;
-    const int segments = (int)(((size_t)rows * c.n * 16 + kSegmentBytes - 1) / kSegmentBytes);
-    u32w *d_rk = nullptr;
-    u64 *d_ctr = nullptr;
-    cudaError_t e = drbg_chains(d_seeds, segments, count, &d_rk, &d_ctr, s);
+    const int segments = key_segments(c);
     const RowModuli fc = row_moduli(c, map);
-    if (e == cudaSuccess)
-        e = for_each_part(count, [&](int64_t done, int64_t part) {
-            return launch(key_expand_kernel, dim3((unsigned)segments, (unsigned)part), kSegmentBlocks, 0, s,
-                          d_rk + (size_t)done * segments * kRoundKeyWords, d_ctr + (size_t)done * segments * 2,
-                          d_poly0 + (size_t)done * serialized_poly_bytes(cc), d_dst + done, fc, cc, (int)c.n, segments);
-        });
-    free_chains(d_rk, d_ctr, segments, count, s);
-    return e;
+    return for_each_part(count, [&](int64_t done, int64_t part) {
+        const size_t at = (size_t)(first + done) * segments;
+        return launch(key_expand_kernel, dim3((unsigned)segments, (unsigned)part), kSegmentBlocks, 0, s,
+                      d_rk + at * kRoundKeyWords, d_ctr + at * 2, d_poly0 + (size_t)done * serialized_poly_bytes(cc),
+                      d_dst + first + done, fc, cc, (int)c.n, segments);
+    });
 }
 
 }  // namespace api

@@ -87,6 +87,7 @@ SYMBOLS = {
     "hecuda_evk_set_galois_key": (C.c_int32, [_VP, C.c_uint32, _VP]),
     "hecuda_evk_galois_device_buffer": (C.c_int32, [_VP, C.c_uint32, C.POINTER(_VP), C.POINTER(C.c_uint64)]),
     "hecuda_evk_create_serialized": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int32, _VP, _VP, C.POINTER(_VP)]),
+    "hecuda_evk_create_serialized_many": (C.c_int32, [_VP, C.c_int32, C.c_int32, _VP, C.c_int32, _VP, _VP, _VP]),
     "hecuda_bfv_apply_galois": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_uint32, _VP, C.c_int64]),
     "hecuda_bfv_apply_galois_device": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_uint32, _VP, C.c_int64, _VP]),
     "hecuda_poly_apply_galois": (C.c_int32, [_VP, C.c_int32, C.c_int32, _VP, _VP, C.c_int32, C.c_int64, C.c_uint32]),
@@ -482,17 +483,7 @@ class EvaluationKey:
         are expanded and poly0 unpacked on the device (hecuda_evk_create_serialized).  relinPoly0: (L, B) uint8 and
         relinSeeds: (L, 32) uint8, B = Bfv.serializationByteCount(context, L + 1, base=BASE_KEYSWITCH), or both None;
         galois: {element: (poly0 (L, B) uint8, seeds (L, 32) uint8)}."""
-        L = context.L
-        size = Bfv.serializationByteCount(context, L + 1, base=BASE_KEYSWITCH)
-
-        def arrays(poly0, seeds):
-            p = np.ascontiguousarray(np.asarray(poly0, dtype=np.uint8))
-            s = np.ascontiguousarray(np.asarray(seeds, dtype=np.uint8))
-            if p.size != L * size or s.size != L * 32:
-                raise HeError(-1, f"serializedBufferSizeMismatch(poly0: {p.size} bytes, seeds: {s.size} bytes, expected "
-                                  f"{L * size} and {L * 32})")
-            return p, s
-
+        arrays = cls._wireArrays(context)
         relin = None
         if relinPoly0 is not None or relinSeeds is not None:
             if relinPoly0 is None or relinSeeds is None:
@@ -512,6 +503,67 @@ class EvaluationKey:
         key = cls.__new__(cls)
         key.context, key.galoisElements, key._h = context, elements, h
         return key
+
+    @staticmethod
+    def _wireArrays(context: Context):
+        """The check of one seeded key's wire arrays: poly0 (L, B) and seeds (L, 32) uint8, returned contiguous."""
+        L = context.L
+        size = Bfv.serializationByteCount(context, L + 1, base=BASE_KEYSWITCH)
+
+        def arrays(poly0, seeds):
+            p = np.ascontiguousarray(np.asarray(poly0, dtype=np.uint8))
+            s = np.ascontiguousarray(np.asarray(seeds, dtype=np.uint8))
+            if p.size != L * size or s.size != L * 32:
+                raise HeError(-1, f"serializedBufferSizeMismatch(poly0: {p.size} bytes, seeds: {s.size} bytes, expected "
+                                  f"{L * size} and {L * 32})")
+            return p, s
+
+        return arrays
+
+    @classmethod
+    def fromSerializedMany(cls, context: Context, forms) -> list:
+        """fromSerialized for many clients in one call (hecuda_evk_create_serialized_many): one DRBG chain pass over
+        every client's seeds, then the expansion in groups of HECUDA_EVK_LOAD_GROUP keys.  forms: one dict per client,
+        as generate(..., wire=True) returns it ({"relinPoly0", "relinSeeds", "galois": {element: (poly0, seeds)}}).
+        Every client must have the same configuration: a relinearization key for all or none, and the same Galois
+        elements (in any order).  Returns one independent EvaluationKey per client."""
+        forms = list(forms)
+        if not forms:
+            raise HeError(-1, "fromSerializedMany: no keys to load")
+        arrays = cls._wireArrays(context)
+
+        def has_relin(f):
+            return f.get("relinPoly0") is not None or f.get("relinSeeds") is not None
+
+        relin = has_relin(forms[0])
+        elements = [int(e) for e in (forms[0].get("galois") or {})]
+        poly0, seeds = [], []
+        for j, f in enumerate(forms):
+            galois = {int(e): v for e, v in (f.get("galois") or {}).items()}
+            if has_relin(f) != relin:
+                raise HeError(-1, f"client {j}: relinearization key {'present' if not relin else 'absent'}, unlike client 0")
+            if relin and (f.get("relinPoly0") is None or f.get("relinSeeds") is None):
+                raise HeError(-1, f"client {j}: relinPoly0 and relinSeeds must both be given or both be None")
+            if sorted(galois) != sorted(elements):
+                raise HeError(-1, f"client {j}: Galois elements {sorted(galois)} differ from client 0's {sorted(elements)}")
+            keys = [arrays(f.get("relinPoly0"), f.get("relinSeeds"))] if relin else []
+            keys += [arrays(*galois[e]) for e in elements]
+            # one buffer per client, in the key-ciphertext order of the call: the relinearization key, then elements
+            poly0.append(np.ascontiguousarray(np.concatenate([k[0].reshape(-1) for k in keys])) if keys else None)
+            seeds.append(np.ascontiguousarray(np.concatenate([k[1].reshape(-1) for k in keys])) if keys else None)
+        K = len(forms)
+        elems = np.ascontiguousarray(elements, dtype=np.uint32)
+        handles = (C.c_void_p * K)()
+        _check(load_library().hecuda_evk_create_serialized_many(
+            context._h, K, int(relin), _ptr(elems) if elements else None, len(elements),
+            (C.c_void_p * K)(*[p.ctypes.data if p is not None else None for p in poly0]),
+            (C.c_void_p * K)(*[s.ctypes.data if s is not None else None for s in seeds]), handles))
+        out = []
+        for h in handles:
+            key = cls.__new__(cls)
+            key.context, key.galoisElements, key._h = context, list(elements), C.c_void_p(h)
+            out.append(key)
+        return out
 
     @classmethod
     def generate(cls, context: Context, config, secretKey, wire: bool = False, aSeeds=None, errorSeeds=None):
