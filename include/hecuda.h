@@ -740,6 +740,84 @@ int32_t hecuda_mulpir_compute_response_clients_wire(const hecuda_context *ctx, c
                                                     int32_t indices_count, int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1,
                                                     uint8_t *out);
 
+/* ---- PIR in the reference's protobuf messages (pir_proto.hpp) ----
+ * Requests as the reference's clients send them and responses as they expect them: pir.v1.EncryptedIndices
+ * (PirConversion.swift:23-53), v1.SerializedEvaluationKey (ConversionHe.swift) and api.pir.v1.PIRResponse
+ * (PirConversionApi.swift:20-49).  A host walk of each message finds its payloads (refusing groups, varints over 10
+ * bytes, lengths past their message, a singular message given twice and a known field of the wrong wire type); the
+ * message then crosses PCIe as it is and the kernels read poly0 and the seeds in place.
+ *
+ * hecuda_pir_request_fields: the walk of an api.pir.v1.PIRRequest (host only, nothing copied): its scalar fields, and
+ * the byte ranges (offsets into `bytes`) of the query (an EncryptedIndices), of evaluation_key.evaluation_key (a
+ * SerializedEvaluationKey), of the configuration hash, the shard id and the key identifier.  The key metadata is
+ * evaluation_key_metadata, or evaluation_key.metadata when that is absent.  Routing by shard and caching keys by
+ * identifier stay the caller's. */
+typedef struct hecuda_pir_request_fields {
+    uint32_t shard_index;
+    int32_t has_shard_id, has_query, has_evaluation_key, has_key_metadata;
+    uint64_t shard_id_offset, shard_id_bytes;
+    uint64_t configuration_hash_offset, configuration_hash_bytes;
+    uint64_t query_offset, query_bytes;
+    uint64_t evaluation_key_offset, evaluation_key_bytes;
+    uint64_t key_timestamp, key_identifier_offset, key_identifier_bytes;
+} hecuda_pir_request_fields;
+int32_t hecuda_pir_request_fields_read(const uint8_t *bytes, uint64_t byte_count, hecuda_pir_request_fields *out);
+
+/* EvaluationKey(deserialize:) of key_count clients' SerializedEvaluationKey messages (message j: message_byte_counts[j]
+ * bytes), as hecuda_evk_create_serialized_many does for the same payloads: the galois_key map (uint64 element ->
+ * SerializedKeySwitchKey of L ciphertexts, entries in any order) and the optional relin_key.  Every key ciphertext must
+ * be .seeded (HECUDA_ERR_UNSUPPORTED for .full keys, which the reference's key generation does not write).  Every
+ * client must resolve to client 0's configuration: a relinearization key for all or none, and the same set of Galois
+ * elements in any map order; a repeated element is refused.  Every message is walked and checked before anything is
+ * allocated; failures name the client ("client <j>: ").  On the device: one upload of all the messages, one DRBG chain
+ * launch over every seed read in place, and one expansion launch.  On any error every out[j] is NULL and nothing is
+ * left allocated. */
+int32_t hecuda_evk_create_proto_many(const hecuda_context *ctx, int32_t key_count, const uint8_t *const *messages,
+                                     const uint64_t *message_byte_counts, hecuda_evk **out);
+
+/* The size of one client's PIRResponse for indices_count replies of chunk_count ciphertexts, each
+ * SerializedCiphertext.full { polys = UInt16 2, poly 0 and poly 1 packed with skip_lsbs_poly0 / skip_lsbs_poly1 dropped
+ * bits, skip_lsbs = [skip0, skip1], correction_factor = 1 }: Response.proto() as SwiftProtobuf writes it. */
+int32_t hecuda_mulpir_response_proto_byte_count(const hecuda_context *ctx, int32_t chunk_count, int32_t indices_count,
+                                                int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1, uint64_t *bytes);
+
+/* hecuda_mulpir_compute_response_clients_wire with one EncryptedIndices message per client in (message c:
+ * message_byte_counts[c] bytes) and one PIRResponse per client out: out is client_count x
+ * hecuda_mulpir_response_proto_byte_count bytes and client c's slice is a complete PIRResponse whose poly bytes are the
+ * bytes hecuda_mulpir_compute_response_clients_wire returns for the same poly0 and seeds.  A query ciphertext may be
+ * .seeded or .full (two polys over L rows with their skip bits, correction factor 1; any other correction factor is
+ * HECUDA_ERR_UNSUPPORTED).  num_pir_calls must equal indices_count, and the ciphertext count must be the one the
+ * parameter's expansion takes (hecuda_mulpir_compute_response's refusals).  Every client is walked and checked before
+ * anything is enqueued; a failure's message starts with "client <c>: " and leaves `out` untouched.  Per group of
+ * HECUDA_MULPIR_CLIENT_GROUP clients: one upload of the group's messages, one seeded expansion reading them in place,
+ * the many-clients response pipeline, one framing launch and one packing launch per reply poly, written straight into
+ * the clients' PIRResponse bytes. */
+int32_t hecuda_mulpir_compute_response_clients_proto(const hecuda_context *ctx, const hecuda_evk *const *evks,
+                                                     int32_t client_count, const hecuda_pir_database *const *databases,
+                                                     int32_t database_count, const int32_t *dimensions,
+                                                     int32_t dimension_count, int32_t chunk_count,
+                                                     const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                                                     int32_t indices_count, int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1,
+                                                     uint8_t *out);
+
+/* Client side, host only.  hecuda_pir_encrypted_indices_write: Query.proto() of ciphertext_count .seeded ciphertexts
+ * (poly0: ciphertext_count x byteCount(L rows), seeds: ciphertext_count x 32) with num_pir_calls = indices_count; with
+ * out NULL only *written is set to the size, else HECUDA_ERR_INVALID_ARGUMENT when capacity is below it.
+ * hecuda_pir_evaluation_key_write: SerializedEvaluationKey.proto() of a seeded key in the arrays of
+ * hecuda_evk_create_serialized (relin_poly0 / relin_seeds NULL: no relinearization key), map entries in elements[]
+ * order.  hecuda_pir_response_read: the offsets in a PIRResponse of every reply ciphertext's poly 0 (poly 1 follows it),
+ * poly_offsets[indices_count x chunk_count], refused unless it holds that many .full ciphertexts with the given skip bits
+ * and one-modulus sizes. */
+int32_t hecuda_pir_encrypted_indices_write(const hecuda_context *ctx, const uint8_t *poly0, const uint8_t *seeds,
+                                           int32_t ciphertext_count, int32_t indices_count, uint8_t *out, uint64_t capacity,
+                                           uint64_t *written);
+int32_t hecuda_pir_evaluation_key_write(const hecuda_context *ctx, const uint8_t *relin_poly0, const uint8_t *relin_seeds,
+                                        const uint32_t *elements, int32_t element_count, const uint8_t *galois_poly0,
+                                        const uint8_t *galois_seeds, uint8_t *out, uint64_t capacity, uint64_t *written);
+int32_t hecuda_pir_response_read(const hecuda_context *ctx, const uint8_t *bytes, uint64_t byte_count, int32_t chunk_count,
+                                 int32_t indices_count, int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1,
+                                 uint64_t *poly_offsets);
+
 /* ---- PNNS server: encrypted vector x plaintext matrix (SURVEY.md section 8f, rank 3) ----
  * Device-resident PlaintextMatrix in `.diagonal(babyStepGiantStep:)` packing (PrivateNearestNeighborSearch/
  * PlaintextMatrix.swift:417-482): nextPowerOfTwo(column_count) * ceil(row_count / N) plaintexts in the order the

@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "capi_internal.hpp"
+#include "pir_proto.hpp"
 
 namespace hecuda {
 std::atomic<unsigned long long> g_kernel_launches{0};
@@ -1003,10 +1004,74 @@ static cudaError_t expand_serialized_keys(const hecuda_context *h, size_t poly_b
     return e;
 }
 
-// `count` clients' keys of one config, every argument already checked: one allocation per key, then the expansion.
-// On error nothing is left allocated and out[] is untouched.
+// SerializedEvaluationKey messages, walked (pirproto::walk_evaluation_key): every message goes to the device as it is,
+// one DRBG chain launch covers every seed and one expansion launch every ciphertext, both reading them in place.
+// Ciphertext i of client j in message order lands at dst[j x per_key + canonical index] (the relinearization key, then
+// elements[] in order).
+struct KeyMessages {
+    const uint8_t *const *messages;
+    const uint64_t *byte_counts;
+    std::vector<pirproto::EvaluationKey> keys;
+};
+
+static cudaError_t expand_proto_keys(const hecuda_context *h, const KeyMessages &km, const uint32_t *elements,
+                                     int32_t element_count, bool relin, const std::vector<u64 *> &dst) {
+    const Context &c = *h->ctx;
+    const int32_t count = (int32_t)km.keys.size();
+    const int64_t per_key = (int64_t)(relin ? c.L : 0) + (int64_t)element_count * c.L, total = per_key * count;
+    std::vector<u64 *> ordered((size_t)total);
+    std::vector<long long> tables((size_t)total * 2);  // poly0 offsets, then seed offsets, into the uploaded messages
+    size_t bytes = 0;
+    for (int32_t j = 0; j < count; ++j) {
+        const pirproto::EvaluationKey &k = km.keys[(size_t)j];
+        for (size_t m = 0; m < k.order.size(); ++m) {
+            const int key = k.order[m].first, i = k.order[m].second;
+            const pirproto::Ciphertext &ct = key < 0 ? k.relin_cts[(size_t)i] : k.galois[(size_t)key].cts[(size_t)i];
+            int64_t canonical = i;
+            if (key >= 0) {
+                const int32_t g = (int32_t)(std::find(elements, elements + element_count, (uint32_t)k.galois[(size_t)key].element) - elements);
+                canonical = (relin ? c.L : 0) + (int64_t)g * c.L + i;
+            }
+            const size_t at = (size_t)(j * per_key) + m;
+            ordered[at] = dst[(size_t)(j * per_key + canonical)];
+            tables[at] = (long long)bytes + ct.poly[0];
+            tables[(size_t)total + at] = (long long)bytes + ct.seed;
+        }
+        bytes += km.byte_counts[j];
+    }
+    WsGuard g(h);
+    if (!g.w) return cudaErrorMemoryAllocation;
+    const cudaStream_t s = g.w->stream;
+    const int segments = key_segments(c);
+    unsigned char *d_msg = nullptr;
+    long long *d_tables = nullptr;
+    u64 **d_dst = nullptr;
+    unsigned int *d_rk = nullptr;
+    u64 *d_ctr = nullptr;
+    cudaError_t e = cudaMallocAsync((void **)&d_msg, std::max<size_t>(bytes, 1), s);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_tables, tables.size() * sizeof(long long), s);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_dst, sizeof(u64 *) * total, s);
+    // each message is one copy: by DMA directly when it is pinned, through the driver's pinned staging when pageable
+    for (size_t j = 0, offset = 0; j < (size_t)count && e == cudaSuccess; offset += km.byte_counts[j++])
+        e = cudaMemcpyAsync(d_msg + offset, km.messages[j], km.byte_counts[j], cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_tables, tables.data(), tables.size() * sizeof(long long), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_dst, ordered.data(), sizeof(u64 *) * total, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = drbg_chains(d_msg, segments, total, &d_rk, &d_ctr, s, d_tables + total);
+    PolyLayout at;
+    at.tag = d_tables, at.frame = 0;
+    if (e == cudaSuccess) e = expand_key_ciphertexts(c, d_rk, d_ctr, 0, total, d_msg, d_dst, s, at);
+    free_chains(d_rk, d_ctr, segments, total, s);
+    for (void *p : {(void *)d_msg, (void *)d_tables, (void *)d_dst})
+        if (p) cudaFreeAsync(p, s);
+    const cudaError_t e2 = wait_stream(s);
+    return e == cudaSuccess ? e2 : e;
+}
+
+// `count` clients' keys of one config, every argument already checked: one allocation per key, then the expansion
+// (of the wire arrays, or of the messages `km`).  On error nothing is left allocated and out[] is untouched.
 static int32_t load_serialized_keys(const hecuda_context *h, uint64_t poly_bytes, int32_t count, bool relin,
-                                    const uint32_t *elements, int32_t element_count, const KeyWire *wire, hecuda_evk **out) {
+                                    const uint32_t *elements, int32_t element_count, const KeyWire *wire, hecuda_evk **out,
+                                    const KeyMessages *km = nullptr) {
     const Context &c = *h->ctx;
     const size_t words = (size_t)c.L * 2 * (c.L + 1) * c.n, ct_words = words / c.L;
     const int64_t cts[2] = {relin ? c.L : 0, (int64_t)element_count * c.L};
@@ -1034,7 +1099,9 @@ static int32_t load_serialized_keys(const hecuda_context *h, uint64_t poly_bytes
         }
         k->loaded = relin;
     }
-    if (e == cudaSuccess && !dst.empty()) e = expand_serialized_keys(h, (size_t)poly_bytes, cts, count, wire, dst);
+    if (e == cudaSuccess && !dst.empty())
+        e = km ? expand_proto_keys(h, *km, elements, element_count, relin, dst)
+               : expand_serialized_keys(h, (size_t)poly_bytes, cts, count, wire, dst);
     if (e != cudaSuccess) {
         for (hecuda_evk *k : keys) hecuda_evk_destroy(k);
         return cuda_fail(e, "evk_create_serialized");
@@ -1090,6 +1157,54 @@ int32_t hecuda_evk_create_serialized_many(const hecuda_context *h, int32_t key_c
         wire[(size_t)j] = KeyWire{{poly0[j], poly0[j] + poly_bytes * relin_cts}, {seeds[j], seeds[j] + 32 * relin_cts}, true};
     }
     return load_serialized_keys(h, poly_bytes, key_count, relin, elements, element_count, wire.data(), out);
+}
+
+int32_t hecuda_evk_create_proto_many(const hecuda_context *h, int32_t key_count, const uint8_t *const *messages,
+                                     const uint64_t *message_byte_counts, hecuda_evk **out) {
+    if (!out) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (key_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "key_count " + std::to_string(key_count) + ": expected at least 1");
+    std::fill(out, out + key_count, nullptr);
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    if (!c.has_ks)
+        return fail(HECUDA_ERR_UNSUPPORTED, "unsupportedHeOperation: a single coefficient modulus leaves no key-switching modulus");
+    if (!messages || !message_byte_counts) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    CodecConsts cc;
+    std::string err;
+    if (!codec_consts(c, c.map_ks(c.L), 0, cc, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+    const pirproto::PolySizes sz = pirproto::poly_sizes(cc, c.n);
+    KeyMessages km{messages, message_byte_counts, std::vector<pirproto::EvaluationKey>((size_t)key_count)};
+    std::vector<uint32_t> elements, sorted;
+    for (int32_t j = 0; j < key_count; ++j) {
+        const std::string who = "client " + std::to_string(j) + ": ";
+        if (!messages[j]) return fail(HECUDA_ERR_INVALID_ARGUMENT, who + "null argument");
+        pirproto::Error e;
+        pirproto::EvaluationKey &k = km.keys[(size_t)j];
+        if (!pirproto::walk_evaluation_key(messages[j], 0, (long long)message_byte_counts[j], sz, c.L, k, e))
+            return fail(e.code, who + e.what);
+        std::vector<uint32_t> mine;
+        for (const pirproto::GaloisKey &gk : k.galois) {
+            if (gk.element > 0xffffffffull || !valid_galois_element((uint32_t)gk.element, c.n))
+                return fail(HECUDA_ERR_INVALID_ARGUMENT, who + "invalid Galois element " + std::to_string(gk.element));
+            mine.push_back((uint32_t)gk.element);
+        }
+        if (j == 0) {
+            elements = mine;  // the call's configuration: client 0's elements, in its map order
+            sorted = mine;
+            std::sort(sorted.begin(), sorted.end());
+            continue;
+        }
+        if (k.relin != km.keys[0].relin)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT,
+                        who + "relinearization key " + (k.relin ? "present" : "absent") + ", unlike client 0");
+        std::sort(mine.begin(), mine.end());
+        if (mine != sorted) return fail(HECUDA_ERR_INVALID_ARGUMENT, who + "Galois elements differ from client 0's");
+    }
+    uint64_t poly_bytes = 0;
+    if ((rc = hecuda_poly_serialized_byte_count(h, HECUDA_BASE_KEYSWITCH, c.L + 1, 0, &poly_bytes))) return rc;
+    return load_serialized_keys(h, poly_bytes, key_count, km.keys[0].relin, elements.data(), (int32_t)elements.size(),
+                                nullptr, out, &km);
 }
 
 static int32_t bfv_apply_galois(const hecuda_context *h, const hecuda_evk *k, const void *ct, int32_t l, uint32_t element,

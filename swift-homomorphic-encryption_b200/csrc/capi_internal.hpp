@@ -212,25 +212,29 @@ cudaError_t relinearize_chunk(const Context &c, u64 *scratch, const u64 *key, co
                               int64_t items, cudaStream_t s, const KsKeyTable *keys = nullptr);
 cudaError_t apply_galois_chunk(const Context &c, u64 *scratch, const u64 *key, const u64 *ct, int l, unsigned element,
                                u64 *out, int64_t items, cudaStream_t s, const KsKeyTable *keys = nullptr);
+// with at.tag: poly0 and seeds read in place from the bytes at d_poly0 (at.tag / at.seed, drbg.cu)
 cudaError_t expand_seeded_device(const Context &c, int l, const unsigned char *d_poly0, const unsigned char *d_seeds, u64 *d_out,
-                                 int64_t batch, cudaStream_t s);
+                                 int64_t batch, cudaStream_t s, const PolyLayout &at = PolyLayout{});
 // Seeded key-switching ciphertexts (K = L + 1 rows, Eval) in two steps: drbg_chains over their seeds with
 // key_segments(c) segments each, then ciphertexts [first, first + count) from those chains: d_poly0 holds their
 // count x byteCount(K rows) bytes, and ciphertext i's 2 x K x N words go to d_dst[i] (a device table of pointers into
-// evaluation keys)
+// evaluation keys).  With layout.tag, ciphertext first + i's poly0 is at d_poly0 + layout.tag[layout.first + i] -
+// layout.base instead.
 int key_segments(const Context &c);
 cudaError_t expand_key_ciphertexts(const Context &c, const unsigned int *d_rk, const u64 *d_ctr, int64_t first, int64_t count,
-                                   const unsigned char *d_poly0, u64 *const *d_dst, cudaStream_t s);
+                                   const unsigned char *d_poly0, u64 *const *d_dst, cudaStream_t s,
+                                   const PolyLayout &layout = PolyLayout{});
 // NistAes128Ctr streams (drbg.cu): the AES tables, then for every 32-byte seed the round keys (segments x 44 words) and
 // counters V (segments x 2 words) of its first `segments` 4096-byte segments; free_chains zeroizes the round keys.
+// Seed b is at d_seeds + 32 b, or at d_seeds + d_seed_at[b] (a device table) when one is given.
 cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, unsigned int **d_rk, u64 **d_ctr,
-                        cudaStream_t s);
+                        cudaStream_t s, const long long *d_seed_at = nullptr);
 void free_chains(unsigned int *d_rk, u64 *d_ctr, int segments, int64_t batch, cudaStream_t s);
 // drbg_chains in two steps: the AES tables (synchronises s), then the chains alone (stream-ordered and graph-capturable
 // once the tables are on the device)
 cudaError_t drbg_upload_tables(cudaStream_t s);
 cudaError_t drbg_chains_uploaded(const unsigned char *d_seeds, int segments, int64_t batch, unsigned int **d_rk, u64 **d_ctr,
-                                 cudaStream_t s);
+                                 cudaStream_t s, const long long *d_seed_at = nullptr);
 cudaError_t drbg_tables(const unsigned char **sbox, const unsigned int **te0);
 // PolyRq.random mod p of `polys` degree-n polynomials from the one stream of the 32-byte d_seed (coefficient k of
 // polynomial j is the stream's (jN + k)-th 128-bit word mod p), stored as sigma(a) = a(x^-1) (simple_pir.cuh)

@@ -48,8 +48,10 @@ __device__ __forceinline__ u128 segment_word(const u32w *rk, const u64 *ctr, con
 }
 
 // two lanes per seed walk its chain of segments: both expand the current key, lane p encrypts counter block V + 1 + p,
-// the pair exchanges the blocks by shuffle and absorbs them (ctrDrbgUpdate); lane 0 leaves (round keys, V) of each segment
-__global__ void __launch_bounds__(64) drbg_chain_kernel(const unsigned char *__restrict__ seeds, u32w *__restrict__ round_keys,
+// the pair exchanges the blocks by shuffle and absorbs them (ctrDrbgUpdate); lane 0 leaves (round keys, V) of each segment.
+// Seed b is the 32 bytes at seeds + seed_at[b] (seeds read in place from a message), or at seeds + 32 b without seed_at.
+__global__ void __launch_bounds__(64) drbg_chain_kernel(const unsigned char *__restrict__ seeds,
+                                                        const long long *__restrict__ seed_at, u32w *__restrict__ round_keys,
                                                         u64 *__restrict__ counters, int segments, long long batch) {
     __shared__ unsigned char sbox[256];
     __shared__ u32w te0[256];
@@ -61,7 +63,7 @@ __global__ void __launch_bounds__(64) drbg_chain_kernel(const unsigned char *__r
     u32w key[4] = {0, 0, 0, 0}, rk[kRoundKeyWords], blk[4], b0[4], b1[4], provided[8];
     u64 hi = 0, lo = 0;
     for (int i = 0; i < 8; ++i) {
-        const unsigned char *p = seeds + 32 * seed + 4 * i;
+        const unsigned char *p = seeds + (seed_at ? seed_at[seed] : 32 * seed) + 4 * i;
         provided[i] = ((u32w)p[0] << 24) | ((u32w)p[1] << 16) | ((u32w)p[2] << 8) | p[3];
     }
     for (int s = -1; s < segments; ++s) {  // s = -1: init(entropy:) (NistCtrDrbg.swift:52-59)
@@ -130,12 +132,14 @@ __global__ void __launch_bounds__(kSegmentBlocks) drbg_one_modulus_fill_kernel(c
 // one CTA per (segment, ciphertext), one thread per coefficient k of the K x N stream.  poly1 = the DRBG word reduced
 // modulo its row's modulus, already in the key's Eval format (encryptZero samples `a` in Eval, Bfv+Encrypt.swift:156-157,
 // and convertFormat to Eval is the identity); poly0 = coefficient k unpacked from the ciphertext's serialized bytes.
-// Both go straight into the ciphertext's 2 x K x N words at dst[ciphertext].
+// Both go straight into the ciphertext's 2 x K x N words at dst[ciphertext].  Ciphertext b's poly0 is at
+// poly0 + b x byteCount, or, with at.tag, at poly0 + at.tag[at.first + b] - at.base (read in place from a message).
 __global__ void __launch_bounds__(kSegmentBlocks) key_expand_kernel(const u32w *__restrict__ round_keys,
                                                                     const u64 *__restrict__ counters,
                                                                     const unsigned char *__restrict__ poly0,
                                                                     u64 *const *__restrict__ dst, const __grid_constant__ RowModuli c,
-                                                                    const __grid_constant__ CodecConsts cc, int n, int segments) {
+                                                                    const __grid_constant__ CodecConsts cc, int n, int segments,
+                                                                    const __grid_constant__ PolyLayout at) {
     __shared__ unsigned char sbox[256];
     __shared__ u32w te0[256];
     __shared__ u32w rk[kRoundKeyWords];
@@ -148,7 +152,8 @@ __global__ void __launch_bounds__(kSegmentBlocks) key_expand_kernel(const u32w *
     const u128 word = segment_word(rk, counters + 2 * ((size_t)b * segments + s), te0, sbox);
     const int row = (int)(k / n);
     const long long i = k - (long long)row * n;
-    const unsigned char *src = poly0 + b * cc.byte_offset[cc.rows] + cc.byte_offset[row];
+    const unsigned char *src =
+        poly0 + (at.tag ? at.tag[at.first + b] - at.base : b * cc.byte_offset[cc.rows]) + cc.byte_offset[row];
     u64 *out = dst[b];
     out[k] = codec_unpack(src, cc.byte_offset[row + 1] - cc.byte_offset[row], cc.width[row], i);
     out[(long long)c.rows * n + k] = (u64)(word % c.p[row]);
@@ -171,16 +176,17 @@ cudaError_t drbg_upload_tables(cudaStream_t s) {
     return cudaStreamSynchronize(s);  // the tables live on this stack frame
 }
 
-cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, u32w **d_rk, u64 **d_ctr, cudaStream_t s) {
+cudaError_t drbg_chains(const unsigned char *d_seeds, int segments, int64_t batch, u32w **d_rk, u64 **d_ctr, cudaStream_t s,
+                        const long long *d_seed_at) {
     const cudaError_t e = drbg_upload_tables(s);
-    return e == cudaSuccess ? drbg_chains_uploaded(d_seeds, segments, batch, d_rk, d_ctr, s) : e;
+    return e == cudaSuccess ? drbg_chains_uploaded(d_seeds, segments, batch, d_rk, d_ctr, s, d_seed_at) : e;
 }
 
 cudaError_t drbg_chains_uploaded(const unsigned char *d_seeds, int segments, int64_t batch, u32w **d_rk, u64 **d_ctr,
-                                 cudaStream_t s) {
+                                 cudaStream_t s, const long long *d_seed_at) {
     cudaError_t e = cudaMallocAsync((void **)d_rk, (size_t)batch * segments * kRoundKeyWords * sizeof(u32w), s);
     if (e == cudaSuccess) e = cudaMallocAsync((void **)d_ctr, (size_t)batch * segments * 2 * sizeof(u64), s);
-    if (e == cudaSuccess) e = launch(drbg_chain_kernel, (unsigned)((batch + 31) / 32), 64, 0, s, d_seeds, *d_rk, *d_ctr, segments, batch);
+    if (e == cudaSuccess) e = launch(drbg_chain_kernel, (unsigned)((batch + 31) / 32), 64, 0, s, d_seeds, d_seed_at, *d_rk, *d_ctr, segments, batch);
     return e;
 }
 
@@ -225,11 +231,11 @@ cudaError_t drbg_tables(const unsigned char **sbox, const u32w **te0) {
 namespace {
 
 cudaError_t random_polys_device(const Context &c, int l, const unsigned char *d_seeds, u64 *d_out, int64_t batch,
-                                cudaStream_t s) {
+                                cudaStream_t s, const long long *d_seed_at = nullptr) {
     const int segments = (int)(((size_t)l * c.n * 16 + kSegmentBytes - 1) / kSegmentBytes);
     u32w *d_rk = nullptr;
     u64 *d_ctr = nullptr;
-    cudaError_t e = drbg_chains(d_seeds, segments, batch, &d_rk, &d_ctr, s);
+    cudaError_t e = drbg_chains(d_seeds, segments, batch, &d_rk, &d_ctr, s, d_seed_at);
     const RowModuli fc = row_moduli(c, c.map_q(l));
     if (e == cudaSuccess)
         e = for_each_part(batch, [&](int64_t done, int64_t part) {
@@ -254,9 +260,12 @@ int32_t check(const hecuda_context *h, const void *seeds, int32_t l, const void 
 namespace hecuda {
 namespace api {
 
-// Ciphertext(deserialize: .seeded) for `batch` ciphertexts, all buffers on the device; d_out: batch x 2 x l x N (Coeff)
+// Ciphertext(deserialize: .seeded) for `batch` ciphertexts, all buffers on the device; d_out: batch x 2 x l x N (Coeff).
+// Contiguous: d_poly0 holds batch x byteCount(l rows) bytes and d_seeds batch x 32.  With at.tag, both are read in place
+// from the bytes at d_poly0 (d_seeds unused): ciphertext b's poly0 at at.tag[b] (frame 0: zero rows where tag[b + 1] ==
+// tag[b]) and its seed at at.seed[b].
 cudaError_t expand_seeded_device(const Context &c, int l, const unsigned char *d_poly0, const unsigned char *d_seeds, u64 *d_out,
-                                 int64_t batch, cudaStream_t s) {
+                                 int64_t batch, cudaStream_t s, const PolyLayout &at) {
     const NttRowMap map = c.map_q(l);
     CodecConsts cc;
     std::string err;
@@ -266,8 +275,9 @@ cudaError_t expand_seeded_device(const Context &c, int l, const unsigned char *d
     cudaError_t e = cudaMallocAsync((void **)&d_a, pw * batch, s);
     if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_p0, pw * batch, s);
     // poly0: PolyRq(deserialize:) ; poly1: random Eval polynomial converted to Coeff (SerializedCiphertext.swift:44-49)
-    if (e == cudaSuccess) e = launch_poly_load(c, cc, 0, d_poly0, d_p0, batch, s);
-    if (e == cudaSuccess) e = random_polys_device(c, l, d_seeds, d_a, batch, s);
+    if (e == cudaSuccess) e = launch_poly_load(c, cc, 0, d_poly0, d_p0, batch, s, at);
+    if (e == cudaSuccess) e = at.tag ? random_polys_device(c, l, d_poly0, d_a, batch, s, at.seed)
+                                     : random_polys_device(c, l, d_seeds, d_a, batch, s);
     if (e == cudaSuccess) e = launch_ntt_inverse(c, map, d_a, d_a, batch * l, kScalePlain, s);
     if (e == cudaSuccess) e = cudaMemcpy2DAsync(d_out, 2 * pw, d_p0, pw, pw, (size_t)batch, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpy2DAsync(d_out + poly_words, 2 * pw, d_a, pw, pw, (size_t)batch, cudaMemcpyDeviceToDevice, s);
@@ -281,7 +291,7 @@ int key_segments(const Context &c) {
 }
 
 cudaError_t expand_key_ciphertexts(const Context &c, const u32w *d_rk, const u64 *d_ctr, int64_t first, int64_t count,
-                                   const unsigned char *d_poly0, u64 *const *d_dst, cudaStream_t s) {
+                                   const unsigned char *d_poly0, u64 *const *d_dst, cudaStream_t s, const PolyLayout &layout) {
     const NttRowMap map = c.map_ks(c.L);  // row K-1 is q_ks
     CodecConsts cc;
     std::string err;
@@ -290,9 +300,12 @@ cudaError_t expand_key_ciphertexts(const Context &c, const u32w *d_rk, const u64
     const RowModuli fc = row_moduli(c, map);
     return for_each_part(count, [&](int64_t done, int64_t part) {
         const size_t at = (size_t)(first + done) * segments;
+        PolyLayout from = layout;
+        from.first += done;
         return launch(key_expand_kernel, dim3((unsigned)segments, (unsigned)part), kSegmentBlocks, 0, s,
-                      d_rk + at * kRoundKeyWords, d_ctr + at * 2, d_poly0 + (size_t)done * serialized_poly_bytes(cc),
-                      d_dst + first + done, fc, cc, (int)c.n, segments);
+                      d_rk + at * kRoundKeyWords, d_ctr + at * 2,
+                      d_poly0 + (layout.tag ? 0 : (size_t)done * serialized_poly_bytes(cc)), d_dst + first + done, fc, cc,
+                      (int)c.n, segments, from);
     });
 }
 

@@ -217,6 +217,8 @@ HE_HD u64 codec_pack(const Word *__restrict__ src, int n, int w, int skip, long 
 // present[p], writes zero rows for a nil plaintext, and atomically lowers *bad to (first + p) * rows + row where a
 // residue is >= its modulus; a serialization writes the framing too (frame_bytes, or a 0 tag for a nil plaintext).
 // With `slot`, plaintext first + p is resident polynomial slot[first + p] of the rows passed, instead of polynomial p.
+// Protobuf messages read in place (pir_proto.hpp) pass each polynomial's own offset in `tag` with frame 0, and for seeded
+// ciphertexts each 32-byte seed's offset in `seed` (drbg.cu).
 constexpr int kMaxFrame = 24;  // two keys and two 10-byte varints at most
 struct PolyLayout {
     const long long *tag = nullptr;
@@ -224,6 +226,7 @@ struct PolyLayout {
     unsigned char *present = nullptr;
     unsigned long long *bad = nullptr;
     const long long *slot = nullptr;
+    const long long *seed = nullptr;
     int frame = 1;
     unsigned char frame_bytes[kMaxFrame] = {1};
 };

@@ -22,6 +22,7 @@
 
 #include "capi_internal.hpp"
 #include "database_io.hpp"
+#include "pir_proto.hpp"
 #include "wire_codec.hpp"
 
 using namespace hecuda;
@@ -736,6 +737,179 @@ int32_t respond_wire(const hecuda_context *h, const hecuda_evk *const *evks, int
     return HECUDA_OK;
 }
 
+// ---------------------------------------------------------------- protobuf messages in and out
+// The framing of one shape's PIRResponse (pirproto::place_response), the same bytes around every reply ciphertext
+struct ResponseFrame {
+    long long replies, chunks, polys, record, reply, size;  // polys: bytes of poly 0 + poly 1
+    int vec_len, head_len, tail_len;
+    unsigned char vec[16], head[24], tail[16];
+};
+
+// one thread per reply ciphertext of every client: its framing bytes (and its reply's opening before its first one)
+__global__ void __launch_bounds__(256) response_frame_kernel(unsigned char *__restrict__ out, long long cts,
+                                                             const __grid_constant__ ResponseFrame f) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= cts) return;
+    const long long client = i / f.replies, r = i - client * f.replies, index = r / f.chunks, chunk = r - index * f.chunks;
+    unsigned char *at = out + client * f.size + index * f.reply + f.vec_len + chunk * f.record;
+    if (chunk == 0)
+        for (int k = 0; k < f.vec_len; ++k) at[k - f.vec_len] = f.vec[k];
+    for (int k = 0; k < f.head_len; ++k) at[k] = f.head[k];
+    at += f.head_len + f.polys;
+    for (int k = 0; k < f.tail_len; ++k) at[k] = f.tail[k];
+}
+
+// One group's query ciphertexts read in place from its messages (uploaded back to back at msg_at[j]): the offset tables
+// of the seeded expansion (tag: poly0, frame 0, a .full ciphertext's entry equal to the next one's so that it expands
+// to zero rows; seed: its seed, or `pad` for a .full one), then per distinct skip value the .full polys' offsets and
+// their slots in the group's batch x 2 x L x N query buffer.
+struct GroupTables {
+    std::vector<long long> tag, seed;
+    std::vector<std::pair<int, std::vector<long long>>> full;  // skip -> offsets, then slots (half and half)
+};
+GroupTables group_tables(const std::vector<pirproto::Query> &queries, int32_t first, int clients,
+                         const std::vector<long long> &msg_at, long long pad) {
+    GroupTables t;
+    const size_t cts = queries[(size_t)first].cts.size(), batch = cts * (size_t)clients;
+    t.tag.assign(batch + 1, 0);
+    t.seed.assign(batch, pad);
+    t.tag[batch] = pad + 1;  // past every poly0
+    std::vector<std::pair<int, std::pair<long long, long long>>> polys;  // (skip, (offset, slot))
+    for (size_t b = batch; b-- > 0;) {
+        const pirproto::Ciphertext &ct = queries[(size_t)first + b / cts].cts[b % cts];
+        const long long base = msg_at[b / cts];
+        t.tag[b] = ct.full ? t.tag[b + 1] : base + ct.poly[0];
+        if (!ct.full) {
+            t.seed[b] = base + ct.seed;
+            continue;
+        }
+        for (int p = 1; p >= 0; --p) polys.push_back({ct.skip[p], {base + ct.poly[p], (long long)(2 * b + p)}});
+    }
+    std::reverse(polys.begin(), polys.end());  // message order: the offsets increase
+    for (const auto &q : polys) {
+        auto it = std::find_if(t.full.begin(), t.full.end(), [&](const auto &f) { return f.first == q.first; });
+        if (it == t.full.end()) it = t.full.insert(t.full.end(), {q.first, {}});
+        it->second.push_back(q.second.first);
+    }
+    for (auto &f : t.full) {  // offsets (plus a sentinel past the last), then the slots
+        f.second.push_back(f.second.back() + 1);
+        for (const auto &q : polys)
+            if (q.first == f.first) f.second.push_back(q.second.second);
+    }
+    return t;
+}
+
+// respond_wire with EncryptedIndices messages in and PIRResponse messages out.  Per group: the group's messages
+// uploaded back to back, the seeded expansion reading poly0 and the seeds in place (and the .full query ciphertexts
+// loaded over theirs), the group's responses, then each reply ciphertext packed straight into its slot of its client's
+// PIRResponse with one framing launch and one packing launch per reply poly.
+int32_t respond_proto(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count,
+                      const hecuda_pir_database *const *dbs, int32_t db_count, const ResponseShape &shape,
+                      const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                      const std::vector<pirproto::Query> &queries, int32_t query_ct_count, int32_t indices_count,
+                      int32_t skip0, int32_t skip1, const pirproto::ResponseLayout &rl, uint8_t *out) {
+    WireCodec wc;
+    int32_t rc = wc.setup(*h->ctx, skip0, skip1);
+    if (rc) return rc;
+    const Context &c = *h->ctx;
+    ResponseFrame frame{};
+    frame.chunks = rl.chunks, frame.replies = rl.indices * rl.chunks, frame.polys = rl.bytes[0] + rl.bytes[1];
+    frame.record = rl.record, frame.reply = rl.reply, frame.size = rl.size;
+    if (rl.vec_head.size() > sizeof(frame.vec) || rl.ct_head.size() > sizeof(frame.head) || rl.ct_tail.size() > sizeof(frame.tail))
+        return fail(HECUDA_ERR_UNSUPPORTED, "PIRResponse framing longer than its template");
+    frame.vec_len = (int)rl.vec_head.size(), frame.head_len = (int)rl.ct_head.size(), frame.tail_len = (int)rl.ct_tail.size();
+    std::copy(rl.vec_head.begin(), rl.vec_head.end(), frame.vec);
+    std::copy(rl.ct_head.begin(), rl.ct_head.end(), frame.head);
+    std::copy(rl.ct_tail.begin(), rl.ct_tail.end(), frame.tail);
+    const int group = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count);
+    const int64_t replies = (int64_t)indices_count * shape.chunk_count;  // per client
+    const size_t ct_words = (size_t)2 * c.L * c.n;
+    size_t msg_bytes = 0;
+    for (int32_t first = 0; first < client_count; first += group) {
+        size_t bytes = 0;
+        for (int32_t j = first; j < std::min<int32_t>(first + group, client_count); ++j) bytes += message_byte_counts[j];
+        msg_bytes = std::max(msg_bytes, bytes);
+    }
+    // reply ciphertext k of a group (client-major) is polys 2k, 2k + 1 of the group's responses; its poly p goes to
+    // byte tag[p][k] of the group's PIRResponses
+    std::vector<long long> pack((size_t)4 * (group * replies + 1));
+    for (int p = 0; p < 2; ++p) {
+        long long *tag = pack.data() + (size_t)2 * p * (group * replies + 1), *slot = tag + group * replies + 1;
+        for (int64_t k = 0; k < group * replies; ++k) {
+            tag[k] = (k / replies) * rl.size + rl.poly_at(k % replies, p);
+            slot[k] = 2 * k + p;
+        }
+        tag[group * replies] = group * rl.size;
+    }
+    WsGuard g(h);
+    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    cudaStream_t s = g.w->stream;
+    StreamBuffers tmp(s);
+    unsigned char *d_msg = nullptr, *d_out = nullptr;
+    u64 *d_query = nullptr, *d_resp = nullptr;
+    long long *d_pack = nullptr, *d_tables = nullptr;
+    const size_t table_words = (size_t)2 * query_ct_count * group + 1 + (size_t)6 * query_ct_count * group;
+    CK(tmp.alloc_bytes((void **)&d_msg, msg_bytes + 32));  // + 32 zero bytes: the seed a .full ciphertext expands
+    CK(tmp.alloc(&d_query, ct_words * query_ct_count * group));
+    CK(tmp.alloc(&d_resp, (size_t)2 * c.n * replies * group));
+    CK(tmp.alloc_bytes((void **)&d_out, (size_t)rl.size * group));
+    CK(tmp.alloc_bytes((void **)&d_pack, pack.size() * sizeof(long long)));
+    CK(tmp.alloc_bytes((void **)&d_tables, table_words * sizeof(long long)));
+    CodecConsts full_cc;
+    std::string err;
+    std::vector<std::vector<long long>> staged;  // host tables stay alive until the stream is drained
+    DrainOnExit drain{s};  // copies of the caller's buffers are in flight on `s` from here on
+    CK(cudaMemcpyAsync(d_pack, pack.data(), pack.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(d_msg + msg_bytes, 0, 32, s));
+    for (int32_t first = 0; first < client_count; first += group) {
+        const int clients = std::min<int32_t>(group, client_count - first);
+        std::vector<long long> msg_at((size_t)clients);
+        long long at = 0;
+        for (int j = 0; j < clients; ++j) {
+            msg_at[(size_t)j] = at;
+            CK(cudaMemcpyAsync(d_msg + at, messages[first + j], message_byte_counts[first + j], cudaMemcpyHostToDevice, s));
+            at += (long long)message_byte_counts[first + j];
+        }
+        const GroupTables t = group_tables(queries, first, clients, msg_at, (long long)msg_bytes);
+        staged.emplace_back(t.tag);
+        std::vector<long long> &flat = staged.back();
+        flat.insert(flat.end(), t.seed.begin(), t.seed.end());
+        for (const auto &f : t.full) flat.insert(flat.end(), f.second.begin(), f.second.end());
+        CK(cudaMemcpyAsync(d_tables, flat.data(), flat.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        PolyLayout seeded;
+        seeded.tag = d_tables, seeded.seed = d_tables + t.tag.size(), seeded.frame = 0;
+        const int64_t batch = (int64_t)query_ct_count * clients;
+        cudaError_t e = expand_seeded_device(c, c.L, d_msg, nullptr, d_query, batch, s, seeded);
+        if (e != cudaSuccess) return cuda_fail(e, "expand seeded query");
+        // .full query ciphertexts (Ciphertext(deserialize:) of .full): both polys over the zero rows expanded above
+        const long long *table = seeded.seed + t.seed.size();
+        for (const auto &f : t.full) {
+            const int64_t count = (int64_t)(f.second.size() - 1) / 2;
+            if (!codec_consts(c, c.map_q(c.L), f.first, full_cc, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+            PolyLayout full;
+            full.tag = table, full.slot = table + count + 1, full.frame = 0;
+            if ((e = launch_poly_load(c, full_cc, f.first, d_msg, d_query, count, s, full)) != cudaSuccess)
+                return cuda_fail(e, "load full query ciphertexts");
+            table += f.second.size();
+        }
+        rc = respond_group(h, evks + first, clients, first, dbs, db_count, shape, d_query, query_ct_count, indices_count,
+                           d_resp, s);
+        if (rc) return rc;
+        const int64_t cts = replies * clients;
+        if ((e = launch(response_frame_kernel, (unsigned)((cts + 255) / 256), 256, 0, s, d_out, (long long)cts, frame)) != cudaSuccess)
+            return cuda_fail(e, "frame response");
+        for (int p = 0; p < 2; ++p) {
+            PolyLayout at;
+            at.tag = d_pack + (size_t)2 * p * (group * replies + 1), at.slot = at.tag + group * replies + 1, at.frame = 0;
+            if ((e = launch_poly_serialize(c, wc.out[p], wc.skip[p], d_resp, d_out, cts, s, at)) != cudaSuccess)
+                return cuda_fail(e, "serialize response");
+        }
+        CK(cudaMemcpyAsync(out + (size_t)rl.size * first, d_out, (size_t)rl.size * clients, cudaMemcpyDeviceToHost, s));
+    }
+    CK(wait_stream(s));
+    return HECUDA_OK;
+}
+
 // Small moduli (the default PIR parameters): keep the rows as uint32 -- half the bytes per scan, half the HBM
 cudaError_t narrow_database(const Context &c, hecuda_pir_database *db) {
     if (!inner_product_plain_small_supported(c, c.L)) return cudaSuccess;
@@ -1431,6 +1605,52 @@ int32_t hecuda_mulpir_compute_response_clients_wire(const hecuda_context *h, con
     if (rc) return rc;
     return respond_wire(h, evks, client_count, false, dbs, db_count, shape, query_poly0, query_seeds, query_ct_count,
                         indices_count, skip_lsbs_poly0, skip_lsbs_poly1, out);
+}
+
+// The walk of every client's EncryptedIndices, checked like hecuda_mulpir_compute_response_clients_wire's arguments
+int32_t hecuda_mulpir_compute_response_clients_proto(const hecuda_context *h, const hecuda_evk *const *evks, int32_t client_count,
+                                                     const hecuda_pir_database *const *dbs, int32_t db_count,
+                                                     const int32_t *dims, int32_t dim_count, int32_t chunk_count,
+                                                     const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                                                     int32_t indices_count, int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1,
+                                                     uint8_t *out) {
+    int32_t rc = check_ctx(h);
+    if (rc) return rc;
+    if (!messages || !message_byte_counts || !dims || dim_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    const Context &c = *h->ctx;
+    int64_t expanded = 0;
+    for (int32_t d = 0; d < dim_count; ++d) expanded += dims[d];
+    // the ciphertext count of the parameter's query (MulPirClient.generateQuery: expandedQueryCount x indicesCount
+    // compressed into ciphertexts of N coefficients)
+    const int64_t query_ct_count = indices_count > 0 && expanded > 0 ? (expanded * indices_count + c.n - 1) / c.n : 1;
+    if (query_ct_count > 0x7fffffff) return fail(HECUDA_ERR_UNSUPPORTED, "too many query ciphertexts");
+    ResponseShape shape;
+    if ((rc = check_clients_args(h, evks, client_count, dbs, db_count, dims, dim_count, chunk_count,
+                                 (const uint64_t *)messages, (int32_t)query_ct_count, indices_count, out, shape)))
+        return rc;
+    uint64_t size = 0;
+    if ((rc = hecuda_mulpir_response_proto_byte_count(h, chunk_count, indices_count, skip_lsbs_poly0, skip_lsbs_poly1, &size)))
+        return rc;
+    CodecConsts qc;
+    std::string err;
+    if (!codec_consts(c, c.map_q(c.L), 0, qc, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+    const pirproto::PolySizes sz = pirproto::poly_sizes(qc, c.n);
+    std::vector<pirproto::Query> queries((size_t)client_count);
+    for (int32_t j = 0; j < client_count; ++j) {
+        const std::string who = "client " + std::to_string(j) + ": ";
+        if (!messages[j]) return fail(HECUDA_ERR_INVALID_ARGUMENT, who + "null argument");
+        pirproto::Error e;
+        if (!pirproto::walk_encrypted_indices(messages[j], 0, (long long)message_byte_counts[j], sz, queries[(size_t)j], e))
+            return fail(e.code, who + e.what);
+        if (!pirproto::check_query(queries[(size_t)j], (uint64_t)indices_count, (size_t)query_ct_count, e))
+            return fail(e.code, who + e.what);
+    }
+    WireCodec wc;
+    if ((rc = wc.setup(c, skip_lsbs_poly0, skip_lsbs_poly1))) return rc;
+    const pirproto::ResponseLayout layout = pirproto::place_response(indices_count, chunk_count, (long long)wc.bytes[0],
+                                                                     (long long)wc.bytes[1], skip_lsbs_poly0, skip_lsbs_poly1);
+    return respond_proto(h, evks, client_count, dbs, db_count, shape, messages, message_byte_counts, queries,
+                         (int32_t)query_ct_count, indices_count, skip_lsbs_poly0, skip_lsbs_poly1, layout, out);
 }
 
 }  // extern "C"

@@ -159,6 +159,15 @@ SYMBOLS = {
     "hecuda_mulpir_compute_response_clients_wire": (C.c_int32, [_VP, C.POINTER(_VP), C.c_int32, C.POINTER(_VP), C.c_int32,
                                                                 C.POINTER(C.c_int32), C.c_int32, C.c_int32, _VP, _VP, C.c_int32,
                                                                 C.c_int32, C.c_int32, C.c_int32, _VP]),
+    "hecuda_pir_request_fields_read": (C.c_int32, [_VP, C.c_uint64, _VP]),
+    "hecuda_evk_create_proto_many": (C.c_int32, [_VP, C.c_int32, _VP, _VP, _VP]),
+    "hecuda_mulpir_response_proto_byte_count": (C.c_int32, [_VP, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _VP]),
+    "hecuda_mulpir_compute_response_clients_proto": (C.c_int32, [_VP, C.POINTER(_VP), C.c_int32, C.POINTER(_VP), C.c_int32,
+                                                                 C.POINTER(C.c_int32), C.c_int32, C.c_int32, _VP, _VP,
+                                                                 C.c_int32, C.c_int32, C.c_int32, _VP]),
+    "hecuda_pir_encrypted_indices_write": (C.c_int32, [_VP, _VP, _VP, C.c_int32, C.c_int32, _VP, C.c_uint64, _VP]),
+    "hecuda_pir_evaluation_key_write": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int32, _VP, _VP, _VP, C.c_uint64, _VP]),
+    "hecuda_pir_response_read": (C.c_int32, [_VP, _VP, C.c_uint64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _VP]),
     "hecuda_pnns_matrix_create": (C.c_int32, [_VP, _VP, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.POINTER(_VP)]),
     "hecuda_pnns_matrix_destroy": (C.c_int32, [_VP]),
     "hecuda_pnns_matrix_result_count": (C.c_int32, [_VP, C.POINTER(C.c_int64)]),
@@ -460,6 +469,45 @@ class SecretKey:
         return cls(context, out[0])
 
 
+def _proto_galois_elements(message: bytes) -> list:
+    """The Galois elements of a SerializedEvaluationKey the library has accepted, in map order (for
+    EvaluationKey.galoisElements): field 1 (galois_key), its field-1 map entries, each entry's field 1."""
+
+    def fields(b):
+        at = 0
+        while at < len(b):
+            key, at = _varint(b, at)
+            number, wire = key >> 3, key & 7
+            if wire == 0:
+                value, at = _varint(b, at)
+                yield number, value
+            elif wire == 2:
+                size, at = _varint(b, at)
+                yield number, b[at:at + size]
+                at += size
+            else:  # fixed-size: the library has refused anything else
+                at += 8 if wire == 1 else 4
+
+    elements = []
+    for number, galois in fields(message):
+        if number == 1:
+            for entry_number, entry in fields(galois):
+                if entry_number == 1:
+                    elements.append(next((v for n, v in fields(entry) if n == 1), 0))
+    return elements
+
+
+def _varint(b: bytes, at: int):
+    value, shift = 0, 0
+    while True:
+        byte = b[at]
+        at += 1
+        value |= (byte & 0x7F) << shift
+        shift += 7
+        if not byte & 0x80:
+            return value, at
+
+
 class EvaluationKey:
     """EvaluationKey<Bfv<UInt64>> holding the relinearization key (Keys.swift:66-99,222)."""
 
@@ -558,6 +606,30 @@ class EvaluationKey:
             context._h, K, int(relin), _ptr(elems) if elements else None, len(elements),
             (C.c_void_p * K)(*[p.ctypes.data if p is not None else None for p in poly0]),
             (C.c_void_p * K)(*[s.ctypes.data if s is not None else None for s in seeds]), handles))
+        out = []
+        for h in handles:
+            key = cls.__new__(cls)
+            key.context, key.galoisElements, key._h = context, list(elements), C.c_void_p(h)
+            out.append(key)
+        return out
+
+    @classmethod
+    def fromProtoMany(cls, context: Context, messages) -> list:
+        """fromSerializedMany of SerializedEvaluationKey messages (hecuda_evk_create_proto_many): one bytes-like message
+        per client, its galois_key map entries in any order.  The messages go to the device as they are; one DRBG chain
+        launch and one expansion launch read their seeds and poly0 in place.  Every key ciphertext must be .seeded, and
+        every client must have client 0's configuration (a relinearization key for all or none, the same Galois
+        elements).  Returns one independent EvaluationKey per client, with client 0's map order as galoisElements."""
+        buffers = [np.frombuffer(bytes(m) if not isinstance(m, (bytes, np.ndarray)) else m, dtype=np.uint8) for m in messages]
+        if not buffers:
+            raise HeError(-1, "fromProtoMany: no keys to load")
+        K = len(buffers)
+        keep = [np.ascontiguousarray(b) if b.size else np.zeros(1, np.uint8) for b in buffers]
+        counts = np.array([b.size for b in buffers], dtype=np.uint64)
+        handles = (C.c_void_p * K)()
+        _check(load_library().hecuda_evk_create_proto_many(
+            context._h, K, (C.c_void_p * K)(*[b.ctypes.data for b in keep]), counts.ctypes.data_as(C.c_void_p), handles))
+        elements = _proto_galois_elements(keep[0][:buffers[0].size].tobytes())
         out = []
         for h in handles:
             key = cls.__new__(cls)

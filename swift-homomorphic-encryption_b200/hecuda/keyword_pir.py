@@ -31,7 +31,7 @@ import numpy as np
 from . import Context, EvaluationKey, SecretKey, _check, _ptr, load_library
 from . import symmetric_pir
 from .pir import IndexPirConfig, IndexPirParameter, MulPir, MulPirClient, MulPirServer, PirError, PirKeyCompressionStrategy, \
-    PirWire, ProcessedDatabase, ShardValidationResult, _save_databases, _validate, bytesPerPlaintext
+    PirWire, ProcessedDatabase, ShardValidationResult, _save_databases, _validate, bytesPerPlaintext, responseFromMessage
 from .symmetric_pir import SymmetricPirClientConfig, SymmetricPirConfig
 
 MAX_SLOT_COUNT = 255  # HashBucket.maxSlotCount
@@ -438,6 +438,20 @@ class KeywordPirClient:
                 return value
         return None
 
+    def queryMessage(self, keyword: bytes, secretKey: SecretKey) -> bytes:
+        """generateQuery as a pir.v1.EncryptedIndices message (MulPirClient.queryMessage at the keyword's hashIndices)."""
+        return self.indexPirClient.queryMessage(self._indices(keyword), secretKey)
+
+    def evaluationKeyMessage(self, secretKey: SecretKey):
+        """(key, SerializedEvaluationKey message) as MulPirClient.evaluationKeyMessage."""
+        return self.indexPirClient.evaluationKeyMessage(secretKey)
+
+    def decryptResponseMessage(self, message: bytes, keyword: bytes, secretKey: SecretKey) -> Optional[bytes]:
+        """decrypt of an api.pir.v1.PIRResponse of hashFunctionCount replies."""
+        response = responseFromMessage(self.context, message, self.keywordParameter.hashFunctionCount,
+                                       self.indexPirClient.parameter)
+        return self.decrypt(response, keyword, secretKey)
+
     def countEntriesInResponse(self, response, secretKey: SecretKey) -> int:
         """KeywordPirClient.countEntriesInResponse (:376-391): the slots of every bucket found in the replies' bytes."""
         found = 0
@@ -514,6 +528,11 @@ class KeywordPirServer:
 
     def computeResponsesWire(self, queryPoly0, querySeeds, evaluationKeys: Sequence[EvaluationKey]):
         return PirWire.computeResponses(self.indexPirServer, queryPoly0, querySeeds, evaluationKeys, self.hashFunctionCount)
+
+    def computeResponsesProto(self, messages: Sequence[bytes], evaluationKeys: Sequence[EvaluationKey]) -> List[bytes]:
+        """One EncryptedIndices message per client in, one PIRResponse per client out, with indicesCount =
+        hashFunctionCount (PirWire.computeResponsesProto)."""
+        return PirWire.computeResponsesProto(self.indexPirServer, messages, evaluationKeys, self.hashFunctionCount)
 
     def validate(self, row: KeywordValuePair, trials: int = 1) -> ShardValidationResult:
         """KeywordDatabase.validateShard (KeywordDatabase.swift:557-630): row = (keyword, value).  Every step runs on the

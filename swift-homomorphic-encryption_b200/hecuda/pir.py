@@ -445,6 +445,75 @@ class PirWire:
         return out, skips
 
 
+    @staticmethod
+    def computeResponsesProto(server: "MulPirServer", messages: Sequence[bytes], evaluationKeys: Sequence[EvaluationKey],
+                              indicesCount: int = 1) -> List[bytes]:
+        """computeResponses with protobuf messages (hecuda_mulpir_compute_response_clients_proto): one
+        pir.v1.EncryptedIndices per client in (num_pir_calls = indicesCount; its ciphertexts .seeded or .full), one
+        api.pir.v1.PIRResponse per client out, whose reply ciphertexts hold the bytes computeResponses returns for the
+        same poly0 and seeds.  The messages cross PCIe as they are; the replies are framed on the device."""
+        ctx = server.context
+        keys = list(evaluationKeys)
+        buffers = [np.frombuffer(m, dtype=np.uint8) if isinstance(m, (bytes, bytearray, memoryview)) else
+                   np.ascontiguousarray(m, dtype=np.uint8).reshape(-1) for m in messages]
+        if not keys or len(buffers) != len(keys):
+            raise HeError(-1, f"computeResponsesProto: {len(buffers)} messages for {len(keys)} evaluation keys")
+        skips = skipLSBsForDecryption(ctx)
+        size = C.c_uint64(0)
+        _check(load_library().hecuda_mulpir_response_proto_byte_count(ctx._h, server.chunkCount, indicesCount, skips[0],
+                                                                       skips[1], C.byref(size)))
+        out = np.empty((len(keys), size.value), dtype=np.uint8)
+        keep = [b if b.size else np.zeros(1, np.uint8) for b in buffers]
+        counts = np.array([b.size for b in buffers], dtype=np.uint64)
+        handles = (C.c_void_p * len(server.databases))(*[db._h for db in server.databases])
+        key_handles = (C.c_void_p * len(keys))(*[k._h for k in keys])
+        dims = (C.c_int32 * len(server.parameter.dimensions))(*server.parameter.dimensions)
+        _check(load_library().hecuda_mulpir_compute_response_clients_proto(
+            ctx._h, key_handles, len(keys), handles, len(server.databases), dims, len(server.parameter.dimensions),
+            server.chunkCount, (C.c_void_p * len(keep))(*[b.ctypes.data for b in keep]), counts.ctypes.data_as(C.c_void_p),
+            indicesCount, skips[0], skips[1], out.ctypes.data_as(C.c_void_p)))
+        return [row.tobytes() for row in out]
+
+
+class PirRequestFields(C.Structure):
+    """hecuda_pir_request_fields (include/hecuda.h)."""
+    _fields_ = [("shard_index", C.c_uint32), ("has_shard_id", C.c_int32), ("has_query", C.c_int32),
+                ("has_evaluation_key", C.c_int32), ("has_key_metadata", C.c_int32),
+                ("shard_id_offset", C.c_uint64), ("shard_id_bytes", C.c_uint64),
+                ("configuration_hash_offset", C.c_uint64), ("configuration_hash_bytes", C.c_uint64),
+                ("query_offset", C.c_uint64), ("query_bytes", C.c_uint64),
+                ("evaluation_key_offset", C.c_uint64), ("evaluation_key_bytes", C.c_uint64),
+                ("key_timestamp", C.c_uint64), ("key_identifier_offset", C.c_uint64), ("key_identifier_bytes", C.c_uint64)]
+
+
+class PirRequest:
+    """api.pir.v1.PIRRequest, the envelope a PIR server receives."""
+
+    @staticmethod
+    def fields(data: bytes) -> dict:
+        """The walk of a PIRRequest (hecuda_pir_request_fields_read), nothing copied on the host side: shardIndex,
+        shardId (None when absent), configurationHash, the key metadata (keyTimestamp, keyIdentifier; from
+        evaluation_key_metadata, or evaluation_key.metadata when that is absent) and the (offset, length) ranges of the
+        query (an EncryptedIndices) and of evaluation_key.evaluation_key (a SerializedEvaluationKey), None when unset.
+        Routing by shard and caching keys by identifier stay the caller's."""
+        b = bytes(data)
+        r = PirRequestFields()
+        _check(load_library().hecuda_pir_request_fields_read(b, len(b), C.byref(r)))
+
+        def span(offset, size):
+            return b[offset:offset + size]
+
+        return {
+            "shardIndex": r.shard_index,
+            "shardId": span(r.shard_id_offset, r.shard_id_bytes).decode() if r.has_shard_id else None,
+            "configurationHash": span(r.configuration_hash_offset, r.configuration_hash_bytes),
+            "keyTimestamp": r.key_timestamp if r.has_key_metadata else None,
+            "keyIdentifier": span(r.key_identifier_offset, r.key_identifier_bytes) if r.has_key_metadata else None,
+            "query": (r.query_offset, r.query_bytes) if r.has_query else None,
+            "evaluationKey": (r.evaluation_key_offset, r.evaluation_key_bytes) if r.has_evaluation_key else None,
+        }
+
+
 class PirUtil:
     """enum PirUtil<Bfv<UInt64>> (PirUtil.swift:573): expansion and response computation on the device."""
 
@@ -456,6 +525,48 @@ class PirUtil:
         out = np.empty((outputCount, 2, context.L, context.degree), dtype=np.uint64)
         _check(load_library().hecuda_mulpir_expand(context._h, evaluationKey._h, _ptr(cts), count, outputCount, _ptr(out)))
         return out
+
+
+def _written(call) -> bytes:
+    """A host-only writer's bytes: its size first, then the bytes."""
+    written = C.c_uint64(0)
+    _check(call(None, 0, C.byref(written)))
+    out = np.empty(max(written.value, 1), dtype=np.uint8)
+    _check(call(out.ctypes.data_as(C.c_void_p), out.size, C.byref(written)))
+    return out[:written.value].tobytes()
+
+
+def evaluationKeyMessage(context: Context, form) -> bytes:
+    """SerializedEvaluationKey.proto() of a seeded key in EvaluationKey.generate(..., wire=True)'s form: the galois_key
+    map in the form's element order, then the relinearization key (hecuda_pir_evaluation_key_write)."""
+    arrays = EvaluationKey._wireArrays(context)
+    relin = arrays(form["relinPoly0"], form["relinSeeds"]) if form.get("relinPoly0") is not None else None
+    galois = {int(e): arrays(*v) for e, v in (form.get("galois") or {}).items()}
+    elements = np.ascontiguousarray(list(galois), dtype=np.uint32)
+    gp = np.ascontiguousarray(np.concatenate([v[0].reshape(-1) for v in galois.values()])) if galois else None
+    gs = np.ascontiguousarray(np.concatenate([v[1].reshape(-1) for v in galois.values()])) if galois else None
+    return _written(lambda out, capacity, written: load_library().hecuda_pir_evaluation_key_write(
+        context._h, _ptr(relin[0]) if relin else None, _ptr(relin[1]) if relin else None,
+        _ptr(elements) if galois else None, len(galois), _ptr(gp) if galois else None, _ptr(gs) if galois else None,
+        out, capacity, written))
+
+
+def responseFromMessage(context: Context, message: bytes, indicesCount: int, parameter) -> np.ndarray:
+    """Response.native() of an api.pir.v1.PIRResponse: (indicesCount, chunkCount, 2, 1, N) Coeff ciphertexts, the
+    replies found by hecuda_pir_response_read and their polys loaded with Bfv.skipLSBsForDecryption."""
+    b = np.frombuffer(bytes(message), dtype=np.uint8)
+    skips = skipLSBsForDecryption(context)
+    sizes = [Bfv.serializationByteCount(context, 1, s) for s in skips]
+    chunks = -(-parameter.encodedEntrySize // bytesPerPlaintext(context))  # MulPirServer.chunkCount
+    offsets = np.empty(indicesCount * chunks, dtype=np.uint64)
+    _check(load_library().hecuda_pir_response_read(context._h, b.ctypes.data_as(C.c_void_p), b.size, chunks, indicesCount,
+                                                   skips[0], skips[1], offsets.ctypes.data_as(C.c_void_p)))
+    polys = []
+    for p, (skip, size) in enumerate(zip(skips, sizes)):
+        start = offsets.astype(np.int64) + (sizes[0] if p else 0)
+        rows = np.stack([b[o:o + size] for o in start])
+        polys.append(Bfv.load(context, rows, 1, skip))
+    return np.stack(polys, axis=1).reshape(indicesCount, chunks, 2, 1, context.degree)
 
 
 class MulPirClient:
@@ -495,6 +606,28 @@ class MulPirClient:
     def generateQuery(self, indices: Sequence[int], secretKey: SecretKey) -> np.ndarray:
         """MulPirClient.generateQuery (MulPir.swift:201-218) with PirUtil.compressBinaryInputs (PirUtil.swift:361-404):
         Query.ciphertexts as (count, 2, L, N) Coeff."""
+        return Bfv.encrypt(self.context, secretKey, self._queryPlaintexts(indices))
+
+    def queryMessage(self, indices: Sequence[int], secretKey: SecretKey, aSeeds=None, errorSeeds=None) -> bytes:
+        """generateQuery as the reference's client sends it: Query.proto(), a pir.v1.EncryptedIndices of .seeded
+        ciphertexts with num_pir_calls = len(indices) (hecuda_pir_encrypted_indices_write)."""
+        poly0, seeds = Bfv.encrypt(self.context, secretKey, self._queryPlaintexts(indices), seeded=True, aSeeds=aSeeds,
+                                   errorSeeds=errorSeeds)
+        return _written(lambda out, capacity, written: load_library().hecuda_pir_encrypted_indices_write(
+            self.context._h, _ptr(poly0), _ptr(seeds), seeds.shape[0], len(indices), out, capacity, written))
+
+    def evaluationKeyMessage(self, secretKey: SecretKey):
+        """generateEvaluationKey as the reference's client sends it: (key, SerializedEvaluationKey.proto() bytes), the
+        key's seeded form framed by hecuda_pir_evaluation_key_write."""
+        key, form = EvaluationKey.generate(self.context, self.evaluationKeyConfig, secretKey, wire=True)
+        return key, evaluationKeyMessage(self.context, form)
+
+    def decryptResponseMessage(self, message: bytes, indices: Sequence[int], secretKey: SecretKey) -> List[bytes]:
+        """decrypt of an api.pir.v1.PIRResponse: its reply ciphertexts found by hecuda_pir_response_read, their polys
+        loaded with Bfv.skipLSBsForDecryption, then decrypt."""
+        return self.decrypt(responseFromMessage(self.context, message, len(indices), self.parameter), indices, secretKey)
+
+    def _queryPlaintexts(self, indices: Sequence[int]) -> np.ndarray:
         ctx, dims = self.context, self.parameter.dimensions
         accumulated, positions = 0, []
         for index in indices:
@@ -514,7 +647,7 @@ class MulPirClient:
             plaintexts.append(raw)
             processed += count
             remaining -= count
-        return Bfv.encrypt(ctx, secretKey, np.stack(plaintexts))
+        return np.stack(plaintexts)
 
     def decryptFull(self, response, secretKey: SecretKey) -> List[bytes]:
         """MulPirClient.decryptFull: every reply's bytes.  response: (replies, chunkCount, 2, 1, N)."""
