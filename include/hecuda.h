@@ -1015,6 +1015,91 @@ int32_t hecuda_pnns_compute_response_clients_wire(const hecuda_context *ctx, con
                                                   int32_t skip_lsbs_poly0, int32_t skip_lsbs_poly1, uint8_t *out,
                                                   int64_t out_capacity, int64_t *out_count);
 
+/* ---- PNNS in the reference's protobuf messages (pnns_proto.hpp, pnns_plan.hpp) ----
+ * Requests as the reference's clients send them and shard responses as they expect them: api.pnns.v1.PNNSRequest and
+ * api.pnns.v1.PNNSShardResponse (api/pnns/v1/pnns.proto), their matrices pnns.v1.SerializedCiphertextMatrix
+ * (PnnsConversion.swift:265-348, PnnsConversionApi.swift).  The walks refuse what the PIR walks refuse (groups, varints
+ * over 10 bytes, lengths past their message, a singular message given twice, a known field of the wrong wire type).
+ *
+ * hecuda_pnns_request_fields_read: the walk of a PNNSRequest (host only, nothing copied): the number of query matrices
+ * and their common num_rows (refused when they differ), the byte ranges (offsets into `bytes`) of config_id, of
+ * evaluation_key.evaluation_key (a SerializedEvaluationKey, ready for hecuda_evk_create_proto_many) and of the key
+ * identifier, the key timestamp (from evaluation_key_metadata, or evaluation_key.metadata when that is absent), the shard
+ * indices and each shard id's (offset, length).  shard_indices / shard_id_ranges (2 x count) may be NULL; otherwise
+ * their capacity must hold every entry.  Routing and key caching stay the caller's. */
+typedef struct hecuda_pnns_request_fields {
+    int32_t query_count;
+    uint32_t query_row_count;
+    int32_t has_evaluation_key, has_key_metadata;
+    int64_t shard_index_count, shard_id_count;
+    uint64_t config_id_offset, config_id_bytes;
+    uint64_t evaluation_key_offset, evaluation_key_bytes;
+    uint64_t key_timestamp, key_identifier_offset, key_identifier_bytes;
+} hecuda_pnns_request_fields;
+int32_t hecuda_pnns_request_fields_read(const uint8_t *bytes, uint64_t byte_count, hecuda_pnns_request_fields *fields,
+                                        uint32_t *shard_indices, int64_t index_capacity, uint64_t *shard_id_ranges,
+                                        int64_t id_capacity);
+
+/* The size of one client's PNNSShardResponse (Response.proto(), as SwiftProtobuf writes it) for a query of
+ * query_row_count rows against matrices[k] on ctxs[k]: per context one .denseColumn SerializedCiphertextMatrix of
+ * database rows x query rows whose ciphertexts are SerializedCiphertext.full with that context's
+ * Bfv.skipLSBsForDecryption (it depends on t), then entry_ids (packed) and every entry_metadatas element (metadata k is
+ * metadata[metadata_offsets[k], metadata_offsets[k + 1])). */
+int32_t hecuda_pnns_shard_response_byte_count(const hecuda_context *const *ctxs, int32_t count,
+                                              const hecuda_pnns_matrix *const *matrices, int32_t query_row_count,
+                                              const uint64_t *entry_ids, int64_t id_count, const uint8_t *metadata,
+                                              const uint64_t *metadata_offsets, int64_t metadata_count, uint64_t *bytes);
+
+/* Server.computeResponse for client_count clients, one PNNSRequest per client in (message c: message_byte_counts[c]
+ * bytes; only its query matrices are read) and one PNNSShardResponse per client out: out holds client_count x
+ * hecuda_pnns_shard_response_byte_count bytes and client c's slice is a complete message.  For every context its reply
+ * poly bytes equal what hecuda_pnns_compute_response_clients_wire returns for the same poly0 and seeds.
+ *
+ * Each request holds one .denseRow matrix per context (wrongCiphertextMatrixCount; wrongMatrixPacking, or unsetOneof
+ * for no packing), of the database's column count (invalidMatrixDimensions) and CiphertextMatrix.ciphertextCount(N,
+ * dims) ciphertexts (wrongCiphertextCount), every matrix of a request and of every client with client 0's row count.
+ * Query ciphertexts may be .seeded or .full (correction factor 1).  The query plan -- each row's ciphertext, mask and
+ * replication count, the packing rotations -- is derived here (pnns_plan.hpp) from the shape and client 0's Galois
+ * elements, once per call; the masks are SIMD-encoded once per context.
+ *
+ * evks[c] may belong to any context with the N, word size and coefficient moduli of every ctxs[k] (BFV keys do not
+ * depend on t): keys loaded once on ctxs[0] serve every plaintext modulus, read in place, with no copy.  Every Galois
+ * key every context's plan needs is found for every client before anything is enqueued; every failure's message starts
+ * with "client <c>: " where a client is at fault, and leaves `out` untouched.
+ *
+ * Per group of HECUDA_PNNS_CLIENT_GROUP clients: one upload of the group's messages; per context the seeded expansion
+ * reading poly0 and seeds in place, the many-clients response pipeline and one packing launch per reply poly writing
+ * into the clients' messages; one framing launch; one download. */
+int32_t hecuda_pnns_compute_response_clients_proto(const hecuda_context *const *ctxs, int32_t count,
+                                                   const hecuda_evk *const *evks, int32_t client_count,
+                                                   const hecuda_pnns_matrix *const *matrices,
+                                                   const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                                                   const uint64_t *entry_ids, int64_t id_count, const uint8_t *metadata,
+                                                   const uint64_t *metadata_offsets, int64_t metadata_count, uint8_t *out);
+
+/* Client side, host only.  hecuda_pnns_request_write: Query.proto() as a PNNSRequest: one .denseRow matrix of
+ * row_count x column_count per context k of ciphertext_count .seeded ciphertexts (poly0[k]: ciphertext_count x
+ * byteCount(L rows), seeds[k]: ciphertext_count x 32), then config_id when config_id_bytes > 0, then, when
+ * evaluation_key is not NULL, evaluation_key { metadata { key_timestamp, key_identifier }, evaluation_key } (a
+ * SerializedEvaluationKey).  With out NULL only *written is set; else capacity must hold it.
+ * hecuda_pnns_shard_response_read: the walk of a PNNSShardResponse against ctxs (one .denseColumn matrix per context of
+ * .full ciphertexts over one modulus, every matrix of one shape): *shape, then, for the arrays that are not NULL,
+ * poly_offsets[k x reply_count + r] (offset of reply r's poly 0 in matrix k; poly 1 follows it), skip_lsbs[2k + p],
+ * entry_ids[id_count] and metadata_ranges[2 x metadata_count] (offset, length). */
+int32_t hecuda_pnns_request_write(const hecuda_context *const *ctxs, int32_t count, uint32_t row_count, uint32_t column_count,
+                                  const uint8_t *const *poly0, const uint8_t *const *seeds, int32_t ciphertext_count,
+                                  const uint8_t *config_id, uint64_t config_id_bytes, const uint8_t *evaluation_key,
+                                  uint64_t evaluation_key_bytes, uint64_t key_timestamp, const uint8_t *key_identifier,
+                                  uint64_t key_identifier_bytes, uint8_t *out, uint64_t capacity, uint64_t *written);
+typedef struct hecuda_pnns_shard_response_shape {
+    int32_t matrix_count, reply_count;
+    uint32_t row_count, column_count;
+    int64_t id_count, metadata_count;
+} hecuda_pnns_shard_response_shape;
+int32_t hecuda_pnns_shard_response_read(const hecuda_context *const *ctxs, int32_t count, const uint8_t *bytes,
+                                        uint64_t byte_count, hecuda_pnns_shard_response_shape *shape, uint64_t *poly_offsets,
+                                        int32_t *skip_lsbs, uint64_t *entry_ids, uint64_t *metadata_ranges);
+
 /* ---- coefficient-wise PolyRq arithmetic (SURVEY.md section 8a, row a7) ----
  * PolyRq += / -= (PolyRq/PolyRq.swift:147-174), *= in Eval format (:184-204, Modulus.multiplyMod Modulus.swift:89-94),
  * negation (negateMod, ModularArithmetic/Scalar.swift:167-175) and *= [T] with one reduced scalar per RNS row

@@ -23,6 +23,7 @@
 #include "capi_internal.hpp"
 #include "database_io.hpp"
 #include "pir_proto.hpp"
+#include "proto_respond.hpp"
 #include "wire_codec.hpp"
 
 using namespace hecuda;
@@ -738,67 +739,6 @@ int32_t respond_wire(const hecuda_context *h, const hecuda_evk *const *evks, int
 }
 
 // ---------------------------------------------------------------- protobuf messages in and out
-// The framing of one shape's PIRResponse (pirproto::place_response), the same bytes around every reply ciphertext
-struct ResponseFrame {
-    long long replies, chunks, polys, record, reply, size;  // polys: bytes of poly 0 + poly 1
-    int vec_len, head_len, tail_len;
-    unsigned char vec[16], head[24], tail[16];
-};
-
-// one thread per reply ciphertext of every client: its framing bytes (and its reply's opening before its first one)
-__global__ void __launch_bounds__(256) response_frame_kernel(unsigned char *__restrict__ out, long long cts,
-                                                             const __grid_constant__ ResponseFrame f) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= cts) return;
-    const long long client = i / f.replies, r = i - client * f.replies, index = r / f.chunks, chunk = r - index * f.chunks;
-    unsigned char *at = out + client * f.size + index * f.reply + f.vec_len + chunk * f.record;
-    if (chunk == 0)
-        for (int k = 0; k < f.vec_len; ++k) at[k - f.vec_len] = f.vec[k];
-    for (int k = 0; k < f.head_len; ++k) at[k] = f.head[k];
-    at += f.head_len + f.polys;
-    for (int k = 0; k < f.tail_len; ++k) at[k] = f.tail[k];
-}
-
-// One group's query ciphertexts read in place from its messages (uploaded back to back at msg_at[j]): the offset tables
-// of the seeded expansion (tag: poly0, frame 0, a .full ciphertext's entry equal to the next one's so that it expands
-// to zero rows; seed: its seed, or `pad` for a .full one), then per distinct skip value the .full polys' offsets and
-// their slots in the group's batch x 2 x L x N query buffer.
-struct GroupTables {
-    std::vector<long long> tag, seed;
-    std::vector<std::pair<int, std::vector<long long>>> full;  // skip -> offsets, then slots (half and half)
-};
-GroupTables group_tables(const std::vector<pirproto::Query> &queries, int32_t first, int clients,
-                         const std::vector<long long> &msg_at, long long pad) {
-    GroupTables t;
-    const size_t cts = queries[(size_t)first].cts.size(), batch = cts * (size_t)clients;
-    t.tag.assign(batch + 1, 0);
-    t.seed.assign(batch, pad);
-    t.tag[batch] = pad + 1;  // past every poly0
-    std::vector<std::pair<int, std::pair<long long, long long>>> polys;  // (skip, (offset, slot))
-    for (size_t b = batch; b-- > 0;) {
-        const pirproto::Ciphertext &ct = queries[(size_t)first + b / cts].cts[b % cts];
-        const long long base = msg_at[b / cts];
-        t.tag[b] = ct.full ? t.tag[b + 1] : base + ct.poly[0];
-        if (!ct.full) {
-            t.seed[b] = base + ct.seed;
-            continue;
-        }
-        for (int p = 1; p >= 0; --p) polys.push_back({ct.skip[p], {base + ct.poly[p], (long long)(2 * b + p)}});
-    }
-    std::reverse(polys.begin(), polys.end());  // message order: the offsets increase
-    for (const auto &q : polys) {
-        auto it = std::find_if(t.full.begin(), t.full.end(), [&](const auto &f) { return f.first == q.first; });
-        if (it == t.full.end()) it = t.full.insert(t.full.end(), {q.first, {}});
-        it->second.push_back(q.second.first);
-    }
-    for (auto &f : t.full) {  // offsets (plus a sentinel past the last), then the slots
-        f.second.push_back(f.second.back() + 1);
-        for (const auto &q : polys)
-            if (q.first == f.first) f.second.push_back(q.second.second);
-    }
-    return t;
-}
-
 // respond_wire with EncryptedIndices messages in and PIRResponse messages out.  Per group: the group's messages
 // uploaded back to back, the seeded expansion reading poly0 and the seeds in place (and the .full query ciphertexts
 // loaded over theirs), the group's responses, then each reply ciphertext packed straight into its slot of its client's
@@ -812,15 +752,10 @@ int32_t respond_proto(const hecuda_context *h, const hecuda_evk *const *evks, in
     int32_t rc = wc.setup(*h->ctx, skip0, skip1);
     if (rc) return rc;
     const Context &c = *h->ctx;
-    ResponseFrame frame{};
-    frame.chunks = rl.chunks, frame.replies = rl.indices * rl.chunks, frame.polys = rl.bytes[0] + rl.bytes[1];
-    frame.record = rl.record, frame.reply = rl.reply, frame.size = rl.size;
-    if (rl.vec_head.size() > sizeof(frame.vec) || rl.ct_head.size() > sizeof(frame.head) || rl.ct_tail.size() > sizeof(frame.tail))
-        return fail(HECUDA_ERR_UNSUPPORTED, "PIRResponse framing longer than its template");
-    frame.vec_len = (int)rl.vec_head.size(), frame.head_len = (int)rl.ct_head.size(), frame.tail_len = (int)rl.ct_tail.size();
-    std::copy(rl.vec_head.begin(), rl.vec_head.end(), frame.vec);
-    std::copy(rl.ct_head.begin(), rl.ct_head.end(), frame.head);
-    std::copy(rl.ct_tail.begin(), rl.ct_tail.end(), frame.tail);
+    FrameRuns frame;  // every reply ciphertext's framing (and its reply's opening before its first one)
+    frame.size = rl.size;
+    for (long long r = 0; r < rl.indices * rl.chunks; ++r)
+        rl.frame(r, [&](long long at, const pirproto::Bytes &b) { frame.put(at, b); });
     const int group = std::min<int32_t>(HECUDA_MULPIR_CLIENT_GROUP, client_count);
     const int64_t replies = (int64_t)indices_count * shape.chunk_count;  // per client
     const size_t ct_words = (size_t)2 * c.L * c.n;
@@ -847,7 +782,8 @@ int32_t respond_proto(const hecuda_context *h, const hecuda_evk *const *evks, in
     StreamBuffers tmp(s);
     unsigned char *d_msg = nullptr, *d_out = nullptr;
     u64 *d_query = nullptr, *d_resp = nullptr;
-    long long *d_pack = nullptr, *d_tables = nullptr;
+    long long *d_pack = nullptr, *d_tables = nullptr, *d_runs = nullptr;
+    unsigned char *d_frame = nullptr;
     const size_t table_words = (size_t)2 * query_ct_count * group + 1 + (size_t)6 * query_ct_count * group;
     CK(tmp.alloc_bytes((void **)&d_msg, msg_bytes + 32));  // + 32 zero bytes: the seed a .full ciphertext expands
     CK(tmp.alloc(&d_query, ct_words * query_ct_count * group));
@@ -855,11 +791,15 @@ int32_t respond_proto(const hecuda_context *h, const hecuda_evk *const *evks, in
     CK(tmp.alloc_bytes((void **)&d_out, (size_t)rl.size * group));
     CK(tmp.alloc_bytes((void **)&d_pack, pack.size() * sizeof(long long)));
     CK(tmp.alloc_bytes((void **)&d_tables, table_words * sizeof(long long)));
+    CK(tmp.alloc_bytes((void **)&d_runs, frame.table.size() * sizeof(long long)));
+    CK(tmp.alloc_bytes((void **)&d_frame, frame.bytes.size()));
     CodecConsts full_cc;
     std::string err;
     std::vector<std::vector<long long>> staged;  // host tables stay alive until the stream is drained
     DrainOnExit drain{s};  // copies of the caller's buffers are in flight on `s` from here on
     CK(cudaMemcpyAsync(d_pack, pack.data(), pack.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_runs, frame.table.data(), frame.table.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_frame, frame.bytes.data(), frame.bytes.size(), cudaMemcpyHostToDevice, s));
     CK(cudaMemsetAsync(d_msg + msg_bytes, 0, 32, s));
     for (int32_t first = 0; first < client_count; first += group) {
         const int clients = std::min<int32_t>(group, client_count - first);
@@ -870,7 +810,9 @@ int32_t respond_proto(const hecuda_context *h, const hecuda_evk *const *evks, in
             CK(cudaMemcpyAsync(d_msg + at, messages[first + j], message_byte_counts[first + j], cudaMemcpyHostToDevice, s));
             at += (long long)message_byte_counts[first + j];
         }
-        const GroupTables t = group_tables(queries, first, clients, msg_at, (long long)msg_bytes);
+        std::vector<const std::vector<pirproto::Ciphertext> *> cts_of((size_t)clients);
+        for (int j = 0; j < clients; ++j) cts_of[(size_t)j] = &queries[(size_t)(first + j)].cts;
+        const GroupTables t = group_tables(cts_of, msg_at, (long long)msg_bytes);
         staged.emplace_back(t.tag);
         std::vector<long long> &flat = staged.back();
         flat.insert(flat.end(), t.seed.begin(), t.seed.end());
@@ -896,7 +838,7 @@ int32_t respond_proto(const hecuda_context *h, const hecuda_evk *const *evks, in
                            d_resp, s);
         if (rc) return rc;
         const int64_t cts = replies * clients;
-        if ((e = launch(response_frame_kernel, (unsigned)((cts + 255) / 256), 256, 0, s, d_out, (long long)cts, frame)) != cudaSuccess)
+        if ((e = launch_frame_runs(d_out, clients, rl.size, d_runs, frame.runs(), d_frame, s)) != cudaSuccess)
             return cuda_fail(e, "frame response");
         for (int p = 0; p < 2; ++p) {
             PolyLayout at;

@@ -14,6 +14,7 @@
 // buffer is client-major, each rotation is one key-switching pass over the whole group with a per-client key table,
 // and the matrix streams once per group (the many-clients scan).  A group of one issues the single-client launches.
 #include <algorithm>
+#include <set>
 
 #include "capi_internal.hpp"
 #include "wire_codec.hpp"
@@ -155,6 +156,7 @@ struct MatrixQuery {
     int32_t column_step;
     const int32_t *pack_rotations;     // single rotations composing rotateColumnsMultiStep(by: matrix.rowCount)
     int32_t pack_rotation_count;
+    const u64 *device_masks = nullptr;  // host_masks already on the device (the protobuf call encodes them there)
 };
 
 // What the matrix and query shapes fix: S query rows per SIMD row of a packed result, G packing groups, the ciphertexts
@@ -352,9 +354,13 @@ int32_t mul_transpose_matrix_device(const hecuda_context *h, const PnnsKeys *key
                              (size_t)clients, cudaMemcpyDeviceToDevice, s));
     } else {
         const unsigned step_element = rotating_columns(q.column_step, n);
-        CK(tmp.alloc(&masks, (size_t)n * R));
         CK(tmp.alloc(&mask_eval, (size_t)L * n * R));
-        CK(cudaMemcpyAsync(masks, q.host_masks, (size_t)n * R * sizeof(u64), cudaMemcpyHostToDevice, s));
+        if (q.device_masks) {
+            masks = const_cast<u64 *>(q.device_masks);
+        } else {
+            CK(tmp.alloc(&masks, (size_t)n * R));
+            CK(cudaMemcpyAsync(masks, q.host_masks, (size_t)n * R * sizeof(u64), cudaMemcpyHostToDevice, s));
+        }
         // ciphertextEval *= plaintextMask (:322-324)
         if (clients == 1) {
             for (int64_t r = 0; r < R; ++r)
@@ -472,7 +478,8 @@ int32_t check_matrix_query(const Context &c, int32_t ciphertext_count, const Mat
     if (ciphertext_count < 1 || q.rows < 1 || q.pack_rotation_count < 0 || (q.pack_rotation_count && !q.pack_rotations))
         return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
     if (q.rows > 1) {
-        if (!q.ciphertext_index || !q.host_masks || !q.rotate_count) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null row descriptors");
+        if (!q.ciphertext_index || !(q.host_masks || q.device_masks) || !q.rotate_count)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "null row descriptors");
         if (q.column_step < 1 || q.column_step > c.n / 2) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
         for (int32_t r = 0; r < q.rows; ++r)
             if (q.ciphertext_index[r] < 0 || q.ciphertext_index[r] >= ciphertext_count || q.rotate_count[r] < 0)
@@ -974,6 +981,289 @@ int32_t hecuda_pnns_compute_response_clients_wire(const hecuda_context *h, const
     WireCodec wc;
     if ((rc = wc.setup(*h->ctx, skip_lsbs_poly0, skip_lsbs_poly1))) return rc;
     return respond_clients(h, keys, m, q, ciphertext_count, *out_count, query_poly0, query_seeds, &wc, out, out_capacity);
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------- protobuf messages in and out
+// PNNSRequest in, PNNSShardResponse out (pnns_proto.hpp), the query plan derived here (pnns_plan.hpp).  The device
+// path is respond_clients' with the messages read in place, as the PIR protobuf path does (proto_respond.hpp).
+#include "pnns_plan.hpp"
+#include "pnns_proto.hpp"
+#include "proto_respond.hpp"
+
+namespace {
+
+// The response of one call: per context its reply codec (Bfv.skipLSBsForDecryption of its t), the replies per client
+// and the PNNSShardResponse layout
+struct ShardReply {
+    std::vector<WireCodec> wc;
+    int64_t outputs = 0;
+    pnnsproto::ShardLayout layout;
+};
+int32_t shard_reply(const hecuda_context *const *ctxs, int32_t count, const hecuda_pnns_matrix *const *ms, int64_t query_rows,
+                    const uint64_t *ids, int64_t id_count, const uint8_t *metadata, const uint64_t *metadata_offsets,
+                    int64_t metadata_count, ShardReply &r) {
+    if (!ctxs || !ms || count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (id_count < 0 || metadata_count < 0 || (id_count && !ids) || (metadata_count && !metadata_offsets))
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    for (int64_t i = 0; i < metadata_count; ++i)
+        if (metadata_offsets[i + 1] < metadata_offsets[i]) return fail(HECUDA_ERR_INVALID_ARGUMENT, "metadata offsets decrease");
+    if (metadata_count && metadata_offsets[metadata_count] > metadata_offsets[0] && !metadata)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (query_rows < 1 || query_rows > 0xffffffffLL) return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions");
+    std::vector<std::array<long long, 2>> bytes;
+    std::vector<std::array<int, 2>> skips;
+    r.wc.assign((size_t)count, WireCodec{});
+    for (int32_t k = 0; k < count; ++k) {
+        int32_t rc = check_ctx(ctxs[k]);
+        if (rc) return rc;
+        if (!ms[k] || ms[k]->owner != ctxs[k])
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongContext: plaintext matrix " + std::to_string(k) + " belongs to another context");
+        if (ms[k]->row_count != ms[0]->row_count || ms[k]->column_count != ms[0]->column_count)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "invalidMatrixDimensions: the plaintext matrices differ in shape");
+        const Context &c = *ctxs[k]->ctx;
+        int skip[2];
+        pnnsproto::skip_lsbs_for_decryption(c.q[0], c.t, c.n, skip);
+        if ((rc = r.wc[(size_t)k].setup(c, skip[0], skip[1]))) return rc;
+        bytes.push_back({(long long)r.wc[(size_t)k].bytes[0], (long long)r.wc[(size_t)k].bytes[1]});
+        skips.push_back({skip[0], skip[1]});
+    }
+    // matrix_shape: S query rows per SIMD row, G packing groups; one reply per pair of groups, or per (row, result)
+    const Context &c = *ctxs[0]->ctx;
+    const int64_t S = (c.n / 2) / ms[0]->row_count, G = S > 0 ? (query_rows + S - 1) / S : 0;
+    r.outputs = S > 0 ? (G + 1) / 2 : query_rows * ms[0]->result_count;
+    r.layout = pnnsproto::place_shard_response(bytes, skips, r.outputs, (uint64_t)ms[0]->row_count, (uint64_t)query_rows, ids,
+                                               id_count, metadata, metadata_offsets, metadata_count);
+    return HECUDA_OK;
+}
+
+// respond_clients with PNNSRequest messages in and PNNSShardResponse messages out.  Per group: the group's messages
+// uploaded back to back; per context the seeded expansion reading them in place (and the .full ciphertexts loaded over
+// theirs), the group's responses and one packing launch per reply poly into the clients' messages; the framing of
+// every message in one launch (before the packing, which writes between its runs); one download.
+int32_t respond_proto(const hecuda_context *const *ctxs, int32_t count, const hecuda_pnns_matrix *const *ms,
+                      int32_t client_count, const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                      const std::vector<std::vector<pnnsproto::Matrix>> &queries, const std::vector<pnnsplan::QueryPlan> &plans,
+                      std::vector<MatrixQuery> &qs, const std::vector<std::vector<PnnsKeys>> &keys, const ShardReply &r,
+                      uint8_t *out) {
+    const hecuda_context *h = ctxs[0];
+    const pnnsproto::ShardLayout &sl = r.layout;
+    const int group = std::min<int32_t>(HECUDA_PNNS_CLIENT_GROUP, client_count);
+    const int64_t outputs = r.outputs, R = plans[0].rows, cts = plans[0].ciphertexts;
+    size_t msg_bytes = 0, ct_words = 0;
+    for (int32_t first = 0; first < client_count; first += group) {
+        size_t bytes = 0;
+        for (int32_t j = first; j < std::min<int32_t>(first + group, client_count); ++j) bytes += message_byte_counts[j];
+        msg_bytes = std::max(msg_bytes, bytes);
+    }
+    for (int32_t k = 0; k < count; ++k) ct_words = std::max(ct_words, (size_t)2 * ctxs[k]->ctx->L * ctxs[k]->ctx->n);
+    FrameRuns frame;
+    frame.size = sl.size;
+    sl.frame([&](long long at, const pnnsproto::Bytes &b) { frame.put(at, b); });
+    // reply ciphertext i of a group (client-major) is polys 2i, 2i + 1 of the group's responses; on context k its poly p
+    // goes to byte tag[i] of the group's messages
+    const size_t span = (size_t)group * outputs + 1;
+    std::vector<long long> pack((size_t)count * 4 * span);
+    for (int32_t k = 0; k < count; ++k)
+        for (int p = 0; p < 2; ++p) {
+            long long *tag = pack.data() + ((size_t)k * 2 + p) * 2 * span, *slot = tag + span;
+            for (int64_t i = 0; i < group * outputs; ++i) {
+                tag[i] = (i / outputs) * sl.size + sl.poly_at((size_t)k, i % outputs, p);
+                slot[i] = 2 * i + p;
+            }
+            tag[span - 1] = group * sl.size;
+        }
+    WsGuard g(h);
+    if (!g.w) return fail(HECUDA_ERR_CUDA, "could not create a CUDA stream / workspace");
+    cudaStream_t s = g.w->stream;
+    StreamBuffers tmp(s);
+    unsigned char *d_msg = nullptr, *d_out = nullptr, *d_frame = nullptr;
+    u64 *d_query = nullptr, *d_resp = nullptr, *d_values = nullptr, *d_masks = nullptr;
+    long long *d_pack = nullptr, *d_tables = nullptr, *d_runs = nullptr;
+    const size_t table_words = (size_t)2 * cts * group + 1 + (size_t)6 * cts * group;
+    const int64_t n = ctxs[0]->ctx->n;
+    CK(tmp.alloc_bytes((void **)&d_msg, msg_bytes + 32));  // + 32 zero bytes: the seed a .full ciphertext expands
+    CK(tmp.alloc(&d_query, ct_words * cts * group));
+    CK(tmp.alloc(&d_resp, (size_t)2 * n * outputs * group));
+    CK(tmp.alloc_bytes((void **)&d_out, (size_t)sl.size * group));
+    CK(tmp.alloc_bytes((void **)&d_pack, pack.size() * sizeof(long long)));
+    CK(tmp.alloc_bytes((void **)&d_tables, table_words * sizeof(long long)));
+    CK(tmp.alloc_bytes((void **)&d_runs, frame.table.size() * sizeof(long long)));
+    CK(tmp.alloc_bytes((void **)&d_frame, frame.bytes.size()));
+    if (R > 1) {
+        CK(tmp.alloc(&d_values, (size_t)R * n));
+        CK(tmp.alloc(&d_masks, (size_t)count * R * n));
+    }
+    CodecConsts full_cc;
+    std::string err;
+    std::vector<std::vector<long long>> staged;  // host tables stay alive until the stream is drained
+    DrainOnExit drain{s};  // copies of the caller's buffers are in flight on `s` from here on
+    CK(cudaMemcpyAsync(d_pack, pack.data(), pack.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_runs, frame.table.data(), frame.table.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_frame, frame.bytes.data(), frame.bytes.size(), cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(d_msg + msg_bytes, 0, 32, s));
+    cudaError_t e;
+    for (int32_t k = 0; k < count && R > 1; ++k) {  // extractDenseRow's masks, SIMD-encoded once per context
+        CK(cudaMemcpyAsync(d_values, plans[(size_t)k].mask_values.data(), (size_t)R * n * sizeof(u64), cudaMemcpyHostToDevice, s));
+        u64 *masks = d_masks + (size_t)k * R * n;
+        if ((e = launch_encode_simd(*ctxs[k]->ctx, d_values, (int)n, 0, masks, nullptr, R, s)) != cudaSuccess)
+            return cuda_fail(e, "encode masks");
+        qs[(size_t)k].device_masks = masks;
+    }
+    for (int32_t first = 0; first < client_count; first += group) {
+        const int clients = std::min<int32_t>(group, client_count - first);
+        std::vector<long long> msg_at((size_t)clients);
+        long long at = 0;
+        for (int j = 0; j < clients; ++j) {
+            msg_at[(size_t)j] = at;
+            CK(cudaMemcpyAsync(d_msg + at, messages[first + j], message_byte_counts[first + j], cudaMemcpyHostToDevice, s));
+            at += (long long)message_byte_counts[first + j];
+        }
+        if ((e = launch_frame_runs(d_out, clients, sl.size, d_runs, frame.runs(), d_frame, s)) != cudaSuccess)
+            return cuda_fail(e, "frame response");
+        for (int32_t k = 0; k < count; ++k) {
+            const Context &c = *ctxs[k]->ctx;
+            std::vector<const std::vector<pnnsproto::Ciphertext> *> cts_of((size_t)clients);
+            for (int j = 0; j < clients; ++j) cts_of[(size_t)j] = &queries[(size_t)(first + j)][(size_t)k].cts;
+            const GroupTables t = group_tables(cts_of, msg_at, (long long)msg_bytes);
+            staged.emplace_back(t.tag);
+            std::vector<long long> &flat = staged.back();
+            flat.insert(flat.end(), t.seed.begin(), t.seed.end());
+            for (const auto &f : t.full) flat.insert(flat.end(), f.second.begin(), f.second.end());
+            CK(cudaMemcpyAsync(d_tables, flat.data(), flat.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+            PolyLayout seeded;
+            seeded.tag = d_tables, seeded.seed = d_tables + t.tag.size(), seeded.frame = 0;
+            const int64_t batch = cts * clients;
+            if ((e = expand_seeded_device(c, c.L, d_msg, nullptr, d_query, batch, s, seeded)) != cudaSuccess)
+                return cuda_fail(e, "expand seeded query");
+            // .full query ciphertexts (Ciphertext(deserialize:) of .full): both polys over the zero rows expanded above
+            const long long *table = seeded.seed + t.seed.size();
+            for (const auto &f : t.full) {
+                const int64_t full = (int64_t)(f.second.size() - 1) / 2;
+                if (!codec_consts(c, c.map_q(c.L), f.first, full_cc, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+                PolyLayout layout;
+                layout.tag = table, layout.slot = table + full + 1, layout.frame = 0;
+                if ((e = launch_poly_load(c, full_cc, f.first, d_msg, d_query, full, s, layout)) != cudaSuccess)
+                    return cuda_fail(e, "load full query ciphertexts");
+                table += f.second.size();
+            }
+            int32_t rc = mul_transpose_matrix_device(ctxs[k], keys[(size_t)k].data() + first, clients, ms[k], d_query, cts,
+                                                     qs[(size_t)k], true, d_resp, s);
+            if (rc) return rc;
+            const WireCodec &wc = r.wc[(size_t)k];
+            for (int p = 0; p < 2; ++p) {
+                PolyLayout to;
+                to.tag = d_pack + ((size_t)k * 2 + p) * 2 * span, to.slot = to.tag + span, to.frame = 0;
+                if ((e = launch_poly_serialize(c, wc.out[p], wc.skip[p], d_resp, d_out, outputs * clients, s, to)) != cudaSuccess)
+                    return cuda_fail(e, "serialize response");
+            }
+        }
+        CK(cudaMemcpyAsync(out + (size_t)sl.size * first, d_out, (size_t)sl.size * clients, cudaMemcpyDeviceToHost, s));
+    }
+    CK(wait_stream(s));
+    return HECUDA_OK;
+}
+
+// The Galois elements a client's key holds (GaloisElement.stepsFor's input for the packing plan)
+std::set<uint64_t> galois_elements(const hecuda_evk *k) {
+    hecuda_evk *km = const_cast<hecuda_evk *>(k);
+    std::lock_guard<std::mutex> g(km->mu);
+    std::set<uint64_t> out;
+    for (const auto &e : km->galois) out.insert(e.first);
+    return out;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t hecuda_pnns_shard_response_byte_count(const hecuda_context *const *ctxs, int32_t count,
+                                              const hecuda_pnns_matrix *const *matrices, int32_t query_row_count,
+                                              const uint64_t *entry_ids, int64_t id_count, const uint8_t *metadata,
+                                              const uint64_t *metadata_offsets, int64_t metadata_count, uint64_t *bytes) {
+    if (!bytes) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    ShardReply r;
+    int32_t rc = shard_reply(ctxs, count, matrices, query_row_count, entry_ids, id_count, metadata, metadata_offsets,
+                             metadata_count, r);
+    if (rc) return rc;
+    *bytes = (uint64_t)r.layout.size;
+    return HECUDA_OK;
+}
+
+int32_t hecuda_pnns_compute_response_clients_proto(const hecuda_context *const *ctxs, int32_t count,
+                                                   const hecuda_evk *const *evks, int32_t client_count,
+                                                   const hecuda_pnns_matrix *const *matrices,
+                                                   const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                                                   const uint64_t *entry_ids, int64_t id_count, const uint8_t *metadata,
+                                                   const uint64_t *metadata_offsets, int64_t metadata_count, uint8_t *out) {
+    if (!ctxs || count < 1 || !matrices || !evks || !messages || !message_byte_counts || !out)
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    if (client_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "client_count must be at least 1");
+    int32_t rc;
+    std::vector<pnnsproto::PolySizes> sizes((size_t)count);
+    for (int32_t k = 0; k < count; ++k) {
+        if ((rc = check_ctx(ctxs[k]))) return rc;
+        if (!matrices[k] || matrices[k]->owner != ctxs[k])
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "wrongContext: plaintext matrix " + std::to_string(k) + " belongs to another context");
+        const Context &c = *ctxs[k]->ctx;
+        CodecConsts qc;
+        std::string err;
+        if (!codec_consts(c, c.map_q(c.L), 0, qc, err)) return fail(HECUDA_ERR_INVALID_ARGUMENT, err);
+        sizes[(size_t)k] = pnnsproto::poly_sizes(qc, c.n);
+    }
+    // every client's request walked and checked against the database, and against client 0's shape
+    std::vector<std::vector<pnnsproto::Matrix>> queries((size_t)client_count);
+    for (int32_t j = 0; j < client_count; ++j) {
+        const std::string who = "client " + std::to_string(j) + ": ";
+        if (!messages[j] && message_byte_counts[j]) return fail(HECUDA_ERR_INVALID_ARGUMENT, who + "null argument");
+        pnnsproto::Error e;
+        pnnsproto::Request req;
+        if (!pnnsproto::walk_pnns_request(messages[j], (long long)message_byte_counts[j], req, e) ||
+            !pnnsproto::walk_query(messages[j], req, sizes, (uint64_t)matrices[0]->column_count, queries[(size_t)j], e))
+            return fail(e.code, who + e.what);
+        if (queries[(size_t)j][0].rows != queries[0][0].rows)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, who + "invalidMatrixDimensions: a query of " +
+                                                         std::to_string(queries[(size_t)j][0].rows) + " rows, client 0's has " +
+                                                         std::to_string(queries[0][0].rows));
+    }
+    const int64_t R = (int64_t)queries[0][0].rows;
+    ShardReply reply;
+    if ((rc = shard_reply(ctxs, count, matrices, R, entry_ids, id_count, metadata, metadata_offsets, metadata_count, reply)))
+        return rc;
+    // keys: any context of the same N, word size and coefficient moduli (EvaluationKey.forContext's test), read in place
+    for (int32_t j = 0; j < client_count; ++j) {
+        const std::string who = "client " + std::to_string(j) + ": ";
+        if (!evks[j]) return fail(HECUDA_ERR_MISSING_KEY, who + "missingGaloisKey");
+        if (!evks[j]->owner) return fail(HECUDA_ERR_MISSING_KEY, who + "null evaluation key");
+        const Context &a = *evks[j]->owner->ctx;
+        for (int32_t k = 0; k < count; ++k) {
+            const Context &b = *ctxs[k]->ctx;
+            if (a.n != b.n || a.word_bits != b.word_bits || a.q != b.q || a.q_ks != b.q_ks)
+                return fail(HECUDA_ERR_INVALID_ARGUMENT, who + "invalidContext: the key's context differs from context " +
+                                                             std::to_string(k) + " in N, word size or coefficient moduli");
+        }
+    }
+    // the query plan, once per call, from the shape and client 0's Galois elements; every key of every client found
+    const std::set<uint64_t> elements = galois_elements(evks[0]);
+    std::vector<pnnsplan::QueryPlan> plans((size_t)count);
+    std::vector<MatrixQuery> qs;
+    std::vector<std::vector<PnnsKeys>> keys((size_t)count, std::vector<PnnsKeys>((size_t)client_count));
+    for (int32_t k = 0; k < count; ++k) {
+        const Context &c = *ctxs[k]->ctx;
+        pnnsplan::QueryPlan &p = plans[(size_t)k];
+        std::string err;
+        if (!pnnsplan::plan_query(c.n, R, matrices[k]->column_count, matrices[k]->row_count, elements, p, err))
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "client 0: " + err);
+        // the masks are encoded on the device by respond_proto (device_masks); the plan is in range by construction
+        qs.push_back(MatrixQuery{p.rows, p.index.data(), nullptr, p.rotate.data(), p.column_step, p.pack.data(),
+                                 (int32_t)p.pack.size()});
+        const MatrixShape sh = matrix_shape(c, matrices[k], qs.back());
+        for (int32_t j = 0; j < client_count; ++j)
+            if ((rc = matrix_keys(evks[j], c.n, matrices[k], qs.back(), sh, keys[(size_t)k][(size_t)j])))
+                return fail(rc, "client " + std::to_string(j) + ": " + last_error_cstr());
+    }
+    return respond_proto(ctxs, count, matrices, client_count, messages, message_byte_counts, queries, plans, qs, keys, reply, out);
 }
 
 }  // extern "C"

@@ -202,6 +202,14 @@ SYMBOLS = {
                                                               C.c_int32, C.POINTER(C.c_int32), _VP, C.POINTER(C.c_int32),
                                                               C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32,
                                                               C.c_int32, _VP, C.c_int64, C.POINTER(C.c_int64)]),
+    "hecuda_pnns_request_fields_read": (C.c_int32, [_VP, C.c_uint64, _VP, _VP, C.c_int64, _VP, C.c_int64]),
+    "hecuda_pnns_shard_response_byte_count": (C.c_int32, [_VP, C.c_int32, _VP, C.c_int32, _VP, C.c_int64, _VP, _VP, C.c_int64,
+                                                          _VP]),
+    "hecuda_pnns_compute_response_clients_proto": (C.c_int32, [_VP, C.c_int32, _VP, C.c_int32, _VP, _VP, _VP, _VP, C.c_int64,
+                                                               _VP, _VP, C.c_int64, _VP]),
+    "hecuda_pnns_request_write": (C.c_int32, [_VP, C.c_int32, C.c_uint32, C.c_uint32, _VP, _VP, C.c_int32, _VP, C.c_uint64,
+                                              _VP, C.c_uint64, C.c_uint64, _VP, C.c_uint64, _VP, C.c_uint64, _VP]),
+    "hecuda_pnns_shard_response_read": (C.c_int32, [_VP, C.c_int32, _VP, C.c_uint64, _VP, _VP, _VP, _VP, _VP]),
     "hecuda_poly_serialized_byte_count": (C.c_int32, [_VP, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
     "hecuda_poly_serialize": (C.c_int32, [_VP, C.c_int32, _VP, C.c_int32, _VP, C.c_int32, C.c_int64]),
     "hecuda_poly_load": (C.c_int32, [_VP, C.c_int32, _VP, C.c_int32, _VP, C.c_int32, C.c_int64]),

@@ -501,6 +501,63 @@ class PnnsWire:
         return out[:, : produced.value], skips
 
 
+class PnnsRequestFields(C.Structure):
+    """hecuda_pnns_request_fields (include/hecuda.h)."""
+    _fields_ = [("query_count", C.c_int32), ("query_row_count", C.c_uint32), ("has_evaluation_key", C.c_int32),
+                ("has_key_metadata", C.c_int32), ("shard_index_count", C.c_int64), ("shard_id_count", C.c_int64),
+                ("config_id_offset", C.c_uint64), ("config_id_bytes", C.c_uint64),
+                ("evaluation_key_offset", C.c_uint64), ("evaluation_key_bytes", C.c_uint64),
+                ("key_timestamp", C.c_uint64), ("key_identifier_offset", C.c_uint64), ("key_identifier_bytes", C.c_uint64)]
+
+
+class PnnsShardResponseShape(C.Structure):
+    """hecuda_pnns_shard_response_shape (include/hecuda.h)."""
+    _fields_ = [("matrix_count", C.c_int32), ("reply_count", C.c_int32), ("row_count", C.c_uint32),
+                ("column_count", C.c_uint32), ("id_count", C.c_int64), ("metadata_count", C.c_int64)]
+
+
+class PnnsRequest:
+    """api.pnns.v1.PNNSRequest, the envelope a PNNS server receives."""
+
+    @staticmethod
+    def fields(message) -> dict:
+        """The walk of a PNNSRequest (hecuda_pnns_request_fields_read), nothing copied on the host side: queryCount and
+        queryRowCount (the matrices' common num_rows), configId, the key metadata (keyTimestamp, keyIdentifier; from
+        evaluation_key_metadata, or evaluation_key.metadata when that is absent), the (offset, length) range of
+        evaluation_key.evaluation_key (a SerializedEvaluationKey for EvaluationKey.fromProtoMany; None when unset),
+        shardIndices and shardIds.  Routing by shard and caching keys by identifier stay the caller's."""
+        b = bytes(message)
+        r = PnnsRequestFields()
+        lib = load_library()
+        _check(lib.hecuda_pnns_request_fields_read(b, len(b), C.byref(r), None, 0, None, 0))
+        indices = (C.c_uint32 * max(1, r.shard_index_count))()
+        ranges = (C.c_uint64 * max(2, 2 * r.shard_id_count))()
+        _check(lib.hecuda_pnns_request_fields_read(b, len(b), C.byref(r), indices, r.shard_index_count, ranges,
+                                                   r.shard_id_count))
+
+        def span(offset, size):
+            return b[offset:offset + size]
+
+        return {
+            "queryCount": r.query_count,
+            "queryRowCount": r.query_row_count,
+            "configId": span(r.config_id_offset, r.config_id_bytes),
+            "keyTimestamp": r.key_timestamp if r.has_key_metadata else None,
+            "keyIdentifier": span(r.key_identifier_offset, r.key_identifier_bytes) if r.has_key_metadata else None,
+            "evaluationKey": (r.evaluation_key_offset, r.evaluation_key_bytes) if r.has_evaluation_key else None,
+            "shardIndices": list(indices[:r.shard_index_count]),
+            "shardIds": [span(ranges[2 * i], ranges[2 * i + 1]).decode() for i in range(r.shard_id_count)],
+        }
+
+
+def _message_buffers(messages):
+    buffers = [np.frombuffer(m, dtype=np.uint8) if isinstance(m, (bytes, bytearray, memoryview)) else
+               np.ascontiguousarray(m, dtype=np.uint8).reshape(-1) for m in messages]
+    keep = [b if b.size else np.zeros(1, np.uint8) for b in buffers]
+    counts = np.array([b.size for b in buffers], dtype=np.uint64)
+    return (C.c_void_p * len(keep))(*[b.ctypes.data for b in keep]), counts, keep
+
+
 def denseRowVector(context, vector) -> np.ndarray:
     """The SIMD values of a one-row `.denseRow` matrix (PlaintextMatrix.swift:341-413): the row padded to a power of
     two and repeated to fill both SIMD rows.  Returns the coefficient plaintext (N,)."""
@@ -899,6 +956,64 @@ class Client:
             out.append((poly0, a) if wire else cts)
         return Query(out, dims, wire)
 
+    def evaluationKeyMessage(self, secretKey):
+        """generateEvaluationKey as the reference's client sends it: (key, SerializedEvaluationKey.proto() bytes) of a
+        seeded key on contexts[0]."""
+        from .pir import evaluationKeyMessage
+        key, form = EvaluationKey.generate(self.contexts[0], self.evaluationKeyConfig, secretKey, wire=True)
+        return key, evaluationKeyMessage(self.contexts[0], form)
+
+    def requestMessage(self, vectors, secretKey, evaluationKey=None, keyTimestamp: int = 0, keyIdentifier: bytes = b"",
+                       configId: bytes = b"", aSeeds=None, errorSeeds=None) -> bytes:
+        """generateQuery as the reference's client sends it: Query.proto() in an api.pnns.v1.PNNSRequest
+        (hecuda_pnns_request_write), one .denseRow matrix of .seeded ciphertexts per plaintext modulus, with
+        generateQuery(wire=True)'s seeds.  evaluationKey: a SerializedEvaluationKey message (evaluationKeyMessage's
+        bytes) to send in evaluation_key, with its metadata; configId: the PNNSConfig identifier."""
+        query = self.generateQuery(vectors, secretKey, wire=True, aSeeds=aSeeds, errorSeeds=errorSeeds)
+        from .pir import _written
+        poly0 = [np.ascontiguousarray(m[0]) for m in query.ciphertextMatrices]
+        seeds = [np.ascontiguousarray(m[1]) for m in query.ciphertextMatrices]
+        count = seeds[0].shape[0]
+        K = len(self.contexts)
+        ctxs = (C.c_void_p * K)(*[c._h.value for c in self.contexts])
+        p0 = (C.c_void_p * K)(*[a.ctypes.data for a in poly0])
+        sd = (C.c_void_p * K)(*[a.ctypes.data for a in seeds])
+        key = bytes(evaluationKey) if evaluationKey is not None else None
+        ident, config = bytes(keyIdentifier), bytes(configId)
+        return _written(lambda out, capacity, written: load_library().hecuda_pnns_request_write(
+            ctxs, K, query.dimensions.rowCount, query.dimensions.columnCount, p0, sd, count, config or None, len(config),
+            key, len(key) if key is not None else 0, keyTimestamp, ident or None, len(ident), out, capacity, written))
+
+    def decryptResponseMessage(self, message, secretKey) -> DatabaseDistances:
+        """decrypt of an api.pnns.v1.PNNSShardResponse: its matrices found by hecuda_pnns_shard_response_read, each
+        reply's polys loaded with its matrix's skip bits, then decrypt; the entry ids and metadata from the message."""
+        b = np.frombuffer(bytes(message), dtype=np.uint8)
+        buf = b if b.size else np.zeros(1, np.uint8)
+        K = len(self.contexts)
+        ctxs = (C.c_void_p * K)(*[c._h.value for c in self.contexts])
+        lib = load_library()
+        shape = PnnsShardResponseShape()
+        _check(lib.hecuda_pnns_shard_response_read(ctxs, K, buf.ctypes.data_as(C.c_void_p), b.size, C.byref(shape), None,
+                                                   None, None, None))
+        offsets = np.empty(max(1, K * shape.reply_count), dtype=np.uint64)
+        skips = np.empty(2 * K, dtype=np.int32)
+        ids = np.empty(max(1, shape.id_count), dtype=np.uint64)
+        ranges = np.empty(max(2, 2 * shape.metadata_count), dtype=np.uint64)
+        _check(lib.hecuda_pnns_shard_response_read(ctxs, K, buf.ctypes.data_as(C.c_void_p), b.size, C.byref(shape),
+                                                   _ptr(offsets), skips.ctypes.data_as(C.c_void_p), _ptr(ids), _ptr(ranges)))
+        from . import Bfv
+        matrices = []
+        for k, ctx in enumerate(self.contexts):
+            s = [int(skips[2 * k]), int(skips[2 * k + 1])]
+            size = sum(Bfv.serializationByteCount(ctx, 1, x) for x in s)
+            rows = np.stack([b[int(o):int(o) + size] for o in offsets[k * shape.reply_count:(k + 1) * shape.reply_count]])
+            matrices.append((rows, s))
+        metadata = [b[int(ranges[2 * i]):int(ranges[2 * i] + ranges[2 * i + 1])].tobytes()
+                    for i in range(shape.metadata_count)]
+        response = Response(matrices, MatrixDimensions(shape.row_count, shape.column_count),
+                            [int(v) for v in ids[:shape.id_count]], metadata)
+        return self.decrypt(response, secretKey)
+
     def decrypt(self, response: Response, secretKey) -> DatabaseDistances:
         """Client.decrypt (Client.swift:99-127) on the device (hecuda_pnns_decrypt_distances): float32 distances,
         database rows x query rows."""
@@ -1140,3 +1255,35 @@ class Server:
         out_dims = MatrixDimensions(self.database.plaintextMatrices[0].dimensions.rowCount, dims.rowCount)
         return [Response([per_matrix[k][c] for k in range(len(per_matrix))], out_dims, list(self.database.entryIds),
                          list(self.database.entryMetadatas)) for c in range(len(queries))]
+
+    def computeResponsesProto(self, messages, evaluationKeys) -> list:
+        """computeResponses with protobuf messages (hecuda_pnns_compute_response_clients_proto): one
+        api.pnns.v1.PNNSRequest per client in (only its query matrices are read; .seeded or .full ciphertexts), one
+        api.pnns.v1.PNNSShardResponse per client out, with the database's entry ids and metadata.  The query plan is
+        derived in the library from the message's shape.  Keys loaded on contexts[0] (e.g. by
+        EvaluationKey.fromProtoMany) serve every plaintext modulus as they are, with no forContext copies."""
+        keys = list(evaluationKeys)
+        ptrs, counts, keep = _message_buffers(messages)
+        if not keys or len(keep) != len(keys):
+            raise PnnsError(f"computeResponsesProto: {len(keep)} messages for {len(keys)} evaluation keys")
+        db = self.database
+        K = len(db.plaintextMatrices)
+        ctxs = (C.c_void_p * K)(*[m.context._h.value for m in db.plaintextMatrices])
+        handles = (C.c_void_p * K)(*[m._h.value for m in db.plaintextMatrices])
+        ids = np.ascontiguousarray(np.asarray(db.entryIds, dtype=np.uint64)).reshape(-1)
+        meta = [bytes(m) for m in db.entryMetadatas]
+        offsets = np.zeros(len(meta) + 1, dtype=np.uint64)
+        offsets[1:] = np.cumsum([len(m) for m in meta], dtype=np.uint64)
+        blob = np.frombuffer(b"".join(meta) or b"\0", dtype=np.uint8)
+        entries = (_ptr(ids) if ids.size else None, ids.size, blob.ctypes.data_as(C.c_void_p), _ptr(offsets), len(meta))
+        lib = load_library()
+        first = PnnsRequest.fields(bytes(keep[0][:int(counts[0])]))
+        size = C.c_uint64(0)
+        _check(lib.hecuda_pnns_shard_response_byte_count(ctxs, K, handles, max(1, first["queryRowCount"]), *entries,
+                                                         C.byref(size)))
+        out = np.empty((len(keys), size.value), dtype=np.uint8)
+        key_handles = (C.c_void_p * len(keys))(*[k._h.value if hasattr(k._h, "value") else k._h for k in keys])
+        _check(lib.hecuda_pnns_compute_response_clients_proto(ctxs, K, key_handles, len(keys), handles, ptrs,
+                                                              counts.ctypes.data_as(C.c_void_p), *entries,
+                                                              out.ctypes.data_as(C.c_void_p)))
+        return [row.tobytes() for row in out]
