@@ -616,6 +616,101 @@ int32_t hecuda_simple_pir_compute_response_shards_device(const hecuda_simple_pir
                                                          const void *requests, int64_t count, void *responses,
                                                          void *stream);
 
+/* ---- SimplePIR in the reference's protobuf messages (simple_pir_proto.hpp) ----
+ * Requests as the reference's clients send them and responses as they expect them: api.pir.v1.SimplePIRRequest
+ * { 1 request (pir.v1.SimplePIRMatrix { 1 row_count  2 col_count  3 data, repeated uint64 row-major })  2 shard_index
+ * 3 configuration_hash } and api.pir.v1.SimplePIRResponse { 1 response (SimplePIRMatrix) } (api/pir/v1/pir.proto,
+ * Array2d.proto() / SimplePIRMatrix.native(), PirConversion.swift:380-401).  The walks refuse what the PIR walks refuse
+ * (groups, varints over 10 bytes, lengths past their message, a singular message given twice, a known field of the wrong
+ * wire type); uint32 fields keep the low 32 bits of their varint.  `data` may be packed, packed in several runs, or
+ * unpacked; every form answers alike.
+ *
+ * hecuda_simple_pir_request_fields_read: the walk of a SimplePIRRequest (host only; data is located, not read): whether
+ * request is set, its row and column counts, shard_index, the number of data runs (a packed run, or one unpacked
+ * element) and their bytes, and the byte range of configuration_hash (the library does not check it; nor does the
+ * reference). */
+typedef struct hecuda_simple_pir_request_fields {
+    int32_t has_request;
+    uint32_t row_count, col_count, shard_index;
+    int64_t data_run_count;
+    uint64_t data_bytes;
+    uint64_t configuration_hash_offset, configuration_hash_bytes;
+} hecuda_simple_pir_request_fields;
+int32_t hecuda_simple_pir_request_fields_read(const uint8_t *bytes, uint64_t byte_count,
+                                              hecuda_simple_pir_request_fields *fields);
+/* The walk of `count` SimplePIRRequests against shards (as hecuda_simple_pir_compute_response_proto refuses them) and
+ * each response's capacity: the SimplePIRResponse of row_count x M_s values below 2^ct, each varint ceil(ct / 7) bytes
+ * long, framed as SwiftProtobuf frames it.  Values are uniform below 2^ct, so actual lengths come close to it. */
+int32_t hecuda_simple_pir_response_proto_byte_count(const hecuda_simple_pir_database *const *shards, int32_t shard_count,
+                                                    const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                                                    int64_t count, uint64_t *capacities);
+/* SimplePirServer.computeResponse(to:) (SimplePir+Server.swift:31-38) for `count` SimplePIRRequests, each to the shard
+ * its shard_index names, answered with SimplePIRResponses: message j's response is written at out + out_offsets[j]
+ * (slots of at least hecuda_simple_pir_response_proto_byte_count's capacity, in order) and is out_lengths[j] bytes
+ * long.  Its data equals hecuda_simple_pir_compute_response's for the message's row_count x K_s words, row-major; a
+ * message with row_count 0 gets an empty 0 x M_s matrix (col_count M_s, no data).  The shards must share ct and
+ * ceil(pt / 8); their word sizes may differ.
+ *
+ * Refused on the host, with nothing enqueued, each refusal naming its message ("message <j>: "): every walk refusal
+ * above, an unset request, shard_index >= shard_count, col_count != the shard's databaseColumns (the reference's
+ * precondition traps there), and more rows to one shard than 2^36 / max(K_s, M_s).  Refused on the device, naming the
+ * first bad message and leaving out and out_lengths untouched: a data varint longer than 10 bytes, one that runs past its
+ * run, a value >= 2^32 to a 32-bit shard (the reference's Scalar(_:) traps there), and a varint count other than
+ * row_count x col_count.  Request bits at or above ct are ignored, as in the reference.
+ *
+ * The messages cross PCIe as they are.  On the device, a scan over the varints' last bytes places every value, which is
+ * decoded straight into its shard's request digit planes; all rows to one shard form its query block for one grouped
+ * response launch per group of at most 32 shards that have rows; the responses are encoded straight from the
+ * accumulators (lengths, a scan of them, then every message whole).  A call makes four decode launches, the response
+ * launches and three encode launches, however many messages it has. */
+int32_t hecuda_simple_pir_compute_response_proto(const hecuda_simple_pir_database *const *shards, int32_t shard_count,
+                                                 const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                                                 int64_t count, uint8_t *out, const uint64_t *out_offsets,
+                                                 uint64_t *out_lengths);
+/* Client side, host only.  hecuda_simple_pir_request_write: Array2d.proto() of row_count x col_count words (data, as
+ * uint64) in a SimplePIRRequest with shard_index and configuration_hash (omitted when hash_bytes is 0), data packed.
+ * With out NULL only *written is set; else capacity must hold it.  hecuda_simple_pir_response_read: a SimplePIRResponse's
+ * dimensions and its row_count x col_count values (at most capacity; refused when the count differs). */
+int32_t hecuda_simple_pir_request_write(uint32_t row_count, uint32_t col_count, const uint64_t *data, uint32_t shard_index,
+                                        const uint8_t *configuration_hash, uint64_t hash_bytes, uint8_t *out,
+                                        uint64_t capacity, uint64_t *written);
+int32_t hecuda_simple_pir_response_read(const uint8_t *bytes, uint64_t byte_count, uint32_t *row_count, uint32_t *col_count,
+                                        uint64_t *data, int64_t capacity);
+/* api.pir.v1.SimplePIRConfig as the SimplePIRProcessDatabase tool writes it (main.swift:193-258): pir.v1.DatabaseMapping
+ * { 1 entries { 1 original_index  2 size  3 chunks { 1 shard_index  2 index } }  2 chunk_size }, one
+ * pir.v1.SimplePIRParameters per shard { 1 encryption_params { 1 lattice_dimension  2 error_std_dev (double)
+ * 3 plaintext_bits  4 ciphertext_bits }  2 a_seed  3 entry_size_in_bytes  4 entries_per_column  5 chunks_per_entry
+ * 6 database_columns }, and one hint identifier per shard (SHA-256 of the hint file) -- DatabaseMap.proto() and
+ * SimplePirParameters.proto() / native() (PirConversion.swift:403-518).
+ * hecuda_simple_pir_config_describe: the counts, after every refusal: the walk's, an errorStdDev other than 3.2 or 6.4
+ * and an a_seed that is not 32 bytes (as native() refuses), and every refusal of hecuda_simple_pir_process's
+ * parameters, with word_bits 32 for ct <= 32 and 64 otherwise (main.swift:369-371).  hecuda_simple_pir_config_read
+ * then fills: per entry its original index, size and chunk count; the chunk locations (shard, index) entry-major; each
+ * shard's params and 32-byte seed; each hint identifier's (offset, length) in `bytes`.
+ * hecuda_simple_pir_config_serialized_byte_count / _serialize: the same fields written as SwiftProtobuf writes them. */
+typedef struct hecuda_simple_pir_config_shape {
+    int64_t entry_count, chunk_count;
+    uint64_t chunk_size;
+    int32_t shard_count, hint_identifier_count;
+} hecuda_simple_pir_config_shape;
+int32_t hecuda_simple_pir_config_describe(const uint8_t *bytes, uint64_t byte_count, hecuda_simple_pir_config_shape *shape);
+int32_t hecuda_simple_pir_config_read(const uint8_t *bytes, uint64_t byte_count, uint64_t *original_indices, uint64_t *sizes,
+                                      uint64_t *chunk_counts, int64_t *chunk_locations, hecuda_simple_pir_params *params,
+                                      uint8_t *seeds, uint64_t *hint_identifier_ranges);
+int32_t hecuda_simple_pir_config_serialized_byte_count(const uint64_t *original_indices, const uint64_t *sizes,
+                                                       const uint64_t *chunk_counts, int64_t entry_count,
+                                                       const int64_t *chunk_locations, uint64_t chunk_size,
+                                                       const hecuda_simple_pir_params *params, const uint8_t *seeds,
+                                                       int32_t shard_count, const uint8_t *const *hint_identifiers,
+                                                       const uint64_t *hint_identifier_bytes, int32_t hint_count,
+                                                       uint64_t *bytes);
+int32_t hecuda_simple_pir_config_serialize(const uint64_t *original_indices, const uint64_t *sizes,
+                                           const uint64_t *chunk_counts, int64_t entry_count, const int64_t *chunk_locations,
+                                           uint64_t chunk_size, const hecuda_simple_pir_params *params, const uint8_t *seeds,
+                                           int32_t shard_count, const uint8_t *const *hint_identifiers,
+                                           const uint64_t *hint_identifier_bytes, int32_t hint_count, uint8_t *out,
+                                           uint64_t capacity);
+
 /* SimplePIR's client (SimplePirClient with DefaultQueryGenerator, SimplePir+Client.swift, SimplePir+Precompute.swift).
  * hecuda_simple_pir_client_create: DefaultQueryGenerator.init (SimplePir+Precompute.swift:328-334) from the hint (M x N
  * words), params and seed (32 bytes, params.seed): the aPolyCount polynomials PolyRq.random draws from

@@ -7,14 +7,17 @@
 //   SimplePirServer(processedDatabase:hint:params:), computeResponse   SimplePir+Server.swift:24-38
 //   DatabaseMap.shardDatabase + per-shard process   SimplePir/DatabaseMap.swift:82-110, SimplePIRProcessDatabase/main.swift:158-253
 //   every shard's responses for SimplePirClientForAllShards   SimplePir/SimplePir+Shards.swift:47-173
+//   SimplePIRRequest in, SimplePIRResponse out   PirConversion.swift:380-401, SimplePir+Server.swift:31-38
 #include <algorithm>
 #include <climits>
+#include <cstring>
 #include <vector>
 
 #include "capi_internal.hpp"
 #include "hostmath.hpp"
 #include "ntt_fast.cuh"
 #include "simple_pir.cuh"
+#include "simple_pir_proto.hpp"
 
 using namespace hecuda;
 using namespace hecuda::api;
@@ -339,6 +342,230 @@ __global__ void __launch_bounds__(kThreads) finish_kernel(const u64 *__restrict_
     if (t < words) out[t] = (W)spir::finish(acc[t], ct);
 }
 
+// ---- requests and responses in protobuf messages (simple_pir.cuh, "requests and responses in protobuf messages").
+// Each tile of kProtoTile virtual bytes (decode) or values (encode) is one CTA of kThreads threads, kProtoItems each.
+struct ProtoRun {  // one data run: its first byte in the uploaded messages, its first virtual byte and its length
+    long long src, vbegin, bytes;
+};
+struct DecodeMsg {  // one request message
+    unsigned char *digits;           // its shard's request digit planes
+    long long plane_bytes, col_tiles, columns, row_base, expected;  // expected = row_count x col_count
+    long long tile_begin, run_begin;  // its first tile and run
+    int word32;
+};
+struct EncodeMsg {  // one response message
+    const u64 *acc;                  // its rows' accumulators: rows x columns, row-major
+    long long rows, columns, tile_begin, tile_end;
+    unsigned long long out;          // its slot in the output
+};
+
+__device__ __forceinline__ int find_last_le(const long long *begin, int count, long long key, int stride) {
+    int lo = 0, hi = count - 1;  // the last i with begin[i * stride] <= key (begin[0] <= key)
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) / 2;
+        if (begin[(long long)mid * stride] <= key) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// exclusive scan of one value per thread over the CTA (kThreads); total gets the CTA's sum
+__device__ __forceinline__ unsigned long long block_scan(unsigned long long v, unsigned long long &total) {
+    __shared__ unsigned long long warp_sums[kThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned long long x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_sums[warp] = x;
+    __syncthreads();
+    unsigned long long before = 0;
+    total = 0;
+#pragma unroll
+    for (int w = 0; w < kThreads / 32; ++w) {
+        before += w < warp ? warp_sums[w] : 0;
+        total += warp_sums[w];
+    }
+    __syncthreads();
+    return before + x - v;
+}
+
+// The virtual bytes of thread threadIdx.x of tile `tile`, visited in order: f(byte pointer, run's first byte pointer,
+// whether it is its run's last byte)
+template <typename F>
+__device__ __forceinline__ void for_each_byte(const unsigned char *msgs, const ProtoRun *runs, int run_count, int run_begin,
+                                              int run_end, long long tile, F f) {
+    const long long v0 = tile * spir::kProtoTile + (long long)threadIdx.x * spir::kProtoItems;
+    if (run_begin >= run_end || v0 < runs[run_begin].vbegin) return;
+    int r = run_begin + find_last_le(&runs[run_begin].vbegin, run_end - run_begin, v0, (int)(sizeof(ProtoRun) / 8));
+    for (long long v = v0; v < v0 + spir::kProtoItems; ++v) {
+        while (r < run_end && v >= runs[r].vbegin + runs[r].bytes) ++r;
+        if (r >= run_end) return;
+        if (v < runs[r].vbegin) continue;
+        const long long off = v - runs[r].vbegin;
+        f(msgs + runs[r].src + off, msgs + runs[r].src, off == runs[r].bytes - 1);
+    }
+}
+
+__device__ __forceinline__ int decode_message(const DecodeMsg *m, int count, long long tile) {
+    return find_last_le(&m[0].tile_begin, count, tile, (int)(sizeof(DecodeMsg) / 8));
+}
+
+// decode 1: the varints (bytes with the top bit clear) of every tile -> tile_sums[tile]
+__global__ void __launch_bounds__(kThreads) proto_count_kernel(const unsigned char *__restrict__ msgs,
+                                                               const ProtoRun *__restrict__ runs, int run_count,
+                                                               const DecodeMsg *__restrict__ m, int count,
+                                                               unsigned long long *__restrict__ tile_sums) {
+    const long long tile = blockIdx.x;
+    const int j = decode_message(m, count, tile);
+    const int run_end = j + 1 < count ? (int)m[j + 1].run_begin : run_count;
+    unsigned long long n = 0;
+    for_each_byte(msgs, runs, run_count, (int)m[j].run_begin, run_end, tile,
+                  [&](const unsigned char *b, const unsigned char *, bool) { n += !(*b & 0x80); });
+    unsigned long long total;
+    block_scan(n, total);
+    if (threadIdx.x == 0) tile_sums[tile] = total;
+}
+
+// sums[0 .. n) -> their exclusive prefix sums, sums[n] = the total; one CTA of 1024 threads
+__global__ void __launch_bounds__(1024) proto_scan_kernel(unsigned long long *__restrict__ sums, long long n) {
+    __shared__ unsigned long long warp_sums[32];
+    __shared__ unsigned long long carry;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    constexpr int kPer = 8;
+    for (long long base = 0; base < n; base += 1024 * kPer) {
+        const long long at = base + (long long)threadIdx.x * kPer;
+        unsigned long long v[kPer], x = 0;
+#pragma unroll
+        for (int i = 0; i < kPer; ++i) {
+            v[i] = at + i < n ? sums[at + i] : 0;
+            x += v[i];
+        }
+        const unsigned long long mine = x;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+            if (lane >= o) x += y;
+        }
+        if (lane == 31) warp_sums[warp] = x;
+        __syncthreads();
+        unsigned long long before = carry, all = carry;
+        for (int w = 0; w < 32; ++w) {
+            before += w < warp ? warp_sums[w] : 0;
+            all += warp_sums[w];
+        }
+        before += x - mine;
+#pragma unroll
+        for (int i = 0; i < kPer; ++i) {
+            if (at + i < n) sums[at + i] = before;
+            before += v[i];
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) carry = all;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) sums[n] = carry;
+}
+
+// decode 2: every varint of every tile into its shard's request digit planes (zeroed before), and the flags of the
+// message it belongs to (simple_pir.cuh, ProtoFlag)
+__global__ void __launch_bounds__(kThreads) proto_decode_kernel(const unsigned char *__restrict__ msgs,
+                                                                const ProtoRun *__restrict__ runs, int run_count,
+                                                                const DecodeMsg *__restrict__ m, int count,
+                                                                const unsigned long long *__restrict__ prefix, int ct,
+                                                                unsigned *__restrict__ flags) {
+    const long long tile = blockIdx.x;
+    const int j = decode_message(m, count, tile);
+    const DecodeMsg d = m[j];
+    const int run_end = j + 1 < count ? (int)m[j + 1].run_begin : run_count;
+    unsigned long long n = 0;
+    for_each_byte(msgs, runs, run_count, (int)d.run_begin, run_end, tile,
+                  [&](const unsigned char *b, const unsigned char *, bool) { n += !(*b & 0x80); });
+    unsigned long long total;
+    unsigned long long index = prefix[tile] - prefix[d.tile_begin] + block_scan(n, total);
+    unsigned flag = 0;
+    const int digits = spir::digits(ct);
+    for_each_byte(msgs, runs, run_count, (int)d.run_begin, run_end, tile,
+                  [&](const unsigned char *b, const unsigned char *run, bool last) {
+                      if (*b & 0x80) {
+                          if (last) flag |= spir::kRunsPast;
+                          return;
+                      }
+                      int length;
+                      const uint64_t v = spir::varint_ending(run, 0, b - run, length);
+                      if (length > spir::kVarintMax) flag |= spir::kLongVarint;
+                      if (d.word32 && (v >> 32)) flag |= spir::kScalarRange;
+                      if ((long long)index < d.expected) {
+                          const long long at = spir::request_digit_at((long long)index, d.columns, d.row_base, d.col_tiles);
+                          for (int k = 0; k < digits; ++k) d.digits[k * d.plane_bytes + at] = (unsigned char)spir::query_digit(v, ct, k);
+                      }
+                      ++index;
+                  });
+    if (flag) atomicOr(flags + j, flag);
+}
+
+// decode 3: each message's varint count against row_count x col_count
+__global__ void __launch_bounds__(kThreads) proto_check_kernel(const DecodeMsg *__restrict__ m, int count,
+                                                               long long tiles, const unsigned long long *__restrict__ prefix,
+                                                               unsigned *__restrict__ flags) {
+    const int j = blockIdx.x * kThreads + threadIdx.x;
+    if (j >= count) return;
+    const long long end = j + 1 < count ? m[j + 1].tile_begin : tiles;
+    if ((long long)(prefix[end] - prefix[m[j].tile_begin]) != m[j].expected) flags[j] |= spir::kWrongCount;
+}
+
+__device__ __forceinline__ int encode_message(const EncodeMsg *m, int count, long long tile) {
+    return find_last_le(&m[0].tile_begin, count, tile, (int)(sizeof(EncodeMsg) / 8));
+}
+
+// encode 1: the varint bytes of every tile's values (acc mod 2^ct) -> tile_sums[tile]
+__global__ void __launch_bounds__(kThreads) proto_length_kernel(const EncodeMsg *__restrict__ m, int count, int ct,
+                                                                unsigned long long *__restrict__ tile_sums) {
+    const long long tile = blockIdx.x;
+    const EncodeMsg d = m[encode_message(m, count, tile)];
+    const long long i0 = (tile - d.tile_begin) * spir::kProtoTile + (long long)threadIdx.x * spir::kProtoItems;
+    const long long values = d.rows * d.columns;
+    unsigned long long n = 0;
+#pragma unroll 4
+    for (int i = 0; i < spir::kProtoItems; ++i)
+        if (i0 + i < values) n += spir::varint_bytes(spir::finish(d.acc[i0 + i], ct));
+    unsigned long long total;
+    block_scan(n, total);
+    if (threadIdx.x == 0) tile_sums[tile] = total;
+}
+
+// encode 2: every message whole -- thread 0 of its first tile writes its framing and length -- and every value's
+// varint after the framing
+__global__ void __launch_bounds__(kThreads) proto_write_kernel(const EncodeMsg *__restrict__ m, int count, int ct,
+                                                               const unsigned long long *__restrict__ prefix,
+                                                               unsigned char *__restrict__ out,
+                                                               unsigned long long *__restrict__ lengths) {
+    const long long tile = blockIdx.x;
+    const int j = encode_message(m, count, tile);
+    const EncodeMsg d = m[j];
+    const long long i0 = (tile - d.tile_begin) * spir::kProtoTile + (long long)threadIdx.x * spir::kProtoItems;
+    const long long values = d.rows * d.columns;
+    unsigned long long n = 0;
+    for (int i = 0; i < spir::kProtoItems; ++i)
+        if (i0 + i < values) n += spir::varint_bytes(spir::finish(d.acc[i0 + i], ct));
+    unsigned long long total;
+    const unsigned long long before = block_scan(n, total);
+    const unsigned long long data = prefix[d.tile_end] - prefix[d.tile_begin];
+    unsigned char *slot = out + d.out;
+    const int header = spir::response_header(d.rows, d.columns, data, nullptr);
+    if (tile == d.tile_begin && threadIdx.x == 0) {
+        spir::response_header(d.rows, d.columns, data, slot);
+        lengths[j] = header + data;
+    }
+    unsigned char *o = slot + header + (prefix[tile] - prefix[d.tile_begin]) + before;
+    for (int i = 0; i < spir::kProtoItems; ++i)
+        if (i0 + i < values) o += spir::put_varint(o, spir::finish(d.acc[i0 + i], ct));
+}
+
 unsigned blocks_for(long long threads) { return (unsigned)((threads + kThreads - 1) / kThreads); }
 
 // ---- parameters: SimplePirEncryptionParams / SimplePirParameters (SimplePir.swift:47-79, 95-160)
@@ -516,19 +743,89 @@ cudaError_t launch_response_shards(const ShardGroup &g, long long items, u64 *ac
     return launch(response_shards_kernel<D>, (unsigned)items, kWarps * 32, 0, s, g, acc);
 }
 
+// The work of a grouped response whose descriptors have their planes, m, k, q, qpc, in_off and out_off set: each
+// shard's K split (desc[i].split_tiles), work items and split_shards_kernel threads, and the scratch layout -- the
+// accumulators (acc_bytes), then each shard's digit planes at digit_at[i] (multiples of 512 bytes)
+struct ShardPlan {
+    std::vector<long long> items, split_threads;
+    std::vector<size_t> digit_at;
+    size_t scratch = 0;
+};
+ShardPlan plan_shards(std::vector<ShardDesc> &desc, size_t acc_bytes, int digits, int sms) {
+    ShardPlan p;
+    long long ctas = 0;
+    for (const ShardDesc &d : desc) ctas += spir::base_ctas(d.m, d.q);
+    p.scratch = acc_bytes;
+    for (ShardDesc &d : desc) {
+        const long long col_tiles = (d.k + spir::kTileCols - 1) / spir::kTileCols;
+        const spir::ItemShape shape = spir::item_shape(d.m, col_tiles, d.q, ctas, sms, kMinSplitTiles);
+        d.split_tiles = shape.split_tiles;
+        p.items.push_back(spir::item_count(shape));
+        const long long q_pad = shape.pairs * spir::kCtaQueries;
+        p.split_threads.push_back(q_pad * col_tiles * (spir::kTileCols / 4));
+        p.digit_at.push_back(p.scratch);
+        p.scratch += (size_t)q_pad * col_tiles * spir::kTileCols * digits;
+    }
+    return p;
+}
+
+// The split (unless d_req is null: the digit planes are written already) and response launches of every group of
+// <= kMaxShards shards of a plan, into the accumulators at the start of d_scratch
+template <typename W>
+cudaError_t launch_shard_groups(const std::vector<ShardDesc> &desc, const ShardPlan &plan, int planes, int ct,
+                                long long in_block, long long out_block, unsigned char *d_scratch, const W *d_req,
+                                cudaStream_t s) {
+    const int digits = spir::digits(ct), shard_count = (int)desc.size();
+    u64 *acc = reinterpret_cast<u64 *>(d_scratch);
+    cudaError_t e = cudaSuccess;
+    for (int first = 0, end = 0; e == cudaSuccess && first < shard_count; first = end) {
+        end = spir::group_end(plan.items.data(), first, shard_count, kMaxShards, INT_MAX);
+        ShardGroup g{};
+        g.count = end - first;
+        g.planes = planes;
+        g.ct = ct;
+        g.in_block = in_block;
+        g.out_block = out_block;
+        long long group_items = 0;
+        for (int j = 0; j < g.count; ++j) {
+            g.shard[j] = desc[first + j];
+            g.shard[j].digits = d_scratch + plan.digit_at[first + j];
+            g.item_begin[j] = group_items;
+            g.split_begin[j] = g.split_threads;
+            group_items += plan.items[first + j];
+            g.split_threads += plan.split_threads[first + j];
+        }
+        if (d_req) e = launch(split_shards_kernel<W>, blocks_for(g.split_threads), kThreads, 0, s, d_req, g);
+        if (e != cudaSuccess) break;
+        switch (digits) {
+            case 1: e = launch_response_shards<1>(g, group_items, acc, s); break;
+            case 2: e = launch_response_shards<2>(g, group_items, acc, s); break;
+            case 3: e = launch_response_shards<3>(g, group_items, acc, s); break;
+            case 4: e = launch_response_shards<4>(g, group_items, acc, s); break;
+            case 5: e = launch_response_shards<5>(g, group_items, acc, s); break;
+            case 6: e = launch_response_shards<6>(g, group_items, acc, s); break;
+            case 7: e = launch_response_shards<7>(g, group_items, acc, s); break;
+            default: e = launch_response_shards<8>(g, group_items, acc, s); break;
+        }
+    }
+    return e;
+}
+
+int sm_count() {
+    int dev = 0, sms = 1;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms;
+}
+
 // the grouped computeResponse for `count` clients already on the device, enqueued on s: one scratch allocation, one
 // memset, a split and a response launch per group of <= kMaxShards shards, one finish
 template <typename W>
 cudaError_t response_shards_device(const hecuda_simple_pir_database *const *shards, int shard_count, int64_t per_shard,
                                    const W *d_req, int64_t count, W *d_out, cudaStream_t s) {
     const int ct = shards[0]->params.ciphertext_modulus_bits, digits = spir::digits(ct);
-    int dev = 0, sms = 1;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     std::vector<ShardDesc> desc(shard_count);
-    std::vector<long long> items(shard_count), split_threads(shard_count);
-    std::vector<size_t> digit_at(shard_count);
-    long long in_block = 0, out_block = 0, ctas = 0;
+    long long in_block = 0, out_block = 0;
     for (int i = 0; i < shard_count; ++i) {
         const hecuda_simple_pir_database &db = *shards[i];
         ShardDesc &d = desc[i];
@@ -542,54 +839,14 @@ cudaError_t response_shards_device(const hecuda_simple_pir_database *const *shar
         d.out_off = out_block;
         in_block += d.qpc * db.k;
         out_block += d.qpc * db.m;
-        ctas += spir::base_ctas(db.m, d.q);
     }
     const size_t acc_bytes = (size_t)count * out_block * sizeof(u64);
-    size_t scratch = acc_bytes;  // the accumulators, then each shard's digit planes (multiples of 512 bytes)
-    for (int i = 0; i < shard_count; ++i) {
-        ShardDesc &d = desc[i];
-        const spir::ItemShape shape = spir::item_shape(d.m, shards[i]->col_tiles, d.q, ctas, sms, kMinSplitTiles);
-        d.split_tiles = shape.split_tiles;
-        items[i] = spir::item_count(shape);
-        const long long q_pad = shape.pairs * spir::kCtaQueries;
-        split_threads[i] = q_pad * shards[i]->col_tiles * (spir::kTileCols / 4);
-        digit_at[i] = scratch;
-        scratch += (size_t)q_pad * shards[i]->col_tiles * spir::kTileCols * digits;
-    }
+    const ShardPlan plan = plan_shards(desc, acc_bytes, digits, sm_count());
     unsigned char *d_scratch = nullptr;
-    cudaError_t e = cudaMallocAsync((void **)&d_scratch, scratch, s);
+    cudaError_t e = cudaMallocAsync((void **)&d_scratch, plan.scratch, s);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_scratch, 0, acc_bytes, s);
     u64 *acc = reinterpret_cast<u64 *>(d_scratch);
-    for (int first = 0, end = 0; e == cudaSuccess && first < shard_count; first = end) {
-        end = spir::group_end(items.data(), first, shard_count, kMaxShards, INT_MAX);
-        ShardGroup g{};
-        g.count = end - first;
-        g.planes = shards[0]->planes;
-        g.ct = ct;
-        g.in_block = in_block;
-        g.out_block = out_block;
-        long long group_items = 0;
-        for (int j = 0; j < g.count; ++j) {
-            g.shard[j] = desc[first + j];
-            g.shard[j].digits = d_scratch + digit_at[first + j];
-            g.item_begin[j] = group_items;
-            g.split_begin[j] = g.split_threads;
-            group_items += items[first + j];
-            g.split_threads += split_threads[first + j];
-        }
-        e = launch(split_shards_kernel<W>, blocks_for(g.split_threads), kThreads, 0, s, d_req, g);
-        if (e != cudaSuccess) break;
-        switch (digits) {
-            case 1: e = launch_response_shards<1>(g, group_items, acc, s); break;
-            case 2: e = launch_response_shards<2>(g, group_items, acc, s); break;
-            case 3: e = launch_response_shards<3>(g, group_items, acc, s); break;
-            case 4: e = launch_response_shards<4>(g, group_items, acc, s); break;
-            case 5: e = launch_response_shards<5>(g, group_items, acc, s); break;
-            case 6: e = launch_response_shards<6>(g, group_items, acc, s); break;
-            case 7: e = launch_response_shards<7>(g, group_items, acc, s); break;
-            default: e = launch_response_shards<8>(g, group_items, acc, s); break;
-        }
-    }
+    if (e == cudaSuccess) e = launch_shard_groups(desc, plan, shards[0]->planes, ct, in_block, out_block, d_scratch, d_req, s);
     if (e == cudaSuccess)
         e = launch(finish_kernel<W>, blocks_for(count * out_block), kThreads, 0, s, (const u64 *)acc, (long long)(count * out_block),
                    ct, d_out);
@@ -632,6 +889,192 @@ bool columns_match(const hecuda_simple_pir_params &p, int64_t rows) {
     const int64_t epc = p.entries_per_column;
     return epc == 1 ? p.database_columns == rows * p.chunks_per_entry
                     : p.database_columns == std::max<int64_t>((rows + epc - 1) / epc, 1);
+}
+
+// ---- requests and responses in protobuf messages: the host walk of every message, then the device call
+struct ProtoWalk {
+    std::vector<spirproto::Request> req;
+    std::vector<uint64_t> capacity;  // each response's slot
+};
+
+// Every refusal of the call, before anything is enqueued: the shards (one ct and digit-plane count, one device), then
+// each message's walk, shard index, column count and size, named "message <j>: "
+int32_t walk_proto_messages(const hecuda_simple_pir_database *const *shards, int32_t shard_count,
+                            const uint8_t *const *messages, const uint64_t *byte_counts, int64_t count, ProtoWalk &w) {
+    if (!shards || shard_count < 1) return fail(HECUDA_ERR_INVALID_ARGUMENT, "no shards");
+    if (count < 0) return fail(HECUDA_ERR_INVALID_ARGUMENT, "negative message count");
+    if (count && (!messages || !byte_counts)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    for (int i = 0; i < shard_count; ++i) {
+        if (!shards[i]) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null shard");
+        if (shards[i]->params.ciphertext_modulus_bits != shards[0]->params.ciphertext_modulus_bits ||
+            shards[i]->planes != shards[0]->planes)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "shards differ in ciphertextModulusBits or ceil(plaintextModulusBits / 8)");
+        if (shards[i]->device != shards[0]->device) return fail(HECUDA_ERR_INVALID_ARGUMENT, "shards on different devices");
+    }
+    const int ct = shards[0]->params.ciphertext_modulus_bits;
+    w.req.assign((size_t)count, spirproto::Request{});
+    w.capacity.assign((size_t)count, 0);
+    std::vector<long long> rows(shard_count, 0);
+    for (int64_t j = 0; j < count; ++j) {
+        const std::string at = "message " + std::to_string(j) + ": ";
+        if (!messages[j] && byte_counts[j]) return fail(HECUDA_ERR_INVALID_ARGUMENT, at + "null message");
+        proto::Error e;
+        spirproto::Request &r = w.req[(size_t)j];
+        if (!spirproto::walk_request(messages[j], (long long)byte_counts[j], r, e)) return fail(e.code, at + e.what);
+        if (!r.has_request) return fail(HECUDA_ERR_INVALID_ARGUMENT, at + "SimplePIRRequest.request is not set");
+        if (r.shard_index >= (uint32_t)shard_count)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, at + "shard_index " + std::to_string(r.shard_index) + " of " +
+                                                         std::to_string(shard_count) + " shards");
+        const hecuda_simple_pir_database &db = *shards[r.shard_index];
+        const long long R = r.matrix.rows;
+        if ((int64_t)r.matrix.columns != db.k)
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, at + "col_count " + std::to_string(r.matrix.columns) +
+                                                         ", expected databaseColumns " + std::to_string(db.k));
+        rows[r.shard_index] += R;
+        if (rows[r.shard_index] > (1ll << 36) / std::max<int64_t>(1, std::max(db.k, db.m)))
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, at + "row_count x col_count too large for one call");
+        w.capacity[(size_t)j] = spir::response_capacity((uint64_t)R, (uint64_t)db.m, ct);
+    }
+    return select_device(shards[0]->device);
+}
+
+// The call after the walk: messages up once, the decode into every shard's digit planes, one grouped response over the
+// shards that have rows, the encode straight from the accumulators, one download
+cudaError_t response_proto(const hecuda_simple_pir_database *const *shards, int shard_count, const uint8_t *const *messages,
+                           const uint64_t *byte_counts, int64_t count, const ProtoWalk &w, std::vector<unsigned char> &out,
+                           std::vector<uint64_t> &slot, std::vector<unsigned long long> &lengths, std::vector<unsigned> &flags) {
+    const int ct = shards[0]->params.ciphertext_modulus_bits, digits = spir::digits(ct);
+    const long long T = spir::kProtoTile;
+    // the shards' query blocks: message j's rows follow those of the messages before it that go to its shard
+    std::vector<long long> shard_rows(shard_count, 0), row_base((size_t)count);
+    for (int64_t j = 0; j < count; ++j) {
+        row_base[(size_t)j] = shard_rows[w.req[(size_t)j].shard_index];
+        shard_rows[w.req[(size_t)j].shard_index] += w.req[(size_t)j].matrix.rows;
+    }
+    std::vector<ShardDesc> desc;
+    std::vector<int> slot_of(shard_count, -1);
+    long long out_words = 0;
+    for (int i = 0; i < shard_count; ++i) {
+        if (!shard_rows[i]) continue;
+        ShardDesc d{};
+        d.planes = shards[i]->d_planes;
+        d.plane_bytes = shards[i]->plane_bytes;
+        d.m = shards[i]->m;
+        d.k = shards[i]->k;
+        d.q = d.qpc = shard_rows[i];
+        d.out_off = out_words;
+        out_words += d.q * d.m;
+        slot_of[i] = (int)desc.size();
+        desc.push_back(d);
+    }
+    const size_t acc_bytes = (size_t)out_words * sizeof(u64);
+    const ShardPlan plan = plan_shards(desc, acc_bytes, digits, sm_count());
+    // the messages' bytes, runs and tiles
+    std::vector<ProtoRun> runs;
+    std::vector<DecodeMsg> dm((size_t)count);
+    std::vector<EncodeMsg> em((size_t)count);
+    std::vector<long long> msg_at((size_t)count + 1, 0);
+    slot.assign((size_t)count + 1, 0);
+    long long tiles = 0, out_tiles = 0;
+    for (int64_t j = 0; j < count; ++j) {
+        const spirproto::Request &r = w.req[(size_t)j];
+        const int s = (int)r.shard_index;
+        const hecuda_simple_pir_database &db = *shards[s];
+        msg_at[(size_t)j + 1] = msg_at[(size_t)j] + (long long)((byte_counts[j] + 15) / 16 * 16);
+        DecodeMsg &d = dm[(size_t)j];
+        d.digits = nullptr;  // set once the scratch is allocated
+        d.col_tiles = db.col_tiles;
+        d.columns = db.k;
+        d.row_base = row_base[(size_t)j];
+        d.expected = (long long)r.matrix.rows * (long long)r.matrix.columns;
+        d.tile_begin = tiles;
+        d.run_begin = (long long)runs.size();
+        d.word32 = db.params.word_bits == 32;
+        long long v = tiles * T;
+        for (const auto &run : r.matrix.runs) {
+            runs.push_back(ProtoRun{msg_at[(size_t)j] + run.first, v, run.second - run.first});
+            v += run.second - run.first;
+        }
+        tiles += std::max<long long>(1, (v - tiles * T + T - 1) / T);
+        EncodeMsg &o = em[(size_t)j];
+        o.rows = r.matrix.rows;
+        o.columns = db.m;
+        o.tile_begin = out_tiles;
+        out_tiles += std::max<long long>(1, (o.rows * o.columns + T - 1) / T);
+        o.tile_end = out_tiles;
+        o.out = slot[(size_t)j];
+        slot[(size_t)j + 1] = slot[(size_t)j] + w.capacity[(size_t)j];
+    }
+    // device buffers: scratch (accumulators, digit planes), messages, runs, descriptors, sums, flags, lengths, output
+    const size_t run_bytes = std::max<size_t>(1, runs.size()) * sizeof(ProtoRun);
+    const size_t sum_words = (size_t)std::max(tiles, out_tiles) + 1;
+    size_t at = 0;
+    auto take = [&](size_t bytes) {
+        const size_t o = at;
+        at += (bytes + 255) / 256 * 256;
+        return o;
+    };
+    const size_t o_scratch = take(plan.scratch), o_msgs = take((size_t)msg_at[(size_t)count]), o_runs = take(run_bytes),
+                 o_dm = take(dm.size() * sizeof(DecodeMsg)), o_em = take(em.size() * sizeof(EncodeMsg)),
+                 o_sums = take(sum_words * 8), o_flags = take((size_t)count * 4), o_len = take((size_t)count * 8),
+                 o_out = take(slot[(size_t)count]);
+    unsigned char *d_all = nullptr;
+    cudaStream_t s = nullptr;
+    cudaError_t e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_all, std::max<size_t>(at, 256), s);
+    unsigned char *d_scratch = d_all + o_scratch, *d_msgs = d_all + o_msgs;
+    for (size_t j = 0; j < dm.size(); ++j) {
+        const int k = slot_of[w.req[j].shard_index];
+        if (k < 0) continue;  // no rows: nothing is decoded into it
+        dm[j].digits = d_scratch + plan.digit_at[(size_t)k];
+        dm[j].plane_bytes = (long long)(desc[(size_t)k].q + spir::kCtaQueries - 1) / spir::kCtaQueries * spir::kCtaQueries *
+                            dm[j].col_tiles * spir::kTileCols;
+        em[j].acc = reinterpret_cast<const u64 *>(d_scratch) + desc[(size_t)k].out_off + dm[j].row_base * desc[(size_t)k].m;
+    }
+    for (size_t j = 0; j < em.size(); ++j)
+        if (!em[j].acc) em[j].acc = reinterpret_cast<const u64 *>(d_scratch);  // no values to read
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_scratch, 0, plan.scratch, s);
+    for (int64_t j = 0; e == cudaSuccess && j < count; ++j)
+        if (byte_counts[j]) e = cudaMemcpyAsync(d_msgs + msg_at[(size_t)j], messages[j], byte_counts[j], cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && !runs.empty()) e = cudaMemcpyAsync(d_all + o_runs, runs.data(), runs.size() * sizeof(ProtoRun), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_all + o_dm, dm.data(), dm.size() * sizeof(DecodeMsg), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_all + o_em, em.data(), em.size() * sizeof(EncodeMsg), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_all + o_flags, 0, (size_t)count * 4, s);
+    const ProtoRun *d_runs = reinterpret_cast<const ProtoRun *>(d_all + o_runs);
+    const DecodeMsg *d_dm = reinterpret_cast<const DecodeMsg *>(d_all + o_dm);
+    const EncodeMsg *d_em = reinterpret_cast<const EncodeMsg *>(d_all + o_em);
+    unsigned long long *d_sums = reinterpret_cast<unsigned long long *>(d_all + o_sums);
+    unsigned *d_flags = reinterpret_cast<unsigned *>(d_all + o_flags);
+    unsigned long long *d_len = reinterpret_cast<unsigned long long *>(d_all + o_len);
+    const int n = (int)count, run_count = (int)runs.size();
+    if (e == cudaSuccess)
+        e = launch(proto_count_kernel, (unsigned)tiles, kThreads, 0, s, (const unsigned char *)d_msgs, d_runs, run_count, d_dm, n, d_sums);
+    if (e == cudaSuccess) e = launch(proto_scan_kernel, 1, 1024, 0, s, d_sums, tiles);
+    if (e == cudaSuccess)
+        e = launch(proto_decode_kernel, (unsigned)tiles, kThreads, 0, s, (const unsigned char *)d_msgs, d_runs, run_count, d_dm, n,
+                   (const unsigned long long *)d_sums, ct, d_flags);
+    if (e == cudaSuccess)
+        e = launch(proto_check_kernel, blocks_for(count), kThreads, 0, s, d_dm, n, tiles, (const unsigned long long *)d_sums, d_flags);
+    if (e == cudaSuccess && !desc.empty())
+        e = launch_shard_groups<u64>(desc, plan, shards[0]->planes, ct, 0, 0, d_scratch, nullptr, s);
+    if (e == cudaSuccess) e = launch(proto_length_kernel, (unsigned)out_tiles, kThreads, 0, s, d_em, n, ct, d_sums);
+    if (e == cudaSuccess) e = launch(proto_scan_kernel, 1, 1024, 0, s, d_sums, out_tiles);
+    if (e == cudaSuccess)
+        e = launch(proto_write_kernel, (unsigned)out_tiles, kThreads, 0, s, d_em, n, ct, (const unsigned long long *)d_sums,
+                   d_all + o_out, d_len);
+    flags.assign((size_t)count, 0);
+    lengths.assign((size_t)count, 0);
+    out.resize(slot[(size_t)count]);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(flags.data(), d_flags, (size_t)count * 4, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(lengths.data(), d_len, (size_t)count * 8, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess && !out.empty()) e = cudaMemcpyAsync(out.data(), d_all + o_out, out.size(), cudaMemcpyDeviceToHost, s);
+    if (d_all) cudaFreeAsync(d_all, s);
+    if (s) {
+        const cudaError_t e2 = cudaStreamSynchronize(s);
+        if (e == cudaSuccess) e = e2;
+        cudaStreamDestroy(s);
+    }
+    return e;
 }
 
 }  // namespace
@@ -980,6 +1423,53 @@ int32_t hecuda_simple_pir_compute_response_shards(const hecuda_simple_pir_databa
         cudaStreamDestroy(s);
     }
     return e == cudaSuccess ? HECUDA_OK : cuda_fail(e, "simple_pir_compute_response_shards");
+}
+
+int32_t hecuda_simple_pir_response_proto_byte_count(const hecuda_simple_pir_database *const *shards, int32_t shard_count,
+                                                    const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                                                    int64_t count, uint64_t *capacities) {
+    if (count && !capacities) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    ProtoWalk w;
+    const int32_t rc = walk_proto_messages(shards, shard_count, messages, message_byte_counts, count, w);
+    if (rc) return rc;
+    std::copy(w.capacity.begin(), w.capacity.end(), capacities);
+    return HECUDA_OK;
+}
+
+int32_t hecuda_simple_pir_compute_response_proto(const hecuda_simple_pir_database *const *shards, int32_t shard_count,
+                                                 const uint8_t *const *messages, const uint64_t *message_byte_counts,
+                                                 int64_t count, uint8_t *out, const uint64_t *out_offsets,
+                                                 uint64_t *out_lengths) {
+    if (count && (!out || !out_offsets || !out_lengths)) return fail(HECUDA_ERR_INVALID_ARGUMENT, "null argument");
+    ProtoWalk w;
+    int32_t rc = walk_proto_messages(shards, shard_count, messages, message_byte_counts, count, w);
+    if (rc || count == 0) return rc;
+    for (int64_t j = 0; j + 1 < count; ++j)
+        if (out_offsets[j] + w.capacity[(size_t)j] > out_offsets[j + 1])
+            return fail(HECUDA_ERR_INVALID_ARGUMENT, "message " + std::to_string(j) + ": its slot of " +
+                                                         std::to_string(out_offsets[j + 1] - std::min(out_offsets[j + 1], out_offsets[j])) +
+                                                         " bytes is below its capacity " + std::to_string(w.capacity[(size_t)j]));
+    std::vector<unsigned char> bytes;
+    std::vector<uint64_t> slot;
+    std::vector<unsigned long long> lengths;
+    std::vector<unsigned> flags;
+    const cudaError_t e = response_proto(shards, shard_count, messages, message_byte_counts, count, w, bytes, slot, lengths, flags);
+    if (e != cudaSuccess) return cuda_fail(e, "simple_pir_compute_response_proto");
+    for (int64_t j = 0; j < count; ++j) {
+        const unsigned f = flags[(size_t)j];
+        if (!f) continue;
+        std::string what = "message " + std::to_string(j) + ": ";
+        if (f & spir::kLongVarint) what += "malformedProtobuf(SimplePIRMatrix.data: a varint longer than 10 bytes)";
+        else if (f & spir::kRunsPast) what += "truncated(SimplePIRMatrix.data: a varint runs past the end)";
+        else if (f & spir::kScalarRange) what += "SimplePIRMatrix.data: a value at or above 2^32 for a 32-bit shard";
+        else what += "SimplePIRMatrix.data: the varint count is not row_count x col_count";
+        return fail(HECUDA_ERR_INVALID_ARGUMENT, what);
+    }
+    for (int64_t j = 0; j < count; ++j) {
+        std::memcpy(out + out_offsets[j], bytes.data() + slot[(size_t)j], lengths[(size_t)j]);
+        out_lengths[j] = lengths[(size_t)j];
+    }
+    return HECUDA_OK;
 }
 
 }  // extern "C"

@@ -198,6 +198,72 @@ SPIR_HD void decode_item(const ItemShape &s, long long col_tiles, long long loca
     k_end = k_begin + s.split_tiles < col_tiles ? k_begin + s.split_tiles : col_tiles;
 }
 
+// ---- requests and responses in protobuf messages (simple_pir.cu, "proto"; the host walk is simple_pir_proto.hpp).
+// A call's data runs are laid end to end in one virtual byte stream, each message's first run starting at a multiple of
+// kProtoTile, so every tile belongs to one message.  A byte whose top bit is clear ends a varint; the varint's index in
+// its message is the number of such bytes before it in the message's runs (a scan over tiles, then inside the tile).
+// The responses' values are laid out the same way, with one tile at least per message so that empty messages get their
+// framing.
+constexpr int kProtoItems = 16;                      // bytes (decode) or values (encode) per thread
+constexpr long long kProtoTile = 256 * kProtoItems;  // per CTA of 256 threads
+constexpr int kVarintMax = 10;
+
+SPIR_HD int varint_bytes(uint64_t v) {
+    int n = 1;
+    while (v >>= 7) ++n;
+    return n;
+}
+SPIR_HD int put_varint(unsigned char *out, uint64_t v) {
+    int n = 0;
+    while (v >= 0x80) {
+        out[n++] = (unsigned char)(v | 0x80);
+        v >>= 7;
+    }
+    out[n++] = (unsigned char)v;
+    return n;
+}
+// The varint ending at b[p] (its last byte) that starts after b[lo - 1]: its value, as proto::read_varint reads it
+// (bits past 64 in a tenth byte are dropped), and its length; length > kVarintMax when the kVarintMax bytes before b[p]
+// all carry the continuation bit, which read_varint refuses.
+SPIR_HD uint64_t varint_ending(const unsigned char *b, long long lo, long long p, int &length) {
+    long long s = p;
+    while (s > lo && (b[s - 1] & 0x80) && p - s < kVarintMax) --s;
+    length = (int)(p - s + 1);
+    uint64_t v = 0;
+    for (long long k = s; k <= p && k - s < kVarintMax; ++k) v |= (uint64_t)(b[k] & 0x7f) << (7 * (k - s));
+    return v;
+}
+// Where varint `index` of a message with `columns` columns goes in its shard's request digit planes: query
+// row_base + index / columns, column index % columns (b_offset)
+SPIR_HD long long request_digit_at(long long index, long long columns, long long row_base, long long col_tiles) {
+    return b_offset(row_base + index / columns, index % columns, col_tiles);
+}
+// The flags of a message the decode refuses
+enum ProtoFlag : unsigned { kLongVarint = 1, kRunsPast = 2, kScalarRange = 4, kWrongCount = 8 };
+
+// A SimplePIRResponse of rows x columns values whose data varints take data_len bytes, as SwiftProtobuf writes it:
+// 0x0a len { [0x08 rows]  0x10 columns  [0x1a data_len data] } -> the framing's length; written to out unless null.
+// proto3 omits a zero row count and an empty data field; the response message is written even when empty.
+SPIR_HD int response_header(uint64_t rows, uint64_t columns, uint64_t data_len, unsigned char *out) {
+    const uint64_t values = rows * columns;
+    const uint64_t body = (rows ? 1 + varint_bytes(rows) : 0) + (columns ? 1 + varint_bytes(columns) : 0) +
+                          (values ? 1 + varint_bytes(data_len) + data_len : 0);
+    if (!out) return (int)(1 + varint_bytes(body) + body - (values ? data_len : 0));
+    unsigned char *o = out;
+    int n = 0;
+    o[n++] = 0x0a;
+    n += put_varint(o + n, body);
+    if (rows) o[n++] = 0x08, n += put_varint(o + n, rows);
+    if (columns) o[n++] = 0x10, n += put_varint(o + n, columns);
+    if (values) o[n++] = 0x1a, n += put_varint(o + n, data_len);
+    return n;
+}
+// The most bytes a response of rows x columns values below 2^ct can take: every varint ceil(ct / 7) bytes long
+SPIR_HD uint64_t response_capacity(uint64_t rows, uint64_t columns, int ct) {
+    const uint64_t data = rows * columns * (uint64_t)((ct + 6) / 7);
+    return (uint64_t)response_header(rows, columns, data, nullptr) + (rows * columns ? data : 0);
+}
+
 // ---- the client (simple_pir_client.cu): PrecomputedQueries.WithoutIndices.init, add(index:), integrate
 //   generateSecretPolys / noiselessSample / encryptZero / extractEntries   SimplePir+Client.swift:20-95
 //   Array2d.multiply(transposing:modulus:)                                  SimplePir+Precompute.swift:122-188

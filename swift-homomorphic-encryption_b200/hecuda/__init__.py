@@ -136,6 +136,18 @@ SYMBOLS = {
     "hecuda_simple_pir_compute_response_shards": (C.c_int32, [_VP, C.c_int32, C.c_int64, _VP, C.c_int64, _VP]),
     "hecuda_simple_pir_compute_response_shards_device": (C.c_int32, [_VP, C.c_int32, C.c_int64, _VP, C.c_int64, _VP,
                                                                      _VP]),
+    "hecuda_simple_pir_request_fields_read": (C.c_int32, [_VP, C.c_uint64, _VP]),
+    "hecuda_simple_pir_response_proto_byte_count": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int64, _VP]),
+    "hecuda_simple_pir_compute_response_proto": (C.c_int32, [_VP, C.c_int32, _VP, _VP, C.c_int64, _VP, _VP, _VP]),
+    "hecuda_simple_pir_request_write": (C.c_int32, [C.c_uint32, C.c_uint32, _VP, C.c_uint32, _VP, C.c_uint64, _VP,
+                                                    C.c_uint64, _VP]),
+    "hecuda_simple_pir_response_read": (C.c_int32, [_VP, C.c_uint64, _VP, _VP, _VP, C.c_int64]),
+    "hecuda_simple_pir_config_describe": (C.c_int32, [_VP, C.c_uint64, _VP]),
+    "hecuda_simple_pir_config_read": (C.c_int32, [_VP, C.c_uint64, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "hecuda_simple_pir_config_serialized_byte_count": (C.c_int32, [_VP, _VP, _VP, C.c_int64, _VP, C.c_uint64, _VP, _VP,
+                                                                   C.c_int32, _VP, _VP, C.c_int32, _VP]),
+    "hecuda_simple_pir_config_serialize": (C.c_int32, [_VP, _VP, _VP, C.c_int64, _VP, C.c_uint64, _VP, _VP, C.c_int32,
+                                                       _VP, _VP, C.c_int32, _VP, C.c_uint64]),
     "hecuda_simple_pir_client_create": (C.c_int32, [_VP, _VP, _VP, C.POINTER(_VP)]),
     "hecuda_simple_pir_client_destroy": (C.c_int32, [_VP]),
     "hecuda_simple_pir_client_precompute": (C.c_int32, [_VP, _VP, _VP, _VP, C.c_int64, _VP, _VP]),

@@ -14,6 +14,8 @@ Names follow Sources/PrivateInformationRetrieval/SimplePir/:
     SimplePirClientForAllShards                             SimplePir/SimplePir+Shards.swift:47-173
     SimplePirServer.validate / SimplePirShardedServer.validate   verifyProcessing, SimplePIRProcessDatabase/main.swift:260-348
     SimplePIRProcessDatabase's sharding and file names      Sources/SimplePIRProcessDatabase/main.swift:158-253
+    SimplePIRRequest / SimplePIRResponse / SimplePIRConfig  ApplicationProtobuf/PirConversion.swift:380-518,
+                                                            api/pir/v1/pir.proto, SimplePIRProcessDatabase/main.swift:193-258
 
 The processed database stays on the device as u8 digit planes; responses are integer tensor-core products there.
 `scalar` is the reference's Scalar type: np.uint32 (UInt32) or np.uint64 (UInt64).
@@ -21,6 +23,7 @@ The processed database stays on the device as u8 digit planes; responses are int
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 import math
 import secrets
 import struct
@@ -266,6 +269,10 @@ class SimplePirServer:
         _check(load_library().hecuda_simple_pir_compute_response_device(self.database._h, C.c_void_p(requests_ptr), count,
                                                                         C.c_void_p(responses_ptr), C.c_void_p(stream)))
 
+    def computeResponsesProto(self, messages) -> list:
+        """One SimplePIRResponse (bytes) per SimplePIRRequest (bytes, shard_index 0), in one device call."""
+        return _responses_proto(_handles([self.database]), 1, messages)
+
 
 # ---- sharding (DatabaseMap.swift, SimplePir+Shards.swift, SimplePIRProcessDatabase/main.swift:158-253)
 @dataclass(frozen=True)
@@ -491,11 +498,35 @@ class SimplePirShardedServer:
             self._h, self.shardCount, requests_per_shard, C.c_void_p(requests_ptr), count, C.c_void_p(responses_ptr),
             C.c_void_p(stream)))
 
-    def save(self, prefix: str):
-        """The tool's files: prefix-i.bin (processed database) and prefix-i.hint.bin for every shard i."""
+    def save(self, prefix: str, configPath: Optional[str] = None):
+        """The tool's files: prefix-i.bin (processed database) and prefix-i.hint.bin for every shard i; with configPath,
+        also the SimplePIRConfig (the databaseMap, every shard's params and the SHA-256 of every hint file,
+        main.swift:231-258)."""
         for i, (db, hint) in enumerate(zip(self.databases, self.hints)):
             db.save(f"{prefix}-{i}.bin")
             save_array2d(hint, f"{prefix}-{i}.hint.bin")
+        if configPath is not None:
+            if self.databaseMap is None:
+                raise PirError("the config needs the databaseMap")
+            ids = []
+            for i in range(self.shardCount):
+                with open(f"{prefix}-{i}.hint.bin", "rb") as f:
+                    ids.append(hashlib.sha256(f.read()).digest())
+            SimplePirConfig(self.databaseMap, self.params, ids).save(configPath)
+
+    @staticmethod
+    def fromConfig(prefix: str, config) -> "SimplePirShardedServer":
+        """The server from the tool's files alone: the SimplePIRConfig (a SimplePirConfig or its path) and every
+        shard's prefix-i.bin and prefix-i.hint.bin, with the tool's Scalar (UInt32 for ct <= 32, else UInt64)."""
+        config = config if isinstance(config, SimplePirConfig) else SimplePirConfig.load(config)
+        server = SimplePirShardedServer.load(prefix, config.params, config.scalar)
+        server.databaseMap = config.databaseMap
+        return server
+
+    def computeResponsesProto(self, messages) -> list:
+        """One SimplePIRResponse (bytes) per SimplePIRRequest (bytes), each answered by the shard its shard_index
+        names, in one device call."""
+        return _responses_proto(self._h, self.shardCount, messages)
 
     @staticmethod
     def load(prefix: str, params: Sequence[SimplePirParameters], scalar=np.uint64) -> "SimplePirShardedServer":
@@ -724,6 +755,223 @@ class SimplePirClientForAllShards:
                 at = i if q.index == row else at
             out += plain[shard][at][:self.shardMap.chunkSize].tobytes()
         return None if entry is None else out[:entry.size]
+
+
+def _sharded_client_from_config(prefix: str, config, errorStdDev: Optional[float] = None) -> "SimplePirClientForAllShards":
+    """SimplePirClientForAllShards from the tool's files alone: the config (or its path) and every prefix-i.hint.bin."""
+    config = config if isinstance(config, SimplePirConfig) else SimplePirConfig.load(config)
+    clients = [SimplePirClient(DefaultQueryGenerator(p, load_array2d(f"{prefix}-{i}.hint.bin", config.scalar), config.scalar,
+                                                     errorStdDev)) for i, p in enumerate(config.params)]
+    return SimplePirClientForAllShards(config.databaseMap, clients)
+
+
+def _request_messages(self, index: int, configurationHash: bytes = b""):
+    """query(for:) as SimplePIRRequests: one message per shard s holding its chunksPerShard x chunksPerEntry_s rows of
+    K_s words, stacked -> (messages, the per-shard [WithQueryIndices] lists for decryptResponseMessages)."""
+    queries = self.query(index)
+    messages = []
+    for s, (client, qs) in enumerate(zip(self.clients, queries)):
+        words = np.concatenate([q.queries.reshape(-1, client.params.databaseColumns) for q in qs])
+        messages.append(SimplePirRequest.write(words, s, configurationHash))
+    return messages, queries
+
+
+def _decrypt_response_messages(self, messages, index: int, queries) -> Optional[bytes]:
+    """decrypt(responses:for:with:) from one SimplePIRResponse per shard (each chunksPerShard x chunksPerEntry_s rows of
+    M_s words); None for an index the map does not hold."""
+    if len(messages) != len(self.clients):
+        raise PirError("validationError: one response message per shard")
+    responses = []
+    for client, message, qs in zip(self.clients, messages, queries):
+        p = client.params
+        words = SimplePirResponse.read(message, client.scalar)
+        if words.shape != (len(qs) * p.chunksPerEntry, p.columnSize):
+            raise PirError(f"validationError: a response of {words.shape}, expected "
+                           f"{(len(qs) * p.chunksPerEntry, p.columnSize)}")
+        responses.append(list(words.reshape(len(qs), p.chunksPerEntry, p.columnSize)))
+    return self.decrypt(responses, index, queries)
+
+
+SimplePirClientForAllShards.fromConfig = staticmethod(_sharded_client_from_config)
+SimplePirClientForAllShards.requestMessages = _request_messages
+SimplePirClientForAllShards.decryptResponseMessages = _decrypt_response_messages
+
+
+# ---- protobuf messages (api/pir/v1/pir.proto, pir/v1/simple_pir.proto; PirConversion.swift:380-518)
+class _RequestFields(C.Structure):  # hecuda_simple_pir_request_fields
+    _fields_ = [("has_request", C.c_int32), ("row_count", C.c_uint32), ("col_count", C.c_uint32),
+                ("shard_index", C.c_uint32), ("data_run_count", C.c_int64), ("data_bytes", C.c_uint64),
+                ("configuration_hash_offset", C.c_uint64), ("configuration_hash_bytes", C.c_uint64)]
+
+
+class _ConfigShape(C.Structure):  # hecuda_simple_pir_config_shape
+    _fields_ = [("entry_count", C.c_int64), ("chunk_count", C.c_int64), ("chunk_size", C.c_uint64),
+                ("shard_count", C.c_int32), ("hint_identifier_count", C.c_int32)]
+
+
+def _bytes_arg(data: bytes):
+    data = bytes(data)
+    return C.create_string_buffer(data, max(len(data), 1)), len(data)
+
+
+def _responses_proto(handles, shard_count: int, messages) -> list:
+    messages = [bytes(m) for m in messages]
+    if not messages:
+        return []
+    # the messages are read in place (c_char_p points into each bytes object, which `messages` keeps alive)
+    ptrs = (C.c_void_p * len(messages))(*[C.cast(C.c_char_p(m), C.c_void_p).value for m in messages])
+    sizes = np.array([len(m) for m in messages], dtype=np.uint64)
+    lib = load_library()
+    caps = np.zeros(len(messages), dtype=np.uint64)
+    _check(lib.hecuda_simple_pir_response_proto_byte_count(handles, shard_count, ptrs, _ptr(sizes), len(messages),
+                                                           _ptr(caps)))
+    offsets = np.zeros(len(messages), dtype=np.uint64)
+    offsets[1:] = np.cumsum(caps)[:-1]
+    out = np.empty(max(int(caps.sum()), 1), dtype=np.uint8)
+    lengths = np.zeros(len(messages), dtype=np.uint64)
+    _check(lib.hecuda_simple_pir_compute_response_proto(handles, shard_count, ptrs, _ptr(sizes), len(messages), _ptr(out),
+                                                        _ptr(offsets), _ptr(lengths)))
+    return [out[int(o):int(o) + int(n)].tobytes() for o, n in zip(offsets, lengths)]
+
+
+class SimplePirRequest:
+    """api.pir.v1.SimplePIRRequest."""
+
+    @staticmethod
+    def fields(message: bytes) -> dict:
+        """The walk of one request (data located, not read): has_request, row_count, col_count, shard_index,
+        data_run_count, data_bytes and configuration_hash."""
+        buf, n = _bytes_arg(message)
+        f = _RequestFields()
+        _check(load_library().hecuda_simple_pir_request_fields_read(buf, n, C.byref(f)))
+        at, size = f.configuration_hash_offset, f.configuration_hash_bytes
+        return {"has_request": bool(f.has_request), "row_count": f.row_count, "col_count": f.col_count,
+                "shard_index": f.shard_index, "data_run_count": f.data_run_count, "data_bytes": f.data_bytes,
+                "configuration_hash": bytes(message)[at:at + size]}
+
+    @staticmethod
+    def write(words, shardIndex: int = 0, configurationHash: bytes = b"") -> bytes:
+        """Array2d.proto() of a rows x columns word matrix in a SimplePIRRequest, data packed."""
+        w = np.ascontiguousarray(np.asarray(words), dtype=np.uint64)
+        if w.ndim != 2:
+            raise PirError("a request is a rows x columns word matrix")
+        h, hn = _bytes_arg(configurationHash)
+        lib, written = load_library(), C.c_uint64(0)
+        data = w if w.size else np.zeros(1, dtype=np.uint64)
+        _check(lib.hecuda_simple_pir_request_write(w.shape[0], w.shape[1], _ptr(data), shardIndex, h, hn, None, 0,
+                                                   C.byref(written)))
+        out = np.empty(max(written.value, 1), dtype=np.uint8)
+        _check(lib.hecuda_simple_pir_request_write(w.shape[0], w.shape[1], _ptr(data), shardIndex, h, hn, _ptr(out),
+                                                   written.value, C.byref(written)))
+        return out[:written.value].tobytes()
+
+
+class SimplePirResponse:
+    """api.pir.v1.SimplePIRResponse."""
+
+    @staticmethod
+    def read(message: bytes, scalar=np.uint64) -> np.ndarray:
+        """SimplePIRMatrix.native(): the rows x columns words (a value the scalar cannot hold is refused, where the
+        reference's Scalar(_:) traps)."""
+        buf, n = _bytes_arg(message)
+        rows, cols = C.c_uint32(0), C.c_uint32(0)
+        lib = load_library()
+        # every value takes one byte at least, so the message's size bounds the count
+        data = np.empty(max(n, 1), dtype=np.uint64)
+        _check(lib.hecuda_simple_pir_response_read(buf, n, C.byref(rows), C.byref(cols), _ptr(data), n))
+        words = data[:rows.value * cols.value]
+        if np.dtype(scalar) == np.dtype(np.uint32) and words.size and int(words.max()) >> 32:
+            raise PirError("SimplePIRMatrix: a value at or above 2^32 for UInt32")
+        return words.astype(scalar).reshape(rows.value, cols.value)
+
+
+class SimplePirConfig:
+    """api.pir.v1.SimplePIRConfig: the databaseMap, one SimplePirParameters per shard and one hint identifier (SHA-256
+    of the hint file) per shard, as the SimplePIRProcessDatabase tool writes them (main.swift:231-240)."""
+
+    def __init__(self, databaseMap: DatabaseMap, params: Sequence[SimplePirParameters], hintIdentifiers: Sequence[bytes]):
+        self.databaseMap, self.params = databaseMap, list(params)
+        self.hintIdentifiers = [bytes(h) for h in hintIdentifiers]
+
+    @property
+    def scalar(self):
+        """The tool's Scalar: UInt32 for ct <= 32, else UInt64 (main.swift:369-371)."""
+        return np.uint32 if self.params and self.params[0].ciphertextModulusBits <= 32 else np.uint64
+
+    def __eq__(self, other):
+        return (isinstance(other, SimplePirConfig) and self.databaseMap == other.databaseMap and
+                self.params == other.params and self.hintIdentifiers == other.hintIdentifiers)
+
+    def _args(self):
+        m = self.databaseMap
+        counts = ((m.sizes + m.chunkSize - 1) // m.chunkSize).astype(np.uint64)
+        index = np.ascontiguousarray(m.originalIndices.astype(np.uint64))
+        sizes = np.ascontiguousarray(m.sizes.astype(np.uint64))
+        locs = np.ascontiguousarray(m.chunkLocations, dtype=np.int64)
+        cparams = (_Params * max(len(self.params), 1))(*[p._c(32 if p.ciphertextModulusBits <= 32 else 64)
+                                                          for p in self.params])
+        seeds = np.frombuffer(b"".join(p.seed for p in self.params) or b"\0", dtype=np.uint8).copy()
+        ids = [C.create_string_buffer(h, max(len(h), 1)) for h in self.hintIdentifiers]
+        id_ptrs = (C.c_void_p * max(len(ids), 1))(*[C.addressof(b) for b in ids])
+        id_sizes = np.array([len(h) for h in self.hintIdentifiers] or [0], dtype=np.uint64)
+        keep = (index, sizes, counts, locs, cparams, seeds, ids, id_ptrs, id_sizes)
+        args = [_ptr(index), _ptr(sizes), _ptr(counts), len(sizes), _ptr(locs), m.chunkSize, cparams, _ptr(seeds),
+                len(self.params), id_ptrs, _ptr(id_sizes), len(self.hintIdentifiers)]
+        return keep, args
+
+    def serialize(self) -> bytes:
+        for p in self.params:
+            if len(p.seed) != SEED_BYTES:
+                raise PirError(f"seed must be {SEED_BYTES} bytes")
+        keep, args = self._args()
+        lib, n = load_library(), C.c_uint64(0)
+        _check(lib.hecuda_simple_pir_config_serialized_byte_count(*args, C.byref(n)))
+        out = np.empty(max(n.value, 1), dtype=np.uint8)
+        _check(lib.hecuda_simple_pir_config_serialize(*args, _ptr(out), n.value))
+        del keep
+        return out[:n.value].tobytes()
+
+    @staticmethod
+    def deserialize(data: bytes, securityLevel: str = "quantum128") -> "SimplePirConfig":
+        """SimplePIRConfig -> its fields, refused as the reference's native() refuses (errorStdDev, a_seed) and as the
+        library refuses parameters; each shard's encryption parameters are checked at securityLevel."""
+        buf, n = _bytes_arg(data)
+        lib, shape = load_library(), _ConfigShape()
+        _check(lib.hecuda_simple_pir_config_describe(buf, n, C.byref(shape)))
+        entries, chunks, shards = shape.entry_count, shape.chunk_count, shape.shard_count
+        index, sizes, counts = (np.zeros(max(entries, 1), dtype=np.uint64) for _ in range(3))
+        locs = np.zeros((max(chunks, 1), 2), dtype=np.int64)
+        cparams = (_Params * max(shards, 1))()
+        seeds = np.zeros(max(shards, 1) * SEED_BYTES, dtype=np.uint8)
+        ranges = np.zeros((max(shape.hint_identifier_count, 1), 2), dtype=np.uint64)
+        _check(lib.hecuda_simple_pir_config_read(buf, n, _ptr(index), _ptr(sizes), _ptr(counts), _ptr(locs), cparams,
+                                                 _ptr(seeds), _ptr(ranges)))
+        size = sizes[:entries].astype(np.int64)
+        chunk_size = int(shape.chunk_size)
+        if chunk_size < 1 and chunks:
+            raise PirError("DatabaseMapping: chunk_size must be positive")
+        if entries and not np.array_equal(counts[:entries].astype(np.int64), (size + max(chunk_size, 1) - 1) // max(chunk_size, 1)):
+            raise PirError("DatabaseMapping: an entry's chunk count is not ceil(size / chunk_size)")
+        database_map = DatabaseMap(index[:entries].astype(np.int64), size, locs[:chunks], chunk_size)
+        params = []
+        for s in range(shards):
+            c = cparams[s]
+            enc = SimplePirEncryptionParams(c.plaintext_modulus_bits, c.ciphertext_modulus_bits, c.lattice_dimension,
+                                            c.error_std_dev, securityLevel)
+            params.append(SimplePirParameters(enc, c.entry_size, c.entries_per_column, c.chunks_per_entry,
+                                              c.database_columns, seeds[SEED_BYTES * s:SEED_BYTES * (s + 1)].tobytes()))
+        raw = bytes(data)
+        ids = [raw[int(a):int(a) + int(b)] for a, b in ranges[:shape.hint_identifier_count]]
+        return SimplePirConfig(database_map, params, ids)
+
+    def save(self, path: str):
+        with open(path, "wb") as f:
+            f.write(self.serialize())
+
+    @staticmethod
+    def load(path: str, securityLevel: str = "quantum128") -> "SimplePirConfig":
+        with open(path, "rb") as f:
+            return SimplePirConfig.deserialize(f.read(), securityLevel)
 
 
 def _validate(trial, trials: int, index: int, expected: bytes):
